@@ -10,14 +10,15 @@ pair i of rank r is synth.make_pair(workload, r + i*W); at 8 GPUs two steps are 
 Prints ONE JSON line (see the task contract):
   value     pairs/s with the raw pairs already resident in HBM when the timed region starts
   e2e       pairs/s through the public API with HOST (pinned) inputs: H2D + collate + forward + D2H of transform + metrics
-  roofline  the dominant kernel family by GPU-time share (tcgen05 3xTF32 GEMMs), algorithmic FLOPs / CUDA-event time, with the
-            measured TF32 dense peak and the committed ncu DRAM traffic; beside it roofline_gse_embed (the structure embedding:
+  roofline  the dominant kernel family by GPU-time share (wgmma 3xTF32 GEMMs), algorithmic FLOPs / CUDA-event time, with the
+            measured TF32 dense peak; beside it roofline_gse_embed (the structure embedding:
             an HBM row with the default tabulated projections, a tensor row with --gse-mode 3) and roofline_attention (HBM)
   config    the STATIC workload description, identical in both arms; run_info = what was measured during the run
   cpu_baseline    the reference's CPU path on this box's host cores, bounded sample (N=1 only): 16-thread and 1-thread numbers
   gpu_eager_port  host collate + the pinned torch restatement executed as eager ops on this GPU (what a drop-in user sees today)
 --impl reference times the CPU path alone (the reference's own C++ collate ops + the oracle port of the forward) on the same
 config, each of its steps a bounded sample (one pair) of the configured step.
+--dump-outputs DIR writes what the timed path returned for the pairs of its last step (all ranks) as DIR/<name>.npy (see dump_outputs).
 """
 import argparse
 import json
@@ -45,14 +46,19 @@ def parse():
     ap.add_argument('--impl', default='ours', choices=['ours', 'reference'])
     ap.add_argument('--workload', default='3dmatch20k')
     ap.add_argument('--gse-mode', type=int, default=None)
-    ap.add_argument('--linear-persistent', type=int, default=None, help='1/0: persistent tile loop of the tcgen05 GEMM')
+    ap.add_argument('--linear-persistent', type=int, default=None, help='1/0: persistent tile loop of the tensor-core GEMM')
     ap.add_argument('--batch', type=int, default=8, help='pairs per forward (GeoTransformer.forward_batch); 1 = one pair per forward')
     ap.add_argument('--streams', type=int, default=None,
                     help='forwards in flight per GPU (one CUDA stream + host thread each); default 2 in batch mode, 4 with --batch 1')
     ap.add_argument('--pairs-per-step', type=int, default=None, help='pairs per GPU and step (default 4 x batch x streams = 64)')
     ap.add_argument('--attention-tma', type=int, default=None, help='1/0: TMA-staged self-attention kernels (default 1)')
     ap.add_argument('--no-cpu-baseline', action='store_true')
-    return ap.parse_args()
+    ap.add_argument('--dump-outputs', default=None, metavar='DIR',
+                    help='write the outputs of the last timed step (resident inputs, all ranks) to DIR/<name>.npy')
+    args = ap.parse_args()
+    if args.dump_outputs and args.impl == 'reference':
+        ap.error('--dump-outputs applies to the GPU path (--impl ours); the reference arm times a bounded CPU sample')
+    return args
 
 
 def dist_env():
@@ -92,17 +98,14 @@ class ClockSampler(threading.Thread):
 
 
 def load_peaks():
-    """(bf16 dense TF/s BURST -- the roofline kernels are timed alone --, sustained, HBM GB/s, source)"""
-    p = os.path.join(ROOT, 'MEASURED_PEAKS.json')
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return d.get('bf16_tflops'), d.get('bf16_tflops_sustained', d.get('bf16_tflops')), d.get('hbm_gbs'), 'measured'
-    return 1690.0, 1400.0, 6650.0, 'fallback (B200_PROFILING.md)'
+    """(bf16 dense TF/s, the same figure as the sustained value, HBM GB/s, source): NVIDIA's H100 SXM data sheet figures for a
+    700 W card, used as denominators only; a card run at a lower power limit reaches less"""
+    return 989.0, 989.0, 3350.0, 'H100 SXM data sheet (not measured)'
 
 
 def measure_tf32_peak(dev):
-    """Dense TF32 tensor throughput of this GPU, measured the way MEASURED_PEAKS.json's bf16 figure was (torch.matmul 8192^3,
-    best of 10, CUDA events) with fp32 operands and allow_tf32=True.  A library GEMM as a yardstick only -- not on the product path."""
+    """Dense TF32 tensor throughput of this GPU (torch.matmul 8192^3, best of 10, CUDA events) with fp32 operands and
+    allow_tf32=True.  A library GEMM as a yardstick only -- not on the product path."""
     try:
         prev = torch.backends.cuda.matmul.allow_tf32
         torch.backends.cuda.matmul.allow_tf32 = True
@@ -126,7 +129,7 @@ def measure_tf32_peak(dev):
         return None
 
 
-def attention_roofline(dev, n_sp, clouds, channels, heads, peak_hbm, traffic):
+def attention_roofline(dev, n_sp, clouds, channels, heads, peak_hbm):
     """HBM roofline of the self-attention (the E stream, N^2 C 4 bytes per cloud and layer, is its only large operand): one
     layer over `clouds` clouds of n_sp superpoints through geob200_attention_batched (q.k pass + TMA-staged E stream + P.v pass),
     CUDA events around the three launches, L2 flushed between repetitions.  achieved = E bytes / time of ALL three launches."""
@@ -167,17 +170,16 @@ def attention_roofline(dev, n_sp, clouds, channels, heads, peak_hbm, traffic):
         e_bytes = float(clouds) * N * N * C * 4
         ach = e_bytes / (ms * 1e-3) / 1e9
         return {'kernel': 'self-attention layer: att_qk_kernel + att_stream_kernel (TMA-staged E stream) + att_pv_kernel', 'bound': 'hbm',
-                'achieved': ach, 'peak': peak_hbm, 'unit': 'GB/s', 'frac': ach / peak_hbm, 'traffic': traffic.get('att_stream_bytes_per_launch'),
+                'achieved': ach, 'peak': peak_hbm, 'unit': 'GB/s', 'frac': ach / peak_hbm,
                 'algorithmic_bytes_per_launch': e_bytes, 'ms_per_layer': ms, 'clouds': clouds, 'superpoints_per_cloud': N,
                 'timing': 'CUDA events around the three launches of one layer (median of 10, L2 flushed), kernels alone on the GPU, after the timed regions',
-                'note': 'achieved counts the E bytes only and divides by the time of ALL three launches; the streaming kernel alone moves '
-                        'E at 5.35 TB/s = 0.81 of the peak (ncu, profiles/r02_top_kernels_ncu_selected.csv)'}
+                'note': 'achieved counts the E bytes only and divides by the time of ALL three launches'}
     except Exception as ex:
         return {'kernel': 'self-attention', 'bound': 'hbm', 'achieved': None, 'note': f'failed: {type(ex).__name__}: {ex}'}
 
 
-def gse_contraction_roofline(dev, emb_mod, n_sp, clouds, peak_tf, peak_src, traffic):
-    """Tensor roofline of the structure embedding IN ITS CONTRACTION FORM (tcgen05 3xFP16 kernel, GSE mode 3 -- the dense
+def gse_contraction_roofline(dev, emb_mod, n_sp, clouds, peak_tf, peak_src):
+    """Tensor roofline of the structure embedding IN ITS CONTRACTION FORM (wgmma 3xFP16 kernel, GSE mode 3 -- the dense
     contraction north_star names), timed alone on a batch-sized problem after the timed regions: the default path does not run it
     any more (tabulated projections, roofline_gse_embed), the number stays in the line for comparison.  Same call sequence as
     tests/gse_table_check.py."""
@@ -210,19 +212,13 @@ def gse_contraction_roofline(dev, emb_mod, n_sp, clouds, peak_tf, peak_src, traf
         ms = ts[len(ts) // 2]
         flops = 2.0 * rows * 4 * C * C
         ach = flops / (ms * 1e-3) / 1e12
-        return {'kernel': f'gse_embed_f16_kernel<{C}> (structure embedding as a tcgen05 3xFP16 contraction; NOT on the default path)', 'bound': 'tensor',
-                'achieved': ach, 'peak': peak_tf, 'unit': 'TFLOP/s', 'frac': ach / peak_tf, 'traffic': traffic.get('gse_embed_bytes_per_launch'),
+        return {'kernel': f'gse_embed_kernel<{C}, fp16> (structure embedding as a wgmma 3xFP16 contraction; NOT on the default path)', 'bound': 'tensor',
+                'achieved': ach, 'peak': peak_tf, 'unit': 'TFLOP/s', 'frac': ach / peak_tf,
                 'ms_per_launch': ms, 'flops_per_launch': flops, 'clouds': clouds, 'superpoints_per_cloud': n_sp,
                 'timing': 'CUDA events around the launch (median of 5, L2 flushed), kernel alone on the GPU, after the timed regions',
-                'peak_source': f'{peak_src} bf16 dense BURST (MEASURED_PEAKS.json; the kernel is timed alone)'}
+                'peak_source': f'{peak_src} bf16 dense (the kernel is timed alone)'}
     except Exception as ex:
-        return {'kernel': 'gse_embed_f16_kernel', 'bound': 'tensor', 'achieved': None, 'note': f'failed: {type(ex).__name__}: {ex}'}
-
-
-def load_traffic():
-    """per-launch DRAM traffic of the roofline kernels from the committed ncu --set full capture (profiles/r02_dram_traffic.json)"""
-    p = os.path.join(ROOT, 'profiles', 'r02_dram_traffic.json')
-    return json.load(open(p)) if os.path.exists(p) else {}
+        return {'kernel': 'gse_embed_kernel', 'bound': 'tensor', 'achieved': None, 'note': f'failed: {type(ex).__name__}: {ex}'}
 
 
 def make_inputs(workload, n_pairs, rank, world):
@@ -236,9 +232,8 @@ def make_inputs(workload, n_pairs, rank, world):
 
 
 def cpu_threads():
-    """Intra-op threads for the CPU reference path.  Measured on the B200 host (128 vCPU): the forward of one demo-size
-    pair takes 1.3 s with 1 thread, 0.1 s with 16, 0.5 s with 64 and 116 s with 128 (oversubscription on the thousands of
-    tiny ATen ops) -- so the baseline uses min(cores, 16), the fastest setting, and reports that number as `cores`."""
+    """Intra-op threads for the CPU reference path: min(cores, 16), because many more threads oversubscribe the thousands of
+    tiny ATen ops of the forward; the number is reported as `cores`."""
     return max(1, min(os.cpu_count() or 1, 16))
 
 
@@ -251,7 +246,7 @@ def _stats(xs):
 def gpu_eager_port(workload, n_pairs, device):
     """What a drop-in user of the reference sees today on this GPU (SURVEY.md 8d, engine/single_tester.py:52-58): collate on the
     host CPU (the reference runs it in DataLoader workers), then the model forward as EAGER torch ops on the GPU.
-    /root/reference is not on the GPU box, so the forward is the pinned torch restatement (oracle/geo_oracle.py, bit-identical
+    The reference's Python package is not part of this repository, so the forward is the pinned torch restatement (oracle/geo_oracle.py, bit-identical
     to the reference on CPU) executed with device tensors -- cuBLAS / ATen kernels, allow_tf32 off as in the reference.
     Returns a dict for the bench line (never raises)."""
     try:
@@ -330,6 +325,30 @@ def cpu_reference_pairs_per_s(workload, n_pairs, threads, return_times=False):
     return n_pairs / total, total, desc
 
 
+DUMP_METRICS = ('PIR', 'IR', 'RRE', 'RTE', 'RMSE', 'RR')
+
+
+def dump_rows(res, first_local, rank, world):
+    """one float64 row per pair of ``res`` (RegistrationEngine.register results of local pairs first_local, first_local + 1, ...):
+    global pair id, estimated_transform (16), metrics (DUMP_METRICS), num_corr, num_superpoints (2)"""
+    return [[float(rank + (first_local + j) * world)] + r['estimated_transform'].reshape(16).tolist() +
+            [float(r['metrics'][k]) for k in DUMP_METRICS] + [float(r['num_corr'])] + [float(n) for n in r['num_superpoints']]
+            for j, r in enumerate(res)]
+
+
+def dump_outputs(out_dir, rows):
+    """The results the timed path returned for the pairs of its last step on every rank (same inputs on every run with the
+    same arguments), in global pair order: pair_id (P,) float64, estimated_transform (P, 4, 4) float32, metrics (P, 6)
+    float32 with the columns PIR, IR, RRE, RTE, RMSE, RR, num_corr (P,) and num_superpoints (P, 2) float64."""
+    os.makedirs(out_dir, exist_ok=True)
+    rows = rows[np.argsort(rows[:, 0], kind='stable')]
+    m = 17 + len(DUMP_METRICS)
+    arrays = {'pair_id': rows[:, 0], 'estimated_transform': rows[:, 1:17].reshape(-1, 4, 4).astype(np.float32),
+              'metrics': rows[:, 17:m].astype(np.float32), 'num_corr': rows[:, m], 'num_superpoints': rows[:, m + 1:m + 3]}
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f'{name}.npy'), np.ascontiguousarray(a))
+
+
 def step_shape(args):
     """(pairs per forward, forwards in flight, pairs per GPU and step) of the GPU arm for these flags"""
     batch = max(1, args.batch)
@@ -348,7 +367,7 @@ def workload_config(args, world):
     return {'workload': args.workload, 'pairs_per_step_per_gpu': per_step, 'pairs_per_forward': batch, 'forwards_in_flight': lanes,
             'points_per_cloud': int(kw['n']), 'sinkhorn_iterations': make_cfg(cfg_name).model.num_sinkhorn_iterations,
             'parallelism': f'pairs sharded over {world} GPU(s), one all_gather of metric rows',
-            'l2': 'a different pair every step; per-pair working set (~0.5 GB incl. 2x75 MB embeddings) exceeds the 126 MB L2',
+            'l2': 'a different pair every step; per-pair working set (~0.5 GB incl. 2x75 MB embeddings) exceeds the 50 MB L2',
             'weights': 'random init (synthetic_state_dict seed 7351)'}
 
 
@@ -379,8 +398,8 @@ def main():
                                  'seconds_per_pair': _stats(per_pair),
                                  'one_thread': {'value': v1, 'unit': 'pairs/s', 'cores': 1, 'sample': desc1},
                                  'host_cpus': os.cpu_count(),
-                                 'threads_note': 'min(cores, 16) intra-op threads is the fastest setting measured on the 128-vCPU host '
-                                                 '(more threads oversubscribe the thousands of tiny ATen ops); the 1-thread number is printed beside it'},
+                                 'threads_note': 'min(cores, 16) intra-op threads (more threads oversubscribe the thousands of tiny '
+                                                 'ATen ops); the 1-thread number is printed beside it'},
                 'e2e': {'value': v, 'unit': 'pairs/s', 'h2d_bytes_per_step': 0, 'd2h_bytes_per_step': 0},
                 'gpu_launches': 0}
         print(json.dumps(line))
@@ -492,7 +511,8 @@ def main():
     lib = _lib.lib()
     l0 = lib.geob200_launch_count()
     GF.EVENTS = {}
-    ms_res = timed(resident, W, K)
+    results_res = []
+    ms_res = timed(resident, W, K, sink=results_res)
     per_rank_res = timed.per_rank
     mallocs_res = segs() - seg0
     launches = (lib.geob200_launch_count() - l0)
@@ -508,7 +528,7 @@ def main():
     GF.EVENTS = {}
     barrier()
     n_solo = min(K * S, max(8, 2 * BATCH))
-    lib.geob200_linear_profile_enable(1)          # CUDA events around every tcgen05 GEMM launch of these pairs
+    lib.geob200_linear_profile_enable(1)          # CUDA events around every tensor-core GEMM launch of these pairs
     solo.register(resident[W * S:W * S + n_solo])
     barrier()
     import ctypes
@@ -532,6 +552,10 @@ def main():
                      m['RR']])
     rows_t = torch.tensor(rows, dtype=torch.float32, device=dev)
     rows_t = gather_metric_rows(rows_t, world)
+    dumped = None
+    if args.dump_outputs:               # the last timed step of the resident region: local pairs (W + K - 1) * S ... (W + K) * S - 1
+        local = torch.tensor(dump_rows(results_res[-S:], (W + K - 1) * S, rank, world), dtype=torch.float64, device=dev)
+        dumped = gather_metric_rows(local, world).cpu().numpy()
     if rank != 0:
         if world > 1:
             dist.destroy_process_group()
@@ -547,12 +571,11 @@ def main():
     clouds_per_launch = 2 * BATCH if BATCH > 1 else 1          # batch mode: ONE structure-embedding launch covers all clouds of the batch
     flops = 2.0 * mean_n2 * 4 * C * C * clouds_per_launch
     peak_tf, peak_tf_sustained, peak_hbm, peak_src = load_peaks()
-    traffic = load_traffic()
     avg_ms = float(np.mean(gse_solo_ms)) if gse_solo_ms else None
     achieved = flops / (avg_ms * 1e-3) / 1e12 if avg_ms else None
     avg_ms_concurrent = float(np.mean(gse_ms)) if gse_ms else None
-    mode_name = {0: 'fp32 CUDA cores', 1: 'tcgen05 3xTF32', 2: 'tcgen05 1xTF32', 3: 'tcgen05 3xFP16 (fp32-accurate split)',
-                 4: 'tcgen05 3xFP16 split, CTA-pair TMA multicast of B',
+    mode_name = {0: 'fp32 CUDA cores', 1: 'wgmma 3xTF32', 2: 'wgmma 1xTF32', 3: 'wgmma 3xFP16 (fp32-accurate split)',
+                 4: 'wgmma 3xFP16 split, CTA-pair TMA multicast of B',
                  5: 'tabulated projections (4 lookups + 3 max + 1 add per row and channel; no contraction)'}[GF.GSE_MODE]
     common = {'avg_ms_per_launch': avg_ms, 'launches_timed': len(gse_solo_ms), 'clouds_per_launch': clouds_per_launch,
               'avg_ms_per_launch_with_other_streams_active': avg_ms_concurrent,
@@ -569,13 +592,13 @@ def main():
                         'algorithmic_bytes_per_launch': e_bytes, 'l2_node_bytes_per_launch': rows * 4 * C * 6,
                         'l2_node_read_GBps': (rows * 4 * C * 6 / (avg_ms * 1e-3) / 1e9) if avg_ms else None,
                         'contraction_flops_replaced_per_launch': flops,
-                        'peak_source': f'{peak_src} HBM copy bandwidth (MEASURED_PEAKS.json)',
+                        'peak_source': f'{peak_src} HBM bandwidth',
                         'note': 'HBM roofline = the compulsory write of E; the kernel is bound by the L2 reads of the table nodes '
                                 '(6 x the E bytes), see l2_node_read_GBps', **common}
     else:
         roofline_gse = {'kernel': 'gse_embed (structure-embedding contraction)', 'bound': 'tensor', 'achieved': achieved, 'peak': peak_tf,
-                        'unit': 'TFLOP/s', 'frac': (achieved / peak_tf) if achieved else None, 'traffic': traffic.get('gse_embed_bytes_per_launch'),
-                        'flops_per_launch': flops, 'peak_source': f'{peak_src} bf16 dense BURST (MEASURED_PEAKS.json; the kernel is timed alone)',
+                        'unit': 'TFLOP/s', 'frac': (achieved / peak_tf) if achieved else None,
+                        'flops_per_launch': flops, 'peak_source': f'{peak_src} bf16 dense (the kernel is timed alone)',
                         **common}
 
     # dominant kernel by share of the step's GPU time: linear_tc_kernel (every nn.Linear and the KPConv contraction; ~80 launches
@@ -592,10 +615,9 @@ def main():
         e[0] += 1; e[1] += t; e[2] += 2.0 * m * n * k; e[3] = max(e[3], m)
     shape_table = [{'n': n, 'k': k, 'launches': c, 'max_m': mm, 'ms_per_pair': round(t / max(n_solo, 1), 4), 'tflops': round(fl / (t * 1e-3) / 1e12, 1)}
                    for (n, k), (c, t, fl, mm) in sorted(by_shape.items(), key=lambda kv: -kv[1][1])[:12]]
-    roofline = {'kernel': 'linear_tc_kernel (tcgen05 3xTF32 GEMM: all nn.Linear + KPConv contraction)', 'bound': 'tensor',
+    roofline = {'kernel': 'linear_tc_kernel (wgmma 3xTF32 GEMM: all nn.Linear + KPConv contraction)', 'bound': 'tensor',
                 'achieved': (g_flops / (g_ms * 1e-3) / 1e12) if g_ms else None, 'peak': peak_tf, 'unit': 'TFLOP/s',
                 'frac': (g_flops / (g_ms * 1e-3) / 1e12 / peak_tf) if g_ms else None,
-                'traffic': traffic.get('linear_tc_bytes_per_launch'), 'traffic_note': traffic.get('note'),
                 'algorithmic_bytes_per_launch': (g_bytes / n_gemm) if n_gemm else None,
                 'tf32_dense_peak_measured': tf32_peak,
                 'frac_of_3xtf32_ceiling': (g_flops / (g_ms * 1e-3) / 1e12 / (tf32_peak / 3.0)) if (g_ms and tf32_peak) else None,
@@ -606,18 +628,17 @@ def main():
                 'share_of_gpu_time': (g_ms / max(n_solo, 1)) / (ms_res / (K * S)) if g_ms else None,
                 'timing': 'CUDA events around every launch, one pair in flight (kernel alone on the GPU), same workload, after the timed regions',
                 'note': 'the ~80 GEMMs of one forward (every nn.Linear + the KPConv contractions), each over the stacked rows of all pairs of the '
-                        'batch; the wide / deep shapes run at 125-133 TFLOP/s (shared-memory-bandwidth ceiling of the 3xTF32 formulation, DESIGN.md 5a), '
-                        'the narrow (N = 32, 64) and the M = 5 100 transformer shapes pull the family average down: see time_by_weight_shape; '
+                        'batch; see time_by_weight_shape for the time per weight shape; '
                         'share_of_gpu_time = its time per pair (kernel alone) / wall time per pair of the timed region',
-                'peak_source': f'{peak_src} bf16 dense BURST (MEASURED_PEAKS.json; launches timed alone); tf32_dense_peak_measured = torch.matmul fp32 '
+                'peak_source': f'{peak_src} bf16 dense (launches timed alone); tf32_dense_peak_measured = torch.matmul fp32 '
                                f'8192^3 with allow_tf32, best of 10, this run; the kernel executes 3 TF32 MMAs per product term'}
 
     roofline_att = None
     roofline_gse_tc = None
     if rank == 0 and C in (128, 256) and n_c:
-        roofline_att = attention_roofline(dev, int(np.mean(n_c)), 2 * BATCH, C, cfg.geotransformer.num_heads, peak_hbm, traffic)
+        roofline_att = attention_roofline(dev, int(np.mean(n_c)), 2 * BATCH, C, cfg.geotransformer.num_heads, peak_hbm)
         if GF.GSE_MODE == 5:
-            roofline_gse_tc = gse_contraction_roofline(dev, model.transformer.embedding, int(np.mean(n_c)), 2 * BATCH, peak_tf, peak_src, traffic)
+            roofline_gse_tc = gse_contraction_roofline(dev, model.transformer.embedding, int(np.mean(n_c)), 2 * BATCH, peak_tf, peak_src)
 
     cpu = None
     if world == 1 and not args.no_cpu_baseline:
@@ -644,13 +665,15 @@ def main():
                 'h2d_bytes_per_step': int(h2d_bytes), 'd2h_bytes_per_step': 96 * S},
         'gpu_launches': int(launches), 'gpu_launches_per_pair': launches / max(K * S, 1),
         'cuda_mallocs': {'timed_region_resident': int(mallocs_res), 'timed_region_e2e': int(mallocs_e2e)},
-        'per_rank_ms': {'value': per_rank_res, 'e2e': per_rank_e2e}, 'roofline': roofline, 'roofline_gse_embed': roofline_gse, 'roofline_gse_contraction_tcgen05': roofline_gse_tc, 'roofline_attention': roofline_att, 'cpu_baseline': cpu, 'gpu_eager_port': eager, 'clocks': sampler.summary(),
+        'per_rank_ms': {'value': per_rank_res, 'e2e': per_rank_e2e}, 'roofline': roofline, 'roofline_gse_embed': roofline_gse, 'roofline_gse_contraction': roofline_gse_tc, 'roofline_attention': roofline_att, 'cpu_baseline': cpu, 'gpu_eager_port': eager, 'clocks': sampler.summary(),
         'quality': {'median_rre_deg': float(rows_t[:, 0].median()), 'median_rte': float(rows_t[:, 1].median()),
                     'mean_correspondences': float(rows_t[:, 2].mean()), 'pairs': int(rows_t.shape[0]),
                     'mean_PIR': float(rows_t[:, 4].nanmean()), 'mean_IR': float(rows_t[:, 5].nanmean()),
                     'registration_recall': float(rows_t[:, 7].mean()),
                     'note': 'random-init weights: the numbers show the metric path runs, not registration quality'},
     }
+    if dumped is not None:
+        dump_outputs(args.dump_outputs, dumped)
     print(json.dumps(line))
     if world > 1:
         dist.destroy_process_group()

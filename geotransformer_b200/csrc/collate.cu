@@ -525,7 +525,7 @@ __global__ void rs_cellsegs_kernel(const RsCloud* __restrict__ clouds, int nb, C
 // entries get the sentinel n_support_total (radius_neighbors_cpu.cpp:78-88).
 // Warp-level bitonic sort of 32 * KPL 64-bit keys held in registers, striped layout: element e = r * 32 + lane lives in
 // register r of lane `lane`.  Partners less than 32 apart are exchanged with shuffles, the others are register pairs of the same
-// lane: no shared-memory round trips and no __syncwarp per step (the shared-memory version spent ~80 % of the query in them).
+// lane: no shared-memory round trips and no __syncwarp per step (a shared-memory sort spends most of the query in them).
 template <int KPL>
 __device__ __forceinline__ void warp_bitonic_sort(unsigned long long (&key)[KPL], int lane) {
 #pragma unroll

@@ -1,4 +1,4 @@
-// Shared helpers for the geob200 CUDA kernels (sm_100a only).
+// Shared helpers for the geob200 CUDA kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -157,7 +157,7 @@ static inline int num_sms() {
         int dev = 0;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        if (n <= 0) n = 148;
+        if (n <= 0) n = 132;
     }
     return n;
 }

@@ -8,7 +8,7 @@
 // E (N,N,C) is written: the O(N^2 k C) intermediate never exists.
 //
 // This file holds the index kernel and the fp32 CUDA-core contraction (exact-fp32 reference path).  The
-// tcgen05 tensor-core contraction lives in gse_tc.cu and is selected by geob200_structure_embedding().
+// wgmma tensor-core contraction lives in gse_tc.cu and is selected by geob200_structure_embedding().
 #include "common.cuh"
 #include "geob200.h"
 
@@ -250,7 +250,7 @@ __global__ void __launch_bounds__(256) gse_embed_generic_kernel(const float* __r
 
 using namespace geob200;
 
-// implemented in gse_tc.cu (tcgen05 tensor-core contraction); returns 1 if it does not handle this shape/mode
+// implemented in gse_tc.cu (wgmma tensor-core contraction); returns 1 if it does not handle this shape/mode
 int geob200_gse_embed_tc(const float* d_idx, const float* a_idx, long long n_pairs, int C, const float* div_term,
                          const float* Wd, const float* Wa, const float* bd, const float* ba, float* E, int mode,
                          void* workspace, size_t workspace_bytes, cudaStream_t st);
@@ -302,8 +302,8 @@ size_t geob200_gse_embed_workspace_bytes(int64_t n, int64_t channels) {
     return (size_t)(4 * channels * channels * 4 * 3 + 4096);   // room for split/packed weight copies of the tensor-core path
 }
 
-// mode: 0 = fp32 CUDA cores (exact-fp32 accumulation), 1 = tcgen05 3xTF32 (fp32-accurate), 2 = tcgen05 1xTF32,
-//       3 = tcgen05 3xFP16 (fp32-accurate, half the tensor-pipe time of 3xTF32; default)
+// mode: 0 = fp32 CUDA cores (exact-fp32 accumulation), 1 = wgmma 3xTF32 (fp32-accurate), 2 = wgmma 1xTF32,
+//       3 = wgmma 3xFP16 (fp32-accurate, half the tensor-pipe time of 3xTF32; default)
 int geob200_gse_embed(const float* d_indices, const float* a_indices, int64_t n, int64_t channels, const float* div_term,
                       const float* wd_t, const float* wa_t, const float* wd, const float* wa, const float* bd, const float* ba,
                       float* embeddings, int mode, void* workspace, size_t workspace_bytes, void* stream) {

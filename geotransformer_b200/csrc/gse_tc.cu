@@ -1,67 +1,44 @@
-// tcgen05 (5th-gen tensor core) contraction of the geometric structure embedding for C = 256.
+// Hopper tensor-core (wgmma) contraction of the geometric structure embedding for C = 256 (and C = 128 in fp16).
 //
 // Reference semantics: geotransformer/modules/geotransformer/geotransformer.py:57-72
-//     E[p,:] = (Wd s(d_p) + bd) + max_k (Wa s(a_pk) + ba)          s(.) = 256-wide interleaved sin/cos embedding
+//     E[p,:] = (Wd s(d_p) + bd) + max_k (Wa s(a_pk) + ba)          s(.) = C-wide interleaved sin/cos embedding
 // Because the distance term does not depend on k it can be folded under the max exactly:
 //     E[p,:] = max_k ( [Wa | Wd] . [s(a_pk) ; s(d_p)] ) + (ba + bd)
-// so EVERY row (p,k) of the problem is one homogeneous GEMM row with K = 512 against ONE operand B = [Wa | Wd]
-// (256 x 512).  A tile is 42 pairs = 126 rows (M = 128, two idle rows), N = 256, K = 512.
+// so EVERY row (p,k) of the problem is one homogeneous GEMM row with K = 2C against ONE operand B = [Wa | Wd]
+// (C x 2C).  A tile is 42 pairs = 126 rows (M = 128, two idle rows), N = C.
 //
-// Pipeline inside one persistent CTA (one per SM), 704 threads:
-//   warps 0-15 generators : compute the sinusoid chunk (128 rows x 32 K) with sincosf and store it straight into
-//                           the canonical K-major SWIZZLE_128B shared-memory layout the UMMA descriptor expects
-//                           (the A operand never exists in HBM)
-//   warp 16    copier     : one lane streams the pre-swizzled B chunk (256 x 32 K = 32 KB, a contiguous image packed
-//                           by gse_pack_b_kernel) with cp.async.bulk (TMA, UBLKCP) onto the stage's mbarrier
-//   warp 17    MMA issuer : one lane issues tcgen05.mma.cta_group::1.kind::tf32 (M128 N256 K8) into a TMEM accumulator,
-//                           tcgen05.commit releases the stage / publishes the accumulator
-//   warps 18-21 epilogue   : tcgen05.ld the accumulator (32 lanes x 32 columns per warp), exchange through shared memory,
-//                           max over the three rows of a pair, add the bias, store E -- while the MMA warp already works
-//                           on the other accumulator (2 x 256 TMEM columns)
-// NPASS = 3 runs the error-compensated 3xTF32 scheme (a_hi b_hi + a_hi b_lo + a_lo b_hi, fp32 accumulate in TMEM), which
-// is fp32-accurate; NPASS = 1 is plain TF32.
+// Pipeline inside one persistent CTA (one per SM), 384 threads:
+//   warps 0-7   consumers  : two warpgroups, tile rows [0,64) and [64,128): wgmma.m64n{C} from shared memory into a register
+//                            accumulator; then the epilogue exchanges 32 columns at a time through shared memory, takes the
+//                            max over the three rows of a pair, adds the bias and stores E
+//   warps 8-11  generators : compute the sinusoid chunk (128 rows x 128 bytes) and store it straight into the K-major
+//                            SWIZZLE_128B layout (the A operand never exists in HBM); their first thread also streams the
+//                            pre-swizzled B chunk (packed once by gse_pack_b*_kernel) with cp.async.bulk onto the stage's mbarrier
+// Variants: 3xTF32 (NPASS = 3: a_hi b_hi + a_hi b_lo + a_lo b_hi, fp32-accurate), plain TF32 (NPASS = 1), and 3xFP16 (below),
+// the last also as a 2-CTA cluster that multicasts every B chunk into both CTAs.
 #include <cuda_fp16.h>
 
 #include "common.cuh"
 #include "geob200.h"
+#include "hopper.cuh"
 
 namespace geob200 {
 namespace tc {
 
+using namespace hop;
+
 constexpr int C = 256;                 // output channels = MMA N
 constexpr int KTOT = 512;              // [angle | distance] sinusoids
 constexpr int KC = 32;                 // K elements per chunk = 128 bytes = one swizzle atom row
-constexpr int NCHUNK = KTOT / KC;      // 16
+constexpr int KC16 = 64;               // fp16 K elements per chunk
 constexpr int PAIRS = 42;              // pairs per tile
-constexpr int ROWS = 128;              // MMA M
+constexpr int ROWS = 128;              // tile rows (two warpgroups of M = 64)
 constexpr int A_BYTES = ROWS * 128;    // 16 KB
-constexpr int B_BYTES = C * 128;       // 32 KB
 constexpr int STAGE_LD = 33;           // epilogue exchange row stride (floats)
-constexpr int NGEN_WARPS = 16;          // sinusoid generator warps (4 per SM sub-partition: latency hiding)
-constexpr int NTHREADS = (NGEN_WARPS + 2 + 4) * 32;
+constexpr int NCONS_WARPS = 8;
+constexpr int NGEN_WARPS = 4;
+constexpr int NTHREADS = (NCONS_WARPS + NGEN_WARPS) * 32;
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.shared::cta.b64 st, [%0];\n\t}" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.expect_tx.shared::cta.b64 st, [%0], %1;\n\t}" ::"r"(smem_u32(bar)), "r"(bytes)
-                 : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    const uint32_t addr = smem_u32(bar);
-    uint32_t done;
-    do {
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                     : "=r"(done)
-                     : "r"(addr), "r"(parity)
-                     : "memory");
-    } while (!done);
-}
 // sin and cos of x for moderate |x| (embedding arguments are < ~100 rad): 3-term Cody-Waite reduction by pi/2 and
 // degree-7/8 minimax polynomials on [-pi/4, pi/4]; ~1 ulp, about a third of the instructions of sincosf.
 __device__ __forceinline__ void sincos_cw(float x, float& s, float& c) {
@@ -97,54 +74,6 @@ __device__ __forceinline__ void sincos_sfu(float x, float& s, float& c) {
     c = ((q + 1) & 2) ? -cc : cc;
 }
 
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {   // waits for remote (cluster-scope) arrivals
-    const uint32_t addr = smem_u32(bar);
-    uint32_t done;
-    do {
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                     : "=r"(done)
-                     : "r"(addr), "r"(parity)
-                     : "memory");
-    } while (!done);
-}
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)),
-                 "l"(src), "r"(bytes), "r"(smem_u32(bar))
-                 : "memory");
-}
-
-// K-major SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor, sm_100 version 1):
-// start address >> 4 [0,14) | LBO >> 4 [16,30) (=1, unused for swizzled K-major) | SBO >> 4 [32,46) (8 rows x 128 B = 1024)
-// | version [46,48) = 1 | layout_type [61,64) = 2 (SWIZZLE_128B)
-__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
-    d |= (uint64_t)1 << 16;
-    d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
-}
-
-// instruction descriptor (cute::UMMA::InstrDescriptor): D = F32 (1 @ bit 4), A = B = TF32 (2 @ bits 7, 10), both K-major,
-// N >> 3 @ bit 17, M >> 4 @ bit 24
-constexpr uint32_t kIdesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(C >> 3) << 17) | ((uint32_t)(ROWS >> 4) << 24);
-
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(kIdesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
 // Packs B = [Wa | Wd] (row n = output channel, 512 K values) into per-chunk shared-memory images:
 // image[kc][n/8][n%8][(e/4) ^ (n%8)][e%4], hi part (tf32, round-to-nearest) and lo part (remainder).
 __global__ void __launch_bounds__(256) gse_pack_b_kernel(const float* __restrict__ Wd, const float* __restrict__ Wa,
@@ -161,226 +90,6 @@ __global__ void __launch_bounds__(256) gse_pack_b_kernel(const float* __restrict
     const int dst = kc * (C * KC) + (n >> 3) * 256 + (n & 7) * 32 + (((e >> 2) ^ (n & 7)) << 2) + (e & 3);
     img_hi[dst] = hi;
     img_lo[dst] = w - hi;
-}
-
-template <int NPASS>
-struct Cfg {
-    static constexpr int STAGE_BYTES = (NPASS == 3) ? 2 * (A_BYTES + B_BYTES) : (A_BYTES + B_BYTES);
-    static constexpr int NSTAGE = (NPASS == 3) ? 2 : 4;
-    static constexpr int SMEM = NSTAGE * STAGE_BYTES + ROWS * STAGE_LD * 4 + 1024 /*alignment slack*/ + 256 /*barriers*/;
-};
-
-template <int NPASS>
-__global__ void __launch_bounds__(NTHREADS, 1) gse_embed_tc_kernel(const float* __restrict__ d_idx, const float* __restrict__ a_idx,
-                                                                   long long n_pairs, const float* __restrict__ div_term,
-                                                                   const float* __restrict__ img_hi, const float* __restrict__ img_lo,
-                                                                   const float* __restrict__ bias_sum, float* __restrict__ E) {
-    using CF = Cfg<NPASS>;
-    constexpr int NSTAGE = CF::NSTAGE;
-    extern __shared__ unsigned char smem_raw[];
-    unsigned char* smem = (unsigned char*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);   // SWIZZLE_128B: 1024 B alignment
-    float* xstage = (float*)(smem + NSTAGE * CF::STAGE_BYTES);                                   // [128][33]
-    uint64_t* bars = (uint64_t*)(xstage + ROWS * STAGE_LD);
-    uint64_t* full = bars;                 // [NSTAGE]
-    uint64_t* empty = bars + NSTAGE;       // [NSTAGE]
-    uint64_t* tfull = bars + 2 * NSTAGE;   // [2]
-    uint64_t* tempty = tfull + 2;          // [2]
-    uint32_t* tmem_slot = (uint32_t*)(tempty + 2);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const long long n_tiles = (n_pairs + PAIRS - 1) / PAIRS;
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < NSTAGE; ++s) { mbar_init(&full[s], NGEN_WARPS + 1); mbar_init(&empty[s], 1); }
-        for (int a = 0; a < 2; ++a) { mbar_init(&tfull[a], 1); mbar_init(&tempty[a], 4); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == NGEN_WARPS + 1) {   // TMEM: 512 columns = two 128 x 256 fp32 accumulators
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(tmem_slot)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp < NGEN_WARPS) {
-        // ===================== generators =====================
-        // work item = (tile row, 16-byte chunk c) -> frequencies f0+2c, f0+2c+1 (sin, cos interleaved).  Angle chunks
-        // (kc < 8) have 126 x 8 items; distance chunks (kc >= 8) have 42 x 8 items whose result is stored to the three
-        // rows (k = 0,1,2) of the pair.
-        {   // padding rows 126,127 of every stage: zero once (their outputs are never read)
-            for (int e = threadIdx.x; e < NSTAGE * ((NPASS == 3) ? 2 : 1) * 64; e += NGEN_WARPS * 32) {
-                const int sidx = e / (((NPASS == 3) ? 2 : 1) * 64), rem = e % (((NPASS == 3) ? 2 : 1) * 64);
-                const int part = rem / 64, w = rem % 64;
-                float* base = (float*)(smem + sidx * CF::STAGE_BYTES + part * A_BYTES + 15 * 1024 + 6 * 128);
-                base[w] = 0.f;
-            }
-            asm volatile("bar.sync 2, %0;" ::"n"(NGEN_WARPS * 32) : "memory");
-        }
-        int s = 0;
-        uint32_t ph = 0;
-        for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-            const long long p0 = tile * PAIRS;
-            for (int kc = 0; kc < NCHUNK; ++kc) {
-                mbar_wait(&empty[s], ph ^ 1u);
-                unsigned char* st = smem + s * CF::STAGE_BYTES;
-                const int f0 = (kc & 7) * 16;
-                const bool angle = kc < 8;
-                const int n_items = (angle ? 3 * PAIRS : PAIRS) * 8;
-                for (int it = threadIdx.x; it < n_items; it += NGEN_WARPS * 32) {
-                    const int c = it & 7, rr = it >> 3;          // rr: tile row (angle) or pair slot (distance)
-                    const int j = angle ? (rr % PAIRS) : rr;
-                    const long long p = p0 + j;
-                    float x = 0.f;
-                    if (p < n_pairs) x = angle ? __ldg(a_idx + p * 3 + rr / PAIRS) : __ldg(d_idx + p);
-                    float s0, c0, s1, c1;
-                    sincos_cw(__fmul_rn(x, __ldg(div_term + f0 + 2 * c)), s0, c0);
-                    sincos_cw(__fmul_rn(x, __ldg(div_term + f0 + 2 * c + 1)), s1, c1);
-                    float4 hi = make_float4(s0, c0, s1, c1), lo = make_float4(0.f, 0.f, 0.f, 0.f);
-                    if (NPASS == 3) {
-                        hi.x = tf32_rn(s0); lo.x = s0 - hi.x;
-                        hi.y = tf32_rn(c0); lo.y = c0 - hi.y;
-                        hi.z = tf32_rn(s1); lo.z = s1 - hi.z;
-                        hi.w = tf32_rn(c1); lo.w = c1 - hi.w;
-                    }
-                    const int nrep = angle ? 1 : 3;
-                    for (int rep = 0; rep < nrep; ++rep) {
-                        const int r = angle ? rr : (rep * PAIRS + j);
-                        const uint32_t off = (uint32_t)((r >> 3) * 1024 + (r & 7) * 128 + ((c ^ (r & 7)) << 4));
-                        *reinterpret_cast<float4*>(st + off) = hi;
-                        if (NPASS == 3) *reinterpret_cast<float4*>(st + A_BYTES + off) = lo;
-                    }
-                }
-                fence_proxy_async();               // generic-proxy stores -> visible to the tensor core (async proxy)
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&full[s]);
-                if (++s == NSTAGE) { s = 0; ph ^= 1u; }
-            }
-        }
-    } else if (warp == NGEN_WARPS) {
-        // ===================== B copier (TMA bulk) =====================
-        if (lane == 0) {
-            int s = 0;
-            uint32_t ph = 0;
-            for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-                for (int kc = 0; kc < NCHUNK; ++kc) {
-                    mbar_wait(&empty[s], ph ^ 1u);
-                    unsigned char* st = smem + s * CF::STAGE_BYTES;
-                    const int a_bytes = (NPASS == 3) ? 2 * A_BYTES : A_BYTES;
-                    mbar_arrive_expect_tx(&full[s], (NPASS == 3) ? 2 * B_BYTES : B_BYTES);
-                    bulk_g2s(st + a_bytes, img_hi + (size_t)kc * (C * KC), B_BYTES, &full[s]);
-                    if (NPASS == 3) bulk_g2s(st + a_bytes + B_BYTES, img_lo + (size_t)kc * (C * KC), B_BYTES, &full[s]);
-                    if (++s == NSTAGE) { s = 0; ph ^= 1u; }
-                }
-            }
-        }
-    } else if (warp == NGEN_WARPS + 1) {
-        // ===================== MMA issuer =====================
-        if (lane == 0) {
-            int s = 0;
-            uint32_t ph = 0;
-            int acc = 0;
-            uint32_t acc_ph[2] = {0, 0};
-            for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-                mbar_wait(&tempty[acc], acc_ph[acc] ^ 1u);       // epilogue has drained this accumulator
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t)(acc * C);
-                for (int kc = 0; kc < NCHUNK; ++kc) {
-                    mbar_wait(&full[s], ph);
-                    tc_fence_after();
-                    const uint32_t st = smem_u32(smem + s * CF::STAGE_BYTES);
-                    const uint32_t a_bytes = (NPASS == 3) ? 2 * A_BYTES : A_BYTES;
-                    const uint64_t da_hi = make_desc(st), db_hi = make_desc(st + a_bytes);
-#pragma unroll
-                    for (int kk = 0; kk < KC / 8; ++kk) {       // 4 MMAs of K = 8 (32 bytes) per chunk
-                        const uint64_t adv = (uint64_t)(kk * 2);     // +32 bytes in 16-byte units
-                        const uint32_t first = (kc == 0 && kk == 0) ? 0u : 1u;
-                        umma_tf32(d_tmem, da_hi + adv, db_hi + adv, first);
-                        if (NPASS == 3) {
-                            const uint64_t da_lo = make_desc(st + A_BYTES), db_lo = make_desc(st + a_bytes + B_BYTES);
-                            umma_tf32(d_tmem, da_hi + adv, db_lo + adv, 1u);
-                            umma_tf32(d_tmem, da_lo + adv, db_hi + adv, 1u);
-                        }
-                    }
-                    umma_commit(&empty[s]);                      // stage reusable once these MMAs have read it
-                    if (++s == NSTAGE) { s = 0; ph ^= 1u; }
-                }
-                umma_commit(&tfull[acc]);                        // accumulator complete
-                acc_ph[acc] ^= 1u;
-                acc ^= 1;
-            }
-        }
-    } else {
-        // ===================== epilogue: 4 warps, TMEM lane quarter = warp % 4 =====================
-        const int q = warp & 3;
-        const int et = (warp - (NGEN_WARPS + 2)) * 32 + lane;                    // 0..127 within the epilogue group
-        int acc = 0;
-        uint32_t acc_ph[2] = {0, 0};
-        for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-            mbar_wait(&tfull[acc], acc_ph[acc]);
-            tc_fence_after();
-            const long long p0 = tile * PAIRS;
-            for (int cc = 0; cc < C / 32; ++cc) {
-                uint32_t v[32];
-                const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * C + cc * 32);
-                asm volatile(
-                    "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                    "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                    "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                    : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-                      "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-                      "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-                      "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-                    : "r"(taddr));
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                float* xr = xstage + (q * 32 + lane) * STAGE_LD;
-#pragma unroll
-                for (int c = 0; c < 32; ++c) xr[c] = __uint_as_float(v[c]);
-                asm volatile("bar.sync 1, 128;" ::: "memory");
-                for (int idx = et; idx < PAIRS * 32; idx += 128) {
-                    const int jj = idx >> 5, c = idx & 31;
-                    const long long p = p0 + jj;
-                    if (p < n_pairs) {
-                        const float m = fmaxf(fmaxf(xstage[jj * STAGE_LD + c], xstage[(PAIRS + jj) * STAGE_LD + c]),
-                                              xstage[(2 * PAIRS + jj) * STAGE_LD + c]);
-                        E[p * C + cc * 32 + c] = m + __ldg(bias_sum + cc * 32 + c);
-                    }
-                }
-                asm volatile("bar.sync 1, 128;" ::: "memory");
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tempty[acc]);
-            acc_ph[acc] ^= 1u;
-            acc ^= 1;
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == NGEN_WARPS + 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
-    }
-}
-
-// ============================================================================================================
-// 3xFP16 variant (default): x = x_hi + x_lo with x_hi = fp16(x), x_lo = fp16(x - x_hi).  fp16 carries the same 11 significant
-// bits as tf32, so hi.hi + hi.lo + lo.hi has the same ~2^-22 relative accuracy as 3xTF32, but kind::f16 MMAs consume K = 16
-// per instruction at the same rate at which kind::tf32 consumes K = 8: half the tensor-pipe time, half the B bytes, half
-// the generator stores.  The sinusoids are in [-1, 1] (lo <= 2^-12: fp16 subnormal spacing 6e-8 = fp32 epsilon); the weights
-// are pre-scaled by a power of two to [0.5, 1) (exact), undone in the epilogue.
-// ============================================================================================================
-constexpr int KC16 = 64;                  // halves per 128-byte row
-constexpr int NCHUNK16 = KTOT / KC16;     // 8
-constexpr uint32_t kIdescF16 = (1u << 4) | ((uint32_t)(C >> 3) << 17) | ((uint32_t)(ROWS >> 4) << 24);   // A = B = F16 (0), D = F32
-
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t accumulate, uint32_t idesc = kIdescF16) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
 }
 
 // scale[0] = 2^-e with max|W| = m 2^e, m in [0.5,1)  ; scale[1] = 2^e
@@ -419,406 +128,248 @@ __global__ void __launch_bounds__(256) gse_pack_b_f16_kernel(const float* __rest
     img_lo[dst] = __float2half_rn(w - __half2float(hi));
 }
 
-constexpr int F16_STAGE_BYTES = 2 * (A_BYTES + B_BYTES);      // hi + lo of both operands = 96 KB
-constexpr int F16_NSTAGE = 2;
-constexpr int F16_SMEM = F16_NSTAGE * F16_STAGE_BYTES + ROWS * STAGE_LD * 4 + 1024 + 256;
 
-template <int CC>
-__global__ void __launch_bounds__(NTHREADS, 1) gse_embed_f16_kernel(const float* __restrict__ d_idx, const float* __restrict__ a_idx,
-                                                                    long long n_pairs, const float* __restrict__ div_term,
-                                                                    const __half* __restrict__ img_hi, const __half* __restrict__ img_lo,
-                                                                    const float* __restrict__ bias_sum, const float* __restrict__ scale,
-                                                                    float* __restrict__ E) {
-    constexpr int NSTAGE = F16_NSTAGE;
-    constexpr int CP = CC / KC16;                         // chunks per part (angle, distance)
-    constexpr int NCH = 2 * CP;                           // K chunks per tile
-    constexpr int BB = CC * 128;                          // bytes of one B chunk (CC rows x 64 halves)
-    constexpr int STB = 2 * (A_BYTES + BB);               // stage: hi + lo of both operands
-    constexpr uint32_t IDESC = (1u << 4) | ((uint32_t)(CC >> 3) << 17) | ((uint32_t)(ROWS >> 4) << 24);
-    extern __shared__ unsigned char smem_raw[];
-    unsigned char* smem = (unsigned char*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    float* xstage = (float*)(smem + NSTAGE * STB);
-    uint64_t* bars = (uint64_t*)(xstage + ROWS * STAGE_LD);
-    uint64_t* full = bars;
-    uint64_t* empty = bars + NSTAGE;
-    uint64_t* tfull = bars + 2 * NSTAGE;
-    uint64_t* tempty = tfull + 2;
-    uint32_t* tmem_slot = (uint32_t*)(tempty + 2);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const long long n_tiles = (n_pairs + PAIRS - 1) / PAIRS;
+// 3xFP16: x = x_hi + x_lo with x_hi = fp16(x), x_lo = fp16(x - x_hi).  fp16 carries the same 11 significant bits as tf32, so
+// hi.hi + hi.lo + lo.hi has the same ~2^-22 relative accuracy as 3xTF32, but an fp16 wgmma consumes K = 16 per instruction at
+// the rate a tf32 one consumes K = 8: half the tensor-pipe time, half the B bytes, half the generator stores.  The sinusoids are
+// in [-1, 1] (lo <= 2^-12: fp16 subnormal spacing 6e-8 = fp32 epsilon); the weights are pre-scaled by a power of two to
+// [0.5, 1) (exact), undone in the epilogue.
+template <int CC, bool F16, int NPASS>
+struct Cfg {
+    static constexpr int KCH = F16 ? KC16 : KC;            // K elements per chunk
+    static constexpr int CP = CC / KCH;                    // chunks per part (angle, distance)
+    static constexpr int NCH = 2 * CP;                     // K chunks per tile
+    static constexpr int BB = CC * 128;                    // bytes of one B chunk
+    static constexpr int NPART = NPASS == 3 ? 2 : 1;       // hi (+ lo) of each operand
+    static constexpr int A_PART = NPART * A_BYTES;
+    static constexpr int STAGE_BYTES = NPART * (A_BYTES + BB);
+    static constexpr int NSTAGE = NPASS == 3 ? 2 : 4;
+    static constexpr int SMEM = NSTAGE * STAGE_BYTES + ROWS * STAGE_LD * 4 + 1024 /*alignment slack*/ + 256 /*barriers*/;
+};
 
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < NSTAGE; ++s) { mbar_init(&full[s], NGEN_WARPS + 1); mbar_init(&empty[s], 1); }
-        for (int a = 0; a < 2; ++a) { mbar_init(&tfull[a], 1); mbar_init(&tempty[a], 4); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == NGEN_WARPS + 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(2 * CC) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp < NGEN_WARPS) {
-        {   // zero the two padding rows (126, 127) of every A buffer once
-            for (int e = threadIdx.x; e < NSTAGE * 2 * 64; e += NGEN_WARPS * 32) {
-                const int sidx = e / 128, rem = e % 128, part = rem / 64, w = rem % 64;
-                float* base = (float*)(smem + sidx * STB + part * A_BYTES + 15 * 1024 + 6 * 128);
-                base[w] = 0.f;
-            }
-            asm volatile("bar.sync 2, %0;" ::"n"(NGEN_WARPS * 32) : "memory");
-        }
-        int s = 0;
-        uint32_t ph = 0;
-        for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-            const long long p0 = tile * PAIRS;
-            for (int kc = 0; kc < NCH; ++kc) {
-                mbar_wait(&empty[s], ph ^ 1u);
-                unsigned char* st = smem + s * STB;
-                const int f0 = (kc % CP) * 32;               // 32 frequencies (64 halves) per chunk
-                const bool angle = kc < CP;
-                const int n_items = (angle ? 3 * PAIRS : PAIRS) * 8;
-                for (int it = threadIdx.x; it < n_items; it += NGEN_WARPS * 32) {
-                    const int c = it & 7, rr = it >> 3;     // 16-byte chunk c = frequencies f0+4c .. f0+4c+3
-                    const int j = angle ? (rr % PAIRS) : rr;
-                    const long long p = p0 + j;
-                    float x = 0.f;
-                    if (p < n_pairs) x = angle ? __ldg(a_idx + p * 3 + rr / PAIRS) : __ldg(d_idx + p);
-                    float v[8];
+// one 16-byte unit c (of 8 per 128-byte row) of the sinusoid row for argument x: tf32 = frequencies f0 + 2c, f0 + 2c + 1
+// (sin, cos interleaved), fp16 = frequencies f0 + 4c .. f0 + 4c + 3; hi part and (3-pass) lo part
+template <bool F16, int NPASS>
+__device__ __forceinline__ void gen_unit(float x, const float* __restrict__ div_term, int f0, int c, uint4& hv, uint4& lv) {
+    if constexpr (F16) {
+        float v[8];
 #pragma unroll
-                    for (int u = 0; u < 4; ++u) sincos_sfu(__fmul_rn(x, __ldg(div_term + f0 + 4 * c + u)), v[2 * u], v[2 * u + 1]);
-                    __half2 hi[4], lo[4];
+        for (int u = 0; u < 4; ++u) sincos_sfu(__fmul_rn(x, __ldg(div_term + f0 + 4 * c + u)), v[2 * u], v[2 * u + 1]);
+        __half2 hi[4], lo[4];
 #pragma unroll
-                    for (int u = 0; u < 4; ++u) {
-                        const __half h0 = __float2half_rn(v[2 * u]), h1 = __float2half_rn(v[2 * u + 1]);
-                        hi[u] = __halves2half2(h0, h1);
-                        lo[u] = __halves2half2(__float2half_rn(v[2 * u] - __half2float(h0)), __float2half_rn(v[2 * u + 1] - __half2float(h1)));
-                    }
-                    const uint4 hv = make_uint4(*reinterpret_cast<uint32_t*>(&hi[0]), *reinterpret_cast<uint32_t*>(&hi[1]),
-                                                *reinterpret_cast<uint32_t*>(&hi[2]), *reinterpret_cast<uint32_t*>(&hi[3]));
-                    const uint4 lv = make_uint4(*reinterpret_cast<uint32_t*>(&lo[0]), *reinterpret_cast<uint32_t*>(&lo[1]),
-                                                *reinterpret_cast<uint32_t*>(&lo[2]), *reinterpret_cast<uint32_t*>(&lo[3]));
-                    const int nrep = angle ? 1 : 3;
-                    for (int rep = 0; rep < nrep; ++rep) {
-                        const int r = angle ? rr : (rep * PAIRS + j);
-                        const uint32_t off = (uint32_t)((r >> 3) * 1024 + (r & 7) * 128 + ((c ^ (r & 7)) << 4));
-                        *reinterpret_cast<uint4*>(st + off) = hv;
-                        *reinterpret_cast<uint4*>(st + A_BYTES + off) = lv;
-                    }
-                }
-                fence_proxy_async();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&full[s]);
-                if (++s == NSTAGE) { s = 0; ph ^= 1u; }
-            }
+        for (int u = 0; u < 4; ++u) {
+            const __half h0 = __float2half_rn(v[2 * u]), h1 = __float2half_rn(v[2 * u + 1]);
+            hi[u] = __halves2half2(h0, h1);
+            lo[u] = __halves2half2(__float2half_rn(v[2 * u] - __half2float(h0)), __float2half_rn(v[2 * u + 1] - __half2float(h1)));
         }
-    } else if (warp == NGEN_WARPS) {
-        if (lane == 0) {
-            int s = 0;
-            uint32_t ph = 0;
-            for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-                for (int kc = 0; kc < NCH; ++kc) {
-                    mbar_wait(&empty[s], ph ^ 1u);
-                    unsigned char* st = smem + s * STB;
-                    mbar_arrive_expect_tx(&full[s], 2 * BB);
-                    bulk_g2s(st + 2 * A_BYTES, img_hi + (size_t)kc * (CC * KC16), BB, &full[s]);
-                    bulk_g2s(st + 2 * A_BYTES + BB, img_lo + (size_t)kc * (CC * KC16), BB, &full[s]);
-                    if (++s == NSTAGE) { s = 0; ph ^= 1u; }
-                }
-            }
-        }
-    } else if (warp == NGEN_WARPS + 1) {
-        if (lane == 0) {
-            int s = 0;
-            uint32_t ph = 0;
-            int acc = 0;
-            uint32_t acc_ph[2] = {0, 0};
-            for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-                mbar_wait(&tempty[acc], acc_ph[acc] ^ 1u);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t)(acc * CC);
-                for (int kc = 0; kc < NCH; ++kc) {
-                    mbar_wait(&full[s], ph);
-                    tc_fence_after();
-                    const uint32_t st = smem_u32(smem + s * STB);
-                    const uint64_t da_hi = make_desc(st), da_lo = make_desc(st + A_BYTES);
-                    const uint64_t db_hi = make_desc(st + 2 * A_BYTES), db_lo = make_desc(st + 2 * A_BYTES + BB);
-#pragma unroll
-                    for (int kk = 0; kk < KC16 / 16; ++kk) {        // 4 MMAs of K = 16 (32 bytes) per operand pair
-                        const uint64_t adv = (uint64_t)(kk * 2);
-                        umma_f16(d_tmem, da_hi + adv, db_hi + adv, (kc == 0 && kk == 0) ? 0u : 1u, IDESC);
-                        umma_f16(d_tmem, da_hi + adv, db_lo + adv, 1u, IDESC);
-                        umma_f16(d_tmem, da_lo + adv, db_hi + adv, 1u, IDESC);
-                    }
-                    umma_commit(&empty[s]);
-                    if (++s == NSTAGE) { s = 0; ph ^= 1u; }
-                }
-                umma_commit(&tfull[acc]);
-                acc_ph[acc] ^= 1u;
-                acc ^= 1;
-            }
-        }
+        hv = make_uint4(*reinterpret_cast<uint32_t*>(&hi[0]), *reinterpret_cast<uint32_t*>(&hi[1]), *reinterpret_cast<uint32_t*>(&hi[2]),
+                        *reinterpret_cast<uint32_t*>(&hi[3]));
+        lv = make_uint4(*reinterpret_cast<uint32_t*>(&lo[0]), *reinterpret_cast<uint32_t*>(&lo[1]), *reinterpret_cast<uint32_t*>(&lo[2]),
+                        *reinterpret_cast<uint32_t*>(&lo[3]));
     } else {
-        const int q = warp & 3;
-        const int et = (warp - (NGEN_WARPS + 2)) * 32 + lane;
-        const float inv_scale = scale[1];
-        int acc = 0;
-        uint32_t acc_ph[2] = {0, 0};
-        for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-            mbar_wait(&tfull[acc], acc_ph[acc]);
-            tc_fence_after();
-            const long long p0 = tile * PAIRS;
-            for (int cc = 0; cc < CC / 32; ++cc) {
-                uint32_t v[32];
-                const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * CC + cc * 32);
-                asm volatile(
-                    "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                    "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                    "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                    : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-                      "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-                      "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-                      "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-                    : "r"(taddr));
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                float* xr = xstage + (q * 32 + lane) * STAGE_LD;
-#pragma unroll
-                for (int c = 0; c < 32; ++c) xr[c] = __uint_as_float(v[c]);
-                asm volatile("bar.sync 1, 128;" ::: "memory");
-                for (int idx = et; idx < PAIRS * 32; idx += 128) {
-                    const int jj = idx >> 5, c = idx & 31;
-                    const long long p = p0 + jj;
-                    if (p < n_pairs) {
-                        const float m = fmaxf(fmaxf(xstage[jj * STAGE_LD + c], xstage[(PAIRS + jj) * STAGE_LD + c]),
-                                              xstage[(2 * PAIRS + jj) * STAGE_LD + c]);
-                        E[p * CC + cc * 32 + c] = fmaf(m, inv_scale, __ldg(bias_sum + cc * 32 + c));
-                    }
-                }
-                asm volatile("bar.sync 1, 128;" ::: "memory");
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tempty[acc]);
-            acc_ph[acc] ^= 1u;
-            acc ^= 1;
+        float s0, c0, s1, c1;
+        sincos_cw(__fmul_rn(x, __ldg(div_term + f0 + 2 * c)), s0, c0);
+        sincos_cw(__fmul_rn(x, __ldg(div_term + f0 + 2 * c + 1)), s1, c1);
+        float4 hi = make_float4(s0, c0, s1, c1), lo = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (NPASS == 3) {
+            hi.x = tf32_rn(s0); lo.x = s0 - hi.x;
+            hi.y = tf32_rn(c0); lo.y = c0 - hi.y;
+            hi.z = tf32_rn(s1); lo.z = s1 - hi.z;
+            hi.w = tf32_rn(c1); lo.w = c1 - hi.w;
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == NGEN_WARPS + 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(2 * CC) : "memory");
+        hv = *reinterpret_cast<uint4*>(&hi);
+        lv = *reinterpret_cast<uint4*>(&lo);
     }
 }
 
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NTHREADS, 1) gse_embed_f16_cluster_kernel(const float* __restrict__ d_idx, const float* __restrict__ a_idx,
-                                                                    long long n_pairs, const float* __restrict__ div_term,
-                                                                    const __half* __restrict__ img_hi, const __half* __restrict__ img_lo,
-                                                                    const float* __restrict__ bias_sum, const float* __restrict__ scale,
-                                                                    float* __restrict__ E) {
-    constexpr int NSTAGE = F16_NSTAGE;
+template <bool F16, int N>
+__device__ __forceinline__ void mma(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t acc) {
+    if constexpr (F16) wgmma_f16<N>(d, da, db, acc);
+    else wgmma_tf32<N>(d, da, db, acc);
+}
+
+// img_hi / img_lo: B images (float for tf32, __half for fp16); scale: fp16 weight scale (scale[1] undoes it), nullptr for tf32.
+// CLUSTER: the two CTAs of a cluster advance in lockstep and each streams one of the two B images into both.
+template <int CC, bool F16, int NPASS, bool CLUSTER>
+__device__ __forceinline__ void gse_embed_body(const float* __restrict__ d_idx, const float* __restrict__ a_idx, long long n_pairs,
+                                               const float* __restrict__ div_term, const void* __restrict__ img_hi,
+                                               const void* __restrict__ img_lo, const float* __restrict__ bias_sum,
+                                               const float* __restrict__ scale, float* __restrict__ E) {
+    using CF = Cfg<CC, F16, NPASS>;
+    constexpr int NSTAGE = CF::NSTAGE, R = CC / 2;
     extern __shared__ unsigned char smem_raw[];
-    unsigned char* smem = (unsigned char*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    float* xstage = (float*)(smem + NSTAGE * F16_STAGE_BYTES);
+    unsigned char* smem = (unsigned char*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);   // SWIZZLE_128B: 1024 B alignment
+    float* xstage = (float*)(smem + NSTAGE * CF::STAGE_BYTES);                                   // [128][33]
     uint64_t* bars = (uint64_t*)(xstage + ROWS * STAGE_LD);
-    uint64_t* full = bars;
-    uint64_t* empty = bars + NSTAGE;
-    uint64_t* tfull = bars + 2 * NSTAGE;
-    uint64_t* tempty = tfull + 2;
-    uint64_t* peer_empty = tempty + 2;     // [NSTAGE]: the peer CTA's stage is free (remote arrive)
-    uint32_t* tmem_slot = (uint32_t*)(peer_empty + NSTAGE);
+    uint64_t* full = bars;                      // [NSTAGE] A generated + B landed
+    uint64_t* empty = bars + NSTAGE;            // [NSTAGE] both consumer warpgroups are done with the stage
+    uint64_t* peer_empty = bars + 2 * NSTAGE;   // [NSTAGE] (cluster) the peer CTA's stage is free (remote arrive)
+
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const long long n_tiles = (n_pairs + PAIRS - 1) / PAIRS;
-    // the two CTAs of a cluster advance in lockstep (they share every B chunk): same number of tile slots for everybody
-    const long long n_iters = (n_tiles + gridDim.x - 1) / gridDim.x;
-    uint32_t cta_rank;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(cta_rank));
+    // cluster: same number of tile slots for every CTA; slots past n_tiles are idle, the pipeline still runs
+    const long long tile_end = CLUSTER ? (n_tiles + gridDim.x - 1) / gridDim.x * gridDim.x : n_tiles;
+    uint32_t cta_rank = 0;
+    if (CLUSTER) asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(cta_rank));
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < NSTAGE; ++s) { mbar_init(&full[s], NGEN_WARPS + 1); mbar_init(&empty[s], 1); mbar_init(&peer_empty[s], 1); }
-        for (int a = 0; a < 2; ++a) { mbar_init(&tfull[a], 1); mbar_init(&tempty[a], 4); }
+        for (int s = 0; s < NSTAGE; ++s) { mbar_init(&full[s], NGEN_WARPS + 1); mbar_init(&empty[s], NCONS_WARPS); mbar_init(&peer_empty[s], 1); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == NGEN_WARPS + 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(tmem_slot)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");   // peer barriers are initialised
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
+    if (CLUSTER) asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 
-    if (warp < NGEN_WARPS) {
-        {   // zero the two padding rows (126, 127) of every A buffer once
-            for (int e = threadIdx.x; e < NSTAGE * 2 * 64; e += NGEN_WARPS * 32) {
-                const int sidx = e / 128, rem = e % 128, part = rem / 64, w = rem % 64;
-                float* base = (float*)(smem + sidx * F16_STAGE_BYTES + part * A_BYTES + 15 * 1024 + 6 * 128);
-                base[w] = 0.f;
+    if (warp >= NCONS_WARPS) {
+        // ===================== generators (+ B copier) =====================
+        const int gt = threadIdx.x - NCONS_WARPS * 32;
+        {   // padding rows 126,127 of every A buffer: zero once (their outputs are never read)
+            for (int e = gt; e < NSTAGE * CF::NPART * 64; e += NGEN_WARPS * 32) {
+                const int sidx = e / (CF::NPART * 64), rem = e % (CF::NPART * 64);
+                float* base = (float*)(smem + sidx * CF::STAGE_BYTES + (rem / 64) * A_BYTES + 15 * 1024 + 6 * 128);
+                base[rem % 64] = 0.f;
             }
             asm volatile("bar.sync 2, %0;" ::"n"(NGEN_WARPS * 32) : "memory");
         }
         int s = 0;
         uint32_t ph = 0;
-        for (long long itile = 0; itile < n_iters; ++itile) {
-            const long long tile = itile * gridDim.x + blockIdx.x;   // tile >= n_tiles: idle slot, pipeline still runs
+        for (long long tile = blockIdx.x; tile < tile_end; tile += gridDim.x) {
             const long long p0 = tile * PAIRS;
-            for (int kc = 0; kc < NCHUNK16; ++kc) {
+            for (int kc = 0; kc < CF::NCH; ++kc) {
                 mbar_wait(&empty[s], ph ^ 1u);
-                unsigned char* st = smem + s * F16_STAGE_BYTES;
-                const int f0 = (kc & 3) * 32;               // 32 frequencies (64 halves) per chunk
-                const bool angle = kc < 4;
+                unsigned char* st = smem + s * CF::STAGE_BYTES;
+                if (gt == 0) {
+                    const size_t off = (size_t)kc * CF::BB;
+                    const unsigned char* hi = (const unsigned char*)img_hi + off;
+                    const unsigned char* lo = (const unsigned char*)img_lo + off;
+                    if (CLUSTER) {
+                        // tell the peer its copy into my stage may start, then wait until the peer's stage s is free too;
+                        // rank 0 streams the hi image, rank 1 the lo image, each multicast into both CTAs: every B byte leaves
+                        // L2 once per CTA pair instead of once per CTA
+                        uint32_t raddr;
+                        asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(raddr) : "r"(smem_u32(&peer_empty[s])), "r"(cta_rank ^ 1u));
+                        asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(raddr) : "memory");
+                        mbar_wait_cluster(&peer_empty[s], ph);
+                        mbar_arrive_expect_tx(&full[s], 2 * CF::BB);       // both halves land here (mine + the peer's multicast)
+                        asm volatile(
+                            "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;" ::"r"(
+                                smem_u32(st + CF::A_PART + (cta_rank == 0 ? 0 : CF::BB))),
+                            "l"(cta_rank == 0 ? hi : lo), "r"((uint32_t)CF::BB), "r"(smem_u32(&full[s])), "h"((unsigned short)3)
+                            : "memory");
+                    } else {
+                        mbar_arrive_expect_tx(&full[s], CF::NPART * CF::BB);
+                        bulk_g2s(st + CF::A_PART, hi, CF::BB, &full[s]);
+                        if (NPASS == 3) bulk_g2s(st + CF::A_PART + CF::BB, lo, CF::BB, &full[s]);
+                    }
+                }
+                // work item = (tile row, 16-byte unit c).  Angle chunks (kc < CP) have 126 x 8 items; distance chunks have
+                // 42 x 8 items whose result is stored to the three rows (k = 0,1,2) of the pair.
+                const int f0 = (kc % CF::CP) * (CF::KCH / 2);
+                const bool angle = kc < CF::CP;
                 const int n_items = (angle ? 3 * PAIRS : PAIRS) * 8;
-                for (int it = threadIdx.x; it < n_items; it += NGEN_WARPS * 32) {
-                    const int c = it & 7, rr = it >> 3;     // 16-byte chunk c = frequencies f0+4c .. f0+4c+3
+                for (int it = gt; it < n_items; it += NGEN_WARPS * 32) {
+                    const int c = it & 7, rr = it >> 3;          // rr: tile row (angle) or pair slot (distance)
                     const int j = angle ? (rr % PAIRS) : rr;
                     const long long p = p0 + j;
                     float x = 0.f;
                     if (p < n_pairs) x = angle ? __ldg(a_idx + p * 3 + rr / PAIRS) : __ldg(d_idx + p);
-                    float v[8];
-#pragma unroll
-                    for (int u = 0; u < 4; ++u) sincos_sfu(__fmul_rn(x, __ldg(div_term + f0 + 4 * c + u)), v[2 * u], v[2 * u + 1]);
-                    __half2 hi[4], lo[4];
-#pragma unroll
-                    for (int u = 0; u < 4; ++u) {
-                        const __half h0 = __float2half_rn(v[2 * u]), h1 = __float2half_rn(v[2 * u + 1]);
-                        hi[u] = __halves2half2(h0, h1);
-                        lo[u] = __halves2half2(__float2half_rn(v[2 * u] - __half2float(h0)), __float2half_rn(v[2 * u + 1] - __half2float(h1)));
-                    }
-                    const uint4 hv = make_uint4(*reinterpret_cast<uint32_t*>(&hi[0]), *reinterpret_cast<uint32_t*>(&hi[1]),
-                                                *reinterpret_cast<uint32_t*>(&hi[2]), *reinterpret_cast<uint32_t*>(&hi[3]));
-                    const uint4 lv = make_uint4(*reinterpret_cast<uint32_t*>(&lo[0]), *reinterpret_cast<uint32_t*>(&lo[1]),
-                                                *reinterpret_cast<uint32_t*>(&lo[2]), *reinterpret_cast<uint32_t*>(&lo[3]));
+                    uint4 hv, lv;
+                    gen_unit<F16, NPASS>(x, div_term, f0, c, hv, lv);
                     const int nrep = angle ? 1 : 3;
                     for (int rep = 0; rep < nrep; ++rep) {
                         const int r = angle ? rr : (rep * PAIRS + j);
                         const uint32_t off = (uint32_t)((r >> 3) * 1024 + (r & 7) * 128 + ((c ^ (r & 7)) << 4));
                         *reinterpret_cast<uint4*>(st + off) = hv;
-                        *reinterpret_cast<uint4*>(st + A_BYTES + off) = lv;
+                        if (NPASS == 3) *reinterpret_cast<uint4*>(st + A_BYTES + off) = lv;
                     }
                 }
-                fence_proxy_async();
+                fence_proxy_async();               // generic-proxy stores -> visible to the tensor core (async proxy)
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&full[s]);
                 if (++s == NSTAGE) { s = 0; ph ^= 1u; }
             }
         }
-    } else if (warp == NGEN_WARPS) {
-        if (lane == 0) {
-            // B copier: rank 0 streams the hi image, rank 1 the lo image, each MULTICAST into both CTAs of the cluster
-            // (cp.async.bulk ... .multicast::cluster): every B byte leaves L2 once per CTA pair instead of once per CTA.
-            const uint32_t peer = cta_rank ^ 1u;
-            int s = 0;
-            uint32_t ph = 0;
-            for (long long itile = 0; itile < n_iters; ++itile) {
-                for (int kc = 0; kc < NCHUNK16; ++kc) {
-                    mbar_wait(&empty[s], ph ^ 1u);                         // my MMAs are done with stage s
-                    {   // tell the peer, then wait until the peer's stage s is free too
-                        uint32_t raddr;
-                        asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(raddr) : "r"(smem_u32(&peer_empty[s])), "r"(peer));
-                        asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(raddr) : "memory");
-                    }
-                    mbar_wait_cluster(&peer_empty[s], ph);
-                    unsigned char* st = smem + s * F16_STAGE_BYTES;
-                    mbar_arrive_expect_tx(&full[s], 2 * B_BYTES);          // both halves land here (mine + the peer's multicast)
-                    const __half* src = (cta_rank == 0 ? img_hi : img_lo) + (size_t)kc * (C * KC16);
-                    unsigned char* dst = st + 2 * A_BYTES + (cta_rank == 0 ? 0 : B_BYTES);
-                    asm volatile(
-                        "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;" ::"r"(
-                            smem_u32(dst)),
-                        "l"(src), "r"((uint32_t)B_BYTES), "r"(smem_u32(&full[s])), "h"((unsigned short)3)
-                        : "memory");
-                    if (++s == NSTAGE) { s = 0; ph ^= 1u; }
-                }
-            }
-        }
-    } else if (warp == NGEN_WARPS + 1) {
-        if (lane == 0) {
-            int s = 0;
-            uint32_t ph = 0;
-            int acc = 0;
-            uint32_t acc_ph[2] = {0, 0};
-            for (long long itile = 0; itile < n_iters; ++itile) {
-                // slots with itile * gridDim.x + blockIdx.x >= n_tiles are idle, the pipeline still runs
-                mbar_wait(&tempty[acc], acc_ph[acc] ^ 1u);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t)(acc * C);
-                for (int kc = 0; kc < NCHUNK16; ++kc) {
-                    mbar_wait(&full[s], ph);
-                    tc_fence_after();
-                    const uint32_t st = smem_u32(smem + s * F16_STAGE_BYTES);
-                    const uint64_t da_hi = make_desc(st), da_lo = make_desc(st + A_BYTES);
-                    const uint64_t db_hi = make_desc(st + 2 * A_BYTES), db_lo = make_desc(st + 2 * A_BYTES + B_BYTES);
-#pragma unroll
-                    for (int kk = 0; kk < KC16 / 16; ++kk) {        // 4 MMAs of K = 16 (32 bytes) per operand pair
-                        const uint64_t adv = (uint64_t)(kk * 2);
-                        umma_f16(d_tmem, da_hi + adv, db_hi + adv, (kc == 0 && kk == 0) ? 0u : 1u);
-                        umma_f16(d_tmem, da_hi + adv, db_lo + adv, 1u);
-                        umma_f16(d_tmem, da_lo + adv, db_hi + adv, 1u);
-                    }
-                    umma_commit(&empty[s]);
-                    if (++s == NSTAGE) { s = 0; ph ^= 1u; }
-                }
-                umma_commit(&tfull[acc]);
-                acc_ph[acc] ^= 1u;
-                acc ^= 1;
-            }
-        }
     } else {
-        const int q = warp & 3;
-        const int et = (warp - (NGEN_WARPS + 2)) * 32 + lane;
-        const float inv_scale = scale[1];
-        int acc = 0;
-        uint32_t acc_ph[2] = {0, 0};
-        for (long long itile = 0; itile < n_iters; ++itile) {
-            const long long tile = itile * gridDim.x + blockIdx.x;   // tile >= n_tiles: idle slot, pipeline still runs
-            mbar_wait(&tfull[acc], acc_ph[acc]);
-            tc_fence_after();
-            const long long p0 = tile * PAIRS;
-            for (int cc = 0; cc < C / 32; ++cc) {
-                uint32_t v[32];
-                const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * C + cc * 32);
-                asm volatile(
-                    "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                    "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                    "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                    : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-                      "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-                      "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-                      "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-                    : "r"(taddr));
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                float* xr = xstage + (q * 32 + lane) * STAGE_LD;
+        // ===================== consumers =====================
+        const int wg = warp >> 2, wq = warp & 3;
+        const float inv_scale = F16 ? scale[1] : 1.0f;
+        int s = 0;
+        uint32_t ph = 0;
+        for (long long tile = blockIdx.x; tile < tile_end; tile += gridDim.x) {
+            float acc[R];
 #pragma unroll
-                for (int c = 0; c < 32; ++c) xr[c] = __uint_as_float(v[c]);
-                asm volatile("bar.sync 1, 128;" ::: "memory");
-                for (int idx = et; idx < PAIRS * 32; idx += 128) {
-                    const int jj = idx >> 5, c = idx & 31;
-                    const long long p = p0 + jj;
-                    if (p < n_pairs) {
-                        const float m = fmaxf(fmaxf(xstage[jj * STAGE_LD + c], xstage[(PAIRS + jj) * STAGE_LD + c]),
-                                              xstage[(2 * PAIRS + jj) * STAGE_LD + c]);
-                        E[p * C + cc * 32 + c] = fmaf(m, inv_scale, __ldg(bias_sum + cc * 32 + c));
+            for (int i = 0; i < R; ++i) acc[i] = 0.f;
+            int prev_s = -1;
+            for (int kc = 0; kc < CF::NCH; ++kc) {
+                mbar_wait(&full[s], ph);
+                const uint32_t st = smem_u32(smem + s * CF::STAGE_BYTES);
+                const uint64_t da_hi = make_desc(st + wg * (A_BYTES / 2)), da_lo = make_desc(st + A_BYTES + wg * (A_BYTES / 2));
+                const uint64_t db_hi = make_desc(st + CF::A_PART), db_lo = make_desc(st + CF::A_PART + CF::BB);
+                wgmma_fence();
+#pragma unroll
+                for (int kk = 0; kk < 4; ++kk) {       // 4 MMAs of 32 bytes of K per 128-byte chunk
+                    const uint64_t adv = (uint64_t)(kk * 2);
+                    mma<F16, CC>(acc, da_hi + adv, db_hi + adv, (kc == 0 && kk == 0) ? 0u : 1u);
+                    if (NPASS == 3) {
+                        mma<F16, CC>(acc, da_hi + adv, db_lo + adv, 1u);
+                        mma<F16, CC>(acc, da_lo + adv, db_hi + adv, 1u);
                     }
                 }
-                asm volatile("bar.sync 1, 128;" ::: "memory");
+                wgmma_commit();
+                wgmma_wait<1>();                     // the previous chunk's MMAs are done: its stage can be refilled
+                if (prev_s >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty[prev_s]); }
+                prev_s = s;
+                if (++s == NSTAGE) { s = 0; ph ^= 1u; }
             }
-            tc_fence_before();
+            wgmma_wait<0>();
+            reg_fence(acc);
             __syncwarp();
-            if (lane == 0) mbar_arrive(&tempty[acc]);
-            acc_ph[acc] ^= 1u;
-            acc ^= 1;
+            if (lane == 0) mbar_arrive(&empty[prev_s]);
+
+            // epilogue, 32 columns at a time: fragment rows rl, rl + 8, columns 8j + 2(lane % 4) + {0, 1}
+            const long long p0 = tile * PAIRS;
+            const int rl = wg * 64 + wq * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+#pragma unroll
+            for (int cc = 0; cc < CC / 32; ++cc) {
+#pragma unroll
+                for (int jj = 0; jj < 4; ++jj) {
+                    const int j = 4 * cc + jj;
+                    xstage[rl * STAGE_LD + 8 * jj + c0] = acc[4 * j];
+                    xstage[rl * STAGE_LD + 8 * jj + c0 + 1] = acc[4 * j + 1];
+                    xstage[(rl + 8) * STAGE_LD + 8 * jj + c0] = acc[4 * j + 2];
+                    xstage[(rl + 8) * STAGE_LD + 8 * jj + c0 + 1] = acc[4 * j + 3];
+                }
+                asm volatile("bar.sync 1, %0;" ::"n"(NCONS_WARPS * 32) : "memory");
+                for (int idx = threadIdx.x; idx < PAIRS * 32; idx += NCONS_WARPS * 32) {
+                    const int jp = idx >> 5, c = idx & 31;
+                    const long long p = p0 + jp;
+                    if (p < n_pairs) {
+                        const float m = fmaxf(fmaxf(xstage[jp * STAGE_LD + c], xstage[(PAIRS + jp) * STAGE_LD + c]),
+                                              xstage[(2 * PAIRS + jp) * STAGE_LD + c]);
+                        E[p * CC + cc * 32 + c] = fmaf(m, inv_scale, __ldg(bias_sum + cc * 32 + c));
+                    }
+                }
+                asm volatile("bar.sync 1, %0;" ::"n"(NCONS_WARPS * 32) : "memory");
+            }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");   // no CTA leaves while its peer may still write to it
-    if (warp == NGEN_WARPS + 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
-    }
+    // no CTA leaves while its peer may still write to it
+    if (CLUSTER) asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+
+template <int CC, bool F16, int NPASS>
+__global__ void __launch_bounds__(NTHREADS, 1) gse_embed_kernel(const float* __restrict__ d_idx, const float* __restrict__ a_idx,
+                                                                long long n_pairs, const float* __restrict__ div_term,
+                                                                const void* __restrict__ img_hi, const void* __restrict__ img_lo,
+                                                                const float* __restrict__ bias_sum, const float* __restrict__ scale,
+                                                                float* __restrict__ E) {
+    gse_embed_body<CC, F16, NPASS, false>(d_idx, a_idx, n_pairs, div_term, img_hi, img_lo, bias_sum, scale, E);
+}
+
+__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NTHREADS, 1)
+    gse_embed_f16_cluster_kernel(const float* __restrict__ d_idx, const float* __restrict__ a_idx, long long n_pairs,
+                                 const float* __restrict__ div_term, const void* __restrict__ img_hi, const void* __restrict__ img_lo,
+                                 const float* __restrict__ bias_sum, const float* __restrict__ scale, float* __restrict__ E) {
+    gse_embed_body<C, true, 3, true>(d_idx, a_idx, n_pairs, div_term, img_hi, img_lo, bias_sum, scale, E);
 }
 
 }  // namespace tc
@@ -844,8 +395,8 @@ int geob200_gse_embed_tc(const float* d_idx, const float* a_idx, long long n_pai
         const int grid = (int)(n_tiles < (long long)num_sms() ? n_tiles : (long long)num_sms());
         tc::gse_absmax_kernel<CC><<<1, 1024, 0, st>>>(Wd, Wa, scale);
         tc::gse_pack_b_f16_kernel<CC><<<(unsigned)((img_halves + 255) / 256), 256, 0, st>>>(Wd, Wa, bd, ba, scale, h_hi, h_lo, bsum);
-        if (ensure_max_smem((const void*)tc::gse_embed_f16_kernel<CC>)) return -1;
-        tc::gse_embed_f16_kernel<CC><<<grid, tc::NTHREADS, tc::F16_SMEM, st>>>(d_idx, a_idx, n_pairs, div_term, h_hi, h_lo, bsum, scale, E);
+        if (ensure_max_smem((const void*)tc::gse_embed_kernel<CC, true, 3>)) return -1;
+        tc::gse_embed_kernel<CC, true, 3><<<grid, tc::NTHREADS, tc::Cfg<CC, true, 3>::SMEM, st>>>(d_idx, a_idx, n_pairs, div_term, h_hi, h_lo, bsum, scale, E);
         GEOB_CHECK_LAUNCH();
         count_launches(3);
         return 0;
@@ -866,24 +417,26 @@ int geob200_gse_embed_tc(const float* d_idx, const float* a_idx, long long n_pai
         float* scale = bsum + tc::C;
         tc::gse_absmax_kernel<tc::C><<<1, 1024, 0, st>>>(Wd, Wa, scale);
         tc::gse_pack_b_f16_kernel<tc::C><<<(unsigned)((img_floats + 255) / 256), 256, 0, st>>>(Wd, Wa, bd, ba, scale, h_hi, h_lo, bsum);
-        if (ensure_max_smem((const void*)tc::gse_embed_f16_kernel<tc::C>) || ensure_max_smem((const void*)tc::gse_embed_f16_cluster_kernel)) return -1;
+        if (ensure_max_smem((const void*)tc::gse_embed_kernel<tc::C, true, 3>) || ensure_max_smem((const void*)tc::gse_embed_f16_cluster_kernel)) return -1;
         if (mode == 4) {
             // CTA pairs (cluster of 2) share every B chunk through TMA multicast; grid = even number of CTAs, one per SM
             int g2 = (int)((n_tiles + 1) / 2 < (long long)(num_sms() / 2) ? (n_tiles + 1) / 2 : (long long)(num_sms() / 2)) * 2;
-            tc::gse_embed_f16_cluster_kernel<<<g2, tc::NTHREADS, tc::F16_SMEM, st>>>(d_idx, a_idx, n_pairs, div_term, h_hi, h_lo, bsum, scale, E);
+            tc::gse_embed_f16_cluster_kernel<<<g2, tc::NTHREADS, tc::Cfg<tc::C, true, 3>::SMEM, st>>>(d_idx, a_idx, n_pairs, div_term, h_hi, h_lo, bsum, scale, E);
         } else
-            tc::gse_embed_f16_kernel<tc::C><<<grid, tc::NTHREADS, tc::F16_SMEM, st>>>(d_idx, a_idx, n_pairs, div_term, h_hi, h_lo, bsum, scale, E);
+            tc::gse_embed_kernel<tc::C, true, 3><<<grid, tc::NTHREADS, tc::Cfg<tc::C, true, 3>::SMEM, st>>>(d_idx, a_idx, n_pairs, div_term, h_hi, h_lo, bsum, scale, E);
         GEOB_CHECK_LAUNCH();
         count_launches(3);
         return 0;
     }
     tc::gse_pack_b_kernel<<<(unsigned)((img_floats + 255) / 256), 256, 0, st>>>(Wd, Wa, bd, ba, img_hi, img_lo, bias_sum);
     if (mode == 1) {
-        if (ensure_max_smem((const void*)tc::gse_embed_tc_kernel<3>)) return -1;
-        tc::gse_embed_tc_kernel<3><<<grid, tc::NTHREADS, tc::Cfg<3>::SMEM, st>>>(d_idx, a_idx, n_pairs, div_term, img_hi, img_lo, bias_sum, E);
+        if (ensure_max_smem((const void*)tc::gse_embed_kernel<tc::C, false, 3>)) return -1;
+        tc::gse_embed_kernel<tc::C, false, 3><<<grid, tc::NTHREADS, tc::Cfg<tc::C, false, 3>::SMEM, st>>>(d_idx, a_idx, n_pairs, div_term, img_hi,
+                                                                                                        img_lo, bias_sum, nullptr, E);
     } else {
-        if (ensure_max_smem((const void*)tc::gse_embed_tc_kernel<1>)) return -1;
-        tc::gse_embed_tc_kernel<1><<<grid, tc::NTHREADS, tc::Cfg<1>::SMEM, st>>>(d_idx, a_idx, n_pairs, div_term, img_hi, img_lo, bias_sum, E);
+        if (ensure_max_smem((const void*)tc::gse_embed_kernel<tc::C, false, 1>)) return -1;
+        tc::gse_embed_kernel<tc::C, false, 1><<<grid, tc::NTHREADS, tc::Cfg<tc::C, false, 1>::SMEM, st>>>(d_idx, a_idx, n_pairs, div_term, img_hi,
+                                                                                                        img_lo, bias_sum, nullptr, E);
     }
     GEOB_CHECK_LAUNCH();
     count_launches(2);

@@ -107,7 +107,7 @@ __global__ void __launch_bounds__(256) row_positive_kernel(const float* __restri
 // KPConv, stage 1 of 2 (tensor-core path): wf[m][k*Cin + c] = sum_h influence[m][h][k] * f[nbr[m][h]][c]   (kpconv.py:91-105)
 // One warp per query point, small shared-memory footprint (many resident warps hide the gather latency); the neighbour
 // rows are fetched eight at a time.  Also emits inv_count[m] = 1 / max(#neighbours with a positive feature sum, 1)
-// (kpconv.py:113-116).  Stage 2 is the 3xTF32 tcgen05 GEMM wf (M x 15 Cin) . W (15 Cin x Cout) with the per-row scale and the
+// (kpconv.py:113-116).  Stage 2 is the 3xTF32 wgmma GEMM wf (M x 15 Cin) . W (15 Cin x Cout) with the per-row scale and the
 // bias applied in its epilogue (linear_tc.cu).
 // CPL = channels per lane: 2 when Cin is a multiple of 64 (every broadcast read of an influence row then feeds 30 FMAs instead
 // of 15; with 15 the kernel is bound by the shared-memory pipe, 4 LDS.128 per 15 FMAs)
@@ -896,7 +896,7 @@ using namespace geob200;
 namespace geob200 {
 int linear_tc(const float* x, int64_t ldx, const float* w, int64_t ldw, const float* bias, const float* row_scale, float* y, int64_t ldy,
               int64_t m, int64_t n, int64_t k, int relu, cudaStream_t st, const GnFuse* gn = nullptr);   // linear_tc.cu
-static int g_linear_mode = 1;   // 1 = tcgen05 3xTF32 where the shape allows, 0 = fp32 CUDA cores only
+static int g_linear_mode = 1;   // 1 = wgmma 3xTF32 where the shape allows, 0 = fp32 CUDA cores only
 }
 
 extern "C" {
@@ -995,11 +995,11 @@ int geob200_linear_batched(const float* x, int64_t ldx, int64_t stride_x, const 
     }
     const unsigned z = (unsigned)batch;
     const long long c64 = ((n + 63) / 64) * ((m + 63) / 64) * batch, c6432 = ((n + 31) / 32) * ((m + 63) / 64) * batch;
-    if (c64 >= 148) {
+    if (c64 >= num_sms()) {
         dim3 grid((unsigned)((n + 63) / 64), (unsigned)((m + 63) / 64), z);
         linear_kernel<64, 64><<<grid, 256, 0, st>>>(x, (int)ldx, weight, (int)ldw, bias, y, (int)ldy, (int)m, (int)n, (int)k, relu,
                                                     stride_x, stride_w, stride_b, stride_y);
-    } else if (c6432 >= 148) {
+    } else if (c6432 >= num_sms()) {
         dim3 grid((unsigned)((n + 31) / 32), (unsigned)((m + 63) / 64), z);
         linear_kernel<64, 32><<<grid, 256, 0, st>>>(x, (int)ldx, weight, (int)ldw, bias, y, (int)ldy, (int)m, (int)n, (int)k, relu,
                                                     stride_x, stride_w, stride_b, stride_y);
@@ -1187,7 +1187,7 @@ int linear_group_norm_impl(const float* x, int64_t ldx, const float* weight, con
 
 extern "C" {
 
-// KPConv (gather + tcgen05 GEMM) -> GroupNorm (+ LeakyReLU): ConvBlock / the conv part of ResidualBlock (modules.py:107-147,205-207)
+// KPConv (gather + tensor-core GEMM) -> GroupNorm (+ LeakyReLU): ConvBlock / the conv part of ResidualBlock (modules.py:107-147,205-207)
 size_t geob200_kpconv_group_norm_workspace_bytes(int64_t n_query, int64_t n_support, int64_t c_in, int64_t c_out, int64_t groups) {
     return align_up(geob200_fused_group_norm_workspace_bytes(n_query, c_out, groups), 256) +
            geob200_kpconv_tc_workspace_bytes(n_query, n_support, c_in);

@@ -1,18 +1,19 @@
-// nn.Linear on the 5th-gen tensor cores: Y[M,N] = X[M,K] . W[N,K]^T + b (optional ReLU), fp32 in / fp32 out.
+// nn.Linear on the Hopper tensor cores (wgmma): Y[M,N] = X[M,K] . W[N,K]^T + b (optional ReLU), fp32 in / fp32 out.
 //
 // The reference's Linears are true fp32 (torch default allow_tf32=False), so the product is computed with the
 // error-compensated 3xTF32 scheme: x = x_hi + x_lo, w = w_hi + w_lo (hi = top 19 bits), D += x_hi w_hi + x_hi w_lo +
-// x_lo w_hi with fp32 accumulation in TMEM (~1e-6 relative, same as an fp32 FMA chain).
+// x_lo w_hi with fp32 accumulation (~1e-6 relative, same as an fp32 FMA chain).
 //
-// One CTA per 128 x BN output tile (BN = min(N,128)), K in chunks of 32 floats (one 128-byte swizzle row):
-//   warp 0      TMA producer : cp.async.bulk.tensor.2d (UTMALDG) of the raw X tile (128 x 32) and W tile (BN x 32) through
-//                              SWIZZLE_128B tensor maps; out-of-bounds rows/columns are zero-filled by the TMA unit
-//   warps 1-8   splitters    : in-place hi = tf32_rn(x), lo = x - hi into a second buffer (generic proxy ->
+// One 128 x BN output tile at a time (BN = min(N,128)), K in chunks of 32 floats (one 128-byte swizzle row); a CTA walks the
+// tiles t = blockIdx.x, blockIdx.x + gridDim.x, ... (one tile per CTA unless the persistent loop is on), 384 threads:
+//   warps 0-7   consumers    : two warpgroups, rows [0,64) and [64,128) of the tile: wgmma.m64n{BN}k8 tf32, 3 per K-step,
+//                              main products and corrections in two register accumulators; then the epilogue straight from
+//                              the registers (row scale, bias, ReLU, stores, optional GroupNorm statistics)
+//   warp 8      TMA producer : cp.async.bulk.tensor.2d of the raw X tile (128 x 32) and W tile (BN x 32) through SWIZZLE_128B
+//                              tensor maps; out-of-bounds rows/columns are zero-filled by the TMA unit
+//   warps 9-11  splitters    : in-place hi = tf32_rn(x), lo = x - hi into a second buffer (generic proxy ->
 //                              fence.proxy.async), so the MMA sees exact tf32 operands
-//   warp 9      MMA issuer   : tcgen05.mma.cta_group::1.kind::tf32 M128 N{BN} K8, 3 per K-step; tcgen05.commit frees the stage
-//   warps 10-13 epilogue     : tcgen05.ld 32x32b, + bias, ReLU, direct row-segment stores (each thread owns one output row);
-//                              optionally the GroupNorm statistics of the output (per-tile column sums through a transposing
-//                              warp butterfly, written as per-tile partials in double)
+// The operand ring runs across tile boundaries: the producer and splitters prepare the next tile while the consumers store.
 #include <cuda.h>
 
 #include <cstdlib>
@@ -21,9 +22,12 @@
 
 #include "common.cuh"
 #include "geob200.h"
+#include "hopper.cuh"
 
 namespace geob200 {
 namespace ltc {
+
+using namespace hop;
 
 constexpr int BM = 128;
 constexpr int KC = 32;
@@ -31,69 +35,19 @@ constexpr int TILE_A = BM * 128;       // 16 KB
 constexpr int TILE_B = 128 * 128;      // 16 KB (BN <= 128 rows)
 constexpr int STAGE = 2 * TILE_A + 2 * TILE_B;   // raw/hi + lo for both operands = 64 KB
 constexpr int NSTAGE = 3;
-constexpr int NSPLIT_WARPS = 8;                       // warps 1..8
-constexpr int MMA_WARP = 1 + NSPLIT_WARPS;            // warp 9
-constexpr int EPI_WARP0 = MMA_WARP + 1;               // warps 10..13 (warp & 3 covers the four TMEM lane quarters)
-constexpr int NTHREADS = (EPI_WARP0 + 4) * 32;        // 448
-// 193.25 KB + the 1 KB the system reserves per CTA fits the 196 KB shared-memory carve-out; anything larger forces the 228 KB
-// configuration and costs ~8 us per launch in carve-out switches against the neighbouring kernels (measured)
-constexpr int SMEM = NSTAGE * STAGE + 1024 + 256;
+constexpr int PRODUCER_WARP = 8;
+constexpr int NSPLIT_WARPS = 3;                       // warps 9..11
+constexpr int NTHREADS = (PRODUCER_WARP + 1 + NSPLIT_WARPS) * 32;   // 384
+// operand stages + barriers + GroupNorm column sums [8 warps][128] float2 + the bias row, after 1024-byte alignment slack
+constexpr int SMEM = NSTAGE * STAGE + 1024 + 256 + 8 * 128 * 8 + 512;
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.shared::cta.b64 st, [%0];\n\t}" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.expect_tx.shared::cta.b64 st, [%0], %1;\n\t}" ::"r"(smem_u32(bar)), "r"(bytes)
-                 : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    const uint32_t addr = smem_u32(bar);
-    uint32_t done;
-    do {
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                     : "=r"(done)
-                     : "r"(addr), "r"(parity)
-                     : "memory");
-    } while (!done);
-}
-__device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
-    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(
-                     smem_u32(dst)),
-                 "l"(map), "r"(c0), "r"(c1), "r"(smem_u32(bar))
-                 : "memory");
-}
-__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {   // K-major SWIZZLE_128B, SBO = 1024 B (see gse_tc.cu)
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
-    d |= (uint64_t)1 << 16;
-    d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
-}
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-// ---- pieces shared by the one-CTA-per-tile kernel and the persistent kernel ---------------------------------------------------
 // splitter: in-place hi = tf32_rn(x), lo = x - hi into the second buffer of each operand (element-wise, so the swizzled
 // positions are irrelevant: same offset in the hi and lo buffers).  Two 16-byte vectors per thread and iteration: their
 // shared-memory round trips overlap.  t = thread index among the NSPLIT_WARPS * 32 splitter threads.
 __device__ __forceinline__ void split_stage(unsigned char* st, int BN, int t) {
     constexpr int NT = NSPLIT_WARPS * 32;
     const int nvec_a = TILE_A / 16, nvec_b = BN * 128 / 16;
-    const int nvec = nvec_a + nvec_b;            // multiple of NT (BN is a multiple of 16)
+    const int nvec = nvec_a + nvec_b;
     for (int v0 = t; v0 < nvec; v0 += 2 * NT) {
         const int v1 = v0 + NT;
         unsigned char* p0 = (v0 < nvec_a) ? (st + v0 * 16) : (st + 2 * TILE_A + (v0 - nvec_a) * 16);
@@ -119,271 +73,48 @@ __device__ __forceinline__ void split_stage(unsigned char* st, int BN, int t) {
             *reinterpret_cast<float4*>(l1) = q1;
         }
     }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    fence_proxy_async();
 }
 
-// the 12 MMAs of one 32-float K chunk: main products and the (2^-11 smaller) correction products go to separate accumulators
-// (columns [acc, acc+128) and [acc+128, acc+256)): the fp32 accumulation in the tensor core truncates, so keeping the number of
-// additions into the main accumulator at K/8 instead of 3K/8 cuts the systematic error by 3x
-__device__ __forceinline__ void issue_chunk_mmas(uint32_t st, uint32_t acc, uint32_t idesc, bool first_chunk) {
-    const uint64_t a_hi = make_desc(st), a_lo = make_desc(st + TILE_A);
-    const uint64_t b_hi = make_desc(st + 2 * TILE_A), b_lo = make_desc(st + 2 * TILE_A + TILE_B);
-#pragma unroll
-    for (int kk = 0; kk < KC / 8; ++kk) {
-        const uint64_t adv = (uint64_t)(kk * 2);
-        const uint32_t first = (first_chunk && kk == 0) ? 0u : 1u;
-        umma_tf32(acc, a_hi + adv, b_hi + adv, idesc, first);
-        umma_tf32(acc + 128, a_hi + adv, b_lo + adv, idesc, first);
-        umma_tf32(acc + 128, a_lo + adv, b_hi + adv, idesc, 1u);
-    }
-}
-
-// 32 columns of both accumulators (main, corrections) of this thread's row
-__device__ __forceinline__ void tmem_ld_pair(uint32_t taddr, uint32_t (&v)[32], uint32_t (&w2)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-          "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]),
-          "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-          "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr));
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(w2[0]), "=r"(w2[1]), "=r"(w2[2]), "=r"(w2[3]), "=r"(w2[4]), "=r"(w2[5]), "=r"(w2[6]), "=r"(w2[7]), "=r"(w2[8]),
-          "=r"(w2[9]), "=r"(w2[10]), "=r"(w2[11]), "=r"(w2[12]), "=r"(w2[13]), "=r"(w2[14]), "=r"(w2[15]), "=r"(w2[16]),
-          "=r"(w2[17]), "=r"(w2[18]), "=r"(w2[19]), "=r"(w2[20]), "=r"(w2[21]), "=r"(w2[22]), "=r"(w2[23]), "=r"(w2[24]),
-          "=r"(w2[25]), "=r"(w2[26]), "=r"(w2[27]), "=r"(w2[28]), "=r"(w2[29]), "=r"(w2[30]), "=r"(w2[31])
-        : "r"(taddr + 128));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// epilogue of one 32-column chunk of this thread's row: (main + corrections) * row scale + bias (+ ReLU), direct row-segment
-// store, and the GroupNorm column sums over the warp's 32 rows (rows past M and columns past N contribute nothing) through the
-// transposing butterfly into gn_sm[q][slot]
-__device__ __forceinline__ void finish_chunk(const uint32_t (&v)[32], const uint32_t (&w2)[32], float rs, const float* bias_s, int cc,
-                                             int relu, bool row_ok, float* yr, int nvalid, const GnFuse& gn, float2* gn_sm, int q,
-                                             int lane) {
-    float o[32];
-#pragma unroll
-    for (int c = 0; c < 32; ++c) {
-        float t = (__uint_as_float(v[c]) + __uint_as_float(w2[c])) * rs + bias_s[cc + c];
-        if (relu) t = fmaxf(t, 0.f);
-        o[c] = t;
-    }
-    if (row_ok) {
-        if (nvalid == 32 && ((reinterpret_cast<uintptr_t>(yr) & 15) == 0)) {
-#pragma unroll
-            for (int c = 0; c < 32; c += 4) *reinterpret_cast<float4*>(yr + c) = make_float4(o[c], o[c + 1], o[c + 2], o[c + 3]);
-        } else {
-#pragma unroll
-            for (int c = 0; c < 32; ++c)
-                if (c < nvalid) yr[c] = o[c];
-        }
-    }
-    if (gn.groups > 0) {
-        float s1[32], s2[32];
-#pragma unroll
-        for (int c = 0; c < 32; ++c) {
-            const float t = (row_ok && c < nvalid) ? o[c] : 0.f;
-            s1[c] = t;
-            s2[c] = t * t;
-        }
-        float a = warp_butterfly(s1, lane), b2 = warp_butterfly(s2, lane);
-        for (int off = 1; off < gn.slot_width; off <<= 1) {
-            a += __shfl_xor_sync(0xffffffffu, a, off);
-            b2 += __shfl_xor_sync(0xffffffffu, b2, off);
-        }
-        if ((lane & (gn.slot_width - 1)) == 0) gn_sm[q * 128 + (cc + lane) / gn.slot_width] = make_float2(a, b2);
-    }
-}
-
-// 4 epilogue warps -> per-tile partial in a fixed order; gn_finalize / gn_seg_finalize (kpconv.cu) fold the tiles afterwards
-// (no fence / ticket here: the CTA must not wait for its output stores to drain).  et = thread index among the 128 epilogue threads.
-__device__ __forceinline__ void write_gn_partials(const GnFuse& gn, const float2* gn_sm, int et, int BN, int N, int n0, int tile_row) {
-    const int slots_tile = BN / gn.slot_width, slots_total = N / gn.slot_width;
-    asm volatile("bar.sync 1, 128;" ::: "memory");
-    if (et < slots_tile) {
-        const float2 p0 = gn_sm[et], p1 = gn_sm[128 + et], p2 = gn_sm[256 + et], p3 = gn_sm[384 + et];
-        double* dst = gn.partial + ((long long)tile_row * slots_total + n0 / gn.slot_width + et) * 2;
-        dst[0] = ((double)p0.x + (double)p1.x) + ((double)p2.x + (double)p3.x);
-        dst[1] = ((double)p0.y + (double)p1.y) + ((double)p2.y + (double)p3.y);
-    }
-}
-
+// BNI = wgmma N (32, 64 or 128) >= BN; B rows [BN, BNI) of a stage hold stale data and only feed output columns that are
+// never stored.  Tile t -> (split z, row tile, column tile), column tile fastest: neighbouring CTAs share their X rows in L2.
+template <int BNI>
 __global__ void __launch_bounds__(NTHREADS, 1) linear_tc_kernel(const __grid_constant__ CUtensorMap map_x,
                                                                 const __grid_constant__ CUtensorMap map_w,
                                                                 const float* __restrict__ bias, const float* __restrict__ row_scale,
                                                                 float* __restrict__ Y, int ldy, int M, int N, int K, int BN, int relu,
-                                                                GnFuse gn, float* __restrict__ splitk_out, int chunks_per_split) {
-    extern __shared__ unsigned char smem_raw[];
-    __shared__ float bias_s[128];
-    unsigned char* smem = (unsigned char*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    uint64_t* bars = (uint64_t*)(smem + NSTAGE * STAGE);
-    uint64_t* raw_full = bars;                  // TMA landed
-    uint64_t* split_full = bars + NSTAGE;       // hi/lo ready
-    uint64_t* empty = bars + 2 * NSTAGE;        // MMAs done with the stage
-    uint64_t* acc_full = bars + 3 * NSTAGE;
-    uint32_t* tmem_slot = (uint32_t*)(acc_full + 1);
-    float2* gn_sm = (float2*)smem;      // GroupNorm column sums [4 warps][128 slots]: stage 0 is idle once acc_full has fired
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN;
-    const int nk = (K + KC - 1) / KC;
-    // split-K: CTA z accumulates K-chunks [kc0, kc1) and stores its raw partial tile; splitk_reduce_kernel finishes the job
-    const int kc0 = blockIdx.z * chunks_per_split, kc1 = min(nk, kc0 + chunks_per_split);
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < NSTAGE; ++s) { mbar_init(&raw_full[s], 1); mbar_init(&split_full[s], NSPLIT_WARPS); mbar_init(&empty[s], 1); }
-        mbar_init(acc_full, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_x) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w) : "memory");
-    }
-    if (warp == MMA_WARP) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 256;" ::"r"(smem_u32(tmem_slot)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp == 0) {
-        if (lane == 0) {
-            int s = 0;
-            uint32_t ph = 0;
-            for (int kc = kc0; kc < kc1; ++kc) {
-                mbar_wait(&empty[s], ph ^ 1u);
-                unsigned char* st = smem + s * STAGE;
-                mbar_arrive_expect_tx(&raw_full[s], (uint32_t)(TILE_A + BN * 128));
-                tma_load_2d(st, &map_x, kc * KC, m0, &raw_full[s]);
-                tma_load_2d(st + 2 * TILE_A, &map_w, kc * KC, n0, &raw_full[s]);
-                if (++s == NSTAGE) { s = 0; ph ^= 1u; }
-            }
-        }
-    } else if (warp <= NSPLIT_WARPS) {
-        const int t = threadIdx.x - 32;              // 0..NSPLIT_WARPS*32-1
-        int s = 0;
-        uint32_t ph = 0;
-        for (int kc = kc0; kc < kc1; ++kc) {
-            mbar_wait(&raw_full[s], ph);
-            split_stage(smem + s * STAGE, BN, t);
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&split_full[s]);
-            if (++s == NSTAGE) { s = 0; ph ^= 1u; }
-        }
-    } else if (warp == MMA_WARP) {
-        if (lane == 0) {
-            const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-            int s = 0;
-            uint32_t ph = 0;
-            for (int kc = kc0; kc < kc1; ++kc) {
-                mbar_wait(&split_full[s], ph);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                issue_chunk_mmas(smem_u32(smem + s * STAGE), tmem_base, idesc, kc == kc0);
-                umma_commit(&empty[s]);
-                if (++s == NSTAGE) { s = 0; ph ^= 1u; }
-            }
-            umma_commit(acc_full);
-        }
-    } else {
-        const int q = warp & 3;
-        // the tile's bias row goes through shared memory once (loaded while the main loop runs): per-element global loads in
-        // the epilogue are a chain of 32 dependent L2 round trips per chunk (~8 us per tile, measured)
-        {
-            const int et = threadIdx.x - EPI_WARP0 * 32;
-            bias_s[et] = (bias != nullptr && n0 + et < N) ? __ldg(bias + n0 + et) : 0.f;
-            asm volatile("bar.sync 1, 128;" ::: "memory");
-        }
-        mbar_wait(acc_full, 0);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const int m = m0 + q * 32 + lane;
-        const float rs = (row_scale != nullptr && m < M) ? row_scale[m] : 1.0f;   // KPConv: 1 / neighbour count
-        for (int cc = 0; cc < BN; cc += 32) {
-            uint32_t v[32], w2[32];
-            tmem_ld_pair(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)cc, v, w2);
-            const int nvalid = min(32, N - (n0 + cc));
-            if (splitk_out != nullptr) {              // raw partial sums of this K-slice (N is a multiple of 16: float4-aligned)
-                if (m < M) {
-                    float* pr = splitk_out + ((long long)blockIdx.z * M + m) * N + n0 + cc;
-#pragma unroll
-                    for (int c = 0; c < 32; c += 4)
-                        if (c < nvalid)
-                            *reinterpret_cast<float4*>(pr + c) =
-                                make_float4(__uint_as_float(v[c]) + __uint_as_float(w2[c]), __uint_as_float(v[c + 1]) + __uint_as_float(w2[c + 1]),
-                                            __uint_as_float(v[c + 2]) + __uint_as_float(w2[c + 2]), __uint_as_float(v[c + 3]) + __uint_as_float(w2[c + 3]));
-                }
-                continue;
-            }
-            finish_chunk(v, w2, rs, bias_s, cc, relu, m < M, Y + (long long)m * ldy + n0 + cc, nvalid, gn, gn_sm, q, lane);
-        }
-        if (gn.groups > 0 && splitk_out == nullptr) write_gn_partials(gn, gn_sm, threadIdx.x - EPI_WARP0 * 32, BN, N, n0, blockIdx.y);
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == MMA_WARP) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 256;" ::"r"(tmem_base) : "memory");
-    }
-}
-
-// ---- persistent variant (multi-wave GEMMs) ----------------------------------------------------------------------------------
-// One CTA per SM walks the output tiles t = blockIdx.x, blockIdx.x + gridDim.x, ...  The operand ring keeps running across
-// tile boundaries and there are TWO accumulator sets in TMEM (2 x (main 128 + corrections 128) = 512 columns): while the four
-// epilogue warps drain, normalise and store tile i, the producer / splitters / MMA issuer are already deep in the K loop of
-// tile i + 1, so the per-tile fixed cost (first TMA round trip, TMEM drain, stores) is hidden instead of paid per CTA.
-// 202.5 KB: 6 KB over the 196 KB carve-out the per-tile kernel stays under, i.e. this kernel runs in the 228 KB shared-memory
-// configuration.  Accepted: it is only chosen for GEMMs of more than one wave of tiles (>= 0.1 ms each in batch mode), where a
-// carve-out switch against a neighbouring kernel (~8 us, measured in round 1) is noise, and the GroupNorm / bias staging must
-// survive across the tile loop next to the three operand stages.
-constexpr int SMEM_PERSIST = SMEM + 4 * 128 * 8 + 512;      // + GroupNorm column sums [4][128] float2 + the bias row
-
-__global__ void __launch_bounds__(NTHREADS, 1) linear_tc_persistent_kernel(const __grid_constant__ CUtensorMap map_x,
-                                                                           const __grid_constant__ CUtensorMap map_w,
-                                                                           const float* __restrict__ bias,
-                                                                           const float* __restrict__ row_scale, float* __restrict__ Y,
-                                                                           int ldy, int M, int N, int K, int BN, int relu, GnFuse gn,
-                                                                           int col_tiles, int num_tiles) {
+                                                                GnFuse gn, float* __restrict__ splitk_out, int chunks_per_split,
+                                                                int col_tiles, int row_tiles, int num_tiles) {
+    constexpr int R = BNI / 2;          // accumulator registers per thread
     extern __shared__ unsigned char smem_raw[];
     unsigned char* smem = (unsigned char*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
     uint64_t* bars = (uint64_t*)(smem + NSTAGE * STAGE);
     uint64_t* raw_full = bars;                  // TMA landed
     uint64_t* split_full = bars + NSTAGE;       // hi/lo ready
     uint64_t* empty = bars + 2 * NSTAGE;        // MMAs done with the stage
-    uint64_t* acc_full = bars + 3 * NSTAGE;     // [2] accumulator set complete
-    uint64_t* acc_empty = acc_full + 2;         // [2] accumulator set drained by the epilogue
-    uint32_t* tmem_slot = (uint32_t*)(acc_empty + 2);
-    float2* gn_sm = (float2*)(smem + NSTAGE * STAGE + 256);
-    float* bias_s = (float*)(smem + NSTAGE * STAGE + 256 + 4 * 128 * 8);
+    float2* gn_sm = (float2*)(smem + NSTAGE * STAGE + 256);        // [8 consumer warps][128 columns] (sum, sum of squares)
+    float* bias_s = (float*)(gn_sm + 8 * 128);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int nk = (K + KC - 1) / KC;
+    const int tiles_per_split = col_tiles * row_tiles;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < NSTAGE; ++s) { mbar_init(&raw_full[s], 1); mbar_init(&split_full[s], NSPLIT_WARPS); mbar_init(&empty[s], 1); }
-        for (int a = 0; a < 2; ++a) { mbar_init(&acc_full[a], 1); mbar_init(&acc_empty[a], 4); }
+        for (int s = 0; s < NSTAGE; ++s) { mbar_init(&raw_full[s], 1); mbar_init(&split_full[s], NSPLIT_WARPS); mbar_init(&empty[s], 8); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_x) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w) : "memory");
     }
-    if (warp == MMA_WARP) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(tmem_slot)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp == PRODUCER_WARP) {
         if (lane == 0) {
             int s = 0;
             uint32_t ph = 0;
             for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-                const int m0 = (t / col_tiles) * BM, n0 = (t % col_tiles) * BN;
-                for (int kc = 0; kc < nk; ++kc) {
+                const int z = t / tiles_per_split, rem = t % tiles_per_split;
+                const int m0 = (rem / col_tiles) * BM, n0 = (rem % col_tiles) * BN;
+                const int kc0 = z * chunks_per_split, kc1 = min(nk, kc0 + chunks_per_split);
+                for (int kc = kc0; kc < kc1; ++kc) {
                     mbar_wait(&empty[s], ph ^ 1u);
                     unsigned char* st = smem + s * STAGE;
                     mbar_arrive_expect_tx(&raw_full[s], (uint32_t)(TILE_A + BN * 128));
@@ -393,73 +124,151 @@ __global__ void __launch_bounds__(NTHREADS, 1) linear_tc_persistent_kernel(const
                 }
             }
         }
-    } else if (warp <= NSPLIT_WARPS) {
-        const int tt = threadIdx.x - 32;
+        return;
+    }
+    if (warp > PRODUCER_WARP) {
+        const int ts = threadIdx.x - (PRODUCER_WARP + 1) * 32;
         int s = 0;
         uint32_t ph = 0;
         for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-            for (int kc = 0; kc < nk; ++kc) {
+            const int z = t / tiles_per_split;
+            const int kc0 = z * chunks_per_split, kc1 = min(nk, kc0 + chunks_per_split);
+            for (int kc = kc0; kc < kc1; ++kc) {
                 mbar_wait(&raw_full[s], ph);
-                split_stage(smem + s * STAGE, BN, tt);
+                split_stage(smem + s * STAGE, BN, ts);
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&split_full[s]);
                 if (++s == NSTAGE) { s = 0; ph ^= 1u; }
             }
         }
-    } else if (warp == MMA_WARP) {
-        if (lane == 0) {
-            const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-            int s = 0;
-            uint32_t ph = 0;
-            int it = 0;
-            for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++it) {
-                const int set = it & 1;
-                mbar_wait(&acc_empty[set], (((uint32_t)it >> 1) & 1u) ^ 1u);      // the epilogue has drained the previous use of this set
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t acc = tmem_base + (uint32_t)(set * 256);
-                for (int kc = 0; kc < nk; ++kc) {
-                    mbar_wait(&split_full[s], ph);
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    issue_chunk_mmas(smem_u32(smem + s * STAGE), acc, idesc, kc == 0);
-                    umma_commit(&empty[s]);
-                    if (++s == NSTAGE) { s = 0; ph ^= 1u; }
-                }
-                umma_commit(&acc_full[set]);
-            }
-        }
-    } else {
-        const int q = warp & 3;
-        const int et = threadIdx.x - EPI_WARP0 * 32;
-        int it = 0;
-        for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++it) {
-            const int set = it & 1;
-            const int ty = t / col_tiles;
-            const int m0 = ty * BM, n0 = (t % col_tiles) * BN;
-            asm volatile("bar.sync 1, 128;" ::: "memory");                          // previous tile's readers of bias_s / gn_sm are done
-            bias_s[et] = (bias != nullptr && n0 + et < N) ? __ldg(bias + n0 + et) : 0.f;
-            asm volatile("bar.sync 1, 128;" ::: "memory");
-            mbar_wait(&acc_full[set], ((uint32_t)it >> 1) & 1u);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const int m = m0 + q * 32 + lane;
-            const float rs = (row_scale != nullptr && m < M) ? row_scale[m] : 1.0f;
-            for (int cc = 0; cc < BN; cc += 32) {
-                uint32_t v[32], w2[32];
-                tmem_ld_pair(tmem_base + (uint32_t)(set * 256) + ((uint32_t)(q * 32) << 16) + (uint32_t)cc, v, w2);
-                if (cc + 32 >= BN) {        // last chunk read: hand the accumulator set back before the stores and statistics
-                    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&acc_empty[set]);
-                }
-                finish_chunk(v, w2, rs, bias_s, cc, relu, m < M, Y + (long long)m * ldy + n0 + cc, min(32, N - (n0 + cc)), gn, gn_sm, q, lane);
-            }
-            if (gn.groups > 0) write_gn_partials(gn, gn_sm, et, BN, N, n0, ty);
-        }
+        return;
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == MMA_WARP) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
+
+    // ---- consumers ----
+    const int wg = warp >> 2, wq = warp & 3;
+    int s = 0;
+    uint32_t ph = 0;
+    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+        const int z = t / tiles_per_split, rem = t % tiles_per_split;
+        const int ty = rem / col_tiles;
+        const int m0 = ty * BM, n0 = (rem % col_tiles) * BN;
+        const int kc0 = z * chunks_per_split, kc1 = min(nk, kc0 + chunks_per_split);
+        // the tile's bias row goes through shared memory once: per-element global loads in the epilogue would be a chain of
+        // dependent L2 round trips
+        asm volatile("bar.sync 1, 256;" ::: "memory");                          // previous tile's readers of bias_s / gn_sm are done
+        if (threadIdx.x < 128) bias_s[threadIdx.x] = (bias != nullptr && (int)threadIdx.x < BN) ? __ldg(bias + n0 + threadIdx.x) : 0.f;
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+
+        // main products and the (2^-11 smaller) correction products go to separate accumulators: keeping the number of
+        // additions into the main accumulator at K/8 instead of 3K/8 lowers the rounding error of the fp32 accumulation
+        float acc[R], cor[R];
+#pragma unroll
+        for (int i = 0; i < R; ++i) { acc[i] = 0.f; cor[i] = 0.f; }
+        int prev_s = -1;
+        for (int kc = kc0; kc < kc1; ++kc) {
+            mbar_wait(&split_full[s], ph);
+            const uint32_t st = smem_u32(smem + s * STAGE);
+            const uint64_t a_hi = make_desc(st + wg * (TILE_A / 2)), a_lo = make_desc(st + TILE_A + wg * (TILE_A / 2));
+            const uint64_t b_hi = make_desc(st + 2 * TILE_A), b_lo = make_desc(st + 2 * TILE_A + TILE_B);
+            wgmma_fence();
+#pragma unroll
+            for (int kk = 0; kk < KC / 8; ++kk) {
+                const uint64_t adv = (uint64_t)(kk * 2);      // +32 bytes in 16-byte units
+                const uint32_t accum = (kc == kc0 && kk == 0) ? 0u : 1u;
+                wgmma_tf32<BNI>(acc, a_hi + adv, b_hi + adv, accum);
+                wgmma_tf32<BNI>(cor, a_hi + adv, b_lo + adv, accum);
+                wgmma_tf32<BNI>(cor, a_lo + adv, b_hi + adv, 1u);
+            }
+            wgmma_commit();
+            wgmma_wait<1>();                    // the previous chunk's MMAs are done: its stage can be refilled
+            if (prev_s >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty[prev_s]); }
+            prev_s = s;
+            if (++s == NSTAGE) { s = 0; ph ^= 1u; }
+        }
+        wgmma_wait<0>();
+        reg_fence(acc);
+        reg_fence(cor);
+        if (prev_s >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty[prev_s]); }
+
+        // epilogue: this thread holds rows r0 and r0 + 8, columns 8j + 2(lane % 4) + {0, 1}
+        const int r0 = m0 + wg * 64 + wq * 16 + (lane >> 2);
+        const int c0 = 2 * (lane & 3);
+        float rs[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) rs[h] = (row_scale != nullptr && r0 + 8 * h < M) ? row_scale[r0 + 8 * h] : 1.0f;
+        if (splitk_out != nullptr) {              // raw partial sums of this K-slice (N is even: float2-aligned)
+#pragma unroll
+            for (int j = 0; j < BNI / 8; ++j)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int m = r0 + 8 * h, col = 8 * j + c0;
+                    if (m < M && col < BN)
+                        *reinterpret_cast<float2*>(splitk_out + ((long long)z * M + m) * N + n0 + col) =
+                            make_float2(acc[4 * j + 2 * h] + cor[4 * j + 2 * h], acc[4 * j + 2 * h + 1] + cor[4 * j + 2 * h + 1]);
+                }
+            continue;
+        }
+        const bool vec2 = ((ldy & 1) == 0) && ((reinterpret_cast<uintptr_t>(Y) & 7) == 0);
+#pragma unroll
+        for (int j = 0; j < BNI / 8; ++j) {
+            const int col = 8 * j + c0;
+            float o[4];
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                float v = (acc[4 * j + e] + cor[4 * j + e]) * rs[e >> 1] + bias_s[col + (e & 1)];
+                if (relu) v = fmaxf(v, 0.f);
+                o[e] = v;
+            }
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int m = r0 + 8 * h;
+                if (m < M && col < BN) {
+                    float* yp = Y + (long long)m * ldy + n0 + col;
+                    if (vec2) *reinterpret_cast<float2*>(yp) = make_float2(o[2 * h], o[2 * h + 1]);
+                    else { yp[0] = o[2 * h]; yp[1] = o[2 * h + 1]; }
+                }
+            }
+            if (gn.groups > 0) {
+                // column sums over the warp's 16 rows (rows past M and columns past BN contribute nothing)
+                const bool ok0 = r0 < M && col < BN, ok1 = r0 + 8 < M && col < BN;
+                float a0 = (ok0 ? o[0] : 0.f) + (ok1 ? o[2] : 0.f), a1 = (ok0 ? o[1] : 0.f) + (ok1 ? o[3] : 0.f);
+                float q0 = (ok0 ? o[0] * o[0] : 0.f) + (ok1 ? o[2] * o[2] : 0.f);
+                float q1 = (ok0 ? o[1] * o[1] : 0.f) + (ok1 ? o[3] * o[3] : 0.f);
+#pragma unroll
+                for (int off = 4; off < 32; off <<= 1) {
+                    a0 += __shfl_xor_sync(0xffffffffu, a0, off);
+                    a1 += __shfl_xor_sync(0xffffffffu, a1, off);
+                    q0 += __shfl_xor_sync(0xffffffffu, q0, off);
+                    q1 += __shfl_xor_sync(0xffffffffu, q1, off);
+                }
+                if (lane < 4) {
+                    gn_sm[warp * 128 + col] = make_float2(a0, q0);
+                    gn_sm[warp * 128 + col + 1] = make_float2(a1, q1);
+                }
+            }
+        }
+        if (gn.groups > 0) {
+            // per-tile partial in a fixed order; gn_finalize / gn_seg_finalize (kpconv.cu) fold the tiles afterwards
+            asm volatile("bar.sync 1, 256;" ::: "memory");
+            const int sw = gn.slot_width, slots_tile = BN / sw, slots_total = N / sw;
+            const int et = threadIdx.x;
+            if (et < slots_tile) {
+                double s1 = 0.0, s2 = 0.0;
+                for (int w = 0; w < 8; ++w) {
+                    float f1 = 0.f, f2 = 0.f;
+                    for (int c = 0; c < sw; ++c) {
+                        const float2 p = gn_sm[w * 128 + et * sw + c];
+                        f1 += p.x;
+                        f2 += p.y;
+                    }
+                    s1 += (double)f1;
+                    s2 += (double)f2;
+                }
+                double* dst = gn.partial + ((long long)ty * slots_total + n0 / sw + et) * 2;
+                dst[0] = s1;
+                dst[1] = s2;
+            }
+        }
     }
 }
 
@@ -561,8 +370,7 @@ int linear_tc(const float* x, int64_t ldx, const float* w, int64_t ldw, const fl
     CUtensorMap mx, mw;
     if (ltc::encode_map(&mx, x, m, k, ldx, ltc::BM)) return -1;
     if (ltc::encode_map(&mw, w, n, k, ldw, BN)) return -1;
-    if (ensure_max_smem((const void*)ltc::linear_tc_kernel)) return -1;
-    dim3 grid((unsigned)(n / BN), (unsigned)((m + ltc::BM - 1) / ltc::BM));
+    const int col_tiles = (int)(n / BN), row_tiles = (int)((m + ltc::BM - 1) / ltc::BM);
     GnFuse g{};
     if (gn != nullptr) {
         g = *gn;
@@ -574,7 +382,7 @@ int linear_tc(const float* x, int64_t ldx, const float* w, int64_t ldw, const fl
     // split-K: a deep K loop on a handful of tiles leaves most SMs idle and is pure latency (1.4 us per 32-wide chunk): give
     // every K-slice of >= 8 chunks its own CTA when the grid would cover less than half of the GPU
     const int nk = (int)((k + ltc::KC - 1) / ltc::KC);
-    const int tiles = (int)(grid.x * grid.y);
+    const int tiles = col_tiles * row_tiles;
     int splits = 1;
     if (g_splitk_on && tiles * 2 <= num_sms() && nk >= 16) {
         splits = nk / 8;
@@ -592,7 +400,6 @@ int linear_tc(const float* x, int64_t ldx, const float* w, int64_t ldw, const fl
         part = splitk_scratch(st, (size_t)splits * (size_t)m * (size_t)n * sizeof(float));
         if (part == nullptr) { splits = 1; cps = nk; }
     }
-    grid.z = (unsigned)splits;
     ProfRec rec{};
     const bool prof = g_prof_on;
     if (prof) {
@@ -601,15 +408,20 @@ int linear_tc(const float* x, int64_t ldx, const float* w, int64_t ldw, const fl
         rec.m = m; rec.n = n; rec.k = k;
         cudaEventRecord(rec.a, st);
     }
+    // one CTA per tile, or (persistent loop) one CTA per SM walking the tiles of a GEMM of more than one wave
+    const int num_tiles = tiles * splits;
     const bool persistent = g_persistent_on && splits == 1 && tiles > num_sms();
-    if (persistent) {
-        if (ensure_max_smem((const void*)ltc::linear_tc_persistent_kernel)) return -1;
-        ltc::linear_tc_persistent_kernel<<<num_sms(), ltc::NTHREADS, ltc::SMEM_PERSIST, st>>>(mx, mw, bias, row_scale, y, (int)ldy, (int)m, (int)n,
-                                                                                            (int)k, BN, relu, g, (int)grid.x, tiles);
-    } else {
-        ltc::linear_tc_kernel<<<grid, ltc::NTHREADS, ltc::SMEM, st>>>(mx, mw, bias, row_scale, y, (int)ldy, (int)m, (int)n, (int)k, BN, relu, g,
-                                                                      part, cps);
-    }
+    const unsigned grid = (unsigned)(persistent ? num_sms() : num_tiles);
+    const void* kern = BN <= 32 ? (const void*)ltc::linear_tc_kernel<32> : BN <= 64 ? (const void*)ltc::linear_tc_kernel<64>
+                                                                                      : (const void*)ltc::linear_tc_kernel<128>;
+    if (ensure_max_smem(kern)) return -1;
+#define GEOB_LTC_LAUNCH(BNI)                                                                                                  \
+    ltc::linear_tc_kernel<BNI><<<grid, ltc::NTHREADS, ltc::SMEM, st>>>(mx, mw, bias, row_scale, y, (int)ldy, (int)m, (int)n, (int)k, \
+                                                                       BN, relu, g, part, cps, col_tiles, row_tiles, num_tiles)
+    if (BN <= 32) GEOB_LTC_LAUNCH(32);
+    else if (BN <= 64) GEOB_LTC_LAUNCH(64);
+    else GEOB_LTC_LAUNCH(128);
+#undef GEOB_LTC_LAUNCH
     if (part != nullptr) {
         const long long mn = (long long)m * n;
         ltc::splitk_reduce_kernel<<<(unsigned)((mn / 4 + 255) / 256), 256, 0, st>>>(part, splits, mn, (int)n, bias, row_scale, y, (int)ldy, relu);

@@ -1,4 +1,4 @@
-"""B200 replacement of the reference's native op module ``geotransformer.ext``.
+"""H100 (CUDA) replacement of the reference's native op module ``geotransformer.ext``.
 
 Same two positional-argument functions as reference ``geotransformer/extensions/pybind.cpp:6-18``:
 

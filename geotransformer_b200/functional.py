@@ -1,7 +1,7 @@
 """Thin torch-tensor wrappers over the C ABI (``include/geob200.h``).
 
 PyTorch is used here only for device memory and the current stream; every computation is a hand-written
-sm_100a kernel inside ``libgeob200.so``.  All functions require CUDA tensors and raise ``RuntimeError`` otherwise
+sm_90a kernel inside ``libgeob200.so``.  All functions require CUDA tensors and raise ``RuntimeError`` otherwise
 (there is no CPU path in the product).
 """
 import math
@@ -12,11 +12,11 @@ from . import _lib as L
 
 _f32, _i64, _u8, _i32 = torch.float32, torch.int64, torch.uint8, torch.int32
 
-# mode of the structure-embedding contraction (see geob200_gse_embed): 0 fp32 CUDA cores, 1 tcgen05 3xTF32, 2 1xTF32,
+# mode of the structure-embedding contraction (see geob200_gse_embed): 0 fp32 CUDA cores, 1 wgmma 3xTF32, 2 1xTF32,
 # 3 3xFP16 (fp32-accurate like 3xTF32 at half the tensor-pipe time), 4 3xFP16 on CTA pairs,
-# 5 tabulated projections (geob200_gse_embed_table: no contraction at all; default -- 6.4x faster than mode 3 and 3x closer to
-# the oracle, profiles/r02_gse_table_check.txt).  Mode 5 needs the ``table`` of the weights (``gse_table``; the modules build and
-# cache it); the functional ops called WITHOUT a table and without an explicit mode run the tcgen05 contraction (mode 3).
+# 5 tabulated projections (geob200_gse_embed_table: no contraction at all; default -- tests/gse_table_check.py compares its
+# accuracy and launch time with mode 3).  Mode 5 needs the ``table`` of the weights (``gse_table``; the modules build and
+# cache it); the functional ops called WITHOUT a table and without an explicit mode run the tensor-core contraction (mode 3).
 GSE_MODE = int(__import__('os').environ.get('GEOB200_GSE_MODE', '5'))
 # tabulation grid of mode 5: step 1 / GSE_TABLE_INV_STEP index units (power of two), distance indices up to GSE_TABLE_D_MAX
 # (larger ones are evaluated directly inside the kernel: correct, slow)
@@ -75,7 +75,7 @@ def _gn_workspace(device, groups, rows=0, channels=0, n_pairs=1):
 
 # ------------------------------------------------------------------------------------------------ backbone
 
-# KPConv formulation: 'tc' = gather kernel + tcgen05 3xTF32 GEMM (default where the shape allows), 'fused' = single fp32 kernel
+# KPConv formulation: 'tc' = gather kernel + wgmma 3xTF32 GEMM (default where the shape allows), 'fused' = single fp32 kernel
 KPCONV_MODE = 'tc'
 
 
@@ -134,7 +134,7 @@ def group_norm(x, weight, bias, groups, eps=1e-5, negative_slope=None, residual=
 
 
 def linear_group_norm(x, weight, bias, gn_weight, gn_bias, groups, eps=1e-5, negative_slope=None, residual=None):
-    """UnaryBlock: leaky(GroupNorm(x @ weight.T + bias) + residual); statistics from the GEMM epilogue on the tcgen05 path"""
+    """UnaryBlock: leaky(GroupNorm(x @ weight.T + bias) + residual); statistics from the GEMM epilogue on the wgmma path"""
     x, weight, bias, gn_weight, gn_bias = _detach(x), _detach(weight), _detach(bias), _detach(gn_weight), _detach(gn_bias)
     if not x.is_cuda or x.dtype != _f32 or x.stride(1) != 1:
         raise RuntimeError('linear_group_norm: x must be a float32 CUDA tensor with unit inner stride')
@@ -443,7 +443,7 @@ def gse_embed_flat(d_indices, a_indices, n_rows, div_term, wd, wa, bd, ba, wd_t,
     if mode == 5 and c in (128, 256):
         return _gse_embed_table(d_indices, a_indices, n_rows, div_term, wd, wa, bd, ba, table, out)
     if c == 128 and mode != 0:
-        mode = 3                     # hidden_dim 128 (KITTI): the 3xFP16 tcgen05 kernel has an N = 128 instantiation
+        mode = 3                     # hidden_dim 128 (KITTI): the 3xFP16 wgmma kernel has an N = 128 instantiation
     elif c != 256:
         mode = 0                     # other widths: fp32 CUDA-core kernel
     lib = L.lib()
@@ -464,7 +464,7 @@ def gse_embed(d_indices, a_indices, div_term, wd, wa, bd, ba, wd_t, wa_t, mode=N
     if mode == 5 and c in (128, 256):
         return _gse_embed_table(d_indices, a_indices, n * n, div_term, wd, wa, bd, ba, table, emb)
     if c == 128 and mode != 0:
-        mode = 3                     # hidden_dim 128 (KITTI): the 3xFP16 tcgen05 kernel has an N = 128 instantiation
+        mode = 3                     # hidden_dim 128 (KITTI): the 3xFP16 wgmma kernel has an N = 128 instantiation
     elif c != 256:
         mode = 0                     # other widths: fp32 CUDA-core kernel
     lib = L.lib()
@@ -593,7 +593,7 @@ def sinkhorn(scores, row_masks, col_masks, alpha, num_iterations, inf=1e12):
     _f(scores, 'scores')
     p, k, k2 = scores.shape
     if k != k2:
-        raise RuntimeError('sinkhorn: the B200 kernel handles square patch score matrices')
+        raise RuntimeError('sinkhorn: the CUDA kernel handles square patch score matrices')
     dev = scores.device
     if row_masks is None:
         row_masks = torch.ones((p, k), dtype=torch.bool, device=dev)

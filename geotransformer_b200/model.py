@@ -1,4 +1,4 @@
-"""GeoTransformer registration model (inference forward) on the B200 path.
+"""GeoTransformer registration model (inference forward) on the H100 path.
 
 Reference: ``experiments/*/model.py:18-217``.  Same attribute names (``backbone``, ``transformer``,
 ``coarse_matching``, ``fine_matching``, ``optimal_transport``) and hence the same ``state_dict`` keys; same

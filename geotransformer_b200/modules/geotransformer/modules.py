@@ -1,4 +1,4 @@
-"""``geotransformer.modules.geotransformer`` on the B200 path: same class names, constructor/forward signatures and
+"""``geotransformer.modules.geotransformer`` on the H100 path: same class names, constructor/forward signatures and
 ``state_dict`` keys as the reference (``geotransformer/modules/geotransformer/{geotransformer.py:9-155,
 superpoint_matching.py:7-50, local_global_registration.py:11-235}``)."""
 import threading

@@ -1,6 +1,6 @@
 """KPConv building blocks with the reference's class names, constructor signatures and ``state_dict`` keys
 (reference ``geotransformer/modules/kpconv/kpconv.py:10-122`` and ``modules.py:33-225``); every forward
-runs hand-written sm_100a kernels through the C ABI (``geotransformer_b200.functional``)."""
+runs hand-written sm_90a kernels through the C ABI (``geotransformer_b200.functional``)."""
 import math
 
 import torch

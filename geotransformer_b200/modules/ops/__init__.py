@@ -1,4 +1,4 @@
-"""Op surface of ``geotransformer.modules.ops`` (reference ``modules/ops/__init__.py:1-21``) on the B200 path."""
+"""Op surface of ``geotransformer.modules.ops`` (reference ``modules/ops/__init__.py:1-21``) on the H100 path."""
 import torch
 
 from ... import ext as _ext

@@ -1,4 +1,4 @@
-"""Transformer blocks with the reference's class names and ``state_dict`` keys; forwards run the fused sm_100a
+"""Transformer blocks with the reference's class names and ``state_dict`` keys; forwards run the fused sm_90a
 kernels.  Reference: ``geotransformer/modules/transformer/{positional_embedding.py:8-34, rpe_transformer.py:18-131,
 vanilla_transformer.py:15-129, output_layer.py:6-21, conditional_transformer.py:73-117}``.
 
@@ -29,7 +29,7 @@ class SinusoidalPositionalEmbedding(nn.Module):
 def _no_masks(**kw):
     for k, v in kw.items():
         if v is not None:
-            raise NotImplementedError(f'{k} is not supported on the B200 inference path (always None in the reference model)')
+            raise NotImplementedError(f'{k} is not supported on the H100 inference path (always None in the reference model)')
 
 
 class _WeightCache:

@@ -1,4 +1,4 @@
-/* geob200 -- C ABI of the B200-native GeoTransformer registration hot path.
+/* geob200 -- C ABI of the H100-native GeoTransformer registration hot path.
  *
  * Drop-in boundary (SURVEY.md section 8b).  Every entry point takes plain pointers and sizes; device
  * pointers unless the name ends in `_h`; `stream` is a cudaStream_t passed as void*.  All functions
@@ -66,7 +66,7 @@ int geob200_kpconv(const float* s_feats, const float* q_points, const float* s_p
 /* nn.Linear: y[m,n] = x[m,k] . weight[n,k]^T + bias (UnaryBlock.mlp, modules.py:78; every transformer Linear).
  * ldx / ldy are row strides in floats (inputs may be column slices). */
 /* Same op, two-stage tensor-core formulation: gather kernel (wf = influence-weighted neighbour features, M x 15 c_in) followed by
- * the 3xTF32 tcgen05 GEMM with the neighbour-count scale and bias in its epilogue.  weights_t is the (15*c_in, c_out) weight
+ * the 3xTF32 wgmma GEMM with the neighbour-count scale and bias in its epilogue.  weights_t is the (15*c_in, c_out) weight
  * matrix transposed to (c_out, 15*c_in). */
 size_t geob200_kpconv_tc_workspace_bytes(int64_t n_query, int64_t n_support, int64_t c_in);
 int geob200_kpconv_tc(const float* s_feats, const float* q_points, const float* s_points, const int64_t* neighbors, int64_t n_query,
@@ -74,7 +74,7 @@ int geob200_kpconv_tc(const float* s_feats, const float* q_points, const float* 
                       const float* bias, int64_t c_in, int64_t c_out, float sigma, float* out, void* workspace, size_t workspace_bytes,
                       void* stream);
 
-/* 1 (default): Linears run on tcgen05 with 3xTF32 when the shape allows; 0: fp32 CUDA cores only */
+/* 1 (default): Linears run on the tensor cores with 3xTF32 when the shape allows; 0: fp32 CUDA cores only */
 void geob200_set_linear_mode(int mode);
 int geob200_linear(const float* x, int64_t ldx, const float* weight, const float* bias, float* y, int64_t ldy, int64_t m,
                    int64_t n, int64_t k, int relu, void* stream);
@@ -92,7 +92,7 @@ int geob200_group_norm(const float* x, int64_t n_rows, int64_t channels, int64_t
 
 /* Fused blocks: Linear -> GroupNorm (+ residual) (+ LeakyReLU) = UnaryBlock and the unary parts of ResidualBlock
  * (modules/kpconv/modules.py:33-104,150-225); KPConv -> GroupNorm -> LeakyReLU = ConvBlock and the conv part of
- * ResidualBlock (modules.py:107-147,205-207).  On the tcgen05 path the GroupNorm statistics are produced by the GEMM
+ * ResidualBlock (modules.py:107-147,205-207).  On the wgmma path the GroupNorm statistics are produced by the GEMM
  * epilogue, so the activations are not re-read for them.  pre_norm receives the Linear / KPConv output, y the result.
  * The GroupNorm workspace (>= geob200_fused_group_norm_workspace_bytes) must be zero-filled once before first use. */
 size_t geob200_fused_group_norm_workspace_bytes(int64_t n_rows, int64_t channels, int64_t groups);
@@ -177,7 +177,7 @@ int geob200_gse_indices_batched(const float* points, int64_t n_clouds, const int
 
 /* GeometricStructureEmbedding.forward (geotransformer.py:57-72) given the indices: sinusoid -> proj_d / proj_a ->
  * max over k -> sum, fused.  wd/wa are the nn.Linear weights (out,in); wd_t/wa_t their transposes (in,out).
- * mode 0: fp32 CUDA cores; 1: tcgen05 3xTF32; 2: tcgen05 1xTF32; 3: tcgen05 3xFP16 split (fp32-accurate, fastest). */
+ * mode 0: fp32 CUDA cores; 1: wgmma 3xTF32; 2: wgmma 1xTF32; 3: wgmma 3xFP16 split (fp32-accurate, fastest). */
 size_t geob200_gse_embed_workspace_bytes(int64_t n, int64_t channels);
 int geob200_gse_embed(const float* d_indices, const float* a_indices, int64_t n, int64_t channels, const float* div_term,
                       const float* wd_t, const float* wa_t, const float* wd, const float* wa, const float* bd, const float* ba,
@@ -307,12 +307,12 @@ int geob200_evaluate_counts(const int64_t* gt_node_corr_indices, const float* gt
                             const float* est_transform, const float* src_points, int64_t n_src_points, int mode, float rmse_threshold,
                             float rre_threshold, float rte_threshold, float* metrics, void* stream);
 
-/* Profiling aid (bench.py roofline): while enabled, every tcgen05 GEMM launch (nn.Linear and the KPConv contraction) is
+/* Profiling aid (bench.py roofline): while enabled, every tensor-core GEMM launch (nn.Linear and the KPConv contraction) is
  * bracketed by CUDA events on its stream; _read synchronises them and returns the count, shapes[3i..] = (m, n, k), ms[i]. */
 int geob200_linear_profile_enable(int on);
 /* split-K for deep-K GEMMs on few tiles (default on); off = every tile runs its whole K loop in one CTA */
 int geob200_set_split_k(int on);
-/* persistent tile loop with two TMEM accumulator sets for GEMMs of more than one wave of tiles (default on) */
+/* persistent tile loop (one CTA per SM) for GEMMs of more than one wave of tiles (default on) */
 int geob200_set_linear_persistent(int on);
 int64_t geob200_linear_profile_read(int64_t capacity, int64_t* shapes, float* ms);
 

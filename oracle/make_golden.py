@@ -1,12 +1,13 @@
 """TEST INFRASTRUCTURE ONLY -- generates the committed fixtures under tests/golden/ by running the REAL reference
 (imported from /root/reference through oracle/ref_harness.py, CPU) and checks the restatement oracle/geo_oracle.py
-against it.  Run in the build container:   python -m oracle.make_golden
+against it.  Run where the reference checkout exists:   python -m oracle.make_golden
 
-Fixtures (compressed npz, a few MB in total):
+Fixtures (compressed npz, under 1 MB each):
   tests/golden/<workload>.npz        reference outputs at the stage boundaries of SURVEY.md section 8a for the
                                      deterministic pair synth.make_pair(workload, 0) and the deterministic weights
                                      weights.synthetic_state_dict(model, 7351)
-The big tensors are stored as strided row samples + float64 checksums (row index arrays are stored alongside).
+The big tensors are stored as strided row samples + float64 checksums (row index arrays are stored alongside); the level
+points and neighbour tables as digests + tie-order rows (oracle/fixture.py: compact / expand).
 """
 import os
 import sys
@@ -29,7 +30,8 @@ LIMITS = {'demo2k': [38, 36, 36, 38], 'modelnet717': [13, 21, 27], 'kitti4k': [2
 
 
 def run(workload, index=0, write=True):
-    """reference run + restatement check on pair ``index`` of the workload; ``write``: pack the fixture (pair 0 is the committed one)"""
+    """reference run + restatement check on pair ``index`` of the workload; ``write``: pack the fixture (pair 0 is the committed one);
+    ``write='reduced'``: return the reduced reference outputs of the pair (oracle/fixture.py: reduce_outputs)"""
     pair = make_pair(workload, index)
     cfg = make_cfg(pair['config'])
     limits = cfg.neighbor_limits or LIMITS[workload]
@@ -139,6 +141,21 @@ def run(workload, index=0, write=True):
     if not write:
         print(f'[{workload}] pair {index}: restatement == reference (no fixture written)')
         return
+    if write == 'reduced':
+        tables = {'neighbor_limits': np.array(limits)}
+        for i, p in enumerate(data['points']):
+            if i > 0:
+                tables[f'points_{i}'] = p.numpy()
+        for key in fixture.TABLE_KEYS:
+            for i, t in enumerate(data[key]):
+                tables[f'{key}_{i}'] = t.numpy().astype(np.uint16 if int(t.max()) < 65536 else np.int32)
+        all_metrics = dict(other_metrics, **{pair['config']: ref_metrics})
+        g = dict(fixture.compact(workload, tables, index), **fixture.reduce_outputs(ref_out, all_metrics))
+        o_all = {v: {k: float(x) for k, x in geo_oracle.evaluate(make_cfg(v), o, data['transform']).items()} for v in all_metrics}
+        bad = fixture.compare_outputs(o, g, o_all)
+        assert not bad, f'reduced comparison disagrees with the live one: {bad}'
+        print(f'[{workload}] pair {index}: restatement == reference, reduced outputs kept')
+        return g
     # ---- fixtures
     g = fixture.pack(data, taps, ref_out, o['node_corr_scores'], limits)
     g['metric_names'] = np.array(sorted(ref_metrics))
@@ -148,7 +165,7 @@ def run(workload, index=0, write=True):
         g['metric_values_' + other] = np.array([rm[k] for k in sorted(rm)], dtype=np.float64)
     os.makedirs(GOLD, exist_ok=True)
     path = os.path.join(GOLD, workload + '.npz')
-    np.savez_compressed(path, **g)
+    np.savez_compressed(path, **fixture.compact(workload, g))
     print(f'[{workload}] wrote {path} ({os.path.getsize(path) / 1e6:.2f} MB)')
 
 
@@ -172,12 +189,28 @@ def run_calibration():
     np.savez_compressed(os.path.join(GOLD, 'calibration.npz'), **g)
 
 
+OTHER_PAIRS = (('demo2k', 1), ('demo2k', 2), ('modelnet717', 1), ('modelnet717', 3), ('kitti4k', 1))
+
+
+def run_other_pairs():
+    """reduced reference outputs of further pairs of all three models -> tests/golden/other_pairs.npz"""
+    out = {'cases': np.array([f'{w}:{i}' for w, i in OTHER_PAIRS])}
+    for w, i in OTHER_PAIRS:
+        out.update({f'{w}:{i}/{k}': v for k, v in run(w, i, write='reduced').items()})
+    path = os.path.join(GOLD, 'other_pairs.npz')
+    np.savez_compressed(path, **out)
+    print(f'wrote {path} ({os.path.getsize(path) / 1e6:.2f} MB)')
+
+
 if __name__ == '__main__':
     assert ref_harness.available(), 'needs /root/reference'
+    # `other_pairs` = tests/golden/other_pairs.npz (reduced outputs of OTHER_PAIRS)
     # `check:<workload>:<pair index>` = compare the restatement with the reference on ANOTHER pair of the workload, write nothing
     for w in (sys.argv[1:] or ['demo2k', 'modelnet717', 'kitti4k', 'calibration']):
         if w.startswith('check:'):
             _, name, idx = w.split(':')
             run(name, int(idx), write=False)
+        elif w == 'other_pairs':
+            run_other_pairs()
         else:
             run_calibration() if w == 'calibration' else run(w)

@@ -4,7 +4,7 @@ Presents the two functions of the reference's pybind module ``geotransformer.ext
 (reference ``geotransformer/extensions/pybind.cpp:6-18``) on CPU torch tensors, backed by the
 UNMODIFIED reference C++ cores compiled by ``oracle/Makefile``.  Used to (a) pin the C restatement
 ``oracle/collate_oracle.c``, (b) serve as ``geotransformer.ext`` when the real reference Python is
-imported by ``oracle/ref_harness.py``, and (c) time the reference CPU collate on the GPU box.
+imported by ``oracle/ref_harness.py``, and (c) time the reference CPU collate in bench.py.
 """
 import ctypes
 import os

@@ -1,8 +1,8 @@
-"""TEST INFRASTRUCTURE ONLY (and only usable where /root/reference exists, i.e. the build container).
+"""TEST INFRASTRUCTURE ONLY (and only usable where the reference checkout exists).
 
 Imports the UNMODIFIED reference Python package from ``/root/reference`` so that
 ``oracle/make_golden.py`` can run the real reference forward on CPU and dump golden vectors into
-``tests/golden/``.  Nothing on the GPU box imports this module.
+``tests/golden/``.  No test imports this module.
 
 What has to be faked for the import to succeed (SURVEY.md section 8c):
   * debug-only third-party imports that are not installed: IPython, ipdb, matplotlib.pyplot,

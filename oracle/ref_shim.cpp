@@ -2,7 +2,7 @@
 //
 // C-ABI shim around the UNMODIFIED reference CPU ops so that the real reference code can be
 // (a) used to validate the restatement in oracle/collate_oracle.c and (b) timed as the
-// "reference" CPU baseline on the GPU box (the built .so travels, /root/reference does not).
+// "reference" CPU baseline on machines where only the built .so is present.
 //
 // The reference sources are compiled where they lie (see oracle/Makefile):
 //   geotransformer/extensions/extra/cloud/cloud.cpp

@@ -11,7 +11,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on the B200 box with -m gpu)')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on the GPU machine with -m gpu)')
 
 
 def pytest_collection_modifyitems(config, items):
@@ -28,8 +28,10 @@ GOLDEN = os.path.join(ROOT, 'tests', 'golden')
 
 @pytest.fixture(scope='session')
 def golden():
+    from oracle import fixture
+
     def load(name):
-        return np.load(os.path.join(GOLDEN, name + '.npz'))
+        return fixture.expand(name, np.load(os.path.join(GOLDEN, name + '.npz')))
     return load
 
 

@@ -1,7 +1,7 @@
-"""Tabulated structure embedding (GSE mode 5, csrc/gse_table.cu) on the GPU box: accuracy against the CPU oracle and the fp32 /
-tcgen05 kernels, the direct-evaluation path for arguments beyond the table, and the time of one batch-sized launch next to
-the tcgen05 3xFP16 kernel.  Prints one JSON line per check.  A CHECKER (lives under tests/ because it imports oracle/), not a
-pytest module: ``python tests/gse_table_check.py`` (profiles/r02_gse_table_check.txt is its output, then still under tools/)."""
+"""Tabulated structure embedding (GSE mode 5, csrc/gse_table.cu) on the GPU: accuracy against the CPU oracle and the fp32 /
+tensor-core kernels, the direct-evaluation path for arguments beyond the table, and the time of one batch-sized launch next to
+the wgmma 3xFP16 kernel.  Prints one JSON line per check.  A CHECKER (lives under tests/ because it imports oracle/), not a
+pytest module: ``python tests/gse_table_check.py``."""
 import json
 import math
 import os
@@ -44,7 +44,7 @@ def accuracy(c, n, sigma_d, extent, seed):
         got = GF.gse_embed(*args, mode=5, table=table_of(cu, **kw)).cpu()
         out[name + '_vs_oracle'] = float((got - want).abs().max())
     out['fp32_kernel_vs_oracle'] = float((GF.gse_embed(*args, mode=0).cpu() - want).abs().max())
-    out['tcgen05_3xfp16_vs_oracle'] = float((GF.gse_embed(*args, mode=3).cpu() - want).abs().max())
+    out['tensor_core_3xfp16_vs_oracle'] = float((GF.gse_embed(*args, mode=3).cpu() - want).abs().max())
     out['scale'] = float(want.abs().max())
     print(json.dumps(out), flush=True)
 
@@ -73,7 +73,7 @@ def timing(c, clouds, n, reps=5):
             if r:
                 ms.append(s.elapsed_time(e))
         res[f'mode{mode}_ms'] = sorted(ms)[len(ms) // 2]
-    res['max_abs_diff_table_vs_tcgen05'] = float((E3 - E5).abs().max())
+    res['max_abs_diff_table_vs_tensor_core'] = float((E3 - E5).abs().max())
     res['E_write_GBps_table'] = tot * c * 4 / (res['mode5_ms'] * 1e-3) / 1e9
     res['node_read_GBps_table'] = tot * 4 * c * 6 / (res['mode5_ms'] * 1e-3) / 1e9
     print(json.dumps(res), flush=True)

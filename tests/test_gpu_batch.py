@@ -54,7 +54,7 @@ def test_group_norm_per_pair_statistics(cloud_rows, c):
     got = GF.group_norm_batched(x.cuda(), gamma.cuda(), beta.cuda(), 32, cloud_rows, negative_slope=0.1, residual=res.cuda())
     err = (got.cpu() - want).abs().max().item()
     assert err < 2e-5, f'group_norm_batched: {err:.2e}'
-    # Linear -> GroupNorm with the statistics from the tcgen05 GEMM epilogue (tile partials folded per pair)
+    # Linear -> GroupNorm with the statistics from the tensor-core GEMM epilogue (tile partials folded per pair)
     k = 64
     w, b = torch.randn(c, k, generator=g) / 8.0, torch.randn(c, generator=g) * 0.1
     xin = torch.randn(n, k, generator=g)

@@ -1,5 +1,5 @@
 """End-to-end parity of the CUDA path against the committed golden fixtures (outputs of the REAL reference run in the
-build container by oracle/make_golden.py) on the deterministic pairs/weights.  Stage-wise with teacher forcing where
+reference checkout by oracle/make_golden.py) on the deterministic pairs/weights.  Stage-wise with teacher forcing where
 the reference itself is ill-conditioned (coarse top-k on random-weight features, SURVEY.md 'hard parts')."""
 import numpy as np
 import pytest
@@ -75,7 +75,7 @@ def check_forward(workload, cfg, model, pair, gold, native=False):
         got = _rows(taps[k], gold[k + '_rows'])
         err = np.abs(got - gold[k + '_sample']).max() / max(np.abs(gold[k + '_sample']).max(), 1.0)
         assert err < tol, f'{k}: rel err {err:.2e}'
-    # structure embedding of the reference cloud (sampled (i, j) rows): E rms ~0.6, budget 2e-5 (3-term split on tcgen05)
+    # structure embedding of the reference cloud (sampled (i, j) rows): E rms ~0.6, budget 2e-5 (3-term split on the tensor cores)
     nc = data['lengths_host'][-1][0]
     emb = model.transformer.embedding(data['points'][-1][:nc].contiguous())
     got = _rows(emb, gold['ref_embeddings_rows'])
@@ -213,7 +213,7 @@ def test_forward_matches_reference(workload, cfg_name, golden, models):
 
 
 # ---- BASELINE.json configs 3 and 4 at full size: the pinned restatement (oracle/geo_oracle.py == the real reference with 0.0
-# difference on the committed fixtures, KITTI branch included: tests/golden/kitti4k.npz) is run LIVE on the box's host cores
+# difference on the committed fixtures, KITTI branch included: tests/golden/kitti4k.npz) is run LIVE on the host cores
 # and packed into the fixture layout, so the headline workload goes through exactly the same stage-wise checks.
 FULL = [('3dmatch20k', '3dmatch'), ('kitti20k', 'kitti')]
 _LIVE = {}

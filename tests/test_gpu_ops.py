@@ -62,7 +62,7 @@ def test_kpconv(cin, cout, h):
             sd['w.bias'].cuda(), 0.12)
     old = GF.KPCONV_MODE
     try:
-        GF.KPCONV_MODE = 'tc'        # gather kernel + tcgen05 3xTF32 GEMM (K = 15*cin: tensor-core accumulation error grows with K)
+        GF.KPCONV_MODE = 'tc'        # gather kernel + wgmma 3xTF32 GEMM (K = 15*cin: tensor-core accumulation error grows with K)
         close(GF.kpconv(*args), want, 2e-5 if cin <= 64 else 5e-5, f'kpconv tc {cin}->{cout}')
         GF.KPCONV_MODE = 'fused'     # single fp32 CUDA-core kernel
         close(GF.kpconv(*args), want, 2e-5, f'kpconv fused {cin}->{cout}')
@@ -84,7 +84,7 @@ def test_linear(m, k, n):
 @pytest.mark.parametrize('m,k,n', [(64, 32, 32), (647, 256, 768), (333, 64, 32), (1000, 1536, 512), (40000, 64, 128), (4100, 1024, 256),
                                    (130, 36, 48), (129, 2048, 1024)])
 def test_linear_tensor_core_3xtf32_matches_fp32(m, k, n):
-    """tcgen05 3xTF32 Linear (default) vs the fp32 CUDA-core kernel and torch: fp32-level agreement"""
+    """wgmma 3xTF32 Linear (default) vs the fp32 CUDA-core kernel and torch: fp32-level agreement"""
     from geotransformer_b200 import _lib
     g = torch.Generator().manual_seed(m + k)
     x, w, b = torch.randn(m, k, generator=g), torch.randn(n, k, generator=g) / math.sqrt(k), torch.randn(n, generator=g)
@@ -136,7 +136,7 @@ def test_linear_split_k(m, k, n):
 @pytest.mark.parametrize('m,k,n,groups', [(40000, 64, 128, 32), (40000, 480, 32, 32), (20011, 32, 128, 32), (24000, 64, 256, 32),
                                           (19000, 96, 128, 0)])
 def test_linear_persistent_tile_loop(m, k, n, groups):
-    """multi-wave GEMMs through the persistent kernel (two TMEM accumulator sets, operand ring running across tiles): bitwise
+    """multi-wave GEMMs through the persistent kernel (operand ring running across tiles): bitwise
     the same output and GroupNorm statistics as one CTA per tile"""
     from geotransformer_b200 import _lib
     g = torch.Generator().manual_seed(m + k)
@@ -191,7 +191,7 @@ def test_group_norm_variants(n, c):
                                           (700, 256, 256, 32), (130, 512, 1024, 32), (257, 256, 2048, 32), (640, 64, 512, 8),
                                           (37, 64, 128, 32), (300, 100, 48, 4)])
 def test_linear_group_norm_fused_statistics(m, k, n, groups):
-    """UnaryBlock as one op: GroupNorm statistics produced by the tcgen05 GEMM epilogue (channels per group 1..64, ragged last
+    """UnaryBlock as one op: GroupNorm statistics produced by the tensor-core GEMM epilogue (channels per group 1..64, ragged last
     row tile, several column tiles) against torch; shapes the tensor-core path rejects fall back to the stand-alone kernels"""
     g = torch.Generator().manual_seed(m + n)
     x = torch.randn(m, k, generator=g)
@@ -390,7 +390,7 @@ def test_gse_indices_and_embedding(mn):
 
 @pytest.mark.parametrize('n', [7, 100, 271])
 def test_gse_embedding_tensor_core_modes(n):
-    """tcgen05 contraction: 3xTF32 (default) must be fp32-accurate, 1xTF32 within TF32 rounding; vs the oracle"""
+    """tensor-core contraction: 3xTF32 (default) must be fp32-accurate, 1xTF32 within TF32 rounding; vs the oracle"""
     g = torch.Generator().manual_seed(n)
     c = 256
     pts = torch.rand(n, 3, generator=g) * 2.0
@@ -511,14 +511,14 @@ def test_gse_embedding_generic_channels():
     got = GF.gse_embed(d, a, cu['e.embedding.div_term'], cu['e.proj_d.weight'], cu['e.proj_a.weight'], cu['e.proj_d.bias'],
                        cu['e.proj_a.bias'], cu['e.proj_d.weight'].t().contiguous(), cu['e.proj_a.weight'].t().contiguous(), mode=0)
     close(got, want, 2e-5, 'structure embedding C=128')
-    # tensor-core path for hidden 128: the 3xFP16 tcgen05 kernel instantiated for N = 128 (two angle + two distance chunks per tile)
+    # tensor-core path for hidden 128: the 3xFP16 wgmma kernel instantiated for N = 128 (two angle + two distance chunks per tile)
     for nn in (40, 173):
         pts = torch.rand(nn, 3, generator=g) * 20
         want = G.structure_embedding(sd, 'e.', pts, 4.8, 15, 3)
         d, a = GF.gse_indices(pts.cuda(), 4.8, 15, 3)
         got = GF.gse_embed(d, a, cu['e.embedding.div_term'], cu['e.proj_d.weight'], cu['e.proj_a.weight'], cu['e.proj_d.bias'],
                            cu['e.proj_a.bias'], cu['e.proj_d.weight'].t().contiguous(), cu['e.proj_a.weight'].t().contiguous(), mode=3)
-        close(got, want, 3e-5, f'structure embedding C=128, tcgen05 3xFP16 (n={nn})')
+        close(got, want, 3e-5, f'structure embedding C=128, wgmma 3xFP16 (n={nn})')
 
 
 def test_transformer_layers(mn, models):

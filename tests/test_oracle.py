@@ -1,5 +1,5 @@
-"""The oracle itself (CPU): plain-C collate restatement vs the real reference build (oracle/_ref), and the
-torch restatement of the forward vs the committed reference fixtures."""
+"""The oracle itself (CPU): plain-C collate restatement and op restatements vs the stored outputs of the real reference
+(tests/golden/reference_ops.npz), and the torch restatement of the forward vs the committed reference fixtures."""
 import numpy as np
 import pytest
 import torch
@@ -7,7 +7,6 @@ import torch
 from geotransformer_b200.synth import make_pair
 from oracle import collate_oracle as co
 from oracle import geo_oracle as G
-from oracle import ref_ext
 
 
 def _stack(pair):
@@ -15,18 +14,19 @@ def _stack(pair):
     return pts, torch.tensor([len(pair['ref_points']), len(pair['src_points'])])
 
 
-@pytest.mark.skipif(not ref_ext.available(), reason='oracle/_ref not built')
+@pytest.fixture(scope='module')
+def reference_ops():
+    """digests of the reference's outputs on the seeded inputs of oracle/ref_vectors.py (tests/golden/reference_ops.npz)"""
+    import os
+    return np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'reference_ops.npz'))
+
+
 @pytest.mark.parametrize('workload,voxel', [('demo2k', 0.05), ('3dmatch20k', 0.05), ('modelnet717', 0.1)])
-def test_c_restatement_matches_reference_build(workload, voxel):
-    pts, lens = _stack(make_pair(workload, 1))
-    for _ in range(3):
-        a, al = ref_ext.grid_subsampling(pts, lens, voxel)
-        b, bl = co.grid_subsampling(pts, lens, voxel)
-        assert torch.equal(al, bl) and torch.equal(a, b)          # values AND unordered_map order
-        pts, lens, voxel = a, al, voxel * 2
-    na = ref_ext.radius_neighbors(pts, pts, lens, lens, voxel * 1.25)
-    nb = co.radius_neighbors(pts, pts, lens, lens, voxel * 1.25)
-    assert torch.equal(na, nb)
+def test_c_restatement_matches_reference_build(workload, voxel, reference_ops):
+    """three grid_subsampling levels (values AND unordered_map order) and the radius_neighbors table of the last level (values
+    AND order) of the plain-C restatement, bit for bit equal to the reference build's on pair 1 of the workload"""
+    from oracle import ref_vectors
+    assert not ref_vectors.mismatches(ref_vectors.collate_results(co, workload, voxel), reference_ops, 'collate:')
 
 
 def test_grid_subsample_golden_order(golden):
@@ -40,16 +40,11 @@ def test_grid_subsample_golden_order(golden):
         v *= 2
 
 
-def test_rehash_schedule_edge_sizes():
-    """clouds whose voxel counts straddle the libstdc++ rehash thresholds (13/14, 29/30, 59/60, 127/128)"""
-    if not ref_ext.available():
-        pytest.skip('oracle/_ref not built')
-    g = torch.Generator().manual_seed(0)
-    for n in (1, 2, 12, 13, 14, 28, 29, 30, 58, 59, 60, 126, 127, 128, 129, 257, 258, 542):
-        pts = torch.rand(n, 3, generator=g) * 100.0          # one point per voxel with high probability
-        a, al = ref_ext.grid_subsampling(pts, torch.tensor([n]), 0.5)
-        b, bl = co.grid_subsampling(pts, torch.tensor([n]), 0.5)
-        assert torch.equal(a, b), n
+def test_rehash_schedule_edge_sizes(reference_ops):
+    """clouds whose voxel counts straddle the libstdc++ rehash thresholds (13/14, 29/30, 59/60, 127/128): grid_subsampling of
+    the restatement bit for bit equal to the reference build's"""
+    from oracle import ref_vectors
+    assert not ref_vectors.mismatches(ref_vectors.collate_results(co, 'rehash'), reference_ops, 'collate:')
 
 
 def test_forward_restatement_matches_reference_fixture(golden, models):
@@ -147,92 +142,48 @@ def test_tabulated_structure_embedding_model_vs_oracle(c, n, sigma_d, extent):
     assert float((coarse - want).abs().max()) < 5e-5
 
 
-@pytest.mark.skipif(not ref_ext.available(), reason='oracle/_ref not built')
-def test_c_restatement_matches_reference_build_on_adversarial_small_inputs():
-    """hypothesis: several ragged clouds per batch, coordinates quantised to a coarse lattice (many points per voxel, exact-distance
-    ties, duplicated points), negative coordinates, 1-point clouds.  grid_subsampling: values AND unordered_map order bit for bit;
-    radius_neighbors: identical rows up to the order inside exact-distance tie groups (std::sort is unstable in both)."""
-    from hypothesis import given, settings, strategies as st
-
-    @settings(max_examples=60, deadline=None, derandomize=True)
-    @given(st.lists(st.integers(1, 40), min_size=1, max_size=4), st.integers(0, 2 ** 31 - 1), st.sampled_from([0.0, 0.05, 0.25]),
-           st.sampled_from([0.3, 0.5, 1.0]))
-    def check(lengths, seed, lattice, voxel):
-        g = torch.Generator().manual_seed(seed)
-        n = sum(lengths)
-        pts = (torch.rand(n, 3, generator=g) - 0.5) * 4.0
-        if lattice > 0:
-            pts = torch.round(pts / lattice) * lattice
-        pts = pts.contiguous()
-        lens = torch.tensor(lengths)
-        a, al = ref_ext.grid_subsampling(pts, lens, voxel)
-        b, bl = co.grid_subsampling(pts, lens, voxel)
-        assert torch.equal(al, bl) and torch.equal(a, b)
-        r = voxel * 1.5
-        na = ref_ext.radius_neighbors(pts, pts, lens, lens, r)
-        nb = co.radius_neighbors(pts, pts, lens, lens, r)
-        assert na.shape == nb.shape
-        assert torch.equal(G.canonical_neighbors(pts, pts, na), G.canonical_neighbors(pts, pts, nb))
-        # sub-sampled queries against the full support (the 'subsampling' tables of the collate)
-        nq = ref_ext.radius_neighbors(a, pts, al, lens, r)
-        nr = co.radius_neighbors(a, pts, al, lens, r)
-        assert nq.shape == nr.shape
-        assert torch.equal(G.canonical_neighbors(a, pts, nq), G.canonical_neighbors(a, pts, nr))
-
-    check()
+def test_c_restatement_matches_reference_build_on_adversarial_small_inputs(reference_ops):
+    """60 seeded cases: several ragged clouds per batch, coordinates quantised to a coarse lattice (many points per voxel,
+    exact-distance ties, duplicated points), negative coordinates, 1-point clouds.  grid_subsampling: values AND unordered_map
+    order bit for bit; radius_neighbors (self and sub-sampled queries): identical rows up to the order inside exact-distance
+    tie groups (std::sort is unstable in both) -- all against the reference build's outputs"""
+    from oracle import ref_vectors
+    assert not ref_vectors.mismatches(ref_vectors.collate_results(co, 'adversarial'), reference_ops, 'collate:')
 
 
-def test_boundary_2_op_restatements_match_the_real_reference_live():
-    """oracle/pin_ops_live.py in its own process (it imports the unmodified reference package and patches Tensor.cuda): the oracle's
-    pairwise_distance / knn_partition / get_point_to_node_indices / point_to_node_partition / ball_query_partition / apply_transform
-    are bit-identical to geotransformer.modules.ops on seeded inputs.  Only where /root/reference exists (the build container)."""
+def test_boundary_2_op_restatements_match_the_reference(reference_ops):
+    """the oracle's pairwise_distance / knn_partition / get_point_to_node_indices / point_to_node_partition / ball_query_partition /
+    apply_transform are bit-identical to geotransformer.modules.ops on seeded inputs (oracle/ref_vectors.py)"""
+    from oracle import ref_vectors
+    assert not ref_vectors.mismatches(ref_vectors.ops_results(G), reference_ops, 'ops:')
+
+
+def test_restatement_matches_the_reference_on_other_pairs(models):
+    """the committed fixtures pin the restatement on pair 0 of each workload; here oracle/geo_oracle.py runs on further seeded
+    pairs of all three models (tests/golden/other_pairs.npz, written by ``python -m oracle.make_golden other_pairs``) and is
+    compared with the reference's outputs on them: collate tables up to tie order (the reference's tie order teacher-forced),
+    features, matching scores, correspondences (as a set when two coarse scores tie to 1e-5), transform, gt superpoint pairs,
+    all three Evaluator variants"""
     import os
-    import subprocess
-    import sys
-    from oracle import ref_harness
-    if not (ref_harness.available() and ref_ext.available()):
-        pytest.skip('needs /root/reference and oracle/_ref (build container only)')
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    r = subprocess.run([sys.executable, '-m', 'oracle.pin_ops_live'], cwd=root, capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0 and 'pinned:' in r.stdout, r.stdout[-2000:] + r.stderr[-2000:]
-
-
-def test_golden_fixtures_regenerate_bit_identically_from_the_real_reference(tmp_path):
-    """python -m oracle.make_golden (the REAL reference package imported from /root/reference, CPU) into a scratch directory gives,
-    array for array, ALL committed fixtures tests/golden/{demo2k,modelnet717,kitti4k,calibration}.npz -- and the script itself asserts that the restatement
-    oracle/geo_oracle.py equals the reference run.  Only in the build container (the GPU box has no /root/reference)."""
-    import os
-    import subprocess
-    import sys
-    from oracle import ref_harness
-    if not (ref_harness.available() and ref_ext.available()):
-        pytest.skip('needs /root/reference and oracle/_ref (build container only)')
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    env = dict(os.environ, GEOB200_GOLDEN_OUT=str(tmp_path))
-    names = ('demo2k', 'modelnet717', 'kitti4k', 'calibration')
-    r = subprocess.run([sys.executable, '-m', 'oracle.make_golden'] + list(names), cwd=root, env=env, capture_output=True, text=True, timeout=1800)
-    assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-2000:]
-    for w in names:
-        new, old = np.load(tmp_path / f'{w}.npz'), np.load(os.path.join(root, 'tests', 'golden', f'{w}.npz'))
-        assert sorted(new.files) == sorted(old.files)
-        for k in new.files:
-            a, b = new[k], old[k]
-            assert a.shape == b.shape and a.dtype == b.dtype, (w, k)
-            assert np.array_equal(a, b, equal_nan=True) if a.dtype.kind == 'f' else np.array_equal(a, b), (w, k)
-
-
-def test_restatement_matches_the_real_reference_on_other_pairs_live():
-    """the committed fixtures pin the restatement on pair 0 of each workload; here the real reference and oracle/geo_oracle.py run
-    LIVE on further seeded pairs of all three models (collate tables up to tie order, features, matching scores, correspondences
-    as a set when two coarse scores tie to 1e-5, transform, gt superpoint pairs, all three Evaluator variants) -- make_golden's
-    own assertions, nothing written.  Build container only."""
-    import os
-    import subprocess
-    import sys
-    from oracle import ref_harness
-    if not (ref_harness.available() and ref_ext.available()):
-        pytest.skip('needs /root/reference and oracle/_ref (build container only)')
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    cases = ['check:demo2k:1', 'check:demo2k:2', 'check:modelnet717:1', 'check:modelnet717:3', 'check:kitti4k:1']
-    r = subprocess.run([sys.executable, '-m', 'oracle.make_golden'] + cases, cwd=root, capture_output=True, text=True, timeout=1800)
-    assert r.returncode == 0 and r.stdout.count('restatement == reference') == len(cases), r.stdout[-3000:] + r.stderr[-3000:]
+    from geotransformer_b200.config import make_cfg
+    from oracle import fixture
+    z = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'other_pairs.npz'))
+    cases = z['cases'].tolist()
+    assert len(cases) == 5
+    for case in cases:
+        workload, index = case.split(':')
+        g = {k[len(case) + 1:]: z[k] for k in z.files if k.startswith(case + '/')}
+        pair = make_pair(workload, int(index))
+        cfg, sd, _ = models(pair['config'])
+        ref = fixture.expand(workload, g, int(index))                      # the reference's level points and tables
+        data = G.collate_pair(pair, cfg, g['neighbor_limits'].tolist())
+        for i in range(1, cfg.backbone.num_stages):
+            assert np.array_equal(data['points'][i].numpy(), ref[f'points_{i}']), (case, i)
+        for key in fixture.TABLE_KEYS:
+            data[key] = [torch.from_numpy(ref[f'{key}_{i}'].astype(np.int64)) for i in range(len(data[key]))]
+        with torch.no_grad():
+            out = G.forward(sd, cfg, data)
+        variants = [k[len('metric_names_'):] for k in g if k.startswith('metric_names_')]
+        metrics = {v: {k: float(x) for k, x in G.evaluate(make_cfg(v), out, data['transform']).items()} for v in variants}
+        assert len(variants) == 3
+        assert not fixture.compare_outputs(out, g, metrics), (case, fixture.compare_outputs(out, g, metrics))

@@ -46,7 +46,7 @@ for s in (1, 4):
           'total', round(sum(sum(v) / len(v) for v in eng.stage_times.values()), 3))
     eng.close()
 
-# is the GPU the limit?  triple the Sinkhorn work (+1.1 ms of full-GPU kernels per pair) and compare
+# is the GPU the limit?  triple the Sinkhorn work (more full-GPU kernel time per pair) and compare
 it0 = model.optimal_transport.num_iterations
 for s, iters in ((4, it0), (4, 3 * it0), (6, it0), (6, 3 * it0)):
     model.optimal_transport.num_iterations = iters

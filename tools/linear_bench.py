@@ -1,4 +1,4 @@
-"""Micro-benchmark of the tcgen05 Linear (dev tool): CUDA-event time per call for the GEMM shapes of the 3DMatch model.
+"""Micro-benchmark of the tensor-core (wgmma) Linear (dev tool): CUDA-event time per call for the GEMM shapes of the 3DMatch model.
 Run from any checkout: uses the package next to this file's parent directory (or GEOB_ROOT)."""
 import os
 import sys

@@ -3,7 +3,7 @@
 metrics the roofline discussion uses, one row per launch, plus a per-kernel summary.
 
     ncu -i capture.ncu-rep --page raw --csv > raw.csv
-    python tools/ncu_select.py raw.csv profiles/r02_ncu_selected.csv
+    python tools/ncu_select.py raw.csv selected.csv
 """
 import csv
 import sys
@@ -16,8 +16,7 @@ KEEP = [
     'sm__inst_executed_pipe_fma.avg.pct_of_peak_sustained_active', 'smsp__issue_active.avg.pct_of_peak_sustained_active',
     'sm__warps_active.avg.pct_of_peak_sustained_active', 'launch__registers_per_thread', 'launch__shared_mem_per_block_dynamic',
     'launch__waves_per_multiprocessor', 'launch__occupancy_limit_registers', 'launch__occupancy_limit_shared_mem',
-    'sm__ops_path_tensor_op_utchmma_src_tf32_dst_fp32_sparsity_off.avg.pct_of_peak_sustained_elapsed',
-    'sm__ops_path_tensor_op_utchmma_src_fp16_dst_fp32_sparsity_off.avg.pct_of_peak_sustained_elapsed',
+    'sm__pipe_tensor_cycles_active.avg.pct_of_peak_sustained_elapsed',
     'sm__inst_executed_pipe_uniform.sum', 'sm__inst_executed_pipe_xu.avg.pct_of_peak_sustained_active',
 ]
 

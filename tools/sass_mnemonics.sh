@@ -1,15 +1,15 @@
 #!/bin/bash
-# Counts the SASS mnemonics that prove which hardware paths each object of libgeob200.so uses (B200_PROFILING.md):
-#   UTCHMMA / UTCQMMA = tcgen05.mma (fp16/bf16/tf32 / fp8-int8 kinds), LDTM = tcgen05.ld (TMEM -> registers), UTCBAR = tcgen05.commit,
-#   UTMALDG = cp.async.bulk.tensor (TMA tiled load), UBLKCP = cp.async.bulk (TMA 1-D bulk copy), SYNCS = mbarrier ops,
-#   LDGSTS = cp.async (per-thread), HMMA/IMMA/DMMA = legacy mma.sync (must be 0: no recompiled wmma/mma.sync kernels).
-# usage: tools/sass_mnemonics.sh > profiles/r02_sass_mnemonics.txt
+# Counts the SASS mnemonics that show which hardware paths each object of libgeob200.so uses:
+#   HGMMA = wgmma.mma_async (warpgroup tensor-core MMA), UTMALDG = cp.async.bulk.tensor (TMA tiled load),
+#   UBLKCP = cp.async.bulk (TMA 1-D bulk copy), SYNCS = mbarrier ops, LDGSTS = cp.async (per-thread),
+#   HMMA/IMMA/DMMA = warp-level mma.sync (expected 0: the tensor-core kernels use wgmma).
+# usage: tools/sass_mnemonics.sh   (after the build)
 cd "$(dirname "$0")/../geotransformer_b200/csrc" || exit 1
-echo "cuobjdump -sass of every object linked into geotransformer_b200/libgeob200.so (nvcc $(nvcc --version | grep -o 'release [0-9.]*'), -gencode arch=compute_100a,code=sm_100a)"
-printf "%-18s %8s %8s %6s %8s %7s %7s %6s %7s %11s\n" object UTCHMMA UTCQMMA LDTM UTMALDG UBLKCP UTCBAR SYNCS LDGSTS legacy_mma
+echo "cuobjdump -sass of every object linked into geotransformer_b200/libgeob200.so (nvcc $(nvcc --version | grep -o 'release [0-9.]*'), -gencode arch=compute_90a,code=sm_90a)"
+printf "%-18s %8s %8s %7s %6s %7s %11s\n" object HGMMA UTMALDG UBLKCP SYNCS LDGSTS warp_mma
 for f in *.o; do
   cuobjdump -sass "$f" 2>/dev/null | awk -v name="$f" '
-    / UTCHMMA/{a++} / UTCQMMA/{q++} / LDTM/{l++} / UTMALDG/{t++} / UBLKCP/{b++} / UTCBAR/{c++} / SYNCS/{s++} / LDGSTS/{g++}
-    /[ .]HMMA|[ .]IMMA|[ .]DMMA/{ if ($0 !~ /UTC/) m++ }
-    END{printf "%-18s %8d %8d %6d %8d %7d %7d %6d %7d %11d\n", name, a, q, l, t, b, c, s, g, m}'
+    / HGMMA/{a++} / UTMALDG/{t++} / UBLKCP/{b++} / SYNCS/{s++} / LDGSTS/{g++}
+    /[ .]HMMA|[ .]IMMA|[ .]DMMA/{ m++ }
+    END{printf "%-18s %8d %8d %7d %6d %7d %11d\n", name, a, t, b, s, g, m}'
 done
