@@ -53,6 +53,7 @@ _sig('geob200_linear_group_norm_batched', c_int, P, I64, P, P, I64, I64, I64, I6
 _sig('geob200_maxpool', c_int, P, P, I64, I64, I64, I64, P, P)
 _sig('geob200_upsample_concat', c_int, P, P, I64, I64, P, I64, I64, I64, P, P)
 _sig('geob200_point_to_node_partition', c_int, P, I64, P, I64, I64, P, P, P, P, P, P, P)
+_sig('geob200_point_to_node_partition_batched', c_int, P, P, I64, P, P, I64, P, P, P, P, P, P)
 _sig('geob200_gather_rows', c_int, P, I64, I64, P, I64, P, P)
 _sig('geob200_knn_partition', c_int, P, I64, P, I64, I64, P, P, P)
 _sig('geob200_pairwise_distance', c_int, P, I64, P, I64, I64, c_int, P, P)
@@ -80,12 +81,23 @@ _sig('geob200_sinkhorn', c_int, P, P, P, P, I64, I64, I64, F, P, P)
 _sig('geob200_lgr_workspace_bytes', SZ, I64, I64, I64)
 _sig('geob200_local_global_registration', c_int, P, P, P, P, P, I64, I64, I64, I64, F, c_int, F, I64, I64, P, P, P, P, P,
      P, P, P, P, P, SZ, P)
+_sig('geob200_superpoint_matching_batched_workspace_bytes', SZ, I64, I64, I64)
+_sig('geob200_superpoint_matching_batched', c_int, P, I64, P, I64, P, I64, c_int, P, P, P, P, SZ, P)
+_sig('geob200_gather_patches_batched', c_int, P, I64, I64, P, P, P, P, I64, P, P, P, P, P)
+_sig('geob200_patch_scores_batched', c_int, P, I64, I64, P, P, P, I64, I64, P, P)
+_sig('geob200_lgr_batched_workspace_bytes', SZ, I64, I64, I64, I64)
+_sig('geob200_local_global_registration_batched', c_int, P, P, P, P, P, I64, I64, I64, I64, I64, F, c_int, F, I64, I64, P, P, P, P,
+     P, P, I64, P, P, P, P, SZ, P)
 _sig('geob200_weighted_procrustes', c_int, P, P, P, I64, I64, F, F, P, P)
 
 _sig('geob200_node_correspondences_workspace_bytes', SZ, I64, I64, I64)
 _sig('geob200_node_correspondences', c_int, P, P, P, P, P, P, P, P, I64, I64, I64, P, F, P, P, P, P, SZ, P)
+_sig('geob200_node_correspondences_batched_workspace_bytes', SZ, I64, I64, I64)
+_sig('geob200_node_correspondences_batched', c_int, P, P, P, P, I64, P, I64, P, F, P, P, P, P, SZ, P)
 _sig('geob200_evaluate', c_int, P, P, I64, F, P, P, I64, P, P, I64, F, P, P, P, I64, c_int, F, F, F, P, P)
 _sig('geob200_evaluate_counts', c_int, P, P, I64, P, F, P, P, I64, P, P, P, I64, P, F, P, P, P, I64, c_int, F, F, F, P, P)
+_sig('geob200_evaluate_batched', c_int, P, P, P, F, P, P, I64, P, P, P, I64, P, F, P, P, I64, P, I64, P, P, c_int, F, F, F, P, I64,
+     P)
 
 _sig('geob200_linear_profile_enable', c_int, c_int)
 _sig('geob200_set_split_k', c_int, c_int)

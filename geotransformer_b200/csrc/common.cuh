@@ -112,6 +112,22 @@ int kpconv_group_norm_impl(const float* s_feats, const float* q_points, const fl
 int maxpool_seg(const float* x, const int64_t* neighbors, int64_t n_query, int64_t n_support, int64_t n_neighbors, int64_t channels,
                 float* y, const GnSeg* seg, const int* cloud_max, void* stream);
 
+// Per-pair stages of a batch (grouping, ground-truth correspondences, matching, patches, LGR, metrics): one launch covers every
+// segment -- a cloud or a pair -- with the segment index in blockIdx.y.  Rows [start[s], start[s] + count[s]) of a row-major
+// array belong to segment s.  A single-pair call is the same kernel with n = 1 (or 2 clouds) and start = 0.  Passed by value.
+struct Segs {
+    int n;
+    int max;                               // largest count: the grid extent per segment
+    int start[GEOB_MAX_CLOUDS];
+    int count[GEOB_MAX_CLOUDS];
+};
+// segments of the given sizes laid out back to back; -1 (error set) when n is out of range or the rows overflow int
+int segs_from_counts(Segs* s, int64_t n, const int64_t* counts);
+Segs segs_one(int64_t count);
+Segs segs_range(const Segs& s, int first, int n);                   // segments first .. first + n - 1 of s
+// per pair p: the n_ref[p] x n_src[p] matrix of pair p, matrices back to back (ref = pairs' ref clouds, src = their src clouds)
+int segs_products(Segs* s, const Segs& ref, const Segs& src);
+
 // Bump allocator over a caller-provided workspace.
 struct Arena {
     char* base;

@@ -21,14 +21,22 @@ __device__ __forceinline__ void xform(const float* T, float x, float y, float z,
     oz = fmaf(z, T[10], fmaf(y, T[9], x * T[8])) + T[11];
 }
 
-// one warp per node: (optionally transformed) node, transformed patch points, enclosing radius over the valid patch points
+// one warp per node: (optionally transformed) node, transformed patch points, enclosing radius over the valid patch points.
+// Cloud s = blockIdx.y (rows at cl.start[s] of every array); clouds s >= t_first are transformed by T + 16 * (s - t_first).
 __global__ void __launch_bounds__(256) nc_prepare_kernel(const float* __restrict__ nodes, const float* __restrict__ knn_pts,
-                                                         const unsigned char* __restrict__ knn_masks, int n_nodes, int K,
-                                                         const float* __restrict__ T, float* __restrict__ nodes_out,
+                                                         const unsigned char* __restrict__ knn_masks, const __grid_constant__ Segs cl, int K,
+                                                         const float* __restrict__ T, int t_first, float* __restrict__ nodes_out,
                                                          float* __restrict__ pts_out, float* __restrict__ max_dist, int* __restrict__ n_valid) {
     const int lane = threadIdx.x & 31;
+    const int s = blockIdx.y;
     const int m = blockIdx.x * 8 + (threadIdx.x >> 5);
-    if (m >= n_nodes) return;
+    if (m >= cl.count[s]) return;
+    {
+        const long long r = cl.start[s];
+        nodes += 3 * r; nodes_out += 3 * r; knn_pts += 3 * r * K; pts_out += 3 * r * K; max_dist += r; n_valid += r;
+        if (knn_masks != nullptr) knn_masks += r * K;
+        T = (T != nullptr && s >= t_first) ? T + 16 * (s - t_first) : nullptr;
+    }
     float nx = nodes[3 * m], ny = nodes[3 * m + 1], nz = nodes[3 * m + 2];
     if (T != nullptr) xform(T, nx, ny, nz, nx, ny, nz);
     float md = 0.f;
@@ -60,8 +68,24 @@ __global__ void __launch_bounds__(256) nc_overlap_kernel(const float* __restrict
                                                          const unsigned char* __restrict__ src_knn_masks,
                                                          const unsigned char* __restrict__ ref_masks, const unsigned char* __restrict__ src_masks,
                                                          const float* __restrict__ ref_max, const float* __restrict__ src_max,
-                                                         const int* __restrict__ ref_nv, const int* __restrict__ src_nv, int M, int N, int K,
-                                                         float pos_radius, float* __restrict__ overlap /* (M,N) */) {
+                                                         const int* __restrict__ ref_nv, const int* __restrict__ src_nv,
+                                                         const __grid_constant__ Segs R, const __grid_constant__ Segs Q,
+                                                         const __grid_constant__ Segs NN, int K, float pos_radius,
+                                                         float* __restrict__ overlap /* (M,N) per pair */) {
+    // pair b = blockIdx.y: ref rows at R.start[b], src rows at Q.start[b], its (M,N) overlaps at NN.start[b]
+    const int b = blockIdx.y;
+    const int M = R.count[b], N = Q.count[b];
+    if ((int)blockIdx.x >= M) return;
+    {
+        const long long r = R.start[b], q = Q.start[b];
+        ref_nodes += 3 * r; ref_pts += 3 * r * K; ref_max += r; ref_nv += r;
+        if (ref_knn_masks != nullptr) ref_knn_masks += r * K;
+        if (ref_masks != nullptr) ref_masks += r;
+        src_nodes += 3 * q; src_pts += 3 * q * K; src_max += q; src_nv += q;
+        if (src_knn_masks != nullptr) src_knn_masks += q * K;
+        if (src_masks != nullptr) src_masks += q;
+        overlap += NN.start[b];
+    }
     extern __shared__ float sm[];
     float4* rp = reinterpret_cast<float4*>(sm);         // [K] (x,y,z,|p|^2), invalid points flagged by w < 0
     float4* sp = rp + K;                                 // [K]
@@ -114,9 +138,13 @@ __global__ void __launch_bounds__(256) nc_overlap_kernel(const float* __restrict
     }
 }
 
-// ordered compaction of overlap > 0 into (C,2) indices + overlaps; single CTA
-__global__ void __launch_bounds__(1024) nc_compact_kernel(const float* __restrict__ overlap, int M, int N, long long* __restrict__ idx,
-                                                          float* __restrict__ ov_out, int* __restrict__ count) {
+// ordered compaction of overlap > 0 into (C,2) indices + overlaps; one CTA per pair blockIdx.x, rows at NN.start of the pair
+__global__ void __launch_bounds__(1024) nc_compact_kernel(const float* __restrict__ overlap, const __grid_constant__ Segs R,
+                                                          const __grid_constant__ Segs Q, const __grid_constant__ Segs NN,
+                                                          long long* __restrict__ idx, float* __restrict__ ov_out, int* __restrict__ count) {
+    const int b = blockIdx.x;
+    const int M = R.count[b], N = Q.count[b];
+    overlap += NN.start[b]; idx += 2ll * NN.start[b]; ov_out += NN.start[b]; count += b;
     __shared__ int warp_tot[32];
     __shared__ int carry;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -161,15 +189,30 @@ __global__ void __launch_bounds__(1024) nc_compact_kernel(const float* __restric
 // mode 0 (3DMatch loss.py:133-145): RMSE of inv(T_gt) T_est x - x, RR = RMSE < rmse_threshold
 // mode 1 (KITTI   loss.py:133-138): no RMSE (NaN), RR = RRE < rre_threshold and RTE < rte_threshold
 // mode 2 (ModelNet loss.py:133-145): RMSE of T_est x - T_gt x, RR as in mode 1
-__global__ void __launch_bounds__(1024) evaluate_kernel(const long long* __restrict__ gt_idx, const float* __restrict__ gt_ov, int n_gt,
-                                                        float acc_overlap, const long long* __restrict__ ref_corr_idx,
-                                                        const long long* __restrict__ src_corr_idx, int n_node_corr,
-                                                        const float* __restrict__ ref_corr_pts, const float* __restrict__ src_corr_pts,
-                                                        int n_corr, float acc_radius, const float* __restrict__ T_gt,
-                                                        const float* __restrict__ T_est, const float* __restrict__ src_points, int n_src,
-                                                        int mode, float acc_rmse, float acc_rre, float acc_rte, float* __restrict__ metrics,
+// One CTA per pair b = blockIdx.x: gt rows at G.start[b] (G.count[b] rows), n_node_corr / n_corr rows per pair, source points at
+// S0.start[b], transforms at 16 * b (gt) and b * t_ld (estimate), metrics at b * m_ld, device counts at b.
+__global__ void __launch_bounds__(1024) evaluate_kernel(const long long* __restrict__ gt_idx, const float* __restrict__ gt_ov,
+                                                        const __grid_constant__ Segs G, float acc_overlap,
+                                                        const long long* __restrict__ ref_corr_idx, const long long* __restrict__ src_corr_idx,
+                                                        int n_node_corr, const float* __restrict__ ref_corr_pts,
+                                                        const float* __restrict__ src_corr_pts, int n_corr, float acc_radius,
+                                                        const float* __restrict__ T_gt, const float* __restrict__ T_est, int t_ld,
+                                                        const float* __restrict__ src_points, const __grid_constant__ Segs S0, int mode,
+                                                        float acc_rmse, float acc_rre, float acc_rte, float* __restrict__ metrics, int m_ld,
                                                         const int* __restrict__ n_gt_dev, const int* __restrict__ n_node_corr_dev,
                                                         const int* __restrict__ n_corr_dev) {
+    const int b = blockIdx.x;
+    int n_gt = G.count[b];
+    gt_idx += 2ll * G.start[b]; gt_ov += G.start[b];
+    ref_corr_idx += (long long)b * n_node_corr; src_corr_idx += (long long)b * n_node_corr;
+    ref_corr_pts += 3ll * b * n_corr; src_corr_pts += 3ll * b * n_corr;
+    T_gt += 16 * b; T_est += (long long)b * t_ld;
+    src_points += 3ll * S0.start[b];
+    const int n_src = S0.count[b];
+    metrics += (long long)b * m_ld;
+    if (n_gt_dev != nullptr) n_gt_dev += b;
+    if (n_node_corr_dev != nullptr) n_node_corr_dev += b;
+    if (n_corr_dev != nullptr) n_corr_dev += b;
     // counts produced on the device by earlier stages (no host read-back between them and this kernel)
     if (n_gt_dev != nullptr) n_gt = *n_gt_dev;
     if (n_node_corr_dev != nullptr) n_node_corr = min(n_node_corr, *n_node_corr_dev);
@@ -277,6 +320,26 @@ size_t geob200_node_correspondences_workspace_bytes(int64_t n_ref, int64_t n_src
            2 * align_up(4 * n, 256) + align_up(4 * m * n, 256) + 256;
 }
 
+size_t geob200_node_correspondences_batched_workspace_bytes(int64_t n_rows, int64_t n_products, int64_t k) {
+    return geob200_node_correspondences_workspace_bytes(n_rows, 0, k) + align_up(4 * (size_t)n_products, 256);
+}
+
+static int nc_overlap_compact(const float* rn, const float* sn, const float* rp, const float* sp, const uint8_t* ref_knn_masks,
+                              const uint8_t* src_knn_masks, const uint8_t* ref_masks, const uint8_t* src_masks, const float* rmax,
+                              const float* smax, const int* rnv, const int* snv, const Segs& R, const Segs& Q, int64_t k, float pos_radius,
+                              float* overlap, int64_t* corr_indices, float* corr_overlaps, int32_t* count, cudaStream_t st) {
+    Segs NN;
+    if (segs_products(&NN, R, Q)) return -1;
+    const size_t smem = (size_t)k * (2 * sizeof(float4) + 2 * sizeof(int));
+    if (R.max > 0)
+        nc_overlap_kernel<<<dim3((unsigned)R.max, R.n), 256, smem, st>>>(rn, sn, rp, sp, ref_knn_masks, src_knn_masks, ref_masks, src_masks,
+                                                                        rmax, smax, rnv, snv, R, Q, NN, (int)k, pos_radius, overlap);
+    nc_compact_kernel<<<R.n, 1024, 0, st>>>(overlap, R, Q, NN, (long long*)corr_indices, corr_overlaps, count);
+    GEOB_CHECK_LAUNCH();
+    count_launches(2);
+    return 0;
+}
+
 // corr_indices (n_ref*n_src, 2) int64 capacity, corr_overlaps (n_ref*n_src) capacity; *count = rows written (row-major order)
 int geob200_node_correspondences(const float* ref_nodes, const float* src_nodes, const float* ref_knn_points, const float* src_knn_points,
                                  const uint8_t* ref_masks, const uint8_t* src_masks, const uint8_t* ref_knn_masks,
@@ -297,14 +360,59 @@ int geob200_node_correspondences(const float* ref_nodes, const float* src_nodes,
     int* snv = ar.take<int>(n_src);
     float* overlap = ar.take<float>((size_t)n_ref * n_src);
     GEOB_REQUIRE(ar.ok(), "node_correspondences: workspace accounting error");
-    nc_prepare_kernel<<<(unsigned)((n_ref + 7) / 8), 256, 0, st>>>(ref_nodes, ref_knn_points, ref_knn_masks, (int)n_ref, (int)k, nullptr, rn, rp, rmax, rnv);
-    nc_prepare_kernel<<<(unsigned)((n_src + 7) / 8), 256, 0, st>>>(src_nodes, src_knn_points, src_knn_masks, (int)n_src, (int)k, transform, sn, sp, smax, snv);
-    const size_t smem = (size_t)k * (2 * sizeof(float4) + 2 * sizeof(int));
-    nc_overlap_kernel<<<(unsigned)n_ref, 256, smem, st>>>(rn, sn, rp, sp, ref_knn_masks, src_knn_masks, ref_masks, src_masks, rmax, smax, rnv,
-                                                         snv, (int)n_ref, (int)n_src, (int)k, pos_radius, overlap);
-    nc_compact_kernel<<<1, 1024, 0, st>>>(overlap, (int)n_ref, (int)n_src, (long long*)corr_indices, corr_overlaps, count);
+    const Segs R = segs_one(n_ref), Q = segs_one(n_src);
+    nc_prepare_kernel<<<dim3((unsigned)((n_ref + 7) / 8), 1), 256, 0, st>>>(ref_nodes, ref_knn_points, ref_knn_masks, R, (int)k, nullptr, 0,
+                                                                          rn, rp, rmax, rnv);
+    nc_prepare_kernel<<<dim3((unsigned)((n_src + 7) / 8), 1), 256, 0, st>>>(src_nodes, src_knn_points, src_knn_masks, Q, (int)k, transform, 0,
+                                                                          sn, sp, smax, snv);
+    count_launches(2);
+    return nc_overlap_compact(rn, sn, rp, sp, ref_knn_masks, src_knn_masks, ref_masks, src_masks, rmax, smax, rnv, snv, R, Q, k, pos_radius,
+                              overlap, corr_indices, corr_overlaps, count, st);
+}
+
+int geob200_node_correspondences_batched(const float* nodes, const float* knn_points, const uint8_t* node_masks, const uint8_t* knn_masks,
+                                         int64_t n_pairs, const int64_t* cloud_nodes, int64_t k, const float* transforms, float pos_radius,
+                                         int64_t* corr_indices, float* corr_overlaps, int32_t* count, void* workspace, size_t workspace_bytes,
+                                         void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    GEOB_REQUIRE(n_pairs > 0 && 2 * n_pairs <= GEOB_MAX_CLOUDS, "node_correspondences_batched: 1..%d pairs", GEOB_MAX_CLOUDS / 2);
+    GEOB_REQUIRE(k > 0 && k <= 1024, "node_correspondences: bad shape");
+    Segs cl, NN;
+    if (segs_from_counts(&cl, 2 * n_pairs, cloud_nodes)) return -1;
+    const int B = (int)n_pairs;
+    const Segs R = segs_range(cl, 0, B), Q = segs_range(cl, B, B);
+    if (segs_products(&NN, R, Q)) return -1;
+    const int64_t rows = (int64_t)cl.start[2 * B - 1] + cl.count[2 * B - 1];
+    const int64_t nn = (int64_t)NN.start[B - 1] + NN.count[B - 1];
+    GEOB_REQUIRE(workspace_bytes >= geob200_node_correspondences_batched_workspace_bytes(rows, nn, k),
+                 "node_correspondences_batched: workspace too small");
+    Arena ar(workspace, workspace_bytes);
+    float* cn = ar.take<float>(3 * rows);
+    float* cp = ar.take<float>(3 * rows * k);
+    float* cmax = ar.take<float>(rows);
+    int* cnv = ar.take<int>(rows);
+    float* overlap = ar.take<float>(nn);
+    GEOB_REQUIRE(ar.ok(), "node_correspondences: workspace accounting error");
+    nc_prepare_kernel<<<dim3((unsigned)((cl.max + 7) / 8 > 0 ? (cl.max + 7) / 8 : 1), 2 * B), 256, 0, st>>>(
+        nodes, knn_points, knn_masks, cl, (int)k, transforms, B, cn, cp, cmax, cnv);
+    count_launches(1);
+    return nc_overlap_compact(cn, cn, cp, cp, knn_masks, knn_masks, node_masks, node_masks, cmax, cmax, cnv, cnv, R, Q, k, pos_radius,
+                              overlap, corr_indices, corr_overlaps, count, st);
+}
+
+static int evaluate_impl(const int64_t* gt_idx, const float* gt_ov, const Segs& G, const int32_t* n_gt_dev, float acceptance_overlap,
+                         const int64_t* ref_idx, const int64_t* src_idx, int64_t n_node_corr, const int32_t* n_node_corr_dev,
+                         const float* ref_pts, const float* src_pts, int64_t n_corr, const int32_t* n_corr_dev, float acceptance_radius,
+                         const float* gt_transform, const float* est_transform, int64_t transform_ld, const float* src_points,
+                         const Segs& S0, int mode, float rmse_threshold, float rre_threshold, float rte_threshold, float* metrics,
+                         int64_t metrics_ld, cudaStream_t st) {
+    GEOB_REQUIRE(mode >= 0 && mode <= 2, "evaluate: mode must be 0 (3DMatch), 1 (KITTI) or 2 (ModelNet)");
+    evaluate_kernel<<<G.n, 1024, 0, st>>>((const long long*)gt_idx, gt_ov, G, acceptance_overlap, (const long long*)ref_idx,
+                                          (const long long*)src_idx, (int)n_node_corr, ref_pts, src_pts, (int)n_corr, acceptance_radius,
+                                          gt_transform, est_transform, (int)transform_ld, src_points, S0, mode, rmse_threshold, rre_threshold,
+                                          rte_threshold, metrics, (int)metrics_ld, n_gt_dev, n_node_corr_dev, n_corr_dev);
     GEOB_CHECK_LAUNCH();
-    count_launches(4);
+    count_launches(1);
     return 0;
 }
 
@@ -325,16 +433,29 @@ int geob200_evaluate_counts(const int64_t* gt_node_corr_indices, const float* gt
                             int64_t n_corr, const int32_t* n_corr_dev, float acceptance_radius, const float* gt_transform,
                             const float* est_transform, const float* src_points, int64_t n_src_points, int mode, float rmse_threshold,
                             float rre_threshold, float rte_threshold, float* metrics, void* stream) {
-    GEOB_REQUIRE(mode >= 0 && mode <= 2, "evaluate: mode must be 0 (3DMatch), 1 (KITTI) or 2 (ModelNet)");
-    evaluate_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>((const long long*)gt_node_corr_indices, gt_node_corr_overlaps, (int)n_gt,
-                                                          acceptance_overlap, (const long long*)ref_node_corr_indices,
-                                                          (const long long*)src_node_corr_indices, (int)n_node_corr, ref_corr_points,
-                                                          src_corr_points, (int)n_corr, acceptance_radius, gt_transform, est_transform,
-                                                          src_points, (int)n_src_points, mode, rmse_threshold, rre_threshold,
-                                                          rte_threshold, metrics, n_gt_dev, n_node_corr_dev, n_corr_dev);
-    GEOB_CHECK_LAUNCH();
-    count_launches(1);
-    return 0;
+    return evaluate_impl(gt_node_corr_indices, gt_node_corr_overlaps, segs_one(n_gt), n_gt_dev, acceptance_overlap, ref_node_corr_indices,
+                         src_node_corr_indices, n_node_corr, n_node_corr_dev, ref_corr_points, src_corr_points, n_corr, n_corr_dev,
+                         acceptance_radius, gt_transform, est_transform, 16, src_points, segs_one(n_src_points), mode, rmse_threshold,
+                         rre_threshold, rte_threshold, metrics, 8, (cudaStream_t)stream);
+}
+
+int geob200_evaluate_batched(const int64_t* gt_node_corr_indices, const float* gt_node_corr_overlaps, const int32_t* n_gt_dev,
+                             float acceptance_overlap, const int64_t* ref_node_corr_indices, const int64_t* src_node_corr_indices,
+                             int64_t n_node_corr, const int32_t* n_node_corr_dev, const float* ref_corr_points, const float* src_corr_points,
+                             int64_t n_corr, const int32_t* n_corr_dev, float acceptance_radius, const float* gt_transforms,
+                             const float* est_transforms, int64_t transform_ld, const float* points, int64_t n_pairs, const int64_t* cloud_nodes,
+                             const int64_t* cloud_points, int mode, float rmse_threshold, float rre_threshold, float rte_threshold,
+                             float* metrics, int64_t metrics_ld, void* stream) {
+    GEOB_REQUIRE(n_pairs > 0 && 2 * n_pairs <= GEOB_MAX_CLOUDS, "evaluate_batched: 1..%d pairs", GEOB_MAX_CLOUDS / 2);
+    GEOB_REQUIRE(transform_ld >= 16 && metrics_ld >= 8, "evaluate_batched: transform_ld >= 16 and metrics_ld >= 8 required");
+    Segs cl, pt, G;
+    if (segs_from_counts(&cl, 2 * n_pairs, cloud_nodes) || segs_from_counts(&pt, 2 * n_pairs, cloud_points)) return -1;
+    const int B = (int)n_pairs;
+    if (segs_products(&G, segs_range(cl, 0, B), segs_range(cl, B, B))) return -1;
+    return evaluate_impl(gt_node_corr_indices, gt_node_corr_overlaps, G, n_gt_dev, acceptance_overlap, ref_node_corr_indices,
+                         src_node_corr_indices, n_node_corr, n_node_corr_dev, ref_corr_points, src_corr_points, n_corr, n_corr_dev,
+                         acceptance_radius, gt_transforms, est_transforms, transform_ld, points, segs_range(pt, B, B), mode, rmse_threshold,
+                         rre_threshold, rte_threshold, metrics, metrics_ld, (cudaStream_t)stream);
 }
 
 }  // extern "C"

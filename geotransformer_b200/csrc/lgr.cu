@@ -189,9 +189,12 @@ __global__ void __launch_bounds__(256) lgr_corr_kernel(const float* __restrict__
     }
 }
 
-// offsets over patches (single CTA), total count
+// offsets over the P patches of pair blockIdx.x (one CTA per pair), total count
 __global__ void __launch_bounds__(1024) lgr_offsets_kernel(const int* __restrict__ patch_count, int P, int* __restrict__ patch_off,
                                                            int* __restrict__ total) {
+    patch_count += (long long)blockIdx.x * P;
+    patch_off += (long long)blockIdx.x * (P + 1);
+    total += blockIdx.x;
     __shared__ int carry;
     __shared__ int warp_tot[32];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -218,14 +221,18 @@ __global__ void __launch_bounds__(1024) lgr_offsets_kernel(const int* __restrict
     if (threadIdx.x == 0) { patch_off[P] = carry; *total = carry; }
 }
 
-// stacked correspondences in (patch, i, j) order (local_global_registration.py:139-142)
+// stacked correspondences in (patch, i, j) order (local_global_registration.py:139-142).  Patch blockIdx.x of pair blockIdx.y
+// (gridDim.x patches per pair); the pair's rows start at blockIdx.y * gridDim.x * cap.
 __global__ void __launch_bounds__(256) lgr_stack_kernel(const int* __restrict__ patch_count, const int* __restrict__ patch_off,
                                                         const int* __restrict__ patch_ij, const float* __restrict__ patch_score, int K,
                                                         int cap, const float* __restrict__ ref_knn_pts, const float* __restrict__ src_knn_pts,
                                                         float* __restrict__ ref_corr, float* __restrict__ src_corr,
                                                         float* __restrict__ corr_scores, int* __restrict__ corr_patch) {
-    const int p = blockIdx.x;
-    const int c = patch_count[p], off = patch_off[p];
+    const int P = gridDim.x, b = blockIdx.y;
+    const long long first = (long long)b * P * cap;
+    ref_corr += 3 * first; src_corr += 3 * first; corr_scores += first; corr_patch += first;
+    const int c = patch_count[b * P + blockIdx.x], off = patch_off[b * (P + 1) + blockIdx.x];
+    const long long p = (long long)b * P + blockIdx.x;
     for (int e = threadIdx.x; e < c; e += blockDim.x) {
         const int ij = patch_ij[(long long)p * cap + e];
         const int i = ij / K, j = ij % K;
@@ -235,19 +242,23 @@ __global__ void __launch_bounds__(256) lgr_stack_kernel(const int* __restrict__ 
         ref_corr[3 * o] = r[0]; ref_corr[3 * o + 1] = r[1]; ref_corr[3 * o + 2] = r[2];
         src_corr[3 * o] = s[0]; src_corr[3 * o + 1] = s[1]; src_corr[3 * o + 2] = s[2];
         corr_scores[o] = patch_score[(long long)p * cap + e];
-        corr_patch[o] = p;
+        corr_patch[o] = blockIdx.x;
     }
 }
 
-// per-patch weighted Kabsch (one warp per patch); patches with < min_corr correspondences are marked invalid
+// per-patch weighted Kabsch (one warp per patch); patches with < min_corr correspondences are marked invalid.  Pair blockIdx.y:
+// its rows start at blockIdx.y * pair_cap.
 __global__ void __launch_bounds__(256) lgr_patch_procrustes_kernel(const int* __restrict__ patch_count, const int* __restrict__ patch_off,
-                                                                   int P, int min_corr, const float* __restrict__ ref_corr,
+                                                                   int P, int min_corr, long long pair_cap, const float* __restrict__ ref_corr,
                                                                    const float* __restrict__ src_corr, const float* __restrict__ corr_scores,
                                                                    float eps, float* __restrict__ T /*[P][16]*/, int* __restrict__ valid) {
     const int lane = threadIdx.x & 31;
-    const int p = blockIdx.x * 8 + (threadIdx.x >> 5);
-    if (p >= P) return;
-    const int c = patch_count[p], off = patch_off[p];
+    const int b = blockIdx.y;
+    const int pl = blockIdx.x * 8 + (threadIdx.x >> 5);
+    if (pl >= P) return;
+    const int p = b * P + pl;
+    ref_corr += 3 * b * pair_cap; src_corr += 3 * b * pair_cap; corr_scores += b * pair_cap;
+    const int c = patch_count[p], off = patch_off[b * (P + 1) + pl];
     if (c < min_corr) { if (lane == 0) valid[p] = 0; return; }
     double sw = 0.0;
     for (int e = lane; e < c; e += 32) sw += (double)fmaxf(corr_scores[off + e], 0.f);
@@ -270,11 +281,14 @@ __global__ void __launch_bounds__(256) lgr_patch_procrustes_kernel(const int* __
     if (lane == 0) { finish_procrustes(W, S1, S2, Sxy, T + 16ll * p); valid[p] = 1; }
 }
 
-// inlier count of every valid hypothesis over ALL correspondences (local_global_registration.py:172-177)
+// inlier count of every valid hypothesis over ALL correspondences of its pair (local_global_registration.py:172-177)
 __global__ void __launch_bounds__(256) lgr_verify_kernel(const float* __restrict__ T, const int* __restrict__ valid,
-                                                         const int* __restrict__ total, const float* __restrict__ ref_corr,
+                                                         const int* __restrict__ total, long long pair_cap, const float* __restrict__ ref_corr,
                                                          const float* __restrict__ src_corr, float radius, int* __restrict__ inliers) {
-    const int p = blockIdx.x;
+    const int b = blockIdx.y;
+    const int p = b * gridDim.x + blockIdx.x;
+    total += b;
+    ref_corr += 3 * b * pair_cap; src_corr += 3 * b * pair_cap;
     if (!valid[p]) { if (threadIdx.x == 0) inliers[p] = -1; return; }
     __shared__ float t[16];
     __shared__ int cnt;
@@ -349,11 +363,19 @@ __device__ void block_procrustes(const float* __restrict__ ref_corr, const float
     __syncthreads();
 }
 
+// one CTA per pair blockIdx.x; its transform goes to Tout + blockIdx.x * t_ld
 __global__ void __launch_bounds__(1024) lgr_refine_kernel(const float* __restrict__ Tpatch, const int* __restrict__ inliers, int P,
-                                                          const int* __restrict__ total, const float* __restrict__ ref_corr,
+                                                          const int* __restrict__ total, long long pair_cap, const float* __restrict__ ref_corr,
                                                           const float* __restrict__ src_corr, const float* __restrict__ corr_scores,
-                                                          float radius, float eps, int num_steps, float* __restrict__ Tout,
+                                                          float radius, float eps, int num_steps, float* __restrict__ Tout, int t_ld,
                                                           int* __restrict__ best_out) {
+    {
+        const int b = blockIdx.x;
+        Tpatch += 16ll * b * P; inliers += (long long)b * P; total += b;
+        ref_corr += 3 * b * pair_cap; src_corr += 3 * b * pair_cap; corr_scores += b * pair_cap;
+        Tout += (long long)b * t_ld;
+        if (best_out != nullptr) best_out += b;
+    }
     __shared__ double red[32 * 16];
     __shared__ float Ta[16], Tb[16];
     __shared__ int best_s;
@@ -427,6 +449,55 @@ size_t geob200_lgr_workspace_bytes(int64_t n_patches, int64_t k, int64_t topk) {
     return align_up(4 * (P + 1), 256) * 4 + align_up(4 * P * cap, 256) * 2 + align_up(64 * P, 256) + 4096;
 }
 
+size_t geob200_lgr_batched_workspace_bytes(int64_t n_pairs, int64_t n_patches, int64_t k, int64_t topk) {
+    return geob200_lgr_workspace_bytes(n_pairs * (n_patches + 1), k, topk);
+}
+
+// B pairs of P patches each, patches of pair b at b * P; outputs of pair b at b * (its capacity), transform at b * transform_ld
+static int lgr_impl(const float* ref_knn_points, const float* src_knn_points, const uint8_t* ref_knn_masks, const uint8_t* src_knn_masks,
+                    const float* log_scores, int B, int P, int64_t k, int64_t score_ld, int64_t topk, float acceptance_radius, int mutual,
+                    float confidence_threshold, int64_t correspondence_threshold, int64_t num_refinement_steps, float* ref_corr_points,
+                    float* src_corr_points, float* corr_scores, int32_t* corr_patch, int32_t* num_corr, float* estimated_transform,
+                    int64_t transform_ld, float* patch_transforms, int32_t* patch_inliers, int32_t* best_patch, void* workspace,
+                    size_t workspace_bytes, cudaStream_t st) {
+    GEOB_REQUIRE(P > 0 && k > 0 && k <= 256, "lgr: bad patch shape");
+    GEOB_REQUIRE(topk >= 1 && topk <= 4, "lgr: topk must be in 1..4");
+    GEOB_REQUIRE(score_ld == k || score_ld == k + 1, "lgr: score matrix must be (P,K,K) or (P,K+1,K+1)");
+    GEOB_REQUIRE(transform_ld >= 16, "lgr: transform_ld must be >= 16");
+    Arena ar(workspace, workspace_bytes);
+    const int PT = B * P, K = (int)k;
+    const int cap = K * (int)(mutual ? topk : 2 * topk);
+    const long long pair_cap = (long long)P * cap;
+    int* patch_count = ar.take<int>(PT + 1);
+    int* patch_off = ar.take<int>((size_t)B * (P + 1));
+    int* valid = ar.take<int>(PT + 1);
+    int* inl_tmp = ar.take<int>(PT + 1);
+    int* patch_ij = ar.take<int>((size_t)PT * cap);
+    float* patch_score = ar.take<float>((size_t)PT * cap);
+    float* T_tmp = ar.take<float>(16 * (size_t)PT);
+    GEOB_REQUIRE(ar.ok(), "lgr: workspace too small");
+    float* Tp = patch_transforms != nullptr ? patch_transforms : T_tmp;
+    int* inl = patch_inliers != nullptr ? patch_inliers : inl_tmp;
+
+    const size_t smem = sizeof(float) * K * (K + 1) + 2 * (size_t)K * K;
+    if (smem > 48 * 1024 && ensure_max_smem((const void*)lgr_corr_kernel<4>)) return -1;
+    lgr_corr_kernel<4><<<PT, 256, smem, st>>>(log_scores, K, (int)score_ld, ref_knn_masks, src_knn_masks, (int)topk,
+                                              confidence_threshold, mutual, patch_count, patch_ij, patch_score);
+    lgr_offsets_kernel<<<B, 1024, 0, st>>>(patch_count, P, patch_off, num_corr);
+    lgr_stack_kernel<<<dim3(P, B), 256, 0, st>>>(patch_count, patch_off, patch_ij, patch_score, K, cap, ref_knn_points, src_knn_points,
+                                                 ref_corr_points, src_corr_points, corr_scores, corr_patch);
+    lgr_patch_procrustes_kernel<<<dim3((P + 7) / 8, B), 256, 0, st>>>(patch_count, patch_off, P, (int)correspondence_threshold, pair_cap,
+                                                                     ref_corr_points, src_corr_points, corr_scores, 1e-5f, Tp, valid);
+    lgr_verify_kernel<<<dim3(P, B), 256, 0, st>>>(Tp, valid, num_corr, pair_cap, ref_corr_points, src_corr_points, acceptance_radius, inl);
+    // reference: 1 procrustes with the best hypothesis' inliers + (num_refinement_steps - 1) refinements
+    lgr_refine_kernel<<<B, 1024, 0, st>>>(Tp, inl, P, num_corr, pair_cap, ref_corr_points, src_corr_points, corr_scores,
+                                          acceptance_radius, 1e-5f, (int)num_refinement_steps, estimated_transform, (int)transform_ld,
+                                          best_patch);
+    GEOB_CHECK_LAUNCH();
+    count_launches(6);
+    return 0;
+}
+
 // Outputs have capacity n_patches*k*topk rows; *num_corr (device int32) receives the number actually written.
 int geob200_local_global_registration(const float* ref_knn_points, const float* src_knn_points, const uint8_t* ref_knn_masks,
                                       const uint8_t* src_knn_masks, const float* log_scores, int64_t n_patches, int64_t k,
@@ -435,41 +506,27 @@ int geob200_local_global_registration(const float* ref_knn_points, const float* 
                                       float* ref_corr_points, float* src_corr_points, float* corr_scores, int32_t* corr_patch,
                                       int32_t* num_corr, float* estimated_transform, float* patch_transforms, int32_t* patch_inliers,
                                       int32_t* best_patch, void* workspace, size_t workspace_bytes, void* stream) {
-    cudaStream_t st = (cudaStream_t)stream;
-    GEOB_REQUIRE(n_patches > 0 && k > 0 && k <= 256, "lgr: bad patch shape");
-    GEOB_REQUIRE(topk >= 1 && topk <= 4, "lgr: topk must be in 1..4");
-    GEOB_REQUIRE(score_ld == k || score_ld == k + 1, "lgr: score matrix must be (P,K,K) or (P,K+1,K+1)");
     GEOB_REQUIRE(workspace_bytes >= geob200_lgr_workspace_bytes(n_patches, k, topk), "lgr: workspace too small");
-    Arena ar(workspace, workspace_bytes);
-    const int P = (int)n_patches, K = (int)k;
-    const int cap = K * (int)(mutual ? topk : 2 * topk);
-    int* patch_count = ar.take<int>(P + 1);
-    int* patch_off = ar.take<int>(P + 1);
-    int* valid = ar.take<int>(P + 1);
-    int* inl_tmp = ar.take<int>(P + 1);
-    int* patch_ij = ar.take<int>((size_t)P * cap);
-    float* patch_score = ar.take<float>((size_t)P * cap);
-    float* T_tmp = ar.take<float>(16 * (size_t)P);
-    GEOB_REQUIRE(ar.ok(), "lgr: workspace accounting error");
-    float* Tp = patch_transforms != nullptr ? patch_transforms : T_tmp;
-    int* inl = patch_inliers != nullptr ? patch_inliers : inl_tmp;
+    return lgr_impl(ref_knn_points, src_knn_points, ref_knn_masks, src_knn_masks, log_scores, 1, (int)n_patches, k, score_ld, topk,
+                    acceptance_radius, mutual, confidence_threshold, correspondence_threshold, num_refinement_steps, ref_corr_points,
+                    src_corr_points, corr_scores, corr_patch, num_corr, estimated_transform, 16, patch_transforms, patch_inliers, best_patch,
+                    workspace, workspace_bytes, (cudaStream_t)stream);
+}
 
-    const size_t smem = sizeof(float) * K * (K + 1) + 2 * (size_t)K * K;
-    if (smem > 48 * 1024 && ensure_max_smem((const void*)lgr_corr_kernel<4>)) return -1;
-    lgr_corr_kernel<4><<<P, 256, smem, st>>>(log_scores, K, (int)score_ld, ref_knn_masks, src_knn_masks, (int)topk,
-                                             confidence_threshold, mutual, patch_count, patch_ij, patch_score);
-    lgr_offsets_kernel<<<1, 1024, 0, st>>>(patch_count, P, patch_off, num_corr);
-    lgr_stack_kernel<<<P, 256, 0, st>>>(patch_count, patch_off, patch_ij, patch_score, K, cap, ref_knn_points, src_knn_points,
-                                        ref_corr_points, src_corr_points, corr_scores, corr_patch);
-    lgr_patch_procrustes_kernel<<<(P + 7) / 8, 256, 0, st>>>(patch_count, patch_off, P, (int)correspondence_threshold,
-                                                            ref_corr_points, src_corr_points, corr_scores, 1e-5f, Tp, valid);
-    lgr_verify_kernel<<<P, 256, 0, st>>>(Tp, valid, num_corr, ref_corr_points, src_corr_points, acceptance_radius, inl);
-    // reference: 1 procrustes with the best hypothesis' inliers + (num_refinement_steps - 1) refinements
-    lgr_refine_kernel<<<1, 1024, 0, st>>>(Tp, inl, P, num_corr, ref_corr_points, src_corr_points, corr_scores,
-                                          acceptance_radius, 1e-5f, (int)num_refinement_steps, estimated_transform, best_patch);
-    GEOB_CHECK_LAUNCH();
-    count_launches(6);
-    return 0;
+int geob200_local_global_registration_batched(const float* ref_knn_points, const float* src_knn_points, const uint8_t* ref_knn_masks,
+                                              const uint8_t* src_knn_masks, const float* log_scores, int64_t n_pairs, int64_t n_patches,
+                                              int64_t k, int64_t score_ld, int64_t topk, float acceptance_radius, int mutual,
+                                              float confidence_threshold, int64_t correspondence_threshold, int64_t num_refinement_steps,
+                                              float* ref_corr_points, float* src_corr_points, float* corr_scores, int32_t* corr_patch,
+                                              int32_t* num_corr, float* estimated_transform, int64_t transform_ld, float* patch_transforms,
+                                              int32_t* patch_inliers, int32_t* best_patch, void* workspace, size_t workspace_bytes,
+                                              void* stream) {
+    GEOB_REQUIRE(n_pairs > 0 && n_pairs <= GEOB_MAX_CLOUDS / 2, "lgr_batched: 1..%d pairs", GEOB_MAX_CLOUDS / 2);
+    GEOB_REQUIRE(workspace_bytes >= geob200_lgr_batched_workspace_bytes(n_pairs, n_patches, k, topk), "lgr_batched: workspace too small");
+    return lgr_impl(ref_knn_points, src_knn_points, ref_knn_masks, src_knn_masks, log_scores, (int)n_pairs, (int)n_patches, k, score_ld,
+                    topk, acceptance_radius, mutual, confidence_threshold, correspondence_threshold, num_refinement_steps, ref_corr_points,
+                    src_corr_points, corr_scores, corr_patch, num_corr, estimated_transform, transform_ld, patch_transforms, patch_inliers,
+                    best_patch, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 int geob200_weighted_procrustes(const float* src_points, const float* ref_points, const float* weights, int64_t batch,

@@ -11,11 +11,57 @@
 
 namespace geob200 {
 
+int segs_from_counts(Segs* s, int64_t n, const int64_t* counts) {
+    if (n < 1 || n > GEOB_MAX_CLOUDS) { set_error("batch: 1..%d segments supported (got %lld)", GEOB_MAX_CLOUDS, (long long)n); return -1; }
+    *s = Segs{};
+    s->n = (int)n;
+    int64_t o = 0;
+    for (int i = 0; i < n; ++i) {
+        if (counts[i] < 0) { set_error("batch: negative segment size"); return -1; }
+        s->start[i] = (int)o;
+        s->count[i] = (int)counts[i];
+        s->max = s->max > (int)counts[i] ? s->max : (int)counts[i];
+        o += counts[i];
+    }
+    if (o >= (1ll << 31)) { set_error("batch: too many rows (%lld)", (long long)o); return -1; }
+    return 0;
+}
+
+Segs segs_one(int64_t count) {
+    Segs s{};
+    s.n = 1;
+    s.max = (int)count;
+    s.count[0] = (int)count;
+    return s;
+}
+
+Segs segs_range(const Segs& s, int first, int n) {
+    Segs r{};
+    r.n = n;
+    for (int i = 0; i < n; ++i) {
+        r.start[i] = s.start[first + i];
+        r.count[i] = s.count[first + i];
+        r.max = r.max > r.count[i] ? r.max : r.count[i];
+    }
+    return r;
+}
+
+int segs_products(Segs* s, const Segs& ref, const Segs& src) {
+    int64_t c[GEOB_MAX_CLOUDS];
+    for (int i = 0; i < ref.n; ++i) c[i] = (int64_t)ref.count[i] * src.count[i];
+    return segs_from_counts(s, ref.n, c);
+}
+
 // ---- superpoint matching ---------------------------------------------------------------------------------
 
-// valid (non-empty) node lists, in index order (torch.nonzero): single CTA, chunked ordered compaction
-__global__ void __launch_bounds__(1024) compact_masks_kernel(const unsigned char* __restrict__ masks, int n, int* __restrict__ idx,
-                                                             int* __restrict__ count) {
+// valid (non-empty) node lists, in index order (torch.nonzero): one CTA per cloud, chunked ordered compaction
+__global__ void __launch_bounds__(1024) compact_masks_kernel(const unsigned char* __restrict__ masks, const __grid_constant__ Segs cl,
+                                                             int* __restrict__ idx, int* __restrict__ count) {
+    const int s = blockIdx.y;
+    masks += cl.start[s];
+    idx += cl.start[s];
+    count += s;
+    const int n = cl.count[s];
     __shared__ int warp_tot[32];
     __shared__ int carry;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -43,11 +89,18 @@ __global__ void __launch_bounds__(1024) compact_masks_kernel(const unsigned char
 }
 
 // S[i][j] = exp(-clamp(2 - 2 <fr_i, fs_j>, 0)) over the valid nodes; row sums.  One CTA per (compacted) row.
+// Pair p = blockIdx.y: ref rows at R.start[p] of fr / ridx / rowsum, src rows at Q.start[p] of fs / sidx, S at NN.start[p].
 __global__ void __launch_bounds__(256) spm_scores_kernel(const float* __restrict__ fr, const float* __restrict__ fs, int C,
                                                          const int* __restrict__ ridx, const int* __restrict__ rcount,
                                                          const int* __restrict__ sidx, const int* __restrict__ scount,
-                                                         int ld, float* __restrict__ S, float* __restrict__ rowsum) {
+                                                         const __grid_constant__ Segs R, const __grid_constant__ Segs Q,
+                                                         const __grid_constant__ Segs NN, float* __restrict__ S, float* __restrict__ rowsum) {
     extern __shared__ float sm[];
+    const int p = blockIdx.y;
+    const int ld = Q.count[p];
+    fr += (long long)R.start[p] * C; ridx += R.start[p]; rcount += p; rowsum += R.start[p];
+    fs += (long long)Q.start[p] * C; sidx += Q.start[p]; scount += p;
+    S += NN.start[p];
     float* a = sm;            // [C]
     float* srow = sm + C;     // [ld]
     const int i = blockIdx.x;
@@ -76,8 +129,12 @@ __global__ void __launch_bounds__(256) spm_scores_kernel(const float* __restrict
     }
 }
 
-__global__ void __launch_bounds__(256) spm_colsum_kernel(const float* __restrict__ S, int ld, const int* __restrict__ rcount,
-                                                         const int* __restrict__ scount, float* __restrict__ colsum) {
+__global__ void __launch_bounds__(256) spm_colsum_kernel(const float* __restrict__ S, const int* __restrict__ rcount,
+                                                         const int* __restrict__ scount, const __grid_constant__ Segs Q,
+                                                         const __grid_constant__ Segs NN, float* __restrict__ colsum) {
+    const int p = blockIdx.y;
+    const int ld = Q.count[p];
+    S += NN.start[p]; rcount += p; scount += p; colsum += Q.start[p];
     const int j = blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= *scount) return;
     const int nr = *rcount;
@@ -87,9 +144,14 @@ __global__ void __launch_bounds__(256) spm_colsum_kernel(const float* __restrict
 }
 
 // dual normalisation into a dense flat (nr*ns) array
-__global__ void __launch_bounds__(256) spm_dual_kernel(const float* __restrict__ S, int ld, const int* __restrict__ rcount,
+__global__ void __launch_bounds__(256) spm_dual_kernel(const float* __restrict__ S, const int* __restrict__ rcount,
                                                        const int* __restrict__ scount, const float* __restrict__ rowsum,
-                                                       const float* __restrict__ colsum, int dual, float* __restrict__ flat) {
+                                                       const float* __restrict__ colsum, const __grid_constant__ Segs R,
+                                                       const __grid_constant__ Segs Q, const __grid_constant__ Segs NN, int dual,
+                                                       float* __restrict__ flat) {
+    const int p = blockIdx.y;
+    const int ld = Q.count[p];
+    S += NN.start[p]; flat += NN.start[p]; rcount += p; scount += p; rowsum += R.start[p]; colsum += Q.start[p];
     const int nr = *rcount, ns = *scount;
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= (long long)nr * ns) return;
@@ -100,12 +162,19 @@ __global__ void __launch_bounds__(256) spm_dual_kernel(const float* __restrict__
 
 // top-k (largest) of a flat positive array: MSB-first 8-bit radix select of the k-th value, then an ordered
 // sweep that keeps everything above the threshold and the lowest-index ties, then a bitonic sort of the k winners.
+// One CTA per pair p = blockIdx.y; its k_req output rows start at p * k_req.
 template <int KMAX>
 __global__ void __launch_bounds__(1024) topk_flat_kernel(const float* __restrict__ flat, const int* __restrict__ rcount,
                                                          const int* __restrict__ scount, int k_req, const int* __restrict__ ridx,
-                                                         const int* __restrict__ sidx, long long* __restrict__ ref_out,
-                                                         long long* __restrict__ src_out, float* __restrict__ score_out,
-                                                         int* __restrict__ k_out) {
+                                                         const int* __restrict__ sidx, const __grid_constant__ Segs R,
+                                                         const __grid_constant__ Segs Q, const __grid_constant__ Segs NN,
+                                                         long long* __restrict__ ref_out, long long* __restrict__ src_out,
+                                                         float* __restrict__ score_out, int* __restrict__ k_out) {
+    {
+        const int p = blockIdx.y;
+        flat += NN.start[p]; rcount += p; scount += p; ridx += R.start[p]; sidx += Q.start[p];
+        ref_out += (long long)p * k_req; src_out += (long long)p * k_req; score_out += (long long)p * k_req; k_out += p;
+    }
     __shared__ unsigned hist[256];
     __shared__ unsigned long long keys[KMAX];
     __shared__ unsigned prefix_s, kth_s;
@@ -198,16 +267,26 @@ __global__ void __launch_bounds__(1024) topk_flat_kernel(const float* __restrict
 }
 
 // ---- patch gathers ---------------------------------------------------------------------------------------
-// out_idx[p][i] = knn[corr[p]][i]; out_mask likewise; out_pts = padded_points[idx]
-__global__ void __launch_bounds__(256) gather_patches_kernel(const long long* __restrict__ corr, int P, const long long* __restrict__ knn,
+// out_idx[p][i] = knn[corr[p]][i]; out_mask likewise; out_pts = padded_points[idx].  Cloud s = blockIdx.y: its node rows
+// (knn table) at Nd.start[s], its points at Pt.start[s]; P patches per cloud at s * P, or with corr == nullptr every node of the
+// cloud is a patch (corr = arange), at Nd.start[s].
+__global__ void __launch_bounds__(256) gather_patches_kernel(const long long* __restrict__ corr, int P_all, const long long* __restrict__ knn,
                                                              const unsigned char* __restrict__ knn_masks, int K,
-                                                             const float* __restrict__ pts, int n_pts,
-                                                             long long* __restrict__ out_idx, unsigned char* __restrict__ out_mask,
-                                                             float* __restrict__ out_pts) {
+                                                             const float* __restrict__ pts, const __grid_constant__ Segs Nd,
+                                                             const __grid_constant__ Segs Pt, long long* __restrict__ out_idx,
+                                                             unsigned char* __restrict__ out_mask, float* __restrict__ out_pts) {
+    const int s = blockIdx.y;
+    const int P = corr != nullptr ? P_all : Nd.count[s];
+    const long long first = corr != nullptr ? (long long)s * P_all : Nd.start[s];
+    if (corr != nullptr) corr += first;
+    knn += (long long)Nd.start[s] * K; knn_masks += (long long)Nd.start[s] * K;
+    pts += 3ll * Pt.start[s];
+    const int n_pts = Pt.count[s];
+    out_idx += first * K; out_mask += first * K; out_pts += 3 * first * K;
     const int t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= P * K) return;
     const int p = t / K, i = t % K;
-    const long long node = corr[p];
+    const long long node = corr != nullptr ? corr[p] : p;
     const long long idx = node >= 0 ? knn[node * K + i] : (long long)n_pts;
     out_idx[t] = idx;
     out_mask[t] = node >= 0 ? knn_masks[node * K + i] : 0;
@@ -219,13 +298,18 @@ __global__ void __launch_bounds__(256) gather_patches_kernel(const long long* __
 
 // scores[p][i][j] = <fr[ridx[p][i]], fs[sidx[p][j]]> / sqrt(C); rows of the sentinel index are zero.
 // One CTA per patch; T = K/16 outputs per thread per dimension.
+// Pair b = blockIdx.y: ref fine rows at R.start[b] of fr, src at Q.start[b] of fs; patches b * gridDim.x + blockIdx.x.
 template <int T>
-__global__ void __launch_bounds__(256) patch_scores_kernel(const float* __restrict__ fr, int nr, const float* __restrict__ fs, int ns,
+__global__ void __launch_bounds__(256) patch_scores_kernel(const float* __restrict__ fr, const float* __restrict__ fs,
+                                                           const __grid_constant__ Segs R, const __grid_constant__ Segs Q,
                                                            int C, const long long* __restrict__ ridx, const long long* __restrict__ sidx,
                                                            float inv_div, float* __restrict__ out) {
     constexpr int K = 16 * T, CH = 32;
     __shared__ float A[K][CH + 1], B[K][CH + 1];
-    const int p = blockIdx.x;
+    const int b = blockIdx.y;
+    fr += (long long)R.start[b] * C; fs += (long long)Q.start[b] * C;
+    const int nr = R.count[b], ns = Q.count[b];
+    const int p = b * gridDim.x + blockIdx.x;
     const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
     float acc[T][T];
 #pragma unroll
@@ -466,6 +550,34 @@ size_t geob200_superpoint_matching_workspace_bytes(int64_t n_ref, int64_t n_src)
     return align_up(4 * nr, 256) * 2 + align_up(4 * ns, 256) * 2 + align_up(4 * nr * ns, 256) * 2 + 1024 + 4096;
 }
 
+size_t geob200_superpoint_matching_batched_workspace_bytes(int64_t n_rows, int64_t n_products, int64_t n_pairs) {
+    const size_t r = (size_t)n_rows, nn = (size_t)n_products;
+    return align_up(4 * r, 256) * 3 + align_up(4 * nn, 256) * 2 + align_up(8 * (size_t)n_pairs, 256) + 4096;
+}
+
+// R / Q: the pairs' ref / src clouds in the row space of ref_feats / src_feats; ref rows of ridx / rowsum at R.start, src rows of
+// sidx / colsum at Q.start; counts[p] / counts[B + p] = valid ref / src nodes of pair p
+static int superpoint_matching_impl(const float* ref_feats, const float* src_feats, int64_t channels, const Segs& R, const Segs& Q,
+                                    const int* ridx, const int* sidx, const int* counts, float* rowsum, float* colsum, float* S, float* flat,
+                                    int64_t num_correspondences, int dual, int64_t* ref_corr_indices, int64_t* src_corr_indices,
+                                    float* corr_scores, int32_t* num_out, cudaStream_t st) {
+    const int B = R.n;
+    Segs NN;
+    if (segs_products(&NN, R, Q)) return -1;
+    const size_t smem = sizeof(float) * (channels + Q.max);
+    GEOB_REQUIRE(smem <= 48 * 1024, "superpoint_matching: row does not fit shared memory");
+    const dim3 g_rows((unsigned)(R.max > 0 ? R.max : 1), B), g_cols((unsigned)((Q.max + 255) / 256 > 0 ? (Q.max + 255) / 256 : 1), B),
+        g_nn((unsigned)((NN.max + 255) / 256 > 0 ? (NN.max + 255) / 256 : 1), B);
+    spm_scores_kernel<<<g_rows, 256, smem, st>>>(ref_feats, src_feats, (int)channels, ridx, counts, sidx, counts + B, R, Q, NN, S, rowsum);
+    spm_colsum_kernel<<<g_cols, 256, 0, st>>>(S, counts, counts + B, Q, NN, colsum);
+    spm_dual_kernel<<<g_nn, 256, 0, st>>>(S, counts, counts + B, rowsum, colsum, R, Q, NN, dual, flat);
+    topk_flat_kernel<1024><<<dim3(1, B), 1024, 0, st>>>(flat, counts, counts + B, (int)num_correspondences, ridx, sidx, R, Q, NN,
+                                                        (long long*)ref_corr_indices, (long long*)src_corr_indices, corr_scores, num_out);
+    GEOB_CHECK_LAUNCH();
+    count_launches(4);
+    return 0;
+}
+
 int geob200_superpoint_matching(const float* ref_feats, const float* src_feats, int64_t n_ref, int64_t n_src, int64_t channels,
                                 const uint8_t* ref_masks, const uint8_t* src_masks, int64_t num_correspondences, int dual,
                                 int64_t* ref_corr_indices, int64_t* src_corr_indices, float* corr_scores, int32_t* num_out,
@@ -483,28 +595,84 @@ int geob200_superpoint_matching(const float* ref_feats, const float* src_feats, 
     float* S = ar.take<float>((size_t)n_ref * n_src);
     float* flat = ar.take<float>((size_t)n_ref * n_src);
     int* counts = ar.take<int>(64);
-    compact_masks_kernel<<<1, 1024, 0, st>>>(ref_masks, (int)n_ref, ridx, counts);
-    compact_masks_kernel<<<1, 1024, 0, st>>>(src_masks, (int)n_src, sidx, counts + 1);
-    const size_t smem = sizeof(float) * (channels + n_src);
-    GEOB_REQUIRE(smem <= 48 * 1024, "superpoint_matching: row does not fit shared memory");
-    spm_scores_kernel<<<(unsigned)n_ref, 256, smem, st>>>(ref_feats, src_feats, (int)channels, ridx, counts, sidx, counts + 1,
-                                                         (int)n_src, S, rowsum);
-    spm_colsum_kernel<<<(unsigned)((n_src + 255) / 256), 256, 0, st>>>(S, (int)n_src, counts, counts + 1, colsum);
-    spm_dual_kernel<<<(unsigned)((n_ref * n_src + 255) / 256), 256, 0, st>>>(S, (int)n_src, counts, counts + 1, rowsum, colsum, dual, flat);
-    topk_flat_kernel<1024><<<1, 1024, 0, st>>>(flat, counts, counts + 1, (int)num_correspondences, ridx, sidx,
-                                               (long long*)ref_corr_indices, (long long*)src_corr_indices, corr_scores, num_out);
-    GEOB_CHECK_LAUNCH();
-    count_launches(6);
-    return 0;
+    const Segs R = segs_one(n_ref), Q = segs_one(n_src);
+    compact_masks_kernel<<<dim3(1, 1), 1024, 0, st>>>(ref_masks, R, ridx, counts);
+    compact_masks_kernel<<<dim3(1, 1), 1024, 0, st>>>(src_masks, Q, sidx, counts + 1);
+    count_launches(2);
+    return superpoint_matching_impl(ref_feats, src_feats, channels, R, Q, ridx, sidx, counts, rowsum, colsum, S, flat, num_correspondences,
+                                    dual, ref_corr_indices, src_corr_indices, corr_scores, num_out, st);
+}
+
+int geob200_superpoint_matching_batched(const float* feats, int64_t channels, const uint8_t* masks, int64_t n_pairs,
+                                        const int64_t* cloud_nodes, int64_t num_correspondences, int dual, int64_t* corr_indices,
+                                        float* corr_scores, int32_t* num_out, void* workspace, size_t workspace_bytes, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    GEOB_REQUIRE(n_pairs > 0 && 2 * n_pairs <= GEOB_MAX_CLOUDS, "superpoint_matching_batched: 1..%d pairs", GEOB_MAX_CLOUDS / 2);
+    GEOB_REQUIRE(num_correspondences > 0 && num_correspondences <= 1024, "superpoint_matching: num_correspondences must be in 1..1024");
+    Segs cl, NN;
+    if (segs_from_counts(&cl, 2 * n_pairs, cloud_nodes)) return -1;
+    const int B = (int)n_pairs;
+    const Segs R = segs_range(cl, 0, B), Q = segs_range(cl, B, B);
+    if (segs_products(&NN, R, Q)) return -1;
+    const int64_t rows = (int64_t)cl.start[2 * B - 1] + cl.count[2 * B - 1];
+    const int64_t nn = (int64_t)NN.start[B - 1] + NN.count[B - 1];
+    GEOB_REQUIRE(workspace_bytes >= geob200_superpoint_matching_batched_workspace_bytes(rows, nn, n_pairs),
+                 "superpoint_matching_batched: workspace too small");
+    Arena ar(workspace, workspace_bytes);
+    int* idx = ar.take<int>(rows);
+    float* rowsum = ar.take<float>(rows);
+    float* colsum = ar.take<float>(rows);
+    float* S = ar.take<float>(nn);
+    float* flat = ar.take<float>(nn);
+    int* counts = ar.take<int>(2 * B);
+    compact_masks_kernel<<<dim3(1, 2 * B), 1024, 0, st>>>(masks, cl, idx, counts);
+    count_launches(1);
+    const int64_t k = num_correspondences;
+    return superpoint_matching_impl(feats, feats, channels, R, Q, idx, idx, counts, rowsum, colsum, S, flat, k, dual, corr_indices,
+                                    corr_indices + B * k, corr_scores, num_out, st);
 }
 
 int geob200_gather_patches(const int64_t* corr_indices, int64_t n_corr, const int64_t* node_knn_indices,
                            const uint8_t* node_knn_masks, int64_t k, const float* points, int64_t n_points,
                            int64_t* out_indices, uint8_t* out_masks, float* out_points, void* stream) {
     if (n_corr == 0) return 0;
-    gather_patches_kernel<<<(unsigned)((n_corr * k + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
-        (const long long*)corr_indices, (int)n_corr, (const long long*)node_knn_indices, node_knn_masks, (int)k, points,
-        (int)n_points, (long long*)out_indices, out_masks, out_points);
+    gather_patches_kernel<<<dim3((unsigned)((n_corr * k + 255) / 256), 1), 256, 0, (cudaStream_t)stream>>>(
+        (const long long*)corr_indices, (int)n_corr, (const long long*)node_knn_indices, node_knn_masks, (int)k, points, segs_one(0),
+        segs_one(n_points), (long long*)out_indices, out_masks, out_points);
+    GEOB_CHECK_LAUNCH();
+    count_launches(1);
+    return 0;
+}
+
+int geob200_gather_patches_batched(const int64_t* corr_indices, int64_t n_corr, int64_t n_clouds, const int64_t* cloud_nodes,
+                                   const int64_t* cloud_points, const int64_t* node_knn_indices, const uint8_t* node_knn_masks, int64_t k,
+                                   const float* points, int64_t* out_indices, uint8_t* out_masks, float* out_points, void* stream) {
+    Segs nd, pt;
+    if (segs_from_counts(&nd, n_clouds, cloud_nodes) || segs_from_counts(&pt, n_clouds, cloud_points)) return -1;
+    const int64_t per = corr_indices != nullptr ? n_corr : nd.max;
+    if (per == 0) return 0;
+    gather_patches_kernel<<<dim3((unsigned)((per * k + 255) / 256), (unsigned)n_clouds), 256, 0, (cudaStream_t)stream>>>(
+        (const long long*)corr_indices, (int)n_corr, (const long long*)node_knn_indices, node_knn_masks, (int)k, points, nd, pt,
+        (long long*)out_indices, out_masks, out_points);
+    GEOB_CHECK_LAUNCH();
+    count_launches(1);
+    return 0;
+}
+
+static int patch_scores_impl(const float* ref_feats, const float* src_feats, const Segs& R, const Segs& Q, int64_t channels,
+                             const int64_t* ref_knn_indices, const int64_t* src_knn_indices, int64_t n_patches, int64_t k, float* scores,
+                             cudaStream_t st) {
+    if (n_patches == 0) return 0;
+    const float div = sqrtf((float)channels);      // feats_f.shape[1] ** 0.5
+    const dim3 grid((unsigned)n_patches, R.n);
+#define LAUNCH_PS(TV) patch_scores_kernel<TV><<<grid, 256, 0, st>>>(ref_feats, src_feats, R, Q, (int)channels,                      \
+                                                                    (const long long*)ref_knn_indices, (const long long*)src_knn_indices, div, scores)
+    if (k == 64) LAUNCH_PS(4);
+    else if (k == 128) LAUNCH_PS(8);
+    else if (k == 32) LAUNCH_PS(2);
+    else
+        GEOB_REQUIRE(false, "patch_scores: num_points_in_patch=%lld unsupported (32, 64, 128)", (long long)k);
+#undef LAUNCH_PS
     GEOB_CHECK_LAUNCH();
     count_launches(1);
     return 0;
@@ -513,23 +681,18 @@ int geob200_gather_patches(const int64_t* corr_indices, int64_t n_corr, const in
 int geob200_patch_scores(const float* ref_feats, int64_t n_ref, const float* src_feats, int64_t n_src, int64_t channels,
                          const int64_t* ref_knn_indices, const int64_t* src_knn_indices, int64_t n_patches, int64_t k,
                          float* scores, void* stream) {
-    cudaStream_t st = (cudaStream_t)stream;
-    if (n_patches == 0) return 0;
-    const float div = sqrtf((float)channels);      // feats_f.shape[1] ** 0.5
-    if (k == 64)
-        patch_scores_kernel<4><<<(unsigned)n_patches, 256, 0, st>>>(ref_feats, (int)n_ref, src_feats, (int)n_src, (int)channels,
-                                                                    (const long long*)ref_knn_indices, (const long long*)src_knn_indices, div, scores);
-    else if (k == 128)
-        patch_scores_kernel<8><<<(unsigned)n_patches, 256, 0, st>>>(ref_feats, (int)n_ref, src_feats, (int)n_src, (int)channels,
-                                                                    (const long long*)ref_knn_indices, (const long long*)src_knn_indices, div, scores);
-    else if (k == 32)
-        patch_scores_kernel<2><<<(unsigned)n_patches, 256, 0, st>>>(ref_feats, (int)n_ref, src_feats, (int)n_src, (int)channels,
-                                                                    (const long long*)ref_knn_indices, (const long long*)src_knn_indices, div, scores);
-    else
-        GEOB_REQUIRE(false, "patch_scores: num_points_in_patch=%lld unsupported (32, 64, 128)", (long long)k);
-    GEOB_CHECK_LAUNCH();
-    count_launches(1);
-    return 0;
+    return patch_scores_impl(ref_feats, src_feats, segs_one(n_ref), segs_one(n_src), channels, ref_knn_indices, src_knn_indices,
+                             n_patches, k, scores, (cudaStream_t)stream);
+}
+
+int geob200_patch_scores_batched(const float* feats, int64_t channels, int64_t n_pairs, const int64_t* cloud_points,
+                                 const int64_t* ref_knn_indices, const int64_t* src_knn_indices, int64_t n_patches, int64_t k,
+                                 float* scores, void* stream) {
+    Segs cl;
+    GEOB_REQUIRE(n_pairs > 0 && 2 * n_pairs <= GEOB_MAX_CLOUDS, "patch_scores_batched: 1..%d pairs", GEOB_MAX_CLOUDS / 2);
+    if (segs_from_counts(&cl, 2 * n_pairs, cloud_points)) return -1;
+    return patch_scores_impl(feats, feats, segs_range(cl, 0, (int)n_pairs), segs_range(cl, (int)n_pairs, (int)n_pairs), channels,
+                             ref_knn_indices, src_knn_indices, n_patches, k, scores, (cudaStream_t)stream);
 }
 
 int geob200_sinkhorn(const float* scores, const uint8_t* row_masks, const uint8_t* col_masks, const float* alpha,

@@ -21,11 +21,18 @@ __device__ __forceinline__ float sqnorm3(float x, float y, float z) {
     return __fadd_rn(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y)), __fmul_rn(z, z));
 }
 
-// argmin over nodes for every point; node occupancy flags
-__global__ void __launch_bounds__(256) p2n_assign_kernel(const float* __restrict__ pts, int N, const float* __restrict__ nodes,
-                                                         int M, long long* __restrict__ point_to_node,
+// argmin over nodes for every point; node occupancy flags.  Cloud s = blockIdx.y: points at Pt.start[s], nodes at Nd.start[s]
+// (indices local to the cloud).
+__global__ void __launch_bounds__(256) p2n_assign_kernel(const float* __restrict__ pts, const float* __restrict__ nodes,
+                                                         const __grid_constant__ Segs Pt, const __grid_constant__ Segs Nd,
+                                                         long long* __restrict__ point_to_node,
                                                          unsigned char* __restrict__ node_masks, int* __restrict__ node_count) {
     extern __shared__ float4 nd[];   // (x,y,z,|n|^2)
+    const int s = blockIdx.y;
+    const int N = Pt.count[s], M = Nd.count[s];
+    if ((int)blockIdx.x * (int)blockDim.x >= N) return;
+    pts += 3ll * Pt.start[s]; point_to_node += Pt.start[s];
+    nodes += 3ll * Nd.start[s]; node_masks += Nd.start[s]; node_count += Nd.start[s];
     for (int m = threadIdx.x; m < M; m += blockDim.x) {
         const float x = nodes[3 * m], y = nodes[3 * m + 1], z = nodes[3 * m + 2];
         nd[m] = make_float4(x, y, z, sqnorm3(x, y, z));
@@ -52,14 +59,25 @@ __global__ void __launch_bounds__(256) p2n_assign_kernel(const float* __restrict
 // candidates are appended to a shared-memory buffer of (d2 bits << 32 | index) keys which is bitonic-sorted and cut back to
 // the best K whenever the next chunk might not fit, so any number of candidates is handled exactly (the former fixed 4096
 // capacity is gone).  d2 in the reference's matmul form, node first: pairwise_distance(nodes, points).
+// Cloud s = blockIdx.y: points (and point_to_node) at Pt.start[s], nodes and output rows at Nd.start[s].
 template <int CAP>
-__global__ void __launch_bounds__(256) knn_select_kernel(const float* __restrict__ pts, int N, const float* __restrict__ nodes,
+__global__ void __launch_bounds__(256) knn_select_kernel(const float* __restrict__ pts, const float* __restrict__ nodes,
+                                                         const __grid_constant__ Segs Pt, const __grid_constant__ Segs Nd,
                                                          const long long* __restrict__ point_to_node, int K,
                                                          long long* __restrict__ knn_indices, unsigned char* __restrict__ knn_masks,
                                                          float* __restrict__ knn_sqdist) {
     __shared__ unsigned long long keys[CAP];
     __shared__ int cnt;
+    const int s = blockIdx.y;
     const int m = blockIdx.x;
+    if (m >= Nd.count[s]) return;
+    const int N = Pt.count[s];
+    pts += 3ll * Pt.start[s];
+    if (point_to_node != nullptr) point_to_node += Pt.start[s];
+    nodes += 3ll * Nd.start[s];
+    knn_indices += (long long)Nd.start[s] * K;
+    if (knn_masks != nullptr) knn_masks += (long long)Nd.start[s] * K;
+    if (knn_sqdist != nullptr) knn_sqdist += (long long)Nd.start[s] * K;
     const int CH = CAP - K;                       // a chunk can add at most CH candidates on top of the K kept ones
     if (threadIdx.x == 0) cnt = 0;
     __syncthreads();
@@ -77,6 +95,7 @@ __global__ void __launch_bounds__(256) knn_select_kernel(const float* __restrict
         }
         __syncthreads();
         const int c = cnt;
+        __syncthreads();                          // every thread has read cnt before the next chunk's atomicAdd changes it
         const bool last = end >= N;
         if (!last && c + CH <= CAP) continue;     // the next chunk still fits: keep appending (uniform branch)
         int n2p = 1;
@@ -181,32 +200,52 @@ using namespace geob200;
 
 extern "C" {
 
+static int point_to_node_partition_impl(const float* points, const float* nodes, const Segs& Pt, const Segs& Nd, int64_t n_nodes,
+                                        int64_t point_limit, int64_t* point_to_node, uint8_t* node_masks, int32_t* node_sizes,
+                                        int64_t* node_knn_indices, uint8_t* node_knn_masks, cudaStream_t st) {
+    GEOB_REQUIRE(point_limit > 0 && point_limit <= 2048, "point_to_node_partition: point_limit must be in 1..2048 (got %lld)",
+                 (long long)point_limit);
+    GEOB_REQUIRE((int64_t)Nd.max * 16 <= 200 * 1024, "point_to_node_partition: too many nodes (%d)", Nd.max);
+    GEOB_CHECK_CUDA(cudaMemsetAsync(node_masks, 0, n_nodes, st));
+    GEOB_CHECK_CUDA(cudaMemsetAsync(node_sizes, 0, 4 * n_nodes, st));
+    if (Pt.max == 0 || Nd.max == 0) return 0;
+    const size_t smem = sizeof(float4) * Nd.max;
+    if (smem > 48 * 1024 && ensure_max_smem((const void*)p2n_assign_kernel)) return -1;
+    p2n_assign_kernel<<<dim3((unsigned)((Pt.max + 255) / 256), Pt.n), 256, smem, st>>>(points, nodes, Pt, Nd, (long long*)point_to_node,
+                                                                                     node_masks, node_sizes);
+    knn_select_kernel<4096><<<dim3((unsigned)Nd.max, Nd.n), 256, 0, st>>>(points, nodes, Pt, Nd, (const long long*)point_to_node,
+                                                                         (int)point_limit, (long long*)node_knn_indices, node_knn_masks, nullptr);
+    GEOB_CHECK_LAUNCH();
+    count_launches(2);
+    return 0;
+}
+
 int geob200_point_to_node_partition(const float* points, int64_t n_points, const float* nodes, int64_t n_nodes,
                                     int64_t point_limit, int64_t* point_to_node, uint8_t* node_masks, int32_t* node_sizes,
                                     int64_t* node_knn_indices, uint8_t* node_knn_masks, int32_t* status, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     GEOB_REQUIRE(n_points > 0 && n_nodes > 0 && point_limit > 0, "point_to_node_partition: empty input");
-    GEOB_REQUIRE(n_nodes * 16 <= 200 * 1024, "point_to_node_partition: too many nodes (%lld)", (long long)n_nodes);
-    GEOB_CHECK_CUDA(cudaMemsetAsync(node_masks, 0, n_nodes, st));
-    GEOB_CHECK_CUDA(cudaMemsetAsync(node_sizes, 0, 4 * n_nodes, st));
     if (status != nullptr) GEOB_CHECK_CUDA(cudaMemsetAsync(status, 0, 4, st));     // kept for ABI stability: always 0 now
-    const size_t smem = sizeof(float4) * n_nodes;
-    if (smem > 48 * 1024 && ensure_max_smem((const void*)p2n_assign_kernel)) return -1;
-    p2n_assign_kernel<<<(unsigned)((n_points + 255) / 256), 256, smem, st>>>(points, (int)n_points, nodes, (int)n_nodes,
-                                                                            (long long*)point_to_node, node_masks, node_sizes);
-    knn_select_kernel<4096><<<(unsigned)n_nodes, 256, 0, st>>>(points, (int)n_points, nodes, (const long long*)point_to_node,
-                                                              (int)point_limit, (long long*)node_knn_indices, node_knn_masks, nullptr);
-    GEOB_CHECK_LAUNCH();
-    count_launches(2);
-    return 0;
+    return point_to_node_partition_impl(points, nodes, segs_one(n_points), segs_one(n_nodes), n_nodes, point_limit, point_to_node,
+                                        node_masks, node_sizes, node_knn_indices, node_knn_masks, st);
+}
+
+int geob200_point_to_node_partition_batched(const float* points, const float* nodes, int64_t n_clouds, const int64_t* cloud_points,
+                                            const int64_t* cloud_nodes, int64_t point_limit, int64_t* point_to_node, uint8_t* node_masks,
+                                            int32_t* node_sizes, int64_t* node_knn_indices, uint8_t* node_knn_masks, void* stream) {
+    Segs Pt, Nd;
+    if (segs_from_counts(&Pt, n_clouds, cloud_points) || segs_from_counts(&Nd, n_clouds, cloud_nodes)) return -1;
+    return point_to_node_partition_impl(points, nodes, Pt, Nd, (int64_t)Nd.start[n_clouds - 1] + Nd.count[n_clouds - 1], point_limit,
+                                        point_to_node, node_masks, node_sizes, node_knn_indices, node_knn_masks, (cudaStream_t)stream);
 }
 
 int geob200_knn_partition(const float* points, int64_t n_points, const float* nodes, int64_t n_nodes, int64_t k,
                           int64_t* knn_indices, float* knn_sq_distances, void* stream) {
     GEOB_REQUIRE(n_points > 0 && n_nodes > 0 && k > 0 && k <= n_points, "knn_partition: need 0 < k <= n_points");
     GEOB_REQUIRE(k <= 2048, "knn_partition: k <= 2048 supported (got %lld)", (long long)k);
-    knn_select_kernel<4096><<<(unsigned)n_nodes, 256, 0, (cudaStream_t)stream>>>(points, (int)n_points, nodes, nullptr, (int)k,
-                                                                                (long long*)knn_indices, nullptr, knn_sq_distances);
+    knn_select_kernel<4096><<<dim3((unsigned)n_nodes, 1), 256, 0, (cudaStream_t)stream>>>(points, nodes, segs_one(n_points), segs_one(n_nodes),
+                                                                                         nullptr, (int)k, (long long*)knn_indices, nullptr,
+                                                                                         knn_sq_distances);
     GEOB_CHECK_LAUNCH();
     count_launches(1);
     return 0;

@@ -4,6 +4,7 @@ PyTorch is used here only for device memory and the current stream; every comput
 sm_90a kernel inside ``libgeob200.so``.  All functions require CUDA tensors and raise ``RuntimeError`` otherwise
 (there is no CPU path in the product).
 """
+import ctypes
 import math
 
 import torch
@@ -711,4 +712,140 @@ def evaluate(gt_node_corr_indices, gt_node_corr_overlaps, ref_node_corr_indices,
                                             est_transform.data_ptr(), src_points.data_ptr(), src_points.shape[0], int(mode),
                                             float(rmse_threshold), float(rre_threshold), float(rte_threshold), out.data_ptr(),
                                             L.stream_ptr()), 'evaluate')
+    return out
+
+
+# ------------------------------------------------------------------------------------------------ batched per-pair stages
+# One launch per stage for all pairs of a batch (GeoTransformer.forward_batch).  Clouds are stacked [ref_1..ref_B, src_1..src_B];
+# ``cloud_nodes`` / ``cloud_points`` are the host lists of the 2B per-cloud row counts.  Each pair gets what the single-pair op gives.
+
+def _host_i64(values):
+    values = [int(v) for v in values]
+    return (ctypes.c_int64 * len(values))(*values)
+
+
+def point_to_node_partition_batched(points, nodes, cloud_points, cloud_nodes, point_limit):
+    """stacked ``point_to_node_partition``: (point_to_node, node_masks, knn_indices, knn_masks), indices local to each cloud"""
+    _f(points, 'points'); _f(nodes, 'nodes')
+    n, m = points.shape[0], nodes.shape[0]
+    dev = points.device
+    p2n = torch.empty((n,), dtype=_i64, device=dev)
+    node_masks = torch.empty((m,), dtype=torch.bool, device=dev)
+    node_sizes = torch.empty((m,), dtype=_i32, device=dev)
+    knn = torch.empty((m, point_limit), dtype=_i64, device=dev)
+    knn_masks = torch.empty((m, point_limit), dtype=torch.bool, device=dev)
+    L.check(L.lib().geob200_point_to_node_partition_batched(points.data_ptr(), nodes.data_ptr(), len(cloud_nodes), _host_i64(cloud_points),
+                                                            _host_i64(cloud_nodes), point_limit, p2n.data_ptr(), node_masks.data_ptr(),
+                                                            node_sizes.data_ptr(), knn.data_ptr(), knn_masks.data_ptr(), L.stream_ptr()),
+            'point_to_node_partition_batched')
+    return p2n, node_masks, knn, knn_masks
+
+
+def gather_patches_batched(corr_indices, n_corr, cloud_nodes, cloud_points, node_knn_indices, node_knn_masks, points):
+    """``corr_indices`` (n_clouds * n_corr,) local node indices, cloud after cloud -> (n_clouds * n_corr, k) patches; ``None``:
+    every node of every cloud is a patch (rows at the superpoint offsets)"""
+    k = node_knn_indices.shape[1]
+    rows = len(cloud_nodes) * n_corr if corr_indices is not None else node_knn_indices.shape[0]
+    dev = points.device
+    idx = torch.empty((rows, k), dtype=_i64, device=dev)
+    msk = torch.empty((rows, k), dtype=torch.bool, device=dev)
+    pts = torch.empty((rows, k, 3), dtype=_f32, device=dev)
+    L.check(L.lib().geob200_gather_patches_batched(L.ptr(corr_indices), n_corr, len(cloud_nodes), _host_i64(cloud_nodes),
+                                                   _host_i64(cloud_points), node_knn_indices.data_ptr(), node_knn_masks.data_ptr(), k,
+                                                   points.data_ptr(), idx.data_ptr(), msk.data_ptr(), pts.data_ptr(), L.stream_ptr()),
+            'gather_patches_batched')
+    return idx, msk, pts
+
+
+def node_correspondences_batched(nodes, knn_points, node_masks, knn_masks, cloud_nodes, transforms, pos_radius):
+    """stacked ``node_correspondences``: (indices (R, 2), overlaps (R,), counts (B,) int32) with pair p's rows at
+    ``sum_{q<p} n_ref(q) * n_src(q)``"""
+    _f(nodes, 'nodes'); _f(knn_points, 'knn_points'); _f(transforms, 'transforms')
+    B = len(cloud_nodes) // 2
+    k = knn_points.shape[1]
+    nn = sum(int(cloud_nodes[p]) * int(cloud_nodes[B + p]) for p in range(B))
+    dev = nodes.device
+    lib = L.lib()
+    ws = L.workspace(lib.geob200_node_correspondences_batched_workspace_bytes(nodes.shape[0], nn, k), dev, tag='node_corr')
+    idx = torch.empty((max(nn, 1), 2), dtype=_i64, device=dev)
+    ov = torch.empty((max(nn, 1),), dtype=_f32, device=dev)
+    cnt = torch.empty((B,), dtype=_i32, device=dev)
+    L.check(lib.geob200_node_correspondences_batched(nodes.data_ptr(), knn_points.data_ptr(), node_masks.data_ptr(), knn_masks.data_ptr(),
+                                                     B, _host_i64(cloud_nodes), k, transforms.data_ptr(), float(pos_radius), idx.data_ptr(),
+                                                     ov.data_ptr(), cnt.data_ptr(), ws.data_ptr(), ws.numel(), L.stream_ptr()),
+            'node_correspondences_batched')
+    return idx, ov, cnt
+
+
+def superpoint_matching_batched(feats, masks, cloud_nodes, num_correspondences, dual_normalization=True):
+    """stacked ``superpoint_matching`` (deferred counts): (corr (2B, k) int64 -- row p ref / row B + p src indices of pair p,
+    scores (B, k), counts (B,) int32)"""
+    _f(feats, 'feats')
+    B = len(cloud_nodes) // 2
+    k = int(num_correspondences)
+    nn = sum(int(cloud_nodes[p]) * int(cloud_nodes[B + p]) for p in range(B))
+    dev = feats.device
+    lib = L.lib()
+    ws = L.workspace(lib.geob200_superpoint_matching_batched_workspace_bytes(feats.shape[0], nn, B), dev)
+    corr = torch.empty((2 * B, k), dtype=_i64, device=dev)
+    sc = torch.empty((B, k), dtype=_f32, device=dev)
+    cnt = torch.empty((B,), dtype=_i32, device=dev)
+    L.check(lib.geob200_superpoint_matching_batched(feats.data_ptr(), feats.shape[1], masks.data_ptr(), B, _host_i64(cloud_nodes), k,
+                                                    int(dual_normalization), corr.data_ptr(), sc.data_ptr(), cnt.data_ptr(), ws.data_ptr(),
+                                                    ws.numel(), L.stream_ptr()), 'superpoint_matching_batched')
+    return corr, sc, cnt
+
+
+def patch_scores_batched(feats, cloud_points, ref_knn_indices, src_knn_indices):
+    """stacked ``patch_scores``: pair p's patches at rows p * (rows / B) of both index tensors"""
+    feats = _detach(feats)
+    B = len(cloud_points) // 2
+    p, k = ref_knn_indices.shape
+    out = torch.empty((p, k, k), dtype=_f32, device=feats.device)
+    L.check(L.lib().geob200_patch_scores_batched(feats.data_ptr(), feats.shape[1], B, _host_i64(cloud_points), ref_knn_indices.data_ptr(),
+                                                 src_knn_indices.data_ptr(), p // B, k, out.data_ptr(), L.stream_ptr()),
+            'patch_scores_batched')
+    return out
+
+
+def local_global_registration_batched(n_pairs, ref_knn_points, src_knn_points, ref_knn_masks, src_knn_masks, score_mat, k,
+                                      acceptance_radius, mutual, confidence_threshold, correspondence_threshold, num_refinement_steps,
+                                      transform_out=None):
+    """stacked ``local_global_registration`` (deferred counts): (ref_c (B, cap, 3), src_c, scores (B, cap), T, counts (B,) int32).
+    ``transform_out``: (B, >= 16) float rows (row stride = its stride(0)) to write the transforms into; else T is (B, 16)."""
+    pt, kk = ref_knn_masks.shape
+    B = int(n_pairs)
+    P = pt // B
+    dev = score_mat.device
+    lib = L.lib()
+    cap = P * kk * k * (1 if mutual else 2)
+    ref_c = torch.empty((B, cap, 3), dtype=_f32, device=dev)
+    src_c = torch.empty((B, cap, 3), dtype=_f32, device=dev)
+    sc = torch.empty((B, cap), dtype=_f32, device=dev)
+    cp = torch.empty((B, cap), dtype=_i32, device=dev)
+    n = torch.empty((B,), dtype=_i32, device=dev)
+    T = torch.empty((B, 16), dtype=_f32, device=dev) if transform_out is None else transform_out
+    ws = L.workspace(lib.geob200_lgr_batched_workspace_bytes(B, P, kk, k), dev)
+    L.check(lib.geob200_local_global_registration_batched(
+        ref_knn_points.data_ptr(), src_knn_points.data_ptr(), ref_knn_masks.data_ptr(), src_knn_masks.data_ptr(), score_mat.data_ptr(),
+        B, P, kk, score_mat.shape[1], k, float(acceptance_radius), int(mutual), float(confidence_threshold), int(correspondence_threshold),
+        int(num_refinement_steps), ref_c.data_ptr(), src_c.data_ptr(), sc.data_ptr(), cp.data_ptr(), n.data_ptr(), T.data_ptr(),
+        T.stride(0), None, None, None, ws.data_ptr(), ws.numel(), L.stream_ptr()), 'local_global_registration_batched')
+    return ref_c, src_c, sc, T, n
+
+
+def evaluate_batched(gt_indices, gt_overlaps, n_gt, corr_indices, n_node_corr, ref_corr_points, src_corr_points, n_corr, gt_transforms,
+                     est_transforms, points, cloud_nodes, cloud_points, mode, acceptance_overlap, acceptance_radius, out,
+                     rmse_threshold=0.0, rre_threshold=0.0, rte_threshold=0.0):
+    """stacked ``evaluate``: row p of ``out`` (B, >= 8 columns, any row stride) = the metrics of pair p; inputs as returned by
+    node_correspondences_batched / superpoint_matching_batched / local_global_registration_batched, ``points`` = the stacked
+    input clouds (``cloud_points`` their 2B counts)"""
+    B = len(cloud_nodes) // 2
+    k = corr_indices.shape[1]
+    L.check(L.lib().geob200_evaluate_batched(
+        gt_indices.data_ptr(), gt_overlaps.data_ptr(), n_gt.data_ptr(), float(acceptance_overlap), corr_indices.data_ptr(),
+        corr_indices[B:].data_ptr(), k, n_node_corr.data_ptr(), ref_corr_points.data_ptr(), src_corr_points.data_ptr(),
+        ref_corr_points.shape[1], n_corr.data_ptr(), float(acceptance_radius), gt_transforms.data_ptr(), est_transforms.data_ptr(),
+        est_transforms.stride(0), points.data_ptr(), B, _host_i64(cloud_nodes), _host_i64(cloud_points), int(mode), float(rmse_threshold),
+        float(rre_threshold), float(rte_threshold), out.data_ptr(), out.stride(0), L.stream_ptr()), 'evaluate_batched')
     return out

@@ -45,8 +45,9 @@ class GeoTransformer(nn.Module):
         order ``[ref_1..ref_B, src_1..src_B]`` at every level) -- the reference asserts batch_size == 1
         (``engine/single_tester.py:39-74``, README "only batch_size=1 is supported").  Backbone and transformer run ONCE over
         the stacked rows of all pairs (per-pair GroupNorm statistics, batched attention launches, one structure-embedding
-        launch); the per-pair stages (grouping, matching, Sinkhorn, LGR, metrics) are enqueued round-robin on
-        ``side_streams`` so that their small kernels overlap.  Per pair the arithmetic is the single-pair forward's.
+        launch); the per-pair stages run once for all pairs too (one launch per stage, the pair index in the grid): grouping and
+        ground-truth correspondences on the first of ``side_streams`` (overlapping the backbone), matching, Sinkhorn, LGR and the
+        metrics on the current stream.  Per pair the arithmetic is the single-pair forward's.
 
         Returns a list of per-pair output dicts (``keep_outputs``), each like ``forward``'s.  With ``results`` (a (B, 24)
         float device tensor) the estimated transform (16) and, with ``evaluator``, the metrics (8) of pair p are written to
@@ -102,26 +103,18 @@ class GeoTransformer(nn.Module):
             def __exit__(self, *e):
                 self.b.__exit__(*e); self.a.__exit__(*e)
 
-        # ---- per-cloud grouping and per-pair ground-truth superpoint correspondences (side streams)
-        part = [None] * (2 * B)
-        gt = [None] * B
+        # ---- grouping of all clouds and ground-truth superpoint correspondences of all pairs (one side stream: overlaps the backbone)
+        cn, cf = [int(v) for v in lens_h[-1]], [int(v) for v in lens_h[fl]]
         transforms = data_dict.get('transform')
-        if transforms is not None and not isinstance(transforms, (list, tuple)):
-            transforms = [transforms[i] for i in range(B)] if transforms.ndim == 3 else [transforms]
+        if transforms is not None:
+            transforms = (torch.stack(list(transforms)) if isinstance(transforms, (list, tuple)) else transforms).reshape(B, 4, 4).contiguous()
+        gt = None
         fork()
-        for p in range(B):
-            with on(p):
-                for c in (p, B + p):
-                    part[c] = GF.point_to_node_partition(cloud(points_f, of, c), cloud(points_c, oc, c), K)
-                if transforms is not None:
-                    rp, sp = part[p], part[B + p]
-                    ref_c, src_c = cloud(points_c, oc, p), cloud(points_c, oc, B + p)
-                    ar_r = GF.scratch_arange(ref_c.shape[0], dev, 'ar_ref')
-                    ar_s = GF.scratch_arange(src_c.shape[0], dev, 'ar_src')
-                    _, _, ref_all = GF.gather_patches(ar_r, rp[2], rp[3], cloud(points_f, of, p))
-                    _, _, src_all = GF.gather_patches(ar_s, sp[2], sp[3], cloud(points_f, of, B + p))
-                    gt[p] = GF.node_correspondences(ref_c, src_c, ref_all, src_all, transforms[p], self.matching_radius, rp[1], sp[1],
-                                                    rp[3], sp[3])
+        with on(0):
+            _, node_masks, knn_idx, knn_masks = GF.point_to_node_partition_batched(points_f, points_c, cf, cn, K)
+            if transforms is not None:
+                _, _, all_pts = GF.gather_patches_batched(None, 0, cn, cf, knn_idx, knn_masks, points_f)
+                gt = GF.node_correspondences_batched(points_c, all_pts, node_masks, knn_masks, cn, transforms, self.matching_radius)
 
         # ---- backbone over all pairs (main stream, overlaps the grouping)
         feats_list = native.backbone_forward(data_dict['features'], data_dict)
@@ -153,47 +146,45 @@ class GeoTransformer(nn.Module):
         y_n = GF.l2_normalize(y)
         mark('transformer')
 
-        # ---- per-pair tail on the side streams
-        join()          # grouping results are consumed below on arbitrary side streams
-        mark('join_grouping+gt')
-        fork()
-        outs = []
-        cm, fm = self.coarse_matching, self.fine_matching
-        for p in range(B):
-            with on(p):
-                rp, sp = part[p], part[B + p]
-                ref_c, src_c = cloud(points_c, oc, p), cloud(points_c, oc, B + p)
-                ref_f, src_f = cloud(points_f, of, p), cloud(points_f, of, B + p)
-                ref_fc, src_fc = cloud(y_n, oc, p), cloud(y_n, oc, B + p)
-                ref_ff, src_ff = cloud(feats_f, of, p), cloud(feats_f, of, B + p)
-                ref_corr, src_corr, node_scores, corr_count = cm(ref_fc, src_fc, rp[1], sp[1], defer_count=True)
-                rk_idx, rk_masks, rk_pts = GF.gather_patches(ref_corr, rp[2], rp[3], ref_f)
-                sk_idx, sk_masks, sk_pts = GF.gather_patches(src_corr, sp[2], sp[3], src_f)
-                scores = GF.patch_scores(ref_ff, src_ff, rk_idx, sk_idx)
-                scores = self.optimal_transport(scores, rk_masks, sk_masks)
-                t_out = results[p, :16] if no_sync else None
-                rc, sc, cs, T, n_corr = GF.local_global_registration(
-                    rk_pts, sk_pts, rk_masks, sk_masks, scores, fm.k, fm.acceptance_radius, fm.mutual, fm.confidence_threshold,
-                    fm.correspondence_threshold, fm.num_refinement_steps, defer_count=True, transform_out=t_out)
-                o = dict(ref_points_c=ref_c, src_points_c=src_c, ref_points_f=ref_f, src_points_f=src_f,
-                         ref_points=cloud(points0, o0, p), src_points=cloud(points0, o0, B + p), ref_feats_c=ref_fc, src_feats_c=src_fc,
-                         ref_feats_f=ref_ff, src_feats_f=src_ff, ref_node_corr_indices=ref_corr, src_node_corr_indices=src_corr,
-                         node_corr_scores=node_scores, ref_node_corr_knn_points=rk_pts, src_node_corr_knn_points=sk_pts,
-                         ref_node_corr_knn_masks=rk_masks, src_node_corr_knn_masks=sk_masks, matching_scores=scores,
-                         ref_corr_points=rc, src_corr_points=sc, corr_scores=cs, estimated_transform=T.reshape(4, 4),
-                         _counts=dict(node_corr=corr_count, corr=n_corr, gt=None if gt[p] is None else gt[p][2]))
-                if gt[p] is not None:
-                    o['gt_node_corr_indices'], o['gt_node_corr_overlaps'] = gt[p][0], gt[p][1]
-                    if evaluator is not None and no_sync:
-                        GF.evaluate(gt[p][0], gt[p][1], ref_corr, src_corr, rc, sc, transforms[p], T, o['src_points'], evaluator.mode,
-                                    evaluator.acceptance_overlap, evaluator.acceptance_radius, evaluator.acceptance_rmse,
-                                    evaluator.acceptance_rre, evaluator.acceptance_rte, out=results[p, 16:], n_gt=gt[p][2],
-                                    n_node_corr=corr_count, n_corr=n_corr)
-                outs.append(o)
+        # ---- matching, patches, Sinkhorn, LGR and metrics of all pairs: one launch per stage on the main stream
         join()
+        mark('join_grouping+gt')
+        cm, fm = self.coarse_matching, self.fine_matching
+        kc = cm.num_correspondences
+        corr, node_scores, corr_count = GF.superpoint_matching_batched(y_n, node_masks, cn, kc, cm.dual_normalization)
+        k_idx, k_masks, k_pts = GF.gather_patches_batched(corr, kc, cn, cf, knn_idx, knn_masks, points_f)
+        r, s = slice(0, B * kc), slice(B * kc, 2 * B * kc)          # patches of the ref clouds, then of the src clouds
+        scores = GF.patch_scores_batched(feats_f, cf, k_idx[r], k_idx[s])
+        scores = self.optimal_transport(scores, k_masks[r], k_masks[s])
+        rc, sc, cs, T, n_corr = GF.local_global_registration_batched(
+            B, k_pts[r], k_pts[s], k_masks[r], k_masks[s], scores, fm.k, fm.acceptance_radius, fm.mutual, fm.confidence_threshold,
+            fm.correspondence_threshold, fm.num_refinement_steps, transform_out=results if no_sync else None)
+        if gt is not None and evaluator is not None and no_sync:
+            GF.evaluate_batched(gt[0], gt[1], gt[2], corr, corr_count, rc, sc, n_corr, transforms, results, points0,
+                                cn, [int(v) for v in lens_h[0]], evaluator.mode, evaluator.acceptance_overlap, evaluator.acceptance_radius,
+                                results[:, 16:], evaluator.acceptance_rmse, evaluator.acceptance_rre, evaluator.acceptance_rte)
         mark('matching+sinkhorn+lgr+metrics')
+        if no_sync and not keep_outputs:
+            return None
+        outs = []
+        g0 = 0
+        for p in range(B):
+            pr, ps = slice(p * kc, (p + 1) * kc), slice((B + p) * kc, (B + p + 1) * kc)
+            o = dict(ref_points_c=cloud(points_c, oc, p), src_points_c=cloud(points_c, oc, B + p), ref_points_f=cloud(points_f, of, p),
+                     src_points_f=cloud(points_f, of, B + p), ref_points=cloud(points0, o0, p), src_points=cloud(points0, o0, B + p),
+                     ref_feats_c=cloud(y_n, oc, p), src_feats_c=cloud(y_n, oc, B + p), ref_feats_f=cloud(feats_f, of, p),
+                     src_feats_f=cloud(feats_f, of, B + p), ref_node_corr_indices=corr[p], src_node_corr_indices=corr[B + p],
+                     node_corr_scores=node_scores[p], ref_node_corr_knn_points=k_pts[pr], src_node_corr_knn_points=k_pts[ps],
+                     ref_node_corr_knn_masks=k_masks[pr], src_node_corr_knn_masks=k_masks[ps], matching_scores=scores[pr],
+                     ref_corr_points=rc[p], src_corr_points=sc[p], corr_scores=cs[p], estimated_transform=T[p, :16].reshape(4, 4),
+                     _counts=dict(node_corr=corr_count[p], corr=n_corr[p], gt=None if gt is None else gt[2][p]))
+            if gt is not None:
+                g1 = g0 + cn[p] * cn[B + p]
+                o['gt_node_corr_indices'], o['gt_node_corr_overlaps'] = gt[0][g0:g1], gt[1][g0:g1]
+                g0 = g1
+            outs.append(o)
         if no_sync:
-            return outs if keep_outputs else None
+            return outs
         # trim the capacity tensors to the counts (one host sync for the whole batch)
         main.synchronize()
         for o in outs:

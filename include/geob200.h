@@ -144,6 +144,17 @@ int geob200_point_to_node_partition(const float* points, int64_t n_points, const
                                     int64_t point_limit, int64_t* point_to_node, uint8_t* node_masks, int32_t* node_sizes,
                                     int64_t* node_knn_indices, uint8_t* node_knn_masks, int32_t* status, void* stream);
 
+/* Batched forms of the per-pair stages (GeoTransformer.forward_batch): one launch per stage covers every cloud or pair of a batch.
+ * Clouds are stacked [ref_1..ref_B, src_1..src_B] as in the batched collate; cloud_nodes / cloud_points are HOST arrays of the 2B
+ * per-cloud row counts at the superpoint / fine (or, for geob200_evaluate_batched, input) level.  Every pair gets exactly what
+ * the single-pair entry point gives it, bit for bit (the single-pair entry points run the same kernels with one pair).
+ * Indices stay local to their cloud.  1 <= B <= 32. */
+/* point_to_node_partition of n_clouds stacked clouds: points / point_to_node at the fine offsets, nodes / node_masks / node_sizes
+ * and the (nodes, point_limit) knn tables at the superpoint offsets.  point_limit <= 2048. */
+int geob200_point_to_node_partition_batched(const float* points, const float* nodes, int64_t n_clouds, const int64_t* cloud_points,
+                                            const int64_t* cloud_nodes, int64_t point_limit, int64_t* point_to_node, uint8_t* node_masks,
+                                            int32_t* node_sizes, int64_t* node_knn_indices, uint8_t* node_knn_masks, void* stream);
+
 /* knn_partition (pointcloud_partition.py:35-57): for every node the k nearest points, ascending by the matmul-form squared
  * distance pairwise_distance(nodes, points) (ties by index).  knn_sq_distances (n_nodes, k) may be NULL.  1 <= k <= min(n_points, 2048). */
 int geob200_knn_partition(const float* points, int64_t n_points, const float* nodes, int64_t n_nodes, int64_t k,
@@ -240,17 +251,35 @@ int geob200_superpoint_matching(const float* ref_feats, const float* src_feats, 
                                 const uint8_t* ref_masks, const uint8_t* src_masks, int64_t num_correspondences, int dual,
                                 int64_t* ref_corr_indices, int64_t* src_corr_indices, float* corr_scores, int32_t* num_out,
                                 void* workspace, size_t workspace_bytes, void* stream);
+/* Batched: feats / masks = the stacked superpoint rows of all 2B clouds.  corr_indices (2B, num_correspondences): row p = ref
+ * indices of pair p, row B + p = its src indices; corr_scores (B, num_correspondences), num_out (B).  Workspace for n_rows stacked
+ * rows and n_products = sum over pairs of n_ref * n_src. */
+size_t geob200_superpoint_matching_batched_workspace_bytes(int64_t n_rows, int64_t n_products, int64_t n_pairs);
+int geob200_superpoint_matching_batched(const float* feats, int64_t channels, const uint8_t* masks, int64_t n_pairs,
+                                        const int64_t* cloud_nodes, int64_t num_correspondences, int dual, int64_t* corr_indices,
+                                        float* corr_scores, int32_t* num_out, void* workspace, size_t workspace_bytes, void* stream);
 
 /* patch gathers of model.py:169-174: indices/masks/points of the k points of each selected superpoint; a negative
  * corr index (padding row of geob200_superpoint_matching) yields an empty patch (sentinel indices, masks 0) */
 int geob200_gather_patches(const int64_t* corr_indices, int64_t n_corr, const int64_t* node_knn_indices,
                            const uint8_t* node_knn_masks, int64_t k, const float* points, int64_t n_points,
                            int64_t* out_indices, uint8_t* out_masks, float* out_points, void* stream);
+/* Batched over n_clouds stacked clouds (knn tables at the superpoint offsets, points at the fine offsets): cloud c gathers the
+ * n_corr patches corr_indices[c * n_corr ..] to rows c * n_corr; with corr_indices = NULL every node of cloud c is a patch
+ * (corr = arange), written at the cloud's superpoint offset. */
+int geob200_gather_patches_batched(const int64_t* corr_indices, int64_t n_corr, int64_t n_clouds, const int64_t* cloud_nodes,
+                                   const int64_t* cloud_points, const int64_t* node_knn_indices, const uint8_t* node_knn_masks, int64_t k,
+                                   const float* points, int64_t* out_indices, uint8_t* out_masks, float* out_points, void* stream);
 
 /* matching_scores = einsum('bnd,bmd->bnm') / sqrt(C) over zero-padded feature tables (model.py:176-188) */
 int geob200_patch_scores(const float* ref_feats, int64_t n_ref, const float* src_feats, int64_t n_src, int64_t channels,
                          const int64_t* ref_knn_indices, const int64_t* src_knn_indices, int64_t n_patches, int64_t k,
                          float* scores, void* stream);
+/* Batched: feats = the stacked fine rows of all 2B clouds; pair p's n_patches patches at p * n_patches of ref_knn_indices,
+ * src_knn_indices and scores. */
+int geob200_patch_scores_batched(const float* feats, int64_t channels, int64_t n_pairs, const int64_t* cloud_points,
+                                 const int64_t* ref_knn_indices, const int64_t* src_knn_indices, int64_t n_patches, int64_t k,
+                                 float* scores, void* stream);
 
 /* LearnableLogOptimalTransport.forward (learnable_sinkhorn.py:20-66): out (n_patches, k+1, k+1) */
 int geob200_sinkhorn(const float* scores, const uint8_t* row_masks, const uint8_t* col_masks, const float* alpha,
@@ -270,6 +299,18 @@ int geob200_local_global_registration(const float* ref_knn_points, const float* 
                                       float* ref_corr_points, float* src_corr_points, float* corr_scores, int32_t* corr_patch,
                                       int32_t* num_corr, float* estimated_transform, float* patch_transforms, int32_t* patch_inliers,
                                       int32_t* best_patch, void* workspace, size_t workspace_bytes, void* stream);
+/* Batched: n_pairs pairs of n_patches patches each (pair p at patch p * n_patches).  Pair p's correspondence rows start at
+ * p * n_patches * k * topk (x2 when not mutual), num_corr / best_patch have n_pairs entries, its transform goes to
+ * estimated_transform + p * transform_ld (>= 16), patch_transforms / patch_inliers are per patch. */
+size_t geob200_lgr_batched_workspace_bytes(int64_t n_pairs, int64_t n_patches, int64_t k, int64_t topk);
+int geob200_local_global_registration_batched(const float* ref_knn_points, const float* src_knn_points, const uint8_t* ref_knn_masks,
+                                              const uint8_t* src_knn_masks, const float* log_scores, int64_t n_pairs, int64_t n_patches,
+                                              int64_t k, int64_t score_ld, int64_t topk, float acceptance_radius, int mutual,
+                                              float confidence_threshold, int64_t correspondence_threshold, int64_t num_refinement_steps,
+                                              float* ref_corr_points, float* src_corr_points, float* corr_scores, int32_t* corr_patch,
+                                              int32_t* num_corr, float* estimated_transform, int64_t transform_ld, float* patch_transforms,
+                                              int32_t* patch_inliers, int32_t* best_patch, void* workspace, size_t workspace_bytes,
+                                              void* stream);
 
 /* weighted_procrustes (modules/registration/procrustes.py:6-73): transforms (batch,4,4); weights may be NULL */
 int geob200_weighted_procrustes(const float* src_points, const float* ref_points, const float* weights, int64_t batch,
@@ -285,6 +326,13 @@ int geob200_node_correspondences(const float* ref_nodes, const float* src_nodes,
                                  const uint8_t* ref_knn_masks, const uint8_t* src_knn_masks, int64_t n_ref, int64_t n_src,
                                  int64_t k, const float* transform, float pos_radius, int64_t* corr_indices,
                                  float* corr_overlaps, int32_t* count, void* workspace, size_t workspace_bytes, void* stream);
+/* Batched: nodes / node_masks and the (rows, k, 3) patch points / (rows, k) masks stacked over the 2B clouds; transforms (B,4,4).
+ * Pair p's rows start at sum_{q<p} n_ref(q) * n_src(q) of corr_indices / corr_overlaps (that many rows of capacity), count (B). */
+size_t geob200_node_correspondences_batched_workspace_bytes(int64_t n_rows, int64_t n_products, int64_t k);
+int geob200_node_correspondences_batched(const float* nodes, const float* knn_points, const uint8_t* node_masks, const uint8_t* knn_masks,
+                                         int64_t n_pairs, const int64_t* cloud_nodes, int64_t k, const float* transforms, float pos_radius,
+                                         int64_t* corr_indices, float* corr_overlaps, int32_t* count, void* workspace, size_t workspace_bytes,
+                                         void* stream);
 
 /* Evaluator.forward (experiments/<exp>/loss.py:95-159; metrics.py:47-112): metrics[8] (device) =
  * {PIR, IR, RRE [deg], RTE, RMSE, RR, #correspondences, #gt superpoint pairs}.  mode 0 = 3DMatch (RMSE of the realigned
@@ -306,6 +354,17 @@ int geob200_evaluate_counts(const int64_t* gt_node_corr_indices, const float* gt
                             int64_t n_corr, const int32_t* n_corr_dev, float acceptance_radius, const float* gt_transform,
                             const float* est_transform, const float* src_points, int64_t n_src_points, int mode, float rmse_threshold,
                             float rre_threshold, float rte_threshold, float* metrics, void* stream);
+/* Batched, one CTA per pair, counts from device memory: ground-truth rows of pair p as laid out by
+ * geob200_node_correspondences_batched (cloud_nodes), n_node_corr / n_corr rows of capacity per pair (pair p at p * that),
+ * gt_transforms (B,4,4), est_transforms at p * transform_ld, the source cloud of pair p = stacked cloud B + p of `points`
+ * (cloud_points: 2B counts), metrics at p * metrics_ld (>= 8). */
+int geob200_evaluate_batched(const int64_t* gt_node_corr_indices, const float* gt_node_corr_overlaps, const int32_t* n_gt_dev,
+                             float acceptance_overlap, const int64_t* ref_node_corr_indices, const int64_t* src_node_corr_indices,
+                             int64_t n_node_corr, const int32_t* n_node_corr_dev, const float* ref_corr_points, const float* src_corr_points,
+                             int64_t n_corr, const int32_t* n_corr_dev, float acceptance_radius, const float* gt_transforms,
+                             const float* est_transforms, int64_t transform_ld, const float* points, int64_t n_pairs, const int64_t* cloud_nodes,
+                             const int64_t* cloud_points, int mode, float rmse_threshold, float rre_threshold, float rte_threshold,
+                             float* metrics, int64_t metrics_ld, void* stream);
 
 /* Profiling aid (bench.py roofline): while enabled, every tensor-core GEMM launch (nn.Linear and the KPConv contraction) is
  * bracketed by CUDA events on its stream; _read synchronises them and returns the count, shapes[3i..] = (m, n, k), ms[i]. */
