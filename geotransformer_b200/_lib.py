@@ -39,6 +39,7 @@ _sig('geob200_kpconv_tc_workspace_bytes', SZ, I64, I64, I64)
 _sig('geob200_kpconv_tc', c_int, P, P, P, P, I64, I64, I64, P, I64, P, P, I64, I64, F, P, P, SZ, P)
 _sig('geob200_set_linear_mode', None, c_int)
 _sig('geob200_linear', c_int, P, I64, P, P, P, I64, I64, I64, I64, c_int, P)
+_sig('geob200_split_tf32', c_int, P, I64, I64, I64, P, P)
 _sig('geob200_linear_batched', c_int, P, I64, I64, P, I64, I64, P, I64, P, I64, I64, I64, I64, I64, I64, c_int, P)
 _sig('geob200_group_norm_workspace_bytes', SZ, I64)
 _sig('geob200_group_norm', c_int, P, I64, I64, I64, P, P, F, P, c_int, F, P, P, SZ, P)

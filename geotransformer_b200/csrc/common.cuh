@@ -101,13 +101,21 @@ int group_norm_impl(const float* x, int64_t n_rows, int64_t channels, int64_t gr
 int linear_group_norm_impl(const float* x, int64_t ldx, const float* weight, const float* bias, int64_t m, int64_t n, int64_t k,
                            int64_t groups, const float* gamma, const float* beta, float eps, const float* residual, int leaky,
                            float slope, float* pre_norm, float* y, void* workspace, size_t workspace_bytes, void* stream,
-                           const GnSeg* seg);
+                           const GnSeg* seg, const float* w_img = nullptr);
 int kpconv_group_norm_impl(const float* s_feats, const float* q_points, const float* s_points, const int64_t* neighbors,
                            int64_t n_query, int64_t n_support, int64_t n_neighbors, const float* kernel_points, int64_t n_kernel,
                            const float* weights_t, const float* bias, int64_t c_in, int64_t c_out, float sigma, int64_t groups,
                            const float* gamma, const float* beta, float eps, int leaky, float slope, float* pre_norm, float* y,
                            void* gn_workspace, size_t gn_workspace_bytes, void* workspace, size_t workspace_bytes, void* stream,
-                           const GnSeg* seg);
+                           const GnSeg* seg, const float* w_img = nullptr);
+// w_img: optional tf32 split image of the GEMM weight (geob200_split_tf32 of weight / weights_t); without one the tensor-core
+// GEMM splits the weight into scratch on every call
+int linear_img(const float* x, int64_t ldx, const float* weight, const float* w_img, const float* bias, float* y, int64_t ldy,
+               int64_t m, int64_t n, int64_t k, int relu, void* stream);
+int kpconv_tc_impl(const float* s_feats, const float* q_points, const float* s_points, const int64_t* neighbors, int64_t n_query,
+                   int64_t n_support, int64_t n_neighbors, const float* kernel_points, int64_t n_kernel, const float* weights_t,
+                   const float* w_img, const float* bias, int64_t c_in, int64_t c_out, float sigma, float* out, void* workspace,
+                   size_t workspace_bytes, void* stream);
 
 int maxpool_seg(const float* x, const int64_t* neighbors, int64_t n_query, int64_t n_support, int64_t n_neighbors, int64_t channels,
                 float* y, const GnSeg* seg, const int* cloud_max, void* stream);

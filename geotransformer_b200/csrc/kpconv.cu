@@ -894,7 +894,7 @@ __global__ void __launch_bounds__(256) upsample_concat_kernel(const float* __res
 using namespace geob200;
 
 namespace geob200 {
-int linear_tc(const float* x, int64_t ldx, const float* w, int64_t ldw, const float* bias, const float* row_scale, float* y, int64_t ldy,
+int linear_tc(const float* x, int64_t ldx, const float* w, int64_t ldw, const float* w_img, const float* bias, const float* row_scale, float* y, int64_t ldy,
               int64_t m, int64_t n, int64_t k, int relu, cudaStream_t st, const GnFuse* gn = nullptr);   // linear_tc.cu
 static int g_linear_mode = 1;   // 1 = wgmma 3xTF32 where the shape allows, 0 = fp32 CUDA cores only
 }
@@ -915,6 +915,16 @@ int geob200_kpconv_tc(const float* s_feats, const float* q_points, const float* 
                       int64_t n_support, int64_t n_neighbors, const float* kernel_points, int64_t n_kernel, const float* weights_t,
                       const float* bias, int64_t c_in, int64_t c_out, float sigma, float* out, void* workspace, size_t workspace_bytes,
                       void* stream) {
+    return geob200::kpconv_tc_impl(s_feats, q_points, s_points, neighbors, n_query, n_support, n_neighbors, kernel_points, n_kernel,
+                                   weights_t, nullptr, bias, c_in, c_out, sigma, out, workspace, workspace_bytes, stream);
+}
+}  // extern "C"
+
+namespace geob200 {
+int kpconv_tc_impl(const float* s_feats, const float* q_points, const float* s_points, const int64_t* neighbors, int64_t n_query,
+                   int64_t n_support, int64_t n_neighbors, const float* kernel_points, int64_t n_kernel, const float* weights_t,
+                   const float* w_img, const float* bias, int64_t c_in, int64_t c_out, float sigma, float* out, void* workspace,
+                   size_t workspace_bytes, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     GEOB_REQUIRE(n_kernel == KP, "kpconv_tc: kernel_size %lld unsupported", (long long)n_kernel);
     GEOB_REQUIRE(n_query > 0 && n_support > 0 && n_neighbors > 0, "kpconv_tc: empty input");
@@ -930,10 +940,22 @@ int geob200_kpconv_tc(const float* s_feats, const float* q_points, const float* 
                          (int)n_support, (int)n_query, (int)c_in, wf, inv_count, st);
     GEOB_CHECK_LAUNCH();
     count_launches(2);
-    const int rc = linear_tc(wf, KP * c_in, weights_t, KP * c_in, bias, inv_count, out, c_out, n_query, c_out, KP * c_in, 0, st);
+    const int rc = linear_tc(wf, KP * c_in, weights_t, KP * c_in, w_img, bias, inv_count, out, c_out, n_query, c_out, KP * c_in, 0, st);
     GEOB_REQUIRE(rc == 0, "kpconv_tc: tensor-core GEMM rejected the shape");
     return 0;
 }
+
+int linear_img(const float* x, int64_t ldx, const float* weight, const float* w_img, const float* bias, float* y, int64_t ldy,
+               int64_t m, int64_t n, int64_t k, int relu, void* stream) {
+    if (g_linear_mode == 1 && m > 0 && n > 0 && k > 0) {
+        const int rc = linear_tc(x, ldx, weight, k, w_img, bias, nullptr, y, ldy, m, n, k, relu, (cudaStream_t)stream);
+        if (rc <= 0) return rc;       // done (0) or hard error (<0); 1 = shape not handled -> fp32 kernel
+    }
+    return geob200_linear(x, ldx, weight, bias, y, ldy, m, n, k, relu, stream);
+}
+}  // namespace geob200
+
+extern "C" {
 
 int geob200_kpconv(const float* s_feats, const float* q_points, const float* s_points, const int64_t* neighbors,
                    int64_t n_query, int64_t n_support, int64_t n_neighbors, const float* kernel_points, int64_t n_kernel,
@@ -990,7 +1012,7 @@ int geob200_linear_batched(const float* x, int64_t ldx, int64_t stride_x, const 
     cudaStream_t st = (cudaStream_t)stream;
     GEOB_REQUIRE(m > 0 && n > 0 && k > 0 && batch > 0, "linear: empty problem");
     if (batch == 1 && g_linear_mode == 1) {
-        const int rc = linear_tc(x, ldx, weight, ldw, bias, nullptr, y, ldy, m, n, k, relu, st);
+        const int rc = linear_tc(x, ldx, weight, ldw, nullptr, bias, nullptr, y, ldy, m, n, k, relu, st);
         if (rc <= 0) return rc;       // done (0) or hard error (<0); 1 = shape not handled -> fp32 kernel below
     }
     const unsigned z = (unsigned)batch;
@@ -1157,7 +1179,7 @@ namespace geob200 {
 int linear_group_norm_impl(const float* x, int64_t ldx, const float* weight, const float* bias, int64_t m, int64_t n, int64_t k,
                            int64_t groups, const float* gamma, const float* beta, float eps, const float* residual, int leaky,
                            float slope, float* pre_norm, float* y, void* workspace, size_t workspace_bytes, void* stream,
-                           const GnSeg* seg) {
+                           const GnSeg* seg, const float* w_img) {
     cudaStream_t st = (cudaStream_t)stream;
     const int64_t np = (seg != nullptr && seg->n_pairs > 1) ? seg->n_pairs : 1;
     GEOB_REQUIRE(m > 0 && n > 0 && k > 0 && groups > 0 && n % groups == 0 && n % 4 == 0, "linear_group_norm: bad shape");
@@ -1166,7 +1188,7 @@ int linear_group_norm_impl(const float* x, int64_t ldx, const float* weight, con
     if (g_linear_mode == 1) {
         const GnWs w = gn_carve(workspace, workspace_bytes, groups, np);
         GnFuse gn{(int)groups, 0, w.partial};
-        const int rc = linear_tc(x, ldx, weight, k, bias, nullptr, pre_norm, n, m, n, k, 0, st, &gn);
+        const int rc = linear_tc(x, ldx, weight, k, w_img, bias, nullptr, pre_norm, n, m, n, k, 0, st, &gn);
         if (rc < 0) return rc;
         if (rc == 0) {
             if (np > 1) {
@@ -1179,7 +1201,7 @@ int linear_group_norm_impl(const float* x, int64_t ldx, const float* weight, con
             return 0;
         }
     }
-    int rc = geob200_linear(x, ldx, weight, bias, pre_norm, n, m, n, k, 0, stream);
+    int rc = linear_img(x, ldx, weight, w_img, bias, pre_norm, n, m, n, k, 0, stream);
     if (rc != 0) return rc;
     return group_norm_impl(pre_norm, m, n, groups, gamma, beta, eps, residual, leaky, slope, y, workspace, workspace_bytes, stream, seg);
 }
@@ -1210,7 +1232,7 @@ int kpconv_group_norm_impl(const float* s_feats, const float* q_points, const fl
                            const float* weights_t, const float* bias, int64_t c_in, int64_t c_out, float sigma, int64_t groups,
                            const float* gamma, const float* beta, float eps, int leaky, float slope, float* pre_norm, float* y,
                            void* gn_workspace, size_t gn_workspace_bytes, void* workspace, size_t workspace_bytes, void* stream,
-                           const GnSeg* seg) {
+                           const GnSeg* seg, const float* w_img) {
     cudaStream_t st = (cudaStream_t)stream;
     const int64_t np = (seg != nullptr && seg->n_pairs > 1) ? seg->n_pairs : 1;
     GEOB_REQUIRE(n_kernel == KP, "kpconv_group_norm: kernel_size %lld unsupported", (long long)n_kernel);
@@ -1234,7 +1256,7 @@ int kpconv_group_norm_impl(const float* s_feats, const float* q_points, const fl
     count_launches(2);
     const GnWs w = gn_carve(gn_workspace, gn_workspace_bytes, groups, np);
     GnFuse gn{(int)groups, 0, w.partial};
-    int rc = linear_tc(wf, KP * c_in, weights_t, KP * c_in, bias, inv_count, pre_norm, c_out, n_query, c_out, KP * c_in, 0, st, &gn);
+    int rc = linear_tc(wf, KP * c_in, weights_t, KP * c_in, w_img, bias, inv_count, pre_norm, c_out, n_query, c_out, KP * c_in, 0, st, &gn);
     if (rc < 0) return rc;
     if (rc == 0) {
         if (np > 1) {
@@ -1247,7 +1269,7 @@ int kpconv_group_norm_impl(const float* s_feats, const float* q_points, const fl
         return 0;
     }
     // group layout not expressible in the epilogue: plain GEMM, then the stand-alone statistics kernel
-    rc = linear_tc(wf, KP * c_in, weights_t, KP * c_in, bias, inv_count, pre_norm, c_out, n_query, c_out, KP * c_in, 0, st);
+    rc = linear_tc(wf, KP * c_in, weights_t, KP * c_in, w_img, bias, inv_count, pre_norm, c_out, n_query, c_out, KP * c_in, 0, st);
     GEOB_REQUIRE(rc == 0, "kpconv_group_norm: tensor-core GEMM rejected the shape");
     return group_norm_impl(pre_norm, n_query, c_out, groups, gamma, beta, eps, nullptr, leaky, slope, y, gn_workspace, gn_workspace_bytes,
                            stream, seg);

@@ -4,16 +4,22 @@
 // error-compensated 3xTF32 scheme: x = x_hi + x_lo, w = w_hi + w_lo (hi = top 19 bits), D += x_hi w_hi + x_hi w_lo +
 // x_lo w_hi with fp32 accumulation (~1e-6 relative, same as an fp32 FMA chain).
 //
+// The weight is split once, outside the GEMM, into a tf32 image [W_hi (N x K) | W_lo (N x K)] (geob200_split_tf32); the
+// activations are split in registers where they are consumed.
+//
 // One 128 x BN output tile at a time (BN = min(N,128)), K in chunks of 32 floats (one 128-byte swizzle row); a CTA walks the
 // tiles t = blockIdx.x, blockIdx.x + gridDim.x, ... (one tile per CTA unless the persistent loop is on), 384 threads:
-//   warps 0-7   consumers    : two warpgroups, rows [0,64) and [64,128) of the tile: wgmma.m64n{BN}k8 tf32, 3 per K-step,
-//                              main products and corrections in two register accumulators; then the epilogue straight from
-//                              the registers (row scale, bias, ReLU, stores, optional GroupNorm statistics)
-//   warp 8      TMA producer : cp.async.bulk.tensor.2d of the raw X tile (128 x 32) and W tile (BN x 32) through SWIZZLE_128B
-//                              tensor maps; out-of-bounds rows/columns are zero-filled by the TMA unit
-//   warps 9-11  splitters    : in-place hi = tf32_rn(x), lo = x - hi into a second buffer (generic proxy ->
-//                              fence.proxy.async), so the MMA sees exact tf32 operands
-// The operand ring runs across tile boundaries: the producer and splitters prepare the next tile while the consumers store.
+//   warps 0-7   consumers    : two warpgroups, rows [0,64) and [64,128) of the tile.  Per 8-wide K-step each thread loads its
+//                              A fragment from the raw fp32 X tile, splits it (hi = tf32_rn(x), lo = x - hi) and issues
+//                              wgmma.m64n{BN}k8 tf32 with A from registers, 3 per K-step, main products and corrections in
+//                              two register accumulators; then the epilogue straight from the registers (row scale, bias,
+//                              ReLU, stores, optional GroupNorm statistics)
+//   warps 8-11  producer     : one thread of warp 8 issues cp.async.bulk.tensor.2d of the X tile (128 x 32) and of the W_hi
+//                              and W_lo tiles (BN x 32 each, two loads through one map of the 2N x K image) through
+//                              SWIZZLE_128B tensor maps; out-of-bounds rows/columns are zero-filled by the TMA unit
+// The producer is a whole warpgroup only so that setmaxnreg can move its registers to the consumers (which hold a chunk's 32
+// A fragment registers besides the 2 x BN/2 accumulator registers): 4 x 32 x 40 + 8 x 32 x 232 <= 65536.
+// The operand ring runs across tile boundaries: the producer loads the next tile while the consumers store.
 #include <cuda.h>
 
 #include <cstdlib>
@@ -33,51 +39,29 @@ constexpr int BM = 128;
 constexpr int KC = 32;
 constexpr int TILE_A = BM * 128;       // 16 KB
 constexpr int TILE_B = 128 * 128;      // 16 KB (BN <= 128 rows)
-constexpr int STAGE = 2 * TILE_A + 2 * TILE_B;   // raw/hi + lo for both operands = 64 KB
-constexpr int NSTAGE = 3;
+constexpr int STAGE = TILE_A + 2 * TILE_B;       // raw X + W_hi + W_lo = 48 KB
+constexpr int NSTAGE = 4;
 constexpr int PRODUCER_WARP = 8;
-constexpr int NSPLIT_WARPS = 3;                       // warps 9..11
-constexpr int NTHREADS = (PRODUCER_WARP + 1 + NSPLIT_WARPS) * 32;   // 384
+constexpr int NTHREADS = (PRODUCER_WARP + 4) * 32;   // 384
 // operand stages + barriers + GroupNorm column sums [8 warps][128] float2 + the bias row, after 1024-byte alignment slack
 constexpr int SMEM = NSTAGE * STAGE + 1024 + 256 + 8 * 128 * 8 + 512;
 
-// splitter: in-place hi = tf32_rn(x), lo = x - hi into the second buffer of each operand (element-wise, so the swizzled
-// positions are irrelevant: same offset in the hi and lo buffers).  Two 16-byte vectors per thread and iteration: their
-// shared-memory round trips overlap.  t = thread index among the NSPLIT_WARPS * 32 splitter threads.
-__device__ __forceinline__ void split_stage(unsigned char* st, int BN, int t) {
-    constexpr int NT = NSPLIT_WARPS * 32;
-    const int nvec_a = TILE_A / 16, nvec_b = BN * 128 / 16;
-    const int nvec = nvec_a + nvec_b;
-    for (int v0 = t; v0 < nvec; v0 += 2 * NT) {
-        const int v1 = v0 + NT;
-        unsigned char* p0 = (v0 < nvec_a) ? (st + v0 * 16) : (st + 2 * TILE_A + (v0 - nvec_a) * 16);
-        unsigned char* l0 = p0 + ((v0 < nvec_a) ? TILE_A : TILE_B);
-        const bool two = v1 < nvec;
-        unsigned char* p1 = !two ? p0 : (v1 < nvec_a) ? (st + v1 * 16) : (st + 2 * TILE_A + (v1 - nvec_a) * 16);
-        unsigned char* l1 = p1 + ((v1 < nvec_a) ? TILE_A : TILE_B);
-        const float4 x0 = *reinterpret_cast<float4*>(p0);
-        const float4 x1 = *reinterpret_cast<float4*>(p1);
-        float4 h0, q0, h1, q1;
-        h0.x = tf32_rn(x0.x); q0.x = x0.x - h0.x;     // round-to-nearest split: |lo| <= 2^-12 |x|, unbiased
-        h0.y = tf32_rn(x0.y); q0.y = x0.y - h0.y;
-        h0.z = tf32_rn(x0.z); q0.z = x0.z - h0.z;
-        h0.w = tf32_rn(x0.w); q0.w = x0.w - h0.w;
-        h1.x = tf32_rn(x1.x); q1.x = x1.x - h1.x;
-        h1.y = tf32_rn(x1.y); q1.y = x1.y - h1.y;
-        h1.z = tf32_rn(x1.z); q1.z = x1.z - h1.z;
-        h1.w = tf32_rn(x1.w); q1.w = x1.w - h1.w;
-        *reinterpret_cast<float4*>(p0) = h0;
-        *reinterpret_cast<float4*>(l0) = q0;
-        if (two) {
-            *reinterpret_cast<float4*>(p1) = h1;
-            *reinterpret_cast<float4*>(l1) = q1;
-        }
+// [hi | lo] image of a row-major (n x k, leading dimension ld) fp32 matrix: out[r][c] = tf32_rn(w), out[n + r][c] = w - hi
+__global__ void __launch_bounds__(256) split_tf32_kernel(const float* __restrict__ w, long long ld, long long n, long long k,
+                                                         float* __restrict__ out) {
+    const long long nk = n * k;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nk; i += (long long)gridDim.x * blockDim.x) {
+        const long long r = i / k, c = i % k;
+        const float x = w[r * ld + c];
+        const float hi = tf32_rn(x);
+        out[i] = hi;
+        out[nk + i] = x - hi;
     }
-    fence_proxy_async();
 }
 
 // BNI = wgmma N (32, 64 or 128) >= BN; B rows [BN, BNI) of a stage hold stale data and only feed output columns that are
 // never stored.  Tile t -> (split z, row tile, column tile), column tile fastest: neighbouring CTAs share their X rows in L2.
+// map_w covers the 2N x K weight image: W_hi rows at n0, W_lo rows at N + n0.
 template <int BNI>
 __global__ void __launch_bounds__(NTHREADS, 1) linear_tc_kernel(const __grid_constant__ CUtensorMap map_x,
                                                                 const __grid_constant__ CUtensorMap map_w,
@@ -89,9 +73,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) linear_tc_kernel(const __grid_con
     extern __shared__ unsigned char smem_raw[];
     unsigned char* smem = (unsigned char*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
     uint64_t* bars = (uint64_t*)(smem + NSTAGE * STAGE);
-    uint64_t* raw_full = bars;                  // TMA landed
-    uint64_t* split_full = bars + NSTAGE;       // hi/lo ready
-    uint64_t* empty = bars + 2 * NSTAGE;        // MMAs done with the stage
+    uint64_t* full = bars;                      // TMA landed
+    uint64_t* empty = bars + NSTAGE;            // MMAs done with the stage
     float2* gn_sm = (float2*)(smem + NSTAGE * STAGE + 256);        // [8 consumer warps][128 columns] (sum, sum of squares)
     float* bias_s = (float*)(gn_sm + 8 * 128);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -99,15 +82,16 @@ __global__ void __launch_bounds__(NTHREADS, 1) linear_tc_kernel(const __grid_con
     const int tiles_per_split = col_tiles * row_tiles;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < NSTAGE; ++s) { mbar_init(&raw_full[s], 1); mbar_init(&split_full[s], NSPLIT_WARPS); mbar_init(&empty[s], 8); }
+        for (int s = 0; s < NSTAGE; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_x) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w) : "memory");
     }
     __syncthreads();
 
-    if (warp == PRODUCER_WARP) {
-        if (lane == 0) {
+    if (warp >= PRODUCER_WARP) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+        if (warp == PRODUCER_WARP && lane == 0) {
             int s = 0;
             uint32_t ph = 0;
             for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
@@ -117,34 +101,19 @@ __global__ void __launch_bounds__(NTHREADS, 1) linear_tc_kernel(const __grid_con
                 for (int kc = kc0; kc < kc1; ++kc) {
                     mbar_wait(&empty[s], ph ^ 1u);
                     unsigned char* st = smem + s * STAGE;
-                    mbar_arrive_expect_tx(&raw_full[s], (uint32_t)(TILE_A + BN * 128));
-                    tma_load_2d(st, &map_x, kc * KC, m0, &raw_full[s]);
-                    tma_load_2d(st + 2 * TILE_A, &map_w, kc * KC, n0, &raw_full[s]);
+                    mbar_arrive_expect_tx(&full[s], (uint32_t)(TILE_A + 2 * BN * 128));
+                    tma_load_2d(st, &map_x, kc * KC, m0, &full[s]);
+                    tma_load_2d(st + TILE_A, &map_w, kc * KC, n0, &full[s]);
+                    tma_load_2d(st + TILE_A + TILE_B, &map_w, kc * KC, N + n0, &full[s]);
                     if (++s == NSTAGE) { s = 0; ph ^= 1u; }
                 }
             }
         }
         return;
     }
-    if (warp > PRODUCER_WARP) {
-        const int ts = threadIdx.x - (PRODUCER_WARP + 1) * 32;
-        int s = 0;
-        uint32_t ph = 0;
-        for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-            const int z = t / tiles_per_split;
-            const int kc0 = z * chunks_per_split, kc1 = min(nk, kc0 + chunks_per_split);
-            for (int kc = kc0; kc < kc1; ++kc) {
-                mbar_wait(&raw_full[s], ph);
-                split_stage(smem + s * STAGE, BN, ts);
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&split_full[s]);
-                if (++s == NSTAGE) { s = 0; ph ^= 1u; }
-            }
-        }
-        return;
-    }
 
     // ---- consumers ----
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
     const int wg = warp >> 2, wq = warp & 3;
     int s = 0;
     uint32_t ph = 0;
@@ -164,31 +133,47 @@ __global__ void __launch_bounds__(NTHREADS, 1) linear_tc_kernel(const __grid_con
         float acc[R], cor[R];
 #pragma unroll
         for (int i = 0; i < R; ++i) { acc[i] = 0.f; cor[i] = 0.f; }
-        int prev_s = -1;
+        // A fragment of this thread: rows g and g + 8 of the warp's 16-row slice, K columns 8kk + (lane % 4) and + 4.  In the
+        // 128-byte swizzle, 16-byte chunk j of row r sits at chunk position j ^ (r % 8) = j ^ g: the 32 lanes of a load hit 32
+        // different banks.
+        const int g = lane >> 2, tq = lane & 3;
+        const int a_off = (wg * 64 + wq * 16 + g) * 128 + tq * 4;
+        // wgmma reads its register operands asynchronously: a chunk's fragments may only be overwritten once its MMAs are
+        // complete, so each chunk waits for its own MMAs (wait_group 0) before the next chunk's fragments are loaded; the
+        // other consumer warpgroup keeps the tensor cores busy meanwhile
         for (int kc = kc0; kc < kc1; ++kc) {
-            mbar_wait(&split_full[s], ph);
-            const uint32_t st = smem_u32(smem + s * STAGE);
-            const uint64_t a_hi = make_desc(st + wg * (TILE_A / 2)), a_lo = make_desc(st + TILE_A + wg * (TILE_A / 2));
-            const uint64_t b_hi = make_desc(st + 2 * TILE_A), b_lo = make_desc(st + 2 * TILE_A + TILE_B);
+            mbar_wait(&full[s], ph);
+            unsigned char* st = smem + s * STAGE;
+            uint32_t f[2][KC / 8][4];           // [hi / lo][k-step][4]
+#pragma unroll
+            for (int kk = 0; kk < KC / 8; ++kk)
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    const int j = 2 * kk + (e >> 1);       // 16-byte chunk of the K column
+                    const float x = *reinterpret_cast<const float*>(st + a_off + (e & 1) * 8 * 128 + ((j ^ g) << 4));
+                    const float hi = tf32_rn(x);        // round-to-nearest split: |lo| <= 2^-12 |x|, unbiased
+                    f[0][kk][e] = __float_as_uint(hi);
+                    f[1][kk][e] = __float_as_uint(x - hi);
+                }
+            const uint32_t sb = smem_u32(st + TILE_A);
+            const uint64_t b_hi = make_desc(sb), b_lo = make_desc(sb + TILE_B);
             wgmma_fence();
 #pragma unroll
             for (int kk = 0; kk < KC / 8; ++kk) {
                 const uint64_t adv = (uint64_t)(kk * 2);      // +32 bytes in 16-byte units
                 const uint32_t accum = (kc == kc0 && kk == 0) ? 0u : 1u;
-                wgmma_tf32<BNI>(acc, a_hi + adv, b_hi + adv, accum);
-                wgmma_tf32<BNI>(cor, a_hi + adv, b_lo + adv, accum);
-                wgmma_tf32<BNI>(cor, a_lo + adv, b_hi + adv, 1u);
+                wgmma_tf32_rs<BNI>(acc, f[0][kk], b_hi + adv, accum);
+                wgmma_tf32_rs<BNI>(cor, f[0][kk], b_lo + adv, accum);
+                wgmma_tf32_rs<BNI>(cor, f[1][kk], b_hi + adv, 1u);
             }
             wgmma_commit();
-            wgmma_wait<1>();                    // the previous chunk's MMAs are done: its stage can be refilled
-            if (prev_s >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty[prev_s]); }
-            prev_s = s;
+            wgmma_wait<0>();                    // this chunk's MMAs are done: its stage can be refilled
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty[s]);
             if (++s == NSTAGE) { s = 0; ph ^= 1u; }
         }
-        wgmma_wait<0>();
         reg_fence(acc);
         reg_fence(cor);
-        if (prev_s >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty[prev_s]); }
 
         // epilogue: this thread holds rows r0 and r0 + 8, columns 8j + 2(lane % 4) + {0, 1}
         const int r0 = m0 + wg * 64 + wq * 16 + (lane >> 2);
@@ -336,13 +321,14 @@ static bool g_prof_on = false;
 static bool g_splitk_on = true;
 static bool g_persistent_on = true;    // persistent tile loop for GEMMs of more than one wave of tiles (geob200_set_linear_persistent)
 
-// ---- split-K scratch: one grow-only buffer per stream (like a BLAS workspace; freed with the process) ---------------------
-struct SplitWs { void* ptr; size_t bytes; };
-static std::vector<std::pair<cudaStream_t, SplitWs>> g_split_ws;
+// ---- per-stream scratch: split-K partials and weight images; one grow-only buffer per stream and use (like a BLAS
+// workspace; freed with the process) ----------------------------------------------------------------------------------------
+struct StreamWs { void* ptr; size_t bytes; };
+static std::vector<std::pair<cudaStream_t, StreamWs>> g_split_ws, g_wimg_ws;
 static std::mutex g_split_mu;
-static float* splitk_scratch(cudaStream_t st, size_t bytes) {
+static float* stream_scratch(std::vector<std::pair<cudaStream_t, StreamWs>>& pool, cudaStream_t st, size_t bytes) {
     std::lock_guard<std::mutex> lk(g_split_mu);
-    for (auto& e : g_split_ws)
+    for (auto& e : pool)
         if (e.first == st) {
             if (e.second.bytes >= bytes) return (float*)e.second.ptr;
             // stream-ordered free: earlier kernels on this stream may still read the old buffer
@@ -352,24 +338,32 @@ static float* splitk_scratch(cudaStream_t st, size_t bytes) {
             e.second.bytes = bytes * 2;
             return (float*)e.second.ptr;
         }
-    SplitWs w{nullptr, 0};
+    StreamWs w{nullptr, 0};
     const size_t cap = bytes * 2 > (16u << 20) ? bytes * 2 : (16u << 20);
     if (cudaMallocAsync(&w.ptr, cap, st) != cudaSuccess) return nullptr;
     w.bytes = cap;
-    g_split_ws.push_back({st, w});
+    pool.push_back({st, w});
     return (float*)w.ptr;
 }
 
-// returns 1 when the shape/alignment is not handled by the tensor-core path (caller falls back to the fp32 kernel)
-int linear_tc(const float* x, int64_t ldx, const float* w, int64_t ldw, const float* bias, const float* row_scale, float* y, int64_t ldy,
-              int64_t m, int64_t n, int64_t k, int relu, cudaStream_t st, const GnFuse* gn) {
-    if (m < 64 || n < 32 || (n % 16) != 0 || (k % 4) != 0 || (ldx % 4) != 0 || (ldw % 4) != 0) return 1;
-    if ((reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(w) & 15)) return 1;
+static void launch_split_tf32(const float* w, int64_t ld, int64_t n, int64_t k, float* out, cudaStream_t st) {
+    const long long nk = (long long)n * k;
+    long long blocks = (nk + 255) / 256;
+    if (blocks > 4LL * num_sms()) blocks = 4LL * num_sms();
+    ltc::split_tf32_kernel<<<(unsigned)(blocks > 0 ? blocks : 1), 256, 0, st>>>(w, ld, n, k, out);
+    count_launches(1);
+}
+
+// Y = X . W^T (+ bias, row scale, ReLU, GroupNorm statistics) on the tensor cores.  w_img is the [hi | lo] tf32 image of W
+// (geob200_split_tf32, 2n x k contiguous); without one, W (leading dimension ldw) is split into per-stream scratch first.
+// Returns 1 when the shape/alignment is not handled by the tensor-core path (caller falls back to the fp32 kernel).
+int linear_tc(const float* x, int64_t ldx, const float* w, int64_t ldw, const float* w_img, const float* bias, const float* row_scale,
+              float* y, int64_t ldy, int64_t m, int64_t n, int64_t k, int relu, cudaStream_t st, const GnFuse* gn) {
+    if (m < 64 || n < 32 || (n % 16) != 0 || (k % 4) != 0 || (ldx % 4) != 0) return 1;
+    if ((reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(w_img) & 15)) return 1;
+    if (w_img == nullptr && ((ldw % 4) != 0 || (reinterpret_cast<uintptr_t>(w) & 15))) return 1;
     if (n > 128 && (n % 128) != 0) return 1;
     const int BN = (int)(n >= 128 ? 128 : n);
-    CUtensorMap mx, mw;
-    if (ltc::encode_map(&mx, x, m, k, ldx, ltc::BM)) return -1;
-    if (ltc::encode_map(&mw, w, n, k, ldw, BN)) return -1;
     const int col_tiles = (int)(n / BN), row_tiles = (int)((m + ltc::BM - 1) / ltc::BM);
     GnFuse g{};
     if (gn != nullptr) {
@@ -397,9 +391,18 @@ int linear_tc(const float* x, int64_t ldx, const float* w, int64_t ldw, const fl
     if (splits > 1) {
         cps = (nk + splits - 1) / splits;
         splits = (nk + cps - 1) / cps;
-        part = splitk_scratch(st, (size_t)splits * (size_t)m * (size_t)n * sizeof(float));
+        part = stream_scratch(g_split_ws, st, (size_t)splits * (size_t)m * (size_t)n * sizeof(float));
         if (part == nullptr) { splits = 1; cps = nk; }
     }
+    float* img = nullptr;
+    if (w_img == nullptr) {
+        img = stream_scratch(g_wimg_ws, st, (size_t)2 * (size_t)n * (size_t)k * sizeof(float));
+        if (img == nullptr) { set_error("linear_tc: weight image scratch allocation failed"); return -1; }
+        w_img = img;
+    }
+    CUtensorMap mx, mw;
+    if (ltc::encode_map(&mx, x, m, k, ldx, ltc::BM)) return -1;
+    if (ltc::encode_map(&mw, w_img, 2 * n, k, k, BN)) return -1;
     ProfRec rec{};
     const bool prof = g_prof_on;
     if (prof) {
@@ -408,6 +411,7 @@ int linear_tc(const float* x, int64_t ldx, const float* w, int64_t ldw, const fl
         rec.m = m; rec.n = n; rec.k = k;
         cudaEventRecord(rec.a, st);
     }
+    if (img != nullptr) launch_split_tf32(w, ldw, n, k, img, st);
     // one CTA per tile, or (persistent loop) one CTA per SM walking the tiles of a GEMM of more than one wave
     const int num_tiles = tiles * splits;
     const bool persistent = g_persistent_on && splits == 1 && tiles > num_sms();
@@ -443,6 +447,14 @@ extern "C" {
 
 int geob200_set_linear_persistent(int on) {
     geob200::g_persistent_on = on != 0;
+    return 0;
+}
+
+// [hi | lo] tf32 image of a row-major weight (n x k, leading dimension ld): out (2n x k, contiguous) = [tf32_rn(w); w - hi]
+int geob200_split_tf32(const float* w, int64_t ld, int64_t n, int64_t k, float* out, void* stream) {
+    GEOB_REQUIRE(n > 0 && k > 0 && ld >= k, "split_tf32: bad shape (%lld x %lld, ld %lld)", (long long)n, (long long)k, (long long)ld);
+    geob200::launch_split_tf32(w, ld, n, k, out, (cudaStream_t)stream);
+    GEOB_CHECK_LAUNCH();
     return 0;
 }
 

@@ -39,8 +39,8 @@ static int run_kpconv(Ctx& c, const geob200_kpconv_t& k, const float* s_feats, c
         const size_t mark = c.ar.off;
         void* ws = c.ar.take<char>(wb);
         GEOB_REQUIRE(c.ar.ok(), "native: arena too small (kpconv)");
-        TRY(geob200_kpconv_tc(s_feats, q_pts, s_pts, nbr, m, ns, h, k.kernel_points, 15, k.weights_t, k.bias, k.c_in, k.c_out, k.sigma,
-                              out, ws, wb, c.stream));
+        TRY(kpconv_tc_impl(s_feats, q_pts, s_pts, nbr, m, ns, h, k.kernel_points, 15, k.weights_t, k.weights_img, k.bias, k.c_in, k.c_out,
+                           k.sigma, out, ws, wb, c.stream));
         c.ar.off = mark;     // stream-ordered reuse: the next kernel that touches this scratch runs after the GEMM
         return 0;
     }
@@ -67,7 +67,8 @@ static int run_kpconv_norm(Ctx& c, const geob200_kpconv_t& k, const geob200_norm
         void* ws = c.ar.take<char>(wb);
         GEOB_REQUIRE(c.ar.ok(), "native: arena too small (kpconv)");
         TRY(kpconv_group_norm_impl(s_feats, q_pts, s_pts, nbr, m, ns, h, k.kernel_points, 15, k.weights_t, k.bias, k.c_in, k.c_out,
-                                   k.sigma, c.groups, n.gamma, n.beta, 1e-5f, 1, 0.1f, y, out, c.gn_ws, c.gn_ws_bytes, ws, wb, c.stream, seg));
+                                   k.sigma, c.groups, n.gamma, n.beta, 1e-5f, 1, 0.1f, y, out, c.gn_ws, c.gn_ws_bytes, ws, wb, c.stream, seg,
+                                   k.weights_img));
         c.ar.off = mark;     // stream-ordered reuse: the next kernel that touches this scratch runs after the GEMM
         return 0;
     }
@@ -81,7 +82,7 @@ static int run_unary(Ctx& c, const geob200_linear_t& l, const geob200_norm_t& n,
     float* t = c.fl(rows, l.c_out);
     GEOB_REQUIRE(c.ar.ok(), "native: arena too small (unary)");
     TRY(linear_group_norm_impl(x, l.c_in, l.weight, l.bias, rows, l.c_out, l.c_in, c.groups, n.gamma, n.beta, 1e-5f, residual, leaky,
-                               0.1f, t, out, c.gn_ws, c.gn_ws_bytes, c.stream, seg));
+                               0.1f, t, out, c.gn_ws, c.gn_ws_bytes, c.stream, seg, l.weight_img));
     return 0;
 }
 
@@ -215,7 +216,7 @@ int geob200_backbone_forward_batched(const geob200_backbone_t* net, const float*
         const geob200_linear_t& l = net->decoders[S - 1 - lvl];
         float* o = out_feats[oi++];
         if (lvl == net->finest_decoder) {
-            TRY(geob200_linear(cat, l.c_in, l.weight, l.bias, o, l.c_out, m, l.c_out, l.c_in, 0, stream));
+            TRY(linear_img(cat, l.c_in, l.weight, l.weight_img, l.bias, o, l.c_out, m, l.c_out, l.c_in, 0, stream));
         } else {
             TRY(run_unary(c, l, net->decoder_norms[S - 1 - lvl], cat, m, nullptr, 1, o, sg[lvl - 1]));
         }
@@ -238,10 +239,10 @@ static int run_tail(Ctx& c, const geob200_tlayer_t& L, const float* hidden, cons
     float* y1 = c.fl(rows, 2 * ch);
     float* y2 = c.fl(rows, ch);
     GEOB_REQUIRE(c.ar.ok(), "native: arena too small (transformer tail)");
-    TRY(geob200_linear(hidden, ch, L.att_linear.weight, L.att_linear.bias, h, ch, rows, ch, ch, 0, c.stream));
+    TRY(linear_img(hidden, ch, L.att_linear.weight, L.att_linear.weight_img, L.att_linear.bias, h, ch, rows, ch, ch, 0, c.stream));
     TRY(geob200_add_layernorm(h, inp, L.att_norm.gamma, L.att_norm.beta, rows, ch, 1e-5f, x, c.stream));
-    TRY(geob200_linear(x, ch, L.expand.weight, L.expand.bias, y1, 2 * ch, rows, 2 * ch, ch, 1, c.stream));
-    TRY(geob200_linear(y1, 2 * ch, L.squeeze.weight, L.squeeze.bias, y2, ch, rows, ch, 2 * ch, 0, c.stream));
+    TRY(linear_img(x, ch, L.expand.weight, L.expand.weight_img, L.expand.bias, y1, 2 * ch, rows, 2 * ch, ch, 1, c.stream));
+    TRY(linear_img(y1, 2 * ch, L.squeeze.weight, L.squeeze.weight_img, L.squeeze.bias, y2, ch, rows, ch, 2 * ch, 0, c.stream));
     TRY(geob200_add_layernorm(x, y2, L.out_norm.gamma, L.out_norm.beta, rows, ch, 1e-5f, out, c.stream));
     return 0;
 }
@@ -303,7 +304,7 @@ int geob200_transformer_forward_batched(const geob200_tlayer_t* layers, int64_t 
             float* qb = c.fl(n, H);
             float* hidden = c.fl(n, C);
             GEOB_REQUIRE(c.ar.ok(), "native: arena too small (self layer)");
-            TRY(geob200_linear(x, C, L.w_qkv, L.b_qkv, qkv, 3 * C, n, 3 * C, C, 0, stream));
+            TRY(linear_img(x, C, L.w_qkv, L.w_qkv_img, L.b_qkv, qkv, 3 * C, n, 3 * C, C, 0, stream));
             const int64_t d = C / H;
             TRY(geob200_linear_batched(qkv, 3 * C, d, L.wp_t, C, d, nullptr, 0, qp, H * C, C, n, C, d, H, 0, stream));
             TRY(geob200_head_bias(qkv, 3 * C, L.bp, n, C, H, qb, stream));
@@ -324,8 +325,8 @@ int geob200_transformer_forward_batched(const geob200_tlayer_t* layers, int64_t 
             float* hid1 = c.fl(Sn, C);
             GEOB_REQUIRE(c.ar.ok(), "native: arena too small (cross layer)");
             // feats0 <- layer(feats0, feats1) for every pair
-            TRY(geob200_linear(x, C, L.w_q, L.b_q, q0, C, R, C, C, 0, stream));
-            TRY(geob200_linear(x + R * C, C, L.w_kv, L.b_kv, kv1, 2 * C, Sn, 2 * C, C, 0, stream));
+            TRY(linear_img(x, C, L.w_q, L.w_q_img, L.b_q, q0, C, R, C, C, 0, stream));
+            TRY(linear_img(x + R * C, C, L.w_kv, L.w_kv_img, L.b_kv, kv1, 2 * C, Sn, 2 * C, C, 0, stream));
             for (int64_t p = 0; p < B; ++p) {
                 const int64_t ro = off[p], so = off[B + p] - R;
                 items[p] = geob200_att_item_t{q0 + ro * C, kv1 + so * 2 * C, kv1 + so * 2 * C + C, nullptr, nullptr, nullptr, hid0 + ro * C,
@@ -334,8 +335,8 @@ int geob200_transformer_forward_batched(const geob200_tlayer_t* layers, int64_t 
             TRY(geob200_attention_batched(items, B, C, 2 * C, 2 * C, C, C, H, att_ws, att_ws_bytes, stream));
             TRY(run_tail(c, L, hid0, x, R, C, y));
             // feats1 <- layer(feats1, UPDATED feats0)   (conditional_transformer.py:109-111, parallel=False)
-            TRY(geob200_linear(x + R * C, C, L.w_q, L.b_q, q1, C, Sn, C, C, 0, stream));
-            TRY(geob200_linear(y, C, L.w_kv, L.b_kv, kv0, 2 * C, R, 2 * C, C, 0, stream));
+            TRY(linear_img(x + R * C, C, L.w_q, L.w_q_img, L.b_q, q1, C, Sn, C, C, 0, stream));
+            TRY(linear_img(y, C, L.w_kv, L.w_kv_img, L.b_kv, kv0, 2 * C, R, 2 * C, C, 0, stream));
             for (int64_t p = 0; p < B; ++p) {
                 const int64_t ro = off[p], so = off[B + p] - R;
                 items[p] = geob200_att_item_t{q1 + so * C, kv0 + ro * 2 * C, kv0 + ro * 2 * C + C, nullptr, nullptr, nullptr, hid1 + so * C,

@@ -121,6 +121,18 @@ def linear(x, weight, bias=None, relu=False, out=None):
     return out
 
 
+def split_tf32(weight):
+    """(n, k) fp32 weight -> (2n, k) image [hi; lo]: hi = weight rounded to tf32 (nearest, ties away from zero), lo = weight - hi.
+    The operand layout in which the tensor-core GEMM reads its weights."""
+    weight = _detach(weight)
+    if not weight.is_cuda or weight.dtype != _f32 or weight.dim() != 2 or weight.stride(1) != 1:
+        raise RuntimeError('split_tf32: weight must be a 2-D float32 CUDA tensor with unit inner stride')
+    n, k = weight.shape
+    out = torch.empty((2 * n, k), dtype=_f32, device=weight.device)
+    L.check(L.lib().geob200_split_tf32(weight.data_ptr(), weight.stride(0), n, k, out.data_ptr(), L.stream_ptr()), 'split_tf32')
+    return out
+
+
 def group_norm(x, weight, bias, groups, eps=1e-5, negative_slope=None, residual=None):
     x, weight, bias = _detach(x), _detach(weight), _detach(bias)
     _f(x, 'x')

@@ -1,7 +1,8 @@
 """ctypes mirror of the native stage drivers (``csrc/native.cu``, structs in ``include/geob200.h``).
 
 ``NativeModel`` snapshots the parameter pointers of a ``GeoTransformer`` module (plus the derived weight layouts: the
-tensor-core KPConv transposes, fused q|k|v and k|v projections, ``proj_p`` transposes) into the C structs and runs the
+tensor-core KPConv transposes, fused q|k|v and k|v projections, ``proj_p`` transposes, and the tf32 split images that the
+tensor-core GEMM reads in place of its weights) into the C structs and runs the
 backbone and the transformer with ONE C call each.  Same kernels, same order as the module path: results are bitwise
 identical (tests/test_gpu_native.py); only the host cost changes (~340 Python ops per pair -> ~40).
 """
@@ -17,7 +18,7 @@ P, I64, I32, F32 = ctypes.c_void_p, ctypes.c_int64, ctypes.c_int32, ctypes.c_flo
 
 
 class LinearT(ctypes.Structure):
-    _fields_ = [('weight', P), ('bias', P), ('c_in', I64), ('c_out', I64)]
+    _fields_ = [('weight', P), ('bias', P), ('c_in', I64), ('c_out', I64), ('weight_img', P)]
 
 
 class NormT(ctypes.Structure):
@@ -25,7 +26,8 @@ class NormT(ctypes.Structure):
 
 
 class KPConvT(ctypes.Structure):
-    _fields_ = [('weights', P), ('weights_t', P), ('bias', P), ('kernel_points', P), ('c_in', I64), ('c_out', I64), ('sigma', F32)]
+    _fields_ = [('weights', P), ('weights_t', P), ('bias', P), ('kernel_points', P), ('c_in', I64), ('c_out', I64), ('sigma', F32),
+                ('weights_img', P)]
 
 
 class ResBlockT(ctypes.Structure):
@@ -42,7 +44,7 @@ class BackboneT(ctypes.Structure):
 class TLayerT(ctypes.Structure):
     _fields_ = [('is_self', I32), ('reserved', I32), ('w_qkv', P), ('b_qkv', P), ('w_q', P), ('b_q', P), ('w_kv', P), ('b_kv', P),
                 ('wp_t', P), ('bp', P), ('att_linear', LinearT), ('att_norm', NormT), ('expand', LinearT), ('squeeze', LinearT),
-                ('out_norm', NormT)]
+                ('out_norm', NormT), ('w_qkv_img', P), ('w_q_img', P), ('w_kv_img', P)]
 
 
 def _ptr(t):
@@ -62,8 +64,14 @@ class NativeModel:
         self.heads = model.transformer.transformer.layers[0].attention.attention.num_heads
 
     # -- descriptors ---------------------------------------------------------------------------------------------
+    def _img(self, w):
+        """tf32 split image of a GEMM weight (geob200_split_tf32): built once here instead of on every GEMM call"""
+        img = GF.split_tf32(w.detach())
+        self._keep.append(img)
+        return _ptr(img)
+
     def _lin(self, mlp):
-        return LinearT(_ptr(mlp.weight), _ptr(mlp.bias), mlp.in_features, mlp.out_features)
+        return LinearT(_ptr(mlp.weight), _ptr(mlp.bias), mlp.in_features, mlp.out_features, self._img(mlp.weight))
 
     def _norm(self, gn):
         return NormT(_ptr(gn.norm.weight), _ptr(gn.norm.bias))
@@ -73,7 +81,8 @@ class NativeModel:
         wt = w.reshape(-1, w.shape[2]).t().contiguous() if w.shape[1] % 32 == 0 else None
         if wt is not None:
             self._keep.append(wt)
-        return KPConvT(_ptr(w), _ptr(wt), _ptr(kp.bias), _ptr(kp.kernel_points), w.shape[1], w.shape[2], float(kp.sigma))
+        return KPConvT(_ptr(w), _ptr(wt), _ptr(kp.bias), _ptr(kp.kernel_points), w.shape[1], w.shape[2], float(kp.sigma),
+                       None if wt is None else self._img(wt))
 
     def _res(self, blk):
         r = ResBlockT()
@@ -122,15 +131,16 @@ class NativeModel:
                 wpt = mha.proj_p.weight.detach().t().contiguous()
                 self._keep += [wqkv, bqkv, wpt]
                 t.w_qkv, t.b_qkv, t.wp_t, t.bp = _ptr(wqkv), _ptr(bqkv), _ptr(wpt), _ptr(mha.proj_p.bias)
+                t.w_qkv_img = self._img(wqkv)
             else:
                 wkv, bkv = cat(('proj_k', 'proj_v'), 'weight'), cat(('proj_k', 'proj_v'), 'bias')
                 self._keep += [wkv, bkv]
                 t.w_q, t.b_q, t.w_kv, t.b_kv = _ptr(mha.proj_q.weight), _ptr(mha.proj_q.bias), _ptr(wkv), _ptr(bkv)
+                t.w_q_img, t.w_kv_img = self._img(mha.proj_q.weight), self._img(wkv)
             att, ffn = layer.attention, layer.output
-            t.att_linear = LinearT(_ptr(att.linear.weight), _ptr(att.linear.bias), att.linear.in_features, att.linear.out_features)
+            t.att_linear = self._lin(att.linear)
             t.att_norm = NormT(_ptr(att.norm.weight), _ptr(att.norm.bias))
-            t.expand = LinearT(_ptr(ffn.expand.weight), _ptr(ffn.expand.bias), ffn.expand.in_features, ffn.expand.out_features)
-            t.squeeze = LinearT(_ptr(ffn.squeeze.weight), _ptr(ffn.squeeze.bias), ffn.squeeze.in_features, ffn.squeeze.out_features)
+            t.expand, t.squeeze = self._lin(ffn.expand), self._lin(ffn.squeeze)
             t.out_norm = NormT(_ptr(ffn.norm.weight), _ptr(ffn.norm.bias))
             arr[i] = t
         return arr, len(tr.layers)

@@ -74,6 +74,11 @@ int geob200_kpconv_tc(const float* s_feats, const float* q_points, const float* 
                       const float* bias, int64_t c_in, int64_t c_out, float sigma, float* out, void* workspace, size_t workspace_bytes,
                       void* stream);
 
+/* tf32 split image of a row-major weight (n x k, row stride ld >= k), the operand layout of the tensor-core GEMM:
+ * out (2n x k, contiguous) = [hi; lo] with hi = w rounded to tf32 (nearest, ties away from zero; low 13 bits zero) and
+ * lo = w - hi in fp32. */
+int geob200_split_tf32(const float* w, int64_t ld, int64_t n, int64_t k, float* out, void* stream);
+
 /* 1 (default): Linears run on the tensor cores with 3xTF32 when the shape allows; 0: fp32 CUDA cores only */
 void geob200_set_linear_mode(int mode);
 int geob200_linear(const float* x, int64_t ldx, const float* weight, const float* bias, float* y, int64_t ldy, int64_t m,
@@ -381,10 +386,12 @@ int64_t geob200_linear_profile_read(int64_t capacity, int64_t* shapes, float* ms
  * instead of milliseconds.  All pointers are device pointers; the structs are plain C (built from a state_dict by
  * geotransformer_b200/native.py). */
 #define GEOB200_MAX_STAGES 6
-typedef struct { const float* weight; const float* bias; int64_t c_in, c_out; } geob200_linear_t;
+/* weight_img / weights_img / *_img: optional tf32 split images (geob200_split_tf32) of weight / weights_t / the fused
+ * projection weights, read by the tensor-core GEMM; NULL = split on every call. */
+typedef struct { const float* weight; const float* bias; int64_t c_in, c_out; const float* weight_img; } geob200_linear_t;
 typedef struct { const float* gamma; const float* beta; } geob200_norm_t;
 typedef struct { const float* weights; const float* weights_t; const float* bias; const float* kernel_points;
-                 int64_t c_in, c_out; float sigma; } geob200_kpconv_t;
+                 int64_t c_in, c_out; float sigma; const float* weights_img; } geob200_kpconv_t;
 /* ResidualBlock (reference geotransformer/modules/kpconv/modules.py:151-225) */
 typedef struct {
     int32_t has_unary1, has_shortcut, strided, reserved;
@@ -432,6 +439,7 @@ typedef struct {
     const float* wp_t; const float* bp;
     geob200_linear_t att_linear; geob200_norm_t att_norm;
     geob200_linear_t expand; geob200_linear_t squeeze; geob200_norm_t out_norm;
+    const float* w_qkv_img; const float* w_q_img; const float* w_kv_img;
 } geob200_tlayer_t;
 size_t geob200_transformer_workspace_bytes(int64_t n0, int64_t n1, int64_t channels, int64_t heads, int64_t num_layers);
 /* RPEConditionalTransformer.forward on stacked features x = [feats0; feats1] (after in_proj), sequential cross updates */
