@@ -13,8 +13,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'libgeob200.so')
 _lib = None
 
-c_void_p, c_int64, c_int32, c_float, c_size_t, c_int = (
-    ctypes.c_void_p, ctypes.c_int64, ctypes.c_int32, ctypes.c_float, ctypes.c_size_t, ctypes.c_int)
+c_void_p, c_int64, c_int32, c_float, c_double, c_size_t, c_int = (
+    ctypes.c_void_p, ctypes.c_int64, ctypes.c_int32, ctypes.c_float, ctypes.c_double, ctypes.c_size_t, ctypes.c_int)
 
 # name -> (restype, argtypes); kept in one table so tests can check it against include/geob200.h
 SIGNATURES = {}
@@ -24,7 +24,7 @@ def _sig(name, restype, *argtypes):
     SIGNATURES[name] = (restype, list(argtypes))
 
 
-P, I64, I32, F, SZ = c_void_p, c_int64, c_int32, c_float, c_size_t
+P, I64, I32, F, D, SZ = c_void_p, c_int64, c_int32, c_float, c_double, c_size_t
 _sig('geob200_last_error', ctypes.c_char_p)
 _sig('geob200_launch_count', ctypes.c_uint64)
 _sig('geob200_grid_subsample_workspace_bytes', SZ, I64, I64)
@@ -99,6 +99,10 @@ _sig('geob200_evaluate', c_int, P, P, I64, F, P, P, I64, P, P, I64, F, P, P, P, 
 _sig('geob200_evaluate_counts', c_int, P, P, I64, P, F, P, P, I64, P, P, P, I64, P, F, P, P, P, I64, c_int, F, F, F, P, P)
 _sig('geob200_evaluate_batched', c_int, P, P, P, F, P, P, I64, P, P, P, I64, P, F, P, P, I64, P, I64, P, P, c_int, F, F, F, P, I64,
      P)
+_sig('geob200_coarse_matching_loss_batched_workspace_bytes', SZ, I64, I64)
+_sig('geob200_coarse_matching_loss_batched', c_int, P, P, I64, I64, P, P, P, P, F, F, F, F, F, F, P, I64, P, SZ, P)
+_sig('geob200_fine_matching_loss_batched_workspace_bytes', SZ, I64, I64)
+_sig('geob200_fine_matching_loss_batched', c_int, P, P, P, P, P, P, I64, I64, I64, P, D, P, P, I64, P, SZ, P)
 
 _sig('geob200_linear_profile_enable', c_int, c_int)
 _sig('geob200_set_split_k', c_int, c_int)

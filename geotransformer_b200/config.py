@@ -32,6 +32,11 @@ def _base(seed=7351):
     c.fine_matching = Cfg(mutual=True, confidence_threshold=0.05, use_dustbin=False, use_global_score=False,
                           correspondence_threshold=3, correspondence_limit=None, num_refinement_steps=5)
     c.eval = Cfg(acceptance_overlap=0.0, inlier_ratio_threshold=0.05)
+    # validation losses (OverallLoss, experiments/*/config.py:127-143; ModelNet 132-148)
+    c.coarse_loss = Cfg(positive_margin=0.1, negative_margin=1.4, positive_optimal=0.1, negative_optimal=1.4, log_scale=24,
+                        positive_overlap=0.1)
+    c.fine_loss = Cfg(positive_radius=0.05)
+    c.loss = Cfg(weight_coarse_loss=1.0, weight_fine_loss=1.0)
     return c
 
 
@@ -53,6 +58,8 @@ def make_cfg(name='3dmatch'):
         c.geotransformer.update(input_dim=2048, hidden_dim=128, sigma_d=4.8)
         c.fine_matching.update(topk=2, acceptance_radius=0.6)
         c.eval.update(acceptance_radius=1.0, rre_threshold=5.0, rte_threshold=2.0)
+        c.coarse_loss.log_scale = 40
+        c.fine_loss.positive_radius = 0.6
         c.neighbor_limits = None  # calibrated (reference utils/data.py:192-217)
     elif name == 'modelnet':
         c.backbone.update(num_stages=3, init_voxel_size=0.05, base_radius=2.5)

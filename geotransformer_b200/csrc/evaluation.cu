@@ -308,6 +308,220 @@ __global__ void __launch_bounds__(1024) evaluate_kernel(const long long* __restr
     }
 }
 
+// ---------------------------------------------------------------------------------------------------- validation losses
+// OverallLoss (experiments/<exp>/loss.py:10-92, modules/loss/circle_loss.py:44-86) as the reference evaluates it in val_step:
+// values only, no gradients.  Every reduction runs in a fixed order (no atomics), so a pair gets the same bits alone and in a batch.
+
+// deterministic block reduction over 256 threads: warp tree, then warp 0..7 in order
+template <typename T, typename Op>
+__device__ __forceinline__ T block_reduce_256(T v, Op op, T* red) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v = op(v, __shfl_xor_sync(0xffffffffu, v, o));
+    __syncthreads();
+    if (lane == 0) red[warp] = v;
+    __syncthreads();
+    T s = red[0];
+    for (int w = 1; w < 8; ++w) s = op(s, red[w]);
+    return s;
+}
+
+// d[i][j] = sqrt(clamp(2 - 2 <f_i, g_j>, 0)) for every (ref i, src j) of pair p = blockIdx.y (ALL superpoints: the loss applies no
+// node mask), o[i][j] = 0.  One CTA per ref row, one warp per entry (lane-strided fmaf + warp_sum, as spm_scores_kernel).
+__global__ void __launch_bounds__(256) closs_dist_kernel(const float* __restrict__ fr, const float* __restrict__ fs, int C,
+                                                         const __grid_constant__ Segs R, const __grid_constant__ Segs Q,
+                                                         const __grid_constant__ Segs NN, float* __restrict__ d, float* __restrict__ o) {
+    extern __shared__ float a[];            // [C]
+    const int p = blockIdx.y, i = blockIdx.x;
+    const int M = R.count[p], N = Q.count[p];
+    if (i >= M) return;
+    fr += ((long long)R.start[p] + i) * C;
+    fs += (long long)Q.start[p] * C;
+    d += NN.start[p] + (long long)i * N;
+    o += NN.start[p] + (long long)i * N;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (int c = threadIdx.x; c < C; c += blockDim.x) a[c] = fr[c];
+    __syncthreads();
+    for (int j = warp; j < N; j += 8) {
+        const float* b = fs + (long long)j * C;
+        float x = 0.f;
+        for (int c = lane; c < C; c += 32) x = fmaf(a[c], b[c], x);
+        x = warp_sum(x);
+        if (lane == 0) {
+            d[j] = sqrtf(fmaxf(__fsub_rn(2.0f, __fmul_rn(2.0f, x)), 0.0f));
+            o[j] = 0.f;
+        }
+    }
+}
+
+// o[i][j] = overlap of the first count[p] ground-truth rows of pair p (rows at NN.start[p])
+__global__ void __launch_bounds__(256) closs_scatter_kernel(const long long* __restrict__ gt_idx, const float* __restrict__ gt_ov,
+                                                            const int* __restrict__ count, const __grid_constant__ Segs Q,
+                                                            const __grid_constant__ Segs NN, float* __restrict__ o) {
+    const int p = blockIdx.y;
+    const int g = blockIdx.x * blockDim.x + threadIdx.x;
+    const int n = min(count[p], NN.count[p]);
+    if (g >= n) return;
+    gt_idx += 2ll * NN.start[p]; gt_ov += NN.start[p];
+    o[NN.start[p] + gt_idx[2ll * g] * Q.count[p] + gt_idx[2ll * g + 1]] = gt_ov[g];
+}
+
+struct CircleParams {
+    float pos_margin, neg_margin, pos_optimal, neg_optimal, log_scale, pos_overlap;
+};
+
+// one CTA per row (blockIdx.z = 0: ref superpoint i over all j) or column (z = 1: src superpoint j over all i) of pair blockIdx.y:
+// both logsumexps (max subtracted first), loss = softplus(Lp + Ln) / log_scale and kept = (has a positive and a negative).
+// Weight-0 entries stay in the sums (exp(0) = 1), as in the reference.  Results at the row's / column's cloud offset.
+__global__ void __launch_bounds__(256) closs_lse_kernel(const float* __restrict__ d, const float* __restrict__ o,
+                                                        const __grid_constant__ Segs R, const __grid_constant__ Segs Q,
+                                                        const __grid_constant__ Segs NN, CircleParams cp, float* __restrict__ ell_r,
+                                                        unsigned char* __restrict__ kept_r, float* __restrict__ ell_c,
+                                                        unsigned char* __restrict__ kept_c) {
+    __shared__ float redf[8];
+    __shared__ int redi[8];
+    const int p = blockIdx.y, col = blockIdx.z;
+    const int M = R.count[p], N = Q.count[p];
+    const int line = blockIdx.x;
+    if (line >= (col ? N : M)) return;
+    const int len = col ? M : N;
+    const long long base = NN.start[p] + (col ? line : (long long)line * N);
+    const long long step = col ? N : 1;
+    auto logits = [&](int e, float& lp, float& ln, int& pos, int& neg) {
+        const float dv = d[base + e * step], ov = o[base + e * step];
+        pos = ov > cp.pos_overlap;
+        neg = ov == 0.f;
+        const float wp = pos ? __fmul_rn(fmaxf(__fsub_rn(dv, cp.pos_optimal), 0.f), sqrtf(ov)) : 0.f;
+        const float wn = neg ? fmaxf(__fsub_rn(cp.neg_optimal, dv), 0.f) : 0.f;
+        lp = __fmul_rn(__fmul_rn(cp.log_scale, __fsub_rn(dv, cp.pos_margin)), wp);
+        ln = __fmul_rn(__fmul_rn(cp.log_scale, __fsub_rn(cp.neg_margin, dv)), wn);
+    };
+    float mp = -INFINITY, mn = -INFINITY;
+    int np_ = 0, nn_ = 0;
+    for (int e = threadIdx.x; e < len; e += blockDim.x) {
+        float lp, ln;
+        int pos, neg;
+        logits(e, lp, ln, pos, neg);
+        mp = fmaxf(mp, lp); mn = fmaxf(mn, ln);
+        np_ |= pos; nn_ |= neg;
+    }
+    auto fmax_op = [](float x, float y) { return fmaxf(x, y); };
+    auto fadd_op = [](float x, float y) { return x + y; };
+    auto ior_op = [](int x, int y) { return x | y; };
+    mp = block_reduce_256(mp, fmax_op, redf);
+    mn = block_reduce_256(mn, fmax_op, redf);
+    const int has = block_reduce_256(np_ | (nn_ << 1), ior_op, redi);
+    float sp = 0.f, sn = 0.f;
+    for (int e = threadIdx.x; e < len; e += blockDim.x) {
+        float lp, ln;
+        int pos, neg;
+        logits(e, lp, ln, pos, neg);
+        sp += expf(lp - mp);
+        sn += expf(ln - mn);
+    }
+    sp = block_reduce_256(sp, fadd_op, redf);
+    sn = block_reduce_256(sn, fadd_op, redf);
+    if (threadIdx.x == 0) {
+        const float x = (mp + logf(sp)) + (mn + logf(sn));
+        const float sp1 = x > 20.f ? x : log1pf(expf(x));            // torch softplus: linear above threshold 20
+        const float l = sp1 / cp.log_scale;
+        const long long r = (col ? Q.start[p] : R.start[p]) + line;
+        (col ? ell_c : ell_r)[r] = l;
+        (col ? kept_c : kept_r)[r] = has == 3;
+    }
+}
+
+// one warp per pair: c_loss = (mean of the kept rows + mean of the kept columns) / 2 (NaN for an empty selection) -> out[p * ld + 1]
+__global__ void __launch_bounds__(32) closs_finalize_kernel(const float* __restrict__ ell_r, const unsigned char* __restrict__ kept_r,
+                                                            const float* __restrict__ ell_c, const unsigned char* __restrict__ kept_c,
+                                                            const __grid_constant__ Segs R, const __grid_constant__ Segs Q,
+                                                            float* __restrict__ out, long long ld) {
+    const int p = blockIdx.x, lane = threadIdx.x;
+    double m[2];
+    for (int side = 0; side < 2; ++side) {
+        const float* ell = side ? ell_c : ell_r;
+        const unsigned char* kept = side ? kept_c : kept_r;
+        const int s0 = side ? Q.start[p] : R.start[p], n = side ? Q.count[p] : R.count[p];
+        double s = 0.0, k = 0.0;
+        for (int i = lane; i < n; i += 32)
+            if (kept[s0 + i]) { s += ell[s0 + i]; k += 1.0; }
+        s = warp_sum_d(s);
+        k = warp_sum_d(k);
+        m[side] = (float)(s / k);              // 0 / 0 = NaN: the mean of an empty selection
+    }
+    if (lane == 0) out[p * ld + 1] = __fdiv_rn(__fadd_rn((float)m[0], (float)m[1]), 2.0f);
+}
+
+// FineMatchingLoss, one CTA per patch q of pair p = blockIdx.y (patch rows at p * P + q): ground-truth labels of the (K+1)^2
+// Sinkhorn block (point pairs closer than the radius after the gt transform, slack row / column for unmatched valid points);
+// partial[p * P + q] = (sum of the labelled scores, #labels).  Scores are read only where a label is set.
+template <int K>
+__global__ void __launch_bounds__(256) floss_patch_kernel(const float* __restrict__ ref_pts, const float* __restrict__ src_pts,
+                                                          const unsigned char* __restrict__ ref_masks,
+                                                          const unsigned char* __restrict__ src_masks, const float* __restrict__ scores,
+                                                          const float* __restrict__ T, int P, const int* __restrict__ count, float r2,
+                                                          double* __restrict__ psum, int* __restrict__ pcnt) {
+    __shared__ float4 rp[K], sp[K];              // (x, y, z, |p|^2), w < 0 = invalid point
+    __shared__ int rhit[K], shit[K];
+    __shared__ double redd[8];
+    __shared__ int redi[8];
+    __shared__ float Tm[16];
+    const int p = blockIdx.y, q = blockIdx.x;
+    const long long patch = (long long)p * P + q;
+    const bool live = count == nullptr || q < count[p];
+    if (threadIdx.x < 16) Tm[threadIdx.x] = T[16 * p + threadIdx.x];
+    __syncthreads();
+    for (int i = threadIdx.x; i < K; i += blockDim.x) {
+        const float* a = ref_pts + (patch * K + i) * 3;
+        const float* b = src_pts + (patch * K + i) * 3;
+        const bool ra = live && ref_masks[patch * K + i], sa = live && src_masks[patch * K + i];
+        float x, y, z;
+        xform(Tm, b[0], b[1], b[2], x, y, z);
+        rp[i] = make_float4(a[0], a[1], a[2], ra ? sqn3(a[0], a[1], a[2]) : -1.f);
+        sp[i] = make_float4(x, y, z, sa ? sqn3(x, y, z) : -1.f);
+        rhit[i] = 0;
+        shit[i] = 0;
+    }
+    __syncthreads();
+    const float* S = scores + patch * (K + 1) * (K + 1);
+    double s = 0.0;
+    int n = 0;
+    for (int e = threadIdx.x; e < K * K; e += blockDim.x) {
+        const int i = e / K, j = e % K;
+        const float4 a = rp[i], b = sp[j];
+        if (a.w >= 0.f && b.w >= 0.f && sqd_mm(a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w) < r2) {
+            rhit[i] = 1;
+            shit[j] = 1;
+            s += S[i * (K + 1) + j];
+            ++n;
+        }
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < K; i += blockDim.x) {
+        if (rp[i].w >= 0.f && !rhit[i]) { s += S[i * (K + 1) + K]; ++n; }
+        if (sp[i].w >= 0.f && !shit[i]) { s += S[K * (K + 1) + i]; ++n; }
+    }
+    s = block_reduce_256(s, [](double x, double y) { return x + y; }, redd);
+    n = block_reduce_256(n, [](int x, int y) { return x + y; }, redi);
+    if (threadIdx.x == 0) { psum[patch] = s; pcnt[patch] = n; }
+}
+
+// one warp per pair: f_loss = -(sum of the labelled scores / #labels) over all patches of the pair -> out[p * ld + 2]; with weights
+// also loss = w_c * out[p * ld + 1] + w_f * f_loss -> out[p * ld + 0]
+__global__ void __launch_bounds__(32) floss_finalize_kernel(const double* __restrict__ psum, const int* __restrict__ pcnt, int P,
+                                                            int with_total, float w_c, float w_f, float* __restrict__ out, long long ld) {
+    const int p = blockIdx.x, lane = threadIdx.x;
+    double s = 0.0, k = 0.0;
+    for (int q = lane; q < P; q += 32) { s += psum[(long long)p * P + q]; k += pcnt[(long long)p * P + q]; }
+    s = warp_sum_d(s);
+    k = warp_sum_d(k);
+    if (lane == 0) {
+        const float f = -(float)(s / k);
+        out[p * ld + 2] = f;
+        if (with_total) out[p * ld] = __fadd_rn(__fmul_rn(w_c, out[p * ld + 1]), __fmul_rn(w_f, f));
+    }
+}
+
 }  // namespace geob200
 
 using namespace geob200;
@@ -456,6 +670,99 @@ int geob200_evaluate_batched(const int64_t* gt_node_corr_indices, const float* g
                          src_node_corr_indices, n_node_corr, n_node_corr_dev, ref_corr_points, src_corr_points, n_corr, n_corr_dev,
                          acceptance_radius, gt_transforms, est_transforms, transform_ld, points, segs_range(pt, B, B), mode, rmse_threshold,
                          rre_threshold, rte_threshold, metrics, metrics_ld, (cudaStream_t)stream);
+}
+
+size_t geob200_coarse_matching_loss_batched_workspace_bytes(int64_t n_rows, int64_t n_products) {
+    const size_t r = (size_t)n_rows, nn = (size_t)n_products;
+    return 2 * align_up(4 * nn, 256) + align_up(4 * r, 256) + align_up(r, 256) + 256;
+}
+
+int geob200_coarse_matching_loss_batched(const float* ref_feats, const float* src_feats, int64_t channels, int64_t n_pairs,
+                                         const int64_t* cloud_nodes, const int64_t* gt_node_corr_indices, const float* gt_node_corr_overlaps,
+                                         const int32_t* gt_count, float positive_margin, float negative_margin, float positive_optimal,
+                                         float negative_optimal, float log_scale, float positive_overlap, float* out, int64_t out_ld,
+                                         void* workspace, size_t workspace_bytes, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    GEOB_REQUIRE(n_pairs > 0 && 2 * n_pairs <= GEOB_MAX_CLOUDS, "coarse_matching_loss_batched: 1..%d pairs", GEOB_MAX_CLOUDS / 2);
+    GEOB_REQUIRE(channels > 0 && channels <= 8192, "coarse_matching_loss_batched: 1..8192 channels");
+    GEOB_REQUIRE(log_scale > 0.f, "coarse_matching_loss_batched: log_scale must be positive");
+    GEOB_REQUIRE(out_ld >= 3, "coarse_matching_loss_batched: out_ld >= 3 required");
+    GEOB_REQUIRE(gt_count != nullptr, "coarse_matching_loss_batched: gt_count (device int32, one per pair) is required");
+    for (int64_t c = 0; c < 2 * n_pairs; ++c) GEOB_REQUIRE(cloud_nodes[c] >= 0, "coarse_matching_loss_batched: negative node count");
+    const int B = (int)n_pairs;
+    Segs R, Q, NN;
+    if (segs_from_counts(&R, B, cloud_nodes) || segs_from_counts(&Q, B, cloud_nodes + B) || segs_products(&NN, R, Q)) return -1;
+    const int64_t rows = (int64_t)R.start[B - 1] + R.count[B - 1] + Q.start[B - 1] + Q.count[B - 1];
+    const int64_t nn = (int64_t)NN.start[B - 1] + NN.count[B - 1];
+    GEOB_REQUIRE(workspace_bytes >= geob200_coarse_matching_loss_batched_workspace_bytes(rows, nn),
+                 "coarse_matching_loss_batched: workspace too small");
+    Arena ar(workspace, workspace_bytes);
+    float* d = ar.take<float>(nn);
+    float* o = ar.take<float>(nn);
+    float* ell = ar.take<float>(rows);
+    unsigned char* kept = ar.take<unsigned char>(rows);
+    GEOB_REQUIRE(ar.ok(), "coarse_matching_loss_batched: workspace accounting error");
+    float* ell_c = ell + R.start[B - 1] + R.count[B - 1];
+    unsigned char* kept_c = kept + R.start[B - 1] + R.count[B - 1];
+    const CircleParams cp{positive_margin, negative_margin, positive_optimal, negative_optimal, log_scale, positive_overlap};
+    int n_launch = 1;
+    if (R.max > 0 && Q.max > 0) {
+        closs_dist_kernel<<<dim3((unsigned)R.max, B), 256, channels * sizeof(float), st>>>(ref_feats, src_feats, (int)channels, R, Q, NN, d, o);
+        closs_scatter_kernel<<<dim3((unsigned)((NN.max + 255) / 256), B), 256, 0, st>>>((const long long*)gt_node_corr_indices,
+                                                                                        gt_node_corr_overlaps, gt_count, Q, NN, o);
+        n_launch += 2;
+    }
+    if (R.max > 0 || Q.max > 0) {
+        closs_lse_kernel<<<dim3((unsigned)(R.max > Q.max ? R.max : Q.max), B, 2), 256, 0, st>>>(d, o, R, Q, NN, cp, ell, kept, ell_c, kept_c);
+        n_launch += 1;
+    }
+    closs_finalize_kernel<<<B, 32, 0, st>>>(ell, kept, ell_c, kept_c, R, Q, out, (long long)out_ld);
+    GEOB_CHECK_LAUNCH();
+    count_launches(n_launch);
+    return 0;
+}
+
+size_t geob200_fine_matching_loss_batched_workspace_bytes(int64_t n_pairs, int64_t n_patches) {
+    const size_t n = (size_t)n_pairs * (size_t)n_patches;
+    return align_up(8 * n, 256) + align_up(4 * n, 256) + 256;
+}
+
+int geob200_fine_matching_loss_batched(const float* ref_knn_points, const float* src_knn_points, const uint8_t* ref_knn_masks,
+                                       const uint8_t* src_knn_masks, const float* matching_scores, const float* transforms, int64_t n_pairs,
+                                       int64_t n_patches, int64_t k, const int32_t* patch_count, double positive_radius,
+                                       const float* loss_weights, float* out, int64_t out_ld, void* workspace, size_t workspace_bytes,
+                                       void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    GEOB_REQUIRE(n_pairs > 0 && n_pairs <= 65535, "fine_matching_loss_batched: 1..65535 pairs");
+    GEOB_REQUIRE(n_patches >= 0 && n_patches < (1 << 30), "fine_matching_loss_batched: negative patch count");
+    GEOB_REQUIRE(k == 64 || k == 128, "fine_matching_loss_batched: k must be 64 or 128, got %lld", (long long)k);
+    GEOB_REQUIRE(positive_radius > 0.0, "fine_matching_loss_batched: positive_radius must be positive");
+    GEOB_REQUIRE(out_ld >= 3, "fine_matching_loss_batched: out_ld >= 3 required");
+    GEOB_REQUIRE(workspace_bytes >= geob200_fine_matching_loss_batched_workspace_bytes(n_pairs, n_patches),
+                 "fine_matching_loss_batched: workspace too small");
+    Arena ar(workspace, workspace_bytes);
+    double* psum = ar.take<double>((size_t)n_pairs * n_patches);
+    int* pcnt = ar.take<int>((size_t)n_pairs * n_patches);
+    GEOB_REQUIRE(ar.ok(), "fine_matching_loss_batched: workspace accounting error");
+    const float r2 = (float)(positive_radius * positive_radius);      // radius ** 2 in double, rounded once (torch.lt against it)
+    const int P = (int)n_patches;
+    float w_c = 0.f, w_f = 0.f;
+    if (loss_weights != nullptr) { w_c = loss_weights[0]; w_f = loss_weights[1]; }
+    int n_launch = 1;
+    if (P > 0) {
+        const dim3 grid((unsigned)P, (unsigned)n_pairs);
+        if (k == 64)
+            floss_patch_kernel<64><<<grid, 256, 0, st>>>(ref_knn_points, src_knn_points, ref_knn_masks, src_knn_masks, matching_scores,
+                                                         transforms, P, patch_count, r2, psum, pcnt);
+        else
+            floss_patch_kernel<128><<<grid, 256, 0, st>>>(ref_knn_points, src_knn_points, ref_knn_masks, src_knn_masks, matching_scores,
+                                                          transforms, P, patch_count, r2, psum, pcnt);
+        n_launch += 1;
+    }
+    floss_finalize_kernel<<<(unsigned)n_pairs, 32, 0, st>>>(psum, pcnt, P, loss_weights != nullptr, w_c, w_f, out, (long long)out_ld);
+    GEOB_CHECK_LAUNCH();
+    count_launches(n_launch);
+    return 0;
 }
 
 }  // extern "C"

@@ -15,6 +15,8 @@ import torch
 from . import _lib
 from .utils.data import registration_collate_fn_stack_mode
 
+LOSS_KEYS = ('loss', 'c_loss', 'f_loss')
+
 
 def pin_host_threads_to_gpu(device):
     """Restrict the calling thread (and the threads it creates afterwards) to the CPUs NVML reports as local to `device`
@@ -39,13 +41,15 @@ def pin_host_threads_to_gpu(device):
 
 class RegistrationEngine:
     def __init__(self, model, cfg, neighbor_limits, num_streams=4, device=None, native=True, evaluator=None, pin_cpu=False,
-                 batch_size=1, side_streams=4):
+                 batch_size=1, side_streams=4, loss_func=None):
         """pin_cpu: bind the calling thread and the worker threads to the CPUs local to the GPU (pin_host_threads_to_gpu).
         evaluator: optional geotransformer_b200.loss.Evaluator; its metrics (PIR, IR, RRE, RTE, RMSE, RR) are then computed
         on the device for every pair and travel back with the transform in the same D2H copy.
         batch_size > 1: every worker registers ``batch_size`` pairs per forward (GeoTransformer.forward_batch: one collate,
         one backbone / transformer pass over the stacked rows of all pairs, per-pair stages on ``side_streams`` extra
-        streams), with ONE host synchronisation per batch besides the collate's size read-backs."""
+        streams), with ONE host synchronisation per batch besides the collate's size read-backs.
+        loss_func: optional geotransformer_b200.loss.OverallLoss; every result then gains 'loss': {'loss', 'c_loss', 'f_loss'}
+        (the reference's val_step losses), computed on the device and read back with the same event."""
         self.model, self.cfg, self.limits = model, cfg, neighbor_limits
         if native and not hasattr(model, '_native'):
             from .model import enable_native
@@ -54,6 +58,7 @@ class RegistrationEngine:
         self.num_streams = num_streams
         self.pinned_cpu = pin_host_threads_to_gpu(self.device) if pin_cpu else False
         self.evaluator = evaluator
+        self.loss_func = loss_func
         self.stage_times = None          # set to {} to collect per-stage CUDA-event times (profiling; adds ~7 events per pair)
         self.streams = [torch.cuda.Stream(self.device) for _ in range(num_streams)]
         self.pool = ThreadPoolExecutor(max_workers=num_streams)
@@ -64,6 +69,9 @@ class RegistrationEngine:
         bs = self.batch_size
         self.r_dev = [torch.zeros((24,) if bs == 1 else (bs, 24), dtype=torch.float32, device=self.device) for _ in range(num_streams)]
         self.r_host = [torch.zeros((24,) if bs == 1 else (bs, 24), dtype=torch.float32).pin_memory() for _ in range(num_streams)]
+        # per slot: [loss, c_loss, f_loss] rows on the device and pinned on the host (only with a loss function)
+        self.l_dev = [torch.zeros((3,) if bs == 1 else (bs, 3), dtype=torch.float32, device=self.device) for _ in range(num_streams)]
+        self.l_host = [torch.zeros((3,) if bs == 1 else (bs, 3), dtype=torch.float32).pin_memory() for _ in range(num_streams)]
         self.sides = [[torch.cuda.Stream(self.device) for _ in range(side_streams)] if bs > 1 else [] for _ in range(num_streams)]
 
     def _one(self, slot, pair, keep):
@@ -85,6 +93,9 @@ class RegistrationEngine:
         if self.evaluator is not None:
             self.evaluator.metrics_tensor(out, data, out=r_dev[16:])
         r_host.copy_(r_dev, non_blocking=True)
+        if self.loss_func is not None:
+            self.loss_func.loss_tensor(out, data, out=self.l_dev[slot])
+            self.l_host[slot].copy_(self.l_dev[slot], non_blocking=True)
         done = torch.cuda.Event()
         done.record(stream)
         done.synchronize()                      # this thread only; the other streams keep running
@@ -96,6 +107,8 @@ class RegistrationEngine:
         if self.evaluator is not None:
             m = r_host[16:].tolist()
             res['metrics'] = dict(zip(('PIR', 'IR', 'RRE', 'RTE', 'RMSE', 'RR'), m[:6]))
+        if self.loss_func is not None:
+            res['loss'] = dict(zip(LOSS_KEYS, self.l_host[slot].tolist()))
         if keep:
             res['output_dict'] = out
         return res, done
@@ -115,11 +128,14 @@ class RegistrationEngine:
         if marks is not None:
             data['_stage_events'] = marks
         r_dev, r_host = self.r_dev[slot][:n], self.r_host[slot][:n]
+        l_dev, l_host, lf = self.l_dev[slot][:n], self.l_host[slot][:n], self.loss_func
         if n == 1:             # a trailing single pair: the one-pair forward
             out = self.model(data)
             r_dev[0, :16].copy_(out['estimated_transform'].reshape(16))
             if self.evaluator is not None:
                 self.evaluator.metrics_tensor(out, data, out=r_dev[0, 16:])
+            if lf is not None:
+                lf.loss_tensor(out, data, out=l_dev[0])
             outs = [out]
         elif keep:             # trimmed per-pair output dicts (one extra host sync for the counts), metrics from them
             outs = self.model.forward_batch(data, side_streams=self.sides[slot])
@@ -127,9 +143,14 @@ class RegistrationEngine:
                 r_dev[p, :16].copy_(o['estimated_transform'].reshape(16))
                 if self.evaluator is not None:
                     self.evaluator.metrics_tensor(o, {'transform': data['transform'][p]}, out=r_dev[p, 16:])
+                if lf is not None:
+                    lf.loss_tensor(o, {'transform': data['transform'][p]}, out=l_dev[p])
         else:
-            outs = self.model.forward_batch(data, evaluator=self.evaluator, results=r_dev, side_streams=self.sides[slot], keep_outputs=False)
+            outs = self.model.forward_batch(data, evaluator=self.evaluator, results=r_dev, side_streams=self.sides[slot], keep_outputs=False,
+                                            loss_func=lf, loss_out=l_dev)
         r_host.copy_(r_dev, non_blocking=True)
+        if lf is not None:
+            l_host.copy_(l_dev, non_blocking=True)
         done = torch.cuda.Event()
         done.record(stream)
         done.synchronize()
@@ -147,6 +168,8 @@ class RegistrationEngine:
                 r['num_corr'] = int(m[6])
             elif n == 1:
                 r['num_corr'] = int(outs[0]['ref_corr_points'].shape[0])
+            if lf is not None:
+                r['loss'] = dict(zip(LOSS_KEYS, l_host[p].tolist()))
             if keep:
                 r['output_dict'] = outs[p]
             res.append(r)

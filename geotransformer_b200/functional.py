@@ -861,3 +861,95 @@ def evaluate_batched(gt_indices, gt_overlaps, n_gt, corr_indices, n_node_corr, r
         est_transforms.stride(0), points.data_ptr(), B, _host_i64(cloud_nodes), _host_i64(cloud_points), int(mode), float(rmse_threshold),
         float(rre_threshold), float(rte_threshold), out.data_ptr(), out.stride(0), L.stream_ptr()), 'evaluate_batched')
     return out
+
+
+# ------------------------------------------------------------------------------------------------ validation losses
+# OverallLoss values (reference experiments/<exp>/loss.py:10-92) without gradients.  ``out``: (B, >= 3 columns, any row stride)
+# rows [loss, c_loss, f_loss]; the coarse call writes column 1, the fine call column 2 and, given ``loss_weights``, column 0 from
+# column 1 -- so run the fine call after the coarse one on the same stream.  Counts are optional DEVICE int32 tensors: no read-back.
+
+def _loss_rows(out, B, dev):
+    if out is None:
+        out = torch.empty((B, 3), dtype=_f32, device=dev)
+    view = out.reshape(1, -1) if out.ndim == 1 else out
+    if view.shape[0] != B or view.shape[1] < 3 or view.stride(1) != 1 or view.dtype != _f32 or not view.is_cuda:
+        raise RuntimeError(f'loss out must be a float32 CUDA tensor of {B} rows with >= 3 contiguous columns')
+    return out, view
+
+
+def coarse_matching_loss_batched(ref_feats, src_feats, cloud_nodes, gt_indices, gt_overlaps, gt_count, positive_margin, negative_margin,
+                                 positive_optimal, negative_optimal, log_scale, positive_overlap, out=None):
+    """CoarseMatchingLoss of B pairs: pair p's superpoints at rows sum_{q<p} n_ref(q) of ``ref_feats`` / sum_{q<p} n_src(q) of
+    ``src_feats`` (``cloud_nodes``: 2B host counts, ref clouds first), its ground-truth rows at sum_{q<p} n_ref(q) * n_src(q) of
+    ``gt_indices`` / ``gt_overlaps`` with ``gt_count[p]`` (device int32) valid.  Writes column 1 of ``out``."""
+    _f(ref_feats, 'ref_feats'); _f(src_feats, 'src_feats'); _f(gt_overlaps, 'gt_node_corr_overlaps')
+    L.require_cuda(gt_indices, 'gt_node_corr_indices', _i64); L.require_cuda(gt_count, 'gt_count', _i32)
+    B = len(cloud_nodes) // 2
+    dev = ref_feats.device
+    out, view = _loss_rows(out, B, dev)
+    rows = sum(int(c) for c in cloud_nodes)
+    nn = sum(int(cloud_nodes[p]) * int(cloud_nodes[B + p]) for p in range(B))
+    lib = L.lib()
+    ws = L.workspace(lib.geob200_coarse_matching_loss_batched_workspace_bytes(rows, nn), dev, tag='coarse_loss')
+    L.check(lib.geob200_coarse_matching_loss_batched(
+        ref_feats.data_ptr(), src_feats.data_ptr(), ref_feats.shape[1], B, _host_i64(cloud_nodes), gt_indices.data_ptr(),
+        gt_overlaps.data_ptr(), gt_count.data_ptr(), float(positive_margin), float(negative_margin), float(positive_optimal),
+        float(negative_optimal), float(log_scale), float(positive_overlap), view.data_ptr(), view.stride(0), ws.data_ptr(), ws.numel(),
+        L.stream_ptr()), 'coarse_matching_loss_batched')
+    return out
+
+
+def fine_matching_loss_batched(n_pairs, ref_knn_points, src_knn_points, ref_knn_masks, src_knn_masks, matching_scores, transforms,
+                               positive_radius, patch_count=None, loss_weights=None, out=None):
+    """FineMatchingLoss of B pairs: patch q of pair p at row p * P + q of the (B * P, k, 3) points, (B * P, k) masks and
+    (B * P, k+1, k+1) Sinkhorn scores; ``transforms`` (B, 4, 4); ``patch_count`` (B,) device int32 or None (all P).  Writes column 2
+    of ``out``; with ``loss_weights`` = (w_coarse, w_fine) also column 0 from column 1."""
+    for t, name in ((ref_knn_points, 'ref_node_corr_knn_points'), (src_knn_points, 'src_node_corr_knn_points'),
+                    (matching_scores, 'matching_scores'), (transforms, 'transform')):
+        _f(t, name)
+    L.require_cuda(ref_knn_masks, 'ref_node_corr_knn_masks', torch.bool); L.require_cuda(src_knn_masks, 'src_node_corr_knn_masks', torch.bool)
+    if patch_count is not None:
+        L.require_cuda(patch_count, 'patch_count', _i32)
+    B = int(n_pairs)
+    rows, k = ref_knn_masks.shape
+    dev = matching_scores.device
+    out, view = _loss_rows(out, B, dev)
+    lib = L.lib()
+    ws = L.workspace(lib.geob200_fine_matching_loss_batched_workspace_bytes(B, rows // B), dev, tag='fine_loss')
+    w = None if loss_weights is None else (ctypes.c_float * 2)(float(loss_weights[0]), float(loss_weights[1]))
+    L.check(lib.geob200_fine_matching_loss_batched(
+        ref_knn_points.data_ptr(), src_knn_points.data_ptr(), ref_knn_masks.data_ptr(), src_knn_masks.data_ptr(),
+        matching_scores.data_ptr(), transforms.data_ptr(), B, rows // B, k, L.ptr(patch_count), float(positive_radius), w,
+        view.data_ptr(), view.stride(0), ws.data_ptr(), ws.numel(), L.stream_ptr()), 'fine_matching_loss_batched')
+    return out
+
+
+def _one_count(n, count, dev):
+    return count.reshape(1) if count is not None else torch.full((1,), int(n), dtype=_i32, device=dev)
+
+
+def coarse_matching_loss(ref_feats, src_feats, gt_node_corr_indices, gt_node_corr_overlaps, positive_margin, negative_margin,
+                         positive_optimal, negative_optimal, log_scale, positive_overlap, out=None, n_gt=None):
+    """CoarseMatchingLoss of one pair (the batched kernels with B = 1); ``out``: (>= 3,) row, column 1 written.
+    ``n_gt``: optional device int32 count of valid ground-truth rows (full-capacity buffers)."""
+    dev = ref_feats.device
+    if out is None:
+        out = torch.empty((3,), dtype=_f32, device=dev)
+    cnt = _one_count(gt_node_corr_indices.shape[0], n_gt, dev)
+    coarse_matching_loss_batched(ref_feats, src_feats, [ref_feats.shape[0], src_feats.shape[0]], gt_node_corr_indices,
+                                 gt_node_corr_overlaps, cnt, positive_margin, negative_margin, positive_optimal, negative_optimal,
+                                 log_scale, positive_overlap, out=out)
+    return out
+
+
+def fine_matching_loss(ref_knn_points, src_knn_points, ref_knn_masks, src_knn_masks, matching_scores, transform, positive_radius,
+                       loss_weights=None, out=None, n_patches=None):
+    """FineMatchingLoss of one pair; ``out``: (>= 3,) row, column 2 (and column 0 given ``loss_weights``) written.
+    ``n_patches``: optional device int32 count of valid patches (full-capacity buffers)."""
+    dev = matching_scores.device
+    if out is None:
+        out = torch.empty((3,), dtype=_f32, device=dev)
+    fine_matching_loss_batched(1, ref_knn_points, src_knn_points, ref_knn_masks, src_knn_masks, matching_scores, transform,
+                               positive_radius, patch_count=None if n_patches is None else n_patches.reshape(1),
+                               loss_weights=loss_weights, out=out)
+    return out

@@ -1,8 +1,12 @@
-"""Evaluator (reference ``experiments/<exp>/loss.py:95-159``): PIR, IR, RRE, RTE, RMSE, RR of one registered pair.
+"""Evaluator (reference ``experiments/<exp>/loss.py:95-159``): PIR, IR, RRE, RTE, RMSE, RR of one registered pair; and the
+validation losses CoarseMatchingLoss / FineMatchingLoss / OverallLoss (``loss.py:10-92``).
 
 Same constructor/forward contract as the reference's three Evaluator classes (3DMatch, KITTI, ModelNet differ in how
 RMSE and RR are defined; ``cfg.name`` selects).  All six numbers come from ONE kernel launch (`geob200_evaluate`); the
 result dict holds 0-dim device tensors like the reference's.  KITTI has no RMSE entry (loss.py:140-151 there).
+
+The losses are the values the reference's ``val_step`` reports on the eval-mode forward.  They carry NO autograd graph:
+backward is not provided (training stays out of scope).  There is no CPU path: non-CUDA inputs raise RuntimeError.
 """
 import torch
 import torch.nn as nn
@@ -37,3 +41,89 @@ class Evaluator(nn.Module):
         if self.mode == 1:
             del res['RMSE']
         return res
+
+
+def _counts(output_dict):
+    """device counts of the valid rows when the output dict holds full-capacity buffers (forward_batch without a host sync)"""
+    return output_dict.get('_counts') or {}
+
+
+class CoarseMatchingLoss(nn.Module):
+    """Weighted circle loss over all superpoint pairs (reference loss.py:10-40); forward returns a 0-dim device tensor."""
+
+    def __init__(self, cfg):
+        super().__init__()
+        c = cfg.coarse_loss
+        self.positive_margin, self.negative_margin = c.positive_margin, c.negative_margin
+        self.positive_optimal, self.negative_optimal = c.positive_optimal, c.negative_optimal
+        self.log_scale, self.positive_overlap = c.log_scale, c.positive_overlap
+
+    def params(self):
+        return (self.positive_margin, self.negative_margin, self.positive_optimal, self.negative_optimal, self.log_scale,
+                self.positive_overlap)
+
+    @torch.no_grad()
+    def write(self, output_dict, out):
+        """c_loss into column 1 of the (>= 3,) device row ``out``"""
+        return GF.coarse_matching_loss(output_dict['ref_feats_c'], output_dict['src_feats_c'], output_dict['gt_node_corr_indices'],
+                                       output_dict['gt_node_corr_overlaps'], *self.params(), out=out, n_gt=_counts(output_dict).get('gt'))
+
+    def forward(self, output_dict):
+        return self.write(output_dict, None)[1]
+
+
+class FineMatchingLoss(nn.Module):
+    """Negative mean Sinkhorn score of the ground-truth labels of all patches (reference loss.py:43-71); 0-dim device tensor."""
+
+    def __init__(self, cfg):
+        super().__init__()
+        self.positive_radius = cfg.fine_loss.positive_radius
+
+    @torch.no_grad()
+    def write(self, output_dict, data_dict, out, loss_weights=None):
+        """f_loss into column 2 of ``out``; with ``loss_weights`` also the weighted total into column 0 (from column 1)"""
+        return GF.fine_matching_loss(output_dict['ref_node_corr_knn_points'], output_dict['src_node_corr_knn_points'],
+                                     output_dict['ref_node_corr_knn_masks'], output_dict['src_node_corr_knn_masks'],
+                                     output_dict['matching_scores'], data_dict['transform'], self.positive_radius,
+                                     loss_weights=loss_weights, out=out, n_patches=_counts(output_dict).get('node_corr'))
+
+    def forward(self, output_dict, data_dict):
+        return self.write(output_dict, data_dict, None)[2]
+
+
+class OverallLoss(nn.Module):
+    """weight_coarse_loss * c_loss + weight_fine_loss * f_loss (reference loss.py:74-92): {'loss', 'c_loss', 'f_loss'} as 0-dim
+    device tensors.  Values only: no gradients."""
+
+    def __init__(self, cfg):
+        super().__init__()
+        self.coarse_loss = CoarseMatchingLoss(cfg)
+        self.fine_loss = FineMatchingLoss(cfg)
+        self.weight_coarse_loss = cfg.loss.weight_coarse_loss
+        self.weight_fine_loss = cfg.loss.weight_fine_loss
+
+    @torch.no_grad()
+    def loss_tensor(self, output_dict, data_dict, out=None):
+        """(3,) device tensor [loss, c_loss, f_loss] -- no host sync"""
+        if out is None:
+            out = torch.empty((3,), dtype=torch.float32, device=output_dict['matching_scores'].device)
+        self.coarse_loss.write(output_dict, out)
+        self.fine_loss.write(output_dict, data_dict, out, loss_weights=(self.weight_coarse_loss, self.weight_fine_loss))
+        return out
+
+    @torch.no_grad()
+    def write_batched(self, feats_c, cloud_nodes, gt, ref_knn_points, src_knn_points, ref_knn_masks, src_knn_masks, scores,
+                      transforms, patch_count, out):
+        """rows [loss, c_loss, f_loss] of all pairs of a batched forward (GeoTransformer.forward_batch) into ``out`` (B, >= 3)"""
+        B = len(cloud_nodes) // 2
+        n_ref = sum(int(c) for c in cloud_nodes[:B])
+        c = self.coarse_loss
+        GF.coarse_matching_loss_batched(feats_c, feats_c[n_ref:], cloud_nodes, gt[0], gt[1], gt[2], *c.params(), out=out)
+        GF.fine_matching_loss_batched(B, ref_knn_points, src_knn_points, ref_knn_masks, src_knn_masks, scores, transforms,
+                                      self.fine_loss.positive_radius, patch_count=patch_count,
+                                      loss_weights=(self.weight_coarse_loss, self.weight_fine_loss), out=out)
+        return out
+
+    def forward(self, output_dict, data_dict):
+        t = self.loss_tensor(output_dict, data_dict)
+        return {'loss': t[0], 'c_loss': t[1], 'f_loss': t[2]}

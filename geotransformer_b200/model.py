@@ -40,7 +40,7 @@ class GeoTransformer(nn.Module):
         self.optimal_transport = LearnableLogOptimalTransport(cfg.model.num_sinkhorn_iterations)
 
     @torch.no_grad()
-    def forward_batch(self, data_dict, evaluator=None, results=None, side_streams=None, keep_outputs=True):
+    def forward_batch(self, data_dict, evaluator=None, results=None, side_streams=None, keep_outputs=True, loss_func=None, loss_out=None):
         """Several pairs per forward (``data_dict['batch_size'] = B > 1`` from ``registration_collate_fn_stack_mode``, stack
         order ``[ref_1..ref_B, src_1..src_B]`` at every level) -- the reference asserts batch_size == 1
         (``engine/single_tester.py:39-74``, README "only batch_size=1 is supported").  Backbone and transformer run ONCE over
@@ -51,7 +51,9 @@ class GeoTransformer(nn.Module):
 
         Returns a list of per-pair output dicts (``keep_outputs``), each like ``forward``'s.  With ``results`` (a (B, 24)
         float device tensor) the estimated transform (16) and, with ``evaluator``, the metrics (8) of pair p are written to
-        row p WITHOUT any host synchronisation in this call (correspondence tensors then stay full-capacity)."""
+        row p WITHOUT any host synchronisation in this call (correspondence tensors then stay full-capacity).  With ``loss_func``
+        (a geotransformer_b200.loss.OverallLoss) and ``loss_out`` (a (B, 3) float device tensor) the validation losses
+        [loss, c_loss, f_loss] of pair p are written to row p of ``loss_out`` after LGR, also without a host synchronisation."""
         native = getattr(self, '_native', None)
         if native is None:
             raise RuntimeError('forward_batch needs the native stage drivers: call enable_native(model) first')
@@ -163,6 +165,8 @@ class GeoTransformer(nn.Module):
             GF.evaluate_batched(gt[0], gt[1], gt[2], corr, corr_count, rc, sc, n_corr, transforms, results, points0,
                                 cn, [int(v) for v in lens_h[0]], evaluator.mode, evaluator.acceptance_overlap, evaluator.acceptance_radius,
                                 results[:, 16:], evaluator.acceptance_rmse, evaluator.acceptance_rre, evaluator.acceptance_rte)
+        if gt is not None and loss_func is not None and loss_out is not None:
+            loss_func.write_batched(y_n, cn, gt, k_pts[r], k_pts[s], k_masks[r], k_masks[s], scores, transforms, corr_count, loss_out)
         mark('matching+sinkhorn+lgr+metrics')
         if no_sync and not keep_outputs:
             return None

@@ -12,13 +12,14 @@ import numpy as np
 import torch
 
 from .engine import RegistrationEngine
-from .loss import Evaluator
+from .loss import Evaluator, OverallLoss
 
 # arrays written per pair, in the order of experiments/geotransformer.3dmatch.*/test.py:73-92
 NPZ_OUTPUT_KEYS = ('ref_points', 'src_points', 'ref_points_f', 'src_points_f', 'ref_points_c', 'src_points_c', 'ref_feats_c',
                    'src_feats_c', 'ref_node_corr_indices', 'src_node_corr_indices', 'ref_corr_points', 'src_corr_points',
                    'corr_scores', 'gt_node_corr_indices', 'gt_node_corr_overlaps', 'estimated_transform')
 METRICS = ('PIR', 'IR', 'RRE', 'RTE', 'RMSE', 'RR')
+LOSSES = ('loss', 'c_loss', 'f_loss')
 
 
 def _np(x):
@@ -26,11 +27,14 @@ def _np(x):
 
 
 class RegistrationTester:
-    def __init__(self, cfg, model, neighbor_limits, output_dir=None, num_streams=4, chunk=16, device=None, batch_size=1):
-        """batch_size > 1: that many pairs per forward (GeoTransformer.forward_batch) on each of the num_streams lanes"""
+    def __init__(self, cfg, model, neighbor_limits, output_dir=None, num_streams=4, chunk=16, device=None, batch_size=1, with_loss=False):
+        """batch_size > 1: that many pairs per forward (GeoTransformer.forward_batch) on each of the num_streams lanes.
+        with_loss: also report the validation losses loss / c_loss / f_loss (OverallLoss) per pair and as means in the summary,
+        as the reference's val_step does (trainval.py: loss_dict.update(result_dict))"""
         self.cfg, self.output_dir, self.chunk = cfg, output_dir, max(1, int(chunk), int(batch_size) * int(num_streams))
+        self.with_loss = bool(with_loss)
         self.engine = RegistrationEngine(model, cfg, neighbor_limits, num_streams=num_streams, device=device, evaluator=Evaluator(cfg),
-                                         batch_size=batch_size)
+                                         batch_size=batch_size, loss_func=OverallLoss(cfg) if self.with_loss else None)
 
     def after_test_step(self, data_dict, output_dict):
         """experiments/*/test.py:65-92"""
@@ -54,14 +58,18 @@ class RegistrationTester:
             results = self.engine.register(tensors, keep_outputs=self.output_dir is not None)
             for it, res in zip(items, results):
                 entry = {'metrics': res['metrics'], 'num_corr': res['num_corr'], 'estimated_transform': res['estimated_transform']}
+                if self.with_loss:
+                    entry.update(res['loss'])
                 if self.output_dir is not None:
                     entry['file'] = self.after_test_step(it, res.pop('output_dict'))
                 per_pair.append(entry)
                 if log is not None:       # single_tester.py:62-66 / test.py:55-63 summary string
                     msg = ', '.join(f'{k}: {res["metrics"][k]:.3f}' for k in METRICS)
                     log(f"{it.get('scene_name', 'scene')}, id0: {it.get('ref_frame', 0)}, id1: {it.get('src_frame', 1)}, {msg}, "
-                        f"nCorr: {res['num_corr']}")
+                        f"nCorr: {res['num_corr']}" + (''.join(f", {k}: {res['loss'][k]:.3f}" for k in LOSSES) if self.with_loss else ''))
         summary = {k: float(np.mean([p['metrics'][k] for p in per_pair])) for k in METRICS} if per_pair else {}
+        if self.with_loss and per_pair:
+            summary.update({k: float(np.mean([p[k] for p in per_pair])) for k in LOSSES})
         return summary, per_pair
 
     def close(self):

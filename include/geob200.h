@@ -371,6 +371,36 @@ int geob200_evaluate_batched(const int64_t* gt_node_corr_indices, const float* g
                              const int64_t* cloud_points, int mode, float rmse_threshold, float rre_threshold, float rte_threshold,
                              float* metrics, int64_t metrics_ld, void* stream);
 
+/* Validation losses (OverallLoss, experiments/<exp>/loss.py:10-92 with modules/loss/circle_loss.py:44-86): the values the reference
+ * computes in val_step, without gradients.  Pair p writes its row out[p * out_ld + {0: loss, 1: c_loss, 2: f_loss}] (out_ld >= 3).
+ * Batched over B pairs like geob200_evaluate_batched (cloud_nodes: HOST array of the 2B per-cloud superpoint counts, ref clouds
+ * first); one pair is B = 1.  Every reduction runs in a fixed order: results are bit-identical run to run, and a pair gets the same
+ * bits alone and in a batch.  Means over empty selections are NaN, as torch reports them.  Bad arguments (unsupported k,
+ * non-positive log_scale or radius, negative counts) are rejected before any launch.
+ *
+ * Coarse (CoarseMatchingLoss + WeightedCircleLoss) over ALL n_ref x n_src superpoints of each pair (no node mask): ref superpoints of
+ * pair p at rows sum_{q<p} n_ref(q) of ref_feats, src superpoints at rows sum_{q<p} n_src(q) of src_feats (both (rows, channels),
+ * L2-normalised).  Ground-truth rows of pair p at sum_{q<p} n_ref(q) * n_src(q) of gt_node_corr_indices / _overlaps as
+ * geob200_node_correspondences_batched lays them out; the first gt_count[p] (device int32, required) are valid.  Writes column 1. */
+size_t geob200_coarse_matching_loss_batched_workspace_bytes(int64_t n_rows, int64_t n_products);
+int geob200_coarse_matching_loss_batched(const float* ref_feats, const float* src_feats, int64_t channels, int64_t n_pairs,
+                                         const int64_t* cloud_nodes, const int64_t* gt_node_corr_indices, const float* gt_node_corr_overlaps,
+                                         const int32_t* gt_count, float positive_margin, float negative_margin, float positive_optimal,
+                                         float negative_optimal, float log_scale, float positive_overlap, float* out, int64_t out_ld,
+                                         void* workspace, size_t workspace_bytes, void* stream);
+/* Fine (FineMatchingLoss): n_patches patches of k (64 or 128) points per pair, patch q of pair p at row p * n_patches + q of the
+ * (rows, k, 3) points, (rows, k) uint8 masks and (rows, k+1, k+1) Sinkhorn scores; transforms (B,4,4) device.  patch_count
+ * (device int32 per pair, may be NULL = all) limits the patches read; padding patches beyond it are never read.  positive_radius is
+ * squared in double and rounded to fp32 once, like the reference's comparison.  Writes column 2; with loss_weights (HOST
+ * {w_coarse, w_fine}, may be NULL) also column 0 = w_coarse * column 1 + w_fine * column 2, so run it after the coarse loss on the
+ * same stream. */
+size_t geob200_fine_matching_loss_batched_workspace_bytes(int64_t n_pairs, int64_t n_patches);
+int geob200_fine_matching_loss_batched(const float* ref_knn_points, const float* src_knn_points, const uint8_t* ref_knn_masks,
+                                       const uint8_t* src_knn_masks, const float* matching_scores, const float* transforms, int64_t n_pairs,
+                                       int64_t n_patches, int64_t k, const int32_t* patch_count, double positive_radius,
+                                       const float* loss_weights, float* out, int64_t out_ld, void* workspace, size_t workspace_bytes,
+                                       void* stream);
+
 /* Profiling aid (bench.py roofline): while enabled, every tensor-core GEMM launch (nn.Linear and the KPConv contraction) is
  * bracketed by CUDA events on its stream; _read synchronises them and returns the count, shapes[3i..] = (m, n, k), ms[i]. */
 int geob200_linear_profile_enable(int on);
