@@ -103,6 +103,11 @@ _sig('geob200_coarse_matching_loss_batched_workspace_bytes', SZ, I64, I64)
 _sig('geob200_coarse_matching_loss_batched', c_int, P, P, I64, I64, P, P, P, P, F, F, F, F, F, F, P, I64, P, SZ, P)
 _sig('geob200_fine_matching_loss_batched_workspace_bytes', SZ, I64, I64)
 _sig('geob200_fine_matching_loss_batched', c_int, P, P, P, P, P, P, I64, I64, I64, P, D, P, P, I64, P, SZ, P)
+_sig('geob200_ransac_correspondences_batched_workspace_bytes', SZ, I64, I64)
+_sig('geob200_ransac_correspondences_batched', c_int, P, P, I64, I64, P, F, I64, I64, ctypes.c_uint64, I64, P, P, P, P, P, P, P, P, P, P,
+     SZ, P)
+_sig('geob200_correspondence_metrics_batched_workspace_bytes', SZ, I64, I64)
+_sig('geob200_correspondence_metrics_batched', c_int, P, P, I64, I64, P, P, I64, F, P, I64, P, SZ, P)
 
 _sig('geob200_linear_profile_enable', c_int, c_int)
 _sig('geob200_set_split_k', c_int, c_int)

@@ -37,6 +37,8 @@ def _base(seed=7351):
                         positive_overlap=0.1)
     c.fine_loss = Cfg(positive_radius=0.05)
     c.loss = Cfg(weight_coarse_loss=1.0, weight_fine_loss=1.0)
+    # correspondence RANSAC of eval.py --method ransac (experiments/*/config.py, _C.ransac); seed keys the sampler
+    c.ransac = Cfg(distance_threshold=0.05, num_points=3, num_iterations=1000, seed=0)
     return c
 
 
@@ -60,6 +62,7 @@ def make_cfg(name='3dmatch'):
         c.eval.update(acceptance_radius=1.0, rre_threshold=5.0, rte_threshold=2.0)
         c.coarse_loss.log_scale = 40
         c.fine_loss.positive_radius = 0.6
+        c.ransac.update(distance_threshold=0.3, num_points=4, num_iterations=50000)
         c.neighbor_limits = None  # calibrated (reference utils/data.py:192-217)
     elif name == 'modelnet':
         c.backbone.update(num_stages=3, init_voxel_size=0.05, base_radius=2.5)

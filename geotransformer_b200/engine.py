@@ -16,6 +16,7 @@ from . import _lib
 from .utils.data import registration_collate_fn_stack_mode
 
 LOSS_KEYS = ('loss', 'c_loss', 'f_loss')
+METRIC_KEYS = ('PIR', 'IR', 'RRE', 'RTE', 'RMSE', 'RR')
 
 
 def pin_host_threads_to_gpu(device):
@@ -41,7 +42,7 @@ def pin_host_threads_to_gpu(device):
 
 class RegistrationEngine:
     def __init__(self, model, cfg, neighbor_limits, num_streams=4, device=None, native=True, evaluator=None, pin_cpu=False,
-                 batch_size=1, side_streams=4, loss_func=None):
+                 batch_size=1, side_streams=4, loss_func=None, ransac=None):
         """pin_cpu: bind the calling thread and the worker threads to the CPUs local to the GPU (pin_host_threads_to_gpu).
         evaluator: optional geotransformer_b200.loss.Evaluator; its metrics (PIR, IR, RRE, RTE, RMSE, RR) are then computed
         on the device for every pair and travel back with the transform in the same D2H copy.
@@ -49,7 +50,10 @@ class RegistrationEngine:
         one backbone / transformer pass over the stacked rows of all pairs, per-pair stages on ``side_streams`` extra
         streams), with ONE host synchronisation per batch besides the collate's size read-backs.
         loss_func: optional geotransformer_b200.loss.OverallLoss; every result then gains 'loss': {'loss', 'c_loss', 'f_loss'}
-        (the reference's val_step losses), computed on the device and read back with the same event."""
+        (the reference's val_step losses), computed on the device and read back with the same event.
+        ransac: optional config section (cfg.ransac: distance_threshold, num_points, num_iterations, seed); every result then gains
+        'ransac': {'estimated_transform', 'fitness', 'inlier_rmse'(, 'metrics' with an evaluator)} -- correspondence RANSAC on the
+        LGR correspondences, run on the lane's stream after LGR (pair p of a forward draws from the stream (seed, p))."""
         self.model, self.cfg, self.limits = model, cfg, neighbor_limits
         if native and not hasattr(model, '_native'):
             from .model import enable_native
@@ -59,6 +63,7 @@ class RegistrationEngine:
         self.pinned_cpu = pin_host_threads_to_gpu(self.device) if pin_cpu else False
         self.evaluator = evaluator
         self.loss_func = loss_func
+        self.ransac = ransac
         self.stage_times = None          # set to {} to collect per-stage CUDA-event times (profiling; adds ~7 events per pair)
         self.streams = [torch.cuda.Stream(self.device) for _ in range(num_streams)]
         self.pool = ThreadPoolExecutor(max_workers=num_streams)
@@ -72,6 +77,10 @@ class RegistrationEngine:
         # per slot: [loss, c_loss, f_loss] rows on the device and pinned on the host (only with a loss function)
         self.l_dev = [torch.zeros((3,) if bs == 1 else (bs, 3), dtype=torch.float32, device=self.device) for _ in range(num_streams)]
         self.l_host = [torch.zeros((3,) if bs == 1 else (bs, 3), dtype=torch.float32).pin_memory() for _ in range(num_streams)]
+        # per slot: [RANSAC transform (16) | fitness | inlier_rmse | metrics of the RANSAC transform (8)] (only with ransac)
+        x_rows = (26,) if bs == 1 else (bs, 26)
+        self.x_dev = [torch.zeros(x_rows, dtype=torch.float32, device=self.device) if ransac is not None else None for _ in range(num_streams)]
+        self.x_host = [torch.zeros(x_rows, dtype=torch.float32).pin_memory() if ransac is not None else None for _ in range(num_streams)]
         self.sides = [[torch.cuda.Stream(self.device) for _ in range(side_streams)] if bs > 1 else [] for _ in range(num_streams)]
 
     def _one(self, slot, pair, keep):
@@ -96,6 +105,9 @@ class RegistrationEngine:
         if self.loss_func is not None:
             self.loss_func.loss_tensor(out, data, out=self.l_dev[slot])
             self.l_host[slot].copy_(self.l_dev[slot], non_blocking=True)
+        if self.ransac is not None:
+            self._ransac_one(out, data['transform'], self.x_dev[slot], 0)
+            self.x_host[slot].copy_(self.x_dev[slot], non_blocking=True)
         done = torch.cuda.Event()
         done.record(stream)
         done.synchronize()                      # this thread only; the other streams keep running
@@ -109,9 +121,26 @@ class RegistrationEngine:
             res['metrics'] = dict(zip(('PIR', 'IR', 'RRE', 'RTE', 'RMSE', 'RR'), m[:6]))
         if self.loss_func is not None:
             res['loss'] = dict(zip(LOSS_KEYS, self.l_host[slot].tolist()))
+        if self.ransac is not None:
+            res['ransac'] = self._ransac_result(self.x_host[slot])
         if keep:
             res['output_dict'] = out
         return res, done
+
+    def _ransac_one(self, out, transform, row, pair):
+        """RANSAC of one pair's (trimmed) correspondences into ``row`` (26,), metrics of its transform with the evaluator"""
+        from .model import write_ransac_rows
+        write_ransac_rows(self.ransac, out['src_corr_points'].unsqueeze(0), out['ref_corr_points'].unsqueeze(0), None, row.reshape(1, -1),
+                          first_pair=pair)
+        if self.evaluator is not None:
+            self.evaluator.metrics_tensor(dict(out, estimated_transform=row[:16].reshape(4, 4)), {'transform': transform}, out=row[18:26])
+
+    def _ransac_result(self, row):
+        v = row.tolist()
+        r = {'estimated_transform': row[:16].reshape(4, 4).clone(), 'fitness': v[16], 'inlier_rmse': v[17]}
+        if self.evaluator is not None:
+            r['metrics'] = dict(zip(METRIC_KEYS, v[18:24]))
+        return r
 
     def _batch(self, slot, chunk, keep):
         """``len(chunk)`` pairs in one forward (batch mode)"""
@@ -129,6 +158,8 @@ class RegistrationEngine:
             data['_stage_events'] = marks
         r_dev, r_host = self.r_dev[slot][:n], self.r_host[slot][:n]
         l_dev, l_host, lf = self.l_dev[slot][:n], self.l_host[slot][:n], self.loss_func
+        rs = self.ransac
+        x_dev, x_host = (self.x_dev[slot][:n], self.x_host[slot][:n]) if rs is not None else (None, None)
         if n == 1:             # a trailing single pair: the one-pair forward
             out = self.model(data)
             r_dev[0, :16].copy_(out['estimated_transform'].reshape(16))
@@ -136,6 +167,8 @@ class RegistrationEngine:
                 self.evaluator.metrics_tensor(out, data, out=r_dev[0, 16:])
             if lf is not None:
                 lf.loss_tensor(out, data, out=l_dev[0])
+            if rs is not None:
+                self._ransac_one(out, data['transform'], x_dev[0], 0)
             outs = [out]
         elif keep:             # trimmed per-pair output dicts (one extra host sync for the counts), metrics from them
             outs = self.model.forward_batch(data, side_streams=self.sides[slot])
@@ -145,12 +178,16 @@ class RegistrationEngine:
                     self.evaluator.metrics_tensor(o, {'transform': data['transform'][p]}, out=r_dev[p, 16:])
                 if lf is not None:
                     lf.loss_tensor(o, {'transform': data['transform'][p]}, out=l_dev[p])
+                if rs is not None:
+                    self._ransac_one(o, data['transform'][p], x_dev[p], p)
         else:
             outs = self.model.forward_batch(data, evaluator=self.evaluator, results=r_dev, side_streams=self.sides[slot], keep_outputs=False,
-                                            loss_func=lf, loss_out=l_dev)
+                                            loss_func=lf, loss_out=l_dev, ransac=rs, ransac_out=x_dev)
         r_host.copy_(r_dev, non_blocking=True)
         if lf is not None:
             l_host.copy_(l_dev, non_blocking=True)
+        if rs is not None:
+            x_host.copy_(x_dev, non_blocking=True)
         done = torch.cuda.Event()
         done.record(stream)
         done.synchronize()
@@ -170,6 +207,8 @@ class RegistrationEngine:
                 r['num_corr'] = int(outs[0]['ref_corr_points'].shape[0])
             if lf is not None:
                 r['loss'] = dict(zip(LOSS_KEYS, l_host[p].tolist()))
+            if rs is not None:
+                r['ransac'] = self._ransac_result(x_host[p])
             if keep:
                 r['output_dict'] = outs[p]
             res.append(r)

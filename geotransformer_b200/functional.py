@@ -953,3 +953,108 @@ def fine_matching_loss(ref_knn_points, src_knn_points, ref_knn_masks, src_knn_ma
                                positive_radius, patch_count=None if n_patches is None else n_patches.reshape(1),
                                loss_weights=loss_weights, out=out)
     return out
+
+
+# ------------------------------------------------------------------------------------------------ correspondence RANSAC
+# Open3D's registration_ransac_based_on_correspondence as the reference calls it (utils/open3d.py:169-198); semantics and the
+# deviations from Open3D (sampler, tie rule, fp32 scoring) in DESIGN.md section 3b.  Pair p's correspondences are rows
+# [0, num_corr[p]) of (B, capacity, 3) tensors -- the layout local_global_registration_batched returns.
+
+RANSAC_KEYS = ('transform', 'fitness', 'inlier_rmse', 'inliers', 'iteration')
+
+
+def ransac_correspondences_batched(src_corr_points, ref_corr_points, distance_threshold, ransac_n, num_iterations, seed=0, num_corr=None,
+                                   records=False, first_pair=0):
+    """RANSAC of B pairs in one launch pair, no host synchronisation.  ``num_corr``: (B,) device int32 counts or None (all rows).
+    Pair p draws its samples from the stream (seed, first_pair + p): a pair gives the same result alone (``first_pair`` = its id)
+    as inside any batch.
+    Returns a dict: transform (B, 4, 4), fitness (B,), inlier_rmse (B,), inliers (B,) int32, iteration (B,) int32 (-1: no
+    hypothesis with an inlier, or fewer than ransac_n correspondences: identity, fitness 0).  ``records``: also the
+    per-hypothesis hyp_transforms (B, I, 4, 4), hyp_inliers (B, I), hyp_rmse (B, I), hyp_samples (B, I, ransac_n) int32."""
+    _f(src_corr_points, 'src_corr_points'); _f(ref_corr_points, 'ref_corr_points')
+    if src_corr_points.ndim != 3 or src_corr_points.shape[2] != 3 or ref_corr_points.shape != src_corr_points.shape:
+        raise ValueError('ransac_correspondences_batched: src / ref must both be (B, capacity, 3)')
+    if not 0 <= int(seed) < 1 << 64:
+        raise ValueError('ransac_correspondences_batched: seed must be a 64-bit unsigned integer')
+    B, cap = src_corr_points.shape[0], src_corr_points.shape[1]
+    I = int(num_iterations)
+    dev = src_corr_points.device
+    if ref_corr_points.device != dev:
+        raise RuntimeError('ransac_correspondences_batched: src and ref must be on one device')
+    if num_corr is not None:
+        L.require_cuda(num_corr, 'num_corr', _i32)
+        if num_corr.numel() != B or num_corr.device != dev:
+            raise ValueError('ransac_correspondences_batched: num_corr must hold one count per pair, on the points\' device')
+    lib = L.lib()
+    T = torch.empty((B, 4, 4), dtype=_f32, device=dev)
+    fit = torch.empty((B,), dtype=_f32, device=dev)
+    rmse = torch.empty((B,), dtype=_f32, device=dev)
+    inl = torch.empty((B,), dtype=_i32, device=dev)
+    it = torch.empty((B,), dtype=_i32, device=dev)
+    rec = None
+    if records:
+        rec = dict(hyp_transforms=torch.empty((B, max(I, 1), 4, 4), dtype=_f32, device=dev),
+                   hyp_inliers=torch.empty((B, max(I, 1)), dtype=_i32, device=dev),
+                   hyp_rmse=torch.empty((B, max(I, 1)), dtype=_f32, device=dev),
+                   hyp_samples=torch.empty((B, max(I, 1), 8), dtype=_i32, device=dev))
+    ws = L.workspace(lib.geob200_ransac_correspondences_batched_workspace_bytes(B, I), dev, tag='ransac')
+    L.check(lib.geob200_ransac_correspondences_batched(
+        ref_corr_points.data_ptr(), src_corr_points.data_ptr(), B, cap, L.ptr(num_corr), float(distance_threshold), int(ransac_n), I,
+        ctypes.c_uint64(int(seed)), int(first_pair), T.data_ptr(), fit.data_ptr(), rmse.data_ptr(), inl.data_ptr(), it.data_ptr(),
+        *(None if rec is None else rec[k].data_ptr() for k in ('hyp_transforms', 'hyp_inliers', 'hyp_rmse', 'hyp_samples')),
+        ws.data_ptr(), ws.numel(), L.stream_ptr()), 'ransac_correspondences_batched')
+    res = dict(transform=T, fitness=fit, inlier_rmse=rmse, inliers=inl, iteration=it)
+    if rec is not None:
+        rec['hyp_samples'] = rec['hyp_samples'][:, :, :int(ransac_n)]
+        res.update(rec)
+    return res
+
+
+def ransac_correspondences(src_corr_points, ref_corr_points, distance_threshold, ransac_n, num_iterations, seed=0, num_corr=None,
+                           records=False, pair=0):
+    """RANSAC of one pair: (N, 3) src / ref correspondence points (``num_corr``: optional (1,) device int32 count of valid rows;
+    ``pair``: the pair id of the random stream, see the batched op).
+    Same dict as the batched op without the pair dimension: transform (4, 4), fitness, inlier_rmse, inliers, iteration."""
+    res = ransac_correspondences_batched(src_corr_points.unsqueeze(0), ref_corr_points.unsqueeze(0), distance_threshold, ransac_n,
+                                         num_iterations, seed=seed, num_corr=None if num_corr is None else num_corr.reshape(1),
+                                         records=records, first_pair=pair)
+    return {k: v[0] for k, v in res.items()}
+
+
+CORRESPONDENCE_METRICS = ('f_IR', 'f_OV', 'f_RS', 'f_NU')
+
+
+def correspondence_metrics_batched(ref_corr_points, src_corr_points, transforms, positive_radius, num_corr=None, out=None):
+    """evaluate_correspondences (utils/registration.py:240-250) of B pairs in the RANSAC layout under ``transforms`` (B, 4, 4) or
+    (B, >= 16) rows: row p of ``out`` (B, >= 4, any row stride) = [f_IR, f_OV, f_RS, f_NU] (inlier ratio, overlap, mean residual,
+    count; the means of an empty pair are NaN)."""
+    _f(ref_corr_points, 'ref_corr_points'); _f(src_corr_points, 'src_corr_points')
+    if src_corr_points.ndim != 3 or src_corr_points.shape[2] != 3 or ref_corr_points.shape != src_corr_points.shape:
+        raise ValueError('correspondence_metrics_batched: src / ref must both be (B, capacity, 3)')
+    B, cap = src_corr_points.shape[0], src_corr_points.shape[1]
+    tr = transforms.reshape(B, -1) if transforms.is_contiguous() else transforms
+    if tr.dtype != _f32 or not tr.is_cuda or tr.shape[1] < 12 or tr.stride(1) != 1:
+        raise RuntimeError('correspondence_metrics_batched: transforms must be float32 CUDA rows of >= 12 contiguous values')
+    dev = src_corr_points.device
+    if ref_corr_points.device != dev or tr.device != dev:
+        raise RuntimeError('correspondence_metrics_batched: points and transforms must be on one device')
+    if num_corr is not None:
+        L.require_cuda(num_corr, 'num_corr', _i32)
+        if num_corr.numel() != B or num_corr.device != dev:
+            raise ValueError('correspondence_metrics_batched: num_corr must hold one count per pair, on the points\' device')
+    if out is None:
+        out = torch.empty((B, 4), dtype=_f32, device=dev)
+    if out.shape[0] != B or out.shape[1] < 4 or out.stride(1) != 1 or out.dtype != _f32 or out.device != dev:
+        raise RuntimeError('correspondence_metrics_batched: out must be float32 CUDA rows of >= 4 contiguous columns')
+    lib = L.lib()
+    ws = L.workspace(lib.geob200_correspondence_metrics_batched_workspace_bytes(B, cap), dev, tag='corr_metrics')
+    L.check(lib.geob200_correspondence_metrics_batched(ref_corr_points.data_ptr(), src_corr_points.data_ptr(), B, cap, L.ptr(num_corr),
+                                                       tr.data_ptr(), tr.stride(0), float(positive_radius), out.data_ptr(), out.stride(0),
+                                                       ws.data_ptr(), ws.numel(), L.stream_ptr()), 'correspondence_metrics_batched')
+    return out
+
+
+def evaluate_correspondences(ref_corr_points, src_corr_points, transform, positive_radius=0.1):
+    """one pair: (4,) device tensor [f_IR, f_OV, f_RS, f_NU]"""
+    return correspondence_metrics_batched(ref_corr_points.unsqueeze(0), src_corr_points.unsqueeze(0), transform.reshape(1, 16).contiguous(),
+                                          positive_radius)[0]

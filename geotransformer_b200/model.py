@@ -40,7 +40,8 @@ class GeoTransformer(nn.Module):
         self.optimal_transport = LearnableLogOptimalTransport(cfg.model.num_sinkhorn_iterations)
 
     @torch.no_grad()
-    def forward_batch(self, data_dict, evaluator=None, results=None, side_streams=None, keep_outputs=True, loss_func=None, loss_out=None):
+    def forward_batch(self, data_dict, evaluator=None, results=None, side_streams=None, keep_outputs=True, loss_func=None, loss_out=None,
+                      ransac=None, ransac_out=None):
         """Several pairs per forward (``data_dict['batch_size'] = B > 1`` from ``registration_collate_fn_stack_mode``, stack
         order ``[ref_1..ref_B, src_1..src_B]`` at every level) -- the reference asserts batch_size == 1
         (``engine/single_tester.py:39-74``, README "only batch_size=1 is supported").  Backbone and transformer run ONCE over
@@ -53,7 +54,11 @@ class GeoTransformer(nn.Module):
         float device tensor) the estimated transform (16) and, with ``evaluator``, the metrics (8) of pair p are written to
         row p WITHOUT any host synchronisation in this call (correspondence tensors then stay full-capacity).  With ``loss_func``
         (a geotransformer_b200.loss.OverallLoss) and ``loss_out`` (a (B, 3) float device tensor) the validation losses
-        [loss, c_loss, f_loss] of pair p are written to row p of ``loss_out`` after LGR, also without a host synchronisation."""
+        [loss, c_loss, f_loss] of pair p are written to row p of ``loss_out`` after LGR, also without a host synchronisation.
+        With ``ransac`` (a config section: distance_threshold, num_points, num_iterations, seed) and ``ransac_out`` (a (B, 26)
+        float device tensor) correspondence RANSAC runs on the LGR correspondences of every pair (pair p draws from the stream
+        (seed, p)); row p receives [transform (16), fitness, inlier_rmse] and, with ``evaluator``, the metrics (8) of the RANSAC
+        transform -- no host synchronisation either."""
         native = getattr(self, '_native', None)
         if native is None:
             raise RuntimeError('forward_batch needs the native stage drivers: call enable_native(model) first')
@@ -165,6 +170,12 @@ class GeoTransformer(nn.Module):
             GF.evaluate_batched(gt[0], gt[1], gt[2], corr, corr_count, rc, sc, n_corr, transforms, results, points0,
                                 cn, [int(v) for v in lens_h[0]], evaluator.mode, evaluator.acceptance_overlap, evaluator.acceptance_radius,
                                 results[:, 16:], evaluator.acceptance_rmse, evaluator.acceptance_rre, evaluator.acceptance_rte)
+        if ransac is not None and ransac_out is not None:
+            write_ransac_rows(ransac, sc, rc, n_corr, ransac_out)
+            if gt is not None and evaluator is not None:
+                GF.evaluate_batched(gt[0], gt[1], gt[2], corr, corr_count, rc, sc, n_corr, transforms, ransac_out, points0,
+                                    cn, [int(v) for v in lens_h[0]], evaluator.mode, evaluator.acceptance_overlap, evaluator.acceptance_radius,
+                                    ransac_out[:, 18:26], evaluator.acceptance_rmse, evaluator.acceptance_rre, evaluator.acceptance_rte)
         if gt is not None and loss_func is not None and loss_out is not None:
             loss_func.write_batched(y_n, cn, gt, k_pts[r], k_pts[s], k_masks[r], k_masks[s], scores, transforms, corr_count, loss_out)
         mark('matching+sinkhorn+lgr+metrics')
@@ -319,3 +330,16 @@ def enable_native(model):
 
 def create_model(cfg):
     return GeoTransformer(cfg)
+
+
+def write_ransac_rows(ransac, src_corr_points, ref_corr_points, num_corr, out, first_pair=0):
+    """Correspondence RANSAC (``ransac``: distance_threshold, num_points, num_iterations, seed) of B pairs of (B, capacity, 3)
+    correspondences (``num_corr``: (B,) device int32 or None) into columns 0..17 of the (B, >= 18) float rows ``out``:
+    [transform (16), fitness, inlier_rmse].  No host synchronisation."""
+    rr = GF.ransac_correspondences_batched(src_corr_points, ref_corr_points, ransac.distance_threshold, ransac.num_points,
+                                           ransac.num_iterations, seed=ransac.get('seed', 0), num_corr=num_corr, first_pair=first_pair)
+    B = out.shape[0]
+    out[:, :16].copy_(rr['transform'].reshape(B, 16))
+    out[:, 16].copy_(rr['fitness'])
+    out[:, 17].copy_(rr['inlier_rmse'])
+    return rr

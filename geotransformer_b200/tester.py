@@ -27,14 +27,19 @@ def _np(x):
 
 
 class RegistrationTester:
-    def __init__(self, cfg, model, neighbor_limits, output_dir=None, num_streams=4, chunk=16, device=None, batch_size=1, with_loss=False):
+    def __init__(self, cfg, model, neighbor_limits, output_dir=None, num_streams=4, chunk=16, device=None, batch_size=1, with_loss=False,
+                 with_ransac=False):
         """batch_size > 1: that many pairs per forward (GeoTransformer.forward_batch) on each of the num_streams lanes.
         with_loss: also report the validation losses loss / c_loss / f_loss (OverallLoss) per pair and as means in the summary,
-        as the reference's val_step does (trainval.py: loss_dict.update(result_dict))"""
+        as the reference's val_step does (trainval.py: loss_dict.update(result_dict)).
+        with_ransac: also run correspondence RANSAC (cfg.ransac) on every pair's correspondences; each entry gains 'ransac'
+        (transform, fitness, inlier_rmse, metrics of the RANSAC transform) and the summary the means as ransac_<name>"""
         self.cfg, self.output_dir, self.chunk = cfg, output_dir, max(1, int(chunk), int(batch_size) * int(num_streams))
         self.with_loss = bool(with_loss)
+        self.with_ransac = bool(with_ransac)
         self.engine = RegistrationEngine(model, cfg, neighbor_limits, num_streams=num_streams, device=device, evaluator=Evaluator(cfg),
-                                         batch_size=batch_size, loss_func=OverallLoss(cfg) if self.with_loss else None)
+                                         batch_size=batch_size, loss_func=OverallLoss(cfg) if self.with_loss else None,
+                                         ransac=cfg.ransac if self.with_ransac else None)
 
     def after_test_step(self, data_dict, output_dict):
         """experiments/*/test.py:65-92"""
@@ -60,6 +65,8 @@ class RegistrationTester:
                 entry = {'metrics': res['metrics'], 'num_corr': res['num_corr'], 'estimated_transform': res['estimated_transform']}
                 if self.with_loss:
                     entry.update(res['loss'])
+                if self.with_ransac:
+                    entry['ransac'] = res['ransac']
                 if self.output_dir is not None:
                     entry['file'] = self.after_test_step(it, res.pop('output_dict'))
                 per_pair.append(entry)
@@ -70,6 +77,9 @@ class RegistrationTester:
         summary = {k: float(np.mean([p['metrics'][k] for p in per_pair])) for k in METRICS} if per_pair else {}
         if self.with_loss and per_pair:
             summary.update({k: float(np.mean([p[k] for p in per_pair])) for k in LOSSES})
+        if self.with_ransac and per_pair:
+            summary.update({f'ransac_{k}': float(np.mean([p['ransac']['metrics'][k] for p in per_pair])) for k in METRICS})
+            summary.update({f'ransac_{k}': float(np.mean([p['ransac'][k] for p in per_pair])) for k in ('fitness', 'inlier_rmse')})
         return summary, per_pair
 
     def close(self):

@@ -401,6 +401,31 @@ int geob200_fine_matching_loss_batched(const float* ref_knn_points, const float*
                                        const float* loss_weights, float* out, int64_t out_ld, void* workspace, size_t workspace_bytes,
                                        void* stream);
 
+/* Correspondence RANSAC (Open3D's registration_ransac_based_on_correspondence as utils/open3d.py:169-198 calls it) for B pairs:
+ * pair p's correspondences are rows [0, num_corr[p]) of (B, capacity, 3) ref / src arrays (num_corr: device int32 or NULL = all
+ * capacity rows).  All num_iterations hypotheses run; hypothesis i draws ransac_n indices with replacement from Philox4x32-10
+ * (key = seed, counter = (i, pair_base + p, j / 4, 0), index = umulhi(word j % 4, n)), fits an unweighted Kabsch, and counts the inliers
+ * ||R src + t - ref||^2 < tau^2 in pinned fp32 arithmetic.  Winner: most inliers, then lowest rmse, then lowest i.  Outputs per
+ * pair: transforms (B, 16) row-major, fitness = inliers / n, inlier_rmse, inlier_count, best_iteration (-1 and identity when no
+ * hypothesis has an inlier or n < ransac_n).  Optional per-hypothesis records (each NULL or (B, num_iterations, ...)):
+ * hyp_transforms (16 floats), hyp_inliers, hyp_rmse, hyp_samples (8 int32, -1 past ransac_n).  ransac_n in 3..8. */
+size_t geob200_ransac_correspondences_batched_workspace_bytes(int64_t n_pairs, int64_t num_iterations);
+int geob200_ransac_correspondences_batched(const float* ref_corr_points, const float* src_corr_points, int64_t n_pairs, int64_t capacity,
+                                           const int32_t* num_corr, float distance_threshold, int64_t ransac_n, int64_t num_iterations,
+                                           uint64_t seed, int64_t pair_base, float* transforms, float* fitness, float* inlier_rmse,
+                                           int32_t* inlier_count,
+                                           int32_t* best_iteration, float* hyp_transforms, int32_t* hyp_inliers, float* hyp_rmse,
+                                           int32_t* hyp_samples, void* workspace, size_t workspace_bytes, void* stream);
+
+/* evaluate_correspondences (utils/registration.py:240-250) for B pairs in the RANSAC layout: row p of out (stride out_ld >= 4)
+ * = [inlier ratio, overlap, mean residual, count] under transforms + p * transform_ld (row-major, >= 12 floats).  The overlap is
+ * the fraction of ref correspondence points whose nearest transformed src correspondence point is closer than positive_radius
+ * (brute force).  The means of an empty pair are NaN. */
+size_t geob200_correspondence_metrics_batched_workspace_bytes(int64_t n_pairs, int64_t capacity);
+int geob200_correspondence_metrics_batched(const float* ref_corr_points, const float* src_corr_points, int64_t n_pairs, int64_t capacity,
+                                           const int32_t* num_corr, const float* transforms, int64_t transform_ld, float positive_radius,
+                                           float* out, int64_t out_ld, void* workspace, size_t workspace_bytes, void* stream);
+
 /* Profiling aid (bench.py roofline): while enabled, every tensor-core GEMM launch (nn.Linear and the KPConv contraction) is
  * bracketed by CUDA events on its stream; _read synchronises them and returns the count, shapes[3i..] = (m, n, k), ms[i]. */
 int geob200_linear_profile_enable(int on);
