@@ -108,6 +108,12 @@ _sig('geob200_ransac_correspondences_batched', c_int, P, P, I64, I64, P, F, I64,
      SZ, P)
 _sig('geob200_correspondence_metrics_batched_workspace_bytes', SZ, I64, I64)
 _sig('geob200_correspondence_metrics_batched', c_int, P, P, I64, I64, P, P, I64, F, P, I64, P, SZ, P)
+_sig('geob200_corr_order_batched', c_int, P, I64, I64, P, I64, P, P)
+_sig('geob200_corr_select_batched', c_int, P, P, P, I64, I64, P, P, I64, I64, P, P, P, P, P)
+_sig('geob200_sparse_correspondence_eval_batched_workspace_bytes', SZ, I64, I64, I64)
+_sig('geob200_sparse_correspondence_eval_batched', c_int, P, P, I64, P, P, I64, P, I64, I64, I64, P, P, SZ, P)
+_sig('geob200_registration_error_batched', c_int, P, I64, P, I64, P, P, I64, c_int, D, D, P, P)
+_sig('geob200_weighted_procrustes_counts', c_int, P, P, P, I64, I64, P, F, F, P, P)
 
 _sig('geob200_linear_profile_enable', c_int, c_int)
 _sig('geob200_set_split_k', c_int, c_int)

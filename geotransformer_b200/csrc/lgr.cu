@@ -334,16 +334,14 @@ __global__ void __launch_bounds__(1024) lgr_refine_kernel(const float* __restric
     if (threadIdx.x < 16) Tout[threadIdx.x] = cur[threadIdx.x];
 }
 
-// generic batched weighted procrustes (modules/registration/procrustes.py:6-73): one warp per problem
-__global__ void __launch_bounds__(256) procrustes_kernel(const float* __restrict__ src, const float* __restrict__ ref,
-                                                         const float* __restrict__ weights, int B, int N, float weight_thresh,
-                                                         float eps, float* __restrict__ T) {
-    const int lane = threadIdx.x & 31;
-    const int b = blockIdx.x * 8 + (threadIdx.x >> 5);
-    if (b >= B) return;
+// generic batched weighted procrustes (modules/registration/procrustes.py:6-73): one warp per problem.  Problem b has rows
+// [0, n) at row b * ld; row e is always taken by lane e % 32, so a problem's result does not depend on ld.
+__device__ __forceinline__ void procrustes_warp(const float* __restrict__ src, const float* __restrict__ ref,
+                                                const float* __restrict__ weights, int b, int ld, int N, float weight_thresh,
+                                                float eps, float* __restrict__ T, int lane) {
     double sw = 0.0;
     for (int e = lane; e < N; e += 32) {
-        float w = (weights != nullptr) ? weights[(long long)b * N + e] : 1.f;
+        float w = (weights != nullptr) ? weights[(long long)b * ld + e] : 1.f;
         if (w < weight_thresh) w = 0.f;
         sw += (double)w;
     }
@@ -351,11 +349,11 @@ __global__ void __launch_bounds__(256) procrustes_kernel(const float* __restrict
     const double inv = 1.0 / (sw + (double)eps);
     double W = 0, S1[3] = {0, 0, 0}, S2[3] = {0, 0, 0}, Sxy[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
     for (int e = lane; e < N; e += 32) {
-        float wf = (weights != nullptr) ? weights[(long long)b * N + e] : 1.f;
+        float wf = (weights != nullptr) ? weights[(long long)b * ld + e] : 1.f;
         if (wf < weight_thresh) wf = 0.f;
         const double w = (double)wf * inv;
-        const float* x = src + ((long long)b * N + e) * 3;
-        const float* y = ref + ((long long)b * N + e) * 3;
+        const float* x = src + ((long long)b * ld + e) * 3;
+        const float* y = ref + ((long long)b * ld + e) * 3;
         W += w;
         for (int a = 0; a < 3; ++a) {
             S1[a] += w * x[a]; S2[a] += w * y[a];
@@ -366,6 +364,24 @@ __global__ void __launch_bounds__(256) procrustes_kernel(const float* __restrict
     for (int a = 0; a < 3; ++a) { S1[a] = warp_sum_d(S1[a]); S2[a] = warp_sum_d(S2[a]); }
     for (int a = 0; a < 9; ++a) Sxy[a] = warp_sum_d(Sxy[a]);
     if (lane == 0) finish_procrustes(W, S1, S2, Sxy, T + 16ll * b);
+}
+
+__global__ void __launch_bounds__(256) procrustes_kernel(const float* __restrict__ src, const float* __restrict__ ref,
+                                                         const float* __restrict__ weights, int B, int N, float weight_thresh,
+                                                         float eps, float* __restrict__ T) {
+    const int b = blockIdx.x * 8 + (threadIdx.x >> 5);
+    if (b >= B) return;
+    procrustes_warp(src, ref, weights, b, N, N, weight_thresh, eps, T, threadIdx.x & 31);
+}
+
+// the same with ragged problems: rows at or beyond counts[b] (device int32) contribute nothing
+__global__ void __launch_bounds__(256) procrustes_counts_kernel(const float* __restrict__ src, const float* __restrict__ ref,
+                                                                const float* __restrict__ weights, int B, int cap,
+                                                                const int* __restrict__ counts, float weight_thresh, float eps,
+                                                                float* __restrict__ T) {
+    const int b = blockIdx.x * 8 + (threadIdx.x >> 5);
+    if (b >= B) return;
+    procrustes_warp(src, ref, weights, b, cap, min(max(counts[b], 0), cap), weight_thresh, eps, T, threadIdx.x & 31);
 }
 
 }  // namespace geob200
@@ -464,6 +480,20 @@ int geob200_weighted_procrustes(const float* src_points, const float* ref_points
     GEOB_REQUIRE(batch > 0 && n > 0, "weighted_procrustes: empty input");
     procrustes_kernel<<<(unsigned)((batch + 7) / 8), 256, 0, (cudaStream_t)stream>>>(src_points, ref_points, weights, (int)batch,
                                                                                    (int)n, weight_thresh, eps, transforms);
+    GEOB_CHECK_LAUNCH();
+    count_launches(1);
+    return 0;
+}
+
+int geob200_weighted_procrustes_counts(const float* src_points, const float* ref_points, const float* weights, int64_t batch,
+                                       int64_t capacity, const int32_t* counts, float weight_thresh, float eps, float* transforms,
+                                       void* stream) {
+    GEOB_REQUIRE(batch > 0 && batch < (1ll << 31) && capacity >= 0 && capacity < (1ll << 31) / 3, "weighted_procrustes_counts: bad shape");
+    GEOB_REQUIRE(counts != nullptr && transforms != nullptr, "weighted_procrustes_counts: null counts or output");
+    GEOB_REQUIRE((src_points != nullptr && ref_points != nullptr) || capacity == 0, "weighted_procrustes_counts: null points");
+    procrustes_counts_kernel<<<(unsigned)((batch + 7) / 8), 256, 0, (cudaStream_t)stream>>>(src_points, ref_points, weights, (int)batch,
+                                                                                         (int)capacity, counts, weight_thresh, eps,
+                                                                                         transforms);
     GEOB_CHECK_LAUNCH();
     count_launches(1);
     return 0;

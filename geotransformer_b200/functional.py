@@ -1058,3 +1058,150 @@ def evaluate_correspondences(ref_corr_points, src_corr_points, transform, positi
     """one pair: (4,) device tensor [f_IR, f_OV, f_RS, f_NU]"""
     return correspondence_metrics_batched(ref_corr_points.unsqueeze(0), src_corr_points.unsqueeze(0), transform.reshape(1, 16).contiguous(),
                                           positive_radius)[0]
+
+
+# ------------------------------------------------------------------------------------------------ benchmark evaluation
+# The per-pair stages of eval.py that RANSAC and the correspondence metrics above do not cover (csrc/benchmark.cu).  Same
+# ragged layout: pair p's rows are [0, count[p]) of (B, capacity, ...) tensors, counts are (B,) device int32 or None (all rows).
+
+CORR_ORDER_KMAX = 8192
+
+
+def _counts(counts, B, dev, what):
+    if counts is not None:
+        L.require_cuda(counts, 'counts', _i32)
+        if counts.numel() != B or counts.device != dev:
+            raise ValueError(f'{what}: counts must hold one int32 count per pair, on the inputs\' device')
+    return counts
+
+
+def corr_order_batched(corr_scores, kmax, num_corr=None):
+    """(B, kmax) int32: row p = np.argsort(-scores[p, :n], kind='stable')[:kmax] (score descending, then row; NaN last), -1 past
+    min(n, kmax).  kmax <= CORR_ORDER_KMAX."""
+    _f(corr_scores, 'corr_scores')
+    if corr_scores.ndim != 2:
+        raise ValueError('corr_order_batched: corr_scores must be (B, capacity)')
+    if not 1 <= int(kmax) <= CORR_ORDER_KMAX:
+        raise ValueError(f'corr_order_batched: kmax must be in 1..{CORR_ORDER_KMAX}')
+    B, cap = corr_scores.shape
+    dev = corr_scores.device
+    _counts(num_corr, B, dev, 'corr_order_batched')
+    order = torch.empty((B, int(kmax)), dtype=_i32, device=dev)
+    L.check(L.lib().geob200_corr_order_batched(corr_scores.data_ptr(), B, cap, L.ptr(num_corr), int(kmax), order.data_ptr(),
+                                               L.stream_ptr()), 'corr_order_batched')
+    return order
+
+
+def corr_select_batched(ref_corr_points, src_corr_points, corr_scores, order, k, num_corr=None):
+    """eval.py's top-k selection with an ``order`` from corr_order_batched: returns (ref (B, K, 3), src (B, K, 3), scores (B, K),
+    count (B,) int32) with K = min(k, capacity) and count = min(n, k).  A pair with n <= k keeps its rows in their order."""
+    _f(ref_corr_points, 'ref_corr_points'); _f(src_corr_points, 'src_corr_points'); _f(corr_scores, 'corr_scores')
+    L.require_cuda(order, 'order', _i32)
+    B, cap = corr_scores.shape
+    if ref_corr_points.shape != (B, cap, 3) or src_corr_points.shape != (B, cap, 3) or order.ndim != 2 or order.shape[0] != B:
+        raise ValueError('corr_select_batched: ref / src must be (B, capacity, 3), scores (B, capacity), order (B, kmax)')
+    dev = corr_scores.device
+    if any(t.device != dev for t in (ref_corr_points, src_corr_points, order)):
+        raise RuntimeError('corr_select_batched: inputs must be on one device')
+    _counts(num_corr, B, dev, 'corr_select_batched')
+    K = min(int(k), cap)
+    ref_o = torch.empty((B, K, 3), dtype=_f32, device=dev)
+    src_o = torch.empty((B, K, 3), dtype=_f32, device=dev)
+    sc_o = torch.empty((B, K), dtype=_f32, device=dev)
+    cnt = torch.empty((B,), dtype=_i32, device=dev)
+    L.check(L.lib().geob200_corr_select_batched(ref_corr_points.data_ptr(), src_corr_points.data_ptr(), corr_scores.data_ptr(), B, cap,
+                                                L.ptr(num_corr), order.data_ptr(), order.shape[1], int(k), ref_o.data_ptr(),
+                                                src_o.data_ptr(), sc_o.data_ptr(), cnt.data_ptr(), L.stream_ptr()), 'corr_select_batched')
+    return ref_o, src_o, sc_o, cnt
+
+
+def sparse_correspondence_eval_batched(ref_node_corr_indices, src_node_corr_indices, gt_node_corr_indices, num_ref_nodes, num_src_nodes,
+                                       pred_count=None, gt_count=None):
+    """evaluate_sparse_correspondences (utils/registration.py:253-281) of B pairs: (B, 3) float64 [precision, recall, hit_ratio],
+    bit-identical to numpy.  Indices: (B, P) int64 ref / src node indices and (B, G, 2) int64 gt pairs; ``num_ref_nodes`` /
+    ``num_src_nodes``: host upper bounds of the node indices (the M x N of the reference's dense matrices)."""
+    for t, name in ((ref_node_corr_indices, 'ref_node_corr_indices'), (src_node_corr_indices, 'src_node_corr_indices'),
+                    (gt_node_corr_indices, 'gt_node_corr_indices')):
+        L.require_cuda(t, name, _i64)
+    B, pcap = ref_node_corr_indices.shape
+    if src_node_corr_indices.shape != (B, pcap) or gt_node_corr_indices.ndim != 3 or gt_node_corr_indices.shape[0] != B \
+            or gt_node_corr_indices.shape[2] != 2:
+        raise ValueError('sparse_correspondence_eval_batched: indices must be (B, P), (B, P) and (B, G, 2)')
+    dev = ref_node_corr_indices.device
+    if src_node_corr_indices.device != dev or gt_node_corr_indices.device != dev:
+        raise RuntimeError('sparse_correspondence_eval_batched: inputs must be on one device')
+    _counts(pred_count, B, dev, 'sparse_correspondence_eval_batched')
+    _counts(gt_count, B, dev, 'sparse_correspondence_eval_batched')
+    lib = L.lib()
+    m, n = int(num_ref_nodes), int(num_src_nodes)
+    out = torch.empty((B, 3), dtype=torch.float64, device=dev)
+    need = lib.geob200_sparse_correspondence_eval_batched_workspace_bytes(B, m, n)
+    ws = L.workspace(need, dev, tag='sparse_eval') if need else None
+    L.check(lib.geob200_sparse_correspondence_eval_batched(
+        ref_node_corr_indices.data_ptr(), src_node_corr_indices.data_ptr(), pcap, L.ptr(pred_count), gt_node_corr_indices.data_ptr(),
+        gt_node_corr_indices.shape[1], L.ptr(gt_count), B, m, n, out.data_ptr(), L.ptr(ws), 0 if ws is None else ws.numel(),
+        L.stream_ptr()), 'sparse_correspondence_eval_batched')
+    return out
+
+
+def _transform_rows(t, B, what):
+    tr = t.reshape(B, -1) if t.is_contiguous() else t
+    if tr.dtype != _f32 or not tr.is_cuda or tr.ndim != 2 or tr.shape[1] < 16 or tr.stride(1) != 1:
+        raise RuntimeError(f'{what}: transforms must be float32 CUDA rows of >= 16 contiguous values')
+    return tr
+
+
+def registration_error_batched(gt_transforms, est_transforms, covariances=None, has_covariance=None, rmse_threshold=None,
+                               rre_threshold=None, rte_threshold=None):
+    """(B, 4) float64 rows [rre (deg), rte, p, accepted], computed in double.  p = compute_transform_error of 3DMatch
+    (threedmatch/utils.py:130-136) with the (B, 6, 6) ``covariances`` where ``has_covariance`` (B,) int32 is set, NaN elsewhere.
+    Acceptance: ``rmse_threshold`` given = p < rmse_threshold**2 (3DMatch); otherwise rre < rre_threshold and rte < rte_threshold
+    (KITTI)."""
+    B = gt_transforms.shape[0]
+    gt = _transform_rows(gt_transforms, B, 'registration_error_batched')
+    est = _transform_rows(est_transforms, B, 'registration_error_batched')
+    dev = gt.device
+    if est.device != dev or est.shape[0] != B:
+        raise RuntimeError('registration_error_batched: gt and est transforms must be B rows on one device')
+    if covariances is not None:
+        _f(covariances, 'covariances')
+        if covariances.numel() != 36 * B or covariances.device != dev:
+            raise ValueError('registration_error_batched: covariances must be (B, 6, 6) on the transforms\' device')
+    _counts(has_covariance, B, dev, 'registration_error_batched')
+    if rmse_threshold is not None:
+        if covariances is None:
+            raise ValueError('registration_error_batched: the rmse acceptance needs covariances')
+        mode, t0, t1 = 0, float(rmse_threshold) ** 2, 0.0
+    elif rre_threshold is not None and rte_threshold is not None:
+        mode, t0, t1 = 1, float(rre_threshold), float(rte_threshold)
+    else:
+        raise ValueError('registration_error_batched: give rmse_threshold, or rre_threshold and rte_threshold')
+    out = torch.empty((B, 4), dtype=torch.float64, device=dev)
+    L.check(L.lib().geob200_registration_error_batched(gt.data_ptr(), gt.stride(0), est.data_ptr(), est.stride(0), L.ptr(covariances),
+                                                       L.ptr(has_covariance), B, mode, t0, t1, out.data_ptr(), L.stream_ptr()),
+            'registration_error_batched')
+    return out
+
+
+def weighted_procrustes_counts(src_points, ref_points, weights, counts, weight_thresh=0.0, eps=1e-5):
+    """weighted_procrustes over ragged problems: problem b = rows [0, counts[b]) of (B, capacity, 3) src / ref and (B, capacity)
+    weights (or None); (B, 4, 4), bit-identical to weighted_procrustes on the trimmed rows."""
+    _f(src_points, 'src_points'); _f(ref_points, 'ref_points')
+    if src_points.ndim != 3 or src_points.shape[2] != 3 or ref_points.shape != src_points.shape:
+        raise ValueError('weighted_procrustes_counts: src / ref must both be (B, capacity, 3)')
+    B, cap = src_points.shape[0], src_points.shape[1]
+    dev = src_points.device
+    if weights is not None:
+        _f(weights, 'weights')
+        if weights.shape != (B, cap) or weights.device != dev:
+            raise ValueError('weighted_procrustes_counts: weights must be (B, capacity) on the points\' device')
+    if ref_points.device != dev:
+        raise RuntimeError('weighted_procrustes_counts: src and ref must be on one device')
+    if counts is None:
+        raise ValueError('weighted_procrustes_counts: counts are required (weighted_procrustes takes full problems)')
+    _counts(counts, B, dev, 'weighted_procrustes_counts')
+    T = torch.empty((B, 4, 4), dtype=_f32, device=dev)
+    L.check(L.lib().geob200_weighted_procrustes_counts(src_points.data_ptr(), ref_points.data_ptr(), L.ptr(weights), B, cap, counts.data_ptr(),
+                                                       float(weight_thresh), float(eps), T.data_ptr(), L.stream_ptr()),
+            'weighted_procrustes_counts')
+    return T

@@ -28,12 +28,17 @@ def _np(x):
 
 class RegistrationTester:
     def __init__(self, cfg, model, neighbor_limits, output_dir=None, num_streams=4, chunk=16, device=None, batch_size=1, with_loss=False,
-                 with_ransac=False):
+                 with_ransac=False, layout='3dmatch'):
         """batch_size > 1: that many pairs per forward (GeoTransformer.forward_batch) on each of the num_streams lanes.
         with_loss: also report the validation losses loss / c_loss / f_loss (OverallLoss) per pair and as means in the summary,
         as the reference's val_step does (trainval.py: loss_dict.update(result_dict)).
         with_ransac: also run correspondence RANSAC (cfg.ransac) on every pair's correspondences; each entry gains 'ransac'
-        (transform, fitness, inlier_rmse, metrics of the RANSAC transform) and the summary the means as ransac_<name>"""
+        (transform, fitness, inlier_rmse, metrics of the RANSAC transform) and the summary the means as ransac_<name>.
+        layout: '3dmatch' writes <output_dir>/<scene_name>/<ref_frame>_<src_frame>.npz with 'overlap' (3DMatch test.py); 'kitti'
+        writes <output_dir>/<seq_id>_<src_frame>_<ref_frame>.npz without it (KITTI test.py:60-85)"""
+        if layout not in ('3dmatch', 'kitti'):
+            raise ValueError(f"layout must be '3dmatch' or 'kitti', got {layout!r}")
+        self.layout = layout
         self.cfg, self.output_dir, self.chunk = cfg, output_dir, max(1, int(chunk), int(batch_size) * int(num_streams))
         self.with_loss = bool(with_loss)
         self.with_ransac = bool(with_ransac)
@@ -43,10 +48,16 @@ class RegistrationTester:
 
     def after_test_step(self, data_dict, output_dict):
         """experiments/*/test.py:65-92"""
-        scene, ref_id, src_id = data_dict.get('scene_name', 'scene'), data_dict.get('ref_frame', 0), data_dict.get('src_frame', 1)
-        os.makedirs(os.path.join(self.output_dir, str(scene)), exist_ok=True)
+        ref_id, src_id = data_dict.get('ref_frame', 0), data_dict.get('src_frame', 1)
         arrays = {k: _np(output_dict[k]) for k in NPZ_OUTPUT_KEYS}
         arrays['transform'] = _np(data_dict['transform'])
+        if self.layout == 'kitti':
+            os.makedirs(self.output_dir, exist_ok=True)
+            path = os.path.join(self.output_dir, f"{data_dict.get('seq_id', 0)}_{src_id}_{ref_id}.npz")
+            np.savez_compressed(path, **arrays)
+            return path
+        scene = data_dict.get('scene_name', 'scene')
+        os.makedirs(os.path.join(self.output_dir, str(scene)), exist_ok=True)
         arrays['overlap'] = data_dict.get('overlap', np.float32('nan'))
         path = os.path.join(self.output_dir, str(scene), f'{ref_id}_{src_id}.npz')
         np.savez_compressed(path, **arrays)

@@ -426,6 +426,42 @@ int geob200_correspondence_metrics_batched(const float* ref_corr_points, const f
                                            const int32_t* num_corr, const float* transforms, int64_t transform_ld, float positive_radius,
                                            float* out, int64_t out_ld, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- benchmark evaluation (the experiments' eval.py; benchmark.cu) -------------------------------------------------------------
+ * Ragged pairs in the (B, capacity, .) layout with device int32 counts (NULL = all capacity rows), one launch for B pairs, no host
+ * sync; a pair gets the same bits alone and in any batch.
+ *
+ * Score order: order[p][0 .. min(n, kmax)) = np.argsort(-scores[p][:n], kind='stable')[:kmax] (score descending, then row
+ * ascending; -0 == +0; NaN after every number), -1 beyond.  kmax in 1..8192.  order: (B, kmax) int32. */
+int geob200_corr_order_batched(const float* scores, int64_t n_pairs, int64_t capacity, const int32_t* num_corr, int64_t kmax, int32_t* order,
+                               void* stream);
+/* Top-k selection as eval.py:125-129 does it: count_out[p] = min(n, k); row i of pair p in the (B, min(k, capacity), .) outputs is
+ * row order[p][i] when n > k and row i (the original order) when n <= k; zeros beyond the count.  order from
+ * geob200_corr_order_batched with the same kmax; k in 1..kmax. */
+int geob200_corr_select_batched(const float* ref_corr_points, const float* src_corr_points, const float* corr_scores, int64_t n_pairs,
+                                int64_t capacity, const int32_t* num_corr, const int32_t* order, int64_t kmax, int64_t k,
+                                float* ref_out, float* src_out, float* scores_out, int32_t* count_out, void* stream);
+/* evaluate_sparse_correspondences (utils/registration.py:253-281): out[p] = [precision, recall, hit_ratio] in double, equal to
+ * numpy's bit for bit.  Predicted pairs: rows [0, pred_count[p]) of (B, pred_cap) int64 ref / src node indices; gt pairs: rows
+ * [0, gt_count[p]) of (B, gt_cap, 2) int64.  Node indices are below m_cap (ref) / n_cap (src); pairs outside are ignored.  The gt
+ * and predicted sets are bitmaps: in shared memory when they fit, otherwise in the workspace (0 bytes when they fit). */
+size_t geob200_sparse_correspondence_eval_batched_workspace_bytes(int64_t n_pairs, int64_t m_cap, int64_t n_cap);
+int geob200_sparse_correspondence_eval_batched(const int64_t* ref_node_corr_indices, const int64_t* src_node_corr_indices, int64_t pred_cap,
+                                               const int32_t* pred_count, const int64_t* gt_node_corr_indices, int64_t gt_cap,
+                                               const int32_t* gt_count, int64_t n_pairs, int64_t m_cap, int64_t n_cap, double* out,
+                                               void* workspace, size_t workspace_bytes, void* stream);
+/* Registration error in double: out[p] = [rre (deg), rte, p, accepted] for the row-major 4x4 transforms at gt_transforms + p * gt_ld
+ * and est_transforms + p * est_ld.  p = compute_transform_error (threedmatch/utils.py:130-136: inv(gt) est, nibabel's mat2quat,
+ * er^T C er / C[0][0]) with the (B, 36) covariances where has_covariance[p] != 0 (NULL = every pair), NaN elsewhere.
+ * mode 0 (3DMatch): accepted = has a covariance and p < threshold0; mode 1 (KITTI): rre < threshold0 and rte < threshold1. */
+int geob200_registration_error_batched(const float* gt_transforms, int64_t gt_ld, const float* est_transforms, int64_t est_ld,
+                                       const float* covariances, const int32_t* has_covariance, int64_t n_pairs, int mode,
+                                       double threshold0, double threshold1, double* out, void* stream);
+/* geob200_weighted_procrustes over ragged problems: problem b = rows [0, counts[b]) of (batch, capacity, 3) src / ref and
+ * (batch, capacity) weights (may be NULL); bit-identical to geob200_weighted_procrustes on the trimmed rows. */
+int geob200_weighted_procrustes_counts(const float* src_points, const float* ref_points, const float* weights, int64_t batch,
+                                       int64_t capacity, const int32_t* counts, float weight_thresh, float eps, float* transforms,
+                                       void* stream);
+
 /* Profiling aid (bench.py roofline): while enabled, every tensor-core GEMM launch (nn.Linear and the KPConv contraction) is
  * bracketed by CUDA events on its stream; _read synchronises them and returns the count, shapes[3i..] = (m, n, k), ms[i]. */
 int geob200_linear_profile_enable(int on);
