@@ -45,28 +45,23 @@ _sig('geob200_group_norm_workspace_bytes', SZ, I64)
 _sig('geob200_group_norm', c_int, P, I64, I64, I64, P, P, F, P, c_int, F, P, P, SZ, P)
 _sig('geob200_fused_group_norm_workspace_bytes', SZ, I64, I64, I64)
 _sig('geob200_linear_group_norm', c_int, P, I64, P, P, I64, I64, I64, I64, P, P, F, P, c_int, F, P, P, P, SZ, P)
-_sig('geob200_kpconv_group_norm_workspace_bytes', SZ, I64, I64, I64, I64, I64)
 _sig('geob200_kpconv_group_norm', c_int, P, P, P, P, I64, I64, I64, P, I64, P, P, I64, I64, F, I64, P, P, F, c_int, F, P, P, P, SZ,
      P, SZ, P)
-_sig('geob200_group_norm_batched_workspace_bytes', SZ, I64, I64, I64, I64)
 _sig('geob200_group_norm_batched', c_int, P, I64, I64, I64, P, P, F, P, c_int, F, P, P, SZ, P, I64, P)
 _sig('geob200_linear_group_norm_batched', c_int, P, I64, P, P, I64, I64, I64, I64, P, P, F, P, c_int, F, P, P, P, SZ, P, I64, P)
 _sig('geob200_maxpool', c_int, P, P, I64, I64, I64, I64, P, P)
 _sig('geob200_upsample_concat', c_int, P, P, I64, I64, P, I64, I64, I64, P, P)
-_sig('geob200_point_to_node_partition', c_int, P, I64, P, I64, I64, P, P, P, P, P, P, P)
 _sig('geob200_point_to_node_partition_batched', c_int, P, P, I64, P, P, I64, P, P, P, P, P, P)
 _sig('geob200_gather_rows', c_int, P, I64, I64, P, I64, P, P)
 _sig('geob200_knn_partition', c_int, P, I64, P, I64, I64, P, P, P)
 _sig('geob200_pairwise_distance', c_int, P, I64, P, I64, I64, c_int, P, P)
 _sig('geob200_point_to_node_indices', c_int, P, I64, P, I64, P, P, P)
 _sig('geob200_apply_transform', c_int, P, I64, P, P, P)
-_sig('geob200_gse_indices', c_int, P, I64, F, F, I64, P, P, P)
 _sig('geob200_gse_indices_batched', c_int, P, I64, P, F, F, I64, P, P, P)
 _sig('geob200_gse_embed_workspace_bytes', SZ, I64, I64)
 _sig('geob200_gse_table_bytes', SZ, I64, I64, F, F)
 _sig('geob200_gse_table_build', c_int, P, P, P, P, P, I64, I64, F, F, P, SZ, P)
 _sig('geob200_gse_embed_table', c_int, P, P, I64, I64, P, SZ, I64, F, F, P, P, P, P, P, P, P)
-_sig('geob200_gse_embed', c_int, P, P, I64, I64, P, P, P, P, P, P, P, P, c_int, P, SZ, P)
 _sig('geob200_gse_embed_pairs', c_int, P, P, I64, I64, P, P, P, P, P, P, P, P, c_int, P, SZ, P)
 _sig('geob200_attention_workspace_bytes', SZ, I64, I64, I64)
 _sig('geob200_attention', c_int, P, I64, P, I64, P, I64, P, P, P, I64, I64, I64, I64, P, I64, P, SZ, P)
@@ -74,28 +69,18 @@ _sig('geob200_set_attention_tma', c_int, c_int)
 _sig('geob200_head_bias', c_int, P, I64, P, I64, I64, I64, P, P)
 _sig('geob200_add_layernorm', c_int, P, P, P, P, I64, I64, F, P, P)
 _sig('geob200_l2_normalize', c_int, P, I64, I64, P, P)
-_sig('geob200_superpoint_matching_workspace_bytes', SZ, I64, I64)
-_sig('geob200_superpoint_matching', c_int, P, P, I64, I64, I64, P, P, I64, c_int, P, P, P, P, P, SZ, P)
-_sig('geob200_gather_patches', c_int, P, I64, P, P, I64, P, I64, P, P, P, P)
-_sig('geob200_patch_scores', c_int, P, I64, P, I64, I64, P, P, I64, I64, P, P)
 _sig('geob200_sinkhorn', c_int, P, P, P, P, I64, I64, I64, F, P, P)
-_sig('geob200_lgr_workspace_bytes', SZ, I64, I64, I64)
-_sig('geob200_local_global_registration', c_int, P, P, P, P, P, I64, I64, I64, I64, F, c_int, F, I64, I64, P, P, P, P, P,
-     P, P, P, P, P, SZ, P)
 _sig('geob200_superpoint_matching_batched_workspace_bytes', SZ, I64, I64, I64)
-_sig('geob200_superpoint_matching_batched', c_int, P, I64, P, I64, P, I64, c_int, P, P, P, P, SZ, P)
+_sig('geob200_superpoint_matching_batched', c_int, P, P, I64, P, P, I64, P, I64, c_int, P, P, P, P, SZ, P)
 _sig('geob200_gather_patches_batched', c_int, P, I64, I64, P, P, P, P, I64, P, P, P, P, P)
-_sig('geob200_patch_scores_batched', c_int, P, I64, I64, P, P, P, I64, I64, P, P)
+_sig('geob200_patch_scores_batched', c_int, P, P, I64, I64, P, P, P, I64, I64, P, P)
 _sig('geob200_lgr_batched_workspace_bytes', SZ, I64, I64, I64, I64)
 _sig('geob200_local_global_registration_batched', c_int, P, P, P, P, P, I64, I64, I64, I64, I64, F, c_int, F, I64, I64, P, P, P, P,
      P, P, I64, P, P, P, P, SZ, P)
 _sig('geob200_weighted_procrustes', c_int, P, P, P, I64, I64, F, F, P, P)
 
-_sig('geob200_node_correspondences_workspace_bytes', SZ, I64, I64, I64)
-_sig('geob200_node_correspondences', c_int, P, P, P, P, P, P, P, P, I64, I64, I64, P, F, P, P, P, P, SZ, P)
 _sig('geob200_node_correspondences_batched_workspace_bytes', SZ, I64, I64, I64)
-_sig('geob200_node_correspondences_batched', c_int, P, P, P, P, I64, P, I64, P, F, P, P, P, P, SZ, P)
-_sig('geob200_evaluate', c_int, P, P, I64, F, P, P, I64, P, P, I64, F, P, P, P, I64, c_int, F, F, F, P, P)
+_sig('geob200_node_correspondences_batched', c_int, P, P, P, P, P, P, P, P, I64, P, I64, P, F, P, P, P, P, SZ, P)
 _sig('geob200_evaluate_counts', c_int, P, P, I64, P, F, P, P, I64, P, P, P, I64, P, F, P, P, P, I64, c_int, F, F, F, P, P)
 _sig('geob200_evaluate_batched', c_int, P, P, P, F, P, P, I64, P, P, P, I64, P, F, P, P, I64, P, I64, P, P, c_int, F, F, F, P, I64,
      P)
@@ -120,13 +105,8 @@ _sig('geob200_set_split_k', c_int, c_int)
 _sig('geob200_set_linear_persistent', c_int, c_int)
 _sig('geob200_linear_profile_read', I64, I64, P, P)
 _sig('geob200_backbone_workspace_bytes', SZ, P, P)
-_sig('geob200_backbone_forward', c_int, P, P, P, P, P, P, P, P, P, P, P, P, SZ, P, SZ, P)
-_sig('geob200_transformer_workspace_bytes', SZ, I64, I64, I64, I64, I64)
-_sig('geob200_transformer_forward', c_int, P, I64, I64, I64, P, I64, I64, P, P, P, P, SZ, P)
-_sig('geob200_backbone_gn_workspace_bytes', SZ, P, P, I64)
 _sig('geob200_backbone_forward_batched', c_int, P, P, P, P, P, P, P, P, P, P, P, P, SZ, P, SZ, P, I64, P, P)
 _sig('geob200_cloud_max_count', c_int, P, I64, I64, I64, I64, P, P, P)
-_sig('geob200_maxpool_batched', c_int, P, P, I64, I64, I64, I64, P, I64, P, P, P)
 _sig('geob200_transformer_batched_workspace_bytes', SZ, I64, P, I64, I64, I64)
 _sig('geob200_transformer_forward_batched', c_int, P, I64, I64, I64, P, I64, P, P, P, P, SZ, P)
 _sig('geob200_attention_batched_workspace_bytes', SZ, P, I64, I64)

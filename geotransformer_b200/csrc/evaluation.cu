@@ -22,20 +22,27 @@ __device__ __forceinline__ void xform(const float* T, float x, float y, float z,
 }
 
 // one warp per node: (optionally transformed) node, transformed patch points, enclosing radius over the valid patch points.
-// Cloud s = blockIdx.y (rows at cl.start[s] of every array); clouds s >= t_first are transformed by T + 16 * (s - t_first).
-__global__ void __launch_bounds__(256) nc_prepare_kernel(const float* __restrict__ nodes, const float* __restrict__ knn_pts,
-                                                         const unsigned char* __restrict__ knn_masks, const __grid_constant__ Segs cl, int K,
-                                                         const float* __restrict__ T, int t_first, float* __restrict__ nodes_out,
+// Cloud s = blockIdx.y; clouds s < B are the ref clouds (inputs from the ref_* block at cl.start[s]), the others the src clouds (inputs
+// from the src_* block, which starts at cloud B), transformed by T + 16 * (s - B).  Outputs are stacked at cl.start[s].
+__global__ void __launch_bounds__(256) nc_prepare_kernel(const float* __restrict__ ref_nodes, const float* __restrict__ src_nodes,
+                                                         const float* __restrict__ ref_knn_pts, const float* __restrict__ src_knn_pts,
+                                                         const unsigned char* __restrict__ ref_knn_masks,
+                                                         const unsigned char* __restrict__ src_knn_masks, const __grid_constant__ Segs cl,
+                                                         int B, int K, const float* __restrict__ T, float* __restrict__ nodes_out,
                                                          float* __restrict__ pts_out, float* __restrict__ max_dist, int* __restrict__ n_valid) {
     const int lane = threadIdx.x & 31;
     const int s = blockIdx.y;
     const int m = blockIdx.x * 8 + (threadIdx.x >> 5);
     if (m >= cl.count[s]) return;
+    const bool src = s >= B;
+    const float* __restrict__ nodes = src ? src_nodes : ref_nodes;
+    const float* __restrict__ knn_pts = src ? src_knn_pts : ref_knn_pts;
+    const unsigned char* __restrict__ knn_masks = src ? src_knn_masks : ref_knn_masks;
     {
-        const long long r = cl.start[s];
-        nodes += 3 * r; nodes_out += 3 * r; knn_pts += 3 * r * K; pts_out += 3 * r * K; max_dist += r; n_valid += r;
-        if (knn_masks != nullptr) knn_masks += r * K;
-        T = (T != nullptr && s >= t_first) ? T + 16 * (s - t_first) : nullptr;
+        const long long r = cl.start[s], r_in = src ? r - cl.start[B] : r;
+        nodes += 3 * r_in; knn_pts += 3 * r_in * K; nodes_out += 3 * r; pts_out += 3 * r * K; max_dist += r; n_valid += r;
+        if (knn_masks != nullptr) knn_masks += r_in * K;
+        T = (T != nullptr && src) ? T + 16 * (s - B) : nullptr;
     }
     float nx = nodes[3 * m], ny = nodes[3 * m + 1], nz = nodes[3 * m + 2];
     if (T != nullptr) xform(T, nx, ny, nz, nx, ny, nz);
@@ -528,75 +535,27 @@ using namespace geob200;
 
 extern "C" {
 
-size_t geob200_node_correspondences_workspace_bytes(int64_t n_ref, int64_t n_src, int64_t k) {
-    const size_t m = (size_t)n_ref, n = (size_t)n_src, kk = (size_t)k;
-    return align_up(12 * m, 256) + align_up(12 * n, 256) + align_up(12 * m * kk, 256) + align_up(12 * n * kk, 256) + 2 * align_up(4 * m, 256) +
-           2 * align_up(4 * n, 256) + align_up(4 * m * n, 256) + 256;
-}
-
 size_t geob200_node_correspondences_batched_workspace_bytes(int64_t n_rows, int64_t n_products, int64_t k) {
-    return geob200_node_correspondences_workspace_bytes(n_rows, 0, k) + align_up(4 * (size_t)n_products, 256);
+    const size_t r = (size_t)n_rows;
+    return align_up(12 * r, 256) + align_up(12 * r * (size_t)k, 256) + 2 * align_up(4 * r, 256) + align_up(4 * (size_t)n_products, 256) + 256;
 }
 
-static int nc_overlap_compact(const float* rn, const float* sn, const float* rp, const float* sp, const uint8_t* ref_knn_masks,
-                              const uint8_t* src_knn_masks, const uint8_t* ref_masks, const uint8_t* src_masks, const float* rmax,
-                              const float* smax, const int* rnv, const int* snv, const Segs& R, const Segs& Q, int64_t k, float pos_radius,
-                              float* overlap, int64_t* corr_indices, float* corr_overlaps, int32_t* count, cudaStream_t st) {
-    Segs NN;
-    if (segs_products(&NN, R, Q)) return -1;
-    const size_t smem = (size_t)k * (2 * sizeof(float4) + 2 * sizeof(int));
-    if (R.max > 0)
-        nc_overlap_kernel<<<dim3((unsigned)R.max, R.n), 256, smem, st>>>(rn, sn, rp, sp, ref_knn_masks, src_knn_masks, ref_masks, src_masks,
-                                                                        rmax, smax, rnv, snv, R, Q, NN, (int)k, pos_radius, overlap);
-    nc_compact_kernel<<<R.n, 1024, 0, st>>>(overlap, R, Q, NN, (long long*)corr_indices, corr_overlaps, count);
-    GEOB_CHECK_LAUNCH();
-    count_launches(2);
-    return 0;
-}
-
-// corr_indices (n_ref*n_src, 2) int64 capacity, corr_overlaps (n_ref*n_src) capacity; *count = rows written (row-major order)
-int geob200_node_correspondences(const float* ref_nodes, const float* src_nodes, const float* ref_knn_points, const float* src_knn_points,
-                                 const uint8_t* ref_masks, const uint8_t* src_masks, const uint8_t* ref_knn_masks,
-                                 const uint8_t* src_knn_masks, int64_t n_ref, int64_t n_src, int64_t k, const float* transform,
-                                 float pos_radius, int64_t* corr_indices, float* corr_overlaps, int32_t* count, void* workspace,
-                                 size_t workspace_bytes, void* stream) {
-    cudaStream_t st = (cudaStream_t)stream;
-    GEOB_REQUIRE(n_ref > 0 && n_src > 0 && k > 0 && k <= 1024, "node_correspondences: bad shape");
-    GEOB_REQUIRE(workspace_bytes >= geob200_node_correspondences_workspace_bytes(n_ref, n_src, k), "node_correspondences: workspace too small");
-    Arena ar(workspace, workspace_bytes);
-    float* rn = ar.take<float>(3 * n_ref);
-    float* sn = ar.take<float>(3 * n_src);
-    float* rp = ar.take<float>(3 * n_ref * k);
-    float* sp = ar.take<float>(3 * n_src * k);
-    float* rmax = ar.take<float>(n_ref);
-    float* smax = ar.take<float>(n_src);
-    int* rnv = ar.take<int>(n_ref);
-    int* snv = ar.take<int>(n_src);
-    float* overlap = ar.take<float>((size_t)n_ref * n_src);
-    GEOB_REQUIRE(ar.ok(), "node_correspondences: workspace accounting error");
-    const Segs R = segs_one(n_ref), Q = segs_one(n_src);
-    nc_prepare_kernel<<<dim3((unsigned)((n_ref + 7) / 8), 1), 256, 0, st>>>(ref_nodes, ref_knn_points, ref_knn_masks, R, (int)k, nullptr, 0,
-                                                                          rn, rp, rmax, rnv);
-    nc_prepare_kernel<<<dim3((unsigned)((n_src + 7) / 8), 1), 256, 0, st>>>(src_nodes, src_knn_points, src_knn_masks, Q, (int)k, transform, 0,
-                                                                          sn, sp, smax, snv);
-    count_launches(2);
-    return nc_overlap_compact(rn, sn, rp, sp, ref_knn_masks, src_knn_masks, ref_masks, src_masks, rmax, smax, rnv, snv, R, Q, k, pos_radius,
-                              overlap, corr_indices, corr_overlaps, count, st);
-}
-
-int geob200_node_correspondences_batched(const float* nodes, const float* knn_points, const uint8_t* node_masks, const uint8_t* knn_masks,
-                                         int64_t n_pairs, const int64_t* cloud_nodes, int64_t k, const float* transforms, float pos_radius,
-                                         int64_t* corr_indices, float* corr_overlaps, int32_t* count, void* workspace, size_t workspace_bytes,
-                                         void* stream) {
+int geob200_node_correspondences_batched(const float* ref_nodes, const float* src_nodes, const float* ref_knn_points,
+                                         const float* src_knn_points, const uint8_t* ref_masks, const uint8_t* src_masks,
+                                         const uint8_t* ref_knn_masks, const uint8_t* src_knn_masks, int64_t n_pairs, const int64_t* cloud_nodes,
+                                         int64_t k, const float* transforms, float pos_radius, int64_t* corr_indices, float* corr_overlaps,
+                                         int32_t* count, void* workspace, size_t workspace_bytes, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     GEOB_REQUIRE(n_pairs > 0 && 2 * n_pairs <= GEOB_MAX_CLOUDS, "node_correspondences_batched: 1..%d pairs", GEOB_MAX_CLOUDS / 2);
     GEOB_REQUIRE(k > 0 && k <= 1024, "node_correspondences: bad shape");
-    Segs cl, NN;
-    if (segs_from_counts(&cl, 2 * n_pairs, cloud_nodes)) return -1;
     const int B = (int)n_pairs;
-    const Segs R = segs_range(cl, 0, B), Q = segs_range(cl, B, B);
+    // cl: all 2B clouds stacked (the workspace rows); R / Q: the ref / src clouds in the row spaces of the ref_* / src_* inputs
+    Segs cl, Q, NN;
+    if (segs_from_counts(&cl, 2 * n_pairs, cloud_nodes) || segs_from_counts(&Q, n_pairs, cloud_nodes + n_pairs)) return -1;
+    const Segs R = segs_range(cl, 0, B);
+    const int64_t ref_rows = cl.start[B], rows = (int64_t)cl.start[2 * B - 1] + cl.count[2 * B - 1];
+    GEOB_REQUIRE(ref_rows > 0 && rows > ref_rows, "node_correspondences: bad shape");
     if (segs_products(&NN, R, Q)) return -1;
-    const int64_t rows = (int64_t)cl.start[2 * B - 1] + cl.count[2 * B - 1];
     const int64_t nn = (int64_t)NN.start[B - 1] + NN.count[B - 1];
     GEOB_REQUIRE(workspace_bytes >= geob200_node_correspondences_batched_workspace_bytes(rows, nn, k),
                  "node_correspondences_batched: workspace too small");
@@ -608,10 +567,16 @@ int geob200_node_correspondences_batched(const float* nodes, const float* knn_po
     float* overlap = ar.take<float>(nn);
     GEOB_REQUIRE(ar.ok(), "node_correspondences: workspace accounting error");
     nc_prepare_kernel<<<dim3((unsigned)((cl.max + 7) / 8 > 0 ? (cl.max + 7) / 8 : 1), 2 * B), 256, 0, st>>>(
-        nodes, knn_points, knn_masks, cl, (int)k, transforms, B, cn, cp, cmax, cnv);
-    count_launches(1);
-    return nc_overlap_compact(cn, cn, cp, cp, knn_masks, knn_masks, node_masks, node_masks, cmax, cmax, cnv, cnv, R, Q, k, pos_radius,
-                              overlap, corr_indices, corr_overlaps, count, st);
+        ref_nodes, src_nodes, ref_knn_points, src_knn_points, ref_knn_masks, src_knn_masks, cl, B, (int)k, transforms, cn, cp, cmax, cnv);
+    const size_t smem = (size_t)k * (2 * sizeof(float4) + 2 * sizeof(int));
+    if (R.max > 0)
+        nc_overlap_kernel<<<dim3((unsigned)R.max, B), 256, smem, st>>>(cn, cn + 3 * ref_rows, cp, cp + 3 * ref_rows * k, ref_knn_masks,
+                                                                      src_knn_masks, ref_masks, src_masks, cmax, cmax + ref_rows, cnv,
+                                                                      cnv + ref_rows, R, Q, NN, (int)k, pos_radius, overlap);
+    nc_compact_kernel<<<B, 1024, 0, st>>>(overlap, R, Q, NN, (long long*)corr_indices, corr_overlaps, count);
+    GEOB_CHECK_LAUNCH();
+    count_launches(3);
+    return 0;
 }
 
 static int evaluate_impl(const int64_t* gt_idx, const float* gt_ov, const Segs& G, const int32_t* n_gt_dev, float acceptance_overlap,
@@ -628,17 +593,6 @@ static int evaluate_impl(const int64_t* gt_idx, const float* gt_ov, const Segs& 
     GEOB_CHECK_LAUNCH();
     count_launches(1);
     return 0;
-}
-
-int geob200_evaluate(const int64_t* gt_node_corr_indices, const float* gt_node_corr_overlaps, int64_t n_gt, float acceptance_overlap,
-                     const int64_t* ref_node_corr_indices, const int64_t* src_node_corr_indices, int64_t n_node_corr,
-                     const float* ref_corr_points, const float* src_corr_points, int64_t n_corr, float acceptance_radius,
-                     const float* gt_transform, const float* est_transform, const float* src_points, int64_t n_src_points, int mode,
-                     float rmse_threshold, float rre_threshold, float rte_threshold, float* metrics, void* stream) {
-    return geob200_evaluate_counts(gt_node_corr_indices, gt_node_corr_overlaps, n_gt, nullptr, acceptance_overlap, ref_node_corr_indices,
-                                   src_node_corr_indices, n_node_corr, nullptr, ref_corr_points, src_corr_points, n_corr, nullptr,
-                                   acceptance_radius, gt_transform, est_transform, src_points, n_src_points, mode, rmse_threshold,
-                                   rre_threshold, rte_threshold, metrics, stream);
 }
 
 int geob200_evaluate_counts(const int64_t* gt_node_corr_indices, const float* gt_node_corr_overlaps, int64_t n_gt, const int32_t* n_gt_dev,

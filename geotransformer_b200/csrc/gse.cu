@@ -8,7 +8,7 @@
 // E (N,N,C) is written: the O(N^2 k C) intermediate never exists.
 //
 // This file holds the index kernel and the fp32 CUDA-core contraction (exact-fp32 reference path).  The
-// wgmma tensor-core contraction lives in gse_tc.cu and is selected by geob200_structure_embedding().
+// wgmma tensor-core contraction lives in gse_tc.cu and is selected by geob200_gse_embed_pairs().
 #include "common.cuh"
 #include "geob200.h"
 
@@ -26,22 +26,20 @@ __device__ __forceinline__ float dist_mm(float ax, float ay, float az, float a2,
 // then the k triplet angles for every j.  d_idx (N,N), a_idx (N,N,KA).
 // Clouds of a batch (blockIdx.y = cloud): stacked points, d / a outputs concatenated cloud after cloud (cloud c at pair_start[c]).
 struct GseClouds {
-    int n_clouds;
     int row_start[GEOB_MAX_CLOUDS + 1];
     long long pair_start[GEOB_MAX_CLOUDS + 1];
 };
 
 template <int KA>
-__global__ void __launch_bounds__(256) gse_indices_kernel(const float* __restrict__ pts_all, int N_single, float sigma_d, float factor_a,
+__global__ void __launch_bounds__(256) gse_indices_kernel(const float* __restrict__ pts_all, float sigma_d, float factor_a,
                                                           float* __restrict__ d_all, float* __restrict__ a_all,
                                                           const __grid_constant__ GseClouds cl) {
     extern __shared__ float4 ps[];     // (x,y,z,|p|^2)
-    // single cloud (n_clouds == 0): the arguments describe it; batch: cloud blockIdx.y of the descriptor
     const int cloud = blockIdx.y;
-    const int N = cl.n_clouds > 0 ? cl.row_start[cloud + 1] - cl.row_start[cloud] : N_single;
-    const float* __restrict__ pts = cl.n_clouds > 0 ? pts_all + 3ll * cl.row_start[cloud] : pts_all;
-    float* __restrict__ d_idx = cl.n_clouds > 0 ? d_all + cl.pair_start[cloud] : d_all;
-    float* __restrict__ a_idx = cl.n_clouds > 0 ? a_all + cl.pair_start[cloud] * KA : a_all;
+    const int N = cl.row_start[cloud + 1] - cl.row_start[cloud];
+    const float* __restrict__ pts = pts_all + 3ll * cl.row_start[cloud];
+    float* __restrict__ d_idx = d_all + cl.pair_start[cloud];
+    float* __restrict__ a_idx = a_all + cl.pair_start[cloud] * KA;
     if ((int)(blockIdx.x * (blockDim.x >> 5)) >= N) return;          // grid.x covers the largest cloud
     for (int n = threadIdx.x; n < N; n += blockDim.x) {
         const float x = pts[3 * n], y = pts[3 * n + 1], z = pts[3 * n + 2];
@@ -257,28 +255,12 @@ int geob200_gse_embed_tc(const float* d_idx, const float* a_idx, long long n_pai
 
 extern "C" {
 
-int geob200_gse_indices(const float* points, int64_t n, float sigma_d, float factor_a, int64_t angle_k, float* d_indices,
-                        float* a_indices, void* stream) {
-    cudaStream_t st = (cudaStream_t)stream;
-    GEOB_REQUIRE(n > 0, "gse_indices: empty cloud");
-    GEOB_REQUIRE(angle_k == 3, "gse_indices: angle_k=%lld unsupported (all shipped models use 3)", (long long)angle_k);
-    GEOB_REQUIRE(n * 16 <= 200 * 1024, "gse_indices: too many superpoints (%lld)", (long long)n);
-    const size_t smem = sizeof(float4) * n;
-    if (smem > 48 * 1024 && ensure_max_smem((const void*)gse_indices_kernel<3>)) return -1;
-    GseClouds none{};
-    gse_indices_kernel<3><<<(unsigned)((n + 7) / 8), 256, smem, st>>>(points, (int)n, sigma_d, factor_a, d_indices, a_indices, none);
-    GEOB_CHECK_LAUNCH();
-    count_launches(1);
-    return 0;
-}
-
 int geob200_gse_indices_batched(const float* points, int64_t n_clouds, const int64_t* cloud_rows_h, float sigma_d, float factor_a,
                                 int64_t angle_k, float* d_indices, float* a_indices, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     GEOB_REQUIRE(n_clouds >= 1 && n_clouds <= GEOB_MAX_CLOUDS, "gse_indices: 1..%d clouds per launch", GEOB_MAX_CLOUDS);
     GEOB_REQUIRE(angle_k == 3, "gse_indices: angle_k=%lld unsupported (all shipped models use 3)", (long long)angle_k);
     GseClouds cl{};
-    cl.n_clouds = (int)n_clouds;
     int64_t max_n = 0;
     for (int64_t c = 0; c < n_clouds; ++c) {
         const int64_t n = cloud_rows_h[c];
@@ -291,7 +273,7 @@ int geob200_gse_indices_batched(const float* points, int64_t n_clouds, const int
     const size_t smem = sizeof(float4) * max_n;
     if (smem > 48 * 1024 && ensure_max_smem((const void*)gse_indices_kernel<3>)) return -1;
     const dim3 grid((unsigned)((max_n + 7) / 8), (unsigned)n_clouds);
-    gse_indices_kernel<3><<<grid, 256, smem, st>>>(points, 0, sigma_d, factor_a, d_indices, a_indices, cl);
+    gse_indices_kernel<3><<<grid, 256, smem, st>>>(points, sigma_d, factor_a, d_indices, a_indices, cl);
     GEOB_CHECK_LAUNCH();
     count_launches(1);
     return 0;
@@ -304,14 +286,6 @@ size_t geob200_gse_embed_workspace_bytes(int64_t n, int64_t channels) {
 
 // mode: 0 = fp32 CUDA cores (exact-fp32 accumulation), 1 = wgmma 3xTF32 (fp32-accurate), 2 = wgmma 1xTF32,
 //       3 = wgmma 3xFP16 (fp32-accurate, half the tensor-pipe time of 3xTF32; default)
-int geob200_gse_embed(const float* d_indices, const float* a_indices, int64_t n, int64_t channels, const float* div_term,
-                      const float* wd_t, const float* wa_t, const float* wd, const float* wa, const float* bd, const float* ba,
-                      float* embeddings, int mode, void* workspace, size_t workspace_bytes, void* stream) {
-    GEOB_REQUIRE(n > 0, "gse_embed: bad shape");
-    return geob200_gse_embed_pairs(d_indices, a_indices, n * n, channels, div_term, wd_t, wa_t, wd, wa, bd, ba, embeddings, mode, workspace,
-                                   workspace_bytes, stream);
-}
-
 int geob200_gse_embed_pairs(const float* d_indices, const float* a_indices, int64_t n_rows, int64_t channels, const float* div_term,
                             const float* wd_t, const float* wa_t, const float* wd, const float* wa, const float* bd, const float* ba,
                             float* embeddings, int mode, void* workspace, size_t workspace_bytes, void* stream) {

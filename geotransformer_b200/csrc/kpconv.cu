@@ -1210,11 +1210,6 @@ int linear_group_norm_impl(const float* x, int64_t ldx, const float* weight, con
 extern "C" {
 
 // KPConv (gather + tensor-core GEMM) -> GroupNorm (+ LeakyReLU): ConvBlock / the conv part of ResidualBlock (modules.py:107-147,205-207)
-size_t geob200_kpconv_group_norm_workspace_bytes(int64_t n_query, int64_t n_support, int64_t c_in, int64_t c_out, int64_t groups) {
-    return align_up(geob200_fused_group_norm_workspace_bytes(n_query, c_out, groups), 256) +
-           geob200_kpconv_tc_workspace_bytes(n_query, n_support, c_in);
-}
-
 int geob200_kpconv_group_norm(const float* s_feats, const float* q_points, const float* s_points, const int64_t* neighbors,
                               int64_t n_query, int64_t n_support, int64_t n_neighbors, const float* kernel_points, int64_t n_kernel,
                               const float* weights_t, const float* bias, int64_t c_in, int64_t c_out, float sigma, int64_t groups,
@@ -1288,10 +1283,6 @@ static int make_seg(GnSeg* g, int64_t n_pairs, const int64_t* cloud_rows_h, int6
 
 extern "C" {
 
-size_t geob200_group_norm_batched_workspace_bytes(int64_t n_rows, int64_t channels, int64_t groups, int64_t n_pairs) {
-    return geob200::fused_group_norm_workspace_bytes_batched(n_rows, channels, groups, n_pairs);
-}
-
 int geob200_group_norm_batched(const float* x, int64_t n_rows, int64_t channels, int64_t groups, const float* gamma, const float* beta,
                                float eps, const float* residual, int leaky, float slope, float* y, void* workspace, size_t workspace_bytes,
                                void* stream, int64_t n_pairs, const int64_t* cloud_rows_h) {
@@ -1321,14 +1312,6 @@ int geob200_cloud_max_count(const int64_t* neighbors, int64_t n_query, int64_t n
     GEOB_CHECK_LAUNCH();
     geob200::count_launches(1);
     return 0;
-}
-
-int geob200_maxpool_batched(const float* x, const int64_t* neighbors, int64_t n_query, int64_t n_support, int64_t n_neighbors,
-                            int64_t channels, float* y, int64_t n_pairs, const int64_t* cloud_rows_h, const int32_t* cloud_max,
-                            void* stream) {
-    geob200::GnSeg seg;
-    if (geob200::make_seg(&seg, n_pairs, cloud_rows_h, n_query)) return -2;
-    return geob200::maxpool_seg(x, neighbors, n_query, n_support, n_neighbors, channels, y, &seg, cloud_max, stream);
 }
 
 }  // extern "C"

@@ -390,22 +390,25 @@ using namespace geob200;
 
 extern "C" {
 
-size_t geob200_lgr_workspace_bytes(int64_t n_patches, int64_t k, int64_t topk) {
-    size_t P = (size_t)n_patches, cap = (size_t)(k * topk * 2);
+size_t geob200_lgr_batched_workspace_bytes(int64_t n_pairs, int64_t n_patches, int64_t k, int64_t topk) {
+    const size_t P = (size_t)(n_pairs * (n_patches + 1)), cap = (size_t)(k * topk * 2);
     return align_up(4 * (P + 1), 256) * 4 + align_up(4 * P * cap, 256) * 2 + align_up(64 * P, 256) + 4096;
 }
 
-size_t geob200_lgr_batched_workspace_bytes(int64_t n_pairs, int64_t n_patches, int64_t k, int64_t topk) {
-    return geob200_lgr_workspace_bytes(n_pairs * (n_patches + 1), k, topk);
-}
-
-// B pairs of P patches each, patches of pair b at b * P; outputs of pair b at b * (its capacity), transform at b * transform_ld
-static int lgr_impl(const float* ref_knn_points, const float* src_knn_points, const uint8_t* ref_knn_masks, const uint8_t* src_knn_masks,
-                    const float* log_scores, int B, int P, int64_t k, int64_t score_ld, int64_t topk, float acceptance_radius, int mutual,
-                    float confidence_threshold, int64_t correspondence_threshold, int64_t num_refinement_steps, float* ref_corr_points,
-                    float* src_corr_points, float* corr_scores, int32_t* corr_patch, int32_t* num_corr, float* estimated_transform,
-                    int64_t transform_ld, float* patch_transforms, int32_t* patch_inliers, int32_t* best_patch, void* workspace,
-                    size_t workspace_bytes, cudaStream_t st) {
+// B pairs of P patches each, patches of pair b at b * P; outputs of pair b at b * (its capacity), transform at b * transform_ld.
+// Correspondence outputs have capacity P*k*topk rows per pair (x2 when not mutual); num_corr[b] (device int32) = rows written.
+int geob200_local_global_registration_batched(const float* ref_knn_points, const float* src_knn_points, const uint8_t* ref_knn_masks,
+                                              const uint8_t* src_knn_masks, const float* log_scores, int64_t n_pairs, int64_t n_patches,
+                                              int64_t k, int64_t score_ld, int64_t topk, float acceptance_radius, int mutual,
+                                              float confidence_threshold, int64_t correspondence_threshold, int64_t num_refinement_steps,
+                                              float* ref_corr_points, float* src_corr_points, float* corr_scores, int32_t* corr_patch,
+                                              int32_t* num_corr, float* estimated_transform, int64_t transform_ld, float* patch_transforms,
+                                              int32_t* patch_inliers, int32_t* best_patch, void* workspace, size_t workspace_bytes,
+                                              void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    GEOB_REQUIRE(n_pairs > 0 && n_pairs <= GEOB_MAX_CLOUDS / 2, "lgr_batched: 1..%d pairs", GEOB_MAX_CLOUDS / 2);
+    GEOB_REQUIRE(workspace_bytes >= geob200_lgr_batched_workspace_bytes(n_pairs, n_patches, k, topk), "lgr_batched: workspace too small");
+    const int B = (int)n_pairs, P = (int)n_patches;
     GEOB_REQUIRE(P > 0 && k > 0 && k <= 256, "lgr: bad patch shape");
     GEOB_REQUIRE(topk >= 1 && topk <= 4, "lgr: topk must be in 1..4");
     GEOB_REQUIRE(score_ld == k || score_ld == k + 1, "lgr: score matrix must be (P,K,K) or (P,K+1,K+1)");
@@ -442,37 +445,6 @@ static int lgr_impl(const float* ref_knn_points, const float* src_knn_points, co
     GEOB_CHECK_LAUNCH();
     count_launches(6);
     return 0;
-}
-
-// Outputs have capacity n_patches*k*topk rows; *num_corr (device int32) receives the number actually written.
-int geob200_local_global_registration(const float* ref_knn_points, const float* src_knn_points, const uint8_t* ref_knn_masks,
-                                      const uint8_t* src_knn_masks, const float* log_scores, int64_t n_patches, int64_t k,
-                                      int64_t score_ld, int64_t topk, float acceptance_radius, int mutual,
-                                      float confidence_threshold, int64_t correspondence_threshold, int64_t num_refinement_steps,
-                                      float* ref_corr_points, float* src_corr_points, float* corr_scores, int32_t* corr_patch,
-                                      int32_t* num_corr, float* estimated_transform, float* patch_transforms, int32_t* patch_inliers,
-                                      int32_t* best_patch, void* workspace, size_t workspace_bytes, void* stream) {
-    GEOB_REQUIRE(workspace_bytes >= geob200_lgr_workspace_bytes(n_patches, k, topk), "lgr: workspace too small");
-    return lgr_impl(ref_knn_points, src_knn_points, ref_knn_masks, src_knn_masks, log_scores, 1, (int)n_patches, k, score_ld, topk,
-                    acceptance_radius, mutual, confidence_threshold, correspondence_threshold, num_refinement_steps, ref_corr_points,
-                    src_corr_points, corr_scores, corr_patch, num_corr, estimated_transform, 16, patch_transforms, patch_inliers, best_patch,
-                    workspace, workspace_bytes, (cudaStream_t)stream);
-}
-
-int geob200_local_global_registration_batched(const float* ref_knn_points, const float* src_knn_points, const uint8_t* ref_knn_masks,
-                                              const uint8_t* src_knn_masks, const float* log_scores, int64_t n_pairs, int64_t n_patches,
-                                              int64_t k, int64_t score_ld, int64_t topk, float acceptance_radius, int mutual,
-                                              float confidence_threshold, int64_t correspondence_threshold, int64_t num_refinement_steps,
-                                              float* ref_corr_points, float* src_corr_points, float* corr_scores, int32_t* corr_patch,
-                                              int32_t* num_corr, float* estimated_transform, int64_t transform_ld, float* patch_transforms,
-                                              int32_t* patch_inliers, int32_t* best_patch, void* workspace, size_t workspace_bytes,
-                                              void* stream) {
-    GEOB_REQUIRE(n_pairs > 0 && n_pairs <= GEOB_MAX_CLOUDS / 2, "lgr_batched: 1..%d pairs", GEOB_MAX_CLOUDS / 2);
-    GEOB_REQUIRE(workspace_bytes >= geob200_lgr_batched_workspace_bytes(n_pairs, n_patches, k, topk), "lgr_batched: workspace too small");
-    return lgr_impl(ref_knn_points, src_knn_points, ref_knn_masks, src_knn_masks, log_scores, (int)n_pairs, (int)n_patches, k, score_ld,
-                    topk, acceptance_radius, mutual, confidence_threshold, correspondence_threshold, num_refinement_steps, ref_corr_points,
-                    src_corr_points, corr_scores, corr_patch, num_corr, estimated_transform, transform_ld, patch_transforms, patch_inliers,
-                    best_patch, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 int geob200_weighted_procrustes(const float* src_points, const float* ref_points, const float* weights, int64_t batch,

@@ -54,11 +54,15 @@ int segs_products(Segs* s, const Segs& ref, const Segs& src) {
 
 // ---- superpoint matching ---------------------------------------------------------------------------------
 
-// valid (non-empty) node lists, in index order (torch.nonzero): one CTA per cloud, chunked ordered compaction
-__global__ void __launch_bounds__(1024) compact_masks_kernel(const unsigned char* __restrict__ masks, const __grid_constant__ Segs cl,
-                                                             int* __restrict__ idx, int* __restrict__ count) {
+// valid (non-empty) node lists, in index order (torch.nonzero): one CTA per cloud, chunked ordered compaction.  Clouds s < B are
+// the ref clouds, read from ref_masks at cl.start[s]; the others from src_masks, whose block starts at cloud B.  NULL masks = all
+// valid.  idx / count are stacked over all 2B clouds.
+__global__ void __launch_bounds__(1024) compact_masks_kernel(const unsigned char* __restrict__ ref_masks,
+                                                             const unsigned char* __restrict__ src_masks, const __grid_constant__ Segs cl,
+                                                             int B, int* __restrict__ idx, int* __restrict__ count) {
     const int s = blockIdx.y;
-    masks += cl.start[s];
+    const unsigned char* __restrict__ masks = s < B ? ref_masks : src_masks;
+    if (masks != nullptr) masks += s < B ? cl.start[s] : cl.start[s] - cl.start[B];
     idx += cl.start[s];
     count += s;
     const int n = cl.count[s];
@@ -69,7 +73,7 @@ __global__ void __launch_bounds__(1024) compact_masks_kernel(const unsigned char
     __syncthreads();
     for (int base = 0; base < n; base += 1024) {
         const int i = base + threadIdx.x;
-        const int f = (i < n && masks[i]) ? 1 : 0;
+        const int f = (i < n && (masks == nullptr || masks[i])) ? 1 : 0;
         const unsigned bal = __ballot_sync(0xffffffffu, f);
         const int pre = __popc(bal & ((1u << lane) - 1u));
         if (lane == 0) warp_tot[warp] = __popc(bal);
@@ -545,102 +549,51 @@ using namespace geob200;
 
 extern "C" {
 
-size_t geob200_superpoint_matching_workspace_bytes(int64_t n_ref, int64_t n_src) {
-    size_t nr = (size_t)n_ref, ns = (size_t)n_src;
-    return align_up(4 * nr, 256) * 2 + align_up(4 * ns, 256) * 2 + align_up(4 * nr * ns, 256) * 2 + 1024 + 4096;
-}
-
 size_t geob200_superpoint_matching_batched_workspace_bytes(int64_t n_rows, int64_t n_products, int64_t n_pairs) {
     const size_t r = (size_t)n_rows, nn = (size_t)n_products;
     return align_up(4 * r, 256) * 3 + align_up(4 * nn, 256) * 2 + align_up(8 * (size_t)n_pairs, 256) + 4096;
 }
 
-// R / Q: the pairs' ref / src clouds in the row space of ref_feats / src_feats; ref rows of ridx / rowsum at R.start, src rows of
-// sidx / colsum at Q.start; counts[p] / counts[B + p] = valid ref / src nodes of pair p
-static int superpoint_matching_impl(const float* ref_feats, const float* src_feats, int64_t channels, const Segs& R, const Segs& Q,
-                                    const int* ridx, const int* sidx, const int* counts, float* rowsum, float* colsum, float* S, float* flat,
-                                    int64_t num_correspondences, int dual, int64_t* ref_corr_indices, int64_t* src_corr_indices,
-                                    float* corr_scores, int32_t* num_out, cudaStream_t st) {
-    const int B = R.n;
-    Segs NN;
-    if (segs_products(&NN, R, Q)) return -1;
-    const size_t smem = sizeof(float) * (channels + Q.max);
-    GEOB_REQUIRE(smem <= 48 * 1024, "superpoint_matching: row does not fit shared memory");
-    const dim3 g_rows((unsigned)(R.max > 0 ? R.max : 1), B), g_cols((unsigned)((Q.max + 255) / 256 > 0 ? (Q.max + 255) / 256 : 1), B),
-        g_nn((unsigned)((NN.max + 255) / 256 > 0 ? (NN.max + 255) / 256 : 1), B);
-    spm_scores_kernel<<<g_rows, 256, smem, st>>>(ref_feats, src_feats, (int)channels, ridx, counts, sidx, counts + B, R, Q, NN, S, rowsum);
-    spm_colsum_kernel<<<g_cols, 256, 0, st>>>(S, counts, counts + B, Q, NN, colsum);
-    spm_dual_kernel<<<g_nn, 256, 0, st>>>(S, counts, counts + B, rowsum, colsum, R, Q, NN, dual, flat);
-    topk_flat_kernel<1024><<<dim3(1, B), 1024, 0, st>>>(flat, counts, counts + B, (int)num_correspondences, ridx, sidx, R, Q, NN,
-                                                        (long long*)ref_corr_indices, (long long*)src_corr_indices, corr_scores, num_out);
-    GEOB_CHECK_LAUNCH();
-    count_launches(4);
-    return 0;
-}
-
-int geob200_superpoint_matching(const float* ref_feats, const float* src_feats, int64_t n_ref, int64_t n_src, int64_t channels,
-                                const uint8_t* ref_masks, const uint8_t* src_masks, int64_t num_correspondences, int dual,
-                                int64_t* ref_corr_indices, int64_t* src_corr_indices, float* corr_scores, int32_t* num_out,
-                                void* workspace, size_t workspace_bytes, void* stream) {
-    cudaStream_t st = (cudaStream_t)stream;
-    GEOB_REQUIRE(n_ref > 0 && n_src > 0, "superpoint_matching: empty input");
-    GEOB_REQUIRE(num_correspondences <= 1024, "superpoint_matching: num_correspondences > 1024 unsupported");
-    GEOB_REQUIRE(workspace_bytes >= geob200_superpoint_matching_workspace_bytes(n_ref, n_src), "superpoint_matching: workspace too small");
-    GEOB_REQUIRE(n_ref * n_src < (1ll << 31), "superpoint_matching: too many node pairs");
-    Arena ar(workspace, workspace_bytes);
-    int* ridx = ar.take<int>(n_ref);
-    int* sidx = ar.take<int>(n_src);
-    float* rowsum = ar.take<float>(n_ref);
-    float* colsum = ar.take<float>(n_src);
-    float* S = ar.take<float>((size_t)n_ref * n_src);
-    float* flat = ar.take<float>((size_t)n_ref * n_src);
-    int* counts = ar.take<int>(64);
-    const Segs R = segs_one(n_ref), Q = segs_one(n_src);
-    compact_masks_kernel<<<dim3(1, 1), 1024, 0, st>>>(ref_masks, R, ridx, counts);
-    compact_masks_kernel<<<dim3(1, 1), 1024, 0, st>>>(src_masks, Q, sidx, counts + 1);
-    count_launches(2);
-    return superpoint_matching_impl(ref_feats, src_feats, channels, R, Q, ridx, sidx, counts, rowsum, colsum, S, flat, num_correspondences,
-                                    dual, ref_corr_indices, src_corr_indices, corr_scores, num_out, st);
-}
-
-int geob200_superpoint_matching_batched(const float* feats, int64_t channels, const uint8_t* masks, int64_t n_pairs,
-                                        const int64_t* cloud_nodes, int64_t num_correspondences, int dual, int64_t* corr_indices,
-                                        float* corr_scores, int32_t* num_out, void* workspace, size_t workspace_bytes, void* stream) {
+int geob200_superpoint_matching_batched(const float* ref_feats, const float* src_feats, int64_t channels, const uint8_t* ref_masks,
+                                        const uint8_t* src_masks, int64_t n_pairs, const int64_t* cloud_nodes, int64_t num_correspondences,
+                                        int dual, int64_t* corr_indices, float* corr_scores, int32_t* num_out, void* workspace,
+                                        size_t workspace_bytes, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     GEOB_REQUIRE(n_pairs > 0 && 2 * n_pairs <= GEOB_MAX_CLOUDS, "superpoint_matching_batched: 1..%d pairs", GEOB_MAX_CLOUDS / 2);
     GEOB_REQUIRE(num_correspondences > 0 && num_correspondences <= 1024, "superpoint_matching: num_correspondences must be in 1..1024");
-    Segs cl, NN;
-    if (segs_from_counts(&cl, 2 * n_pairs, cloud_nodes)) return -1;
     const int B = (int)n_pairs;
-    const Segs R = segs_range(cl, 0, B), Q = segs_range(cl, B, B);
+    // cl: all 2B clouds stacked (the workspace rows); R / Q: the ref / src clouds in the row spaces of ref_feats / src_feats
+    Segs cl, Q, NN;
+    if (segs_from_counts(&cl, 2 * n_pairs, cloud_nodes) || segs_from_counts(&Q, n_pairs, cloud_nodes + n_pairs)) return -1;
+    const Segs R = segs_range(cl, 0, B);
+    const int64_t ref_rows = cl.start[B], rows = (int64_t)cl.start[2 * B - 1] + cl.count[2 * B - 1];
+    GEOB_REQUIRE(ref_rows > 0 && rows > ref_rows, "superpoint_matching: empty input");
     if (segs_products(&NN, R, Q)) return -1;
-    const int64_t rows = (int64_t)cl.start[2 * B - 1] + cl.count[2 * B - 1];
     const int64_t nn = (int64_t)NN.start[B - 1] + NN.count[B - 1];
     GEOB_REQUIRE(workspace_bytes >= geob200_superpoint_matching_batched_workspace_bytes(rows, nn, n_pairs),
                  "superpoint_matching_batched: workspace too small");
+    const size_t smem = sizeof(float) * (channels + Q.max);
+    GEOB_REQUIRE(smem <= 48 * 1024, "superpoint_matching: row does not fit shared memory");
     Arena ar(workspace, workspace_bytes);
-    int* idx = ar.take<int>(rows);
+    int* idx = ar.take<int>(rows);               // ref clouds' valid nodes, then the src clouds' (at ref_rows)
     float* rowsum = ar.take<float>(rows);
     float* colsum = ar.take<float>(rows);
     float* S = ar.take<float>(nn);
     float* flat = ar.take<float>(nn);
-    int* counts = ar.take<int>(2 * B);
-    compact_masks_kernel<<<dim3(1, 2 * B), 1024, 0, st>>>(masks, cl, idx, counts);
-    count_launches(1);
+    int* counts = ar.take<int>(2 * B);           // counts[p] / counts[B + p] = valid ref / src nodes of pair p
+    const int* ridx = idx;
+    const int* sidx = idx + ref_rows;
+    const dim3 g_rows((unsigned)(R.max > 0 ? R.max : 1), B), g_cols((unsigned)((Q.max + 255) / 256 > 0 ? (Q.max + 255) / 256 : 1), B),
+        g_nn((unsigned)((NN.max + 255) / 256 > 0 ? (NN.max + 255) / 256 : 1), B);
     const int64_t k = num_correspondences;
-    return superpoint_matching_impl(feats, feats, channels, R, Q, idx, idx, counts, rowsum, colsum, S, flat, k, dual, corr_indices,
-                                    corr_indices + B * k, corr_scores, num_out, st);
-}
-
-int geob200_gather_patches(const int64_t* corr_indices, int64_t n_corr, const int64_t* node_knn_indices,
-                           const uint8_t* node_knn_masks, int64_t k, const float* points, int64_t n_points,
-                           int64_t* out_indices, uint8_t* out_masks, float* out_points, void* stream) {
-    if (n_corr == 0) return 0;
-    gather_patches_kernel<<<dim3((unsigned)((n_corr * k + 255) / 256), 1), 256, 0, (cudaStream_t)stream>>>(
-        (const long long*)corr_indices, (int)n_corr, (const long long*)node_knn_indices, node_knn_masks, (int)k, points, segs_one(0),
-        segs_one(n_points), (long long*)out_indices, out_masks, out_points);
+    compact_masks_kernel<<<dim3(1, 2 * B), 1024, 0, st>>>(ref_masks, src_masks, cl, B, idx, counts);
+    spm_scores_kernel<<<g_rows, 256, smem, st>>>(ref_feats, src_feats, (int)channels, ridx, counts, sidx, counts + B, R, Q, NN, S, rowsum);
+    spm_colsum_kernel<<<g_cols, 256, 0, st>>>(S, counts, counts + B, Q, NN, colsum);
+    spm_dual_kernel<<<g_nn, 256, 0, st>>>(S, counts, counts + B, rowsum, colsum, R, Q, NN, dual, flat);
+    topk_flat_kernel<1024><<<dim3(1, B), 1024, 0, st>>>(flat, counts, counts + B, (int)k, ridx, sidx, R, Q, NN, (long long*)corr_indices,
+                                                        (long long*)corr_indices + B * k, corr_scores, num_out);
     GEOB_CHECK_LAUNCH();
-    count_launches(1);
+    count_launches(5);
     return 0;
 }
 
@@ -659,9 +612,13 @@ int geob200_gather_patches_batched(const int64_t* corr_indices, int64_t n_corr, 
     return 0;
 }
 
-static int patch_scores_impl(const float* ref_feats, const float* src_feats, const Segs& R, const Segs& Q, int64_t channels,
-                             const int64_t* ref_knn_indices, const int64_t* src_knn_indices, int64_t n_patches, int64_t k, float* scores,
-                             cudaStream_t st) {
+int geob200_patch_scores_batched(const float* ref_feats, const float* src_feats, int64_t channels, int64_t n_pairs, const int64_t* cloud_points,
+                                 const int64_t* ref_knn_indices, const int64_t* src_knn_indices, int64_t n_patches, int64_t k,
+                                 float* scores, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    GEOB_REQUIRE(n_pairs > 0 && 2 * n_pairs <= GEOB_MAX_CLOUDS, "patch_scores_batched: 1..%d pairs", GEOB_MAX_CLOUDS / 2);
+    Segs R, Q;
+    if (segs_from_counts(&R, n_pairs, cloud_points) || segs_from_counts(&Q, n_pairs, cloud_points + n_pairs)) return -1;
     if (n_patches == 0) return 0;
     const float div = sqrtf((float)channels);      // feats_f.shape[1] ** 0.5
     const dim3 grid((unsigned)n_patches, R.n);
@@ -676,23 +633,6 @@ static int patch_scores_impl(const float* ref_feats, const float* src_feats, con
     GEOB_CHECK_LAUNCH();
     count_launches(1);
     return 0;
-}
-
-int geob200_patch_scores(const float* ref_feats, int64_t n_ref, const float* src_feats, int64_t n_src, int64_t channels,
-                         const int64_t* ref_knn_indices, const int64_t* src_knn_indices, int64_t n_patches, int64_t k,
-                         float* scores, void* stream) {
-    return patch_scores_impl(ref_feats, src_feats, segs_one(n_ref), segs_one(n_src), channels, ref_knn_indices, src_knn_indices,
-                             n_patches, k, scores, (cudaStream_t)stream);
-}
-
-int geob200_patch_scores_batched(const float* feats, int64_t channels, int64_t n_pairs, const int64_t* cloud_points,
-                                 const int64_t* ref_knn_indices, const int64_t* src_knn_indices, int64_t n_patches, int64_t k,
-                                 float* scores, void* stream) {
-    Segs cl;
-    GEOB_REQUIRE(n_pairs > 0 && 2 * n_pairs <= GEOB_MAX_CLOUDS, "patch_scores_batched: 1..%d pairs", GEOB_MAX_CLOUDS / 2);
-    if (segs_from_counts(&cl, 2 * n_pairs, cloud_points)) return -1;
-    return patch_scores_impl(feats, feats, segs_range(cl, 0, (int)n_pairs), segs_range(cl, (int)n_pairs, (int)n_pairs), channels,
-                             ref_knn_indices, src_knn_indices, n_patches, k, scores, (cudaStream_t)stream);
 }
 
 int geob200_sinkhorn(const float* scores, const uint8_t* row_masks, const uint8_t* col_masks, const float* alpha,

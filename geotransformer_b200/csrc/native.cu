@@ -135,20 +135,6 @@ size_t geob200_backbone_workspace_bytes(const geob200_backbone_t* net, const int
     return total;
 }
 
-int geob200_backbone_forward(const geob200_backbone_t* net, const float* feats, const float* const* points, const int64_t* level_rows,
-                             const int64_t* const* neighbors, const int64_t* neighbor_width, const int64_t* const* subsampling,
-                             const int64_t* subsampling_width, const int64_t* const* upsampling, const int64_t* upsampling_width,
-                             float* const* out_feats /* [num_stages - finest_decoder + 1], coarse first */, void* gn_workspace,
-                             size_t gn_workspace_bytes, void* workspace, size_t workspace_bytes, void* stream) {
-    return geob200_backbone_forward_batched(net, feats, points, level_rows, neighbors, neighbor_width, subsampling, subsampling_width,
-                                            upsampling, upsampling_width, out_feats, gn_workspace, gn_workspace_bytes, workspace,
-                                            workspace_bytes, stream, 1, nullptr, nullptr);
-}
-
-size_t geob200_backbone_gn_workspace_bytes(const geob200_backbone_t* net, const int64_t* level_rows, int64_t n_pairs) {
-    return fused_group_norm_workspace_bytes_batched(level_rows[0], (int64_t)net->init_dim << net->num_stages, net->groups, n_pairs);
-}
-
 int geob200_backbone_forward_batched(const geob200_backbone_t* net, const float* feats, const float* const* points,
                                      const int64_t* level_rows, const int64_t* const* neighbors, const int64_t* neighbor_width,
                                      const int64_t* const* subsampling, const int64_t* subsampling_width,
@@ -228,11 +214,6 @@ int geob200_backbone_forward_batched(const geob200_backbone_t* net, const float*
 
 // ---- transformer -------------------------------------------------------------------------------------------
 
-size_t geob200_transformer_workspace_bytes(int64_t n0, int64_t n1, int64_t channels, int64_t heads, int64_t num_layers) {
-    const int64_t rows[2] = {n0, n1};
-    return geob200_transformer_batched_workspace_bytes(1, rows, channels, heads, num_layers);
-}
-
 static int run_tail(Ctx& c, const geob200_tlayer_t& L, const float* hidden, const float* inp, int64_t rows, int64_t ch, float* out) {
     float* h = c.fl(rows, ch);
     float* x = c.fl(rows, ch);
@@ -245,15 +226,6 @@ static int run_tail(Ctx& c, const geob200_tlayer_t& L, const float* hidden, cons
     TRY(linear_img(y1, 2 * ch, L.squeeze.weight, L.squeeze.weight_img, L.squeeze.bias, y2, ch, rows, ch, 2 * ch, 0, c.stream));
     TRY(geob200_add_layernorm(x, y2, L.out_norm.gamma, L.out_norm.beta, rows, ch, 1e-5f, out, c.stream));
     return 0;
-}
-
-// x: stacked [feats0; feats1] (n0+n1, C) hidden features (after in_proj); emb0 (n0,n0,C), emb1 (n1,n1,C); out (n0+n1, C).
-int geob200_transformer_forward(const geob200_tlayer_t* layers, int64_t num_layers, int64_t channels, int64_t heads, const float* x_in,
-                                int64_t n0, int64_t n1, const float* emb0, const float* emb1, float* out, void* workspace,
-                                size_t workspace_bytes, void* stream) {
-    const int64_t rows[2] = {n0, n1};
-    const float* embs[2] = {emb0, emb1};
-    return geob200_transformer_forward_batched(layers, num_layers, channels, heads, x_in, 1, rows, embs, out, workspace, workspace_bytes, stream);
 }
 
 size_t geob200_transformer_batched_workspace_bytes(int64_t n_pairs, const int64_t* cloud_rows_h, int64_t channels, int64_t heads,

@@ -200,15 +200,19 @@ using namespace geob200;
 
 extern "C" {
 
-static int point_to_node_partition_impl(const float* points, const float* nodes, const Segs& Pt, const Segs& Nd, int64_t n_nodes,
-                                        int64_t point_limit, int64_t* point_to_node, uint8_t* node_masks, int32_t* node_sizes,
-                                        int64_t* node_knn_indices, uint8_t* node_knn_masks, cudaStream_t st) {
+int geob200_point_to_node_partition_batched(const float* points, const float* nodes, int64_t n_clouds, const int64_t* cloud_points,
+                                            const int64_t* cloud_nodes, int64_t point_limit, int64_t* point_to_node, uint8_t* node_masks,
+                                            int32_t* node_sizes, int64_t* node_knn_indices, uint8_t* node_knn_masks, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    Segs Pt, Nd;
+    if (segs_from_counts(&Pt, n_clouds, cloud_points) || segs_from_counts(&Nd, n_clouds, cloud_nodes)) return -1;
+    GEOB_REQUIRE(Pt.max > 0 && Nd.max > 0, "point_to_node_partition: empty input");
     GEOB_REQUIRE(point_limit > 0 && point_limit <= 2048, "point_to_node_partition: point_limit must be in 1..2048 (got %lld)",
                  (long long)point_limit);
     GEOB_REQUIRE((int64_t)Nd.max * 16 <= 200 * 1024, "point_to_node_partition: too many nodes (%d)", Nd.max);
+    const int64_t n_nodes = (int64_t)Nd.start[n_clouds - 1] + Nd.count[n_clouds - 1];
     GEOB_CHECK_CUDA(cudaMemsetAsync(node_masks, 0, n_nodes, st));
     GEOB_CHECK_CUDA(cudaMemsetAsync(node_sizes, 0, 4 * n_nodes, st));
-    if (Pt.max == 0 || Nd.max == 0) return 0;
     const size_t smem = sizeof(float4) * Nd.max;
     if (smem > 48 * 1024 && ensure_max_smem((const void*)p2n_assign_kernel)) return -1;
     p2n_assign_kernel<<<dim3((unsigned)((Pt.max + 255) / 256), Pt.n), 256, smem, st>>>(points, nodes, Pt, Nd, (long long*)point_to_node,
@@ -218,25 +222,6 @@ static int point_to_node_partition_impl(const float* points, const float* nodes,
     GEOB_CHECK_LAUNCH();
     count_launches(2);
     return 0;
-}
-
-int geob200_point_to_node_partition(const float* points, int64_t n_points, const float* nodes, int64_t n_nodes,
-                                    int64_t point_limit, int64_t* point_to_node, uint8_t* node_masks, int32_t* node_sizes,
-                                    int64_t* node_knn_indices, uint8_t* node_knn_masks, int32_t* status, void* stream) {
-    cudaStream_t st = (cudaStream_t)stream;
-    GEOB_REQUIRE(n_points > 0 && n_nodes > 0 && point_limit > 0, "point_to_node_partition: empty input");
-    if (status != nullptr) GEOB_CHECK_CUDA(cudaMemsetAsync(status, 0, 4, st));     // kept for ABI stability: always 0 now
-    return point_to_node_partition_impl(points, nodes, segs_one(n_points), segs_one(n_nodes), n_nodes, point_limit, point_to_node,
-                                        node_masks, node_sizes, node_knn_indices, node_knn_masks, st);
-}
-
-int geob200_point_to_node_partition_batched(const float* points, const float* nodes, int64_t n_clouds, const int64_t* cloud_points,
-                                            const int64_t* cloud_nodes, int64_t point_limit, int64_t* point_to_node, uint8_t* node_masks,
-                                            int32_t* node_sizes, int64_t* node_knn_indices, uint8_t* node_knn_masks, void* stream) {
-    Segs Pt, Nd;
-    if (segs_from_counts(&Pt, n_clouds, cloud_points) || segs_from_counts(&Nd, n_clouds, cloud_nodes)) return -1;
-    return point_to_node_partition_impl(points, nodes, Pt, Nd, (int64_t)Nd.start[n_clouds - 1] + Nd.count[n_clouds - 1], point_limit,
-                                        point_to_node, node_masks, node_sizes, node_knn_indices, node_knn_masks, (cudaStream_t)stream);
 }
 
 int geob200_knn_partition(const float* points, int64_t n_points, const float* nodes, int64_t n_nodes, int64_t k,

@@ -72,60 +72,15 @@ class RegistrationEngine:
         if self.batch_size > 32:
             raise ValueError('RegistrationEngine: at most 32 pairs per forward (the kernels carry the 2 x batch cloud offsets by value)')
         bs = self.batch_size
-        self.r_dev = [torch.zeros((24,) if bs == 1 else (bs, 24), dtype=torch.float32, device=self.device) for _ in range(num_streams)]
-        self.r_host = [torch.zeros((24,) if bs == 1 else (bs, 24), dtype=torch.float32).pin_memory() for _ in range(num_streams)]
+        self.r_dev = [torch.zeros((bs, 24), dtype=torch.float32, device=self.device) for _ in range(num_streams)]
+        self.r_host = [torch.zeros((bs, 24), dtype=torch.float32).pin_memory() for _ in range(num_streams)]
         # per slot: [loss, c_loss, f_loss] rows on the device and pinned on the host (only with a loss function)
-        self.l_dev = [torch.zeros((3,) if bs == 1 else (bs, 3), dtype=torch.float32, device=self.device) for _ in range(num_streams)]
-        self.l_host = [torch.zeros((3,) if bs == 1 else (bs, 3), dtype=torch.float32).pin_memory() for _ in range(num_streams)]
+        self.l_dev = [torch.zeros((bs, 3), dtype=torch.float32, device=self.device) for _ in range(num_streams)]
+        self.l_host = [torch.zeros((bs, 3), dtype=torch.float32).pin_memory() for _ in range(num_streams)]
         # per slot: [RANSAC transform (16) | fitness | inlier_rmse | metrics of the RANSAC transform (8)] (only with ransac)
-        x_rows = (26,) if bs == 1 else (bs, 26)
-        self.x_dev = [torch.zeros(x_rows, dtype=torch.float32, device=self.device) if ransac is not None else None for _ in range(num_streams)]
-        self.x_host = [torch.zeros(x_rows, dtype=torch.float32).pin_memory() if ransac is not None else None for _ in range(num_streams)]
+        self.x_dev = [torch.zeros((bs, 26), dtype=torch.float32, device=self.device) if ransac is not None else None for _ in range(num_streams)]
+        self.x_host = [torch.zeros((bs, 26), dtype=torch.float32).pin_memory() if ransac is not None else None for _ in range(num_streams)]
         self.sides = [[torch.cuda.Stream(self.device) for _ in range(side_streams)] if bs > 1 else [] for _ in range(num_streams)]
-
-    def _one(self, slot, pair, keep):
-        stream = self.streams[slot]
-        b = self.cfg.backbone
-        marks = None
-        if self.stage_times is not None:
-            marks = []
-            e = torch.cuda.Event(enable_timing=True)
-            e.record()
-            marks.append(('begin', e))
-        data = registration_collate_fn_stack_mode([pair], b.num_stages, b.init_voxel_size, b.init_radius, self.limits,
-                                                  device=self.device)
-        if marks is not None:
-            data['_stage_events'] = marks
-        out = self.model(data)
-        r_dev, r_host = self.r_dev[slot], self.r_host[slot]
-        r_dev[:16].copy_(out['estimated_transform'].reshape(16))
-        if self.evaluator is not None:
-            self.evaluator.metrics_tensor(out, data, out=r_dev[16:])
-        r_host.copy_(r_dev, non_blocking=True)
-        if self.loss_func is not None:
-            self.loss_func.loss_tensor(out, data, out=self.l_dev[slot])
-            self.l_host[slot].copy_(self.l_dev[slot], non_blocking=True)
-        if self.ransac is not None:
-            self._ransac_one(out, data['transform'], self.x_dev[slot], 0)
-            self.x_host[slot].copy_(self.x_dev[slot], non_blocking=True)
-        done = torch.cuda.Event()
-        done.record(stream)
-        done.synchronize()                      # this thread only; the other streams keep running
-        if marks is not None:          # per-stage GPU time of this pair (stage label = the interval ending at that mark)
-            for (_, e0), (label, e1) in zip(marks[:-1], marks[1:]):
-                self.stage_times.setdefault('collate' if label == 'start' else label, []).append(e0.elapsed_time(e1))
-        res = {'estimated_transform': r_host[:16].reshape(4, 4).clone(), 'num_corr': int(out['ref_corr_points'].shape[0]),
-               'num_superpoints': (int(out['ref_points_c'].shape[0]), int(out['src_points_c'].shape[0]))}
-        if self.evaluator is not None:
-            m = r_host[16:].tolist()
-            res['metrics'] = dict(zip(('PIR', 'IR', 'RRE', 'RTE', 'RMSE', 'RR'), m[:6]))
-        if self.loss_func is not None:
-            res['loss'] = dict(zip(LOSS_KEYS, self.l_host[slot].tolist()))
-        if self.ransac is not None:
-            res['ransac'] = self._ransac_result(self.x_host[slot])
-        if keep:
-            res['output_dict'] = out
-        return res, done
 
     def _ransac_one(self, out, transform, row, pair):
         """RANSAC of one pair's (trimmed) correspondences into ``row`` (26,), metrics of its transform with the evaluator"""
@@ -143,7 +98,7 @@ class RegistrationEngine:
         return r
 
     def _batch(self, slot, chunk, keep):
-        """``len(chunk)`` pairs in one forward (batch mode)"""
+        """``len(chunk)`` pairs in one forward"""
         stream = self.streams[slot]
         b = self.cfg.backbone
         n = len(chunk)
@@ -160,7 +115,7 @@ class RegistrationEngine:
         l_dev, l_host, lf = self.l_dev[slot][:n], self.l_host[slot][:n], self.loss_func
         rs = self.ransac
         x_dev, x_host = (self.x_dev[slot][:n], self.x_host[slot][:n]) if rs is not None else (None, None)
-        if n == 1:             # a trailing single pair: the one-pair forward
+        if n == 1:             # one pair (batch_size 1, or the trailing pair of a batch): the one-pair forward
             out = self.model(data)
             r_dev[0, :16].copy_(out['estimated_transform'].reshape(16))
             if self.evaluator is not None:
@@ -229,11 +184,8 @@ class RegistrationEngine:
                     cursor[0] += bs
                 if i >= len(pairs):
                     return last
-                if bs == 1:
-                    results[i], last = self._one(slot, pairs[i], keep)
-                else:
-                    res, last = self._batch(slot, pairs[i:i + bs], keep)
-                    results[i:i + len(res)] = res
+                res, last = self._batch(slot, pairs[i:i + bs], keep)
+                results[i:i + len(res)] = res
 
     def register(self, pairs, start_event=None, keep_outputs=False):
         """pairs: list of dicts with ref_points/src_points/ref_feats/src_feats/transform (numpy, CPU or CUDA tensors).

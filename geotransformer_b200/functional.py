@@ -13,7 +13,7 @@ from . import _lib as L
 
 _f32, _i64, _u8, _i32 = torch.float32, torch.int64, torch.uint8, torch.int32
 
-# mode of the structure-embedding contraction (see geob200_gse_embed): 0 fp32 CUDA cores, 1 wgmma 3xTF32, 2 1xTF32,
+# mode of the structure-embedding contraction (see geob200_gse_embed_pairs): 0 fp32 CUDA cores, 1 wgmma 3xTF32, 2 1xTF32,
 # 3 3xFP16 (fp32-accurate like 3xTF32 at half the tensor-pipe time), 4 3xFP16 on CTA pairs,
 # 5 tabulated projections (geob200_gse_embed_table: no contraction at all; default -- tests/gse_table_check.py compares its
 # accuracy and launch time with mode 3).  Mode 5 needs the ``table`` of the weights (``gse_table``; the modules build and
@@ -193,9 +193,9 @@ def kpconv_group_norm(s_feats, q_points, s_points, neighbor_indices, kernel_poin
     return y
 
 
-def _cloud_rows(cloud_rows):
-    import ctypes
-    return (ctypes.c_int64 * len(cloud_rows))(*[int(r) for r in cloud_rows])
+def _host_i64(values):
+    values = [int(v) for v in values]
+    return (ctypes.c_int64 * len(values))(*values)
 
 
 def group_norm_batched(x, weight, bias, groups, cloud_rows, eps=1e-5, negative_slope=None, residual=None):
@@ -208,7 +208,7 @@ def group_norm_batched(x, weight, bias, groups, cloud_rows, eps=1e-5, negative_s
     y = torch.empty_like(x)
     L.check(L.lib().geob200_group_norm_batched(x.data_ptr(), n, c, groups, weight.data_ptr(), bias.data_ptr(), float(eps), L.ptr(residual),
                                                int(negative_slope is not None), float(negative_slope or 0.0), y.data_ptr(), ws.data_ptr(),
-                                               ws.numel(), L.stream_ptr(), np_, _cloud_rows(cloud_rows)), 'group_norm_batched')
+                                               ws.numel(), L.stream_ptr(), np_, _host_i64(cloud_rows)), 'group_norm_batched')
     return y
 
 
@@ -224,7 +224,7 @@ def linear_group_norm_batched(x, weight, bias, gn_weight, gn_bias, groups, cloud
     L.check(L.lib().geob200_linear_group_norm_batched(x.data_ptr(), x.stride(0), weight.data_ptr(), L.ptr(bias), m, n, k, groups,
                                                       gn_weight.data_ptr(), gn_bias.data_ptr(), float(eps), L.ptr(residual),
                                                       int(negative_slope is not None), float(negative_slope or 0.0), pre.data_ptr(),
-                                                      y.data_ptr(), ws.data_ptr(), ws.numel(), L.stream_ptr(), np_, _cloud_rows(cloud_rows)),
+                                                      y.data_ptr(), ws.data_ptr(), ws.numel(), L.stream_ptr(), np_, _host_i64(cloud_rows)),
             'linear_group_norm_batched')
     return y
 
@@ -262,21 +262,7 @@ def nearest_upsample(x, upsample_indices):
 # ------------------------------------------------------------------------------------------------ partition
 
 def point_to_node_partition(points, nodes, point_limit, return_count=False):
-    _f(points, 'points'); _f(nodes, 'nodes')
-    n, m = points.shape[0], nodes.shape[0]
-    dev = points.device
-    p2n = torch.empty((n,), dtype=_i64, device=dev)
-    node_masks = torch.empty((m,), dtype=torch.bool, device=dev)
-    node_sizes = torch.empty((m,), dtype=_i32, device=dev)
-    knn = torch.empty((m, point_limit), dtype=_i64, device=dev)
-    knn_masks = torch.empty((m, point_limit), dtype=torch.bool, device=dev)
-    L.check(L.lib().geob200_point_to_node_partition(points.data_ptr(), n, nodes.data_ptr(), m, point_limit,
-                                                    p2n.data_ptr(), node_masks.data_ptr(), node_sizes.data_ptr(),
-                                                    knn.data_ptr(), knn_masks.data_ptr(), None,
-                                                    L.stream_ptr()), 'point_to_node_partition')
-    if return_count:
-        return p2n, node_sizes.long(), node_masks, knn, knn_masks
-    return p2n, node_masks, knn, knn_masks
+    return point_to_node_partition_batched(points, nodes, [points.shape[0]], [nodes.shape[0]], point_limit, return_count)
 
 
 def knn_partition(points, nodes, k, return_distance=False):
@@ -352,10 +338,7 @@ def gse_indices(points, sigma_d, sigma_a, angle_k, out=None):
     else:
         d = torch.empty((n, n), dtype=_f32, device=points.device)
         a = torch.empty((n, n, angle_k), dtype=_f32, device=points.device)
-    factor_a = 180.0 / (sigma_a * math.pi)
-    L.check(L.lib().geob200_gse_indices(points.data_ptr(), n, float(sigma_d), float(factor_a), angle_k, d.data_ptr(),
-                                        a.data_ptr(), L.stream_ptr()), 'gse_indices')
-    return d, a
+    return gse_indices_batched(points, [n], sigma_d, sigma_a, angle_k, d, a)
 
 
 def gse_indices_batched(points, cloud_rows, sigma_d, sigma_a, angle_k, d_out, a_out):
@@ -363,7 +346,7 @@ def gse_indices_batched(points, cloud_rows, sigma_d, sigma_a, angle_k, d_out, a_
     clouds' index arrays one after the other (the layout ``gse_embed_flat`` consumes)"""
     _f(points, 'points')
     factor_a = 180.0 / (sigma_a * math.pi)
-    L.check(L.lib().geob200_gse_indices_batched(points.data_ptr(), len(cloud_rows), _cloud_rows(cloud_rows), float(sigma_d), float(factor_a),
+    L.check(L.lib().geob200_gse_indices_batched(points.data_ptr(), len(cloud_rows), _host_i64(cloud_rows), float(sigma_d), float(factor_a),
                                                 angle_k, d_out.data_ptr(), a_out.data_ptr(), L.stream_ptr()), 'gse_indices_batched')
     return d_out, a_out
 
@@ -470,24 +453,10 @@ def gse_embed_flat(d_indices, a_indices, n_rows, div_term, wd, wa, bd, ba, wd_t,
 
 
 def gse_embed(d_indices, a_indices, div_term, wd, wa, bd, ba, wd_t, wa_t, mode=None, out=None, table=None):
+    """structure embedding of one cloud: d (n, n), a (n, n, k) -> (n, n, C)"""
     n = d_indices.shape[0]
-    c = wd.shape[0]
-    mode = _gse_mode(mode, table)
-    emb = torch.empty((n, n, c), dtype=_f32, device=d_indices.device) if out is None else out
-    if mode == 5 and c in (128, 256):
-        return _gse_embed_table(d_indices, a_indices, n * n, div_term, wd, wa, bd, ba, table, emb)
-    if c == 128 and mode != 0:
-        mode = 3                     # hidden_dim 128 (KITTI): the 3xFP16 wgmma kernel has an N = 128 instantiation
-    elif c != 256:
-        mode = 0                     # other widths: fp32 CUDA-core kernel
-    lib = L.lib()
-    ws = L.workspace(lib.geob200_gse_embed_workspace_bytes(n, c), d_indices.device, 'gse')
-    with _timed('gse_embed'):
-        L.check(lib.geob200_gse_embed(d_indices.data_ptr(), a_indices.data_ptr(), n, c, div_term.data_ptr(),
-                                      wd_t.data_ptr(), wa_t.data_ptr(), wd.data_ptr(), wa.data_ptr(), bd.data_ptr(),
-                                      ba.data_ptr(), emb.data_ptr(), int(mode), ws.data_ptr(), ws.numel(), L.stream_ptr()),
-                'gse_embed')
-    return emb
+    emb = torch.empty((n, n, wd.shape[0]), dtype=_f32, device=d_indices.device) if out is None else out
+    return gse_embed_flat(d_indices, a_indices, n * n, div_term, wd, wa, bd, ba, wd_t, wa_t, emb, mode=mode, table=table)
 
 
 def _rows(t, name):
@@ -555,24 +524,9 @@ def superpoint_matching(ref_feats, src_feats, ref_masks, src_masks, num_correspo
     """reference ``superpoint_matching.py:13-50``.  The number of rows is min(k, #valid ref x #valid src): it is read back
     from the device (one small D2H) unless ``defer_count`` -- then the full-capacity tensors (padding rows: index -1, score 0,
     which ``gather_patches`` turns into empty patches) and the device count are returned and the caller trims later."""
-    _f(ref_feats, 'ref_feats'); _f(src_feats, 'src_feats')
-    dev = ref_feats.device
-    nr, ns, c = ref_feats.shape[0], src_feats.shape[0], ref_feats.shape[1]
-    if ref_masks is None:
-        ref_masks = torch.ones((nr,), dtype=torch.bool, device=dev)
-    if src_masks is None:
-        src_masks = torch.ones((ns,), dtype=torch.bool, device=dev)
-    lib = L.lib()
-    ws = L.workspace(lib.geob200_superpoint_matching_workspace_bytes(nr, ns), dev)
-    k = int(num_correspondences)
-    ri = torch.empty((k,), dtype=_i64, device=dev)
-    si = torch.empty((k,), dtype=_i64, device=dev)
-    sc = torch.empty((k,), dtype=_f32, device=dev)
-    cnt = torch.empty((1,), dtype=_i32, device=dev)
-    L.check(lib.geob200_superpoint_matching(ref_feats.data_ptr(), src_feats.data_ptr(), nr, ns, c, ref_masks.data_ptr(),
-                                            src_masks.data_ptr(), k, int(dual_normalization), ri.data_ptr(),
-                                            si.data_ptr(), sc.data_ptr(), cnt.data_ptr(), ws.data_ptr(), ws.numel(),
-                                            L.stream_ptr()), 'superpoint_matching')
+    corr, sc, cnt = _superpoint_matching(ref_feats, src_feats, ref_masks, src_masks, [ref_feats.shape[0], src_feats.shape[0]],
+                                         num_correspondences, dual_normalization)
+    ri, si, sc = corr[0], corr[1], sc[0]
     if defer_count:
         return ri, si, sc, cnt
     kk = int(cnt.item())
@@ -580,25 +534,12 @@ def superpoint_matching(ref_feats, src_feats, ref_masks, src_masks, num_correspo
 
 
 def gather_patches(corr_indices, node_knn_indices, node_knn_masks, points):
-    p, k = corr_indices.shape[0], node_knn_indices.shape[1]
-    dev = points.device
-    idx = torch.empty((p, k), dtype=_i64, device=dev)
-    msk = torch.empty((p, k), dtype=torch.bool, device=dev)
-    pts = torch.empty((p, k, 3), dtype=_f32, device=dev)
-    L.check(L.lib().geob200_gather_patches(corr_indices.data_ptr(), p, node_knn_indices.data_ptr(),
-                                           node_knn_masks.data_ptr(), k, points.data_ptr(), points.shape[0],
-                                           idx.data_ptr(), msk.data_ptr(), pts.data_ptr(), L.stream_ptr()), 'gather_patches')
-    return idx, msk, pts
+    return gather_patches_batched(corr_indices, corr_indices.shape[0], [node_knn_indices.shape[0]], [points.shape[0]], node_knn_indices,
+                                  node_knn_masks, points)
 
 
 def patch_scores(ref_feats, src_feats, ref_knn_indices, src_knn_indices):
-    ref_feats, src_feats = _detach(ref_feats), _detach(src_feats)
-    p, k = ref_knn_indices.shape
-    out = torch.empty((p, k, k), dtype=_f32, device=ref_feats.device)
-    L.check(L.lib().geob200_patch_scores(ref_feats.data_ptr(), ref_feats.shape[0], src_feats.data_ptr(),
-                                         src_feats.shape[0], ref_feats.shape[1], ref_knn_indices.data_ptr(),
-                                         src_knn_indices.data_ptr(), p, k, out.data_ptr(), L.stream_ptr()), 'patch_scores')
-    return out
+    return _patch_scores(ref_feats, src_feats, [ref_feats.shape[0], src_feats.shape[0]], ref_knn_indices, src_knn_indices)
 
 
 def sinkhorn(scores, row_masks, col_masks, alpha, num_iterations, inf=1e12):
@@ -623,32 +564,17 @@ def local_global_registration(ref_knn_points, src_knn_points, ref_knn_masks, src
                               return_details=False, defer_count=False, transform_out=None):
     """``defer_count``: no host read-back -- returns the full-capacity correspondence tensors and the device count
     ``(ref_c, src_c, scores, T, n)``; rows ``[:n]`` are valid.  ``transform_out``: (16,) float view to write T into."""
-    p, kk = ref_knn_masks.shape
-    ld = score_mat.shape[1]
-    dev = score_mat.device
-    lib = L.lib()
-    cap = p * kk * k * (1 if mutual else 2)
-    ref_c = torch.empty((cap, 3), dtype=_f32, device=dev)
-    src_c = torch.empty((cap, 3), dtype=_f32, device=dev)
-    sc = torch.empty((cap,), dtype=_f32, device=dev)
-    cp = torch.empty((cap,), dtype=_i32, device=dev)
-    n = torch.empty((1,), dtype=_i32, device=dev)
-    T = torch.empty((4, 4), dtype=_f32, device=dev) if transform_out is None else transform_out
-    pT = torch.empty((p, 4, 4), dtype=_f32, device=dev)
-    pin = torch.empty((p,), dtype=_i32, device=dev)
-    best = torch.empty((1,), dtype=_i32, device=dev)
-    ws = L.workspace(lib.geob200_lgr_workspace_bytes(p, kk, k), dev)
-    L.check(lib.geob200_local_global_registration(
-        ref_knn_points.data_ptr(), src_knn_points.data_ptr(), ref_knn_masks.data_ptr(), src_knn_masks.data_ptr(),
-        score_mat.data_ptr(), p, kk, ld, k, float(acceptance_radius), int(mutual), float(confidence_threshold),
-        int(correspondence_threshold), int(num_refinement_steps), ref_c.data_ptr(), src_c.data_ptr(), sc.data_ptr(),
-        cp.data_ptr(), n.data_ptr(), T.data_ptr(), pT.data_ptr(), pin.data_ptr(), best.data_ptr(), ws.data_ptr(),
-        ws.numel(), L.stream_ptr()), 'local_global_registration')
+    T = torch.empty((4, 4), dtype=_f32, device=score_mat.device) if transform_out is None else transform_out
+    res = local_global_registration_batched(1, ref_knn_points, src_knn_points, ref_knn_masks, src_knn_masks, score_mat, k, acceptance_radius,
+                                            mutual, confidence_threshold, correspondence_threshold, num_refinement_steps,
+                                            transform_out=T.view(1, 16), details=return_details)
+    ref_c, src_c, sc, n = res[0][0], res[1][0], res[2][0], res[4]
     if defer_count:
         return ref_c, src_c, sc, T, n
     c = int(n.item())    # the one D2H of the stage: the number of correspondences sizes the returned tensors
     if return_details:
-        return ref_c[:c], src_c[:c], sc[:c], T, dict(corr_patch=cp[:c], patch_transforms=pT, patch_inliers=pin, best=best)
+        det = res[5]
+        return ref_c[:c], src_c[:c], sc[:c], T, dict(det, corr_patch=det['corr_patch'][0][:c])
     return ref_c[:c], src_c[:c], sc[:c], T
 
 
@@ -677,19 +603,9 @@ def node_correspondences(ref_nodes, src_nodes, ref_knn_points, src_knn_points, t
             L.require_cuda(t, name, torch.bool)
             if tuple(t.shape) != shape:
                 raise ValueError('node_correspondences: %s must have shape %s' % (name, shape))
-    dev = ref_nodes.device
-    lib = L.lib()
-    ws = L.workspace(lib.geob200_node_correspondences_workspace_bytes(m, n, k), dev, tag='node_corr')
     cap = (m * n + 65535) // 65536 * 65536          # rounded: same block sizes from pair to pair (no allocator churn)
-    idx = torch.empty((cap, 2), dtype=_i64, device=dev)
-    ov = torch.empty((cap,), dtype=_f32, device=dev)
-    cnt = torch.empty((1,), dtype=_i32, device=dev)
-    L.check(lib.geob200_node_correspondences(ref_nodes.data_ptr(), src_nodes.data_ptr(), ref_knn_points.data_ptr(),
-                                             src_knn_points.data_ptr(), L.ptr(ref_masks), L.ptr(src_masks),
-                                             L.ptr(ref_knn_masks), L.ptr(src_knn_masks), m, n, k, transform.data_ptr(),
-                                             float(pos_radius), idx.data_ptr(), ov.data_ptr(), cnt.data_ptr(), ws.data_ptr(),
-                                             ws.numel(), L.stream_ptr()), 'node_correspondences')
-    return idx, ov, cnt
+    return _node_correspondences(ref_nodes, src_nodes, ref_knn_points, src_knn_points, ref_masks, src_masks, ref_knn_masks, src_knn_masks,
+                                 [m, n], transform, pos_radius, capacity=cap)
 
 
 def finish_node_correspondences(idx, ov, cnt):
@@ -728,16 +644,13 @@ def evaluate(gt_node_corr_indices, gt_node_corr_overlaps, ref_node_corr_indices,
 
 
 # ------------------------------------------------------------------------------------------------ batched per-pair stages
-# One launch per stage for all pairs of a batch (GeoTransformer.forward_batch).  Clouds are stacked [ref_1..ref_B, src_1..src_B];
-# ``cloud_nodes`` / ``cloud_points`` are the host lists of the 2B per-cloud row counts.  Each pair gets what the single-pair op gives.
+# One launch per stage for all pairs of a batch (GeoTransformer.forward_batch); the single-pair ops above are these with B = 1.
+# Clouds are stacked [ref_1..ref_B, src_1..src_B]; ``cloud_nodes`` / ``cloud_points`` are the host lists of the 2B per-cloud row
+# counts.  A pair gets the same bits alone and in any batch.
 
-def _host_i64(values):
-    values = [int(v) for v in values]
-    return (ctypes.c_int64 * len(values))(*values)
-
-
-def point_to_node_partition_batched(points, nodes, cloud_points, cloud_nodes, point_limit):
-    """stacked ``point_to_node_partition``: (point_to_node, node_masks, knn_indices, knn_masks), indices local to each cloud"""
+def point_to_node_partition_batched(points, nodes, cloud_points, cloud_nodes, point_limit, return_count=False):
+    """stacked ``point_to_node_partition``: (point_to_node[, node_sizes], node_masks, knn_indices, knn_masks), indices local to each
+    cloud"""
     _f(points, 'points'); _f(nodes, 'nodes')
     n, m = points.shape[0], nodes.shape[0]
     dev = points.device
@@ -750,6 +663,8 @@ def point_to_node_partition_batched(points, nodes, cloud_points, cloud_nodes, po
                                                             _host_i64(cloud_nodes), point_limit, p2n.data_ptr(), node_masks.data_ptr(),
                                                             node_sizes.data_ptr(), knn.data_ptr(), knn_masks.data_ptr(), L.stream_ptr()),
             'point_to_node_partition_batched')
+    if return_count:
+        return p2n, node_sizes.long(), node_masks, knn, knn_masks
     return p2n, node_masks, knn, knn_masks
 
 
@@ -769,62 +684,97 @@ def gather_patches_batched(corr_indices, n_corr, cloud_nodes, cloud_points, node
     return idx, msk, pts
 
 
+def _ref_rows(cloud_rows):
+    """rows of the B ref clouds at the head of a stack [ref_1..ref_B, src_1..src_B]: where the src block starts"""
+    return sum(int(c) for c in cloud_rows[:len(cloud_rows) // 2])
+
+
 def node_correspondences_batched(nodes, knn_points, node_masks, knn_masks, cloud_nodes, transforms, pos_radius):
     """stacked ``node_correspondences``: (indices (R, 2), overlaps (R,), counts (B,) int32) with pair p's rows at
     ``sum_{q<p} n_ref(q) * n_src(q)``"""
-    _f(nodes, 'nodes'); _f(knn_points, 'knn_points'); _f(transforms, 'transforms')
+    r = _ref_rows(cloud_nodes)
+    return _node_correspondences(nodes[:r], nodes[r:], knn_points[:r], knn_points[r:], node_masks[:r], node_masks[r:], knn_masks[:r],
+                                 knn_masks[r:], cloud_nodes, transforms, pos_radius)
+
+
+def _node_correspondences(ref_nodes, src_nodes, ref_knn_points, src_knn_points, ref_masks, src_masks, ref_knn_masks, src_knn_masks,
+                          cloud_nodes, transforms, pos_radius, capacity=None):
+    """``node_correspondences_batched`` with the ref clouds' nodes / (rows, k, 3) patch points / masks (None = all valid) in the
+    ref_* tensors and the src clouds' in the src_* tensors (the two blocks of the C entry point); ``capacity``: rows of the outputs
+    (default: the sum of n_ref * n_src over all pairs)."""
+    _f(ref_nodes, 'ref_nodes'); _f(src_nodes, 'src_nodes'); _f(ref_knn_points, 'ref_knn_points'); _f(src_knn_points, 'src_knn_points')
+    _f(transforms, 'transforms')
     B = len(cloud_nodes) // 2
-    k = knn_points.shape[1]
+    k = ref_knn_points.shape[1]
     nn = sum(int(cloud_nodes[p]) * int(cloud_nodes[B + p]) for p in range(B))
-    dev = nodes.device
+    rows = sum(int(c) for c in cloud_nodes)
+    cap = max(nn, 1) if capacity is None else capacity
+    dev = ref_nodes.device
     lib = L.lib()
-    ws = L.workspace(lib.geob200_node_correspondences_batched_workspace_bytes(nodes.shape[0], nn, k), dev, tag='node_corr')
-    idx = torch.empty((max(nn, 1), 2), dtype=_i64, device=dev)
-    ov = torch.empty((max(nn, 1),), dtype=_f32, device=dev)
+    ws = L.workspace(lib.geob200_node_correspondences_batched_workspace_bytes(rows, nn, k), dev, tag='node_corr')
+    idx = torch.empty((cap, 2), dtype=_i64, device=dev)
+    ov = torch.empty((cap,), dtype=_f32, device=dev)
     cnt = torch.empty((B,), dtype=_i32, device=dev)
-    L.check(lib.geob200_node_correspondences_batched(nodes.data_ptr(), knn_points.data_ptr(), node_masks.data_ptr(), knn_masks.data_ptr(),
-                                                     B, _host_i64(cloud_nodes), k, transforms.data_ptr(), float(pos_radius), idx.data_ptr(),
-                                                     ov.data_ptr(), cnt.data_ptr(), ws.data_ptr(), ws.numel(), L.stream_ptr()),
-            'node_correspondences_batched')
+    L.check(lib.geob200_node_correspondences_batched(ref_nodes.data_ptr(), src_nodes.data_ptr(), ref_knn_points.data_ptr(),
+                                                     src_knn_points.data_ptr(), L.ptr(ref_masks), L.ptr(src_masks), L.ptr(ref_knn_masks),
+                                                     L.ptr(src_knn_masks), B, _host_i64(cloud_nodes), k, transforms.data_ptr(),
+                                                     float(pos_radius), idx.data_ptr(), ov.data_ptr(), cnt.data_ptr(), ws.data_ptr(),
+                                                     ws.numel(), L.stream_ptr()), 'node_correspondences_batched')
     return idx, ov, cnt
 
 
 def superpoint_matching_batched(feats, masks, cloud_nodes, num_correspondences, dual_normalization=True):
     """stacked ``superpoint_matching`` (deferred counts): (corr (2B, k) int64 -- row p ref / row B + p src indices of pair p,
     scores (B, k), counts (B,) int32)"""
-    _f(feats, 'feats')
+    r = _ref_rows(cloud_nodes)
+    return _superpoint_matching(feats[:r], feats[r:], masks[:r], masks[r:], cloud_nodes, num_correspondences, dual_normalization)
+
+
+def _superpoint_matching(ref_feats, src_feats, ref_masks, src_masks, cloud_nodes, num_correspondences, dual_normalization):
+    """``superpoint_matching_batched`` with the ref clouds' rows in ``ref_feats`` / ``ref_masks`` and the src clouds' in
+    ``src_feats`` / ``src_masks`` (masks None = all valid)"""
+    _f(ref_feats, 'ref_feats'); _f(src_feats, 'src_feats')
     B = len(cloud_nodes) // 2
     k = int(num_correspondences)
     nn = sum(int(cloud_nodes[p]) * int(cloud_nodes[B + p]) for p in range(B))
-    dev = feats.device
+    rows = sum(int(c) for c in cloud_nodes)
+    dev = ref_feats.device
     lib = L.lib()
-    ws = L.workspace(lib.geob200_superpoint_matching_batched_workspace_bytes(feats.shape[0], nn, B), dev)
+    ws = L.workspace(lib.geob200_superpoint_matching_batched_workspace_bytes(rows, nn, B), dev)
     corr = torch.empty((2 * B, k), dtype=_i64, device=dev)
     sc = torch.empty((B, k), dtype=_f32, device=dev)
     cnt = torch.empty((B,), dtype=_i32, device=dev)
-    L.check(lib.geob200_superpoint_matching_batched(feats.data_ptr(), feats.shape[1], masks.data_ptr(), B, _host_i64(cloud_nodes), k,
-                                                    int(dual_normalization), corr.data_ptr(), sc.data_ptr(), cnt.data_ptr(), ws.data_ptr(),
-                                                    ws.numel(), L.stream_ptr()), 'superpoint_matching_batched')
+    L.check(lib.geob200_superpoint_matching_batched(ref_feats.data_ptr(), src_feats.data_ptr(), ref_feats.shape[1], L.ptr(ref_masks),
+                                                    L.ptr(src_masks), B, _host_i64(cloud_nodes), k, int(dual_normalization), corr.data_ptr(),
+                                                    sc.data_ptr(), cnt.data_ptr(), ws.data_ptr(), ws.numel(), L.stream_ptr()),
+            'superpoint_matching_batched')
     return corr, sc, cnt
 
 
 def patch_scores_batched(feats, cloud_points, ref_knn_indices, src_knn_indices):
     """stacked ``patch_scores``: pair p's patches at rows p * (rows / B) of both index tensors"""
-    feats = _detach(feats)
+    r = _ref_rows(cloud_points)
+    return _patch_scores(feats[:r], feats[r:], cloud_points, ref_knn_indices, src_knn_indices)
+
+
+def _patch_scores(ref_feats, src_feats, cloud_points, ref_knn_indices, src_knn_indices):
+    """``patch_scores_batched`` with the ref clouds' fine rows in ``ref_feats`` and the src clouds' in ``src_feats``"""
+    ref_feats, src_feats = _detach(ref_feats), _detach(src_feats)
     B = len(cloud_points) // 2
     p, k = ref_knn_indices.shape
-    out = torch.empty((p, k, k), dtype=_f32, device=feats.device)
-    L.check(L.lib().geob200_patch_scores_batched(feats.data_ptr(), feats.shape[1], B, _host_i64(cloud_points), ref_knn_indices.data_ptr(),
-                                                 src_knn_indices.data_ptr(), p // B, k, out.data_ptr(), L.stream_ptr()),
-            'patch_scores_batched')
+    out = torch.empty((p, k, k), dtype=_f32, device=ref_feats.device)
+    L.check(L.lib().geob200_patch_scores_batched(ref_feats.data_ptr(), src_feats.data_ptr(), ref_feats.shape[1], B, _host_i64(cloud_points),
+                                                 ref_knn_indices.data_ptr(), src_knn_indices.data_ptr(), p // B, k, out.data_ptr(),
+                                                 L.stream_ptr()), 'patch_scores_batched')
     return out
 
 
 def local_global_registration_batched(n_pairs, ref_knn_points, src_knn_points, ref_knn_masks, src_knn_masks, score_mat, k,
                                       acceptance_radius, mutual, confidence_threshold, correspondence_threshold, num_refinement_steps,
-                                      transform_out=None):
+                                      transform_out=None, details=False):
     """stacked ``local_global_registration`` (deferred counts): (ref_c (B, cap, 3), src_c, scores (B, cap), T, counts (B,) int32).
-    ``transform_out``: (B, >= 16) float rows (row stride = its stride(0)) to write the transforms into; else T is (B, 16)."""
+    ``transform_out``: (B, >= 16) float rows (row stride = its stride(0)) to write the transforms into; else T is (B, 16).
+    ``details``: also a dict corr_patch (B, cap), patch_transforms (B * P, 4, 4), patch_inliers (B * P,), best (B,)."""
     pt, kk = ref_knn_masks.shape
     B = int(n_pairs)
     P = pt // B
@@ -837,12 +787,19 @@ def local_global_registration_batched(n_pairs, ref_knn_points, src_knn_points, r
     cp = torch.empty((B, cap), dtype=_i32, device=dev)
     n = torch.empty((B,), dtype=_i32, device=dev)
     T = torch.empty((B, 16), dtype=_f32, device=dev) if transform_out is None else transform_out
+    det = None
+    if details:
+        det = dict(corr_patch=cp, patch_transforms=torch.empty((pt, 4, 4), dtype=_f32, device=dev),
+                   patch_inliers=torch.empty((pt,), dtype=_i32, device=dev), best=torch.empty((B,), dtype=_i32, device=dev))
     ws = L.workspace(lib.geob200_lgr_batched_workspace_bytes(B, P, kk, k), dev)
     L.check(lib.geob200_local_global_registration_batched(
         ref_knn_points.data_ptr(), src_knn_points.data_ptr(), ref_knn_masks.data_ptr(), src_knn_masks.data_ptr(), score_mat.data_ptr(),
         B, P, kk, score_mat.shape[1], k, float(acceptance_radius), int(mutual), float(confidence_threshold), int(correspondence_threshold),
         int(num_refinement_steps), ref_c.data_ptr(), src_c.data_ptr(), sc.data_ptr(), cp.data_ptr(), n.data_ptr(), T.data_ptr(),
-        T.stride(0), None, None, None, ws.data_ptr(), ws.numel(), L.stream_ptr()), 'local_global_registration_batched')
+        T.stride(0), *(None if det is None else det[key].data_ptr() for key in ('patch_transforms', 'patch_inliers', 'best')),
+        ws.data_ptr(), ws.numel(), L.stream_ptr()), 'local_global_registration_batched')
+    if details:
+        return ref_c, src_c, sc, T, n, det
     return ref_c, src_c, sc, T, n
 
 

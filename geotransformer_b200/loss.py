@@ -2,7 +2,7 @@
 validation losses CoarseMatchingLoss / FineMatchingLoss / OverallLoss (``loss.py:10-92``).
 
 Same constructor/forward contract as the reference's three Evaluator classes (3DMatch, KITTI, ModelNet differ in how
-RMSE and RR are defined; ``cfg.name`` selects).  All six numbers come from ONE kernel launch (`geob200_evaluate`); the
+RMSE and RR are defined; ``cfg.name`` selects).  All six numbers come from ONE kernel launch (`geob200_evaluate_counts`); the
 result dict holds 0-dim device tensors like the reference's.  KITTI has no RMSE entry (loss.py:140-151 there).
 
 The losses are the values the reference's ``val_step`` reports on the eval-mode forward.  They carry NO autograd graph:

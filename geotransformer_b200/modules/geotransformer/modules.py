@@ -100,7 +100,7 @@ class GeometricTransformer(nn.Module):
         GF.linear(ref_feats, self.in_proj.weight, self.in_proj.bias, out=x[:n0])
         GF.linear(src_feats, self.in_proj.weight, self.in_proj.bias, out=x[n0:])
         if native is not None:
-            x = native.transformer_forward(x, n0, ref_emb, src_emb)
+            x = native.transformer_forward_batched(x, [n0, n1], [ref_emb, src_emb])
         else:
             x = self.transformer.forward_stacked(x, n0, ref_emb, src_emb)
         y = GF.linear(x, self.out_proj.weight, self.out_proj.bias)

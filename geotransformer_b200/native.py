@@ -165,6 +165,7 @@ class NativeModel:
         ws = L.workspace(ws_bytes, dev, 'native_backbone')
         n_pairs = int(data_dict.get('batch_size', 1))
         gn = GF._gn_workspace(dev, self.backbone.groups, pts[0].shape[0], self.backbone.init_dim << S, n_pairs=n_pairs)
+        carr = marr = None               # one pair: no per-pair statistics or table widths
         if n_pairs > 1:
             # batch of pairs in stack order [ref_1..ref_B, src_1..src_B]: per-pair GroupNorm statistics need the cloud rows
             lens = data_dict['lengths_host']
@@ -176,19 +177,16 @@ class NativeModel:
                 L.check(lib.geob200_cloud_max_count(sub[l].data_ptr(), sub[l].shape[0], pts[l].shape[0], sub[l].shape[1], n_pairs, keep[l + 1],
                                                     cmax[l].data_ptr(), L.stream_ptr()), 'cloud_max_count')
             marr = (P * S)(*([cmax[l].data_ptr() for l in range(S - 1)] + [None]))
-            L.check(lib.geob200_backbone_forward_batched(ctypes.byref(self.backbone), feats.data_ptr(), parr, rows, narr, nw, sarr, sw,
-                                                         uarr, uw, oarr, gn.data_ptr(), gn.numel(), ws.data_ptr(), ws.numel(),
-                                                         L.stream_ptr(), n_pairs, carr, marr), 'backbone_forward_batched')
-        else:
-            L.check(lib.geob200_backbone_forward(ctypes.byref(self.backbone), feats.data_ptr(), parr, rows, narr, nw, sarr, sw, uarr, uw,
-                                                 oarr, gn.data_ptr(), gn.numel(), ws.data_ptr(), ws.numel(), L.stream_ptr()),
-                    'backbone_forward')
+        L.check(lib.geob200_backbone_forward_batched(ctypes.byref(self.backbone), feats.data_ptr(), parr, rows, narr, nw, sarr, sw, uarr, uw,
+                                                     oarr, gn.data_ptr(), gn.numel(), ws.data_ptr(), ws.numel(), L.stream_ptr(), n_pairs, carr,
+                                                     marr), 'backbone_forward_batched')
         outs.reverse()
         return outs
 
     def transformer_forward_batched(self, x, cloud_rows, embeddings):
-        """RPEConditionalTransformer over a batch of pairs: x rows in stack order [ref_1..ref_B, src_1..src_B],
-        ``cloud_rows`` their 2B row counts (host ints), ``embeddings`` the 2B structure embeddings (device tensors)."""
+        """RPEConditionalTransformer over a batch of pairs (one pair: x = [ref; src], ``cloud_rows`` = [n_ref, n_src]): x rows in
+        stack order [ref_1..ref_B, src_1..src_B], ``cloud_rows`` their 2B row counts (host ints), ``embeddings`` the 2B structure
+        embeddings (device tensors)."""
         lib = L.lib()
         nc = len(cloud_rows)
         rows = (I64 * nc)(*[int(r) for r in cloud_rows])
@@ -199,16 +197,4 @@ class NativeModel:
         L.check(lib.geob200_transformer_forward_batched(self.layers, self.num_layers, self.hidden, self.heads, x.data_ptr(), nc // 2, rows,
                                                         earr, out.data_ptr(), ws.data_ptr(), ws.numel(), L.stream_ptr()),
                 'transformer_forward_batched')
-        return out
-
-    def transformer_forward(self, x, n0, emb0, emb1):
-        """RPEConditionalTransformer.forward_stacked"""
-        lib = L.lib()
-        n1 = x.shape[0] - n0
-        out = torch.empty_like(x)
-        ws_bytes = lib.geob200_transformer_workspace_bytes(n0, n1, self.hidden, self.heads, self.num_layers)
-        ws = L.workspace(ws_bytes, x.device, 'native_transformer')
-        L.check(lib.geob200_transformer_forward(self.layers, self.num_layers, self.hidden, self.heads, x.data_ptr(), n0, n1, emb0.data_ptr(),
-                                                emb1.data_ptr(), out.data_ptr(), ws.data_ptr(), ws.numel(), L.stream_ptr()),
-                'transformer_forward')
         return out

@@ -104,7 +104,7 @@ size_t geob200_fused_group_norm_workspace_bytes(int64_t n_rows, int64_t channels
 int geob200_linear_group_norm(const float* x, int64_t ldx, const float* weight, const float* bias, int64_t m, int64_t n, int64_t k,
                               int64_t groups, const float* gamma, const float* beta, float eps, const float* residual, int leaky,
                               float slope, float* pre_norm, float* y, void* workspace, size_t workspace_bytes, void* stream);
-size_t geob200_kpconv_group_norm_workspace_bytes(int64_t n_query, int64_t n_support, int64_t c_in, int64_t c_out, int64_t groups);
+/* workspace: geob200_kpconv_tc_workspace_bytes(n_query, n_support, c_in) */
 int geob200_kpconv_group_norm(const float* s_feats, const float* q_points, const float* s_points, const int64_t* neighbors,
                               int64_t n_query, int64_t n_support, int64_t n_neighbors, const float* kernel_points, int64_t n_kernel,
                               const float* weights_t, const float* bias, int64_t c_in, int64_t c_out, float sigma, int64_t groups,
@@ -113,8 +113,8 @@ int geob200_kpconv_group_norm(const float* s_feats, const float* q_points, const
 
 /* Batched forms (several pairs per forward, rows in stack order [ref_1..ref_B, src_1..src_B], cloud_rows_h[2 * n_pairs] host row
  * counts): the statistics are taken per PAIR (cloud c belongs to pair c % n_pairs), everything else is identical.
- * Workspace: geob200_group_norm_batched_workspace_bytes, zero-filled once. */
-size_t geob200_group_norm_batched_workspace_bytes(int64_t n_rows, int64_t channels, int64_t groups, int64_t n_pairs);
+ * Workspace: geob200_fused_group_norm_workspace_bytes(n_rows, channels, groups) + 8 * groups * n_pairs + 512 bytes (the per-pair
+ * statistics), zero-filled once. */
 int geob200_group_norm_batched(const float* x, int64_t n_rows, int64_t channels, int64_t groups, const float* gamma, const float* beta,
                                float eps, const float* residual, int leaky, float slope, float* y, void* workspace, size_t workspace_bytes,
                                void* stream, int64_t n_pairs, const int64_t* cloud_rows_h);
@@ -127,13 +127,11 @@ int geob200_linear_group_norm_batched(const float* x, int64_t ldx, const float* 
 int geob200_maxpool(const float* x, const int64_t* neighbors, int64_t n_query, int64_t n_support, int64_t n_neighbors,
                     int64_t channels, float* y, void* stream);
 
-/* Batched maxpool over a table that is wider than a pair's own (radius_search.py:25-26 cuts to the pair's max count):
- * columns past min(n_neighbors, max(cloud_max[p], cloud_max[B + p])) are ignored for the rows of pair p. */
+/* cloud_max[c] (device int32[2 * n_pairs]) = widest row (number of real neighbours) among the query rows of cloud c: the batched
+ * backbone's maxpool ignores the columns of pair p past min(n_neighbors, max(cloud_max[p], cloud_max[B + p])), as
+ * radius_search.py:25-26 cuts each pair's table to its own max count. */
 int geob200_cloud_max_count(const int64_t* neighbors, int64_t n_query, int64_t n_support, int64_t n_neighbors, int64_t n_pairs,
                             const int64_t* cloud_rows_h, int32_t* cloud_max, void* stream);
-int geob200_maxpool_batched(const float* x, const int64_t* neighbors, int64_t n_query, int64_t n_support, int64_t n_neighbors,
-                            int64_t channels, float* y, int64_t n_pairs, const int64_t* cloud_rows_h, const int32_t* cloud_max,
-                            void* stream);
 
 /* y[m] = [ x_pad[up_indices[m*up_stride]] | skip[m] ]: nearest_upsample (functional.py:6-22) fused with the
  * torch.cat of the decoder (backbone.py:75-76).  skip may be NULL (c2 = 0). */
@@ -142,20 +140,16 @@ int geob200_upsample_concat(const float* x, const int64_t* up_indices, int64_t u
 
 /* ---- point-to-node grouping ------------------------------------------------------------------------------ */
 
-/* point_to_node_partition (reference geotransformer/modules/ops/pointcloud_partition.py:60-107).
- * node_masks / node_knn_masks are uint8 (torch.bool); node_sizes int32.  Exact for any number of points per node (chunked
- * selection); status (may be NULL) is kept for ABI stability and always receives 0. */
-int geob200_point_to_node_partition(const float* points, int64_t n_points, const float* nodes, int64_t n_nodes,
-                                    int64_t point_limit, int64_t* point_to_node, uint8_t* node_masks, int32_t* node_sizes,
-                                    int64_t* node_knn_indices, uint8_t* node_knn_masks, int32_t* status, void* stream);
-
-/* Batched forms of the per-pair stages (GeoTransformer.forward_batch): one launch per stage covers every cloud or pair of a batch.
- * Clouds are stacked [ref_1..ref_B, src_1..src_B] as in the batched collate; cloud_nodes / cloud_points are HOST arrays of the 2B
- * per-cloud row counts at the superpoint / fine (or, for geob200_evaluate_batched, input) level.  Every pair gets exactly what
- * the single-pair entry point gives it, bit for bit (the single-pair entry points run the same kernels with one pair).
- * Indices stay local to their cloud.  1 <= B <= 32. */
-/* point_to_node_partition of n_clouds stacked clouds: points / point_to_node at the fine offsets, nodes / node_masks / node_sizes
- * and the (nodes, point_limit) knn tables at the superpoint offsets.  point_limit <= 2048. */
+/* The per-pair stages (grouping, structure-embedding indices, ground-truth correspondences, matching, patches, LGR, metrics) have
+ * one entry point each, batched over the pairs of a forward: one launch per stage covers every cloud or pair, and one pair is
+ * B = 1 (one cloud: n_clouds = 1).  Clouds are stacked [ref_1..ref_B, src_1..src_B] as in the batched collate; cloud_nodes /
+ * cloud_points are HOST arrays of the 2B per-cloud row counts at the superpoint / fine (or, for geob200_evaluate_batched, input)
+ * level.  Entry points with separate ref_* / src_* inputs take the B ref clouds stacked in the ref block and the B src clouds in
+ * the src block.  A pair gets the same bits alone and in any batch.  Indices stay local to their cloud.  1 <= B <= 32. */
+/* point_to_node_partition (reference geotransformer/modules/ops/pointcloud_partition.py:60-107) of n_clouds stacked clouds:
+ * points / point_to_node at the fine offsets, nodes / node_masks / node_sizes and the (nodes, point_limit) knn tables at the
+ * superpoint offsets.  node_masks / node_knn_masks are uint8 (torch.bool); node_sizes int32.  Exact for any number of points per
+ * node (chunked selection).  point_limit <= 2048. */
 int geob200_point_to_node_partition_batched(const float* points, const float* nodes, int64_t n_clouds, const int64_t* cloud_points,
                                             const int64_t* cloud_nodes, int64_t point_limit, int64_t* point_to_node, uint8_t* node_masks,
                                             int32_t* node_sizes, int64_t* node_knn_indices, uint8_t* node_knn_masks, void* stream);
@@ -181,26 +175,19 @@ int geob200_gather_rows(const float* table, int64_t n_rows, int64_t channels, co
 
 /* ---- geometric transformer -------------------------------------------------------------------------------- */
 
-/* GeometricStructureEmbedding.get_embedding_indices (geotransformer.py:27-55) for one cloud:
- * d_indices (n,n) = sqrt(pairwise_distance)/sigma_d, a_indices (n,n,3) = atan2(|ref x anc|, ref.anc) * factor_a */
-int geob200_gse_indices(const float* points, int64_t n, float sigma_d, float factor_a, int64_t angle_k, float* d_indices,
-                        float* a_indices, void* stream);
-
-/* The same for n_clouds stacked clouds in ONE launch (cloud_rows_h: host row counts): points (sum rows, 3); the outputs are
- * concatenated cloud after cloud: d_indices (sum n_c^2), a_indices (sum n_c^2, 3) -- the layout geob200_gse_embed_pairs takes. */
+/* GeometricStructureEmbedding.get_embedding_indices (geotransformer.py:27-55) of n_clouds stacked clouds in ONE launch
+ * (cloud_rows_h: host row counts; points (sum rows, 3)): per cloud, d_indices (n,n) = sqrt(pairwise_distance)/sigma_d and
+ * a_indices (n,n,3) = atan2(|ref x anc|, ref.anc) * factor_a, concatenated cloud after cloud: d_indices (sum n_c^2), a_indices
+ * (sum n_c^2, 3) -- the layout geob200_gse_embed_pairs takes. */
 int geob200_gse_indices_batched(const float* points, int64_t n_clouds, const int64_t* cloud_rows_h, float sigma_d, float factor_a,
                                 int64_t angle_k, float* d_indices, float* a_indices, void* stream);
 
 /* GeometricStructureEmbedding.forward (geotransformer.py:57-72) given the indices: sinusoid -> proj_d / proj_a ->
- * max over k -> sum, fused.  wd/wa are the nn.Linear weights (out,in); wd_t/wa_t their transposes (in,out).
+ * max over k -> sum, fused, over a flat list of n_rows (anchor, point) index rows -- the n*n (i, j) pairs of one cloud, or of several
+ * clouds concatenated: d_indices (n_rows,), a_indices (n_rows, 3) -> embeddings (n_rows, channels).  wd/wa are the nn.Linear
+ * weights (out,in); wd_t/wa_t their transposes (in,out).
  * mode 0: fp32 CUDA cores; 1: wgmma 3xTF32; 2: wgmma 1xTF32; 3: wgmma 3xFP16 split (fp32-accurate, fastest). */
 size_t geob200_gse_embed_workspace_bytes(int64_t n, int64_t channels);
-int geob200_gse_embed(const float* d_indices, const float* a_indices, int64_t n, int64_t channels, const float* div_term,
-                      const float* wd_t, const float* wa_t, const float* wd, const float* wa, const float* bd, const float* ba,
-                      float* embeddings, int mode, void* workspace, size_t workspace_bytes, void* stream);
-
-/* Same over a flat list of n_rows (anchor, point) index rows -- the (i, j) pairs of several clouds concatenated:
- * d_indices (n_rows,), a_indices (n_rows, 3) -> embeddings (n_rows, channels).  One launch for a whole batch of clouds. */
 int geob200_gse_embed_pairs(const float* d_indices, const float* a_indices, int64_t n_rows, int64_t channels, const float* div_term,
                             const float* wd_t, const float* wa_t, const float* wd, const float* wa, const float* bd, const float* ba,
                             float* embeddings, int mode, void* workspace, size_t workspace_bytes, void* stream);
@@ -249,40 +236,31 @@ int geob200_l2_normalize(const float* x, int64_t n, int64_t channels, float* y, 
 
 /* ---- matching ---------------------------------------------------------------------------------------------- */
 
-/* SuperPointMatching.forward (superpoint_matching.py:13-50); num_out (device int32) = number of rows written =
- * min(num_correspondences, #valid ref nodes x #valid src nodes); rows past it receive index -1 / score 0. */
-size_t geob200_superpoint_matching_workspace_bytes(int64_t n_ref, int64_t n_src);
-int geob200_superpoint_matching(const float* ref_feats, const float* src_feats, int64_t n_ref, int64_t n_src, int64_t channels,
-                                const uint8_t* ref_masks, const uint8_t* src_masks, int64_t num_correspondences, int dual,
-                                int64_t* ref_corr_indices, int64_t* src_corr_indices, float* corr_scores, int32_t* num_out,
-                                void* workspace, size_t workspace_bytes, void* stream);
-/* Batched: feats / masks = the stacked superpoint rows of all 2B clouds.  corr_indices (2B, num_correspondences): row p = ref
- * indices of pair p, row B + p = its src indices; corr_scores (B, num_correspondences), num_out (B).  Workspace for n_rows stacked
- * rows and n_products = sum over pairs of n_ref * n_src. */
+/* SuperPointMatching.forward (superpoint_matching.py:13-50): ref_feats / ref_masks hold the superpoint rows of the B ref clouds,
+ * src_feats / src_masks those of the B src clouds; masks are uint8 (torch.bool) or NULL (= all valid).  corr_indices
+ * (2B, num_correspondences): row p = ref indices of pair p, row B + p = its src indices; corr_scores (B, num_correspondences);
+ * num_out[p] (device int32) = number of rows written = min(num_correspondences, #valid ref nodes x #valid src nodes); rows past it
+ * receive index -1 / score 0.  num_correspondences in 1..1024.  Workspace for n_rows = all 2B clouds' rows and n_products = sum over
+ * pairs of n_ref * n_src. */
 size_t geob200_superpoint_matching_batched_workspace_bytes(int64_t n_rows, int64_t n_products, int64_t n_pairs);
-int geob200_superpoint_matching_batched(const float* feats, int64_t channels, const uint8_t* masks, int64_t n_pairs,
-                                        const int64_t* cloud_nodes, int64_t num_correspondences, int dual, int64_t* corr_indices,
-                                        float* corr_scores, int32_t* num_out, void* workspace, size_t workspace_bytes, void* stream);
+int geob200_superpoint_matching_batched(const float* ref_feats, const float* src_feats, int64_t channels, const uint8_t* ref_masks,
+                                        const uint8_t* src_masks, int64_t n_pairs, const int64_t* cloud_nodes, int64_t num_correspondences,
+                                        int dual, int64_t* corr_indices, float* corr_scores, int32_t* num_out, void* workspace,
+                                        size_t workspace_bytes, void* stream);
 
-/* patch gathers of model.py:169-174: indices/masks/points of the k points of each selected superpoint; a negative
- * corr index (padding row of geob200_superpoint_matching) yields an empty patch (sentinel indices, masks 0) */
-int geob200_gather_patches(const int64_t* corr_indices, int64_t n_corr, const int64_t* node_knn_indices,
-                           const uint8_t* node_knn_masks, int64_t k, const float* points, int64_t n_points,
-                           int64_t* out_indices, uint8_t* out_masks, float* out_points, void* stream);
-/* Batched over n_clouds stacked clouds (knn tables at the superpoint offsets, points at the fine offsets): cloud c gathers the
- * n_corr patches corr_indices[c * n_corr ..] to rows c * n_corr; with corr_indices = NULL every node of cloud c is a patch
- * (corr = arange), written at the cloud's superpoint offset. */
+/* patch gathers of model.py:169-174 over n_clouds stacked clouds (knn tables at the superpoint offsets, points at the fine
+ * offsets): indices/masks/points of the k points of each selected superpoint.  Cloud c gathers the n_corr patches
+ * corr_indices[c * n_corr ..] to rows c * n_corr; a negative corr index (padding row of geob200_superpoint_matching_batched) yields
+ * an empty patch (sentinel indices, masks 0).  With corr_indices = NULL every node of cloud c is a patch (corr = arange), written at
+ * the cloud's superpoint offset. */
 int geob200_gather_patches_batched(const int64_t* corr_indices, int64_t n_corr, int64_t n_clouds, const int64_t* cloud_nodes,
                                    const int64_t* cloud_points, const int64_t* node_knn_indices, const uint8_t* node_knn_masks, int64_t k,
                                    const float* points, int64_t* out_indices, uint8_t* out_masks, float* out_points, void* stream);
 
-/* matching_scores = einsum('bnd,bmd->bnm') / sqrt(C) over zero-padded feature tables (model.py:176-188) */
-int geob200_patch_scores(const float* ref_feats, int64_t n_ref, const float* src_feats, int64_t n_src, int64_t channels,
-                         const int64_t* ref_knn_indices, const int64_t* src_knn_indices, int64_t n_patches, int64_t k,
-                         float* scores, void* stream);
-/* Batched: feats = the stacked fine rows of all 2B clouds; pair p's n_patches patches at p * n_patches of ref_knn_indices,
- * src_knn_indices and scores. */
-int geob200_patch_scores_batched(const float* feats, int64_t channels, int64_t n_pairs, const int64_t* cloud_points,
+/* matching_scores = einsum('bnd,bmd->bnm') / sqrt(C) over zero-padded feature tables (model.py:176-188): ref_feats / src_feats hold
+ * the fine rows of the B ref / src clouds; pair p's n_patches patches at p * n_patches of ref_knn_indices, src_knn_indices and
+ * scores. */
+int geob200_patch_scores_batched(const float* ref_feats, const float* src_feats, int64_t channels, int64_t n_pairs, const int64_t* cloud_points,
                                  const int64_t* ref_knn_indices, const int64_t* src_knn_indices, int64_t n_patches, int64_t k,
                                  float* scores, void* stream);
 
@@ -293,20 +271,11 @@ int geob200_sinkhorn(const float* scores, const uint8_t* row_masks, const uint8_
 /* ---- local-to-global registration -------------------------------------------------------------------------- */
 
 /* LocalGlobalRegistration.forward (local_global_registration.py:196-235), use_dustbin=False, use_global_score=False,
- * correspondence_limit=None.  log_scores (P, score_ld, score_ld) with score_ld = k or k+1 (dustbin row/col ignored).
- * Correspondence outputs have capacity P*k*topk rows; num_corr (device int32) = rows written, in (patch,i,j) order.
- * patch_transforms (P,4,4), patch_inliers (P, -1 = patch below correspondence_threshold), best_patch may be NULL. */
-size_t geob200_lgr_workspace_bytes(int64_t n_patches, int64_t k, int64_t topk);
-int geob200_local_global_registration(const float* ref_knn_points, const float* src_knn_points, const uint8_t* ref_knn_masks,
-                                      const uint8_t* src_knn_masks, const float* log_scores, int64_t n_patches, int64_t k,
-                                      int64_t score_ld, int64_t topk, float acceptance_radius, int mutual,
-                                      float confidence_threshold, int64_t correspondence_threshold, int64_t num_refinement_steps,
-                                      float* ref_corr_points, float* src_corr_points, float* corr_scores, int32_t* corr_patch,
-                                      int32_t* num_corr, float* estimated_transform, float* patch_transforms, int32_t* patch_inliers,
-                                      int32_t* best_patch, void* workspace, size_t workspace_bytes, void* stream);
-/* Batched: n_pairs pairs of n_patches patches each (pair p at patch p * n_patches).  Pair p's correspondence rows start at
- * p * n_patches * k * topk (x2 when not mutual), num_corr / best_patch have n_pairs entries, its transform goes to
- * estimated_transform + p * transform_ld (>= 16), patch_transforms / patch_inliers are per patch. */
+ * correspondence_limit=None, for n_pairs pairs of n_patches patches each (pair p at patch p * n_patches).  log_scores
+ * (P, score_ld, score_ld) with score_ld = k or k+1 (dustbin row/col ignored).  Pair p's correspondence rows start at
+ * p * n_patches * k * topk (x2 when not mutual); num_corr[p] (device int32) = rows written, in (patch,i,j) order.  Its transform goes
+ * to estimated_transform + p * transform_ld (>= 16).  patch_transforms (P,4,4), patch_inliers (P, -1 = patch below
+ * correspondence_threshold) and best_patch (n_pairs) may be NULL. */
 size_t geob200_lgr_batched_workspace_bytes(int64_t n_pairs, int64_t n_patches, int64_t k, int64_t topk);
 int geob200_local_global_registration_batched(const float* ref_knn_points, const float* src_knn_points, const uint8_t* ref_knn_masks,
                                               const uint8_t* src_knn_masks, const float* log_scores, int64_t n_pairs, int64_t n_patches,
@@ -322,37 +291,24 @@ int geob200_weighted_procrustes(const float* src_points, const float* ref_points
                                 int64_t n, float weight_thresh, float eps, float* transforms, void* stream);
 
 /* get_node_correspondences (modules/registration/matching.py:231-315): ground-truth superpoint pairs and their overlap
- * ratios under `transform` (4x4, device).  Masks are uint8 (torch.bool) or NULL (= all valid).  corr_indices (capacity
- * n_ref*n_src rows of 2 int64) and corr_overlaps (capacity n_ref*n_src) receive the pairs with overlap > 0 in row-major
- * (ref, src) order, `count` (device int32) their number. */
-size_t geob200_node_correspondences_workspace_bytes(int64_t n_ref, int64_t n_src, int64_t k);
-int geob200_node_correspondences(const float* ref_nodes, const float* src_nodes, const float* ref_knn_points,
-                                 const float* src_knn_points, const uint8_t* ref_masks, const uint8_t* src_masks,
-                                 const uint8_t* ref_knn_masks, const uint8_t* src_knn_masks, int64_t n_ref, int64_t n_src,
-                                 int64_t k, const float* transform, float pos_radius, int64_t* corr_indices,
-                                 float* corr_overlaps, int32_t* count, void* workspace, size_t workspace_bytes, void* stream);
-/* Batched: nodes / node_masks and the (rows, k, 3) patch points / (rows, k) masks stacked over the 2B clouds; transforms (B,4,4).
- * Pair p's rows start at sum_{q<p} n_ref(q) * n_src(q) of corr_indices / corr_overlaps (that many rows of capacity), count (B). */
+ * ratios under transforms (B,4,4, device).  ref_nodes / ref_masks and the (rows, k, 3) patch points / (rows, k) masks of the B ref
+ * clouds in the ref_* block, those of the B src clouds in the src_* block; masks are uint8 (torch.bool) or NULL (= all valid).
+ * Pair p's rows start at sum_{q<p} n_ref(q) * n_src(q) of corr_indices (rows of 2 int64) / corr_overlaps (that many rows of
+ * capacity) and receive the pairs with overlap > 0 in row-major (ref, src) order, count[p] (device int32) their number. */
 size_t geob200_node_correspondences_batched_workspace_bytes(int64_t n_rows, int64_t n_products, int64_t k);
-int geob200_node_correspondences_batched(const float* nodes, const float* knn_points, const uint8_t* node_masks, const uint8_t* knn_masks,
-                                         int64_t n_pairs, const int64_t* cloud_nodes, int64_t k, const float* transforms, float pos_radius,
-                                         int64_t* corr_indices, float* corr_overlaps, int32_t* count, void* workspace, size_t workspace_bytes,
-                                         void* stream);
+int geob200_node_correspondences_batched(const float* ref_nodes, const float* src_nodes, const float* ref_knn_points,
+                                         const float* src_knn_points, const uint8_t* ref_masks, const uint8_t* src_masks,
+                                         const uint8_t* ref_knn_masks, const uint8_t* src_knn_masks, int64_t n_pairs, const int64_t* cloud_nodes,
+                                         int64_t k, const float* transforms, float pos_radius, int64_t* corr_indices, float* corr_overlaps,
+                                         int32_t* count, void* workspace, size_t workspace_bytes, void* stream);
 
-/* Evaluator.forward (experiments/<exp>/loss.py:95-159; metrics.py:47-112): metrics[8] (device) =
+/* Evaluator.forward (experiments/<exp>/loss.py:95-159; metrics.py:47-112) of one pair: metrics[8] (device) =
  * {PIR, IR, RRE [deg], RTE, RMSE, RR, #correspondences, #gt superpoint pairs}.  mode 0 = 3DMatch (RMSE of the realigned
  * source cloud, RR = RMSE < rmse_threshold), 1 = KITTI (no RMSE: NaN; RR = RRE < rre_threshold and RTE < rte_threshold),
- * 2 = ModelNet (RMSE of T_est x - T_gt x; RR as KITTI).  Means over empty sets are NaN, as torch reports them. */
-int geob200_evaluate(const int64_t* gt_node_corr_indices, const float* gt_node_corr_overlaps, int64_t n_gt,
-                     float acceptance_overlap, const int64_t* ref_node_corr_indices, const int64_t* src_node_corr_indices,
-                     int64_t n_node_corr, const float* ref_corr_points, const float* src_corr_points, int64_t n_corr,
-                     float acceptance_radius, const float* gt_transform, const float* est_transform, const float* src_points,
-                     int64_t n_src_points, int mode, float rmse_threshold, float rre_threshold, float rte_threshold,
-                     float* metrics, void* stream);
-
-/* Same with the three row counts optionally taken from DEVICE memory (int32, produced by geob200_node_correspondences /
- * geob200_superpoint_matching / geob200_local_global_registration): a non-NULL *_dev pointer overrides the host value
- * (n_node_corr: the smaller of the two), so a whole forward can be enqueued without a host read-back in between. */
+ * 2 = ModelNet (RMSE of T_est x - T_gt x; RR as KITTI).  Means over empty sets are NaN, as torch reports them.
+ * The three row counts are optionally taken from DEVICE memory (int32, as geob200_node_correspondences_batched /
+ * geob200_superpoint_matching_batched / geob200_local_global_registration_batched write them): a non-NULL *_dev pointer overrides
+ * the host value (n_node_corr: the smaller of the two), so a whole forward can be enqueued without a host read-back in between. */
 int geob200_evaluate_counts(const int64_t* gt_node_corr_indices, const float* gt_node_corr_overlaps, int64_t n_gt, const int32_t* n_gt_dev,
                             float acceptance_overlap, const int64_t* ref_node_corr_indices, const int64_t* src_node_corr_indices,
                             int64_t n_node_corr, const int32_t* n_node_corr_dev, const float* ref_corr_points, const float* src_corr_points,
@@ -472,10 +428,10 @@ int geob200_set_linear_persistent(int on);
 int64_t geob200_linear_profile_read(int64_t capacity, int64_t* shapes, float* ms);
 
 /* ---- native stage drivers (native.cu) ------------------------------------------------------------------------
- * The whole KPConv-FPN backbone / geometric transformer as ONE call: same kernels in the same order as the per-op entry
- * points above (bitwise-identical results), driven from C++ so that the host cost per pair is a few hundred microseconds
- * instead of milliseconds.  All pointers are device pointers; the structs are plain C (built from a state_dict by
- * geotransformer_b200/native.py). */
+ * The whole KPConv-FPN backbone / geometric transformer as ONE call for a batch of pairs (one pair: n_pairs = 1): same kernels in
+ * the same order as the per-op entry points above (bitwise-identical results), driven from C++ so that the host cost per pair is a
+ * few hundred microseconds instead of milliseconds.  All pointers are device pointers; the structs are plain C (built from a
+ * state_dict by geotransformer_b200/native.py). */
 #define GEOB200_MAX_STAGES 6
 /* weight_img / weights_img / *_img: optional tf32 split images (geob200_split_tf32) of weight / weights_t / the fused
  * projection weights, read by the tensor-core GEMM; NULL = split on every call. */
@@ -502,20 +458,14 @@ typedef struct {
     geob200_norm_t decoder_norms[GEOB200_MAX_STAGES];
 } geob200_backbone_t;
 size_t geob200_backbone_workspace_bytes(const geob200_backbone_t* net, const int64_t* level_rows);
-/* out_feats[0] = coarsest encoder output (rows level_rows[S-1]); out_feats[i>0] = decoder outputs, coarse to fine. */
-int geob200_backbone_forward(const geob200_backbone_t* net, const float* feats, const float* const* points, const int64_t* level_rows,
-                             const int64_t* const* neighbors, const int64_t* neighbor_width, const int64_t* const* subsampling,
-                             const int64_t* subsampling_width, const int64_t* const* upsampling, const int64_t* upsampling_width,
-                             float* const* out_feats, void* gn_workspace, size_t gn_workspace_bytes, void* workspace,
-                             size_t workspace_bytes, void* stream);
-
-/* Batched form (several pairs per forward, stack order [ref_1..ref_B, src_1..src_B] at every level like the reference collate
- * with batch_size B, utils/data.py:144): identical kernels over the stacked rows; the GroupNorm statistics are taken per pair
- * (modules/kpconv/modules.py:46-50 normalises over the stacked rows of ONE pair).  cloud_rows_h[level][2 * n_pairs]: host row
- * counts per cloud.  n_pairs <= 32.  The GroupNorm workspace needs geob200_backbone_gn_workspace_bytes (zero-filled once).
- * sub_cloud_max[level][2 * n_pairs] (device int32, geob200_cloud_max_count of the subsampling tables): the strided blocks'
- * maxpool must see every pair's table at the width the pair's own collate would have cut it to (geob200_maxpool_batched). */
-size_t geob200_backbone_gn_workspace_bytes(const geob200_backbone_t* net, const int64_t* level_rows, int64_t n_pairs);
+/* KPConvFPN.forward over n_pairs pairs in stack order [ref_1..ref_B, src_1..src_B] at every level (the reference collate with
+ * batch_size B, utils/data.py:144): identical kernels over the stacked rows; the GroupNorm statistics are taken per pair
+ * (modules/kpconv/modules.py:46-50 normalises over the stacked rows of ONE pair).  n_pairs <= 32.  out_feats[0] = coarsest encoder
+ * output (rows level_rows[S-1]); out_feats[i>0] = decoder outputs, coarse to fine.  The GroupNorm workspace
+ * (geob200_fused_group_norm_workspace_bytes(level_rows[0], init_dim << num_stages, groups) + 8 * groups * n_pairs + 512 bytes) is
+ * zero-filled once.  With n_pairs > 1: cloud_rows_h[level][2 * n_pairs] = host row counts per cloud, and
+ * sub_cloud_max[level][2 * n_pairs] (device int32, geob200_cloud_max_count of the subsampling tables) lets the strided blocks'
+ * maxpool see every pair's table at the width the pair's own collate would have cut it to; with one pair both may be NULL. */
 int geob200_backbone_forward_batched(const geob200_backbone_t* net, const float* feats, const float* const* points,
                                      const int64_t* level_rows, const int64_t* const* neighbors, const int64_t* neighbor_width,
                                      const int64_t* const* subsampling, const int64_t* subsampling_width,
@@ -532,15 +482,10 @@ typedef struct {
     geob200_linear_t expand; geob200_linear_t squeeze; geob200_norm_t out_norm;
     const float* w_qkv_img; const float* w_q_img; const float* w_kv_img;
 } geob200_tlayer_t;
-size_t geob200_transformer_workspace_bytes(int64_t n0, int64_t n1, int64_t channels, int64_t heads, int64_t num_layers);
-/* RPEConditionalTransformer.forward on stacked features x = [feats0; feats1] (after in_proj), sequential cross updates */
-int geob200_transformer_forward(const geob200_tlayer_t* layers, int64_t num_layers, int64_t channels, int64_t heads, const float* x,
-                                int64_t n0, int64_t n1, const float* emb0, const float* emb1, float* out, void* workspace,
-                                size_t workspace_bytes, void* stream);
-
-/* Batched form: x rows in stack order [ref_1..ref_B, src_1..src_B] (cloud_rows_h[2B], host); embeddings_h[c] = device pointer
- * of the structure embedding (rows_c, rows_c, C) of cloud c.  Linears / LayerNorms run once over all rows; attention is one
- * batched launch pair per phase (geob200_attention_batched).  Same arithmetic per pair as geob200_transformer_forward. */
+/* RPEConditionalTransformer.forward (after in_proj, sequential cross updates) over n_pairs pairs: x rows in stack order
+ * [ref_1..ref_B, src_1..src_B] (cloud_rows_h[2B], host; one pair: [ref; src]); embeddings_h[c] = device pointer of the structure
+ * embedding (rows_c, rows_c, C) of cloud c.  Linears / LayerNorms run once over all rows; attention is one batched launch pair per
+ * phase (geob200_attention_batched).  A pair gets the same bits alone and in any batch. */
 size_t geob200_transformer_batched_workspace_bytes(int64_t n_pairs, const int64_t* cloud_rows_h, int64_t channels, int64_t heads,
                                                    int64_t num_layers);
 int geob200_transformer_forward_batched(const geob200_tlayer_t* layers, int64_t num_layers, int64_t channels, int64_t heads,

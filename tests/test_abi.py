@@ -36,11 +36,11 @@ def test_no_torch_types_in_the_abi():
     assert 'extern "C"' in open(os.path.join(ROOT, 'include', 'geob200.h')).read()
 
 
-def test_pure_host_queries_work_without_gpu():
+def test_workspace_queries_work_without_gpu():
     lib = L.lib()
     assert lib.geob200_grid_subsample_workspace_bytes(40000, 2) > 40000 * 40
     assert lib.geob200_radius_search_workspace_bytes(40000, 40000, 2) > 40000 * 20
-    assert lib.geob200_lgr_workspace_bytes(256, 64, 3) > 0
+    assert lib.geob200_lgr_batched_workspace_bytes(1, 256, 64, 3) > 0
     assert lib.geob200_launch_count() == 0
 
 
@@ -62,7 +62,7 @@ def test_structure_embedding_table_size_and_argument_checks():
     assert lib.geob200_launch_count() == 0
 
 
-def test_entry_points_reject_bad_arguments_before_any_launch():
+def test_bad_arguments_are_rejected_before_any_launch():
     """error behaviour of the boundary (the reference raises through TORCH_CHECK, extensions/common/torch_helper.h:6-35): bad sizes /
     empty clouds / non-positive voxel or radius give a negative return code and a message, checked BEFORE any CUDA call -- so this
     runs without a GPU and the launch counter stays at zero"""
@@ -81,8 +81,10 @@ def test_entry_points_reject_bad_arguments_before_any_launch():
     assert lib.geob200_radius_search(p, 0, p, 5, p, p, 1, 0.1, 8, p, p, p, p, 1 << 16, None) < 0 and 'empty input' in err()
     assert lib.geob200_radius_search(p, 5, p, 5, p, p, 1, -1.0, 8, p, p, p, p, 1 << 16, None) < 0 and 'radius' in err()
     assert lib.geob200_neighbor_histogram(p, 0, 8, 5, 16, p, None) < 0 and 'empty input' in err()
-    assert lib.geob200_gse_indices(p, 0, 0.2, 3.8, 3, p, p, None) < 0 and 'empty cloud' in err()
-    assert lib.geob200_gse_indices(p, 10, 0.2, 3.8, 5, p, p, None) < 0 and 'angle_k' in err()
+    rows = (ctypes.c_int64 * 1)(0)
+    assert lib.geob200_gse_indices_batched(p, 1, rows, 0.2, 3.8, 3, p, p, None) < 0 and 'empty cloud' in err()
+    rows[0] = 10
+    assert lib.geob200_gse_indices_batched(p, 1, rows, 0.2, 3.8, 5, p, p, None) < 0 and 'angle_k' in err()
     assert lib.geob200_launch_count() == 0
 
 

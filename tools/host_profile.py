@@ -72,7 +72,7 @@ with torch.cuda.stream(stream), _lib.stream_scope(stream.cuda_stream):
     t0 = time.perf_counter()
     pr.enable()
     for p in pairs[:16]:
-        eng._one(0, p, False)
+        eng._batch(0, [p], False)
     pr.disable()
     dt = time.perf_counter() - t0
 print(f'single stream, profiled: {dt / 16 * 1e3:.2f} ms per pair wall')
