@@ -91,6 +91,12 @@ _sig('geob200_fine_matching_loss_batched', c_int, P, P, P, P, P, P, I64, I64, I6
 _sig('geob200_ransac_correspondences_batched_workspace_bytes', SZ, I64, I64)
 _sig('geob200_ransac_correspondences_batched', c_int, P, P, I64, I64, P, F, I64, I64, ctypes.c_uint64, I64, P, P, P, P, P, P, P, P, P, P,
      SZ, P)
+_sig('geob200_feature_nn_batched_workspace_bytes', SZ, I64, I64, I64)
+_sig('geob200_feature_nn_batched', c_int, P, P, I64, I64, I64, I64, P, P, P, P, P, P, P, SZ, P)
+_sig('geob200_feature_corr_indices', c_int, P, P, P, P, I64, I64, I32, P, P, P, P, P)
+_sig('geob200_ransac_features_batched_workspace_bytes', SZ, I64, I64, I64, I64, I64)
+_sig('geob200_ransac_features_batched', c_int, P, P, P, P, I64, I64, I64, I64, P, P, F, I64, I64, I64, ctypes.c_uint64, I64, P, P, P, P, P,
+     P, P, P, P, P, P, P, P, P, SZ, P)
 _sig('geob200_correspondence_metrics_batched_workspace_bytes', SZ, I64, I64)
 _sig('geob200_correspondence_metrics_batched', c_int, P, P, I64, I64, P, P, I64, F, P, I64, P, SZ, P)
 _sig('geob200_corr_order_batched', c_int, P, I64, I64, P, I64, P, P)

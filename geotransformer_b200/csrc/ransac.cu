@@ -18,6 +18,7 @@
 //     a best hypothesis without inliers, or n < ransac_n, gives Open3D's default result (identity, fitness 0, rmse 0).
 #include "common.cuh"
 #include "geob200.h"
+#include "feature_match.cuh"
 #include "kabsch.cuh"
 
 namespace geob200 {
@@ -280,6 +281,283 @@ __global__ void __launch_bounds__(32) cm_finish_kernel(const double* __restrict_
     }
 }
 
+// ---- feature-matching RANSAC (utils/open3d.py:133-166, Open3D 0.11 registration_ransac_based_on_feature_matching) ---------------
+// The src -> ref descriptor matches come from feature_match.cu.  Then, per pair (DESIGN.md section 3b):
+//   build     one thread per iteration: Philox sample (the stream above), edge-length check, Kabsch, distance check -> pass flag;
+//   validate  one CTA per pair: ordered prefix count over the pass flags -> the first V passing iterations;
+//   grid      a hashed uniform grid of the ref cloud (cell 1.001 tau, so every point within tau lies in the 27 cells around);
+//   score     one CTA per validated hypothesis: every src point transformed (pinned fp32), nearest ref point over the 27 cells;
+//   select    ransac_select_kernel over the validated slots (slot order = iteration order), then slot -> iteration.
+constexpr int FR_THREADS = 128, FR_SCORE_THREADS = 256;
+constexpr double FR_CELL = 1.001;
+
+// Grid (ceil(I / 128), B).  Iteration i of pair p; coordinates in double, every operation rounded on its own.
+__global__ void __launch_bounds__(FR_THREADS) fr_build_kernel(const float* __restrict__ src, const float* __restrict__ ref, int cap_s, int cap_r,
+                                                              const int32_t* __restrict__ ns_c, const int32_t* __restrict__ nr_c,
+                                                              const int64_t* __restrict__ match, double tau, int rn, int I, uint32_t key0,
+                                                              uint32_t key1, uint32_t pair_base, float* __restrict__ hyp_rt,
+                                                              int* __restrict__ pass, int* __restrict__ rec_samples) {
+    const int p = blockIdx.y, i = blockIdx.x * FR_THREADS + threadIdx.x;
+    if (i >= I) return;
+    const int n = rs_count(ns_c, p, cap_s), nr = rs_count(nr_c, p, cap_r);
+    src += 3ll * p * cap_s; ref += 3ll * p * cap_r; match += (long long)p * cap_s;
+    int idx[RS_MAX_N];
+#pragma unroll
+    for (int j = 0; j < RS_MAX_N; ++j) idx[j] = -1;
+    int ok = 0;
+    if (n >= rn && nr > 0) {
+        uint32_t c[4];
+        float s[RS_MAX_N][3], t[RS_MAX_N][3];
+#pragma unroll
+        for (int j = 0; j < RS_MAX_N; ++j) {
+            if (j % 4 == 0) { c[0] = (uint32_t)i; c[1] = pair_base + (uint32_t)p; c[2] = (uint32_t)(j / 4); c[3] = 0u; philox4x32_10(c, key0, key1); }
+            if (j < rn) {
+                idx[j] = (int)__umulhi(c[j % 4], (uint32_t)n);
+                const long long m = match[idx[j]];
+                for (int a = 0; a < 3; ++a) { s[j][a] = src[3 * idx[j] + a]; t[j][a] = ref[3 * m + a]; }
+            }
+        }
+        ok = 1;
+        // CorrespondenceCheckerBasedOnEdgeLength(0.9): every edge of the sample, |s_j - s_k| against |t_j - t_k|
+#pragma unroll
+        for (int j = 0; j < RS_MAX_N; ++j)
+#pragma unroll
+            for (int k = j + 1; k < RS_MAX_N; ++k)
+                if (k < rn) {
+                    double ds = 0.0, dt = 0.0;
+                    for (int a = 0; a < 3; ++a) {
+                        const double u = __dsub_rn((double)s[j][a], (double)s[k][a]), v = __dsub_rn((double)t[j][a], (double)t[k][a]);
+                        ds = __dadd_rn(ds, __dmul_rn(u, u)); dt = __dadd_rn(dt, __dmul_rn(v, v));
+                    }
+                    ds = sqrt(ds); dt = sqrt(dt);
+                    if (ds < __dmul_rn(0.9, dt) || dt < __dmul_rn(0.9, ds)) ok = 0;
+                }
+        if (ok) {
+            double cs[3] = {0, 0, 0}, cr[3] = {0, 0, 0};
+#pragma unroll
+            for (int j = 0; j < RS_MAX_N; ++j)
+                if (j < rn)
+                    for (int a = 0; a < 3; ++a) { cs[a] += (double)s[j][a]; cr[a] += (double)t[j][a]; }
+            for (int a = 0; a < 3; ++a) { cs[a] /= rn; cr[a] /= rn; }
+            double H[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}, R[9], tr[3];
+#pragma unroll
+            for (int j = 0; j < RS_MAX_N; ++j)
+                if (j < rn)
+                    for (int a = 0; a < 3; ++a)
+                        for (int b = 0; b < 3; ++b) H[3 * a + b] += ((double)s[j][a] - cs[a]) * ((double)t[j][b] - cr[b]);
+            kabsch_rotation(H, R);
+            for (int a = 0; a < 3; ++a) tr[a] = cr[a] - (R[3 * a] * cs[0] + R[3 * a + 1] * cs[1] + R[3 * a + 2] * cs[2]);
+            // CorrespondenceCheckerBasedOnDistance(tau): |R s_j + t - t_j| <= tau for every sample, on the double (R, t)
+#pragma unroll
+            for (int j = 0; j < RS_MAX_N; ++j)
+                if (j < rn) {
+                    double d2 = 0.0;
+                    for (int a = 0; a < 3; ++a) {
+                        const double y = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(R[3 * a], (double)s[j][0]), __dmul_rn(R[3 * a + 1], (double)s[j][1])),
+                                                             __dmul_rn(R[3 * a + 2], (double)s[j][2])), tr[a]);
+                        const double e = __dsub_rn(y, (double)t[j][a]);
+                        d2 = __dadd_rn(d2, __dmul_rn(e, e));
+                    }
+                    if (sqrt(d2) > tau) ok = 0;
+                }
+            if (ok) {
+                float* o = hyp_rt + 12 * ((long long)p * I + i);
+                for (int a = 0; a < 3; ++a) {
+                    for (int b = 0; b < 3; ++b) o[4 * a + b] = (float)R[3 * a + b];
+                    o[4 * a + 3] = (float)tr[a];
+                }
+            }
+        }
+    }
+    pass[(long long)p * I + i] = ok;
+    if (rec_samples != nullptr)
+        for (int j = 0; j < RS_MAX_N; ++j) rec_samples[((long long)p * I + i) * RS_MAX_N + j] = idx[j];
+}
+
+// One CTA of 1024 threads per pair: val_ids[p][k] = the k-th passing iteration (k < V), -1 beyond; nval[p] = their number.
+__global__ void __launch_bounds__(1024) fr_validate_kernel(const int* __restrict__ pass, int I, int V, int* __restrict__ val_ids,
+                                                           int32_t* __restrict__ nval) {
+    __shared__ int wsum[32];
+    const int p = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    pass += (long long)p * I; val_ids += (long long)p * V;
+    int base = 0;
+    for (int c0 = 0; c0 < I && base < V; c0 += 1024) {              // base is uniform over the CTA
+        const int i = c0 + tid;
+        const int f = i < I ? pass[i] : 0;
+        int incl = f;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const int v = __shfl_up_sync(0xffffffffu, incl, o);
+            if (lane >= o) incl += v;
+        }
+        if (lane == 31) wsum[warp] = incl;
+        __syncthreads();
+        if (warp == 0) {
+            const int w = wsum[lane];
+            int wi = w;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const int v = __shfl_up_sync(0xffffffffu, wi, o);
+                if (lane >= o) wi += v;
+            }
+            wsum[lane] = wi - w;
+        }
+        __syncthreads();
+        const int k = base + wsum[warp] + incl - f;
+        if (f && k < V) val_ids[k] = i;
+        const int last = __shfl_sync(0xffffffffu, wsum[warp] + incl, 31);
+        __syncthreads();
+        if (tid == 1023) wsum[0] = last;
+        __syncthreads();
+        base += wsum[0];
+        __syncthreads();
+    }
+    const int nv = min(base, V);
+    for (int k = nv + tid; k < V; k += 1024) val_ids[k] = -1;
+    if (tid == 0) nval[p] = nv;
+}
+
+__device__ __forceinline__ long long fr_cell(float x, double inv_cell) {
+    return (long long)fmin(fmax(floor((double)x * inv_cell), -1e15), 1e15);
+}
+
+__device__ __forceinline__ int fr_hash(long long x, long long y, long long z, int H) {
+    return (int)(((unsigned long long)x * 73856093ull ^ (unsigned long long)y * 19349663ull ^ (unsigned long long)z * 83492791ull) &
+                 (unsigned long long)(H - 1));
+}
+
+// Grid (ceil(cap_r / 256), B): bucket of every ref point, and the bucket sizes.
+__global__ void __launch_bounds__(256) fr_hash_kernel(const float* __restrict__ ref, int cap_r, const int32_t* __restrict__ nr_c, double inv_cell,
+                                                      int H, int* __restrict__ key, int* __restrict__ bcount) {
+    const int p = blockIdx.y, j = blockIdx.x * 256 + threadIdx.x;
+    if (j >= rs_count(nr_c, p, cap_r)) return;
+    const float* r = ref + 3ll * ((long long)p * cap_r + j);
+    const int b = fr_hash(fr_cell(r[0], inv_cell), fr_cell(r[1], inv_cell), fr_cell(r[2], inv_cell), H);
+    key[(long long)p * cap_r + j] = b;
+    atomicAdd(bcount + (long long)p * (H + 1) + b, 1);
+}
+
+// One CTA of 1024 threads per pair: bucket sizes -> exclusive bucket starts (entry H = the point count), copied to the cursors.
+__global__ void __launch_bounds__(1024) fr_scan_kernel(int* __restrict__ bstart, int* __restrict__ cursor, int H) {
+    __shared__ int wsum[32];
+    const int p = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    bstart += (long long)p * (H + 1); cursor += (long long)p * (H + 1);
+    int base = 0;
+    for (int c0 = 0; c0 <= H; c0 += 1024) {
+        const int i = c0 + tid;
+        const int f = i < H ? bstart[i] : 0;
+        int incl = f;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const int v = __shfl_up_sync(0xffffffffu, incl, o);
+            if (lane >= o) incl += v;
+        }
+        if (lane == 31) wsum[warp] = incl;
+        __syncthreads();
+        if (warp == 0) {
+            const int w = wsum[lane];
+            int wi = w;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const int v = __shfl_up_sync(0xffffffffu, wi, o);
+                if (lane >= o) wi += v;
+            }
+            wsum[lane] = wi - w;
+        }
+        __syncthreads();
+        const int start = base + wsum[warp] + incl - f;
+        if (i <= H) { bstart[i] = start; cursor[i] = start; }
+        const int last = __shfl_sync(0xffffffffu, wsum[warp] + incl, 31);
+        __syncthreads();
+        if (tid == 1023) wsum[0] = last;
+        __syncthreads();
+        base += wsum[0];
+        __syncthreads();
+    }
+}
+
+// Ref points into bucket order (the order inside a bucket is arbitrary: the score only takes minima over it).
+__global__ void __launch_bounds__(256) fr_scatter_kernel(const float* __restrict__ ref, int cap_r, const int32_t* __restrict__ nr_c, int H,
+                                                         const int* __restrict__ key, int* __restrict__ cursor, float4* __restrict__ sorted) {
+    const int p = blockIdx.y, j = blockIdx.x * 256 + threadIdx.x;
+    if (j >= rs_count(nr_c, p, cap_r)) return;
+    const long long q = (long long)p * cap_r + j;
+    const int pos = atomicAdd(cursor + (long long)p * (H + 1) + key[q], 1);
+    sorted[(long long)p * cap_r + pos] = make_float4(ref[3 * q], ref[3 * q + 1], ref[3 * q + 2], 0.f);
+}
+
+// Grid (V, B), 256 threads: validated slot v of pair p.  Per src point: position under (R, t) as rs_residual2 forms it, nearest
+// ref point over the 27 cells with d^2 = (dx^2 + dy^2) + dz^2 pinned; inlier when d^2 < tau^2.  Fixed reduction order.
+__global__ void __launch_bounds__(FR_SCORE_THREADS, 1) fr_score_kernel(const float* __restrict__ src, int cap_s, int cap_r,
+                                                                    const int32_t* __restrict__ ns_c, const float* __restrict__ hyp_rt, int I,
+                                                                    const int* __restrict__ val_ids, const int32_t* __restrict__ nval, int V,
+                                                                    const int* __restrict__ bstart, const float4* __restrict__ sorted, int H,
+                                                                    double inv_cell, float tau2, float* __restrict__ v_rt,
+                                                                    int* __restrict__ v_cnt, float* __restrict__ v_rmse,
+                                                                    float* __restrict__ rec_T) {
+    __shared__ float h[12];
+    __shared__ int rc[FR_SCORE_THREADS / 32];
+    __shared__ double rsum[FR_SCORE_THREADS / 32];
+    const int p = blockIdx.y, v = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const long long q = (long long)p * V + v;
+    const bool live = v < nval[p];
+    if (tid < 12) h[tid] = live ? hyp_rt[12 * ((long long)p * I + val_ids[q]) + tid] : ((tid % 5 == 0) ? 1.f : 0.f);
+    __syncthreads();
+    int cnt = 0;
+    double sum = 0.0;
+    if (live) {
+        const int n = rs_count(ns_c, p, cap_s);
+        src += 3ll * p * cap_s; bstart += (long long)p * (H + 1); sorted += (long long)p * cap_r;
+        for (int j = tid; j < n; j += FR_SCORE_THREADS) {
+            const float x = src[3 * j], y = src[3 * j + 1], z = src[3 * j + 2];
+            const float ax = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(h[0], x), __fmul_rn(h[1], y)), __fmul_rn(h[2], z)), h[3]);
+            const float ay = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(h[4], x), __fmul_rn(h[5], y)), __fmul_rn(h[6], z)), h[7]);
+            const float az = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(h[8], x), __fmul_rn(h[9], y)), __fmul_rn(h[10], z)), h[11]);
+            const long long cx = fr_cell(ax, inv_cell), cy = fr_cell(ay, inv_cell), cz = fr_cell(az, inv_cell);
+            float best = INFINITY;
+#pragma unroll 1
+            for (int cell = 0; cell < 27; ++cell) {
+                const int b = fr_hash(cx + cell % 3 - 1, cy + (cell / 3) % 3 - 1, cz + cell / 9 - 1, H);
+                const int e = bstart[b + 1];
+                for (int k = bstart[b]; k < e; ++k) {
+                    const float4 r = sorted[k];
+                    const float ex = __fsub_rn(ax, r.x), ey = __fsub_rn(ay, r.y), ez = __fsub_rn(az, r.z);
+                    best = fminf(best, __fadd_rn(__fadd_rn(__fmul_rn(ex, ex), __fmul_rn(ey, ey)), __fmul_rn(ez, ez)));
+                }
+            }
+            if (best < tau2) { ++cnt; sum += (double)best; }
+        }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+    sum = warp_sum_d(sum);
+    if (lane == 0) { rc[warp] = cnt; rsum[warp] = sum; }
+    __syncthreads();
+    if (tid < 12) v_rt[12 * q + tid] = h[tid];
+    if (rec_T != nullptr && tid < 16) rec_T[16 * q + tid] = tid < 12 ? h[tid] : (tid == 15 ? 1.f : 0.f);
+    if (tid == 0) {
+        int c = 0;
+        double s = 0.0;
+        for (int w = 0; w < FR_SCORE_THREADS / 32; ++w) { c += rc[w]; s += rsum[w]; }
+        v_cnt[q] = c;
+        v_rmse[q] = c > 0 ? (float)__dsqrt_rn(__ddiv_rn(s, (double)c)) : 0.f;
+    }
+}
+
+// slot -> iteration; the default result for the degenerate arguments (no launch of the pipeline at all)
+__global__ void fr_finish_kernel(int B, const int* __restrict__ val_ids, int V, int* __restrict__ best_iter, float* __restrict__ T,
+                                 float* __restrict__ fitness, float* __restrict__ rmse, int* __restrict__ inliers, int32_t* __restrict__ nval,
+                                 bool degenerate) {
+    const int p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= B) return;
+    if (degenerate) {
+        for (int e = 0; e < 16; ++e) T[16ll * p + e] = (e % 5 == 0) ? 1.f : 0.f;
+        fitness[p] = 0.f; rmse[p] = 0.f; inliers[p] = 0; best_iter[p] = -1; nval[p] = 0;
+    } else if (best_iter[p] >= 0) {
+        best_iter[p] = val_ids[(long long)p * V + best_iter[p]];
+    }
+}
+
 }  // namespace geob200
 
 using namespace geob200;
@@ -323,6 +601,105 @@ int geob200_ransac_correspondences_batched(const float* ref_corr_points, const f
                                             best_iteration);
     GEOB_CHECK_LAUNCH();
     count_launches(2);
+    return 0;
+}
+
+static int fr_hash_size(int64_t cap_ref) {
+    int H = 1024;
+    while (H < 2 * cap_ref) H <<= 1;
+    return H;
+}
+
+size_t geob200_ransac_features_batched_workspace_bytes(int64_t n_pairs, int64_t cap_src, int64_t cap_ref, int64_t num_iterations,
+                                                       int64_t val_iterations) {
+    const size_t B = (size_t)(n_pairs > 0 ? n_pairs : 0), cs = (size_t)(cap_src > 0 ? cap_src : 0), cr = (size_t)(cap_ref > 0 ? cap_ref : 0);
+    const size_t I = (size_t)(num_iterations > 0 ? num_iterations : 0);
+    const size_t V = std::min(I, (size_t)(val_iterations > 0 ? val_iterations : 0));
+    const size_t H = (size_t)fr_hash_size((int64_t)cr);
+    return feature_nn_workspace(n_pairs, cap_src, cap_ref) + align_up(8 * B * cs, 256) + align_up(8 * B * cs, 256) +
+           align_up(48 * B * I, 256) + align_up(4 * B * I, 256) + align_up(4 * B * V, 256) + align_up(48 * B * V, 256) +
+           2 * align_up(4 * B * V, 256) + 2 * align_up(4 * B * (H + 1), 256) + align_up(4 * B * cr, 256) + align_up(16 * B * cr, 256) + 256;
+}
+
+int geob200_ransac_features_batched(const float* src_points, const float* ref_points, const float* src_feats, const float* ref_feats,
+                                    int64_t n_pairs, int64_t cap_src, int64_t cap_ref, int64_t channels, const int32_t* n_src,
+                                    const int32_t* n_ref, float distance_threshold, int64_t ransac_n, int64_t num_iterations,
+                                    int64_t val_iterations, uint64_t seed, int64_t pair_base, float* transforms, float* fitness,
+                                    float* inlier_rmse, int32_t* inlier_count, int32_t* best_iteration, int32_t* num_validated,
+                                    int64_t* rec_matches, int32_t* rec_samples, int32_t* rec_pass, int32_t* rec_val_ids,
+                                    float* rec_transforms, int32_t* rec_inliers, float* rec_rmse, void* workspace, size_t workspace_bytes,
+                                    void* stream) {
+    GEOB_REQUIRE(ransac_n >= 0 && ransac_n <= RS_MAX_N, "ransac_features: ransac_n must be in 0..%d", RS_MAX_N);
+    GEOB_REQUIRE(num_iterations >= 0 && num_iterations <= (1ll << 30), "ransac_features: num_iterations must be in 0..2^30");
+    GEOB_REQUIRE(val_iterations >= 0 && val_iterations <= (1ll << 30), "ransac_features: val_iterations must be in 0..2^30");
+    GEOB_REQUIRE(channels >= 1 && channels <= 1024, "ransac_features: channels must be in 1..1024");
+    GEOB_REQUIRE(n_pairs > 0 && n_pairs <= 65535, "ransac_features: 1..65535 pairs");
+    GEOB_REQUIRE(pair_base >= 0 && pair_base + n_pairs <= (1ll << 32), "ransac_features: pair ids must fit 32 bits");
+    GEOB_REQUIRE(cap_src >= 0 && cap_ref >= 0 && cap_src < (1ll << 28) && cap_ref < (1ll << 28), "ransac_features: capacities must be in 0..2^28");
+    GEOB_REQUIRE((src_points != nullptr && src_feats != nullptr) || cap_src == 0, "ransac_features: null src points / descriptors");
+    GEOB_REQUIRE((ref_points != nullptr && ref_feats != nullptr) || cap_ref == 0, "ransac_features: null ref points / descriptors");
+    GEOB_REQUIRE(transforms != nullptr && fitness != nullptr && inlier_rmse != nullptr && inlier_count != nullptr && best_iteration != nullptr &&
+                     num_validated != nullptr, "ransac_features: null output");
+    GEOB_REQUIRE(workspace != nullptr && workspace_bytes >= geob200_ransac_features_batched_workspace_bytes(n_pairs, cap_src, cap_ref,
+                                                                                                          num_iterations, val_iterations),
+                 "ransac_features: workspace too small");
+    const int B = (int)n_pairs, cs = (int)cap_src, cr = (int)cap_ref, rn = (int)ransac_n, I = (int)num_iterations;
+    const int V = (int)std::min(num_iterations, val_iterations), H = fr_hash_size(cap_ref);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (rn < 3 || !(distance_threshold > 0.f) || V == 0) {      // Open3D's default result
+        fr_finish_kernel<<<(B + 127) / 128, 128, 0, st>>>(B, nullptr, 0, best_iteration, transforms, fitness, inlier_rmse, inlier_count,
+                                                          num_validated, true);
+        GEOB_CHECK_LAUNCH();
+        count_launches(1);
+        return 0;
+    }
+    const size_t nn_ws = feature_nn_workspace(n_pairs, cap_src, cap_ref);
+    Arena ar((char*)workspace + nn_ws, workspace_bytes - nn_ws);
+    int64_t* match = ar.take<int64_t>((size_t)B * cs);
+    double* mdist = ar.take<double>((size_t)B * cs);
+    float* hyp_rt = ar.take<float>((size_t)B * I * 12);
+    int* pass = ar.take<int>((size_t)B * I);
+    int* val_ids = ar.take<int>((size_t)B * V);
+    float* v_rt = ar.take<float>((size_t)B * V * 12);
+    int* v_cnt = ar.take<int>((size_t)B * V);
+    float* v_rmse = ar.take<float>((size_t)B * V);
+    int* bstart = ar.take<int>((size_t)B * (H + 1));
+    int* cursor = ar.take<int>((size_t)B * (H + 1));
+    int* key = ar.take<int>((size_t)B * cr);
+    float4* sorted = ar.take<float4>((size_t)B * cr);
+    GEOB_REQUIRE(ar.ok(), "ransac_features: workspace too small");
+    if (rec_matches != nullptr) match = rec_matches;
+    if (rec_pass != nullptr) pass = rec_pass;
+    if (rec_val_ids != nullptr) val_ids = rec_val_ids;
+    if (rec_inliers != nullptr) v_cnt = rec_inliers;
+    if (rec_rmse != nullptr) v_rmse = rec_rmse;
+    int nl = 0;
+    if (feature_nn_launch(src_feats, ref_feats, B, cs, cr, (int)channels, n_src, n_ref, match, mdist, nullptr, nullptr, workspace, nn_ws, st,
+                          &nl) != 0)
+        return -1;
+    const double tau = (double)distance_threshold, inv_cell = 1.0 / (FR_CELL * tau);
+    fr_build_kernel<<<dim3((unsigned)((I + FR_THREADS - 1) / FR_THREADS), B), FR_THREADS, 0, st>>>(
+        src_points, ref_points, cs, cr, n_src, n_ref, match, tau, rn, I, (uint32_t)seed, (uint32_t)(seed >> 32), (uint32_t)pair_base, hyp_rt,
+        pass, rec_samples);
+    fr_validate_kernel<<<B, 1024, 0, st>>>(pass, I, V, val_ids, num_validated);
+    GEOB_CHECK_CUDA(cudaMemsetAsync(bstart, 0, 4 * (size_t)B * (H + 1), st));
+    nl += 2;
+    if (cr > 0) {
+        fr_hash_kernel<<<dim3((cr + 255) / 256, B), 256, 0, st>>>(ref_points, cr, n_ref, inv_cell, H, key, bstart);
+        fr_scan_kernel<<<B, 1024, 0, st>>>(bstart, cursor, H);
+        fr_scatter_kernel<<<dim3((cr + 255) / 256, B), 256, 0, st>>>(ref_points, cr, n_ref, H, key, cursor, sorted);
+        nl += 3;
+    }
+    fr_score_kernel<<<dim3((unsigned)V, B), FR_SCORE_THREADS, 0, st>>>(src_points, cs, cr, n_src, hyp_rt, I, val_ids, num_validated, V, bstart,
+                                                                       sorted, H, inv_cell, (float)(distance_threshold * distance_threshold),
+                                                                       v_rt, v_cnt, v_rmse, rec_transforms);
+    ransac_select_kernel<<<B, 256, 0, st>>>(n_src, cs, rn, V, v_rt, v_cnt, v_rmse, transforms, fitness, inlier_rmse, inlier_count,
+                                            best_iteration);
+    fr_finish_kernel<<<(B + 127) / 128, 128, 0, st>>>(B, val_ids, V, best_iteration, transforms, fitness, inlier_rmse, inlier_count,
+                                                      num_validated, false);
+    nl += 3;
+    GEOB_CHECK_LAUNCH();
+    count_launches(nl);
     return 0;
 }
 

@@ -978,6 +978,150 @@ def ransac_correspondences(src_corr_points, ref_corr_points, distance_threshold,
     return {k: v[0] for k, v in res.items()}
 
 
+# ------------------------------------------------------------------------------------------------ feature matching
+# get_nearest_neighbor / extract_corr_indices_from_feats (utils/pointcloud.py:11-22, utils/registration.py:179-234) and Open3D 0.11's
+# registration_ransac_based_on_feature_matching as utils/open3d.py:133-166 calls it (csrc/feature_match.cu, csrc/ransac.cu;
+# semantics and deviations in DESIGN.md section 3b).  Ragged layout: pair p's rows are [0, count[p]) of (B, capacity, .) tensors.
+
+def _ragged(x, name, B=None, width=None):
+    _f(x, name)
+    if x.ndim != 3 or (B is not None and x.shape[0] != B) or (width is not None and x.shape[2] != width):
+        raise ValueError(f'{name} must be (B, capacity, {width or "C"})')
+    return x
+
+
+def feature_nearest_neighbor_batched(query, support, num_query=None, num_support=None, bidirectional=False):
+    """Exact nearest support row of every query row: (B, cap_q, C) and (B, cap_s, C) float32, C in 1..1024; counts (B,) device int32
+    or None.  Returns (index (B, cap_q) int64, distance (B, cap_q) float64) -- index = argmin of the fp64 squared distance (lowest
+    index on exact ties), distance = its sqrt; rows past the count: -1 / NaN.  ``bidirectional``: also the nearest query row of
+    every support row, as a second (index, distance) pair."""
+    _ragged(query, 'query'); _ragged(support, 'support', query.shape[0], query.shape[2])
+    B, cq, C = query.shape
+    cs = support.shape[1]
+    dev = query.device
+    if support.device != dev:
+        raise RuntimeError('feature_nearest_neighbor_batched: query and support must be on one device')
+    _counts(num_query, B, dev, 'feature_nearest_neighbor_batched')
+    _counts(num_support, B, dev, 'feature_nearest_neighbor_batched')
+    lib = L.lib()
+    qi = torch.empty((B, cq), dtype=_i64, device=dev)
+    qd = torch.empty((B, cq), dtype=torch.float64, device=dev)
+    si = torch.empty((B, cs), dtype=_i64, device=dev) if bidirectional else None
+    sd = torch.empty((B, cs), dtype=torch.float64, device=dev) if bidirectional else None
+    ws = L.workspace(lib.geob200_feature_nn_batched_workspace_bytes(B, cq, cs), dev, tag='feature_nn')
+    L.check(lib.geob200_feature_nn_batched(query.data_ptr(), support.data_ptr(), B, cq, cs, C, L.ptr(num_query), L.ptr(num_support),
+                                           qi.data_ptr(), qd.data_ptr(), L.ptr(si), L.ptr(sd), ws.data_ptr(), ws.numel(), L.stream_ptr()),
+            'feature_nearest_neighbor_batched')
+    return (qi, qd, si, sd) if bidirectional else (qi, qd)
+
+
+def feature_nearest_neighbor(query, support, bidirectional=False):
+    """One pair: (N, C) query, (M, C) support -> (index (N,) int64, distance (N,) float64)[, (M,) support -> query pair]."""
+    res = feature_nearest_neighbor_batched(query.unsqueeze(0), support.unsqueeze(0), bidirectional=bidirectional)
+    return tuple(v[0] for v in res)
+
+
+CORR_MODES = {'plain': 0, 'mutual': 1, 'bilateral': 2}
+
+
+def feature_correspondences(ref_nn, ref_dist, src_nn=None, src_dist=None, mode='plain'):
+    """extract_corr_indices_from_feats from the two nearest-neighbour directions of one pair (ref -> src: ref_nn / ref_dist (N,);
+    src -> ref: src_nn / src_dist (M,), needed for 'mutual' and 'bilateral').  Returns (ref indices, src indices) int64 and the
+    listed pairs' descriptor distances (float32).  The mutual count is read back to the host (the lists' length)."""
+    m = CORR_MODES[mode]
+    for t, name in ((ref_nn, 'ref_nn'), (src_nn, 'src_nn')):
+        if t is not None:
+            L.require_cuda(t, name, _i64)
+    for t, name in ((ref_dist, 'ref_dist'), (src_dist, 'src_dist')):
+        if t is not None:
+            L.require_cuda(t, name, torch.float64)
+    if m and (src_nn is None or src_dist is None):
+        raise ValueError(f'feature_correspondences: mode {mode!r} needs both directions')
+    n, k = ref_nn.numel(), (0 if src_nn is None else src_nn.numel())
+    dev = ref_nn.device
+    rows = n + k if m == 2 else n
+    ref_corr = torch.empty((rows,), dtype=_i64, device=dev)
+    src_corr = torch.empty((rows,), dtype=_i64, device=dev)
+    dist = torch.empty((rows,), dtype=_f32, device=dev)
+    cnt = torch.empty((1,), dtype=_i32, device=dev)
+    L.check(L.lib().geob200_feature_corr_indices(ref_nn.data_ptr(), ref_dist.data_ptr(), L.ptr(src_nn), L.ptr(src_dist), n, k, m,
+                                                 ref_corr.data_ptr(), src_corr.data_ptr(), dist.data_ptr(), cnt.data_ptr(),
+                                                 L.stream_ptr()), 'feature_correspondences')
+    if m == 1:
+        c = int(cnt.item())
+        ref_corr, src_corr, dist = ref_corr[:c], src_corr[:c], dist[:c]
+    return ref_corr, src_corr, dist
+
+
+FEATURE_RANSAC_KEYS = RANSAC_KEYS + ('num_validated',)
+
+
+def ransac_features_batched(src_points, ref_points, src_feats, ref_feats, distance_threshold, ransac_n, num_iterations, val_iterations,
+                            seed=0, num_src=None, num_ref=None, records=False, first_pair=0):
+    """Feature-matching RANSAC of B pairs in one call, no host synchronisation: src (B, cap_src, 3) points and (B, cap_src, C)
+    descriptors, ref likewise; num_src / num_ref (B,) device int32 or None.  Pair p draws from the stream (seed, first_pair + p), so
+    a pair gives the same bits alone (``first_pair`` = its id) as inside any batch.
+    Returns a dict: transform (B, 4, 4), fitness, inlier_rmse, inliers int32, iteration int32 (the winning iteration, -1 for the
+    default result: identity, fitness 0), num_validated int32.  ``records``: also matches (B, cap_src) int64, samples
+    (B, I, ransac_n) int32, pass_flags (B, I) int32, val_ids (B, V') int32 (-1 past num_validated), val_transforms (B, V', 4, 4),
+    val_inliers (B, V'), val_rmse (B, V') with V' = min(val_iterations, num_iterations)."""
+    _ragged(src_points, 'src_points', width=3)
+    B = src_points.shape[0]
+    _ragged(ref_points, 'ref_points', B, 3)
+    _ragged(src_feats, 'src_feats', B); _ragged(ref_feats, 'ref_feats', B, src_feats.shape[2])
+    if src_feats.shape[1] != src_points.shape[1] or ref_feats.shape[1] != ref_points.shape[1]:
+        raise ValueError('ransac_features_batched: points and descriptors need the same capacity')
+    if not 0 <= int(seed) < 1 << 64:
+        raise ValueError('ransac_features_batched: seed must be a 64-bit unsigned integer')
+    dev = src_points.device
+    if any(t.device != dev for t in (ref_points, src_feats, ref_feats)):
+        raise RuntimeError('ransac_features_batched: all inputs must be on one device')
+    _counts(num_src, B, dev, 'ransac_features_batched')
+    _counts(num_ref, B, dev, 'ransac_features_batched')
+    cs, cr, C = src_points.shape[1], ref_points.shape[1], src_feats.shape[2]
+    I, V = int(num_iterations), int(val_iterations)
+    Vr = max(min(I, V), 1)
+    lib = L.lib()
+    T = torch.empty((B, 4, 4), dtype=_f32, device=dev)
+    fit = torch.empty((B,), dtype=_f32, device=dev)
+    rmse = torch.empty((B,), dtype=_f32, device=dev)
+    inl = torch.empty((B,), dtype=_i32, device=dev)
+    it = torch.empty((B,), dtype=_i32, device=dev)
+    nv = torch.empty((B,), dtype=_i32, device=dev)
+    rec = None
+    if records:
+        rec = dict(matches=torch.full((B, max(cs, 1)), -1, dtype=_i64, device=dev),
+                   samples=torch.full((B, max(I, 1), 8), -1, dtype=_i32, device=dev),
+                   pass_flags=torch.zeros((B, max(I, 1)), dtype=_i32, device=dev),
+                   val_ids=torch.full((B, Vr), -1, dtype=_i32, device=dev),
+                   val_transforms=torch.zeros((B, Vr, 4, 4), dtype=_f32, device=dev),
+                   val_inliers=torch.zeros((B, Vr), dtype=_i32, device=dev),
+                   val_rmse=torch.zeros((B, Vr), dtype=_f32, device=dev))
+    ws = L.workspace(lib.geob200_ransac_features_batched_workspace_bytes(B, cs, cr, I, V), dev, tag='ransac_features')
+    L.check(lib.geob200_ransac_features_batched(
+        src_points.data_ptr(), ref_points.data_ptr(), src_feats.data_ptr(), ref_feats.data_ptr(), B, cs, cr, C, L.ptr(num_src),
+        L.ptr(num_ref), float(distance_threshold), int(ransac_n), I, V, ctypes.c_uint64(int(seed)), int(first_pair), T.data_ptr(),
+        fit.data_ptr(), rmse.data_ptr(), inl.data_ptr(), it.data_ptr(), nv.data_ptr(),
+        *(None if rec is None else rec[k].data_ptr() for k in ('matches', 'samples', 'pass_flags', 'val_ids', 'val_transforms',
+                                                                'val_inliers', 'val_rmse')),
+        ws.data_ptr(), ws.numel(), L.stream_ptr()), 'ransac_features_batched')
+    res = dict(transform=T, fitness=fit, inlier_rmse=rmse, inliers=inl, iteration=it, num_validated=nv)
+    if rec is not None:
+        rec['samples'] = rec['samples'][:, :, :max(int(ransac_n), 0)]
+        res.update(rec)
+    return res
+
+
+def ransac_features(src_points, ref_points, src_feats, ref_feats, distance_threshold, ransac_n, num_iterations, val_iterations, seed=0,
+                    records=False, pair=0):
+    """Feature-matching RANSAC of one pair: (N, 3) / (N, C) src, (M, 3) / (M, C) ref (``pair``: the pair id of the random stream).
+    Same dict as the batched op without the pair dimension."""
+    res = ransac_features_batched(src_points.unsqueeze(0), ref_points.unsqueeze(0), src_feats.unsqueeze(0), ref_feats.unsqueeze(0),
+                                  distance_threshold, ransac_n, num_iterations, val_iterations, seed=seed, records=records,
+                                  first_pair=pair)
+    return {k: v[0] for k, v in res.items()}
+
+
 CORRESPONDENCE_METRICS = ('f_IR', 'f_OV', 'f_RS', 'f_NU')
 
 

@@ -1,7 +1,9 @@
-"""Correspondence RANSAC with the reference's interface (geotransformer/utils/open3d.py:169-198), on the device, without Open3D.
+"""Correspondence RANSAC and feature-matching RANSAC with the reference's interface (geotransformer/utils/open3d.py:133-198), on
+the device, without Open3D.
 
-The estimate follows Open3D's registration_ransac_based_on_correspondence as the reference calls it; the sampler, the tie rule
-and the fp32 scoring differ from Open3D (DESIGN.md section 3b), so the transform is not Open3D's bit for bit.
+The estimates follow Open3D's registration_ransac_based_on_correspondence and (0.11's) registration_ransac_based_on_feature_matching
+as the reference calls them; the sampler, the tie rule and the fp32 scoring differ from Open3D (DESIGN.md section 3b), so the
+transform is not Open3D's bit for bit.
 """
 import numpy as np
 import torch
@@ -45,6 +47,34 @@ def registration_with_ransac_from_correspondences(src_points, ref_points, corres
     elif src.shape[0] != ref.shape[0]:
         raise ValueError('registration_with_ransac_from_correspondences: without correspondences src and ref need the same rows')
     res = GF.ransac_correspondences(src, ref, distance_threshold, ransac_n, num_iterations, seed=seed)
+    if on_device:
+        return res['transform']
+    return res['transform'].cpu().numpy().astype(np.float64)
+
+
+def registration_with_ransac_from_feats(src_points, ref_points, src_feats, ref_feats, distance_threshold=0.05, ransac_n=3,
+                                        num_iterations=50000, val_iterations=1000, seed=0):
+    r"""Compute the transformation matrix from src_points to ref_points by RANSAC on descriptor matches.
+
+    Follows Open3D 0.11's registration_ransac_based_on_feature_matching as the reference calls it (every src point matched to its
+    nearest ref descriptor, edge-length checker 0.9, distance checker ``distance_threshold``, ``num_iterations`` iterations of which
+    at most ``val_iterations`` passing ones are scored against the whole ref cloud); the sampler, the validated set (the first
+    passing iterations) and the fp32 scoring are the package's (DESIGN.md section 3b).  numpy inputs give a float64 (4, 4) numpy
+    array; CUDA tensors give a float32 (4, 4) device tensor.  ``seed`` keys the sampler."""
+    on_device = any(isinstance(x, torch.Tensor) for x in (src_points, ref_points, src_feats, ref_feats))
+    device = torch.device('cuda', torch.cuda.current_device())
+    for x in (src_points, ref_points, src_feats, ref_feats):
+        if isinstance(x, torch.Tensor):
+            device = x.device
+            break
+    src = _points(src_points, 'src_points', device).reshape(-1, 3)
+    ref = _points(ref_points, 'ref_points', device).reshape(-1, 3)
+    sf = _points(src_feats, 'src_feats', device)
+    rf = _points(ref_feats, 'ref_feats', device)
+    sf, rf = sf.reshape(sf.shape[0], -1), rf.reshape(rf.shape[0], -1)
+    if sf.shape[0] != src.shape[0] or rf.shape[0] != ref.shape[0]:
+        raise ValueError('registration_with_ransac_from_feats: one descriptor row per point')
+    res = GF.ransac_features(src, ref, sf, rf, distance_threshold, ransac_n, num_iterations, val_iterations, seed=seed)
     if on_device:
         return res['transform']
     return res['transform'].cpu().numpy().astype(np.float64)

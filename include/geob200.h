@@ -382,6 +382,49 @@ int geob200_correspondence_metrics_batched(const float* ref_corr_points, const f
                                            const int32_t* num_corr, const float* transforms, int64_t transform_ld, float positive_radius,
                                            float* out, int64_t out_ld, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- feature matching (utils/pointcloud.py:11-22, utils/registration.py:179-234, utils/open3d.py:133-166) --------------------
+ * Exact nearest neighbour in descriptor space for B pairs (feature_match.cu): query (B, cap_query, C) and support
+ * (B, cap_support, C) fp32, device int32 counts n_query / n_support (NULL = all capacity rows), C in 1..1024.  For every query row
+ * q: query_index = argmin over the support rows s of D(q, s) = sum_c (q_c - s_c)^2 in fp64 (c in order, no FMA), the lowest s on
+ * exact ties, and query_dist = sqrt(D).  With support_index / support_dist (both or neither) also every support row's nearest
+ * query row.  Rows past the count: index -1, distance NaN; an empty other side: index -1, distance +inf. */
+size_t geob200_feature_nn_batched_workspace_bytes(int64_t n_pairs, int64_t cap_query, int64_t cap_support);
+int geob200_feature_nn_batched(const float* query, const float* support, int64_t n_pairs, int64_t cap_query, int64_t cap_support,
+                               int64_t channels, const int32_t* n_query, const int32_t* n_support, int64_t* query_index,
+                               double* query_dist, int64_t* support_index, double* support_dist, void* workspace, size_t workspace_bytes,
+                               void* stream);
+/* Correspondence lists of one pair from its two nearest-neighbour directions (extract_corr_indices_from_feats): mode 0 plain
+ * (r <-> ref_nn[r] for every ref row), 1 mutual (only the r with src_nn[ref_nn[r]] == r, increasing r), 2 bilateral (plain, then
+ * src_nn[s] <-> s for every src row).  Outputs hold n_ref (+ n_src for bilateral) rows; count (device) = the rows written;
+ * feat_dist (may be NULL) = the listed pairs' descriptor distances in fp32. */
+int geob200_feature_corr_indices(const int64_t* ref_nn, const double* ref_dist, const int64_t* src_nn, const double* src_dist,
+                                 int64_t n_ref, int64_t n_src, int32_t mode, int64_t* ref_corr, int64_t* src_corr, float* feat_dist,
+                                 int32_t* count, void* stream);
+/* Feature-matching RANSAC (Open3D 0.11's registration_ransac_based_on_feature_matching as utils/open3d.py:133-166 calls it:
+ * edge-length checker 0.9, distance checker tau, RANSACConvergenceCriteria(num_iterations, val_iterations)) for B pairs:
+ * src (B, cap_src, 3) points + (B, cap_src, C) descriptors, ref likewise, device counts n_src / n_ref (NULL = all).
+ * Source row s matches m(s) = its nearest ref descriptor.  Iteration i draws ransac_n src rows with replacement (the Philox stream of
+ * the correspondence RANSAC, counter (i, pair_base + p, j / 4, 0), index = umulhi(word, n_src)); it passes when every sampled edge
+ * satisfies 0.9 d_tgt <= d_src and 0.9 d_src <= d_tgt and the unweighted Kabsch fit leaves every sample within tau (both in
+ * double).  The first min(val_iterations, #passing) passing iterations in iteration order are scored against the WHOLE ref
+ * cloud: a src point is an inlier when its transformed position's nearest ref point has pinned-fp32 d^2 < tau^2; fitness =
+ * inliers / n_src, rmse = sqrt(sum d^2 / inliers).  Winner: higher fitness, then lower rmse, then lower iteration; none with an
+ * inlier, ransac_n < 3, tau <= 0, num_iterations == 0 or val_iterations == 0: identity, fitness 0, rmse 0, iteration -1.
+ * Outputs per pair: transforms (B, 16), fitness, inlier_rmse, inlier_count, best_iteration, num_validated.  Optional records
+ * (each NULL or written): rec_matches (B, cap_src) int64 = m(s), rec_samples (B, I, 8) (-1 past ransac_n), rec_pass (B, I),
+ * rec_val_ids (B, V') (-1 past num_validated), rec_transforms (B, V', 16), rec_inliers (B, V'), rec_rmse (B, V') with
+ * V' = min(val_iterations, num_iterations).  ransac_n in 0..8, C in 1..1024. */
+size_t geob200_ransac_features_batched_workspace_bytes(int64_t n_pairs, int64_t cap_src, int64_t cap_ref, int64_t num_iterations,
+                                                       int64_t val_iterations);
+int geob200_ransac_features_batched(const float* src_points, const float* ref_points, const float* src_feats, const float* ref_feats,
+                                    int64_t n_pairs, int64_t cap_src, int64_t cap_ref, int64_t channels, const int32_t* n_src,
+                                    const int32_t* n_ref, float distance_threshold, int64_t ransac_n, int64_t num_iterations,
+                                    int64_t val_iterations, uint64_t seed, int64_t pair_base, float* transforms, float* fitness,
+                                    float* inlier_rmse, int32_t* inlier_count, int32_t* best_iteration, int32_t* num_validated,
+                                    int64_t* rec_matches, int32_t* rec_samples, int32_t* rec_pass, int32_t* rec_val_ids,
+                                    float* rec_transforms, int32_t* rec_inliers, float* rec_rmse, void* workspace, size_t workspace_bytes,
+                                    void* stream);
+
 /* ---- benchmark evaluation (the experiments' eval.py; benchmark.cu) -------------------------------------------------------------
  * Ragged pairs in the (B, capacity, .) layout with device int32 counts (NULL = all capacity rows), one launch for B pairs, no host
  * sync; a pair gets the same bits alone and in any batch.
