@@ -70,10 +70,14 @@ _sig('geob200_head_bias', c_int, P, I64, P, I64, I64, I64, P, P)
 _sig('geob200_add_layernorm', c_int, P, P, P, P, I64, I64, F, P, P)
 _sig('geob200_l2_normalize', c_int, P, I64, I64, P, P)
 _sig('geob200_sinkhorn', c_int, P, P, P, P, I64, I64, I64, F, P, P)
+_sig('geob200_sinkhorn_backward_workspace_bytes', SZ, I64, I64, I64)
+_sig('geob200_sinkhorn_backward', c_int, P, P, P, P, I64, I64, I64, F, P, P, P, P, SZ, P)
 _sig('geob200_superpoint_matching_batched_workspace_bytes', SZ, I64, I64, I64)
 _sig('geob200_superpoint_matching_batched', c_int, P, P, I64, P, P, I64, P, I64, c_int, P, P, P, P, SZ, P)
 _sig('geob200_gather_patches_batched', c_int, P, I64, I64, P, P, P, P, I64, P, P, P, P, P)
 _sig('geob200_patch_scores_batched', c_int, P, P, I64, I64, P, P, P, I64, I64, P, P)
+_sig('geob200_patch_scores_backward_batched_workspace_bytes', SZ, I64, I64, I64, I64)
+_sig('geob200_patch_scores_backward_batched', c_int, P, P, I64, I64, P, P, P, I64, I64, P, P, P, P, SZ, P)
 _sig('geob200_lgr_batched_workspace_bytes', SZ, I64, I64, I64, I64)
 _sig('geob200_local_global_registration_batched', c_int, P, P, P, P, P, I64, I64, I64, I64, I64, F, c_int, F, I64, I64, P, P, P, P,
      P, P, I64, P, P, P, P, SZ, P)
@@ -88,6 +92,10 @@ _sig('geob200_coarse_matching_loss_batched_workspace_bytes', SZ, I64, I64)
 _sig('geob200_coarse_matching_loss_batched', c_int, P, P, I64, I64, P, P, P, P, F, F, F, F, F, F, P, I64, P, SZ, P)
 _sig('geob200_fine_matching_loss_batched_workspace_bytes', SZ, I64, I64)
 _sig('geob200_fine_matching_loss_batched', c_int, P, P, P, P, P, P, I64, I64, I64, P, D, P, P, I64, P, SZ, P)
+_sig('geob200_coarse_matching_loss_backward_batched_workspace_bytes', SZ, I64, I64, I64)
+_sig('geob200_coarse_matching_loss_backward_batched', c_int, P, P, I64, I64, P, P, P, P, F, F, F, F, F, F, P, I64, P, P, P, P, SZ, P)
+_sig('geob200_fine_matching_loss_backward_batched_workspace_bytes', SZ, I64, I64)
+_sig('geob200_fine_matching_loss_backward_batched', c_int, P, P, P, P, P, I64, I64, I64, P, D, P, I64, P, P, P, SZ, P)
 _sig('geob200_ransac_correspondences_batched_workspace_bytes', SZ, I64, I64)
 _sig('geob200_ransac_correspondences_batched', c_int, P, P, I64, I64, P, F, I64, I64, ctypes.c_uint64, I64, P, P, P, P, P, P, P, P, P, P,
      SZ, P)

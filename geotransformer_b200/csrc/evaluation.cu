@@ -335,9 +335,11 @@ __device__ __forceinline__ T block_reduce_256(T v, Op op, T* red) {
 
 // d[i][j] = sqrt(clamp(2 - 2 <f_i, g_j>, 0)) for every (ref i, src j) of pair p = blockIdx.y (ALL superpoints: the loss applies no
 // node mask), o[i][j] = 0.  One CTA per ref row, one warp per entry (lane-strided fmaf + warp_sum, as spm_scores_kernel).
+// live (may be NULL): 2 - 2 <f_i, g_j> >= 0, where the clamp passes its gradient (the backward).
 __global__ void __launch_bounds__(256) closs_dist_kernel(const float* __restrict__ fr, const float* __restrict__ fs, int C,
                                                          const __grid_constant__ Segs R, const __grid_constant__ Segs Q,
-                                                         const __grid_constant__ Segs NN, float* __restrict__ d, float* __restrict__ o) {
+                                                         const __grid_constant__ Segs NN, float* __restrict__ d, float* __restrict__ o,
+                                                         unsigned char* __restrict__ live) {
     extern __shared__ float a[];            // [C]
     const int p = blockIdx.y, i = blockIdx.x;
     const int M = R.count[p], N = Q.count[p];
@@ -346,6 +348,7 @@ __global__ void __launch_bounds__(256) closs_dist_kernel(const float* __restrict
     fs += (long long)Q.start[p] * C;
     d += NN.start[p] + (long long)i * N;
     o += NN.start[p] + (long long)i * N;
+    if (live != nullptr) live += NN.start[p] + (long long)i * N;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     for (int c = threadIdx.x; c < C; c += blockDim.x) a[c] = fr[c];
     __syncthreads();
@@ -355,8 +358,10 @@ __global__ void __launch_bounds__(256) closs_dist_kernel(const float* __restrict
         for (int c = lane; c < C; c += 32) x = fmaf(a[c], b[c], x);
         x = warp_sum(x);
         if (lane == 0) {
-            d[j] = sqrtf(fmaxf(__fsub_rn(2.0f, __fmul_rn(2.0f, x)), 0.0f));
+            const float y = __fsub_rn(2.0f, __fmul_rn(2.0f, x));
+            d[j] = sqrtf(fmaxf(y, 0.0f));
             o[j] = 0.f;
+            if (live != nullptr) live[j] = y >= 0.0f;
         }
     }
 }
@@ -377,14 +382,27 @@ struct CircleParams {
     float pos_margin, neg_margin, pos_optimal, neg_optimal, log_scale, pos_overlap;
 };
 
+// circle_loss.py:56-76 for one entry: positive / negative flags, the detached weights wp / wn and the logits lp / ln
+__device__ __forceinline__ void circle_logits(const CircleParams& cp, float dv, float ov, float& lp, float& ln, int& pos, int& neg, float& wp,
+                                              float& wn) {
+    pos = ov > cp.pos_overlap;
+    neg = ov == 0.f;
+    wp = pos ? __fmul_rn(fmaxf(__fsub_rn(dv, cp.pos_optimal), 0.f), sqrtf(ov)) : 0.f;
+    wn = neg ? fmaxf(__fsub_rn(cp.neg_optimal, dv), 0.f) : 0.f;
+    lp = __fmul_rn(__fmul_rn(cp.log_scale, __fsub_rn(dv, cp.pos_margin)), wp);
+    ln = __fmul_rn(__fmul_rn(cp.log_scale, __fsub_rn(cp.neg_margin, dv)), wn);
+}
+
 // one CTA per row (blockIdx.z = 0: ref superpoint i over all j) or column (z = 1: src superpoint j over all i) of pair blockIdx.y:
 // both logsumexps (max subtracted first), loss = softplus(Lp + Ln) / log_scale and kept = (has a positive and a negative).
 // Weight-0 entries stay in the sums (exp(0) = 1), as in the reference.  Results at the row's / column's cloud offset.
+// lse_r / lse_c (may be NULL): the two logsumexps of the line (the backward).
 __global__ void __launch_bounds__(256) closs_lse_kernel(const float* __restrict__ d, const float* __restrict__ o,
                                                         const __grid_constant__ Segs R, const __grid_constant__ Segs Q,
                                                         const __grid_constant__ Segs NN, CircleParams cp, float* __restrict__ ell_r,
                                                         unsigned char* __restrict__ kept_r, float* __restrict__ ell_c,
-                                                        unsigned char* __restrict__ kept_c) {
+                                                        unsigned char* __restrict__ kept_c, float2* __restrict__ lse_r,
+                                                        float2* __restrict__ lse_c) {
     __shared__ float redf[8];
     __shared__ int redi[8];
     const int p = blockIdx.y, col = blockIdx.z;
@@ -395,13 +413,8 @@ __global__ void __launch_bounds__(256) closs_lse_kernel(const float* __restrict_
     const long long base = NN.start[p] + (col ? line : (long long)line * N);
     const long long step = col ? N : 1;
     auto logits = [&](int e, float& lp, float& ln, int& pos, int& neg) {
-        const float dv = d[base + e * step], ov = o[base + e * step];
-        pos = ov > cp.pos_overlap;
-        neg = ov == 0.f;
-        const float wp = pos ? __fmul_rn(fmaxf(__fsub_rn(dv, cp.pos_optimal), 0.f), sqrtf(ov)) : 0.f;
-        const float wn = neg ? fmaxf(__fsub_rn(cp.neg_optimal, dv), 0.f) : 0.f;
-        lp = __fmul_rn(__fmul_rn(cp.log_scale, __fsub_rn(dv, cp.pos_margin)), wp);
-        ln = __fmul_rn(__fmul_rn(cp.log_scale, __fsub_rn(cp.neg_margin, dv)), wn);
+        float wp, wn;
+        circle_logits(cp, d[base + e * step], o[base + e * step], lp, ln, pos, neg, wp, wn);
     };
     float mp = -INFINITY, mn = -INFINITY;
     int np_ = 0, nn_ = 0;
@@ -435,6 +448,82 @@ __global__ void __launch_bounds__(256) closs_lse_kernel(const float* __restrict_
         const long long r = (col ? Q.start[p] : R.start[p]) + line;
         (col ? ell_c : ell_r)[r] = l;
         (col ? kept_c : kept_r)[r] = has == 3;
+        if (lse_r != nullptr) (col ? lse_c : lse_r)[r] = make_float2(mp + logf(sp), mn + logf(sn));
+    }
+}
+
+// Backward of c_loss.  Per pair: g = upstream gradient of c_loss (grad[p * gld + 1] + w_c * grad[p * gld] given weights); the mean
+// over the kept rows / columns turns it into scale[2p] = (g / 2) / #kept rows, scale[2p + 1] = (g / 2) / #kept columns.
+__global__ void __launch_bounds__(32) closs_grad_scale_kernel(const unsigned char* __restrict__ kept_r, const unsigned char* __restrict__ kept_c,
+                                                              const __grid_constant__ Segs R, const __grid_constant__ Segs Q,
+                                                              const float* __restrict__ grad, long long gld, int with_w, float w_c,
+                                                              float* __restrict__ scale) {
+    const int p = blockIdx.x, lane = threadIdx.x;
+    const float g = with_w ? grad[p * gld + 1] + w_c * grad[p * gld] : grad[p * gld + 1];
+    for (int side = 0; side < 2; ++side) {
+        const unsigned char* kept = side ? kept_c : kept_r;
+        const int s0 = side ? Q.start[p] : R.start[p], n = side ? Q.count[p] : R.count[p];
+        int k = 0;
+        for (int i = lane; i < n; i += 32) k += kept[s0 + i];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) k += __shfl_xor_sync(0xffffffffu, k, o);
+        if (lane == 0) scale[2 * p + side] = (g / 2.0f) / (float)k;
+    }
+}
+
+// torch softplus backward (beta 1, threshold 20) of l = softplus(x) / log_scale, for a line whose loss enters the mean with `scale`
+__device__ __forceinline__ float closs_line_grad(float2 lse, bool kept, float scale, float log_scale) {
+    if (!kept) return 0.f;
+    const float x = lse.x + lse.y, gl = scale / log_scale;
+    if (x > 20.f) return gl;
+    const float z = expf(x);
+    return gl * z / (z + 1.f);
+}
+
+// dc_loss / d<f_i, g_j> for every entry (i, j) of pair p, written over o: the logsumexp softmaxes of the entry's row and column, the
+// detached weights, then sqrt (grad / (2 d)) and the clamp (zero where 2 - 2 <f, g> < 0) in torch's order -- so an entry at d = 0
+// gives inf or NaN exactly where torch autograd does.
+__global__ void __launch_bounds__(256) closs_grad_kernel(const float* __restrict__ d, float* __restrict__ o, const unsigned char* __restrict__ live,
+                                                         const float2* __restrict__ lse_r, const float2* __restrict__ lse_c,
+                                                         const unsigned char* __restrict__ kept_r, const unsigned char* __restrict__ kept_c,
+                                                         const __grid_constant__ Segs R, const __grid_constant__ Segs Q,
+                                                         const __grid_constant__ Segs NN, CircleParams cp, const float* __restrict__ scale) {
+    const int p = blockIdx.y;
+    const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= NN.count[p]) return;
+    const int N = Q.count[p];
+    const int i = (int)(t / N), j = (int)(t % N);
+    const long long e = NN.start[p] + t;
+    const float dv = d[e];
+    float lp, ln, wp, wn;
+    int pos, neg;
+    circle_logits(cp, dv, o[e], lp, ln, pos, neg, wp, wn);
+    const float2 lr = lse_r[R.start[p] + i], lc = lse_c[Q.start[p] + j];
+    const float gr = closs_line_grad(lr, kept_r[R.start[p] + i], scale[2 * p], cp.log_scale);
+    const float gc = closs_line_grad(lc, kept_c[Q.start[p] + j], scale[2 * p + 1], cp.log_scale);
+    const float glp = gr * expf(lp - lr.x) + gc * expf(lp - lc.x);
+    const float gln = gr * expf(ln - lr.y) + gc * expf(ln - lc.y);
+    const float gd = (glp * wp) * cp.log_scale - (gln * wn) * cp.log_scale;
+    const float gsq = live[e] ? gd / (2.0f * dv) : 0.f;
+    o[e] = -gsq * 2.0f;
+}
+
+// grad_ref[i] = sum_j G[i][j] fs[j] (side 0, blockIdx.z) and grad_src[j] = sum_i G[i][j] fr[i] (side 1), summed in index order
+__global__ void __launch_bounds__(128) closs_feat_grad_kernel(const float* __restrict__ G, const float* __restrict__ fr,
+                                                              const float* __restrict__ fs, int C, const __grid_constant__ Segs R,
+                                                              const __grid_constant__ Segs Q, const __grid_constant__ Segs NN,
+                                                              float* __restrict__ grad_ref, float* __restrict__ grad_src) {
+    const int p = blockIdx.y, side = blockIdx.z, line = blockIdx.x;
+    const int M = R.count[p], N = Q.count[p];
+    if (line >= (side ? N : M)) return;
+    G += NN.start[p];
+    const float* other = side ? fr + (long long)R.start[p] * C : fs + (long long)Q.start[p] * C;
+    float* out = side ? grad_src + ((long long)Q.start[p] + line) * C : grad_ref + ((long long)R.start[p] + line) * C;
+    const int n = side ? M : N;
+    for (int c = threadIdx.x; c < C; c += blockDim.x) {
+        float s = 0.f;
+        for (int k = 0; k < n; ++k) s += G[side ? (long long)k * N + line : (long long)line * N + k] * other[(long long)k * C + c];
+        out[c] = s;
     }
 }
 
@@ -462,12 +551,16 @@ __global__ void __launch_bounds__(32) closs_finalize_kernel(const float* __restr
 // FineMatchingLoss, one CTA per patch q of pair p = blockIdx.y (patch rows at p * P + q): ground-truth labels of the (K+1)^2
 // Sinkhorn block (point pairs closer than the radius after the gt transform, slack row / column for unmatched valid points);
 // partial[p * P + q] = (sum of the labelled scores, #labels).  Scores are read only where a label is set.
-template <int K>
+// MODE 0: the values above; 1: #labels only (scores unread); 2: the backward -- every entry of the block gets -g_p / n_p on a label
+// and 0 elsewhere, with n_p = the pair's #labels from a MODE 1 pass in pcnt and g_p the upstream gradient of f_loss (grad[p * gld + 2]
+// + w_f * grad[p * gld] given weights) -- written to scores.
+template <int K, int MODE>
 __global__ void __launch_bounds__(256) floss_patch_kernel(const float* __restrict__ ref_pts, const float* __restrict__ src_pts,
                                                           const unsigned char* __restrict__ ref_masks,
-                                                          const unsigned char* __restrict__ src_masks, const float* __restrict__ scores,
+                                                          const unsigned char* __restrict__ src_masks, float* __restrict__ scores,
                                                           const float* __restrict__ T, int P, const int* __restrict__ count, float r2,
-                                                          double* __restrict__ psum, int* __restrict__ pcnt) {
+                                                          double* __restrict__ psum, int* __restrict__ pcnt, const float* __restrict__ grad,
+                                                          long long gld, int with_w, float w_f) {
     __shared__ float4 rp[K], sp[K];              // (x, y, z, |p|^2), w < 0 = invalid point
     __shared__ int rhit[K], shit[K];
     __shared__ double redd[8];
@@ -490,27 +583,50 @@ __global__ void __launch_bounds__(256) floss_patch_kernel(const float* __restric
         shit[i] = 0;
     }
     __syncthreads();
-    const float* S = scores + patch * (K + 1) * (K + 1);
+    float* S = scores + patch * (K + 1) * (K + 1);
     double s = 0.0;
     int n = 0;
+    auto hit = [&](int i, int j) {
+        const float4 a = rp[i], b = sp[j];
+        return a.w >= 0.f && b.w >= 0.f && sqd_mm(a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w) < r2;
+    };
     for (int e = threadIdx.x; e < K * K; e += blockDim.x) {
         const int i = e / K, j = e % K;
-        const float4 a = rp[i], b = sp[j];
-        if (a.w >= 0.f && b.w >= 0.f && sqd_mm(a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w) < r2) {
+        if (hit(i, j)) {
             rhit[i] = 1;
             shit[j] = 1;
-            s += S[i * (K + 1) + j];
+            if (MODE == 0) s += S[i * (K + 1) + j];
             ++n;
         }
     }
     __syncthreads();
-    for (int i = threadIdx.x; i < K; i += blockDim.x) {
-        if (rp[i].w >= 0.f && !rhit[i]) { s += S[i * (K + 1) + K]; ++n; }
-        if (sp[i].w >= 0.f && !shit[i]) { s += S[K * (K + 1) + i]; ++n; }
+    if constexpr (MODE == 2) {
+        int np = 0;
+        for (int k = threadIdx.x; k < P; k += blockDim.x) np += pcnt[(long long)p * P + k];
+        np = block_reduce_256(np, [](int x, int y) { return x + y; }, redi);
+        const float g = with_w ? grad[p * gld + 2] + w_f * grad[p * gld] : grad[p * gld + 2];
+        const float val = np > 0 ? -g / (float)np : 0.f;
+        for (int e = threadIdx.x; e < (K + 1) * (K + 1); e += blockDim.x) {
+            const int i = e / (K + 1), j = e % (K + 1);
+            bool lab;
+            if (i < K && j < K) lab = hit(i, j);
+            else if (i < K && j == K) lab = rp[i].w >= 0.f && !rhit[i];
+            else if (i == K && j < K) lab = sp[j].w >= 0.f && !shit[j];
+            else lab = false;
+            S[e] = lab ? val : 0.f;
+        }
+    } else {
+        for (int i = threadIdx.x; i < K; i += blockDim.x) {
+            if (rp[i].w >= 0.f && !rhit[i]) { if (MODE == 0) s += S[i * (K + 1) + K]; ++n; }
+            if (sp[i].w >= 0.f && !shit[i]) { if (MODE == 0) s += S[K * (K + 1) + i]; ++n; }
+        }
+        if (MODE == 0) s = block_reduce_256(s, [](double x, double y) { return x + y; }, redd);
+        n = block_reduce_256(n, [](int x, int y) { return x + y; }, redi);
+        if (threadIdx.x == 0) {
+            if (MODE == 0) psum[patch] = s;
+            pcnt[patch] = n;
+        }
     }
-    s = block_reduce_256(s, [](double x, double y) { return x + y; }, redd);
-    n = block_reduce_256(n, [](int x, int y) { return x + y; }, redi);
-    if (threadIdx.x == 0) { psum[patch] = s; pcnt[patch] = n; }
 }
 
 // one warp per pair: f_loss = -(sum of the labelled scores / #labels) over all patches of the pair -> out[p * ld + 2]; with weights
@@ -661,13 +777,15 @@ int geob200_coarse_matching_loss_batched(const float* ref_feats, const float* sr
     const CircleParams cp{positive_margin, negative_margin, positive_optimal, negative_optimal, log_scale, positive_overlap};
     int n_launch = 1;
     if (R.max > 0 && Q.max > 0) {
-        closs_dist_kernel<<<dim3((unsigned)R.max, B), 256, channels * sizeof(float), st>>>(ref_feats, src_feats, (int)channels, R, Q, NN, d, o);
+        closs_dist_kernel<<<dim3((unsigned)R.max, B), 256, channels * sizeof(float), st>>>(ref_feats, src_feats, (int)channels, R, Q, NN, d, o,
+                                                                                           nullptr);
         closs_scatter_kernel<<<dim3((unsigned)((NN.max + 255) / 256), B), 256, 0, st>>>((const long long*)gt_node_corr_indices,
                                                                                         gt_node_corr_overlaps, gt_count, Q, NN, o);
         n_launch += 2;
     }
     if (R.max > 0 || Q.max > 0) {
-        closs_lse_kernel<<<dim3((unsigned)(R.max > Q.max ? R.max : Q.max), B, 2), 256, 0, st>>>(d, o, R, Q, NN, cp, ell, kept, ell_c, kept_c);
+        closs_lse_kernel<<<dim3((unsigned)(R.max > Q.max ? R.max : Q.max), B, 2), 256, 0, st>>>(d, o, R, Q, NN, cp, ell, kept, ell_c, kept_c,
+                                                                                                nullptr, nullptr);
         n_launch += 1;
     }
     closs_finalize_kernel<<<B, 32, 0, st>>>(ell, kept, ell_c, kept_c, R, Q, out, (long long)out_ld);
@@ -706,16 +824,119 @@ int geob200_fine_matching_loss_batched(const float* ref_knn_points, const float*
     if (P > 0) {
         const dim3 grid((unsigned)P, (unsigned)n_pairs);
         if (k == 64)
-            floss_patch_kernel<64><<<grid, 256, 0, st>>>(ref_knn_points, src_knn_points, ref_knn_masks, src_knn_masks, matching_scores,
-                                                         transforms, P, patch_count, r2, psum, pcnt);
+            floss_patch_kernel<64, 0><<<grid, 256, 0, st>>>(ref_knn_points, src_knn_points, ref_knn_masks, src_knn_masks,
+                                                            const_cast<float*>(matching_scores), transforms, P, patch_count, r2, psum, pcnt,
+                                                            nullptr, 0, 0, 0.f);
         else
-            floss_patch_kernel<128><<<grid, 256, 0, st>>>(ref_knn_points, src_knn_points, ref_knn_masks, src_knn_masks, matching_scores,
-                                                          transforms, P, patch_count, r2, psum, pcnt);
+            floss_patch_kernel<128, 0><<<grid, 256, 0, st>>>(ref_knn_points, src_knn_points, ref_knn_masks, src_knn_masks,
+                                                             const_cast<float*>(matching_scores), transforms, P, patch_count, r2, psum, pcnt,
+                                                             nullptr, 0, 0, 0.f);
         n_launch += 1;
     }
     floss_finalize_kernel<<<(unsigned)n_pairs, 32, 0, st>>>(psum, pcnt, P, loss_weights != nullptr, w_c, w_f, out, (long long)out_ld);
     GEOB_CHECK_LAUNCH();
     count_launches(n_launch);
+    return 0;
+}
+
+size_t geob200_coarse_matching_loss_backward_batched_workspace_bytes(int64_t n_rows, int64_t n_products, int64_t n_pairs) {
+    const size_t r = (size_t)n_rows, nn = (size_t)n_products;
+    return geob200_coarse_matching_loss_batched_workspace_bytes(n_rows, n_products) + align_up(nn, 256) + align_up(8 * r, 256) +
+           align_up(8 * (size_t)n_pairs, 256) + 1024;
+}
+
+int geob200_coarse_matching_loss_backward_batched(const float* ref_feats, const float* src_feats, int64_t channels, int64_t n_pairs,
+                                                  const int64_t* cloud_nodes, const int64_t* gt_node_corr_indices,
+                                                  const float* gt_node_corr_overlaps, const int32_t* gt_count, float positive_margin,
+                                                  float negative_margin, float positive_optimal, float negative_optimal, float log_scale,
+                                                  float positive_overlap, const float* grad_rows, int64_t grad_ld, const float* loss_weights,
+                                                  float* grad_ref_feats, float* grad_src_feats, void* workspace, size_t workspace_bytes,
+                                                  void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    GEOB_REQUIRE(n_pairs > 0 && 2 * n_pairs <= GEOB_MAX_CLOUDS, "coarse_matching_loss_backward_batched: 1..%d pairs", GEOB_MAX_CLOUDS / 2);
+    GEOB_REQUIRE(channels > 0 && channels <= 8192, "coarse_matching_loss_backward_batched: 1..8192 channels");
+    GEOB_REQUIRE(log_scale > 0.f, "coarse_matching_loss_backward_batched: log_scale must be positive");
+    GEOB_REQUIRE(grad_ld >= 3, "coarse_matching_loss_backward_batched: grad_ld >= 3 required");
+    GEOB_REQUIRE(gt_count != nullptr && grad_rows != nullptr && grad_ref_feats != nullptr && grad_src_feats != nullptr,
+                 "coarse_matching_loss_backward_batched: null pointer");
+    for (int64_t c = 0; c < 2 * n_pairs; ++c) GEOB_REQUIRE(cloud_nodes[c] >= 0, "coarse_matching_loss_backward_batched: negative node count");
+    const int B = (int)n_pairs;
+    Segs R, Q, NN;
+    if (segs_from_counts(&R, B, cloud_nodes) || segs_from_counts(&Q, B, cloud_nodes + B) || segs_products(&NN, R, Q)) return -1;
+    const int64_t n_ref = (int64_t)R.start[B - 1] + R.count[B - 1];
+    const int64_t rows = n_ref + Q.start[B - 1] + Q.count[B - 1];
+    const int64_t nn = (int64_t)NN.start[B - 1] + NN.count[B - 1];
+    GEOB_REQUIRE(workspace_bytes >= geob200_coarse_matching_loss_backward_batched_workspace_bytes(rows, nn, n_pairs),
+                 "coarse_matching_loss_backward_batched: workspace too small");
+    Arena ar(workspace, workspace_bytes);
+    float* d = ar.take<float>(nn);
+    float* o = ar.take<float>(nn);                           // overlaps, then dc_loss / d<f, g>
+    float* ell = ar.take<float>(rows);
+    unsigned char* kept = ar.take<unsigned char>(rows);
+    unsigned char* live = ar.take<unsigned char>(nn);
+    float2* lse = ar.take<float2>(rows);
+    float* scale = ar.take<float>(2 * (size_t)B);
+    GEOB_REQUIRE(ar.ok(), "coarse_matching_loss_backward_batched: workspace accounting error");
+    const CircleParams cp{positive_margin, negative_margin, positive_optimal, negative_optimal, log_scale, positive_overlap};
+    const float w_c = loss_weights != nullptr ? loss_weights[0] : 0.f;
+    int n_launch = 1;
+    if (R.max > 0 && Q.max > 0) {
+        closs_dist_kernel<<<dim3((unsigned)R.max, B), 256, channels * sizeof(float), st>>>(ref_feats, src_feats, (int)channels, R, Q, NN, d, o,
+                                                                                           live);
+        closs_scatter_kernel<<<dim3((unsigned)((NN.max + 255) / 256), B), 256, 0, st>>>((const long long*)gt_node_corr_indices,
+                                                                                        gt_node_corr_overlaps, gt_count, Q, NN, o);
+        closs_lse_kernel<<<dim3((unsigned)(R.max > Q.max ? R.max : Q.max), B, 2), 256, 0, st>>>(d, o, R, Q, NN, cp, ell, kept, ell + n_ref,
+                                                                                                kept + n_ref, lse, lse + n_ref);
+        closs_grad_scale_kernel<<<B, 32, 0, st>>>(kept, kept + n_ref, R, Q, grad_rows, (long long)grad_ld, loss_weights != nullptr, w_c,
+                                                  scale);
+        closs_grad_kernel<<<dim3((unsigned)((NN.max + 255) / 256), B), 256, 0, st>>>(d, o, live, lse, lse + n_ref, kept, kept + n_ref, R,
+                                                                                      Q, NN, cp, scale);
+        n_launch += 5;
+    }
+    // every feature row is written (zeros for a cloud whose partner is empty)
+    closs_feat_grad_kernel<<<dim3((unsigned)(R.max > Q.max ? R.max : Q.max) + (R.max == 0 && Q.max == 0), B, 2), 128, 0, st>>>(
+        o, ref_feats, src_feats, (int)channels, R, Q, NN, grad_ref_feats, grad_src_feats);
+    GEOB_CHECK_LAUNCH();
+    count_launches(n_launch);
+    return 0;
+}
+
+size_t geob200_fine_matching_loss_backward_batched_workspace_bytes(int64_t n_pairs, int64_t n_patches) {
+    return align_up(4 * (size_t)n_pairs * (size_t)n_patches, 256) + 256;
+}
+
+int geob200_fine_matching_loss_backward_batched(const float* ref_knn_points, const float* src_knn_points, const uint8_t* ref_knn_masks,
+                                                const uint8_t* src_knn_masks, const float* transforms, int64_t n_pairs, int64_t n_patches,
+                                                int64_t k, const int32_t* patch_count, double positive_radius, const float* grad_rows,
+                                                int64_t grad_ld, const float* loss_weights, float* grad_scores, void* workspace,
+                                                size_t workspace_bytes, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    GEOB_REQUIRE(n_pairs > 0 && n_pairs <= 65535, "fine_matching_loss_backward_batched: 1..65535 pairs");
+    GEOB_REQUIRE(n_patches >= 0 && n_patches < (1 << 30), "fine_matching_loss_backward_batched: negative patch count");
+    GEOB_REQUIRE(k == 64 || k == 128, "fine_matching_loss_backward_batched: k must be 64 or 128, got %lld", (long long)k);
+    GEOB_REQUIRE(positive_radius > 0.0, "fine_matching_loss_backward_batched: positive_radius must be positive");
+    GEOB_REQUIRE(grad_ld >= 3, "fine_matching_loss_backward_batched: grad_ld >= 3 required");
+    GEOB_REQUIRE(grad_rows != nullptr && (n_patches == 0 || grad_scores != nullptr), "fine_matching_loss_backward_batched: null pointer");
+    GEOB_REQUIRE(workspace_bytes >= geob200_fine_matching_loss_backward_batched_workspace_bytes(n_pairs, n_patches),
+                 "fine_matching_loss_backward_batched: workspace too small");
+    if (n_patches == 0) return 0;
+    Arena ar(workspace, workspace_bytes);
+    int* pcnt = ar.take<int>((size_t)n_pairs * n_patches);
+    GEOB_REQUIRE(ar.ok(), "fine_matching_loss_backward_batched: workspace accounting error");
+    const float r2 = (float)(positive_radius * positive_radius);
+    const int P = (int)n_patches;
+    const float w_f = loss_weights != nullptr ? loss_weights[1] : 0.f;
+    const int with_w = loss_weights != nullptr;
+    const dim3 grid((unsigned)P, (unsigned)n_pairs);
+#define LAUNCH_FLB(KV, MODE)                                                                                                          \
+    floss_patch_kernel<KV, MODE><<<grid, 256, 0, st>>>(ref_knn_points, src_knn_points, ref_knn_masks, src_knn_masks, grad_scores,      \
+                                                       transforms, P, patch_count, r2, nullptr, pcnt, grad_rows, (long long)grad_ld,   \
+                                                       with_w, w_f)
+    if (k == 64) { LAUNCH_FLB(64, 1); LAUNCH_FLB(64, 2); }
+    else { LAUNCH_FLB(128, 1); LAUNCH_FLB(128, 2); }
+#undef LAUNCH_FLB
+    GEOB_CHECK_LAUNCH();
+    count_launches(2);
     return 0;
 }
 

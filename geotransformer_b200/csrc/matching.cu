@@ -543,6 +543,386 @@ __global__ void __launch_bounds__(MAXT) sinkhorn_reg_kernel(const float* __restr
     }
 }
 
+// ---- Sinkhorn backward -----------------------------------------------------------------------------------
+// Reverse sweep of learnable_sinkhorn.py:13-18 for one patch per CTA, same ownership as sinkhorn_reg_kernel: thread (slot, sub) owns
+// the entries (slot, sub + LPR k) of row `slot` and (sub + LPR k, slot) of column `slot`; Z stays in shared memory and dZ of a thread's
+// row entries in registers.  The row half-step's terms (computed by the column owners) pass through shared memory (D) and are added
+// by the row owners before the next column half-step, so dZ accumulates G, then the terms of iteration T, T-1, ... in autograd's order:
+// the running sum stays small (two separate accumulators would each grow to ~iters terms and cancel only at the end).  The CTA first re-runs the forward iterations and streams the log-sum-exp of every half-step (Lu_t, Lv_t,
+// t = 1..iters) to its slice of `hist`; the reverse sweep reads them back from the last iteration to the first:
+//   column half-step (row owners):    P^v_ij = exp(x^v_ij - Lv_j),  dZ_ij -= gv_j P^v_ij,  gu_i = [t = T] rowsum(G)_i - sum_j gv_j P^v_ij
+//   row half-step (column owners):    P^u_ij = exp(x^u_ij - Lu_i),  dZ_ij -= gu_i P^u_ij,  gv_j = -sum_i gu_i P^u_ij
+// with the logits x^v_ij = Z_ij + u_i, x^u_ij = Z_ij + v_j.  A masked line (row or column whose mask is false) is -inf on all its
+// entries; the logits of such a line drop the constant (x^u_ij = v_j on a masked row, x^v_ij = u_i on a masked column) and its
+// potential is -L instead of log_mu - L: the inf -> infinity limit of the reference's arithmetic, which fp64 autograd follows and fp32
+// loses (1e12 swallows the potentials).  So an upstream gradient on masked entries stays finite.  The output gradient is zero on masked
+// entries (masked_fill); dalpha_part[p] = the sum of dZ over the unmasked dustbin entries.  A padding patch (no valid row and no valid
+// column) writes zeros and a zero partial.
+template <int K, int LPR, int MAXT, int MINB>
+__global__ void __launch_bounds__(MAXT, MINB) sinkhorn_bwd_kernel(const float* __restrict__ scores, const unsigned char* __restrict__ row_masks,
+                                                           const unsigned char* __restrict__ col_masks, const float* __restrict__ alpha_p,
+                                                           int iters, float inf, const float* __restrict__ grad,
+                                                           float* __restrict__ hist, float* __restrict__ dscores,
+                                                           float* __restrict__ dalpha_part) {
+    constexpr int K1 = K + 1, ld = K1 | 1, NE = (K1 + LPR - 1) / LPR;
+    extern __shared__ float sm[];
+    float* Z = sm;                           // [K1][ld]; after the sweep: the accumulated dZ
+    float* D = Z + K1 * ld;                  // [K1][ld]: the last row half-step's dZ terms
+    float* pu = D + K1 * ld;                 // u_t
+    float* pv = pu + K1;                     // v_t (forward), v_{t-1} (sweep)
+    float* Lu = pv + K1;
+    float* Lv = Lu + K1;
+    float* gu = Lv + K1;
+    float* gv = gu + K1;
+    unsigned char* rmk = reinterpret_cast<unsigned char*>(gv + K1);     // row i is masked (all -inf)
+    unsigned char* cmk = rmk + K1;
+    __shared__ int cnt_s[2];
+    const int p = blockIdx.x;
+    row_masks += (long long)p * K; col_masks += (long long)p * K;
+    grad += (long long)p * K1 * K1;
+    hist += (long long)p * 2 * iters * K1;
+    dscores += (long long)p * K * K;
+    if (threadIdx.x < 2) cnt_s[threadIdx.x] = 0;
+    __syncthreads();
+    {
+        int cr = 0, cc = 0;
+        for (int i = threadIdx.x; i < K; i += blockDim.x) { cr += row_masks[i] ? 1 : 0; cc += col_masks[i] ? 1 : 0; }
+        if (cr) atomicAdd(&cnt_s[0], cr);
+        if (cc) atomicAdd(&cnt_s[1], cc);
+    }
+    __syncthreads();
+    const int nr = cnt_s[0], nc = cnt_s[1];
+    if (nr == 0 && nc == 0) {
+        for (int e = threadIdx.x; e < K * K; e += blockDim.x) dscores[e] = 0.f;
+        if (threadIdx.x == 0) dalpha_part[p] = 0.f;
+        return;
+    }
+    const float nvr = (float)nr, nvc = (float)nc;
+    const float norm = -logf(nvr + nvc);
+    const float alpha = *alpha_p;
+    for (int e = threadIdx.x; e < K1 * K1; e += blockDim.x) {
+        const int i = e / K1, j = e % K1;
+        float z = (i < K && j < K) ? scores[((long long)p * K + i) * K + j] : alpha;
+        if ((i < K && !row_masks[i]) || (j < K && !col_masks[j])) z = -inf;
+        Z[i * ld + j] = z;
+        D[i * ld + j] = 0.f;
+    }
+    for (int i = threadIdx.x; i < K1; i += blockDim.x) {
+        rmk[i] = i < K && !row_masks[i];
+        cmk[i] = i < K && !col_masks[i];
+        pu[i] = 0.f; pv[i] = 0.f;
+    }
+    __syncthreads();
+    // marginals of unmasked lines (a masked line's potential does not use them)
+    auto lmu = [&](int i) { return i < K ? norm : logf(nvc) + norm; };
+    auto lnu = [&](int j) { return j < K ? norm : logf(nvr) + norm; };
+    const int slot = threadIdx.x / LPR, sub = threadIdx.x % LPR;
+    const bool act = slot < K1;
+    const int ij = act ? slot : K1 - 1;
+    const bool rm_own = rmk[ij], cm_own = cmk[ij];
+    // line log-sum-exp over this thread's entries + the LPR-lane shuffle reduction
+    auto lse = [&](const float (&x)[NE]) {
+        float mx = -INFINITY;
+#pragma unroll
+        for (int k = 0; k < NE; ++k) mx = fmaxf(mx, x[k]);
+#pragma unroll
+        for (int o = LPR / 2; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+        float s = 0.f;
+#pragma unroll
+        for (int k = 0; k < NE; ++k) s += expf(x[k] - mx);
+#pragma unroll
+        for (int o = LPR / 2; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+        return mx + logf(s);
+    };
+    auto lane_sum = [&](float s) {
+#pragma unroll
+        for (int o = LPR / 2; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+        return s;
+    };
+    // ---- forward re-run: the log-sum-exp history
+    for (int it = 0; it < iters; ++it) {
+        {
+            float x[NE];
+#pragma unroll
+            for (int k = 0; k < NE; ++k) {
+                const int o = sub + LPR * k;
+                x[k] = o < K1 ? (rm_own ? pv[o] : Z[ij * ld + o] + pv[o]) : -INFINITY;
+            }
+            const float L = lse(x);
+            if (act && sub == 0) {
+                hist[(long long)it * 2 * K1 + ij] = L;
+                pu[ij] = rm_own ? -L : lmu(ij) - L;
+            }
+        }
+        __syncthreads();
+        {
+            float x[NE];
+#pragma unroll
+            for (int k = 0; k < NE; ++k) {
+                const int o = sub + LPR * k;
+                x[k] = o < K1 ? (cm_own ? pu[o] : Z[o * ld + ij] + pu[o]) : -INFINITY;
+            }
+            const float L = lse(x);
+            if (act && sub == 0) {
+                hist[(long long)it * 2 * K1 + K1 + ij] = L;
+                pv[ij] = cm_own ? -L : lnu(ij) - L;
+            }
+        }
+        __syncthreads();
+    }
+    // ---- reverse sweep
+    float dz[NE];                            // dZ of my row entries, starting from G
+    {
+        float sr = 0.f, sc = 0.f;
+#pragma unroll
+        for (int k = 0; k < NE; ++k) {
+            const int o = sub + LPR * k;
+            dz[k] = o < K1 ? grad[(long long)ij * K1 + o] : 0.f;
+            if (o < K1) { sr += dz[k]; sc += grad[(long long)o * K1 + ij]; }
+        }
+        sr = lane_sum(sr);
+        sc = lane_sum(sc);
+        if (act && sub == 0) { gu[ij] = sr; gv[ij] = sc; }
+    }
+    for (int it = iters - 1; it >= 0; --it) {
+        const float* h = hist + (long long)it * 2 * K1;
+        for (int i = threadIdx.x; i < K1; i += blockDim.x) {
+            const float lu = h[i], lv = h[K1 + i];
+            Lu[i] = lu; Lv[i] = lv;
+            pu[i] = rmk[i] ? -lu : lmu(i) - lu;
+            pv[i] = it == 0 ? 0.f : (cmk[i] ? -h[K1 + i - 2 * K1] : lnu(i) - h[K1 + i - 2 * K1]);
+        }
+        __syncthreads();
+        {   // column half-step of iteration it (v_t = log_nu - LSE_i(Z + u_t)), row owners
+            const float ui = pu[ij];
+            float s = 0.f;
+#pragma unroll
+            for (int k = 0; k < NE; ++k) {
+                const int o = sub + LPR * k;
+                if (o < K1) {
+                    dz[k] += D[ij * ld + o];        // the row half-step of iteration it + 1 (zero before the last iteration)
+                    const float x = cmk[o] ? ui : Z[ij * ld + o] + ui;
+                    const float w = gv[o] * expf(x - Lv[o]);
+                    dz[k] -= w;
+                    s += w;
+                }
+            }
+            s = lane_sum(s);
+            if (act && sub == 0) gu[ij] = (it == iters - 1 ? gu[ij] : 0.f) - s;
+        }
+        __syncthreads();
+        {   // row half-step (u_t = log_mu - LSE_j(Z + v_{t-1})), column owners
+            const float vj = pv[ij];
+            float s = 0.f;
+#pragma unroll
+            for (int k = 0; k < NE; ++k) {
+                const int o = sub + LPR * k;
+                if (o < K1) {
+                    const float x = rmk[o] ? vj : Z[o * ld + ij] + vj;
+                    const float w = gu[o] * expf(x - Lu[o]);
+                    D[o * ld + ij] = -w;
+                    s += w;
+                }
+            }
+            s = lane_sum(s);
+            if (act && sub == 0) gv[ij] = -s;
+        }
+        __syncthreads();
+    }
+    // the first iteration's row half-step, then dZ into Z's storage
+#pragma unroll
+    for (int k = 0; k < NE; ++k) {
+        const int o = sub + LPR * k;
+        if (act && o < K1) Z[ij * ld + o] = dz[k] + D[ij * ld + o];
+    }
+    __syncthreads();
+    for (int e = threadIdx.x; e < K * K; e += blockDim.x) {
+        const int i = e / K, j = e % K;
+        dscores[e] = (rmk[i] || cmk[j]) ? 0.f : Z[i * ld + j];
+    }
+    if (threadIdx.x < 32) {
+        float s = 0.f;
+        for (int e = threadIdx.x; e < 2 * K + 1; e += 32) {
+            const int i = e < K ? e : K, j = e < K ? K : e - K;     // (e, K) for e < K, then (K, e - K) for e - K in 0..K
+            if (!rmk[i] && !cmk[j]) s += Z[i * ld + j];
+        }
+        s = warp_sum(s);
+        if (threadIdx.x == 0) dalpha_part[p] = s;
+    }
+}
+
+// out[0] = sum of the n partials in a fixed order (thread-strided sums, then a fixed tree): deterministic for a given n
+__global__ void __launch_bounds__(256) sum_partials_kernel(const float* __restrict__ part, int n, float* __restrict__ out) {
+    __shared__ float red[8];
+    float s = 0.f;
+    for (int i = threadIdx.x; i < n; i += 256) s += part[i];
+    s = warp_sum(s);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        float t = 0.f;
+        for (int w = 0; w < 8; ++w) t += red[w];
+        out[0] = t;
+    }
+}
+
+// ---- patch-score backward --------------------------------------------------------------------------------
+// Per (patch, slot) gradient rows: side 0 (blockIdx.z): tmp[p K + a] = sum_b (dS_p[a][b] / sqrt(C)) fs[sidx[p][b]]; side 1:
+// tmp[P_all K + p K + b] = sum_a (dS_p[a][b] / sqrt(C)) fr[ridx[p][a]].  Sentinel rows read as zero.  One CTA per patch and side,
+// dS_p (transposed for side 1) in shared memory; each thread owns K/32 rows x 4 channels of a 32-channel chunk.
+template <int K>
+__global__ void __launch_bounds__(256) patch_scores_bwd_kernel(const float* __restrict__ fr, const float* __restrict__ fs,
+                                                               const __grid_constant__ Segs R, const __grid_constant__ Segs Q, int C,
+                                                               const long long* __restrict__ ridx, const long long* __restrict__ sidx,
+                                                               float div, const float* __restrict__ dS, float* __restrict__ tmp) {
+    constexpr int CH = 32, RT = K / 32;
+    extern __shared__ float sm[];
+    float* D = sm;                           // [K][K + 1]
+    float* F = sm + K * (K + 1);             // [K][CH + 1]
+    const int side = blockIdx.z, b = blockIdx.y;
+    const long long p = (long long)b * gridDim.x + blockIdx.x;
+    const long long P_all = (long long)gridDim.x * gridDim.y;
+    const float* other = side ? fr + (long long)R.start[b] * C : fs + (long long)Q.start[b] * C;
+    const int n_other = side ? R.count[b] : Q.count[b];
+    const long long* idx = (side ? ridx : sidx) + p * K;
+    dS += p * K * K;
+    tmp += ((long long)side * P_all + p) * K * C;
+    for (int e = threadIdx.x; e < K * K; e += 256) {
+        const int a = e / K, c = e % K;
+        const float g = dS[e] / div;
+        if (side) D[c * (K + 1) + a] = g; else D[a * (K + 1) + c] = g;
+    }
+    const int ty = threadIdx.x >> 3, tx = threadIdx.x & 7;
+    for (int c0 = 0; c0 < C; c0 += CH) {
+        for (int e = threadIdx.x; e < K * CH; e += 256) {
+            const int r = e / CH, c = e % CH;
+            const long long id = idx[r];
+            F[r * (CH + 1) + c] = (id >= 0 && id < n_other && c0 + c < C) ? other[id * C + c0 + c] : 0.f;
+        }
+        __syncthreads();
+        float acc[RT][4];
+#pragma unroll
+        for (int r = 0; r < RT; ++r)
+#pragma unroll
+            for (int q = 0; q < 4; ++q) acc[r][q] = 0.f;
+#pragma unroll 4
+        for (int m = 0; m < K; ++m) {
+            float fv[4];
+#pragma unroll
+            for (int q = 0; q < 4; ++q) fv[q] = F[m * (CH + 1) + tx + 8 * q];
+#pragma unroll
+            for (int r = 0; r < RT; ++r) {
+                const float dv = D[(ty + 32 * r) * (K + 1) + m];
+#pragma unroll
+                for (int q = 0; q < 4; ++q) acc[r][q] = fmaf(dv, fv[q], acc[r][q]);
+            }
+        }
+#pragma unroll
+        for (int r = 0; r < RT; ++r)
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+                const int c = c0 + tx + 8 * q;
+                if (c < C) tmp[(long long)(ty + 32 * r) * C + c] = acc[r][q];
+            }
+        __syncthreads();
+    }
+}
+
+// Inverse index of the (side, patch, slot) entries: entry e < 2 P_all K refers to feature row row_of(e) of the stacked row space
+// (ref rows, then src rows) or to nothing (sentinel).  Rows get their entries grouped by a counting sort and ordered by entry id, so
+// each row's gradient is summed in (patch, slot) order: deterministic, and a pair's rows see only the pair's own patches.
+struct PatchRows {
+    const long long* ridx;
+    const long long* sidx;
+    long long per_side;                      // P_all * K
+    int K, P, n_ref_rows;
+    __device__ __forceinline__ int row_of(long long e, const Segs& R, const Segs& Q) const {
+        const int side = e >= per_side;
+        const long long r = side ? e - per_side : e;
+        const int b = (int)(r / ((long long)P * K));
+        const long long id = (side ? sidx : ridx)[r];
+        const Segs& S = side ? Q : R;
+        if (id < 0 || id >= S.count[b]) return -1;
+        return (side ? n_ref_rows : 0) + S.start[b] + (int)id;
+    }
+};
+
+__global__ void __launch_bounds__(256) patch_rows_count_kernel(PatchRows pr, const __grid_constant__ Segs R, const __grid_constant__ Segs Q,
+                                                               int* __restrict__ cnt) {
+    const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= 2 * pr.per_side) return;
+    const int row = pr.row_of(e, R, Q);
+    if (row >= 0) atomicAdd(&cnt[row], 1);
+}
+
+// exclusive prefix sum of cnt[0..n) into off[0..n]; one CTA, chunked as compact_masks_kernel
+__global__ void __launch_bounds__(1024) exclusive_scan_kernel(const int* __restrict__ cnt, int n, int* __restrict__ off) {
+    __shared__ int warp_tot[32];
+    __shared__ int carry;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (threadIdx.x == 0) carry = 0;
+    __syncthreads();
+    for (int base = 0; base < n; base += 1024) {
+        const int i = base + threadIdx.x;
+        const int v = i < n ? cnt[i] : 0;
+        int x = v;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const int y = __shfl_up_sync(0xffffffffu, x, o);
+            if (lane >= o) x += y;
+        }
+        if (lane == 31) warp_tot[warp] = x;
+        __syncthreads();
+        int w_off = carry;
+        for (int w = 0; w < warp; ++w) w_off += warp_tot[w];
+        if (i < n) off[i] = w_off + x - v;
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            int t = 0;
+            for (int w = 0; w < 32; ++w) t += warp_tot[w];
+            carry += t;
+        }
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) off[n] = carry;
+}
+
+// bucket fill (arbitrary order inside a bucket), then every entry's rank inside its bucket = the number of smaller entry ids
+__global__ void __launch_bounds__(256) patch_rows_fill_kernel(PatchRows pr, const __grid_constant__ Segs R, const __grid_constant__ Segs Q,
+                                                              const int* __restrict__ off, int* __restrict__ cur, int* __restrict__ keys) {
+    const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= 2 * pr.per_side) return;
+    const int row = pr.row_of(e, R, Q);
+    if (row >= 0) keys[off[row] + atomicAdd(&cur[row], 1)] = (int)e;
+}
+
+__global__ void __launch_bounds__(256) patch_rows_rank_kernel(PatchRows pr, const __grid_constant__ Segs R, const __grid_constant__ Segs Q,
+                                                              const int* __restrict__ off, const int* __restrict__ keys,
+                                                              int* __restrict__ sorted) {
+    const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= 2 * pr.per_side) return;
+    const int row = pr.row_of(e, R, Q);
+    if (row < 0) return;
+    const int b = off[row], n = off[row + 1] - b;
+    int rank = 0;
+    for (int s = 0; s < n; ++s) rank += keys[b + s] < (int)e;
+    sorted[b + rank] = (int)e;
+}
+
+// grad row r = sum over its entries, in entry order, of tmp[entry]; rows without entries get zeros.  One CTA per row.
+__global__ void __launch_bounds__(128) patch_rows_reduce_kernel(const float* __restrict__ tmp, int C, const int* __restrict__ off,
+                                                                const int* __restrict__ sorted, int n_ref_rows, float* __restrict__ gref,
+                                                                float* __restrict__ gsrc) {
+    const int row = blockIdx.x;
+    float* out = row < n_ref_rows ? gref + (long long)row * C : gsrc + (long long)(row - n_ref_rows) * C;
+    const int b = off[row], n = off[row + 1] - b;
+    for (int c = threadIdx.x; c < C; c += blockDim.x) {
+        float s = 0.f;
+        for (int k = 0; k < n; ++k) s += tmp[(long long)sorted[b + k] * C + c];
+        out[c] = s;
+    }
+}
+
 }  // namespace geob200
 
 using namespace geob200;
@@ -658,6 +1038,120 @@ int geob200_sinkhorn(const float* scores, const uint8_t* row_masks, const uint8_
 #undef LAUNCH_SK_REG
     GEOB_CHECK_LAUNCH();
     count_launches(1);
+    return 0;
+}
+
+size_t geob200_sinkhorn_backward_workspace_bytes(int64_t n_patches, int64_t k, int64_t num_iterations) {
+    const size_t K1 = (size_t)k + 1;
+    return align_up(4 * (size_t)n_patches * 2 * (size_t)num_iterations * K1, 256) + align_up(4 * (size_t)n_patches, 256) + 256;
+}
+
+int geob200_sinkhorn_backward(const float* scores, const uint8_t* row_masks, const uint8_t* col_masks, const float* alpha, int64_t n_patches,
+                              int64_t k, int64_t num_iterations, float inf, const float* grad_out, float* grad_scores, float* grad_alpha,
+                              void* workspace, size_t workspace_bytes, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    GEOB_REQUIRE(n_patches >= 0 && n_patches <= 0x7fffffff, "sinkhorn_backward: bad patch count");
+    GEOB_REQUIRE(k == 32 || k == 64 || k == 128, "sinkhorn_backward: k must be 32, 64 or 128, got %lld", (long long)k);
+    GEOB_REQUIRE(num_iterations >= 1 && num_iterations <= 100000, "sinkhorn_backward: num_iterations must be in 1..100000");
+    GEOB_REQUIRE(inf > 0.f, "sinkhorn_backward: inf must be positive");
+    GEOB_REQUIRE(scores != nullptr && row_masks != nullptr && col_masks != nullptr && alpha != nullptr && grad_out != nullptr &&
+                     grad_scores != nullptr && grad_alpha != nullptr,
+                 "sinkhorn_backward: null pointer");
+    GEOB_REQUIRE(workspace_bytes >= geob200_sinkhorn_backward_workspace_bytes(n_patches, k, num_iterations),
+                 "sinkhorn_backward: workspace too small");
+    const int K1 = (int)k + 1, ld = K1 | 1;
+    const size_t smem = sizeof(float) * (2 * (size_t)K1 * ld + 6 * K1) + 2 * (size_t)K1;
+    Arena ar(workspace, workspace_bytes);
+    float* hist = ar.take<float>((size_t)n_patches * 2 * num_iterations * K1);
+    float* part = ar.take<float>((size_t)n_patches);
+    GEOB_REQUIRE(ar.ok(), "sinkhorn_backward: workspace accounting error");
+    int n_launch = 1;
+    if (n_patches > 0) {
+#define LAUNCH_SK_BWD(KV, LPRV, MT, MB)                                                                                               \
+    {                                                                                                                                 \
+        if (smem > 48 * 1024 && ensure_max_smem((const void*)sinkhorn_bwd_kernel<KV, LPRV, MT, MB>)) return -1;                       \
+        sinkhorn_bwd_kernel<KV, LPRV, MT, MB><<<(unsigned)n_patches, MT, smem, st>>>(scores, row_masks, col_masks, alpha,                 \
+                                                                                 (int)num_iterations, inf, grad_out, hist,            \
+                                                                                 grad_scores, part);                                  \
+    }
+        if (k == 32) LAUNCH_SK_BWD(32, 8, 288, 2)             // two CTAs per SM where registers allow, one at K = 128
+        else if (k == 64) LAUNCH_SK_BWD(64, 8, 544, 2)
+        else LAUNCH_SK_BWD(128, 4, 544, 1)
+#undef LAUNCH_SK_BWD
+        n_launch += 1;
+    }
+    sum_partials_kernel<<<1, 256, 0, st>>>(part, (int)n_patches, grad_alpha);
+    GEOB_CHECK_LAUNCH();
+    count_launches(n_launch);
+    return 0;
+}
+
+size_t geob200_patch_scores_backward_batched_workspace_bytes(int64_t n_rows, int64_t n_patches_total, int64_t k, int64_t channels) {
+    const size_t e = 2 * (size_t)n_patches_total * (size_t)k, r = (size_t)n_rows;
+    return align_up(4 * e * (size_t)channels, 256) + 2 * align_up(4 * e, 256) + 2 * align_up(4 * r, 256) + align_up(4 * (r + 1), 256) + 256;
+}
+
+int geob200_patch_scores_backward_batched(const float* ref_feats, const float* src_feats, int64_t channels, int64_t n_pairs,
+                                          const int64_t* cloud_points, const int64_t* ref_knn_indices, const int64_t* src_knn_indices,
+                                          int64_t n_patches, int64_t k, const float* grad_scores, float* grad_ref_feats,
+                                          float* grad_src_feats, void* workspace, size_t workspace_bytes, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    GEOB_REQUIRE(n_pairs > 0 && 2 * n_pairs <= GEOB_MAX_CLOUDS, "patch_scores_backward_batched: 1..%d pairs", GEOB_MAX_CLOUDS / 2);
+    GEOB_REQUIRE(k == 32 || k == 64 || k == 128, "patch_scores_backward_batched: num_points_in_patch=%lld unsupported (32, 64, 128)",
+                 (long long)k);
+    GEOB_REQUIRE(channels >= 1 && channels <= 65536, "patch_scores_backward_batched: 1..65536 channels");
+    GEOB_REQUIRE(n_patches >= 0 && n_patches <= 65535, "patch_scores_backward_batched: 0..65535 patches per pair");
+    GEOB_REQUIRE(grad_ref_feats != nullptr && grad_src_feats != nullptr, "patch_scores_backward_batched: null gradient pointer");
+    Segs R, Q;
+    if (segs_from_counts(&R, n_pairs, cloud_points) || segs_from_counts(&Q, n_pairs, cloud_points + n_pairs)) return -1;
+    const int64_t n_ref = (int64_t)R.start[R.n - 1] + R.count[R.n - 1], n_src = (int64_t)Q.start[Q.n - 1] + Q.count[Q.n - 1];
+    const int64_t rows = n_ref + n_src, P_all = n_pairs * n_patches, E = 2 * P_all * k;
+    GEOB_REQUIRE(rows < (1ll << 31) - 1 && E < (1ll << 31), "patch_scores_backward_batched: too many rows or patch entries");
+    GEOB_REQUIRE(E == 0 || (grad_scores != nullptr && ref_knn_indices != nullptr && src_knn_indices != nullptr),
+                 "patch_scores_backward_batched: null pointer");
+    GEOB_REQUIRE(workspace_bytes >= geob200_patch_scores_backward_batched_workspace_bytes(rows, P_all, k, channels),
+                 "patch_scores_backward_batched: workspace too small");
+    Arena ar(workspace, workspace_bytes);
+    float* tmp = ar.take<float>((size_t)E * channels);
+    int* keys = ar.take<int>((size_t)E);
+    int* sorted = ar.take<int>((size_t)E);
+    int* cnt = ar.take<int>((size_t)rows);
+    int* cur = ar.take<int>((size_t)rows);
+    int* off = ar.take<int>((size_t)rows + 1);
+    GEOB_REQUIRE(ar.ok(), "patch_scores_backward_batched: workspace accounting error");
+    const size_t smem = sizeof(float) * ((size_t)k * (k + 1) + (size_t)k * 33);
+    if (smem > 48 * 1024) {
+        const void* fn = k == 128 ? (const void*)patch_scores_bwd_kernel<128> : k == 64 ? (const void*)patch_scores_bwd_kernel<64>
+                                                                                        : (const void*)patch_scores_bwd_kernel<32>;
+        if (ensure_max_smem(fn)) return -1;
+    }
+    if (rows == 0) return 0;
+    int n_launch = 0;
+    const PatchRows pr{(const long long*)ref_knn_indices, (const long long*)src_knn_indices, P_all * k, (int)k, (int)n_patches, (int)n_ref};
+    if (E > 0) {
+        const float div = sqrtf((float)channels);      // as the forward: feats_f.shape[1] ** 0.5
+        const dim3 grid((unsigned)n_patches, (unsigned)n_pairs, 2);
+#define LAUNCH_PSB(KV) patch_scores_bwd_kernel<KV><<<grid, 256, smem, st>>>(ref_feats, src_feats, R, Q, (int)channels,                  \
+                                                                            (const long long*)ref_knn_indices,                          \
+                                                                            (const long long*)src_knn_indices, div, grad_scores, tmp)
+        if (k == 128) LAUNCH_PSB(128);
+        else if (k == 64) LAUNCH_PSB(64);
+        else LAUNCH_PSB(32);
+#undef LAUNCH_PSB
+        GEOB_CHECK_CUDA(cudaMemsetAsync(cnt, 0, sizeof(int) * (size_t)rows, st));
+        GEOB_CHECK_CUDA(cudaMemsetAsync(cur, 0, sizeof(int) * (size_t)rows, st));
+        const unsigned ge = (unsigned)((E + 255) / 256);
+        patch_rows_count_kernel<<<ge, 256, 0, st>>>(pr, R, Q, cnt);
+        exclusive_scan_kernel<<<1, 1024, 0, st>>>(cnt, (int)rows, off);
+        patch_rows_fill_kernel<<<ge, 256, 0, st>>>(pr, R, Q, off, cur, keys);
+        patch_rows_rank_kernel<<<ge, 256, 0, st>>>(pr, R, Q, off, keys, sorted);
+        n_launch += 5;
+    } else {
+        GEOB_CHECK_CUDA(cudaMemsetAsync(off, 0, sizeof(int) * ((size_t)rows + 1), st));
+    }
+    patch_rows_reduce_kernel<<<(unsigned)rows, 128, 0, st>>>(tmp, (int)channels, off, sorted, (int)n_ref, grad_ref_feats, grad_src_feats);
+    GEOB_CHECK_LAUNCH();
+    count_launches(n_launch + 1);
     return 0;
 }
 

@@ -56,6 +56,11 @@ def _detach(t):
     return t.detach() if t is not None and t.requires_grad else t
 
 
+def _needs_grad(*ts):
+    """the autograd path of the differentiable ops: grad mode on and an input requiring grad (else the value-only path, same kernels)"""
+    return torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in ts)
+
+
 _GN_WS = {}
 
 
@@ -539,24 +544,69 @@ def gather_patches(corr_indices, node_knn_indices, node_knn_masks, points):
 
 
 def patch_scores(ref_feats, src_feats, ref_knn_indices, src_knn_indices):
+    """differentiable w.r.t. ``ref_feats`` / ``src_feats`` (see ``patch_scores_backward_batched``)"""
     return _patch_scores(ref_feats, src_feats, [ref_feats.shape[0], src_feats.shape[0]], ref_knn_indices, src_knn_indices)
 
 
 def sinkhorn(scores, row_masks, col_masks, alpha, num_iterations, inf=1e12):
-    scores, alpha = _detach(scores), _detach(alpha)
-    _f(scores, 'scores')
-    p, k, k2 = scores.shape
-    if k != k2:
-        raise RuntimeError('sinkhorn: the CUDA kernel handles square patch score matrices')
+    """learnable_sinkhorn.py:20-66; differentiable w.r.t. ``scores`` and ``alpha`` (``sinkhorn_backward``)"""
+    p, k = scores.shape[0], scores.shape[1]
     dev = scores.device
     if row_masks is None:
         row_masks = torch.ones((p, k), dtype=torch.bool, device=dev)
     if col_masks is None:
         col_masks = torch.ones((p, k), dtype=torch.bool, device=dev)
-    out = torch.empty((p, k + 1, k + 1), dtype=_f32, device=dev)
+    if _needs_grad(scores, alpha):
+        return _Sinkhorn.apply(scores, row_masks, col_masks, alpha, int(num_iterations), float(inf))
+    return _sinkhorn(scores, row_masks, col_masks, alpha, num_iterations, inf)
+
+
+def _sinkhorn(scores, row_masks, col_masks, alpha, num_iterations, inf):
+    scores, alpha = _detach(scores), _detach(alpha)
+    _f(scores, 'scores')
+    p, k, k2 = scores.shape
+    if k != k2:
+        raise RuntimeError('sinkhorn: the CUDA kernel handles square patch score matrices')
+    out = torch.empty((p, k + 1, k + 1), dtype=_f32, device=scores.device)
     L.check(L.lib().geob200_sinkhorn(scores.data_ptr(), row_masks.data_ptr(), col_masks.data_ptr(), alpha.data_ptr(), p, k,
                                      int(num_iterations), float(inf), out.data_ptr(), L.stream_ptr()), 'sinkhorn')
     return out
+
+
+def sinkhorn_backward(scores, row_masks, col_masks, alpha, num_iterations, grad_out, inf=1e12):
+    """(grad_scores (P, k, k), grad_alpha (0-dim)) of ``sinkhorn`` for the upstream gradient ``grad_out`` (P, k+1, k+1); k = 32, 64
+    or 128.  Masked entries get zero; masked lines follow the inf -> infinity limit, so any finite ``grad_out`` gives a finite result."""
+    for t, name in ((scores, 'scores'), (alpha, 'alpha'), (grad_out, 'grad_out')):
+        _f(t, name)
+    L.require_cuda(row_masks, 'row_masks', torch.bool); L.require_cuda(col_masks, 'col_masks', torch.bool)
+    p, k, _ = scores.shape
+    if tuple(grad_out.shape) != (p, k + 1, k + 1):
+        raise RuntimeError(f'sinkhorn_backward: grad_out must be ({p}, {k + 1}, {k + 1}), got {tuple(grad_out.shape)}')
+    dev = scores.device
+    lib = L.lib()
+    gs = torch.empty((p, k, k), dtype=_f32, device=dev)
+    ga = torch.empty((), dtype=_f32, device=dev)
+    ws = L.workspace(lib.geob200_sinkhorn_backward_workspace_bytes(p, k, int(num_iterations)), dev, tag='sinkhorn_backward')
+    L.check(lib.geob200_sinkhorn_backward(scores.data_ptr(), row_masks.data_ptr(), col_masks.data_ptr(), alpha.data_ptr(), p, k,
+                                          int(num_iterations), float(inf), grad_out.data_ptr(), gs.data_ptr(), ga.data_ptr(),
+                                          ws.data_ptr(), ws.numel(), L.stream_ptr()), 'sinkhorn_backward')
+    return gs, ga
+
+
+class _Sinkhorn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, scores, row_masks, col_masks, alpha, num_iterations, inf):
+        ctx.save_for_backward(scores, row_masks, col_masks, alpha)
+        ctx.args = (num_iterations, inf)
+        return _sinkhorn(scores, row_masks, col_masks, alpha, num_iterations, inf)
+
+    @staticmethod
+    def backward(ctx, grad):
+        scores, row_masks, col_masks, alpha = ctx.saved_tensors
+        num_iterations, inf = ctx.args
+        gs, ga = sinkhorn_backward(scores, row_masks, col_masks, alpha, num_iterations, grad.contiguous(), inf)
+        return (gs if ctx.needs_input_grad[0] else None, None, None, ga.reshape(alpha.shape) if ctx.needs_input_grad[3] else None,
+                None, None)
 
 
 def local_global_registration(ref_knn_points, src_knn_points, ref_knn_masks, src_knn_masks, score_mat, k, acceptance_radius,
@@ -759,6 +809,8 @@ def patch_scores_batched(feats, cloud_points, ref_knn_indices, src_knn_indices):
 
 def _patch_scores(ref_feats, src_feats, cloud_points, ref_knn_indices, src_knn_indices):
     """``patch_scores_batched`` with the ref clouds' fine rows in ``ref_feats`` and the src clouds' in ``src_feats``"""
+    if _needs_grad(ref_feats, src_feats):
+        return _PatchScores.apply(ref_feats, src_feats, tuple(int(c) for c in cloud_points), ref_knn_indices, src_knn_indices)
     ref_feats, src_feats = _detach(ref_feats), _detach(src_feats)
     B = len(cloud_points) // 2
     p, k = ref_knn_indices.shape
@@ -767,6 +819,42 @@ def _patch_scores(ref_feats, src_feats, cloud_points, ref_knn_indices, src_knn_i
                                                  ref_knn_indices.data_ptr(), src_knn_indices.data_ptr(), p // B, k, out.data_ptr(),
                                                  L.stream_ptr()), 'patch_scores_batched')
     return out
+
+
+def patch_scores_backward_batched(ref_feats, src_feats, cloud_points, ref_knn_indices, src_knn_indices, grad_scores):
+    """(grad_ref_feats, grad_src_feats) of ``_patch_scores`` (ref / src blocks as there) for the upstream gradient ``grad_scores``
+    (P, k, k): each feature row sums its (patch, slot) contributions in (patch, slot) order; rows no patch reads get zeros."""
+    _f(ref_feats, 'ref_feats'); _f(src_feats, 'src_feats'); _f(grad_scores, 'grad_scores')
+    L.require_cuda(ref_knn_indices, 'ref_knn_indices', _i64); L.require_cuda(src_knn_indices, 'src_knn_indices', _i64)
+    B = len(cloud_points) // 2
+    p, k = ref_knn_indices.shape
+    if tuple(grad_scores.shape) != (p, k, k) or tuple(src_knn_indices.shape) != (p, k):
+        raise RuntimeError(f'patch_scores_backward_batched: grad_scores must be ({p}, {k}, {k}) and the index tensors ({p}, {k})')
+    dev = ref_feats.device
+    lib = L.lib()
+    gr, gs = torch.empty_like(ref_feats), torch.empty_like(src_feats)
+    rows = ref_feats.shape[0] + src_feats.shape[0]
+    ws = L.workspace(lib.geob200_patch_scores_backward_batched_workspace_bytes(rows, p, k, ref_feats.shape[1]), dev,
+                     tag='patch_scores_backward')
+    L.check(lib.geob200_patch_scores_backward_batched(ref_feats.data_ptr(), src_feats.data_ptr(), ref_feats.shape[1], B,
+                                                      _host_i64(cloud_points), ref_knn_indices.data_ptr(), src_knn_indices.data_ptr(),
+                                                      p // B, k, grad_scores.data_ptr(), gr.data_ptr(), gs.data_ptr(), ws.data_ptr(),
+                                                      ws.numel(), L.stream_ptr()), 'patch_scores_backward_batched')
+    return gr, gs
+
+
+class _PatchScores(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, ref_feats, src_feats, cloud_points, ref_knn_indices, src_knn_indices):
+        ctx.save_for_backward(ref_feats, src_feats, ref_knn_indices, src_knn_indices)
+        ctx.cloud_points = cloud_points
+        return _patch_scores(ref_feats, src_feats, cloud_points, ref_knn_indices, src_knn_indices)
+
+    @staticmethod
+    def backward(ctx, grad):
+        ref_feats, src_feats, ri, si = ctx.saved_tensors
+        gr, gs = patch_scores_backward_batched(ref_feats, src_feats, ctx.cloud_points, ri, si, grad.contiguous())
+        return gr if ctx.needs_input_grad[0] else None, gs if ctx.needs_input_grad[1] else None, None, None, None
 
 
 def local_global_registration_batched(n_pairs, ref_knn_points, src_knn_points, ref_knn_masks, src_knn_masks, score_mat, k,
@@ -821,9 +909,12 @@ def evaluate_batched(gt_indices, gt_overlaps, n_gt, corr_indices, n_node_corr, r
 
 
 # ------------------------------------------------------------------------------------------------ validation losses
-# OverallLoss values (reference experiments/<exp>/loss.py:10-92) without gradients.  ``out``: (B, >= 3 columns, any row stride)
+# OverallLoss values (reference experiments/<exp>/loss.py:10-92).  ``out``: (B, >= 3 columns, any row stride)
 # rows [loss, c_loss, f_loss]; the coarse call writes column 1, the fine call column 2 and, given ``loss_weights``, column 0 from
 # column 1 -- so run the fine call after the coarse one on the same stream.  Counts are optional DEVICE int32 tensors: no read-back.
+# When gradients are required (grad mode on and the features / scores require grad) the calls return fresh (B, 3) rows (zeros in the
+# columns they do not write) carrying the graph to ``ref_feats`` / ``src_feats`` (coarse) and ``matching_scores`` (fine); ``out`` must
+# then be None.  The values are the same kernels' either way.
 
 def _loss_rows(out, B, dev):
     if out is None:
@@ -839,6 +930,22 @@ def coarse_matching_loss_batched(ref_feats, src_feats, cloud_nodes, gt_indices, 
     """CoarseMatchingLoss of B pairs: pair p's superpoints at rows sum_{q<p} n_ref(q) of ``ref_feats`` / sum_{q<p} n_src(q) of
     ``src_feats`` (``cloud_nodes``: 2B host counts, ref clouds first), its ground-truth rows at sum_{q<p} n_ref(q) * n_src(q) of
     ``gt_indices`` / ``gt_overlaps`` with ``gt_count[p]`` (device int32) valid.  Writes column 1 of ``out``."""
+    coarse = dict(cloud_nodes=tuple(int(c) for c in cloud_nodes), gt_indices=gt_indices, gt_overlaps=gt_overlaps, gt_count=gt_count,
+                  params=(positive_margin, negative_margin, positive_optimal, negative_optimal, log_scale, positive_overlap))
+    if _needs_grad(ref_feats, src_feats):
+        _no_out(out)
+        return _LossRows.apply(ref_feats, src_feats, None, coarse, None, None)
+    return _coarse_loss_values(ref_feats, src_feats, out=out, **coarse)
+
+
+def _no_out(out):
+    if out is not None:
+        raise RuntimeError('loss out= is a value-only buffer: pass out=None when gradients are required')
+
+
+def _coarse_loss_values(ref_feats, src_feats, cloud_nodes, gt_indices, gt_overlaps, gt_count, params, out):
+    ref_feats, src_feats = _detach(ref_feats), _detach(src_feats)
+    positive_margin, negative_margin, positive_optimal, negative_optimal, log_scale, positive_overlap = params
     _f(ref_feats, 'ref_feats'); _f(src_feats, 'src_feats'); _f(gt_overlaps, 'gt_node_corr_overlaps')
     L.require_cuda(gt_indices, 'gt_node_corr_indices', _i64); L.require_cuda(gt_count, 'gt_count', _i32)
     B = len(cloud_nodes) // 2
@@ -861,6 +968,16 @@ def fine_matching_loss_batched(n_pairs, ref_knn_points, src_knn_points, ref_knn_
     """FineMatchingLoss of B pairs: patch q of pair p at row p * P + q of the (B * P, k, 3) points, (B * P, k) masks and
     (B * P, k+1, k+1) Sinkhorn scores; ``transforms`` (B, 4, 4); ``patch_count`` (B,) device int32 or None (all P).  Writes column 2
     of ``out``; with ``loss_weights`` = (w_coarse, w_fine) also column 0 from column 1."""
+    fine = dict(n_pairs=int(n_pairs), ref_knn_points=ref_knn_points, src_knn_points=src_knn_points, ref_knn_masks=ref_knn_masks,
+                src_knn_masks=src_knn_masks, transforms=transforms, positive_radius=positive_radius, patch_count=patch_count)
+    if _needs_grad(matching_scores):
+        _no_out(out)
+        return _LossRows.apply(None, None, matching_scores, None, fine, loss_weights)
+    return _fine_loss_values(matching_scores=_detach(matching_scores), loss_weights=loss_weights, out=out, **fine)
+
+
+def _fine_loss_values(n_pairs, ref_knn_points, src_knn_points, ref_knn_masks, src_knn_masks, matching_scores, transforms, positive_radius,
+                      patch_count, loss_weights, out):
     for t, name in ((ref_knn_points, 'ref_node_corr_knn_points'), (src_knn_points, 'src_node_corr_knn_points'),
                     (matching_scores, 'matching_scores'), (transforms, 'transform')):
         _f(t, name)
@@ -881,6 +998,101 @@ def fine_matching_loss_batched(n_pairs, ref_knn_points, src_knn_points, ref_knn_
     return out
 
 
+def _grad_rows(grad_rows, B):
+    _f(grad_rows, 'grad_rows')
+    if grad_rows.dim() != 2 or grad_rows.shape[0] != B or grad_rows.shape[1] < 3:
+        raise RuntimeError(f'grad_rows must be ({B}, >= 3)')
+    return grad_rows
+
+
+def _host_weights(loss_weights):
+    return None if loss_weights is None else (ctypes.c_float * 2)(float(loss_weights[0]), float(loss_weights[1]))
+
+
+def coarse_matching_loss_backward_batched(ref_feats, src_feats, cloud_nodes, gt_indices, gt_overlaps, gt_count, params, grad_rows,
+                                          loss_weights=None):
+    """(grad_ref_feats, grad_src_feats) of ``coarse_matching_loss_batched`` (``params``: its six float arguments in order) for the
+    upstream gradient ``grad_rows`` (B, >= 3) of the [loss, c_loss, f_loss] rows; column 0 reaches c_loss through loss_weights[0]."""
+    _f(ref_feats, 'ref_feats'); _f(src_feats, 'src_feats'); _f(gt_overlaps, 'gt_node_corr_overlaps')
+    L.require_cuda(gt_indices, 'gt_node_corr_indices', _i64); L.require_cuda(gt_count, 'gt_count', _i32)
+    B = len(cloud_nodes) // 2
+    grad_rows = _grad_rows(grad_rows, B)
+    dev = ref_feats.device
+    rows = sum(int(c) for c in cloud_nodes)
+    nn = sum(int(cloud_nodes[p]) * int(cloud_nodes[B + p]) for p in range(B))
+    lib = L.lib()
+    gr, gs = torch.empty_like(ref_feats), torch.empty_like(src_feats)
+    ws = L.workspace(lib.geob200_coarse_matching_loss_backward_batched_workspace_bytes(rows, nn, B), dev, tag='coarse_loss_backward')
+    L.check(lib.geob200_coarse_matching_loss_backward_batched(
+        ref_feats.data_ptr(), src_feats.data_ptr(), ref_feats.shape[1], B, _host_i64(cloud_nodes), gt_indices.data_ptr(),
+        gt_overlaps.data_ptr(), gt_count.data_ptr(), *(float(v) for v in params), grad_rows.data_ptr(), grad_rows.stride(0),
+        _host_weights(loss_weights), gr.data_ptr(), gs.data_ptr(), ws.data_ptr(), ws.numel(), L.stream_ptr()),
+        'coarse_matching_loss_backward_batched')
+    return gr, gs
+
+
+def fine_matching_loss_backward_batched(n_pairs, ref_knn_points, src_knn_points, ref_knn_masks, src_knn_masks, transforms, positive_radius,
+                                        grad_rows, patch_count=None, loss_weights=None):
+    """grad of ``fine_matching_loss_batched`` w.r.t. its (B * P, k+1, k+1) matching scores for the upstream gradient ``grad_rows``
+    (B, >= 3): -g_p / #labels of pair p on the label entries, 0 elsewhere; column 0 reaches f_loss through loss_weights[1]."""
+    for t, name in ((ref_knn_points, 'ref_node_corr_knn_points'), (src_knn_points, 'src_node_corr_knn_points'), (transforms, 'transform')):
+        _f(t, name)
+    L.require_cuda(ref_knn_masks, 'ref_node_corr_knn_masks', torch.bool); L.require_cuda(src_knn_masks, 'src_node_corr_knn_masks', torch.bool)
+    if patch_count is not None:
+        L.require_cuda(patch_count, 'patch_count', _i32)
+    B = int(n_pairs)
+    grad_rows = _grad_rows(grad_rows, B)
+    rows, k = ref_knn_masks.shape
+    dev = ref_knn_points.device
+    lib = L.lib()
+    g = torch.empty((rows, k + 1, k + 1), dtype=_f32, device=dev)
+    ws = L.workspace(lib.geob200_fine_matching_loss_backward_batched_workspace_bytes(B, rows // B), dev, tag='fine_loss_backward')
+    L.check(lib.geob200_fine_matching_loss_backward_batched(
+        ref_knn_points.data_ptr(), src_knn_points.data_ptr(), ref_knn_masks.data_ptr(), src_knn_masks.data_ptr(), transforms.data_ptr(), B,
+        rows // B, k, L.ptr(patch_count), float(positive_radius), grad_rows.data_ptr(), grad_rows.stride(0), _host_weights(loss_weights),
+        g.data_ptr(), ws.data_ptr(), ws.numel(), L.stream_ptr()), 'fine_matching_loss_backward_batched')
+    return g
+
+
+class _LossRows(torch.autograd.Function):
+    """[loss, c_loss, f_loss] rows (B, 3) of the coarse loss (``coarse``: the arguments of _coarse_loss_values), the fine loss
+    (``fine``) or both, from the value kernels; backward through the loss backward kernels.  With ``weights`` (w_coarse, w_fine)
+    column 0 is the weighted total, as the fine value kernel writes it."""
+
+    @staticmethod
+    def forward(ctx, ref_feats, src_feats, scores, coarse, fine, weights):
+        B = len(coarse['cloud_nodes']) // 2 if coarse is not None else fine['n_pairs']
+        dev = (scores if scores is not None else ref_feats).device
+        out = torch.zeros((B, 3), dtype=_f32, device=dev)
+        if coarse is not None:
+            _coarse_loss_values(ref_feats, src_feats, out=out, **coarse)
+        if fine is not None:
+            _fine_loss_values(matching_scores=scores, loss_weights=weights, out=out, **fine)
+        ctx.save_for_backward(ref_feats, src_feats)
+        ctx.coarse, ctx.fine, ctx.weights = coarse, fine, weights
+        return out
+
+    @staticmethod
+    def backward(ctx, grad):
+        ref_feats, src_feats = ctx.saved_tensors
+        grad = grad.contiguous()
+        gr = gs = gsc = None
+        if ctx.coarse is not None and (ctx.needs_input_grad[0] or ctx.needs_input_grad[1]):
+            gr, gs = coarse_matching_loss_backward_batched(ref_feats, src_feats, grad_rows=grad, loss_weights=ctx.weights, **ctx.coarse)
+        if ctx.fine is not None and ctx.needs_input_grad[2]:
+            gsc = fine_matching_loss_backward_batched(grad_rows=grad, loss_weights=ctx.weights, **ctx.fine)
+        return gr, gs, gsc, None, None, None
+
+
+def matching_losses_batched(ref_feats, src_feats, matching_scores, coarse, fine, loss_weights):
+    """OverallLoss rows (B, 3) [loss, c_loss, f_loss] with gradients: ``coarse`` / ``fine`` are the keyword arguments of
+    ``coarse_matching_loss_batched`` (cloud_nodes, gt_indices, gt_overlaps, gt_count, params = the six floats) and
+    ``fine_matching_loss_batched`` (n_pairs, ref_knn_points, src_knn_points, ref_knn_masks, src_knn_masks, transforms, positive_radius,
+    patch_count) without the differentiable inputs."""
+    coarse = dict(coarse, cloud_nodes=tuple(int(c) for c in coarse['cloud_nodes']))
+    return _LossRows.apply(ref_feats, src_feats, matching_scores, coarse, fine, tuple(loss_weights))
+
+
 def _one_count(n, count, dev):
     return count.reshape(1) if count is not None else torch.full((1,), int(n), dtype=_i32, device=dev)
 
@@ -890,12 +1102,15 @@ def coarse_matching_loss(ref_feats, src_feats, gt_node_corr_indices, gt_node_cor
     """CoarseMatchingLoss of one pair (the batched kernels with B = 1); ``out``: (>= 3,) row, column 1 written.
     ``n_gt``: optional device int32 count of valid ground-truth rows (full-capacity buffers)."""
     dev = ref_feats.device
+    cnt = _one_count(gt_node_corr_indices.shape[0], n_gt, dev)
+    args = ([ref_feats.shape[0], src_feats.shape[0]], gt_node_corr_indices, gt_node_corr_overlaps, cnt, positive_margin, negative_margin,
+            positive_optimal, negative_optimal, log_scale, positive_overlap)
+    if _needs_grad(ref_feats, src_feats):
+        _no_out(out)
+        return coarse_matching_loss_batched(ref_feats, src_feats, *args).reshape(3)
     if out is None:
         out = torch.empty((3,), dtype=_f32, device=dev)
-    cnt = _one_count(gt_node_corr_indices.shape[0], n_gt, dev)
-    coarse_matching_loss_batched(ref_feats, src_feats, [ref_feats.shape[0], src_feats.shape[0]], gt_node_corr_indices,
-                                 gt_node_corr_overlaps, cnt, positive_margin, negative_margin, positive_optimal, negative_optimal,
-                                 log_scale, positive_overlap, out=out)
+    coarse_matching_loss_batched(ref_feats, src_feats, *args, out=out)
     return out
 
 
@@ -904,11 +1119,14 @@ def fine_matching_loss(ref_knn_points, src_knn_points, ref_knn_masks, src_knn_ma
     """FineMatchingLoss of one pair; ``out``: (>= 3,) row, column 2 (and column 0 given ``loss_weights``) written.
     ``n_patches``: optional device int32 count of valid patches (full-capacity buffers)."""
     dev = matching_scores.device
+    kw = dict(patch_count=None if n_patches is None else n_patches.reshape(1), loss_weights=loss_weights)
+    args = (1, ref_knn_points, src_knn_points, ref_knn_masks, src_knn_masks, matching_scores, transform, positive_radius)
+    if _needs_grad(matching_scores):
+        _no_out(out)
+        return fine_matching_loss_batched(*args, **kw).reshape(3)
     if out is None:
         out = torch.empty((3,), dtype=_f32, device=dev)
-    fine_matching_loss_batched(1, ref_knn_points, src_knn_points, ref_knn_masks, src_knn_masks, matching_scores, transform,
-                               positive_radius, patch_count=None if n_patches is None else n_patches.reshape(1),
-                               loss_weights=loss_weights, out=out)
+    fine_matching_loss_batched(*args, **kw, out=out)
     return out
 
 

@@ -5,8 +5,10 @@ Same constructor/forward contract as the reference's three Evaluator classes (3D
 RMSE and RR are defined; ``cfg.name`` selects).  All six numbers come from ONE kernel launch (`geob200_evaluate_counts`); the
 result dict holds 0-dim device tensors like the reference's.  KITTI has no RMSE entry (loss.py:140-151 there).
 
-The losses are the values the reference's ``val_step`` reports on the eval-mode forward.  They carry NO autograd graph:
-backward is not provided (training stays out of scope).  There is no CPU path: non-CUDA inputs raise RuntimeError.
+The losses are the values the reference's ``val_step`` reports on the eval-mode forward.  When grad mode is on and the coarse
+features (``ref_feats_c`` / ``src_feats_c``) or the Sinkhorn ``matching_scores`` require grad, the loss modules return 0-dim tensors
+carrying the graph back to them (the backward runs on the device: ``functional.*_backward_batched``); the values are the same kernels'
+bits either way.  There is no CPU path: non-CUDA inputs raise RuntimeError.
 """
 import torch
 import torch.nn as nn
@@ -69,6 +71,10 @@ class CoarseMatchingLoss(nn.Module):
                                        output_dict['gt_node_corr_overlaps'], *self.params(), out=out, n_gt=_counts(output_dict).get('gt'))
 
     def forward(self, output_dict):
+        rf, sf = output_dict['ref_feats_c'], output_dict['src_feats_c']
+        if GF._needs_grad(rf, sf):
+            return GF.coarse_matching_loss(rf, sf, output_dict['gt_node_corr_indices'], output_dict['gt_node_corr_overlaps'], *self.params(),
+                                           n_gt=_counts(output_dict).get('gt'))[1]
         return self.write(output_dict, None)[1]
 
 
@@ -88,12 +94,20 @@ class FineMatchingLoss(nn.Module):
                                      loss_weights=loss_weights, out=out, n_patches=_counts(output_dict).get('node_corr'))
 
     def forward(self, output_dict, data_dict):
+        if GF._needs_grad(output_dict['matching_scores']):
+            return GF.fine_matching_loss(*self.inputs(output_dict, data_dict), self.positive_radius,
+                                         n_patches=_counts(output_dict).get('node_corr'))[2]
         return self.write(output_dict, data_dict, None)[2]
+
+    @staticmethod
+    def inputs(output_dict, data_dict):
+        return (output_dict['ref_node_corr_knn_points'], output_dict['src_node_corr_knn_points'], output_dict['ref_node_corr_knn_masks'],
+                output_dict['src_node_corr_knn_masks'], output_dict['matching_scores'], data_dict['transform'])
 
 
 class OverallLoss(nn.Module):
     """weight_coarse_loss * c_loss + weight_fine_loss * f_loss (reference loss.py:74-92): {'loss', 'c_loss', 'f_loss'} as 0-dim
-    device tensors.  Values only: no gradients."""
+    device tensors, differentiable w.r.t. the coarse features and the matching scores when they require grad."""
 
     def __init__(self, cfg):
         super().__init__()
@@ -125,5 +139,24 @@ class OverallLoss(nn.Module):
         return out
 
     def forward(self, output_dict, data_dict):
-        t = self.loss_tensor(output_dict, data_dict)
+        rf, sf, sc = output_dict['ref_feats_c'], output_dict['src_feats_c'], output_dict['matching_scores']
+        if GF._needs_grad(rf, sf, sc):
+            t = self.graph_rows(output_dict, data_dict)[0]
+        else:
+            t = self.loss_tensor(output_dict, data_dict)
         return {'loss': t[0], 'c_loss': t[1], 'f_loss': t[2]}
+
+    def graph_rows(self, output_dict, data_dict):
+        """(1, 3) [loss, c_loss, f_loss] with gradients to the coarse features and the matching scores (the value kernels' bits)"""
+        rf, sf = output_dict['ref_feats_c'], output_dict['src_feats_c']
+        counts = _counts(output_dict)
+        gi = output_dict['gt_node_corr_indices']
+        n_gt = counts.get('gt')
+        n_gt = n_gt.reshape(1) if n_gt is not None else torch.full((1,), gi.shape[0], dtype=torch.int32, device=rf.device)
+        coarse = dict(cloud_nodes=(rf.shape[0], sf.shape[0]), gt_indices=gi, gt_overlaps=output_dict['gt_node_corr_overlaps'],
+                      gt_count=n_gt, params=self.coarse_loss.params())
+        rp, sp, rm, sm, scores, T = FineMatchingLoss.inputs(output_dict, data_dict)
+        n_p = counts.get('node_corr')
+        fine = dict(n_pairs=1, ref_knn_points=rp, src_knn_points=sp, ref_knn_masks=rm, src_knn_masks=sm, transforms=T,
+                    positive_radius=self.fine_loss.positive_radius, patch_count=None if n_p is None else n_p.reshape(1))
+        return GF.matching_losses_batched(rf, sf, scores, coarse, fine, (self.weight_coarse_loss, self.weight_fine_loss))

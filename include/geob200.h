@@ -264,9 +264,31 @@ int geob200_patch_scores_batched(const float* ref_feats, const float* src_feats,
                                  const int64_t* ref_knn_indices, const int64_t* src_knn_indices, int64_t n_patches, int64_t k,
                                  float* scores, void* stream);
 
+/* Backward of geob200_patch_scores_batched (same layout): grad_scores (n_pairs * n_patches, k, k) -> grad_ref_feats / grad_src_feats
+ * with the shapes of ref_feats / src_feats, every row written (zero where no patch reads it).  dR_p = dS_p Fs_p / sqrt(C) and
+ * dS'_p = dS_p^T Fr_p / sqrt(C) per patch, then each feature row sums its (patch, slot) entries in (patch, slot) order (counting sort
+ * of the entries by row; no float atomics).  Sentinel indices (>= the cloud's row count) receive nothing.  n_rows of the workspace
+ * query = all ref + src rows; n_patches_total = n_pairs * n_patches. */
+size_t geob200_patch_scores_backward_batched_workspace_bytes(int64_t n_rows, int64_t n_patches_total, int64_t k, int64_t channels);
+int geob200_patch_scores_backward_batched(const float* ref_feats, const float* src_feats, int64_t channels, int64_t n_pairs,
+                                          const int64_t* cloud_points, const int64_t* ref_knn_indices, const int64_t* src_knn_indices,
+                                          int64_t n_patches, int64_t k, const float* grad_scores, float* grad_ref_feats,
+                                          float* grad_src_feats, void* workspace, size_t workspace_bytes, void* stream);
+
 /* LearnableLogOptimalTransport.forward (learnable_sinkhorn.py:20-66): out (n_patches, k+1, k+1) */
 int geob200_sinkhorn(const float* scores, const uint8_t* row_masks, const uint8_t* col_masks, const float* alpha,
                      int64_t n_patches, int64_t k, int64_t num_iterations, float inf, float* out, void* stream);
+
+/* Backward of geob200_sinkhorn: grad_out (n_patches, k+1, k+1) -> grad_scores (n_patches, k, k), zero on masked entries, and
+ * grad_alpha (one device float) = the sum of the gradient over the unmasked dustbin entries of all patches, summed per patch and then
+ * over the patches in index order (no atomics: a patch gives the same bits alone and in any batch).  The CTA of a patch re-runs the
+ * forward iterations and keeps their log-sum-exps in the workspace (2 * num_iterations * (k+1) floats per patch), then sweeps them in
+ * reverse.  Masked lines follow the inf -> infinity limit (finite for any grad_out); a patch without a valid row and without a valid
+ * column gets zeros.  k must be 32, 64 or 128. */
+size_t geob200_sinkhorn_backward_workspace_bytes(int64_t n_patches, int64_t k, int64_t num_iterations);
+int geob200_sinkhorn_backward(const float* scores, const uint8_t* row_masks, const uint8_t* col_masks, const float* alpha, int64_t n_patches,
+                              int64_t k, int64_t num_iterations, float inf, const float* grad_out, float* grad_scores, float* grad_alpha,
+                              void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---- local-to-global registration -------------------------------------------------------------------------- */
 
@@ -356,6 +378,27 @@ int geob200_fine_matching_loss_batched(const float* ref_knn_points, const float*
                                        int64_t n_patches, int64_t k, const int32_t* patch_count, double positive_radius,
                                        const float* loss_weights, float* out, int64_t out_ld, void* workspace, size_t workspace_bytes,
                                        void* stream);
+
+/* Backward of the two losses.  grad_rows (device, n_pairs rows of stride grad_ld >= 3) is the upstream gradient of the [loss, c_loss,
+ * f_loss] rows; with loss_weights (HOST {w_coarse, w_fine}, may be NULL) column 0 reaches c_loss / f_loss through the weights.  The
+ * arguments otherwise mirror the forward entry points.  Coarse: grad_ref_feats / grad_src_feats (shapes of ref_feats / src_feats); a
+ * half (rows or columns) of a pair with no kept line contributes zero, as torch autograd gives on the NaN loss, and an entry at feature
+ * distance 0 gives inf / NaN where torch's sqrt backward does.  Fine: grad_scores (n_pairs * n_patches, k+1, k+1) = -g / #labels of
+ * the pair on the label entries, 0 elsewhere (and everywhere for a pair without labels or a patch at or beyond patch_count[p]). */
+size_t geob200_coarse_matching_loss_backward_batched_workspace_bytes(int64_t n_rows, int64_t n_products, int64_t n_pairs);
+int geob200_coarse_matching_loss_backward_batched(const float* ref_feats, const float* src_feats, int64_t channels, int64_t n_pairs,
+                                                  const int64_t* cloud_nodes, const int64_t* gt_node_corr_indices,
+                                                  const float* gt_node_corr_overlaps, const int32_t* gt_count, float positive_margin,
+                                                  float negative_margin, float positive_optimal, float negative_optimal, float log_scale,
+                                                  float positive_overlap, const float* grad_rows, int64_t grad_ld, const float* loss_weights,
+                                                  float* grad_ref_feats, float* grad_src_feats, void* workspace, size_t workspace_bytes,
+                                                  void* stream);
+size_t geob200_fine_matching_loss_backward_batched_workspace_bytes(int64_t n_pairs, int64_t n_patches);
+int geob200_fine_matching_loss_backward_batched(const float* ref_knn_points, const float* src_knn_points, const uint8_t* ref_knn_masks,
+                                                const uint8_t* src_knn_masks, const float* transforms, int64_t n_pairs, int64_t n_patches,
+                                                int64_t k, const int32_t* patch_count, double positive_radius, const float* grad_rows,
+                                                int64_t grad_ld, const float* loss_weights, float* grad_scores, void* workspace,
+                                                size_t workspace_bytes, void* stream);
 
 /* Correspondence RANSAC (Open3D's registration_ransac_based_on_correspondence as utils/open3d.py:169-198 calls it) for B pairs:
  * pair p's correspondences are rows [0, num_corr[p]) of (B, capacity, 3) ref / src arrays (num_corr: device int32 or NULL = all
