@@ -366,16 +366,20 @@ __global__ void __launch_bounds__(256) closs_dist_kernel(const float* __restrict
     }
 }
 
-// o[i][j] = overlap of the first count[p] ground-truth rows of pair p (rows at NN.start[p])
+// o[i][j] = overlap of the first count[p] ground-truth rows of pair p (rows at NN.start[p]); a row whose (i, j) lies outside the
+// pair's n_ref x n_src matrix is skipped (the indices come from the caller's output dict)
 __global__ void __launch_bounds__(256) closs_scatter_kernel(const long long* __restrict__ gt_idx, const float* __restrict__ gt_ov,
-                                                            const int* __restrict__ count, const __grid_constant__ Segs Q,
-                                                            const __grid_constant__ Segs NN, float* __restrict__ o) {
+                                                            const int* __restrict__ count, const __grid_constant__ Segs R,
+                                                            const __grid_constant__ Segs Q, const __grid_constant__ Segs NN,
+                                                            float* __restrict__ o) {
     const int p = blockIdx.y;
     const int g = blockIdx.x * blockDim.x + threadIdx.x;
     const int n = min(count[p], NN.count[p]);
     if (g >= n) return;
     gt_idx += 2ll * NN.start[p]; gt_ov += NN.start[p];
-    o[NN.start[p] + gt_idx[2ll * g] * Q.count[p] + gt_idx[2ll * g + 1]] = gt_ov[g];
+    const long long i = gt_idx[2ll * g], j = gt_idx[2ll * g + 1];
+    if ((unsigned long long)i >= (unsigned long long)R.count[p] || (unsigned long long)j >= (unsigned long long)Q.count[p]) return;
+    o[NN.start[p] + i * Q.count[p] + j] = gt_ov[g];
 }
 
 struct CircleParams {
@@ -780,7 +784,7 @@ int geob200_coarse_matching_loss_batched(const float* ref_feats, const float* sr
         closs_dist_kernel<<<dim3((unsigned)R.max, B), 256, channels * sizeof(float), st>>>(ref_feats, src_feats, (int)channels, R, Q, NN, d, o,
                                                                                            nullptr);
         closs_scatter_kernel<<<dim3((unsigned)((NN.max + 255) / 256), B), 256, 0, st>>>((const long long*)gt_node_corr_indices,
-                                                                                        gt_node_corr_overlaps, gt_count, Q, NN, o);
+                                                                                        gt_node_corr_overlaps, gt_count, R, Q, NN, o);
         n_launch += 2;
     }
     if (R.max > 0 || Q.max > 0) {
@@ -884,7 +888,7 @@ int geob200_coarse_matching_loss_backward_batched(const float* ref_feats, const 
         closs_dist_kernel<<<dim3((unsigned)R.max, B), 256, channels * sizeof(float), st>>>(ref_feats, src_feats, (int)channels, R, Q, NN, d, o,
                                                                                            live);
         closs_scatter_kernel<<<dim3((unsigned)((NN.max + 255) / 256), B), 256, 0, st>>>((const long long*)gt_node_corr_indices,
-                                                                                        gt_node_corr_overlaps, gt_count, Q, NN, o);
+                                                                                        gt_node_corr_overlaps, gt_count, R, Q, NN, o);
         closs_lse_kernel<<<dim3((unsigned)(R.max > Q.max ? R.max : Q.max), B, 2), 256, 0, st>>>(d, o, R, Q, NN, cp, ell, kept, ell + n_ref,
                                                                                                 kept + n_ref, lse, lse + n_ref);
         closs_grad_scale_kernel<<<B, 32, 0, st>>>(kept, kept + n_ref, R, Q, grad_rows, (long long)grad_ld, loss_weights != nullptr, w_c,

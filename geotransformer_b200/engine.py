@@ -13,6 +13,7 @@ from concurrent.futures import ThreadPoolExecutor
 import torch
 
 from . import _lib
+from .model import trim_outputs
 from .utils.data import registration_collate_fn_stack_mode
 
 LOSS_KEYS = ('loss', 'c_loss', 'f_loss')
@@ -46,9 +47,9 @@ class RegistrationEngine:
         """pin_cpu: bind the calling thread and the worker threads to the CPUs local to the GPU (pin_host_threads_to_gpu).
         evaluator: optional geotransformer_b200.loss.Evaluator; its metrics (PIR, IR, RRE, RTE, RMSE, RR) are then computed
         on the device for every pair and travel back with the transform in the same D2H copy.
-        batch_size > 1: every worker registers ``batch_size`` pairs per forward (GeoTransformer.forward_batch: one collate,
+        batch_size: every worker registers up to ``batch_size`` pairs per forward (GeoTransformer.forward_batch: one collate,
         one backbone / transformer pass over the stacked rows of all pairs, per-pair stages on ``side_streams`` extra
-        streams), with ONE host synchronisation per batch besides the collate's size read-backs.
+        streams when batch_size > 1), with ONE host synchronisation per forward besides the collate's size read-backs.
         loss_func: optional geotransformer_b200.loss.OverallLoss; every result then gains 'loss': {'loss', 'c_loss', 'f_loss'}
         (the reference's val_step losses), computed on the device and read back with the same event.
         ransac: optional config section (cfg.ransac: distance_threshold, num_points, num_iterations, seed); every result then gains
@@ -82,14 +83,6 @@ class RegistrationEngine:
         self.x_host = [torch.zeros((bs, 26), dtype=torch.float32).pin_memory() if ransac is not None else None for _ in range(num_streams)]
         self.sides = [[torch.cuda.Stream(self.device) for _ in range(side_streams)] if bs > 1 else [] for _ in range(num_streams)]
 
-    def _ransac_one(self, out, transform, row, pair):
-        """RANSAC of one pair's (trimmed) correspondences into ``row`` (26,), metrics of its transform with the evaluator"""
-        from .model import write_ransac_rows
-        write_ransac_rows(self.ransac, out['src_corr_points'].unsqueeze(0), out['ref_corr_points'].unsqueeze(0), None, row.reshape(1, -1),
-                          first_pair=pair)
-        if self.evaluator is not None:
-            self.evaluator.metrics_tensor(dict(out, estimated_transform=row[:16].reshape(4, 4)), {'transform': transform}, out=row[18:26])
-
     def _ransac_result(self, row):
         v = row.tolist()
         r = {'estimated_transform': row[:16].reshape(4, 4).clone(), 'fitness': v[16], 'inlier_rmse': v[17]}
@@ -115,29 +108,8 @@ class RegistrationEngine:
         l_dev, l_host, lf = self.l_dev[slot][:n], self.l_host[slot][:n], self.loss_func
         rs = self.ransac
         x_dev, x_host = (self.x_dev[slot][:n], self.x_host[slot][:n]) if rs is not None else (None, None)
-        if n == 1:             # one pair (batch_size 1, or the trailing pair of a batch): the one-pair forward
-            out = self.model(data)
-            r_dev[0, :16].copy_(out['estimated_transform'].reshape(16))
-            if self.evaluator is not None:
-                self.evaluator.metrics_tensor(out, data, out=r_dev[0, 16:])
-            if lf is not None:
-                lf.loss_tensor(out, data, out=l_dev[0])
-            if rs is not None:
-                self._ransac_one(out, data['transform'], x_dev[0], 0)
-            outs = [out]
-        elif keep:             # trimmed per-pair output dicts (one extra host sync for the counts), metrics from them
-            outs = self.model.forward_batch(data, side_streams=self.sides[slot])
-            for p, o in enumerate(outs):
-                r_dev[p, :16].copy_(o['estimated_transform'].reshape(16))
-                if self.evaluator is not None:
-                    self.evaluator.metrics_tensor(o, {'transform': data['transform'][p]}, out=r_dev[p, 16:])
-                if lf is not None:
-                    lf.loss_tensor(o, {'transform': data['transform'][p]}, out=l_dev[p])
-                if rs is not None:
-                    self._ransac_one(o, data['transform'][p], x_dev[p], p)
-        else:
-            outs = self.model.forward_batch(data, evaluator=self.evaluator, results=r_dev, side_streams=self.sides[slot], keep_outputs=False,
-                                            loss_func=lf, loss_out=l_dev, ransac=rs, ransac_out=x_dev)
+        outs = self.model.forward_batch(data, evaluator=self.evaluator, results=r_dev, side_streams=self.sides[slot], keep_outputs=keep,
+                                        loss_func=lf, loss_out=l_dev, ransac=rs, ransac_out=x_dev)
         r_host.copy_(r_dev, non_blocking=True)
         if lf is not None:
             l_host.copy_(l_dev, non_blocking=True)
@@ -146,6 +118,8 @@ class RegistrationEngine:
         done = torch.cuda.Event()
         done.record(stream)
         done.synchronize()
+        if keep:
+            trim_outputs(outs)
         if marks is not None:          # per-stage GPU time of this batch on its main stream (label = the interval ending at that mark)
             for (_, e0), (label, e1) in zip(marks[:-1], marks[1:]):
                 self.stage_times.setdefault('collate' if label == 'start' else label, []).append(e0.elapsed_time(e1))
@@ -153,13 +127,11 @@ class RegistrationEngine:
         res = []
         for p in range(n):
             row = r_host[p]
-            r = {'estimated_transform': row[:16].reshape(4, 4).clone(), 'num_superpoints': (int(lens_c[p]), int(lens_c[n + p]))}
+            m = row[16:].tolist()
+            r = {'estimated_transform': row[:16].reshape(4, 4).clone(), 'num_superpoints': (int(lens_c[p]), int(lens_c[n + p])),
+                 'num_corr': int(m[6])}
             if self.evaluator is not None:
-                m = row[16:].tolist()
-                r['metrics'] = dict(zip(('PIR', 'IR', 'RRE', 'RTE', 'RMSE', 'RR'), m[:6]))
-                r['num_corr'] = int(m[6])
-            elif n == 1:
-                r['num_corr'] = int(outs[0]['ref_corr_points'].shape[0])
+                r['metrics'] = dict(zip(METRIC_KEYS, m[:6]))
             if lf is not None:
                 r['loss'] = dict(zip(LOSS_KEYS, l_host[p].tolist()))
             if rs is not None:

@@ -372,18 +372,6 @@ def scratch(shape, device, tag):
 
 
 _SCRATCH = {}
-_ARANGE = {}
-
-
-def scratch_arange(n, device, tag='arange'):
-    """arange(n) int64 from a cached, read-only per-device table (no launch, no allocation in steady state)."""
-    key = device.index if device.index is not None else torch.cuda.current_device()
-    buf = _ARANGE.get(key)
-    if buf is None or buf.numel() < n:
-        buf = torch.arange(max(int(n) * 2, 4096), dtype=_i64, device=device)
-        torch.cuda.current_stream(device).synchronize()      # other streams may read it right away
-        _ARANGE[key] = buf
-    return buf[:n]
 
 
 class GseTable:
@@ -539,8 +527,8 @@ def superpoint_matching(ref_feats, src_feats, ref_masks, src_masks, num_correspo
 
 
 def gather_patches(corr_indices, node_knn_indices, node_knn_masks, points):
-    return gather_patches_batched(corr_indices, corr_indices.shape[0], [node_knn_indices.shape[0]], [points.shape[0]], node_knn_indices,
-                                  node_knn_masks, points)
+    return gather_patches_batched(corr_indices.reshape(1, -1), corr_indices.shape[0], [node_knn_indices.shape[0]], [points.shape[0]],
+                                  node_knn_indices, node_knn_masks, points)
 
 
 def patch_scores(ref_feats, src_feats, ref_knn_indices, src_knn_indices):
@@ -718,10 +706,31 @@ def point_to_node_partition_batched(points, nodes, cloud_points, cloud_nodes, po
     return p2n, node_masks, knn, knn_masks
 
 
+def _min_rows(t, rows, name):
+    """host check before a launch: the stacked tensor ``t`` holds the ``rows`` rows its clouds address"""
+    if t.shape[0] < rows:
+        raise RuntimeError(f'{name} has {t.shape[0]} rows, its clouds need {rows}')
+
+
+def _patch_tables(name, rows, k, *tables):
+    """host check before a launch: the (rows, k[, ...]) patch tensors of one call agree"""
+    for t in tables:
+        if tuple(t.shape[:2]) != (rows, k):
+            raise RuntimeError(f'{name}: patch tensors must all have ({rows}, {k}) leading dimensions, got {tuple(t.shape)}')
+
+
 def gather_patches_batched(corr_indices, n_corr, cloud_nodes, cloud_points, node_knn_indices, node_knn_masks, points):
-    """``corr_indices`` (n_clouds * n_corr,) local node indices, cloud after cloud -> (n_clouds * n_corr, k) patches; ``None``:
+    """``corr_indices`` (n_clouds, n_corr) int64 local node indices, cloud after cloud -> (n_clouds * n_corr, k) patches; ``None``:
     every node of every cloud is a patch (rows at the superpoint offsets)"""
+    _f(points, 'points'); L.require_cuda(node_knn_indices, 'node_knn_indices', _i64); L.require_cuda(node_knn_masks, 'node_knn_masks', torch.bool)
     k = node_knn_indices.shape[1]
+    _patch_tables('gather_patches_batched', node_knn_indices.shape[0], k, node_knn_masks)
+    _min_rows(node_knn_indices, sum(int(c) for c in cloud_nodes), 'node_knn_indices')
+    _min_rows(points, sum(int(c) for c in cloud_points), 'points')
+    if corr_indices is not None:
+        L.require_cuda(corr_indices, 'corr_indices', _i64)
+        if tuple(corr_indices.shape) != (len(cloud_nodes), n_corr):
+            raise RuntimeError(f'gather_patches_batched: corr_indices must be ({len(cloud_nodes)}, {n_corr}), got {tuple(corr_indices.shape)}')
     rows = len(cloud_nodes) * n_corr if corr_indices is not None else node_knn_indices.shape[0]
     dev = points.device
     idx = torch.empty((rows, k), dtype=_i64, device=dev)
@@ -812,8 +821,15 @@ def _patch_scores(ref_feats, src_feats, cloud_points, ref_knn_indices, src_knn_i
     if _needs_grad(ref_feats, src_feats):
         return _PatchScores.apply(ref_feats, src_feats, tuple(int(c) for c in cloud_points), ref_knn_indices, src_knn_indices)
     ref_feats, src_feats = _detach(ref_feats), _detach(src_feats)
+    _f(ref_feats, 'ref_feats'); _f(src_feats, 'src_feats')
+    L.require_cuda(ref_knn_indices, 'ref_knn_indices', _i64); L.require_cuda(src_knn_indices, 'src_knn_indices', _i64)
     B = len(cloud_points) // 2
     p, k = ref_knn_indices.shape
+    if B < 1 or p % B:
+        raise RuntimeError(f'patch_scores_batched: {p} patch rows are not a multiple of {B} pairs')
+    _patch_tables('patch_scores_batched', p, k, src_knn_indices)
+    _min_rows(ref_feats, _ref_rows(cloud_points), 'ref_feats')
+    _min_rows(src_feats, sum(int(c) for c in cloud_points[B:]), 'src_feats')
     out = torch.empty((p, k, k), dtype=_f32, device=ref_feats.device)
     L.check(L.lib().geob200_patch_scores_batched(ref_feats.data_ptr(), src_feats.data_ptr(), ref_feats.shape[1], B, _host_i64(cloud_points),
                                                  ref_knn_indices.data_ptr(), src_knn_indices.data_ptr(), p // B, k, out.data_ptr(),
@@ -863,8 +879,18 @@ def local_global_registration_batched(n_pairs, ref_knn_points, src_knn_points, r
     """stacked ``local_global_registration`` (deferred counts): (ref_c (B, cap, 3), src_c, scores (B, cap), T, counts (B,) int32).
     ``transform_out``: (B, >= 16) float rows (row stride = its stride(0)) to write the transforms into; else T is (B, 16).
     ``details``: also a dict corr_patch (B, cap), patch_transforms (B * P, 4, 4), patch_inliers (B * P,), best (B,)."""
+    for t, name in ((ref_knn_points, 'ref_knn_points'), (src_knn_points, 'src_knn_points'), (score_mat, 'score_mat')):
+        _f(t, name)
+    L.require_cuda(ref_knn_masks, 'ref_knn_masks', torch.bool); L.require_cuda(src_knn_masks, 'src_knn_masks', torch.bool)
     pt, kk = ref_knn_masks.shape
     B = int(n_pairs)
+    if B < 1 or pt % B:
+        raise RuntimeError(f'local_global_registration_batched: {pt} patch rows are not a multiple of {B} pairs')
+    _patch_tables('local_global_registration_batched', pt, kk, src_knn_masks, ref_knn_points, src_knn_points)
+    if ref_knn_points.shape[2:] != (3,) or src_knn_points.shape[2:] != (3,):
+        raise RuntimeError('local_global_registration_batched: patch points must be (rows, k, 3)')
+    if score_mat.shape[0] != pt:
+        raise RuntimeError(f'local_global_registration_batched: score_mat must have {pt} patch rows, got {tuple(score_mat.shape)}')
     P = pt // B
     dev = score_mat.device
     lib = L.lib()
@@ -898,6 +924,20 @@ def evaluate_batched(gt_indices, gt_overlaps, n_gt, corr_indices, n_node_corr, r
     node_correspondences_batched / superpoint_matching_batched / local_global_registration_batched, ``points`` = the stacked
     input clouds (``cloud_points`` their 2B counts)"""
     B = len(cloud_nodes) // 2
+    L.require_cuda(gt_indices, 'gt_indices', _i64); L.require_cuda(corr_indices, 'corr_indices', _i64); _f(gt_overlaps, 'gt_overlaps')
+    _f(ref_corr_points, 'ref_corr_points'); _f(src_corr_points, 'src_corr_points'); _f(points, 'points')
+    for t, name in ((n_gt, 'n_gt'), (n_node_corr, 'n_node_corr'), (n_corr, 'n_corr')):
+        L.require_cuda(t, name, _i32)
+        if t.numel() < B:
+            raise RuntimeError(f'evaluate_batched: {name} must hold {B} counts')
+    if corr_indices.ndim != 2 or corr_indices.shape[0] != 2 * B:
+        raise RuntimeError(f'evaluate_batched: corr_indices must be ({2 * B}, k), got {tuple(corr_indices.shape)}')
+    if ref_corr_points.ndim != 3 or ref_corr_points.shape[0] != B or ref_corr_points.shape[2] != 3 or src_corr_points.shape != ref_corr_points.shape:
+        raise RuntimeError(f'evaluate_batched: correspondence points must both be ({B}, capacity, 3)')
+    nn = sum(int(cloud_nodes[p]) * int(cloud_nodes[B + p]) for p in range(B))
+    _min_rows(gt_indices, nn, 'gt_indices')
+    _min_rows(gt_overlaps, nn, 'gt_overlaps')
+    _min_rows(points, sum(int(c) for c in cloud_points), 'points')
     k = corr_indices.shape[1]
     L.check(L.lib().geob200_evaluate_batched(
         gt_indices.data_ptr(), gt_overlaps.data_ptr(), n_gt.data_ptr(), float(acceptance_overlap), corr_indices.data_ptr(),

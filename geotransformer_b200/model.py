@@ -41,27 +41,42 @@ class GeoTransformer(nn.Module):
 
     @torch.no_grad()
     def forward_batch(self, data_dict, evaluator=None, results=None, side_streams=None, keep_outputs=True, loss_func=None, loss_out=None,
-                      ransac=None, ransac_out=None):
-        """Several pairs per forward (``data_dict['batch_size'] = B > 1`` from ``registration_collate_fn_stack_mode``, stack
-        order ``[ref_1..ref_B, src_1..src_B]`` at every level) -- the reference asserts batch_size == 1
+                      ransac=None, ransac_out=None, taps=None):
+        """B pairs per forward (``data_dict['batch_size']`` from ``registration_collate_fn_stack_mode``, stack order
+        ``[ref_1..ref_B, src_1..src_B]`` at every level) -- the reference asserts batch_size == 1
         (``engine/single_tester.py:39-74``, README "only batch_size=1 is supported").  Backbone and transformer run ONCE over
         the stacked rows of all pairs (per-pair GroupNorm statistics, batched attention launches, one structure-embedding
         launch); the per-pair stages run once for all pairs too (one launch per stage, the pair index in the grid): grouping and
-        ground-truth correspondences on the first of ``side_streams`` (overlapping the backbone), matching, Sinkhorn, LGR and the
-        metrics on the current stream.  Per pair the arithmetic is the single-pair forward's.
+        ground-truth correspondences on the first of ``side_streams`` (overlapping the backbone; without side streams on the
+        current stream), matching, Sinkhorn, LGR and the metrics on the current stream.  Backbone and transformer run through
+        the native stage drivers after ``enable_native``, else through the modules (one pair only): the drivers' bit-for-bit
+        reference.
 
-        Returns a list of per-pair output dicts (``keep_outputs``), each like ``forward``'s.  With ``results`` (a (B, 24)
-        float device tensor) the estimated transform (16) and, with ``evaluator``, the metrics (8) of pair p are written to
-        row p WITHOUT any host synchronisation in this call (correspondence tensors then stay full-capacity).  With ``loss_func``
+        Returns a list of per-pair output dicts (``keep_outputs``), trimmed to their counts after one host synchronisation.
+        With ``results`` (a (B, 24) float device tensor) the estimated transform (16), the number of LGR correspondences
+        (column 22) and, with ``evaluator``, the metrics (8, from column 16) of pair p are written to row p WITHOUT any host
+        synchronisation in this call; the output dicts then keep the full-capacity buffers and the device counts under
+        ``_counts`` (``trim_outputs``).  With ``loss_func``
         (a geotransformer_b200.loss.OverallLoss) and ``loss_out`` (a (B, 3) float device tensor) the validation losses
         [loss, c_loss, f_loss] of pair p are written to row p of ``loss_out`` after LGR, also without a host synchronisation.
         With ``ransac`` (a config section: distance_threshold, num_points, num_iterations, seed) and ``ransac_out`` (a (B, 26)
         float device tensor) correspondence RANSAC runs on the LGR correspondences of every pair (pair p draws from the stream
         (seed, p)); row p receives [transform (16), fitness, inlier_rmse] and, with ``evaluator``, the metrics (8) of the RANSAC
-        transform -- no host synchronisation either."""
+        transform -- no host synchronisation either.
+
+        Test hooks for one pair: ``taps`` (a dict) receives the pair's ref_/src_ node_masks, node_knn_indices and
+        node_knn_masks, the backbone's ``feats_c`` / ``feats_f`` and ``matching_scores_raw`` (before Sinkhorn);
+        ``data_dict['forced_node_corr']`` (ref indices, src indices, scores) replaces the superpoint matching."""
+        B = int(data_dict.get('batch_size', 1))
+        forced = data_dict.get('forced_node_corr')
+        if B > 1 and (taps is not None or forced is not None):
+            raise ValueError('forward_batch: taps and forced_node_corr apply to one pair per forward')
         native = getattr(self, '_native', None)
-        if native is None:
-            raise RuntimeError('forward_batch needs the native stage drivers: call enable_native(model) first')
+        if native is None and B > 1:
+            raise RuntimeError('forward_batch of several pairs needs the native stage drivers: call enable_native(model) first')
+        dev = data_dict['features'].device
+        if forced is not None:
+            forced = _forced_node_corr(forced, dev)
         marks = data_dict.get('_stage_events')            # profiling hook: list receiving (label, CUDA event) pairs
 
         def mark(label):
@@ -70,10 +85,8 @@ class GeoTransformer(nn.Module):
                 e.record()
                 marks.append((label, e))
         mark('start')
-        B = int(data_dict['batch_size'])
         lens_h = data_dict.get('lengths_host') or [l.tolist() for l in data_dict['lengths']]
         fl, K = self.fine_level, self.num_points_in_patch
-        dev = data_dict['features'].device
         offs = []
         for lv in lens_h:
             o = [0]
@@ -124,7 +137,8 @@ class GeoTransformer(nn.Module):
                 gt = GF.node_correspondences_batched(points_c, all_pts, node_masks, knn_masks, cn, transforms, self.matching_radius)
 
         # ---- backbone over all pairs (main stream, overlaps the grouping)
-        feats_list = native.backbone_forward(data_dict['features'], data_dict)
+        feats = data_dict['features']
+        feats_list = native.backbone_forward(feats, data_dict) if native is not None else self.backbone(feats, data_dict)
         feats_c, feats_f = feats_list[-1], feats_list[0]
         mark('backbone')
 
@@ -148,7 +162,10 @@ class GeoTransformer(nn.Module):
         embs = [E_all[eo[c]:eo[c + 1]] for c in range(2 * B)]
         mark('structure_embedding')
         x = GF.linear(feats_c, tr.in_proj.weight, tr.in_proj.bias)
-        x = native.transformer_forward_batched(x, rows_c, embs)
+        if native is not None:
+            x = native.transformer_forward_batched(x, rows_c, embs)
+        else:
+            x = tr.transformer.forward_stacked(x, rows_c[0], embs[0], embs[1])
         y = GF.linear(x, tr.out_proj.weight, tr.out_proj.bias)
         y_n = GF.l2_normalize(y)
         mark('transformer')
@@ -157,19 +174,27 @@ class GeoTransformer(nn.Module):
         join()
         mark('join_grouping+gt')
         cm, fm = self.coarse_matching, self.fine_matching
-        kc = cm.num_correspondences
-        corr, node_scores, corr_count = GF.superpoint_matching_batched(y_n, node_masks, cn, kc, cm.dual_normalization)
+        if forced is None:
+            kc = cm.num_correspondences
+            corr, node_scores, corr_count = GF.superpoint_matching_batched(y_n, node_masks, cn, kc, cm.dual_normalization)
+        else:
+            corr, node_scores = forced
+            kc = corr.shape[1]
+            corr_count = torch.full((1,), kc, dtype=torch.int32, device=dev)
         k_idx, k_masks, k_pts = GF.gather_patches_batched(corr, kc, cn, cf, knn_idx, knn_masks, points_f)
         r, s = slice(0, B * kc), slice(B * kc, 2 * B * kc)          # patches of the ref clouds, then of the src clouds
-        scores = GF.patch_scores_batched(feats_f, cf, k_idx[r], k_idx[s])
-        scores = self.optimal_transport(scores, k_masks[r], k_masks[s])
+        raw_scores = GF.patch_scores_batched(feats_f, cf, k_idx[r], k_idx[s])
+        scores = self.optimal_transport(raw_scores, k_masks[r], k_masks[s])
         rc, sc, cs, T, n_corr = GF.local_global_registration_batched(
             B, k_pts[r], k_pts[s], k_masks[r], k_masks[s], scores, fm.k, fm.acceptance_radius, fm.mutual, fm.confidence_threshold,
             fm.correspondence_threshold, fm.num_refinement_steps, transform_out=results if no_sync else None)
-        if gt is not None and evaluator is not None and no_sync:
-            GF.evaluate_batched(gt[0], gt[1], gt[2], corr, corr_count, rc, sc, n_corr, transforms, results, points0,
-                                cn, [int(v) for v in lens_h[0]], evaluator.mode, evaluator.acceptance_overlap, evaluator.acceptance_radius,
-                                results[:, 16:], evaluator.acceptance_rmse, evaluator.acceptance_rre, evaluator.acceptance_rte)
+        if no_sync:
+            if gt is not None and evaluator is not None:
+                GF.evaluate_batched(gt[0], gt[1], gt[2], corr, corr_count, rc, sc, n_corr, transforms, results, points0,
+                                    cn, [int(v) for v in lens_h[0]], evaluator.mode, evaluator.acceptance_overlap, evaluator.acceptance_radius,
+                                    results[:, 16:], evaluator.acceptance_rmse, evaluator.acceptance_rre, evaluator.acceptance_rte)
+            else:
+                results[:, 22].copy_(n_corr)          # the metrics' #corr column
         if ransac is not None and ransac_out is not None:
             write_ransac_rows(ransac, sc, rc, n_corr, ransac_out)
             if gt is not None and evaluator is not None:
@@ -179,8 +204,15 @@ class GeoTransformer(nn.Module):
         if gt is not None and loss_func is not None and loss_out is not None:
             loss_func.write_batched(y_n, cn, gt, k_pts[r], k_pts[s], k_masks[r], k_masks[s], scores, transforms, corr_count, loss_out)
         mark('matching+sinkhorn+lgr+metrics')
-        if no_sync and not keep_outputs:
-            return None
+        if taps is not None:
+            nr = cn[0]
+            taps.update(ref_node_masks=node_masks[:nr], src_node_masks=node_masks[nr:], ref_node_knn_indices=knn_idx[:nr],
+                        src_node_knn_indices=knn_idx[nr:], ref_node_knn_masks=knn_masks[:nr], src_node_knn_masks=knn_masks[nr:],
+                        feats_c=feats_c, feats_f=feats_f, matching_scores_raw=raw_scores)
+        if no_sync:
+            if not keep_outputs:
+                return None
+            T = T[:, :16].clone()          # the output dicts outlive the caller's reuse of its result rows
         outs = []
         g0 = 0
         for p in range(B):
@@ -200,116 +232,14 @@ class GeoTransformer(nn.Module):
             outs.append(o)
         if no_sync:
             return outs
-        # trim the capacity tensors to the counts (one host sync for the whole batch)
         main.synchronize()
-        for o in outs:
-            cnt = o.pop('_counts')
-            kk, c = int(cnt['node_corr'].item()), int(cnt['corr'].item())
-            for key in ('ref_node_corr_indices', 'src_node_corr_indices', 'node_corr_scores', 'ref_node_corr_knn_points',
-                        'src_node_corr_knn_points', 'ref_node_corr_knn_masks', 'src_node_corr_knn_masks', 'matching_scores'):
-                o[key] = o[key][:kk]
-            for key in ('ref_corr_points', 'src_corr_points', 'corr_scores'):
-                o[key] = o[key][:c]
-            if cnt['gt'] is not None:
-                g = int(cnt['gt'].item())
-                o['gt_node_corr_indices'], o['gt_node_corr_overlaps'] = o['gt_node_corr_indices'][:g], o['gt_node_corr_overlaps'][:g]
-        return outs
+        return trim_outputs(outs)
 
-    @torch.no_grad()
     def forward(self, data_dict, taps=None):
-        if int(data_dict.get('batch_size', 1)) > 1:
-            return self.forward_batch(data_dict)
-        out = {}
-        marks = data_dict.get('_stage_events')            # profiling hook: list receiving (label, CUDA event) pairs
-        def mark(label):
-            if marks is not None:
-                e = torch.cuda.Event(enable_timing=True)
-                e.record()
-                marks.append((label, e))
-        mark('start')
-        feats = data_dict['features']
-        lens = data_dict['lengths']
-        fl = self.fine_level
-        # lengths are needed on the host to slice ref/src (the reference does three .item() syncs, model.py:76-78);
-        # the collate keeps host copies so no sync happens here
-        lens_h = data_dict.get('lengths_host')
-        if lens_h is None:
-            lens_h = [l.tolist() for l in lens]
-        nc, nf, n0 = int(lens_h[-1][0]), int(lens_h[fl][0]), int(lens_h[0][0])
-        points_c, points_f, points = data_dict['points'][-1], data_dict['points'][fl], data_dict['points'][0]
-        ref_c, src_c = points_c[:nc], points_c[nc:]
-        ref_f, src_f = points_f[:nf], points_f[nf:]
-        out.update(ref_points_c=ref_c, src_points_c=src_c, ref_points_f=ref_f, src_points_f=src_f,
-                   ref_points=points[:n0], src_points=points[n0:])
-
-        K = self.num_points_in_patch
-        _, ref_node_masks, ref_knn_idx, ref_knn_masks = GF.point_to_node_partition(ref_f, ref_c, K)
-        _, src_node_masks, src_knn_idx, src_knn_masks = GF.point_to_node_partition(src_f, src_c, K)
-        if taps is not None:
-            taps.update(ref_node_masks=ref_node_masks, src_node_masks=src_node_masks, ref_node_knn_indices=ref_knn_idx,
-                        src_node_knn_indices=src_knn_idx, ref_node_knn_masks=ref_knn_masks, src_node_knn_masks=src_knn_masks)
-
-        # ground-truth superpoint correspondences (reference model.py:106-126).  Launched here, read back after the last
-        # host sync of the forward so that it costs no extra synchronisation.
-        gt_pending = None
-        transform = data_dict.get('transform')
-        if transform is not None:
-            ar_r = GF.scratch_arange(ref_c.shape[0], ref_c.device, 'ar_ref')
-            ar_s = GF.scratch_arange(src_c.shape[0], src_c.device, 'ar_src')
-            _, _, ref_all_pts = GF.gather_patches(ar_r, ref_knn_idx, ref_knn_masks, ref_f)
-            _, _, src_all_pts = GF.gather_patches(ar_s, src_knn_idx, src_knn_masks, src_f)
-            gt_pending = GF.node_correspondences(ref_c, src_c, ref_all_pts, src_all_pts, transform, self.matching_radius,
-                                                 ref_node_masks, src_node_masks, ref_knn_masks, src_knn_masks)
-
-        mark('partition+gt')
-        native = getattr(self, '_native', None)          # NativeModel: backbone / transformer as one C call each
-        feats_list = native.backbone_forward(feats, data_dict) if native is not None else self.backbone(feats, data_dict)
-        feats_c, feats_f = feats_list[-1], feats_list[0]
-        mark('backbone')
-        if taps is not None:
-            taps['feats_c'], taps['feats_f'] = feats_c, feats_f
-
-        ref_fc, src_fc = self.transformer(ref_c, src_c, feats_c[:nc], feats_c[nc:], native=native)
-        mark('transformer')
-        ref_fc_n, src_fc_n = GF.l2_normalize(ref_fc), GF.l2_normalize(src_fc)
-        ref_ff, src_ff = feats_f[:nf], feats_f[nf:]
-        out.update(ref_feats_c=ref_fc_n, src_feats_c=src_fc_n, ref_feats_f=ref_ff, src_feats_f=src_ff)
-
-        # fewer than num_correspondences rows exist only when #valid ref x #valid src superpoints is smaller (tiny clouds):
-        # the count stays on the device, the padding rows become empty patches (no fine correspondences, so LGR is
-        # unaffected) and the per-patch outputs are trimmed after the forward's last host sync
-        ref_corr, src_corr, node_scores, corr_count = self.coarse_matching(ref_fc_n, src_fc_n, ref_node_masks, src_node_masks,
-                                                                           defer_count=True)
-        forced = data_dict.get('forced_node_corr')       # test hook: teacher-forced coarse correspondences
-        if forced is not None:
-            ref_corr, src_corr, node_scores = forced
-            corr_count = None
-        out.update(ref_node_corr_indices=ref_corr, src_node_corr_indices=src_corr, node_corr_scores=node_scores)
-
-        rk_idx, rk_masks, rk_pts = GF.gather_patches(ref_corr, ref_knn_idx, ref_knn_masks, ref_f)
-        sk_idx, sk_masks, sk_pts = GF.gather_patches(src_corr, src_knn_idx, src_knn_masks, src_f)
-        out.update(ref_node_corr_knn_points=rk_pts, src_node_corr_knn_points=sk_pts, ref_node_corr_knn_masks=rk_masks,
-                   src_node_corr_knn_masks=sk_masks)
-
-        scores = GF.patch_scores(ref_ff, src_ff, rk_idx, sk_idx)
-        if taps is not None:
-            taps['matching_scores_raw'] = scores
-        scores = self.optimal_transport(scores, rk_masks, sk_masks)
-        out['matching_scores'] = scores
-        mark('matching+sinkhorn')
-
-        rc, sc, cs, T = self.fine_matching(rk_pts, sk_pts, rk_masks, sk_masks, scores, node_scores)
-        out.update(ref_corr_points=rc, src_corr_points=sc, corr_scores=cs, estimated_transform=T)
-        mark('lgr')
-        if gt_pending is not None:
-            out['gt_node_corr_indices'], out['gt_node_corr_overlaps'] = GF.finish_node_correspondences(*gt_pending)
-        if corr_count is not None:
-            kk = int(corr_count.item())          # already complete: LGR synchronised the stream
-            if kk < ref_corr.shape[0]:
-                for key in ('ref_node_corr_indices', 'src_node_corr_indices', 'node_corr_scores', 'ref_node_corr_knn_points',
-                            'src_node_corr_knn_points', 'ref_node_corr_knn_masks', 'src_node_corr_knn_masks', 'matching_scores'):
-                    out[key] = out[key][:kk]
-        return out
+        """``forward_batch`` with its defaults: the output dict of a single pair (the reference's contract), the list of output
+        dicts for a batch of several pairs.  ``taps`` and ``data_dict['forced_node_corr']``: see ``forward_batch``."""
+        outs = self.forward_batch(data_dict, taps=taps)
+        return outs[0] if int(data_dict.get('batch_size', 1)) == 1 else outs
 
 
 def enable_native(model):
@@ -332,12 +262,42 @@ def create_model(cfg):
     return GeoTransformer(cfg)
 
 
-def write_ransac_rows(ransac, src_corr_points, ref_corr_points, num_corr, out, first_pair=0):
+def _forced_node_corr(forced, device):
+    """teacher-forced coarse correspondences (ref indices (k',), src indices (k',), scores (k',)) -> the superpoint matching's
+    layout for one pair: corr (2, k') int64, scores (1, k') float32"""
+    ref, src, scores = forced
+    for t, dtype, name in ((ref, torch.int64, 'ref indices'), (src, torch.int64, 'src indices'), (scores, torch.float32, 'scores')):
+        if t.ndim != 1 or t.dtype != dtype or t.device != device:
+            raise ValueError(f'forced_node_corr: the {name} must be a 1-D {dtype} tensor on {device}')
+    if not ref.shape[0] == src.shape[0] == scores.shape[0]:
+        raise ValueError('forced_node_corr: the ref indices, src indices and scores must have the same length')
+    return torch.stack([ref, src]), scores.reshape(1, -1)
+
+
+def trim_outputs(outs):
+    """Cut the per-pair output dicts of ``forward_batch(results=...)`` to their device counts and drop ``_counts`` (in place;
+    returns ``outs``).  The rows past a count are uninitialised, so call it only after the forward's stream has been
+    synchronised."""
+    for o in outs:
+        cnt = o.pop('_counts')
+        kk, c = int(cnt['node_corr'].item()), int(cnt['corr'].item())
+        for key in ('ref_node_corr_indices', 'src_node_corr_indices', 'node_corr_scores', 'ref_node_corr_knn_points',
+                    'src_node_corr_knn_points', 'ref_node_corr_knn_masks', 'src_node_corr_knn_masks', 'matching_scores'):
+            o[key] = o[key][:kk]
+        for key in ('ref_corr_points', 'src_corr_points', 'corr_scores'):
+            o[key] = o[key][:c]
+        if cnt['gt'] is not None:
+            g = int(cnt['gt'].item())
+            o['gt_node_corr_indices'], o['gt_node_corr_overlaps'] = o['gt_node_corr_indices'][:g], o['gt_node_corr_overlaps'][:g]
+    return outs
+
+
+def write_ransac_rows(ransac, src_corr_points, ref_corr_points, num_corr, out):
     """Correspondence RANSAC (``ransac``: distance_threshold, num_points, num_iterations, seed) of B pairs of (B, capacity, 3)
     correspondences (``num_corr``: (B,) device int32 or None) into columns 0..17 of the (B, >= 18) float rows ``out``:
-    [transform (16), fitness, inlier_rmse].  No host synchronisation."""
+    [transform (16), fitness, inlier_rmse]; pair p draws from the stream (seed, p).  No host synchronisation."""
     rr = GF.ransac_correspondences_batched(src_corr_points, ref_corr_points, ransac.distance_threshold, ransac.num_points,
-                                           ransac.num_iterations, seed=ransac.get('seed', 0), num_corr=num_corr, first_pair=first_pair)
+                                           ransac.num_iterations, seed=ransac.get('seed', 0), num_corr=num_corr)
     B = out.shape[0]
     out[:, :16].copy_(rr['transform'].reshape(B, 16))
     out[:, 16].copy_(rr['fitness'])

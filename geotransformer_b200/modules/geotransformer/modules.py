@@ -86,7 +86,7 @@ class GeometricTransformer(nn.Module):
                                                      activation_fn=activation_fn)
         self.out_proj = nn.Linear(hidden_dim, output_dim)
 
-    def forward(self, ref_points, src_points, ref_feats, src_feats, ref_masks=None, src_masks=None, native=None):
+    def forward(self, ref_points, src_points, ref_feats, src_feats, ref_masks=None, src_masks=None):
         if ref_masks is not None or src_masks is not None:
             raise NotImplementedError('masks are None on the inference path (EXP*/model.py:135-140)')
         batched = ref_points.ndim == 3
@@ -99,10 +99,7 @@ class GeometricTransformer(nn.Module):
         x = torch.empty((n0 + n1, self.in_proj.out_features), dtype=torch.float32, device=ref_feats.device)
         GF.linear(ref_feats, self.in_proj.weight, self.in_proj.bias, out=x[:n0])
         GF.linear(src_feats, self.in_proj.weight, self.in_proj.bias, out=x[n0:])
-        if native is not None:
-            x = native.transformer_forward_batched(x, [n0, n1], [ref_emb, src_emb])
-        else:
-            x = self.transformer.forward_stacked(x, n0, ref_emb, src_emb)
+        x = self.transformer.forward_stacked(x, n0, ref_emb, src_emb)
         y = GF.linear(x, self.out_proj.weight, self.out_proj.bias)
         rf, sf = y[:n0], y[n0:]
         if batched:
@@ -117,9 +114,9 @@ class SuperPointMatching(nn.Module):
         super().__init__()
         self.num_correspondences, self.dual_normalization = num_correspondences, dual_normalization
 
-    def forward(self, ref_feats, src_feats, ref_masks=None, src_masks=None, defer_count=False):
+    def forward(self, ref_feats, src_feats, ref_masks=None, src_masks=None):
         return GF.superpoint_matching(ref_feats, src_feats, ref_masks, src_masks, self.num_correspondences,
-                                      self.dual_normalization, defer_count=defer_count)
+                                      self.dual_normalization)
 
 
 class LocalGlobalRegistration(nn.Module):

@@ -155,8 +155,50 @@ def test_forward_batch_equals_single_pair_forward(workload, cfg_name, ids, model
                 assert rre < 0.05 and rte < 1e-3 * scale, f'pair {p}: transforms differ by {rre:.4f} deg / {rte:.5f}'
 
 
+ONE_PAIR_KEYS = {'ref_points_c', 'src_points_c', 'ref_points_f', 'src_points_f', 'ref_points', 'src_points', 'ref_feats_c', 'src_feats_c',
+                 'ref_feats_f', 'src_feats_f', 'ref_node_corr_indices', 'src_node_corr_indices', 'node_corr_scores',
+                 'ref_node_corr_knn_points', 'src_node_corr_knn_points', 'ref_node_corr_knn_masks', 'src_node_corr_knn_masks',
+                 'matching_scores', 'ref_corr_points', 'src_corr_points', 'corr_scores', 'estimated_transform', 'gt_node_corr_indices',
+                 'gt_node_corr_overlaps'}
+
+
+@pytest.mark.parametrize('n_points', [None, 150])
+@pytest.mark.parametrize('native', [False, True])
+def test_one_pair_output_contract(n_points, native, models):
+    """model(data) of one pair: the reference's key set, every tensor trimmed to its count (no '_counts', no padding row), also for a
+    pair with fewer valid superpoint pairs than num_correspondences (the 150 points of each demo2k cloud nearest to its first point:
+    8 x 9 superpoints)"""
+    from geotransformer_b200.loss import Evaluator
+    cfg, sd, model = models('3dmatch')
+    model = model.cuda().eval()
+    if native:
+        enable_native(model)
+    elif hasattr(model, '_native'):
+        del model._native
+    d = _pairs('demo2k', [0])[0]
+    if n_points is not None:
+        for side in ('ref', 'src'):
+            pts = d[side + '_points']
+            keep = np.argsort(((pts - pts[0]) ** 2).sum(1), kind='stable')[:n_points]
+            d[side + '_points'], d[side + '_feats'] = pts[keep], d[side + '_feats'][keep]
+    data = _collate([d], cfg, cfg.neighbor_limits)
+    out = model(data)
+    assert set(out) == ONE_PAIR_KEYS
+    kk = out['ref_node_corr_indices'].shape[0]
+    if n_points is not None:
+        assert kk < cfg.coarse_matching.num_correspondences
+    for k in ('src_node_corr_indices', 'node_corr_scores', 'ref_node_corr_knn_points', 'src_node_corr_knn_points', 'ref_node_corr_knn_masks',
+              'src_node_corr_knn_masks', 'matching_scores'):
+        assert out[k].shape[0] == kk, k
+    assert int(out['ref_node_corr_indices'].min()) >= 0 and int(out['src_node_corr_indices'].min()) >= 0
+    n_corr = int(Evaluator(cfg).metrics_tensor(out, data)[6].item())
+    for k in ('ref_corr_points', 'src_corr_points', 'corr_scores'):
+        assert out[k].shape[0] == n_corr, k
+
+
 def test_engine_batch_mode_matches_stream_mode(models):
-    """RegistrationEngine(batch_size=B): same transforms and metrics as one pair per forward"""
+    """RegistrationEngine(batch_size=B): same transforms and metrics as one pair per forward; at batch_size 1 the engine's output
+    dicts are model(data)'s, bit for bit"""
     from geotransformer_b200.engine import RegistrationEngine
     from geotransformer_b200.loss import Evaluator
     cfg, sd, model = models('3dmatch')
@@ -164,8 +206,18 @@ def test_engine_batch_mode_matches_stream_mode(models):
     pairs = _pairs('demo2k', range(7))
     ev = Evaluator(cfg)
     one = RegistrationEngine(model, cfg, cfg.neighbor_limits, num_streams=2, evaluator=ev)
-    want = one.register(pairs)
+    want = one.register(pairs, keep_outputs=True)
     one.close()
+    torch.cuda.synchronize()
+    for p, (d, r) in enumerate(zip(pairs, want)):
+        out = model(_collate([d], cfg, cfg.neighbor_limits))
+        assert set(r['output_dict']) == set(out), p
+        for k, v in out.items():
+            a = r['output_dict'][k]
+            if v.dtype == torch.float32:          # bit for bit, NaN included
+                a, v = a.view(torch.int32), v.view(torch.int32)
+            assert torch.equal(a, v), (p, k)
+        assert r['num_corr'] == out['ref_corr_points'].shape[0]
     eng = RegistrationEngine(model, cfg, cfg.neighbor_limits, num_streams=2, evaluator=ev, batch_size=3, side_streams=3)
     got = eng.register(pairs)            # 7 pairs = 3 + 3 + 1: also covers the trailing single pair
     eng.close()

@@ -95,6 +95,18 @@ def test_forward_batch_needs_the_native_drivers(models):
         model.forward_batch({'batch_size': 2})
 
 
+def test_forward_batch_test_hooks_are_for_one_pair(models):
+    """taps and forced coarse correspondences describe one pair: a batch of two is refused before anything touches the device"""
+    cfg, sd, model = models('3dmatch')
+    if hasattr(model, '_native'):
+        del model._native
+    with pytest.raises(ValueError, match='one pair'):
+        model.forward_batch({'batch_size': 2}, taps={})
+    forced = (torch.zeros(4, dtype=torch.int64), torch.zeros(4, dtype=torch.int64), torch.zeros(4))
+    with pytest.raises(ValueError, match='one pair'):
+        model.forward_batch({'batch_size': 2, 'forced_node_corr': forced})
+
+
 def test_unsupported_module_options_are_rejected():
     from geotransformer_b200.modules.geotransformer import LocalGlobalRegistration, GeometricStructureEmbedding
     with pytest.raises(NotImplementedError):
