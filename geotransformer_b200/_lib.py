@@ -51,6 +51,16 @@ _sig('geob200_group_norm_batched', c_int, P, I64, I64, I64, P, P, F, P, c_int, F
 _sig('geob200_linear_group_norm_batched', c_int, P, I64, P, P, I64, I64, I64, I64, P, P, F, P, c_int, F, P, P, P, SZ, P, I64, P)
 _sig('geob200_maxpool', c_int, P, P, I64, I64, I64, I64, P, P)
 _sig('geob200_upsample_concat', c_int, P, P, I64, I64, P, I64, I64, I64, P, P)
+_sig('geob200_kpconv_backward_workspace_bytes', SZ, I64, I64, I64, I64, I64)
+_sig('geob200_kpconv_backward', c_int, P, P, P, P, I64, I64, I64, P, I64, P, I64, I64, F, P, P, P, P, P, SZ, P)
+_sig('geob200_linear_backward_workspace_bytes', SZ, I64, I64, I64, c_int)
+_sig('geob200_linear_backward', c_int, P, I64, P, P, I64, I64, I64, P, P, P, P, P, SZ, P)
+_sig('geob200_group_norm_backward_batched_workspace_bytes', SZ, I64, I64, I64, I64)
+_sig('geob200_group_norm_backward_batched', c_int, P, P, I64, I64, I64, P, F, c_int, F, P, P, P, P, P, P, SZ, P, I64, P)
+_sig('geob200_maxpool_backward_batched_workspace_bytes', SZ, I64, I64, I64, I64)
+_sig('geob200_maxpool_backward_batched', c_int, P, P, I64, I64, I64, I64, P, I64, P, P, P, P, SZ, P)
+_sig('geob200_upsample_concat_backward_workspace_bytes', SZ, I64, I64)
+_sig('geob200_upsample_concat_backward', c_int, P, I64, I64, I64, I64, I64, P, P, P, P, SZ, P)
 _sig('geob200_point_to_node_partition_batched', c_int, P, P, I64, P, P, I64, P, P, P, P, P, P)
 _sig('geob200_gather_rows', c_int, P, I64, I64, P, I64, P, P)
 _sig('geob200_knn_partition', c_int, P, I64, P, I64, I64, P, P, P)

@@ -12,24 +12,12 @@
 // Feature tables are L2-resident; the compulsory HBM traffic is the index table + the output.
 #include "common.cuh"
 #include "geob200.h"
+#include "kpconv.cuh"
 
 namespace geob200 {
 
-constexpr int KP = 15;        // kernel points of every shipped model (config.py: backbone.kernel_size)
-constexpr int KP_PAD = 16;
 constexpr int TQ = 32;        // queries per CTA
 constexpr int CC = 32;        // input-channel chunk staged in shared memory (one float per lane per neighbour row)
-
-__device__ __forceinline__ void influence15(const float* __restrict__ kp_s, float rx, float ry, float rz, float inv_dummy,
-                                            float sigma, float* w) {
-#pragma unroll
-    for (int k = 0; k < KP; ++k) {
-        const float dx = rx - kp_s[3 * k], dy = ry - kp_s[3 * k + 1], dz = rz - kp_s[3 * k + 2];
-        const float sq = __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
-        w[k] = fmaxf(1.0f - sqrtf(sq) / sigma, 0.0f);      // kpconv.py:96-99
-    }
-    (void)inv_dummy;
-}
 
 // First layer of every backbone: Cin == 1 (features are all-ones columns, model input_dim = 1).
 // out[m][c'] = (sum_k (sum_h w[h][k] f[h]) W[k][0][c']) / max(#{h: f[h] > 0}, 1) + bias
@@ -196,6 +184,15 @@ static void launch_kpconv_gather(const float* s_feats, const unsigned char* pos,
     else
         kpconv_gather_kernel<1><<<grid, 256, 0, st>>>(s_feats, pos, q_points, s_points, neighbors, n_neighbors, kernel_points, sigma,
                                                      n_support, n_query, c_in, wf, inv_count);
+}
+
+void kpconv_gather(const float* s_feats, const float* q_points, const float* s_points, const long long* neighbors, int n_neighbors,
+                   const float* kernel_points, float sigma, int n_support, int n_query, int c_in, unsigned char* pos, float* wf,
+                   float* inv_count, cudaStream_t st) {
+    row_positive_kernel<<<(unsigned)((n_support + 7) / 8), 256, 0, st>>>(s_feats, n_support, c_in, pos);
+    launch_kpconv_gather(s_feats, pos, q_points, s_points, neighbors, n_neighbors, kernel_points, sigma, n_support, n_query, c_in, wf,
+                         inv_count, st);
+    count_launches(2);
 }
 
 // General KPConv, Cin % 32 == 0 and Cout % 32 == 0 (mid channels 32..512 of the bottleneck blocks).
@@ -1272,11 +1269,15 @@ int kpconv_group_norm_impl(const float* s_feats, const float* q_points, const fl
 }  // namespace geob200
 
 namespace geob200 {
-static int make_seg(GnSeg* g, int64_t n_pairs, const int64_t* cloud_rows_h, int64_t n_rows) {
-    GEOB_REQUIRE(n_pairs >= 1 && 2 * n_pairs <= GEOB_MAX_CLOUDS && cloud_rows_h != nullptr, "group_norm: 1 <= pairs per batch <= %d", GEOB_MAX_CLOUDS / 2);
+int make_seg(GnSeg* g, int64_t n_pairs, const int64_t* cloud_rows_h, int64_t n_rows, const char* what) {
+    GEOB_REQUIRE(n_pairs >= 1 && 2 * n_pairs <= GEOB_MAX_CLOUDS && cloud_rows_h != nullptr, "%s: 1 <= pairs per batch <= %d", what,
+                 GEOB_MAX_CLOUDS / 2);
     g->n_pairs = (int)n_pairs; g->n_clouds = (int)(2 * n_pairs); g->start[0] = 0;
-    for (int c = 0; c < g->n_clouds; ++c) g->start[c + 1] = g->start[c] + (int)cloud_rows_h[c];
-    GEOB_REQUIRE(g->start[g->n_clouds] == n_rows, "group_norm: cloud rows do not add up to n_rows");
+    for (int c = 0; c < g->n_clouds; ++c) {
+        GEOB_REQUIRE(cloud_rows_h[c] >= 0, "%s: negative cloud row count", what);
+        g->start[c + 1] = g->start[c] + (int)cloud_rows_h[c];
+    }
+    GEOB_REQUIRE(g->start[g->n_clouds] == n_rows, "%s: cloud rows do not add up to n_rows", what);
     return 0;
 }
 }  // namespace geob200
@@ -1287,7 +1288,7 @@ int geob200_group_norm_batched(const float* x, int64_t n_rows, int64_t channels,
                                float eps, const float* residual, int leaky, float slope, float* y, void* workspace, size_t workspace_bytes,
                                void* stream, int64_t n_pairs, const int64_t* cloud_rows_h) {
     geob200::GnSeg seg;
-    if (geob200::make_seg(&seg, n_pairs, cloud_rows_h, n_rows)) return -2;
+    if (geob200::make_seg(&seg, n_pairs, cloud_rows_h, n_rows, "group_norm")) return -2;
     return geob200::group_norm_impl(x, n_rows, channels, groups, gamma, beta, eps, residual, leaky, slope, y, workspace, workspace_bytes,
                                     stream, &seg);
 }
@@ -1297,7 +1298,7 @@ int geob200_linear_group_norm_batched(const float* x, int64_t ldx, const float* 
                                       float slope, float* pre_norm, float* y, void* workspace, size_t workspace_bytes, void* stream,
                                       int64_t n_pairs, const int64_t* cloud_rows_h) {
     geob200::GnSeg seg;
-    if (geob200::make_seg(&seg, n_pairs, cloud_rows_h, m)) return -2;
+    if (geob200::make_seg(&seg, n_pairs, cloud_rows_h, m, "group_norm")) return -2;
     return geob200::linear_group_norm_impl(x, ldx, weight, bias, m, n, k, groups, gamma, beta, eps, residual, leaky, slope, pre_norm, y,
                                            workspace, workspace_bytes, stream, &seg);
 }
@@ -1306,7 +1307,7 @@ int geob200_linear_group_norm_batched(const float* x, int64_t ldx, const float* 
 int geob200_cloud_max_count(const int64_t* neighbors, int64_t n_query, int64_t n_support, int64_t n_neighbors, int64_t n_pairs,
                             const int64_t* cloud_rows_h, int32_t* cloud_max, void* stream) {
     geob200::GnSeg seg;
-    if (geob200::make_seg(&seg, n_pairs, cloud_rows_h, n_query)) return -2;
+    if (geob200::make_seg(&seg, n_pairs, cloud_rows_h, n_query, "group_norm")) return -2;
     geob200::cloud_max_count_kernel<<<seg.n_clouds, 256, 0, (cudaStream_t)stream>>>((const long long*)neighbors, (int)n_neighbors,
                                                                                    (int)n_support, seg, cloud_max);
     GEOB_CHECK_LAUNCH();

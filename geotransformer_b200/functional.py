@@ -86,7 +86,14 @@ KPCONV_MODE = 'tc'
 
 
 def kpconv(s_feats, q_points, s_points, neighbor_indices, kernel_points, weights, bias, sigma, weights_t=None):
-    """weights_t: optional cached (c_out, 15*c_in) transpose of the weights for the tensor-core path"""
+    """weights_t: optional cached (c_out, 15*c_in) transpose of the weights for the tensor-core path.  Differentiable w.r.t.
+    ``s_feats``, ``weights`` and ``bias`` (``kpconv_backward``)."""
+    if _needs_grad(s_feats, weights, bias):
+        return _KPConv.apply(s_feats, weights, bias, q_points, s_points, neighbor_indices, kernel_points, float(sigma), weights_t)
+    return _kpconv(s_feats, q_points, s_points, neighbor_indices, kernel_points, weights, bias, sigma, weights_t)
+
+
+def _kpconv(s_feats, q_points, s_points, neighbor_indices, kernel_points, weights, bias, sigma, weights_t=None):
     s_feats, weights, bias = _detach(s_feats), _detach(weights), _detach(bias)
     _f(s_feats, 's_feats'); _f(q_points, 'q_points'); _f(s_points, 's_points')
     L.require_cuda(neighbor_indices, 'neighbor_indices', _i64)
@@ -111,8 +118,58 @@ def kpconv(s_feats, q_points, s_points, neighbor_indices, kernel_points, weights
     return out
 
 
+def kpconv_backward(s_feats, q_points, s_points, neighbor_indices, kernel_points, weights, sigma, grad_out, need_feats=True,
+                    need_weights=True, need_bias=True):
+    """(grad_s_feats, grad_weights, grad_bias) of ``kpconv`` for the upstream gradient ``grad_out`` (n_query, c_out); the neighbour
+    count n_valid is the forward's, a constant.  A gradient not requested is None."""
+    for t, name in ((s_feats, 's_feats'), (q_points, 'q_points'), (s_points, 's_points'), (kernel_points, 'kernel_points'),
+                    (weights, 'weights'), (grad_out, 'grad_out')):
+        _f(_detach(t), name)
+    L.require_cuda(neighbor_indices, 'neighbor_indices', _i64)
+    s_feats, weights = _detach(s_feats), _detach(weights)
+    m, h = neighbor_indices.shape
+    ns = s_points.shape[0]
+    k, cin, cout = weights.shape
+    if tuple(grad_out.shape) != (m, cout) or tuple(s_feats.shape) != (ns, cin):
+        raise RuntimeError(f'kpconv_backward: grad_out must be ({m}, {cout}) and s_feats ({ns}, {cin})')
+    dev = s_feats.device
+    gf = torch.empty((ns, cin), dtype=_f32, device=dev) if need_feats else None
+    gw = torch.empty((k, cin, cout), dtype=_f32, device=dev) if need_weights else None
+    gb = torch.empty((cout,), dtype=_f32, device=dev) if need_bias else None
+    lib = L.lib()
+    ws = L.workspace(lib.geob200_kpconv_backward_workspace_bytes(m, ns, h, cin, cout), dev, 'kpconv_backward')
+    L.check(lib.geob200_kpconv_backward(s_feats.data_ptr(), q_points.data_ptr(), s_points.data_ptr(), neighbor_indices.data_ptr(), m, ns, h,
+                                        kernel_points.data_ptr(), k, weights.data_ptr(), cin, cout, float(sigma), grad_out.data_ptr(),
+                                        L.ptr(gf), L.ptr(gw), L.ptr(gb), ws.data_ptr(), ws.numel(), L.stream_ptr()), 'kpconv_backward')
+    return gf, gw, gb
+
+
+class _KPConv(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, s_feats, weights, bias, q_points, s_points, neighbor_indices, kernel_points, sigma, weights_t):
+        ctx.save_for_backward(s_feats, weights, q_points, s_points, neighbor_indices, kernel_points)
+        ctx.sigma = sigma
+        return _kpconv(s_feats, q_points, s_points, neighbor_indices, kernel_points, weights, bias, sigma, weights_t)
+
+    @staticmethod
+    def backward(ctx, grad):
+        s_feats, weights, q, s, nbr, kp = ctx.saved_tensors
+        nf, nw, nb = ctx.needs_input_grad[:3]
+        gf, gw, gb = kpconv_backward(s_feats, q, s, nbr, kp, weights, ctx.sigma, grad.contiguous(), nf, nw, nb)
+        return gf, gw, gb, None, None, None, None, None, None
+
+
 def linear(x, weight, bias=None, relu=False, out=None):
-    """y = x @ weight.T + bias; x may be a column slice of a wider row-major tensor (stride(1) == 1)."""
+    """y = x @ weight.T + bias (ReLU'd with ``relu``); x may be a column slice of a wider row-major tensor (stride(1) == 1).
+    Differentiable w.r.t. ``x``, ``weight`` and ``bias`` (``linear_backward``); with ``out`` the result is copied into it, which
+    then carries the graph."""
+    if _needs_grad(x, weight, bias):
+        y = _Linear.apply(x, weight, bias, bool(relu))
+        return y if out is None else out.copy_(y)
+    return _linear(x, weight, bias, relu, out)
+
+
+def _linear(x, weight, bias=None, relu=False, out=None):
     x, weight, bias = _detach(x), _detach(weight), _detach(bias)
     if not x.is_cuda or x.dtype != _f32 or x.stride(1) != 1:
         raise RuntimeError('linear: x must be a float32 CUDA tensor with unit inner stride')
@@ -124,6 +181,48 @@ def linear(x, weight, bias=None, relu=False, out=None):
     L.check(L.lib().geob200_linear(x.data_ptr(), x.stride(0), weight.data_ptr(), L.ptr(bias), out.data_ptr(),
                                    out.stride(0), m, n, k, int(relu), L.stream_ptr()), 'linear')
     return out
+
+
+def linear_backward(x, weight, grad_y, need_x=True, need_weight=True, need_bias=True, relu_y=None):
+    """(grad_x (m, k), grad_weight (n, k), grad_bias (n,)) of ``linear`` for the upstream gradient ``grad_y`` (m, n); x may be a column
+    slice; ``relu_y``: the forward's output when it applied the ReLU.  grad_x runs through the forward's GEMM (3xTF32 on the tensor
+    cores where the shape allows), grad_weight / grad_bias are fp32 sums over the rows in a fixed order.  An output not requested is
+    None."""
+    x, weight = _detach(x), _detach(weight)
+    if not x.is_cuda or x.dtype != _f32 or x.stride(1) != 1:
+        raise RuntimeError('linear_backward: x must be a float32 CUDA tensor with unit inner stride')
+    L.require_cuda(weight, 'weight', _f32); _f(grad_y, 'grad_y')
+    m, k = x.shape
+    n = weight.shape[0]
+    if tuple(grad_y.shape) != (m, n) or weight.shape[1] != k:
+        raise RuntimeError(f'linear_backward: grad_y must be ({m}, {n}) and weight ({n}, {k})')
+    if relu_y is not None:
+        _f(relu_y, 'relu_y')
+        if tuple(relu_y.shape) != (m, n):
+            raise RuntimeError(f'linear_backward: relu_y must be ({m}, {n})')
+    dev = x.device
+    wt = weight.t().contiguous() if need_x else None
+    gx = torch.empty((m, k), dtype=_f32, device=dev) if need_x else None
+    gw = torch.empty((n, k), dtype=_f32, device=dev) if need_weight else None
+    gb = torch.empty((n,), dtype=_f32, device=dev) if need_bias else None
+    lib = L.lib()
+    ws = L.workspace(lib.geob200_linear_backward_workspace_bytes(m, n, k, int(relu_y is not None)), dev, 'linear_backward')
+    L.check(lib.geob200_linear_backward(x.data_ptr(), x.stride(0), L.ptr(wt), L.ptr(_detach(relu_y)), m, n, k, grad_y.data_ptr(), L.ptr(gx),
+                                        L.ptr(gw), L.ptr(gb), ws.data_ptr(), ws.numel(), L.stream_ptr()), 'linear_backward')
+    return gx, gw, gb
+
+
+class _Linear(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, weight, bias, relu):
+        y = _linear(x, weight, bias, relu)
+        ctx.save_for_backward(x, weight, y if relu else None)
+        return y
+
+    @staticmethod
+    def backward(ctx, grad):
+        x, weight, y = ctx.saved_tensors
+        return (*linear_backward(x, weight, grad.contiguous(), *ctx.needs_input_grad[:3], relu_y=y), None)
 
 
 def split_tf32(weight):
@@ -139,7 +238,60 @@ def split_tf32(weight):
 
 
 def group_norm(x, weight, bias, groups, eps=1e-5, negative_slope=None, residual=None):
-    x, weight, bias = _detach(x), _detach(weight), _detach(bias)
+    """leaky(GroupNorm(x) + residual) over all rows (one pair); differentiable w.r.t. x, weight, bias and residual"""
+    if _needs_grad(x, weight, bias, residual):
+        return _GroupNorm.apply(x, weight, bias, residual, int(groups), float(eps), negative_slope)
+    return _group_norm(x, weight, bias, groups, eps, negative_slope, residual)
+
+
+def group_norm_backward_batched(x, y, weight, groups, cloud_rows, grad_y, eps=1e-5, negative_slope=None, need_residual=False,
+                                need_weight=True, need_bias=True):
+    """(grad_x, grad_weight, grad_bias, grad_residual) of ``leaky(GroupNorm(x) + residual)`` with per-pair statistics (``cloud_rows``:
+    2B host ints, as ``group_norm_batched``; one pair: ``[n_rows, 0]``).  ``x`` is the pre-norm input and ``y`` the forward's output
+    (its sign gives the LeakyReLU's derivative).  The statistics are recomputed from x; every sum runs in a fixed order."""
+    x, y, weight = _detach(x), _detach(y), _detach(weight)
+    _f(x, 'x'); _f(weight, 'weight'); _f(grad_y, 'grad_y')
+    leaky = negative_slope is not None
+    if leaky:
+        _f(y, 'y')
+    n, c = x.shape
+    if tuple(grad_y.shape) != (n, c) or (leaky and tuple(y.shape) != (n, c)):
+        raise RuntimeError(f'group_norm_backward_batched: grad_y and y must be ({n}, {c})')
+    dev = x.device
+    np_ = len(cloud_rows) // 2
+    gx = torch.empty_like(x)
+    gw = torch.empty((c,), dtype=_f32, device=dev) if need_weight else None
+    gb = torch.empty((c,), dtype=_f32, device=dev) if need_bias else None
+    gr = torch.empty_like(x) if need_residual else None
+    lib = L.lib()
+    ws = L.workspace(lib.geob200_group_norm_backward_batched_workspace_bytes(n, c, groups, np_), dev, 'group_norm_backward')
+    L.check(lib.geob200_group_norm_backward_batched(x.data_ptr(), L.ptr(y) if leaky else None, n, c, groups, weight.data_ptr(), float(eps),
+                                                    int(leaky), float(negative_slope or 0.0), grad_y.data_ptr(), gx.data_ptr(), L.ptr(gw),
+                                                    L.ptr(gb), L.ptr(gr), ws.data_ptr(), ws.numel(), L.stream_ptr(), np_,
+                                                    _host_i64(cloud_rows)), 'group_norm_backward_batched')
+    return gx, gw, gb, gr
+
+
+class _GroupNorm(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, weight, bias, residual, groups, eps, negative_slope):
+        y = _group_norm(x, weight, bias, groups, eps, negative_slope, residual)
+        ctx.save_for_backward(x, y, weight)
+        ctx.args = (groups, eps, negative_slope)
+        return y
+
+    @staticmethod
+    def backward(ctx, grad):
+        x, y, weight = ctx.saved_tensors
+        groups, eps, slope = ctx.args
+        need = ctx.needs_input_grad
+        gx, gw, gb, gr = group_norm_backward_batched(x, y, weight, groups, [x.shape[0], 0], grad.contiguous(), eps, slope, need[3], need[1],
+                                                     need[2])
+        return gx if need[0] else None, gw, gb, gr, None, None, None
+
+
+def _group_norm(x, weight, bias, groups, eps=1e-5, negative_slope=None, residual=None):
+    x, weight, bias, residual = _detach(x), _detach(weight), _detach(bias), _detach(residual)
     _f(x, 'x')
     n, c = x.shape
     ws = _gn_workspace(x.device, groups)
@@ -152,14 +304,44 @@ def group_norm(x, weight, bias, groups, eps=1e-5, negative_slope=None, residual=
 
 
 def linear_group_norm(x, weight, bias, gn_weight, gn_bias, groups, eps=1e-5, negative_slope=None, residual=None):
-    """UnaryBlock: leaky(GroupNorm(x @ weight.T + bias) + residual); statistics from the GEMM epilogue on the wgmma path"""
+    """UnaryBlock: leaky(GroupNorm(x @ weight.T + bias) + residual); statistics from the GEMM epilogue on the wgmma path.
+    Differentiable w.r.t. every float input (the autograd path keeps its own copy of the pre-norm activation)."""
+    if _needs_grad(x, weight, bias, gn_weight, gn_bias, residual):
+        return _LinearGroupNorm.apply(x, weight, bias, gn_weight, gn_bias, residual, int(groups), float(eps), negative_slope)
+    return _linear_group_norm(x, weight, bias, gn_weight, gn_bias, groups, eps, negative_slope, residual)
+
+
+class _LinearGroupNorm(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, weight, bias, gn_weight, gn_bias, residual, groups, eps, negative_slope):
+        pre = torch.empty((x.shape[0], weight.shape[0]), dtype=_f32, device=x.device)
+        y = _linear_group_norm(x, weight, bias, gn_weight, gn_bias, groups, eps, negative_slope, residual, pre=pre)
+        ctx.save_for_backward(x, weight, gn_weight, pre, y)
+        ctx.args = (groups, eps, negative_slope)
+        return y
+
+    @staticmethod
+    def backward(ctx, grad):
+        x, weight, gn_weight, pre, y = ctx.saved_tensors
+        groups, eps, slope = ctx.args
+        need = ctx.needs_input_grad
+        gpre, ggw, ggb, gr = group_norm_backward_batched(pre, y, gn_weight, groups, [pre.shape[0], 0], grad.contiguous(), eps, slope,
+                                                         need[5], need[3], need[4])
+        gx, gw, gb = linear_backward(x, weight, gpre, need[0], need[1], need[2]) if any(need[:3]) else (None, None, None)
+        return gx, gw, gb, ggw, ggb, gr, None, None, None
+
+
+def _linear_group_norm(x, weight, bias, gn_weight, gn_bias, groups, eps=1e-5, negative_slope=None, residual=None, pre=None):
+    """``pre``: tensor to receive the pre-norm activation (default: a shared scratch buffer)"""
     x, weight, bias, gn_weight, gn_bias = _detach(x), _detach(weight), _detach(bias), _detach(gn_weight), _detach(gn_bias)
+    residual = _detach(residual)
     if not x.is_cuda or x.dtype != _f32 or x.stride(1) != 1:
         raise RuntimeError('linear_group_norm: x must be a float32 CUDA tensor with unit inner stride')
     L.require_cuda(weight, 'weight', _f32)
     m, k = x.shape
     n = weight.shape[0]
-    pre = scratch((m, n), x.device, 'pre_norm')
+    if pre is None:
+        pre = scratch((m, n), x.device, 'pre_norm')
     y = torch.empty((m, n), dtype=_f32, device=x.device)
     ws = _gn_workspace(x.device, groups, m, n)
     L.check(L.lib().geob200_linear_group_norm(x.data_ptr(), x.stride(0), weight.data_ptr(), L.ptr(bias), m, n, k, groups,
@@ -171,12 +353,46 @@ def linear_group_norm(x, weight, bias, gn_weight, gn_bias, groups, eps=1e-5, neg
 
 def kpconv_group_norm(s_feats, q_points, s_points, neighbor_indices, kernel_points, weights, bias, sigma, gn_weight, gn_bias, groups,
                       eps=1e-5, negative_slope=0.1, weights_t=None):
-    """ConvBlock / conv part of ResidualBlock: leaky(GroupNorm(KPConv(...)))"""
+    """ConvBlock / conv part of ResidualBlock: leaky(GroupNorm(KPConv(...))).  Differentiable w.r.t. s_feats, the weights,
+    the biases and the GroupNorm affine (the autograd path keeps its own copy of the pre-norm activation)."""
     m, h = neighbor_indices.shape
     k, cin, cout = weights.shape
     if not (KPCONV_MODE == 'tc' and cin % 32 == 0 and cout % 16 == 0 and cout >= 32 and (cout <= 128 or cout % 128 == 0) and m >= 64):
         x = kpconv(s_feats, q_points, s_points, neighbor_indices, kernel_points, weights, bias, sigma, weights_t=weights_t)
         return group_norm(x, gn_weight, gn_bias, groups, eps, negative_slope=negative_slope)
+    if _needs_grad(s_feats, weights, bias, gn_weight, gn_bias):
+        return _KPConvGroupNorm.apply(s_feats, weights, bias, gn_weight, gn_bias, q_points, s_points, neighbor_indices, kernel_points,
+                                      float(sigma), int(groups), float(eps), negative_slope, weights_t)
+    return _kpconv_group_norm(s_feats, q_points, s_points, neighbor_indices, kernel_points, weights, bias, sigma, gn_weight, gn_bias,
+                              groups, eps, negative_slope, weights_t)
+
+
+class _KPConvGroupNorm(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, s_feats, weights, bias, gn_weight, gn_bias, q_points, s_points, neighbor_indices, kernel_points, sigma, groups, eps,
+                negative_slope, weights_t):
+        pre = torch.empty((neighbor_indices.shape[0], weights.shape[2]), dtype=_f32, device=s_feats.device)
+        y = _kpconv_group_norm(s_feats, q_points, s_points, neighbor_indices, kernel_points, weights, bias, sigma, gn_weight, gn_bias,
+                               groups, eps, negative_slope, weights_t, pre=pre)
+        ctx.save_for_backward(s_feats, weights, gn_weight, q_points, s_points, neighbor_indices, kernel_points, pre, y)
+        ctx.args = (sigma, groups, eps, negative_slope)
+        return y
+
+    @staticmethod
+    def backward(ctx, grad):
+        s_feats, weights, gn_weight, q, s, nbr, kp, pre, y = ctx.saved_tensors
+        sigma, groups, eps, slope = ctx.args
+        need = ctx.needs_input_grad
+        gpre, ggw, ggb, _ = group_norm_backward_batched(pre, y, gn_weight, groups, [pre.shape[0], 0], grad.contiguous(), eps, slope, False,
+                                                        need[3], need[4])
+        gf, gw, gb = kpconv_backward(s_feats, q, s, nbr, kp, weights, sigma, gpre, need[0], need[1], need[2])
+        return gf, gw, gb, ggw, ggb, None, None, None, None, None, None, None, None, None
+
+
+def _kpconv_group_norm(s_feats, q_points, s_points, neighbor_indices, kernel_points, weights, bias, sigma, gn_weight, gn_bias, groups,
+                       eps=1e-5, negative_slope=0.1, weights_t=None, pre=None):
+    m, h = neighbor_indices.shape
+    k, cin, cout = weights.shape
     s_feats, weights, bias, gn_weight, gn_bias = _detach(s_feats), _detach(weights), _detach(bias), _detach(gn_weight), _detach(gn_bias)
     _f(s_feats, 's_feats'); _f(q_points, 'q_points'); _f(s_points, 's_points')
     L.require_cuda(neighbor_indices, 'neighbor_indices', _i64)
@@ -185,7 +401,8 @@ def kpconv_group_norm(s_feats, q_points, s_points, neighbor_indices, kernel_poin
     if weights_t is None:
         weights_t = weights.reshape(k * cin, cout).t().contiguous()
     lib = L.lib()
-    pre = scratch((m, cout), dev, 'pre_norm')
+    if pre is None:
+        pre = scratch((m, cout), dev, 'pre_norm')
     y = torch.empty((m, cout), dtype=_f32, device=dev)
     gws = _gn_workspace(dev, groups, m, cout)
     ws = L.workspace(lib.geob200_kpconv_tc_workspace_bytes(m, ns, cin), dev, 'kpconv_tc')
@@ -235,6 +452,13 @@ def linear_group_norm_batched(x, weight, bias, gn_weight, gn_bias, groups, cloud
 
 
 def maxpool(x, neighbor_indices):
+    """differentiable w.r.t. x (``maxpool_backward_batched``)"""
+    if _needs_grad(x):
+        return _Maxpool.apply(x, neighbor_indices)
+    return _maxpool(x, neighbor_indices)
+
+
+def _maxpool(x, neighbor_indices):
     x = _detach(x)
     _f(x, 'x'); L.require_cuda(neighbor_indices, 'neighbor_indices', _i64)
     m, h = neighbor_indices.shape
@@ -244,9 +468,88 @@ def maxpool(x, neighbor_indices):
     return y
 
 
-def upsample_concat(x, upsample_indices, skip=None):
-    """[nearest_upsample(x, upsample_indices) | skip]; ``upsample_indices`` (M, H) -- only column 0 is used."""
+def maxpool_backward_batched(x, neighbor_indices, cloud_rows, grad_y, cloud_max=None):
+    """grad_x of the max-pool for the upstream gradient ``grad_y`` (n_query, C): each output's gradient goes to the neighbour column
+    that won the forward's max (ties: the lowest column), none when the zero shadow row won.  ``cloud_rows``: query rows per cloud
+    (2B host ints); ``cloud_max`` (device int32 (2B,), ``geob200_cloud_max_count``): cut pair p's rows to the batched forward's width,
+    None = every column (``maxpool``)."""
     x = _detach(x)
+    _f(x, 'x'); _f(grad_y, 'grad_y'); L.require_cuda(neighbor_indices, 'neighbor_indices', _i64)
+    if cloud_max is not None:
+        L.require_cuda(cloud_max, 'cloud_max', _i32)
+        if cloud_max.numel() != len(cloud_rows):
+            raise RuntimeError('maxpool_backward_batched: cloud_max needs one entry per cloud')
+    m, h = neighbor_indices.shape
+    ns, c = x.shape
+    if tuple(grad_y.shape) != (m, c):
+        raise RuntimeError(f'maxpool_backward_batched: grad_y must be ({m}, {c})')
+    gx = torch.empty_like(x)
+    lib = L.lib()
+    ws = L.workspace(lib.geob200_maxpool_backward_batched_workspace_bytes(m, ns, h, c), x.device, 'maxpool_backward')
+    L.check(lib.geob200_maxpool_backward_batched(x.data_ptr(), neighbor_indices.data_ptr(), m, ns, h, c, L.ptr(cloud_max), len(cloud_rows) // 2,
+                                                 _host_i64(cloud_rows), grad_y.data_ptr(), gx.data_ptr(), ws.data_ptr(), ws.numel(),
+                                                 L.stream_ptr()), 'maxpool_backward_batched')
+    return gx
+
+
+class _Maxpool(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, neighbor_indices):
+        ctx.save_for_backward(x, neighbor_indices)
+        return _maxpool(x, neighbor_indices)
+
+    @staticmethod
+    def backward(ctx, grad):
+        x, nbr = ctx.saved_tensors
+        return maxpool_backward_batched(x, nbr, [nbr.shape[0], 0], grad.contiguous()), None
+
+
+def upsample_concat(x, upsample_indices, skip=None):
+    """[nearest_upsample(x, upsample_indices) | skip]; ``upsample_indices`` (M, H) -- only column 0 is used.  Differentiable w.r.t.
+    x and skip (``upsample_concat_backward``)."""
+    if _needs_grad(x, skip):
+        return _UpsampleConcat.apply(x, skip, upsample_indices)
+    return _upsample_concat(x, upsample_indices, skip)
+
+
+def upsample_concat_backward(upsample_indices, n_support, c1, grad_y, need_skip=True):
+    """(grad_x (n_support, c1), grad_skip (n_query, C - c1) or None) of ``upsample_concat``: each coarse row sums the gradient rows of
+    the fine rows that copied it, in fine-row order; sentinel indices contribute nothing"""
+    _f(grad_y, 'grad_y')
+    if not upsample_indices.is_cuda or upsample_indices.dtype != _i64:
+        raise RuntimeError('upsample_indices must be an int64 CUDA tensor')
+    m = upsample_indices.shape[0]
+    stride = upsample_indices.stride(0) if upsample_indices.ndim == 2 else 1
+    c2 = grad_y.shape[1] - c1
+    if grad_y.shape[0] != m or c2 < 0:
+        raise RuntimeError(f'upsample_concat_backward: grad_y must have {m} rows and at least {c1} columns')
+    dev = grad_y.device
+    gx = torch.empty((n_support, c1), dtype=_f32, device=dev)
+    gs = torch.empty((m, c2), dtype=_f32, device=dev) if need_skip and c2 > 0 else None
+    lib = L.lib()
+    ws = L.workspace(lib.geob200_upsample_concat_backward_workspace_bytes(m, n_support), dev, 'upsample_concat_backward')
+    L.check(lib.geob200_upsample_concat_backward(upsample_indices.data_ptr(), stride, m, n_support, c1, c2, grad_y.data_ptr(), gx.data_ptr(),
+                                                 L.ptr(gs), ws.data_ptr(), ws.numel(), L.stream_ptr()), 'upsample_concat_backward')
+    return gx, gs
+
+
+class _UpsampleConcat(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, skip, upsample_indices):
+        ctx.save_for_backward(upsample_indices)
+        ctx.shape = tuple(x.shape)
+        return _upsample_concat(x, upsample_indices, skip)
+
+    @staticmethod
+    def backward(ctx, grad):
+        up, = ctx.saved_tensors
+        ns, c1 = ctx.shape
+        gx, gs = upsample_concat_backward(up, ns, c1, grad.contiguous(), ctx.needs_input_grad[1])
+        return gx if ctx.needs_input_grad[0] else None, gs, None
+
+
+def _upsample_concat(x, upsample_indices, skip=None):
+    x, skip = _detach(x), _detach(skip)
     _f(x, 'x')
     if not upsample_indices.is_cuda or upsample_indices.dtype != _i64:
         raise RuntimeError('upsample_indices must be an int64 CUDA tensor')

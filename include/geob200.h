@@ -138,6 +138,56 @@ int geob200_cloud_max_count(const int64_t* neighbors, int64_t n_query, int64_t n
 int geob200_upsample_concat(const float* x, const int64_t* up_indices, int64_t up_stride, int64_t n_support,
                             const float* skip, int64_t n_query, int64_t c1, int64_t c2, float* y, void* stream);
 
+/* ---- backbone backward (kpconv_grad.cu) ---------------------------------------------------------------------------------------
+ * Gradients of the ops above for an upstream gradient of their output.  No float atomics: every reduction has a fixed order, so
+ * two calls give the same bits.  Support rows sum their (query row, column) entries in that order through a CSR transpose of the
+ * index table; reductions over rows fold 256-row chunk partials in chunk order.  Index entries outside [0, n_support) are sentinels
+ * and contribute nothing.  Every argument check runs before the first launch.  An output pointer may be NULL to skip that
+ * gradient where noted. */
+
+/* KPConv (c_in = 1 or a multiple of 32): grad_weights (15, c_in, c_out) = wf^T (grad_out / n_valid) with wf recomputed by the
+ * forward's gather, grad_bias = column sums of grad_out, grad_feats (n_support, c_in) = the transposed gather of
+ * (grad_out / n_valid) . W_flat^T with the forward's influences.  n_valid is the forward's count, a constant (it depends on the
+ * signs of the feature-row sums only).  Each of the three may be NULL. */
+size_t geob200_kpconv_backward_workspace_bytes(int64_t n_query, int64_t n_support, int64_t n_neighbors, int64_t c_in, int64_t c_out);
+int geob200_kpconv_backward(const float* s_feats, const float* q_points, const float* s_points, const int64_t* neighbors, int64_t n_query,
+                            int64_t n_support, int64_t n_neighbors, const float* kernel_points, int64_t n_kernel, const float* weights,
+                            int64_t c_in, int64_t c_out, float sigma, const float* grad_out, float* grad_feats, float* grad_weights,
+                            float* grad_bias, void* workspace, size_t workspace_bytes, void* stream);
+
+/* Linear y = x . weight^T + b, optionally followed by a ReLU: grad_x (m, k) = grad_y . weight through the forward's GEMM with
+ * weight_t = weight^T (k, n) contiguous; grad_weight (n, k) = grad_y^T x and grad_bias (n) in fp32 with the fixed-order fold.  relu_y:
+ * the forward's output when it applied the ReLU (the gradient passes where it is positive), else NULL.  Each output may be NULL. */
+size_t geob200_linear_backward_workspace_bytes(int64_t m, int64_t n, int64_t k, int relu);
+int geob200_linear_backward(const float* x, int64_t ldx, const float* weight_t, const float* relu_y, int64_t m, int64_t n, int64_t k,
+                            const float* grad_y, float* grad_x, float* grad_weight, float* grad_bias, void* workspace, size_t workspace_bytes,
+                            void* stream);
+
+/* y = leaky(GroupNorm(x) + residual) with per-pair statistics (layout of geob200_group_norm_batched; one pair: cloud_rows_h =
+ * {n_rows, 0}).  x is the pre-norm input, y the forward's output (read for the LeakyReLU's derivative, which follows the sign of
+ * the pre-activation: slope at 0; may be NULL without leaky; slope >= 0).  The statistics are recomputed from x in double.  grad_residual
+ * receives the gradient after the LeakyReLU (NULL: no residual); grad_gamma / grad_beta may be NULL. */
+size_t geob200_group_norm_backward_batched_workspace_bytes(int64_t n_rows, int64_t channels, int64_t groups, int64_t n_pairs);
+int geob200_group_norm_backward_batched(const float* x, const float* y, int64_t n_rows, int64_t channels, int64_t groups, const float* gamma,
+                                        float eps, int leaky, float slope, const float* grad_y, float* grad_x, float* grad_gamma,
+                                        float* grad_beta, float* grad_residual, void* workspace, size_t workspace_bytes, void* stream,
+                                        int64_t n_pairs, const int64_t* cloud_rows_h);
+
+/* maxpool: the gradient of y[m][c] goes to the neighbour column that won the forward's max (ties: the lowest column); a winning
+ * zero shadow row drops it.  cloud_max (device, may be NULL = all n_neighbors columns, as geob200_maxpool) cuts pair p's rows to
+ * the width of the batched forward; cloud_rows_h[2 * n_pairs] are the query rows per cloud. */
+size_t geob200_maxpool_backward_batched_workspace_bytes(int64_t n_query, int64_t n_support, int64_t n_neighbors, int64_t channels);
+int geob200_maxpool_backward_batched(const float* x, const int64_t* neighbors, int64_t n_query, int64_t n_support, int64_t n_neighbors,
+                                     int64_t channels, const int32_t* cloud_max, int64_t n_pairs, const int64_t* cloud_rows_h,
+                                     const float* grad_y, float* grad_x, void* workspace, size_t workspace_bytes, void* stream);
+
+/* upsample_concat: grad_x (n_support, c1) = per coarse row the sum, in fine-row order, of the first c1 columns of grad_y over the
+ * fine rows that copied it; grad_skip (n_query, c2) = the last c2 columns (may be NULL). */
+size_t geob200_upsample_concat_backward_workspace_bytes(int64_t n_query, int64_t n_support);
+int geob200_upsample_concat_backward(const int64_t* up_indices, int64_t up_stride, int64_t n_query, int64_t n_support, int64_t c1, int64_t c2,
+                                     const float* grad_y, float* grad_x, float* grad_skip, void* workspace, size_t workspace_bytes,
+                                     void* stream);
+
 /* ---- point-to-node grouping ------------------------------------------------------------------------------ */
 
 /* The per-pair stages (grouping, structure-embedding indices, ground-truth correspondences, matching, patches, LGR, metrics) have
