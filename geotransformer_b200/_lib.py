@@ -79,6 +79,15 @@ _sig('geob200_set_attention_tma', c_int, c_int)
 _sig('geob200_head_bias', c_int, P, I64, P, I64, I64, I64, P, P)
 _sig('geob200_add_layernorm', c_int, P, P, P, P, I64, I64, F, P, P)
 _sig('geob200_l2_normalize', c_int, P, I64, I64, P, P)
+_sig('geob200_add_layernorm_backward_workspace_bytes', SZ, I64, I64)
+_sig('geob200_add_layernorm_backward', c_int, P, P, P, I64, I64, F, P, P, P, P, P, SZ, P)
+_sig('geob200_l2_normalize_backward', c_int, P, I64, I64, P, P, P)
+_sig('geob200_head_project_backward_workspace_bytes', SZ, I64, I64, I64)
+_sig('geob200_head_project_backward', c_int, P, I64, P, P, I64, I64, I64, P, P, P, I64, P, P, P, SZ, P)
+_sig('geob200_attention_backward_batched_workspace_bytes', SZ, P, I64, I64)
+_sig('geob200_attention_backward_batched', c_int, P, P, I64, I64, I64, I64, I64, I64, I64, I64, I64, I64, P, SZ, P)
+_sig('geob200_gse_embed_backward_workspace_bytes', SZ, I64, I64)
+_sig('geob200_gse_embed_backward', c_int, P, P, I64, I64, I64, P, SZ, I64, F, F, P, P, P, P, P, P, P, P, P, SZ, P)
 _sig('geob200_sinkhorn', c_int, P, P, P, P, I64, I64, I64, F, P, P)
 _sig('geob200_sinkhorn_backward_workspace_bytes', SZ, I64, I64, I64)
 _sig('geob200_sinkhorn_backward', c_int, P, P, P, P, I64, I64, I64, F, P, P, P, P, SZ, P)

@@ -300,7 +300,7 @@ __global__ void __launch_bounds__(512) att_softmax_pv_kernel(const __grid_consta
     const int N = item.N, M = item.M;
     const int n0 = blockIdx.x * ATT_R;
     if (n0 >= N) return;                          // grid.x covers the largest item of the batch
-    const float* __restrict__ S = item.S;
+    const float* S = item.S;                      // overwritten by P below
     const float* __restrict__ v = item.v;
     float* __restrict__ out = item.out;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -323,7 +323,11 @@ __global__ void __launch_bounds__(512) att_softmax_pv_kernel(const __grid_consta
             sum += e;
         }
         sum = warp_sum(sum);
-        for (int m = lane; m < M; m += 32) s[m] = s[m] / sum;
+        float* dst = item.S + ((long long)(n0 + r) * H + (rh % H)) * M;      // S keeps P, as the TMA kernels leave it (backward)
+        for (int m = lane; m < M; m += 32) {
+            s[m] = s[m] / sum;
+            dst[m] = s[m];
+        }
     }
     __syncthreads();
     // P.V: thread = (4 channels, one of ATT_KQ key ranges); 16-byte value loads, 4 of them in flight; ranges folded through smem

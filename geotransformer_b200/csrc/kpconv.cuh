@@ -39,4 +39,10 @@ void kpconv_gather(const float* s_feats, const float* q_points, const float* s_p
                    const float* kernel_points, float sigma, int n_support, int n_query, int c_in, unsigned char* pos, float* wf,
                    float* inv_count, cudaStream_t st);
 
+// C[i][j] = sum_m A[m][i] * (B[m][j] * s[m]) (i < ka, j < n) over fixed 256-row chunks folded in chunk order in double
+// (kpconv_grad.cu); A == nullptr: a column of ones (ka = 1, column sums), s == nullptr: ones.  `part` holds atb_bytes(M, ka, n).
+size_t atb_bytes(int64_t M, int64_t ka, int64_t n);
+void atb(const float* A, long long lda, const float* B, long long ldb, const float* s, int64_t M, int64_t ka, int64_t n, float* C,
+         float* part, cudaStream_t st);
+
 }  // namespace geob200

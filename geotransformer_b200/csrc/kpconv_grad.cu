@@ -152,13 +152,13 @@ __global__ void __launch_bounds__(256) atb_fold_kernel(const float* __restrict__
     C[i] = (float)s;
 }
 
-static size_t atb_bytes(int64_t M, int64_t ka, int64_t n) {
+size_t atb_bytes(int64_t M, int64_t ka, int64_t n) {
     const int64_t chunks = (M + ATB_ROWS - 1) / ATB_ROWS;
     return chunks > 1 ? align_up((size_t)chunks * ka * n * 4, 256) : 0;
 }
 
-static void atb(const float* A, long long lda, const float* B, long long ldb, const float* s, int64_t M, int64_t ka, int64_t n, float* C,
-                float* part, cudaStream_t st) {
+void atb(const float* A, long long lda, const float* B, long long ldb, const float* s, int64_t M, int64_t ka, int64_t n, float* C,
+         float* part, cudaStream_t st) {
     const int chunks = (int)((M + ATB_ROWS - 1) / ATB_ROWS);
     const dim3 grid((unsigned)((n + ATB_T - 1) / ATB_T), (unsigned)((ka + ATB_T - 1) / ATB_T), (unsigned)chunks);
     if (chunks == 1) {

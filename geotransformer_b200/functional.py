@@ -729,7 +729,17 @@ def _gse_mode(mode, table):
 
 def gse_embed_flat(d_indices, a_indices, n_rows, div_term, wd, wa, bd, ba, wd_t, wa_t, out, mode=None, table=None):
     """structure embedding of ``n_rows`` (anchor, point) pairs given as flat index arrays -- the (i, j) pairs of SEVERAL clouds
-    concatenated (d (n_rows,), a (n_rows, k)) -> out (n_rows, C): one launch for a whole batch of clouds."""
+    concatenated (d (n_rows,), a (n_rows, k)) -> out (n_rows, C): one launch for a whole batch of clouds.  Differentiable w.r.t.
+    ``wd``, ``wa``, ``bd`` and ``ba`` (``gse_embed_backward``; C = 128 or 256), which then needs the ``table`` of these weights
+    whatever the mode; with ``out`` the result is copied into it, which then carries the graph."""
+    if _needs_grad(wd, wa, bd, ba):
+        y = _GseEmbed.apply(wd, wa, bd, ba, d_indices, a_indices, int(n_rows), div_term, wd_t, wa_t, mode, table)
+        return y if out is None else out.copy_(y)
+    return _gse_embed_flat(d_indices, a_indices, n_rows, div_term, wd, wa, bd, ba, wd_t, wa_t, out, mode, table)
+
+
+def _gse_embed_flat(d_indices, a_indices, n_rows, div_term, wd, wa, bd, ba, wd_t, wa_t, out, mode=None, table=None):
+    wd, wa, bd, ba = _detach(wd), _detach(wa), _detach(bd), _detach(ba)
     c = wd.shape[0]
     mode = _gse_mode(mode, table)
     if mode == 5 and c in (128, 256):
@@ -748,10 +758,61 @@ def gse_embed_flat(d_indices, a_indices, n_rows, div_term, wd, wa, bd, ba, wd_t,
     return out
 
 
+def gse_embed_backward(d_indices, a_indices, n_rows, div_term, wa, ba, table, grad_embed):
+    """(grad_wd, grad_bd, grad_wa, grad_ba) of the structure embedding for the upstream gradient ``grad_embed`` (n_rows, C), C = 128 or
+    256.  The winning angle term of every (row, channel) is the one the tabulated forward picks: it comes from the lookups into
+    ``table`` (the GseTable of the current weights).  The sinusoid is evaluated on the fly, never stored."""
+    wa, ba = _detach(wa), _detach(ba)
+    for t, name in ((d_indices, 'd_indices'), (a_indices, 'a_indices'), (div_term, 'div_term'), (wa, 'wa'), (ba, 'ba'),
+                    (grad_embed, 'grad_embed')):
+        _f(t, name)
+    c = int(wa.shape[0])
+    if table is None or table.channels != c:
+        raise RuntimeError('gse_embed_backward needs the GseTable of these weights (functional.gse_table)')
+    n_rows = int(n_rows)
+    if grad_embed.numel() != n_rows * c or d_indices.numel() < n_rows or a_indices.numel() % max(n_rows, 1) != 0:
+        raise RuntimeError(f'gse_embed_backward: grad_embed must hold ({n_rows}, {c}) values and the indices {n_rows} rows')
+    dev = grad_embed.device
+    gwd, gwa = (torch.empty((c, c), dtype=_f32, device=dev) for _ in range(2))
+    gbd, gba = (torch.empty((c,), dtype=_f32, device=dev) for _ in range(2))
+    lib = L.lib()
+    ws = L.workspace(lib.geob200_gse_embed_backward_workspace_bytes(n_rows, c), dev, 'gse_embed_backward')
+    with _timed('gse_embed_backward'):
+        L.check(lib.geob200_gse_embed_backward(d_indices.data_ptr(), a_indices.data_ptr(), n_rows, a_indices.numel() // n_rows, c,
+                                               table.blob.data_ptr(), table.blob.numel(), table.inv_step, table.d_max, table.a_max,
+                                               div_term.data_ptr(), wa.data_ptr(), ba.data_ptr(), grad_embed.data_ptr(), gwd.data_ptr(),
+                                               gbd.data_ptr(), gwa.data_ptr(), gba.data_ptr(), ws.data_ptr(), ws.numel(), L.stream_ptr()),
+                'gse_embed_backward')
+    return gwd, gbd, gwa, gba
+
+
+class _GseEmbed(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, wd, wa, bd, ba, d_indices, a_indices, n_rows, div_term, wd_t, wa_t, mode, table):
+        if table is None:
+            raise RuntimeError('gse_embed: the backward needs the GseTable of these weights (functional.gse_table)')
+        out = torch.empty((n_rows, wd.shape[0]), dtype=_f32, device=d_indices.device)
+        _gse_embed_flat(d_indices, a_indices, n_rows, div_term, wd, wa, bd, ba, wd_t, wa_t, out, mode, table)
+        ctx.save_for_backward(d_indices, a_indices, div_term, wa, ba)
+        ctx.n_rows, ctx.table = n_rows, table
+        return out
+
+    @staticmethod
+    def backward(ctx, grad):
+        d, a, div_term, wa, ba = ctx.saved_tensors
+        gwd, gbd, gwa, gba = gse_embed_backward(d, a, ctx.n_rows, div_term, wa, ba, ctx.table, grad.contiguous())
+        return gwd, gwa, gbd, gba, None, None, None, None, None, None, None, None
+
+
 def gse_embed(d_indices, a_indices, div_term, wd, wa, bd, ba, wd_t, wa_t, mode=None, out=None, table=None):
     """structure embedding of one cloud: d (n, n), a (n, n, k) -> (n, n, C)"""
     n = d_indices.shape[0]
-    emb = torch.empty((n, n, wd.shape[0]), dtype=_f32, device=d_indices.device) if out is None else out
+    c = wd.shape[0]
+    if _needs_grad(wd, wa, bd, ba):
+        emb = gse_embed_flat(d_indices, a_indices, n * n, div_term, wd, wa, bd, ba, wd_t, wa_t, None, mode=mode, table=table)
+        emb = emb.view(n, n, c)
+        return emb if out is None else out.copy_(emb)
+    emb = torch.empty((n, n, c), dtype=_f32, device=d_indices.device) if out is None else out
     return gse_embed_flat(d_indices, a_indices, n * n, div_term, wd, wa, bd, ba, wd_t, wa_t, emb, mode=mode, table=table)
 
 
@@ -763,22 +824,178 @@ def _rows(t, name):
 
 def attention(q, k, v, heads, qp=None, qb=None, embed=None, out=None, streaming=True):
     """q, k, v may be column slices of a fused projection buffer (row stride != channels).  streaming=False forces the
-    single-kernel path (the only one for channel counts other than 128 / 256)."""
+    single-kernel path (the only one for channel counts other than 128 / 256).  Differentiable w.r.t. q, k, v, qp, qb and embed
+    (``attention_backward_batched``; C = 128 or 256, streaming): the forward then leaves its softmax probabilities in a tensor owned
+    by the autograd node; with ``out`` the result is copied into it, which then carries the graph."""
+    if _needs_grad(q, k, v, qp, qb, embed):
+        if not streaming:
+            raise RuntimeError('attention: the backward needs the probabilities of the streaming forward')
+        srcs, keys, where = [], [], []
+        for t in (q, k, v):
+            base, r0, col = _column_source(t)
+            key = (id(base), r0, t.shape[0])
+            if key not in keys:
+                keys.append(key)
+                srcs.append(base if (r0 == 0 and t.shape[0] == base.shape[0]) else base[r0:r0 + t.shape[0]])
+            where.append((keys.index(key), col))
+        y = _Attention.apply(int(heads), int(q.shape[1]), tuple(where), qp, qb, embed, *srcs)
+        return y if out is None else out.copy_(y)
+    return _attention(q, k, v, heads, qp, qb, embed, out, streaming)
+
+
+def _attention(q, k, v, heads, qp=None, qb=None, embed=None, out=None, streaming=True, probs=None):
+    """``probs``: a uint8 tensor of geob200_attention_workspace_bytes to run the streaming path in, instead of the shared scratch;
+    it holds the (n, heads, m) probabilities afterwards"""
+    q, k, v, qp, qb, embed = (_detach(t) for t in (q, k, v, qp, qb, embed))
     _rows(q, 'q'); _rows(k, 'k'); _rows(v, 'v')
     n, c = q.shape
     m = k.shape[0]
     if out is None:
         out = torch.empty((n, c), dtype=_f32, device=q.device)
     lib = L.lib()
-    ws = L.workspace(lib.geob200_attention_workspace_bytes(n, m, heads), q.device, tag='attention') if streaming else None
+    ws = probs if probs is not None else (
+        L.workspace(lib.geob200_attention_workspace_bytes(n, m, heads), q.device, tag='attention') if streaming else None)
     L.check(lib.geob200_attention(q.data_ptr(), q.stride(0), k.data_ptr(), k.stride(0), v.data_ptr(), v.stride(0),
                                   L.ptr(qp), L.ptr(qb), L.ptr(embed), n, m, c, heads, out.data_ptr(), out.stride(0),
                                   L.ptr(ws), 0 if ws is None else ws.numel(), L.stream_ptr()), 'attention')
     return out
 
 
+def _column_source(t):
+    """(base, r0, col): ``t`` is rows r0 .. r0 + t.shape[0], columns col .. col + t.shape[1] of the 2-D tensor ``base`` it is a view
+    of (or of itself).  The backward writes the gradient of every slice of one row block into one (rows, base width) tensor, so a
+    fused projection (q|k|v, k|v) gets one contiguous upstream gradient."""
+    base = t._base if t._base is not None else t
+    if base.dim() != 2 or base.stride(1) != 1 or t.stride(1) != 1 or t.stride(0) != base.stride(0):
+        return t, 0, 0
+    r0, col = divmod(t.storage_offset() - base.storage_offset(), base.stride(0))
+    return base, r0, col
+
+
+class _AttItem(ctypes.Structure):
+    """geob200_att_item_t"""
+    _fields_ = [(n, ctypes.c_void_p) for n in ('q', 'k', 'v', 'qp', 'qb', 'embed', 'out')] + [('n_query', ctypes.c_int64),
+                                                                                            ('n_key', ctypes.c_int64)]
+
+
+class _AttGradItem(ctypes.Structure):
+    """geob200_att_grad_item_t"""
+    _fields_ = [(n, ctypes.c_void_p) for n in ('probs', 'grad_out', 'grad_q', 'grad_k', 'grad_v', 'grad_qp', 'grad_qb', 'grad_embed')]
+
+
+def attention_probs(n, m, heads, device):
+    """buffer for the (n, heads, m) probabilities of one ``attention`` forward (its streaming workspace) and the float view of them"""
+    buf = torch.empty(L.lib().geob200_attention_workspace_bytes(n, m, heads), dtype=_u8, device=device)
+    return buf, buf[:n * m * heads * 4].view(_f32).view(n, heads, m)
+
+
+def attention_backward_batched(items, heads):
+    """Gradients of ``attention`` for a list of items in one call.  Every item is a dict with the forward's q, k, v (column slices
+    allowed), out (its output), probs ((n, heads, m) probabilities of that forward, ``attention_probs``), grad_out (n, C) and, for
+    self-attention, qp, qb and embed; optionally grad_q / grad_k / grad_v, (n, C) / (m, C) views to write the gradients into (column
+    slices of one fused gradient allowed), and structure=False to skip grad_qp / grad_embed (the E pass).  The items share channels and
+    row strides.  Returns per item (grad_q, grad_k, grad_v, grad_qp, grad_qb, grad_embed), the last three None for cross-attention."""
+    if not items:
+        raise RuntimeError('attention_backward_batched: no items')
+    arr, garr, res = (_AttItem * len(items))(), (_AttGradItem * len(items))(), []
+    strides = gstrides = None
+    for j, it in enumerate(items):
+        q, k, v, o = (_rows(_detach(it[name]), name) for name in ('q', 'k', 'v', 'out'))
+        qp, qb, e = (_detach(it.get(name)) for name in ('qp', 'qb', 'embed'))
+        probs, go = _detach(it['probs']), _f(_detach(it['grad_out']), 'grad_out')
+        n, c = q.shape
+        m = k.shape[0]
+        st = (q.stride(0), k.stride(0), v.stride(0), o.stride(0), c)
+        if strides is not None and st != strides:
+            raise RuntimeError('attention_backward_batched: the items must share channels and row strides')
+        strides = st
+        if tuple(go.shape) != (n, c) or tuple(o.shape) != (n, c) or tuple(v.shape) != (m, c) or probs.numel() < n * m * heads:
+            raise RuntimeError(f'attention_backward_batched: item {j}: out / grad_out must be ({n}, {c}), v ({m}, {c}), probs {n * m * heads} values')
+        if probs.dtype != _f32 or not probs.is_contiguous():
+            raise RuntimeError('attention_backward_batched: probs must be a contiguous float32 view (attention_probs)')
+        if e is not None:
+            _f(qp, 'qp'); _f(qb, 'qb'); _f(e, 'embed')
+            if tuple(qp.shape) != (n, heads, c) or tuple(qb.shape) != (n, heads) or e.numel() != n * m * c:
+                raise RuntimeError(f'attention_backward_batched: item {j}: qp ({n}, {heads}, {c}), qb ({n}, {heads}), embed ({n}, {m}, {c})')
+        dev = q.device
+        g = []
+        for name, rows in (('grad_q', n), ('grad_k', m), ('grad_v', m)):
+            t = it.get(name)
+            if t is None:
+                t = torch.empty((rows, c), dtype=_f32, device=dev)
+            elif not t.is_cuda or t.dtype != _f32 or tuple(t.shape) != (rows, c) or t.stride(1) != 1:
+                raise RuntimeError(f'attention_backward_batched: item {j}: {name} must be a ({rows}, {c}) float32 CUDA view with unit inner stride')
+            g.append(t)
+        gst = tuple(t.stride(0) for t in g)
+        if gstrides is not None and gst != gstrides:
+            raise RuntimeError('attention_backward_batched: the items\' gradients must share row strides')
+        gstrides = gst
+        structure = e is not None and it.get('structure', True)
+        g += ([torch.empty((n, heads, c), dtype=_f32, device=dev), torch.empty((n, heads), dtype=_f32, device=dev),
+               torch.empty((n, m, c), dtype=_f32, device=dev)] if structure else [None, None, None])
+        arr[j] = _AttItem(q.data_ptr(), k.data_ptr(), v.data_ptr(), L.ptr(qp), L.ptr(qb), L.ptr(e), o.data_ptr(), n, m)
+        garr[j] = _AttGradItem(probs.data_ptr(), go.data_ptr(), *(L.ptr(t) for t in g))
+        res.append(tuple(g))
+    lib = L.lib()
+    ldq, ldk, ldv, ldo, c = strides
+    ws = L.workspace(lib.geob200_attention_backward_batched_workspace_bytes(arr, len(items), heads), dev, 'attention_backward')
+    with _timed('attention_backward'):
+        L.check(lib.geob200_attention_backward_batched(arr, garr, len(items), ldq, ldk, ldv, ldo, *gstrides, c, heads, ws.data_ptr(),
+                                                       ws.numel(), L.stream_ptr()), 'attention_backward_batched')
+    return res
+
+
+def _source_grads(srcs, where, c):
+    """one gradient per source (zero where no slice of it reads) and the (rows, c) views of it at the given column offsets"""
+    covered = [set() for _ in srcs]
+    for i, col in where:
+        covered[i].update(range(col, col + c))
+    gs = [(torch.empty if len(cov) == s.shape[1] else torch.zeros)(tuple(s.shape), dtype=_f32, device=s.device)
+          for s, cov in zip(srcs, covered)]
+    return gs, [gs[i][:, col:col + c] for i, col in where]
+
+
+class _Attention(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, heads, c, where, qp, qb, embed, *srcs):
+        q, k, v = (srcs[i][:, col:col + c] for i, col in where)
+        n, m = q.shape[0], k.shape[0]
+        # the streaming forward (the one that leaves the probabilities in its workspace) takes C = 128 / 256 and the keys whose
+        # scores fit its softmax kernel's shared memory (attention_streaming_batch)
+        if c not in (128, 256) or 4 * (2 * heads * ((m + 3) // 4 * 4) + 16 * c) > 200 * 1024:
+            raise RuntimeError(f'attention backward: channels {c} (128 or 256) or keys {m} outside the streaming forward')
+        buf, probs = attention_probs(n, m, heads, q.device)
+        out = _attention(q, k, v, heads, qp, qb, embed, probs=buf)
+        ctx.save_for_backward(qp, qb, embed, out, probs, *srcs)
+        ctx.heads, ctx.c, ctx.where = heads, c, where
+        return out
+
+    @staticmethod
+    def backward(ctx, grad):
+        qp, qb, embed, out, probs, *srcs = ctx.saved_tensors
+        c, where = ctx.c, ctx.where
+        q, k, v = (srcs[i][:, col:col + c] for i, col in where)
+        gsrc, (gq, gk, gv) = _source_grads(srcs, where, c)
+        n_qp, n_qb, n_e = ctx.needs_input_grad[3:6]
+        item = dict(q=q, k=k, v=v, out=out, probs=probs, grad_out=grad.contiguous(), qp=qp, qb=qb, embed=embed, grad_q=gq, grad_k=gk,
+                    grad_v=gv, structure=n_qp or n_qb or n_e)
+        g = attention_backward_batched([item], ctx.heads)[0]
+        return (None, None, None, g[3] if n_qp else None, g[4] if n_qb else None, g[5] if n_e else None,
+                *(gs if need else None for gs, need in zip(gsrc, ctx.needs_input_grad[6:])))
+
+
 def head_project(q, wp_t, bp, heads):
-    """qp[n,h,:] = Wp[h*d:(h+1)*d, :]^T q[n,h*d:(h+1)*d]  and  qb[n,h] = q_h . bp_h   (proj_p moved onto q)."""
+    """qp[n,h,:] = Wp[h*d:(h+1)*d, :]^T q[n,h*d:(h+1)*d]  and  qb[n,h] = q_h . bp_h   (proj_p moved onto q).  Differentiable w.r.t. q,
+    wp_t and bp (``head_project_backward``); wp_t may then be the transposed view ``proj_p.weight.t()``."""
+    if _needs_grad(q, wp_t, bp):
+        base, r0, col = _column_source(q)
+        src = base if (r0 == 0 and q.shape[0] == base.shape[0]) else base[r0:r0 + q.shape[0]]
+        return _HeadProject.apply(src, col, int(q.shape[1]), wp_t, bp, int(heads))
+    return _head_project(q, wp_t, bp, heads)
+
+
+def _head_project(q, wp_t, bp, heads):
+    q, wp_t, bp = _detach(q), _detach(wp_t), _detach(bp)
     _rows(q, 'q')
     n, c = q.shape
     d = c // heads
@@ -793,8 +1010,63 @@ def head_project(q, wp_t, bp, heads):
     return qp, qb
 
 
+def head_project_backward(q, wp, bp, heads, grad_qp, grad_qb, need_q=True, need_wp=True, need_bp=True, grad_q=None):
+    """(grad_q (n, C), grad_wp (C, C), grad_bp (C,)) of ``head_project`` with wp = proj_p.weight (the transpose of its wp_t).  grad_q
+    runs through the forward's batched GEMM (into the given ``grad_q`` view, a column slice allowed), grad_wp / grad_bp are
+    fixed-order sums over the rows.  An output not requested is None."""
+    q, wp, bp = _rows(_detach(q), 'q'), _detach(wp), _detach(bp)
+    _f(wp, 'wp'); _f(bp, 'bp'); _f(grad_qp, 'grad_qp'); _f(grad_qb, 'grad_qb')
+    n, c = q.shape
+    if tuple(wp.shape) != (c, c) or tuple(grad_qp.shape) != (n, heads, c) or tuple(grad_qb.shape) != (n, heads):
+        raise RuntimeError(f'head_project_backward: wp must be ({c}, {c}), grad_qp ({n}, {heads}, {c}) and grad_qb ({n}, {heads})')
+    dev = q.device
+    gq = (torch.empty((n, c), dtype=_f32, device=dev) if grad_q is None else grad_q) if need_q else None
+    if gq is not None and (tuple(gq.shape) != (n, c) or gq.dtype != _f32 or gq.stride(1) != 1 or not gq.is_cuda):
+        raise RuntimeError(f'head_project_backward: grad_q must be a ({n}, {c}) float32 CUDA view with unit inner stride')
+    gw = torch.empty((c, c), dtype=_f32, device=dev) if need_wp else None
+    gb = torch.empty((c,), dtype=_f32, device=dev) if need_bp else None
+    lib = L.lib()
+    ws = L.workspace(lib.geob200_head_project_backward_workspace_bytes(n, c, heads), dev, 'head_project_backward')
+    L.check(lib.geob200_head_project_backward(q.data_ptr(), q.stride(0), wp.data_ptr(), bp.data_ptr(), n, c, heads, grad_qp.data_ptr(),
+                                              grad_qb.data_ptr(), L.ptr(gq), c if gq is None else gq.stride(0), L.ptr(gw), L.ptr(gb),
+                                              ws.data_ptr(), ws.numel(),
+                                              L.stream_ptr()), 'head_project_backward')
+    return gq, gw, gb
+
+
+class _HeadProject(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, src, col, c, wp_t, bp, heads):
+        qp, qb = _head_project(src[:, col:col + c], wp_t.contiguous(), bp, heads)
+        ctx.save_for_backward(src, wp_t, bp)
+        ctx.col, ctx.c, ctx.heads = col, c, heads
+        return qp, qb
+
+    @staticmethod
+    def backward(ctx, grad_qp, grad_qb):
+        src, wp_t, bp = ctx.saved_tensors
+        col, c = ctx.col, ctx.c
+        q = src[:, col:col + c]
+        n = q.shape[0]
+        grad_qp = torch.zeros((n, ctx.heads, c), dtype=_f32, device=q.device) if grad_qp is None else grad_qp.contiguous()
+        grad_qb = torch.zeros((n, ctx.heads), dtype=_f32, device=q.device) if grad_qb is None else grad_qb.contiguous()
+        nq, nw, nb = ctx.needs_input_grad[0], ctx.needs_input_grad[3], ctx.needs_input_grad[4]
+        gsrc, (gq,) = _source_grads([src], [(0, col)], c) if nq else ([None], [None])
+        _, gw, gb = head_project_backward(q, wp_t.t().contiguous(), bp, ctx.heads, grad_qp, grad_qb, nq, nw, nb, grad_q=gq)
+        return gsrc[0], None, None, (gw.t() if gw is not None else None), gb, None
+
+
 def add_layernorm(a, b, weight, bias, eps=1e-5, out=None):
-    weight, bias = _detach(weight), _detach(bias)
+    """y = LayerNorm(a + b) (b may be None).  Differentiable w.r.t. a, b, weight and bias (``add_layernorm_backward``); with ``out``
+    the result is copied into it, which then carries the graph."""
+    if _needs_grad(a, b, weight, bias):
+        y = _AddLayerNorm.apply(a, b, weight, bias, float(eps))
+        return y if out is None else out.copy_(y)
+    return _add_layernorm(a, b, weight, bias, eps, out)
+
+
+def _add_layernorm(a, b, weight, bias, eps=1e-5, out=None):
+    a, b, weight, bias = _detach(a), _detach(b), _detach(weight), _detach(bias)
     L.require_cuda(a, 'a', _f32)
     if b is not None:
         L.require_cuda(b, 'b', _f32)
@@ -807,11 +1079,79 @@ def add_layernorm(a, b, weight, bias, eps=1e-5, out=None):
     return y
 
 
+def add_layernorm_backward(a, b, weight, grad_y, eps=1e-5, need_weight=True, need_bias=True):
+    """(grad_x, grad_weight, grad_bias) of ``add_layernorm``: grad_x is the gradient of both summands; the statistics are recomputed
+    from a + b.  grad_weight / grad_bias are fixed-order sums over the rows (None when not requested)."""
+    a, b, weight = _detach(a), _detach(b), _detach(weight)
+    L.require_cuda(a, 'a', _f32); _f(weight, 'weight'); _f(grad_y, 'grad_y')
+    if b is not None:
+        L.require_cuda(b, 'b', _f32)
+    n, c = a.shape
+    if tuple(grad_y.shape) != (n, c) or (b is not None and tuple(b.shape) != (n, c)) or weight.numel() != c:
+        raise RuntimeError(f'add_layernorm_backward: b and grad_y must be ({n}, {c}), weight ({c},)')
+    dev = a.device
+    gx = torch.empty((n, c), dtype=_f32, device=dev)
+    gw = torch.empty((c,), dtype=_f32, device=dev) if need_weight else None
+    gb = torch.empty((c,), dtype=_f32, device=dev) if need_bias else None
+    lib = L.lib()
+    ws = L.workspace(lib.geob200_add_layernorm_backward_workspace_bytes(n, c), dev, 'add_layernorm_backward')
+    L.check(lib.geob200_add_layernorm_backward(a.data_ptr(), L.ptr(b), weight.data_ptr(), n, c, float(eps), grad_y.data_ptr(),
+                                               gx.data_ptr(), L.ptr(gw), L.ptr(gb), ws.data_ptr(), ws.numel(), L.stream_ptr()),
+            'add_layernorm_backward')
+    return gx, gw, gb
+
+
+class _AddLayerNorm(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, a, b, weight, bias, eps):
+        ctx.save_for_backward(a, b, weight)
+        ctx.eps = eps
+        return _add_layernorm(a, b, weight, bias, eps)
+
+    @staticmethod
+    def backward(ctx, grad):
+        a, b, weight = ctx.saved_tensors
+        na, nb, nw, nbias = ctx.needs_input_grad[:4]
+        gx, gw, gb = add_layernorm_backward(a, b, weight, grad.contiguous(), ctx.eps, nw, nbias)
+        return (gx if na else None), (gx if (nb and b is not None) else None), gw, gb, None
+
+
 def l2_normalize(x):
+    """F.normalize(x, p=2, dim=1).  Differentiable w.r.t. x (``l2_normalize_backward``)."""
+    if _needs_grad(x):
+        return _L2Normalize.apply(x)
+    return _l2_normalize(x)
+
+
+def _l2_normalize(x):
+    x = _detach(x)
     _f(x, 'x')
     y = torch.empty_like(x)
     L.check(L.lib().geob200_l2_normalize(x.data_ptr(), x.shape[0], x.shape[1], y.data_ptr(), L.stream_ptr()), 'l2_normalize')
     return y
+
+
+def l2_normalize_backward(x, grad_y):
+    """grad_x of ``l2_normalize``, with the max(|x|, 1e-12) clamp of F.normalize (below it the gradient is grad_y / 1e-12)"""
+    x = _detach(x)
+    _f(x, 'x'); _f(grad_y, 'grad_y')
+    if grad_y.shape != x.shape or x.dim() != 2:
+        raise RuntimeError('l2_normalize_backward: x and grad_y must be the same (n, C) shape')
+    gx = torch.empty_like(x)
+    L.check(L.lib().geob200_l2_normalize_backward(x.data_ptr(), x.shape[0], x.shape[1], grad_y.data_ptr(), gx.data_ptr(), L.stream_ptr()),
+            'l2_normalize_backward')
+    return gx
+
+
+class _L2Normalize(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x):
+        ctx.save_for_backward(x)
+        return _l2_normalize(x)
+
+    @staticmethod
+    def backward(ctx, grad):
+        return l2_normalize_backward(ctx.saved_tensors[0], grad.contiguous())
 
 
 # ------------------------------------------------------------------------------------------------ matching

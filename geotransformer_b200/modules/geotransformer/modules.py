@@ -34,6 +34,11 @@ class GeometricStructureEmbedding(nn.Module):
         c = self.proj_d.out_features
         if GF.GSE_MODE != 5 or c not in (128, 256):
             return None
+        return self._weights_table()
+
+    def _weights_table(self):
+        """the version-keyed table of ``table`` whatever GF.GSE_MODE: the structure embedding's backward picks the winning angle
+        term with its lookups"""
         params = (self.proj_d.weight, self.proj_d.bias, self.proj_a.weight, self.proj_a.bias)
         key = tuple((p.data_ptr(), p._version) for p in params) + (GF.GSE_TABLE_INV_STEP, GF.GSE_TABLE_D_MAX, float(self.sigma_a))
         hit = self._table
@@ -59,7 +64,8 @@ class GeometricStructureEmbedding(nn.Module):
 
     def forward(self, points, scratch_tag=None):
         """``scratch_tag``: write E into the grow-only scratch buffer of that name (valid until the next call with the same
-        tag on this stream) instead of a fresh allocation; used by GeometricTransformer for its two embeddings."""
+        tag on this stream) instead of a fresh allocation; used by GeometricTransformer for its two embeddings.  E carries no
+        graph: ``forward_grad`` is the differentiable form."""
         squeeze = points.ndim == 3
         if squeeze and points.shape[0] != 1:
             raise NotImplementedError('one cloud per call (the reference model always passes B=1)')
@@ -72,6 +78,17 @@ class GeometricStructureEmbedding(nn.Module):
         emb = GF.gse_embed(d, a, self.embedding.div_term, self.proj_d.weight.detach(), self.proj_a.weight.detach(),
                            self.proj_d.bias.detach(), self.proj_a.bias.detach(), wd_t, wa_t, out=out, table=self.table())
         return emb.unsqueeze(0) if squeeze else emb
+
+    def forward_grad(self, points):
+        """``forward`` of one (N, 3) cloud with the graph to proj_d / proj_a (when they require grad in grad mode): E is a fresh tensor
+        the backward keeps (not a scratch view), computed by the same kernels, so its values are ``forward``'s bit for bit.  GeometricTransformer uses it in grad
+        mode; the backward takes the winning angle terms from the table of the current weights whatever GF.GSE_MODE."""
+        pts = points.contiguous()
+        d, a = GF.gse_indices(pts, self.sigma_d, self.sigma_a, self.angle_k)
+        wd_t = self._cache.get('wd_t', self.proj_d.weight, lambda w: w.t().contiguous())
+        wa_t = self._cache.get('wa_t', self.proj_a.weight, lambda w: w.t().contiguous())
+        return GF.gse_embed(d, a, self.embedding.div_term, self.proj_d.weight, self.proj_a.weight, self.proj_d.bias, self.proj_a.bias,
+                            wd_t, wa_t, table=self._weights_table())
 
 
 class GeometricTransformer(nn.Module):
@@ -92,8 +109,13 @@ class GeometricTransformer(nn.Module):
         batched = ref_points.ndim == 3
         if batched:
             ref_points, src_points, ref_feats, src_feats = ref_points[0], src_points[0], ref_feats[0], src_feats[0]
-        ref_emb = self.embedding(ref_points, scratch_tag='gse_ref')     # consumed inside this forward only
-        src_emb = self.embedding(src_points, scratch_tag='gse_src')
+        if GF._needs_grad(ref_feats, src_feats, *self.parameters()):
+            # the graph's attention nodes keep E: fresh tensors, never the scratch the next forward overwrites (also with a frozen
+            # embedding, when forward_grad runs the no-grad kernels into a fresh tensor)
+            ref_emb, src_emb = self.embedding.forward_grad(ref_points), self.embedding.forward_grad(src_points)
+        else:
+            ref_emb = self.embedding(ref_points, scratch_tag='gse_ref')     # consumed inside this forward only
+            src_emb = self.embedding(src_points, scratch_tag='gse_src')
         n0, n1 = ref_feats.shape[0], src_feats.shape[0]
         # both clouds share every weight: keep them stacked [ref; src] through the whole transformer
         x = torch.empty((n0 + n1, self.in_proj.out_features), dtype=torch.float32, device=ref_feats.device)

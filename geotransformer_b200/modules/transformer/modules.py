@@ -242,7 +242,10 @@ class RPEConditionalTransformer(nn.Module):
     def forward_stacked(self, x, n0, embeddings0, embeddings1):
         """Same computation on the stacked features [feats0; feats1] (they share every layer's weights): the q|k|v
         projections of both clouds are ONE GEMM, the attention kernel reads them as column slices, and the
-        Linear/LayerNorm/FFN tail runs once per layer on all rows."""
+        Linear/LayerNorm/FFN tail runs once per layer on all rows.  In grad mode the same kernels build the autograd graph
+        (``_forward_stacked_grad``)."""
+        if GF._needs_grad(x, embeddings0, embeddings1, *self.parameters()):
+            return self._forward_stacked_grad(x, n0, embeddings0, embeddings1)
         if not hasattr(self, '_cache'):
             self._cache = _WeightCache()
         c = x.shape[1]
@@ -276,3 +279,43 @@ class RPEConditionalTransformer(nn.Module):
                 _tail(layer, hid1, x[n0:], out=y[n0:])
                 x = y
         return x
+
+    def _forward_stacked_grad(self, x, n0, embeddings0, embeddings1):
+        """``forward_stacked`` with the graph: the fused projection weights are concatenated from the parameters (autograd splits
+        their gradient back onto proj_q / proj_k / proj_v), proj_p enters head_project as its transposed view, and the two clouds'
+        halves are fresh tensors stacked by torch.cat (no in-place write into a tensor whose view a backward has saved).  Every
+        kernel is the no-grad path's, so the values are bit-identical."""
+        for i in range(len(self.blocks)):
+            x = self._layer_grad(i, x, n0, embeddings0, embeddings1)
+        return x
+
+    def _layer_grad(self, i, x, n0, embeddings0, embeddings1):
+        """layer i of ``_forward_stacked_grad`` on the stacked rows x"""
+        c = x.shape[1]
+        block, layer = self.blocks[i], self.layers[i]
+        mha = layer.attention.attention
+        h = mha.num_heads
+        if block == 'self':
+            w, b = _concat(mha, ('proj_q', 'proj_k', 'proj_v'))
+            qkv = GF.linear(x, w, b)                                          # (N0+N1, 3C)
+            q, k, v = qkv[:, :c], qkv[:, c:2 * c], qkv[:, 2 * c:]
+            qp, qb = GF.head_project(q, mha.proj_p.weight.t(), mha.proj_p.bias, h)
+            hid0 = GF.attention(q[:n0], k[:n0], v[:n0], h, qp=qp[:n0], qb=qb[:n0], embed=embeddings0)
+            hid1 = GF.attention(q[n0:], k[n0:], v[n0:], h, qp=qp[n0:], qb=qb[n0:], embed=embeddings1)
+            x = _tail(layer, torch.cat([hid0, hid1]), x)
+        else:
+            wkv, bkv = _concat(mha, ('proj_k', 'proj_v'))
+            q0 = GF.linear(x[:n0], mha.proj_q.weight, mha.proj_q.bias)
+            kv1 = GF.linear(x[n0:], wkv, bkv)
+            y0 = _tail(layer, GF.attention(q0, kv1[:, :c], kv1[:, c:], h), x[:n0])
+            mem = x[:n0] if self.parallel else y0
+            q1 = GF.linear(x[n0:], mha.proj_q.weight, mha.proj_q.bias)
+            kv0 = GF.linear(mem, wkv, bkv)
+            y1 = _tail(layer, GF.attention(q1, kv0[:, :c], kv0[:, c:], h), x[n0:])
+            x = torch.cat([y0, y1])
+        return x
+
+
+def _concat(mha, names):
+    """the fused projection weight / bias of ``_fused``, concatenated from the parameters themselves (with their graph)"""
+    return (torch.cat([getattr(mha, n).weight for n in names], dim=0), torch.cat([getattr(mha, n).bias for n in names], dim=0))

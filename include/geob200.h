@@ -284,6 +284,45 @@ int geob200_add_layernorm(const float* a, const float* b, const float* gamma, co
 /* F.normalize(x, p=2, dim=1) */
 int geob200_l2_normalize(const float* x, int64_t n, int64_t channels, float* y, void* stream);
 
+/* ---- geometric transformer: backward ----------------------------------------------------------------------- */
+/* No float atomics: two runs give the same bits.  Sums over rows run on fixed row chunks folded in chunk order in double. */
+
+/* y = LayerNorm(a + b) gamma + beta: grad_x (n, C) is the gradient of both summands; the statistics are recomputed per row from
+ * a + b (b may be NULL).  grad_gamma / grad_beta may be NULL.  channels <= 1024. */
+size_t geob200_add_layernorm_backward_workspace_bytes(int64_t n, int64_t channels);
+int geob200_add_layernorm_backward(const float* a, const float* b, const float* gamma, int64_t n, int64_t channels, float eps,
+                                   const float* grad_y, float* grad_x, float* grad_gamma, float* grad_beta, void* workspace,
+                                   size_t workspace_bytes, void* stream);
+/* y = x / max(|x|, 1e-12) per row: grad_x (n, C); needs no workspace. */
+int geob200_l2_normalize_backward(const float* x, int64_t n, int64_t channels, const float* grad_y, float* grad_x, void* stream);
+/* head_project (qp[n,h,:] = Wp_h^T q_h, qb[n,h] = q_h . bp_h, Wp_h = rows h d .. h d + d - 1 of the nn.Linear weight wp (C, C)):
+ * grad_q (row stride ldgq, may be a column slice) through geob200_linear_batched over heads, grad_wp (C, C) and grad_bp (C) as
+ * fixed-order row sums.  Each output may be NULL. */
+size_t geob200_head_project_backward_workspace_bytes(int64_t n, int64_t channels, int64_t heads);
+int geob200_head_project_backward(const float* q, int64_t ldq, const float* wp, const float* bp, int64_t n, int64_t channels, int64_t heads,
+                                  const float* grad_qp, const float* grad_qb, float* grad_q, int64_t ldgq, float* grad_wp, float* grad_bp,
+                                  void* workspace, size_t workspace_bytes, void* stream);
+/* Attention backward for the items of a forward (geob200_att_item_t: the forward's inputs, `out` its output with row stride ldo).
+ * Per item: probs = the (n_query, H, n_key) softmax probabilities the streaming forward leaves in its workspace, grad_out the
+ * (n_query, C) contiguous upstream gradient; grad_q / grad_k / grad_v (row strides ldgq / ldgk / ldgv: column slices of one fused
+ * gradient allowed; each may be NULL) and, for self-attention items, grad_qp (n_query, H, C), grad_qb (n_query, H) and
+ * grad_embed (n_query, n_key, C) (grad_qp and grad_embed together; NULL skips the E pass).  channels 128 or 256. */
+typedef struct { const float* probs; const float* grad_out; float* grad_q; float* grad_k; float* grad_v; float* grad_qp; float* grad_qb;
+                 float* grad_embed; } geob200_att_grad_item_t;
+size_t geob200_attention_backward_batched_workspace_bytes(const geob200_att_item_t* items_h, int64_t n_items, int64_t heads);
+int geob200_attention_backward_batched(const geob200_att_item_t* items_h, const geob200_att_grad_item_t* grads_h, int64_t n_items,
+                                       int64_t ldq, int64_t ldk, int64_t ldv, int64_t ldo, int64_t ldgq, int64_t ldgk, int64_t ldgv,
+                                       int64_t channels, int64_t heads, void* workspace, size_t workspace_bytes, void* stream);
+/* Structure embedding E = proj_d(s(d)) + max_k proj_a(s(a_k)) given grad_embed (n_rows, C): grad_wd / grad_wa (C, C, nn.Linear
+ * layout) and grad_bd = grad_ba (C).  The winning angle term of every (row, channel) comes from the lookups of
+ * geob200_gse_embed_table with the table of the current weights (same table arguments); the sinusoid is evaluated with sincosf.
+ * channels 128 or 256, angle_k 3. */
+size_t geob200_gse_embed_backward_workspace_bytes(int64_t n_rows, int64_t channels);
+int geob200_gse_embed_backward(const float* d_indices, const float* a_indices, int64_t n_rows, int64_t angle_k, int64_t channels,
+                               const void* table, size_t table_bytes, int64_t inv_step, float d_max, float a_max, const float* div_term,
+                               const float* wa, const float* ba, const float* grad_embed, float* grad_wd, float* grad_bd, float* grad_wa,
+                               float* grad_ba, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- matching ---------------------------------------------------------------------------------------------- */
 
 /* SuperPointMatching.forward (superpoint_matching.py:13-50): ref_feats / ref_masks hold the superpoint rows of the B ref clouds,
