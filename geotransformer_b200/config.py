@@ -39,6 +39,8 @@ def _base(seed=7351):
     c.loss = Cfg(weight_coarse_loss=1.0, weight_fine_loss=1.0)
     # correspondence RANSAC of eval.py --method ransac (experiments/*/config.py, _C.ransac); seed keys the sampler
     c.ransac = Cfg(distance_threshold=0.05, num_points=3, num_iterations=1000, seed=0)
+    # training (experiments/*/config.py, _C.optim; train.batch_size = 1): Adam with L2 weight decay; the schedule per experiment
+    c.optim = Cfg(lr=1e-4, weight_decay=1e-6, grad_acc_steps=1)
     return c
 
 
@@ -53,6 +55,7 @@ def make_cfg(name='3dmatch'):
         c.fine_matching.update(topk=3, acceptance_radius=0.1)
         c.eval.update(acceptance_radius=0.1, rmse_threshold=0.2, rre_threshold=15.0, rte_threshold=0.3)
         c.neighbor_limits = [38, 36, 36, 38]  # reference demo.py:52
+        c.optim.update(lr_decay=0.95, lr_decay_steps=1, max_epoch=40)            # StepLR per epoch
     elif name == 'kitti':
         c.backbone.update(num_stages=5, init_voxel_size=0.3, base_radius=4.25)
         c.model.update(ground_truth_matching_radius=0.6, num_points_in_patch=128, fine_level=1)
@@ -63,6 +66,7 @@ def make_cfg(name='3dmatch'):
         c.coarse_loss.log_scale = 40
         c.fine_loss.positive_radius = 0.6
         c.ransac.update(distance_threshold=0.3, num_points=4, num_iterations=50000)
+        c.optim.update(lr_decay=0.95, lr_decay_steps=4, max_epoch=160)           # StepLR per epoch
         c.neighbor_limits = None  # calibrated (reference utils/data.py:192-217)
     elif name == 'modelnet':
         c.backbone.update(num_stages=3, init_voxel_size=0.05, base_radius=2.5)
@@ -71,6 +75,7 @@ def make_cfg(name='3dmatch'):
         c.geotransformer.update(input_dim=512, hidden_dim=256, sigma_d=0.2)
         c.fine_matching.update(topk=3, acceptance_radius=0.1)
         c.eval.update(acceptance_radius=0.1, rre_threshold=1.0, rte_threshold=0.1)
+        c.optim.update(warmup_steps=10000, eta_init=0.1, eta_min=0.1, max_iteration=400000)   # warm-up cosine per iteration
         c.neighbor_limits = None
     else:
         raise ValueError(f'unknown config {name}')

@@ -8,6 +8,7 @@
 // shared memory; nothing but the input scores and the final log-assignment touches HBM.
 #include "common.cuh"
 #include "geob200.h"
+#include "radix_select.cuh"
 
 namespace geob200 {
 
@@ -190,34 +191,9 @@ __global__ void __launch_bounds__(1024) topk_flat_kernel(const float* __restrict
     // rows past the number of existing candidates are padding: index -1 (gather_patches turns it into an empty patch)
     for (int i = k + threadIdx.x; i < k_req; i += blockDim.x) { ref_out[i] = -1; src_out[i] = -1; score_out[i] = 0.f; }
     if (k == 0) { if (threadIdx.x == 0) *k_out = 0; return; }
-    unsigned prefix = 0, mask = 0;
-    int remaining = k;
-    for (int shift = 24; shift >= 0; shift -= 8) {
-        for (int i = threadIdx.x; i < 256; i += blockDim.x) hist[i] = 0;
-        __syncthreads();
-        for (long long t = threadIdx.x; t < total; t += blockDim.x) {
-            const unsigned b = __float_as_uint(flat[t]);
-            if ((b & mask) == prefix) atomicAdd(&hist[(b >> shift) & 255u], 1u);
-        }
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            int rem = remaining;
-            int d = 255;
-            for (; d > 0; --d) {
-                if ((int)hist[d] >= rem) break;
-                rem -= (int)hist[d];
-            }
-            prefix_s = prefix | ((unsigned)d << shift);
-            kth_s = (unsigned)rem;
-        }
-        __syncthreads();
-        prefix = prefix_s;
-        remaining = (int)kth_s;
-        mask |= (255u << shift);
-        __syncthreads();
-    }
-    const unsigned thr = prefix;          // bit pattern of the k-th largest value
-    const int need_eq = remaining;        // how many ties at the threshold are kept (lowest flat indices)
+    unsigned thr;          // bit pattern of the k-th largest value
+    int need_eq;           // how many ties at the threshold are kept (lowest flat indices)
+    radix_select_kth(total, k, [&](long long t) { return __float_as_uint(flat[t]); }, hist, &prefix_s, &kth_s, thr, need_eq);
     const int n_gt = k - need_eq;
     if (threadIdx.x == 0) { carry_gt = 0; carry_eq = 0; }
     __syncthreads();

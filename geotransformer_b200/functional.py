@@ -2207,3 +2207,76 @@ def weighted_procrustes_counts(src_points, ref_points, weights, counts, weight_t
                                                        float(weight_thresh), float(eps), T.data_ptr(), L.stream_ptr()),
             'weighted_procrustes_counts')
     return T
+
+
+# ------------------------------------------------------------------------------------------------ training step
+# The ground-truth superpoint targets of the training-mode forward and the non-finite gradient guard (csrc/train.cu).  Neither
+# reads anything back to the host.
+
+def superpoint_targets_batched(gt_indices, gt_overlaps, gt_count, cloud_nodes, overlap_threshold, num_targets, seed, iteration,
+                               pair_base=0):
+    """SuperPointTargetGenerator of B pairs on the stacked output of ``node_correspondences_batched``: (corr (2B, num_targets) int64
+    -- row p ref / row B + p src indices of pair p, scores (B, num_targets) = the selected overlaps, counts (B,) device int32), the
+    layout of ``superpoint_matching_batched``.  Pair p takes all of its gt rows with overlap > ``overlap_threshold`` in gt order when
+    there are at most ``num_targets``, else a uniform subset of ``num_targets`` of them drawn from the Philox stream
+    (seed, iteration, pair_base + p), in gt order."""
+    L.require_cuda(gt_indices, 'gt_indices', _i64); _f(gt_overlaps, 'gt_overlaps'); L.require_cuda(gt_count, 'gt_count', _i32)
+    B = len(cloud_nodes) // 2
+    if B < 1 or len(cloud_nodes) != 2 * B:
+        raise RuntimeError('superpoint_targets_batched: cloud_nodes must hold 2B counts')
+    if gt_indices.ndim != 2 or gt_indices.shape[1] != 2:
+        raise RuntimeError(f'superpoint_targets_batched: gt_indices must be (R, 2), got {tuple(gt_indices.shape)}')
+    if gt_count.numel() < B:
+        raise RuntimeError(f'superpoint_targets_batched: gt_count must hold {B} counts')
+    nn = sum(int(cloud_nodes[p]) * int(cloud_nodes[B + p]) for p in range(B))
+    _min_rows(gt_indices, nn, 'gt_indices')
+    _min_rows(gt_overlaps, nn, 'gt_overlaps')
+    seed, iteration = int(seed), int(iteration)
+    if not (0 <= seed < 1 << 64 and 0 <= iteration < 1 << 64):
+        raise ValueError('superpoint_targets_batched: seed and iteration must be 64-bit unsigned integers')
+    k = int(num_targets)
+    dev = gt_indices.device
+    lib = L.lib()
+    ws = L.workspace(lib.geob200_superpoint_targets_batched_workspace_bytes(nn), dev, tag='superpoint_targets')
+    corr = torch.empty((2 * B, k), dtype=_i64, device=dev)
+    sc = torch.empty((B, k), dtype=_f32, device=dev)
+    cnt = torch.empty((B,), dtype=_i32, device=dev)
+    L.check(lib.geob200_superpoint_targets_batched(gt_indices.data_ptr(), gt_overlaps.data_ptr(), gt_count.data_ptr(), B,
+                                                   _host_i64(cloud_nodes), float(overlap_threshold), k, seed, iteration, int(pair_base),
+                                                   corr.data_ptr(), sc.data_ptr(), cnt.data_ptr(), ws.data_ptr(), ws.numel(),
+                                                   L.stream_ptr()), 'superpoint_targets_batched')
+    return corr, sc, cnt
+
+
+_NF_TABLES = {}
+
+
+def nonfinite_check(tensors, found_inf=None):
+    """0-dim (or 1-element) fp32 device tensor ``found_inf`` = 1.0 when any element of the fp32 CUDA ``tensors`` is NaN or +-Inf, else 0.0; one
+    launch.  The device table of (pointer, numel) is cached per set of tensors and refreshed by a non-blocking copy when their
+    storage moves, so the call never waits for the device."""
+    tensors = list(tensors)
+    if not tensors:
+        raise ValueError('nonfinite_check: no tensors')
+    for i, t in enumerate(tensors):
+        _f(t, f'tensors[{i}]')
+    dev = tensors[0].device
+    if any(t.device != dev for t in tensors):
+        raise RuntimeError('nonfinite_check: all tensors must be on one device')
+    if found_inf is None:
+        found_inf = torch.empty((), dtype=_f32, device=dev)        # 0-dim: the form torch's fused Adam takes as ``found_inf``
+    _f(found_inf, 'found_inf')
+    if found_inf.numel() != 1 or found_inf.device != dev:
+        raise RuntimeError('nonfinite_check: found_inf must be a 1-element float32 tensor on the tensors\' device')
+    key = (dev, tuple((t.data_ptr(), t.numel()) for t in tensors))
+    table = _NF_TABLES.get(key)
+    if table is None:
+        host = torch.tensor([p for p, _ in key[1]] + [n for _, n in key[1]], dtype=_i64).pin_memory()
+        table = host.to(dev, non_blocking=True)          # the pinned block is held by the host allocator until the copy is done
+        if len(_NF_TABLES) > 64:
+            _NF_TABLES.clear()
+        _NF_TABLES[key] = table
+    n = len(tensors)
+    L.check(L.lib().geob200_nonfinite_check(table.data_ptr(), table[n:].data_ptr(), n, max(t.numel() for t in tensors),
+                                            found_inf.data_ptr(), L.stream_ptr()), 'nonfinite_check')
+    return found_inf

@@ -235,6 +235,75 @@ class GeoTransformer(nn.Module):
         main.synchronize()
         return trim_outputs(outs)
 
+    def forward_train(self, data_dict, seed, iteration, targets=None):
+        """The reference's training-mode forward (``experiments/*/model.py``, step 7 "Random select ground truth node
+        correspondences during training") of ONE pair (``data_dict['batch_size']`` must be 1, as the reference trains).
+
+        Grouping and ground-truth superpoint correspondences as ``forward_batch``; the backbone and the transformer through the
+        modules (the native drivers carry no graph), so ``ref_feats_c`` / ``src_feats_c`` / ``matching_scores`` carry the graph
+        to every parameter.  ``ref_/src_node_corr_indices`` hold the superpoint matching (no graph, as the reference; the Evaluator's
+        PIR reads them), while the fine-matching patches come from ``superpoint_targets_batched``: at most
+        ``cfg.coarse_matching.num_targets`` gt correspondences with overlap > ``overlap_threshold``, drawn from the Philox stream
+        (``seed``, ``iteration``, pair 0).  ``targets`` = (ref indices (k',), src indices (k',), overlaps (k',)) replaces the draw.
+        LGR runs on the detached scores.  Returns one output dict with full-capacity buffers and the device counts under
+        ``_counts``: ``node_corr`` = the target patches (rows of the patch tensors, ``node_corr_scores``, ``matching_scores``),
+        ``coarse`` = the superpoint matching rows, ``corr`` = LGR, ``gt`` = ground truth.  No host synchronisation."""
+        if int(data_dict.get('batch_size', 1)) != 1:
+            raise ValueError('forward_train: one pair per training forward (data_dict["batch_size"] must be 1)')
+        transform = data_dict.get('transform')
+        if transform is None:
+            raise ValueError('forward_train: the training forward needs the ground-truth transform')
+        dev = data_dict['features'].device
+        if targets is not None:
+            targets = _forced_node_corr(targets, dev)
+        lens_h = data_dict.get('lengths_host') or [l.tolist() for l in data_dict['lengths']]
+        fl, K = self.fine_level, self.num_points_in_patch
+        cn, cf, c0 = [int(v) for v in lens_h[-1]], [int(v) for v in lens_h[fl]], [int(v) for v in lens_h[0]]
+        points_c, points_f, points0 = data_dict['points'][-1], data_dict['points'][fl], data_dict['points'][0]
+        transforms = transform.reshape(1, 4, 4).contiguous()
+        n0, nf, np0 = cn[0], cf[0], c0[0]
+
+        _, node_masks, knn_idx, knn_masks = GF.point_to_node_partition_batched(points_f, points_c, cf, cn, K)
+        _, _, all_pts = GF.gather_patches_batched(None, 0, cn, cf, knn_idx, knn_masks, points_f)
+        gt_idx, gt_ov, gt_cnt = GF.node_correspondences_batched(points_c, all_pts, node_masks, knn_masks, cn, transforms,
+                                                                self.matching_radius)
+
+        feats_list = self.backbone(data_dict['features'], data_dict)
+        feats_c, feats_f = feats_list[-1], feats_list[0]
+        rc, sc = self.transformer(points_c[:n0].contiguous(), points_c[n0:].contiguous(), feats_c[:n0], feats_c[n0:])
+        y_n = GF.l2_normalize(torch.cat([rc, sc]))
+
+        cm, fm = self.coarse_matching, self.fine_matching
+        with torch.no_grad():
+            m_corr, _, m_count = GF.superpoint_matching_batched(y_n.detach(), node_masks, cn, cm.num_correspondences,
+                                                                cm.dual_normalization)
+            if targets is None:
+                kc = self.cfg.coarse_matching.num_targets
+                corr, node_scores, corr_count = GF.superpoint_targets_batched(
+                    gt_idx, gt_ov, gt_cnt, cn, self.cfg.coarse_matching.overlap_threshold, kc, seed, iteration)
+            else:
+                corr, node_scores = targets
+                kc = corr.shape[1]
+                corr_count = torch.full((1,), kc, dtype=torch.int32, device=dev)
+            k_idx, k_masks, k_pts = GF.gather_patches_batched(corr, kc, cn, cf, knn_idx, knn_masks, points_f)
+        r, s = slice(0, kc), slice(kc, 2 * kc)
+        raw_scores = GF.patch_scores_batched(feats_f, cf, k_idx[r], k_idx[s])
+        scores = self.optimal_transport(raw_scores, k_masks[r], k_masks[s])
+        with torch.no_grad():
+            rcp, scp, cs, T, n_corr = GF.local_global_registration_batched(
+                1, k_pts[r], k_pts[s], k_masks[r], k_masks[s], scores.detach(), fm.k, fm.acceptance_radius, fm.mutual,
+                fm.confidence_threshold, fm.correspondence_threshold, fm.num_refinement_steps)
+        return dict(ref_points_c=points_c[:n0], src_points_c=points_c[n0:], ref_points_f=points_f[:nf], src_points_f=points_f[nf:],
+                    ref_points=points0[:np0], src_points=points0[np0:], ref_feats_c=y_n[:n0], src_feats_c=y_n[n0:],
+                    ref_feats_f=feats_f[:nf], src_feats_f=feats_f[nf:], gt_node_corr_indices=gt_idx, gt_node_corr_overlaps=gt_ov,
+                    ref_node_corr_indices=m_corr[0], src_node_corr_indices=m_corr[1], node_corr_scores=node_scores[0],
+                    ref_node_corr_knn_points=k_pts[r], src_node_corr_knn_points=k_pts[s], ref_node_corr_knn_masks=k_masks[r],
+                    src_node_corr_knn_masks=k_masks[s], matching_scores=scores, ref_corr_points=rcp[0], src_corr_points=scp[0],
+                    corr_scores=cs[0], estimated_transform=T[0].reshape(4, 4),
+                    _counts=dict(node_corr=corr_count[0], coarse=m_count[0], corr=n_corr[0], gt=gt_cnt[0]),
+                    _stacked=dict(gt=(gt_idx, gt_ov, gt_cnt), coarse=(m_corr, m_count), lgr=(rcp, scp, n_corr), transforms=T,
+                                  cloud_nodes=cn, cloud_points=c0, points=points0))
+
     def forward(self, data_dict, taps=None):
         """``forward_batch`` with its defaults: the output dict of a single pair (the reference's contract), the list of output
         dicts for a batch of several pairs.  ``taps`` and ``data_dict['forced_node_corr']``: see ``forward_batch``."""

@@ -667,6 +667,25 @@ int geob200_transformer_forward_batched(const geob200_tlayer_t* layers, int64_t 
                                         const float* x, int64_t n_pairs, const int64_t* cloud_rows_h, const float* const* embeddings_h,
                                         float* out, void* workspace, size_t workspace_bytes, void* stream);
 
+/* Ground-truth superpoint targets of the training-mode forward (SuperPointTargetGenerator, modules/geotransformer/
+ * superpoint_target.py), one CTA per pair.  Inputs: the gt rows of geob200_node_correspondences_batched (indices (R, 2), overlaps
+ * (R,), the first gt_count[p] (device int32) of pair p's n_ref * n_src rows valid, laid out by cloud_nodes (2B counts)).  The
+ * candidates j = 0 .. n-1 are the rows with overlap > overlap_threshold, in gt order.  n <= num_targets: all of them; otherwise the
+ * num_targets smallest keys (philox(seed; j, iteration, pair_base + p) << 32) | j (Philox4x32-10, key = seed, counter = (j,
+ * iteration lo, iteration hi, pair_base + p), word 0), in ascending j.  Outputs in the layout of
+ * geob200_superpoint_matching_batched: corr_indices (2B, num_targets) int64 (row p ref / row B + p src indices of pair p, -1 past
+ * the count), corr_scores (B, num_targets) = the selected overlaps (0 past the count), num_out (B,) device int32. */
+size_t geob200_superpoint_targets_batched_workspace_bytes(int64_t n_gt_rows);
+int geob200_superpoint_targets_batched(const int64_t* gt_indices, const float* gt_overlaps, const int32_t* gt_count, int64_t n_pairs,
+                                       const int64_t* cloud_nodes, float overlap_threshold, int64_t num_targets, uint64_t seed,
+                                       uint64_t iteration, int64_t pair_base, int64_t* corr_indices, float* corr_scores, int32_t* num_out,
+                                       void* workspace, size_t workspace_bytes, void* stream);
+
+/* Gradient guard of the training step: found_inf[0] (device fp32) = 1 when any element of the n_tensors fp32 tensors listed in the
+ * DEVICE tables ptrs / numels is NaN or +-Inf, else 0.  max_numel (host) = the largest numel, sizes the grid.  One launch. */
+int geob200_nonfinite_check(const float* const* ptrs, const int64_t* numels, int64_t n_tensors, int64_t max_numel, float* found_inf,
+                            void* stream);
+
 #ifdef __cplusplus
 }
 #endif
