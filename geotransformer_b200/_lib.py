@@ -144,9 +144,14 @@ _sig('geob200_transformer_batched_workspace_bytes', SZ, I64, P, I64, I64, I64)
 _sig('geob200_transformer_forward_batched', c_int, P, I64, I64, I64, P, I64, P, P, P, P, SZ, P)
 _sig('geob200_attention_batched_workspace_bytes', SZ, P, I64, I64)
 _sig('geob200_attention_batched', c_int, P, I64, I64, I64, I64, I64, I64, I64, P, SZ, P)
+_sig('geob200_attention_batched_keeps_probs', c_int, P, I64, I64, I64)
 _sig('geob200_superpoint_targets_batched_workspace_bytes', SZ, I64)
 _sig('geob200_superpoint_targets_batched', c_int, P, P, P, I64, P, F, I64, ctypes.c_uint64, ctypes.c_uint64, I64, P, P, P, P, SZ, P)
 _sig('geob200_nonfinite_check', c_int, P, P, I64, I64, P, P)
+_sig('geob200_batch_loss_weights', c_int, P, I64, I64, P, P, P, P, P)
+_sig('geob200_kpconv_group_norm_batched', c_int, P, P, P, P, I64, I64, I64, P, I64, P, P, I64, I64, F, I64, P, P, F, c_int, F, P, P, P,
+     SZ, P, SZ, P, I64, P)
+_sig('geob200_maxpool_batched', c_int, P, P, I64, I64, I64, I64, P, I64, P, P, P)
 
 
 def lib():

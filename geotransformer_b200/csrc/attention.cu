@@ -456,6 +456,12 @@ size_t geob200_attention_workspace_bytes(int64_t n_query, int64_t n_key, int64_t
     return (size_t)n_query * (size_t)n_key * (size_t)heads * sizeof(float) + 256;
 }
 
+// whether the streaming path takes an item: C = 128 / 256 and the softmax / P.V kernel's scores of one query tile fit its shared memory
+static bool streaming_fits(int64_t n_key, int64_t channels, int64_t heads) {
+    const size_t smem_pv = sizeof(float) * (ATT_R * heads * (size_t)((n_key + 3) / 4 * 4) + ATT_KQ * ATT_R * channels);
+    return (channels == 128 || channels == 256) && smem_pv <= 200 * 1024;
+}
+
 // Streaming path for a batch of items sharing channels / heads / row strides.  Returns 1 when the shape is not handled by it.
 static int attention_streaming_batch(const geob200_att_item_t* items, int64_t n_items, int64_t ldq, int64_t ldk, int64_t ldv, int64_t ldo,
                                      int64_t channels, int64_t heads, void* workspace, size_t workspace_bytes, cudaStream_t st) {
@@ -474,8 +480,7 @@ static int attention_streaming_batch(const geob200_att_item_t* items, int64_t n_
         GEOB_REQUIRE(((uintptr_t)it.q % 16) == 0 && ((uintptr_t)it.k % 16) == 0 && ((uintptr_t)it.v % 16) == 0 &&
                          (it.qp == nullptr || ((uintptr_t)it.qp % 16) == 0) && (it.embed == nullptr || ((uintptr_t)it.embed % 16) == 0),
                      "attention: q, k, v, qp, embed must be 16-byte aligned");
-        const size_t smem_pv = sizeof(float) * (ATT_R * heads * (size_t)((it.n_key + 3) / 4 * 4) + ATT_KQ * ATT_R * channels);
-        if (smem_pv > 200 * 1024) return 1;
+        if (!streaming_fits(it.n_key, channels, heads)) return 1;
         AttItem& d = b.it[i];
         d.q = it.q; d.k = it.k; d.v = it.v; d.qp = it.qp; d.qb = it.qb; d.E = it.embed; d.out = it.out;
         d.N = (int)it.n_query; d.M = (int)it.n_key;
@@ -520,6 +525,13 @@ static int attention_check(int64_t channels, int64_t heads, int64_t ldq, int64_t
 int geob200_set_attention_tma(int on) {
     g_att_tma = on != 0;
     return 0;
+}
+
+int geob200_attention_batched_keeps_probs(const geob200_att_item_t* items, int64_t n_items, int64_t channels, int64_t heads) {
+    if (items == nullptr || n_items < 1 || n_items > ATT_MAX_ITEMS) return 0;
+    for (int64_t i = 0; i < n_items; ++i)
+        if (items[i].n_query < 1 || items[i].n_key < 1 || !streaming_fits(items[i].n_key, channels, heads)) return 0;
+    return 1;
 }
 
 size_t geob200_attention_batched_workspace_bytes(const geob200_att_item_t* items, int64_t n_items, int64_t heads) {

@@ -1328,3 +1328,36 @@ int maxpool_seg(const float* x, const int64_t* neighbors, int64_t n_query, int64
     return 0;
 }
 }  // namespace geob200
+
+extern "C" {
+
+// KPConv -> GroupNorm -> LeakyReLU with per-pair GroupNorm statistics (rows in stack order, cloud_rows_h[2 * n_pairs]): the
+// epilogue partials of the tensor-core GEMM folded per pair (gn_seg_finalize / gn_seg_apply), the kernels of the batched
+// native backbone.  pre_norm (n_query, c_out) is the caller's and receives the KPConv output.
+int geob200_kpconv_group_norm_batched(const float* s_feats, const float* q_points, const float* s_points, const int64_t* neighbors,
+                                      int64_t n_query, int64_t n_support, int64_t n_neighbors, const float* kernel_points, int64_t n_kernel,
+                                      const float* weights_t, const float* bias, int64_t c_in, int64_t c_out, float sigma, int64_t groups,
+                                      const float* gamma, const float* beta, float eps, int leaky, float slope, float* pre_norm, float* y,
+                                      void* gn_workspace, size_t gn_workspace_bytes, void* workspace, size_t workspace_bytes, void* stream,
+                                      int64_t n_pairs, const int64_t* cloud_rows_h) {
+    geob200::GnSeg seg;
+    if (geob200::make_seg(&seg, n_pairs, cloud_rows_h, n_query, "kpconv_group_norm")) return -2;
+    GEOB_REQUIRE(pre_norm != nullptr && y != nullptr, "kpconv_group_norm: null output");
+    return geob200::kpconv_group_norm_impl(s_feats, q_points, s_points, neighbors, n_query, n_support, n_neighbors, kernel_points, n_kernel,
+                                           weights_t, bias, c_in, c_out, sigma, groups, gamma, beta, eps, leaky, slope, pre_norm, y,
+                                           gn_workspace, gn_workspace_bytes, workspace, workspace_bytes, stream, &seg);
+}
+
+// Max-pool of the batched backbone's strided blocks: pair p's rows see only the first min(n_neighbors, max(cloud_max[p],
+// cloud_max[B + p])) columns of the table (maxpool_seg_kernel, the forward of geob200_maxpool_backward_batched with cloud_max)
+int geob200_maxpool_batched(const float* x, const int64_t* neighbors, int64_t n_query, int64_t n_support, int64_t n_neighbors,
+                            int64_t channels, const int32_t* cloud_max, int64_t n_pairs, const int64_t* cloud_rows_h, float* y,
+                            void* stream) {
+    geob200::GnSeg seg;
+    if (geob200::make_seg(&seg, n_pairs, cloud_rows_h, n_query, "maxpool")) return -2;
+    GEOB_REQUIRE(n_query > 0 && n_support > 0 && n_neighbors > 0 && channels > 0, "maxpool: empty input");
+    GEOB_REQUIRE(x != nullptr && neighbors != nullptr && cloud_max != nullptr && y != nullptr, "maxpool: null pointer");
+    return geob200::maxpool_seg(x, neighbors, n_query, n_support, n_neighbors, channels, y, &seg, cloud_max, stream);
+}
+
+}  // extern "C"

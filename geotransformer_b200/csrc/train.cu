@@ -129,6 +129,37 @@ __global__ void __launch_bounds__(256) nonfinite_check_kernel(const float* const
     if (__syncthreads_or(bad) && threadIdx.x == 0) *found_inf = 1.0f;
 }
 
+// Loss weights of a batched step: one thread walks the B rows in pair order, so the mean is a fixed-order fp32 sum (no atomics).
+// __fmul_rn / __fadd_rn keep the compiler from contracting the sum into FMAs: the numpy restatement rounds every product.
+__global__ void __launch_bounds__(32) batch_loss_weights_kernel(const float* __restrict__ rows, int ld, int B, float* __restrict__ w,
+                                                                float* __restrict__ mean_row, float* __restrict__ n_valid,
+                                                                float* __restrict__ found_inf) {
+    if (threadIdx.x != 0) return;
+    int n = 0;
+    for (int p = 0; p < B; ++p) {
+        const float* r = rows + (long long)p * ld;
+        n += (isfinite(r[0]) && isfinite(r[1]) && isfinite(r[2])) ? 1 : 0;
+    }
+    const float inv = n > 0 ? __fdiv_rn(1.0f, (float)n) : 0.0f;
+    float acc0 = 0.0f, acc1 = 0.0f, acc2 = 0.0f;
+    for (int p = 0; p < B; ++p) {
+        const float* r = rows + (long long)p * ld;
+        const bool ok = isfinite(r[0]) && isfinite(r[1]) && isfinite(r[2]);
+        w[p] = ok ? inv : 0.0f;
+        if (ok) {
+            acc0 = __fadd_rn(acc0, __fmul_rn(inv, r[0]));
+            acc1 = __fadd_rn(acc1, __fmul_rn(inv, r[1]));
+            acc2 = __fadd_rn(acc2, __fmul_rn(inv, r[2]));
+        }
+    }
+    if (n == 0) {
+        acc0 = acc1 = acc2 = __int_as_float(0x7fc00000);      // the mean over no pair is NaN, and the step is skipped
+        *found_inf = 1.0f;
+    }
+    mean_row[0] = acc0; mean_row[1] = acc1; mean_row[2] = acc2;
+    if (n_valid != nullptr) *n_valid = (float)n;
+}
+
 }  // namespace geob200
 
 using namespace geob200;
@@ -181,6 +212,19 @@ int geob200_nonfinite_check(const float* const* ptrs, const int64_t* numels, int
     const unsigned gx = (unsigned)max(1ll, min(per, 4ll * num_sms()));
     GEOB_CHECK_CUDA(cudaMemsetAsync(found_inf, 0, sizeof(float), st));
     nonfinite_check_kernel<<<dim3(gx, (unsigned)n_tensors), 256, 0, st>>>(ptrs, (const long long*)numels, found_inf);
+    GEOB_CHECK_LAUNCH();
+    count_launches(1);
+    return 0;
+}
+
+int geob200_batch_loss_weights(const float* loss_rows, int64_t ld_rows, int64_t n_pairs, float* weights, float* mean_row, float* n_valid,
+                               float* found_inf, void* stream) {
+    GEOB_REQUIRE(n_pairs >= 1 && 2 * n_pairs <= GEOB_MAX_CLOUDS, "batch_loss_weights: 1..%d pairs", GEOB_MAX_CLOUDS / 2);
+    GEOB_REQUIRE(ld_rows >= 3 && ld_rows <= (1ll << 30), "batch_loss_weights: ld_rows must be in 3..2^30");
+    GEOB_REQUIRE(loss_rows != nullptr && weights != nullptr && mean_row != nullptr && found_inf != nullptr,
+                 "batch_loss_weights: null pointer");
+    batch_loss_weights_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(loss_rows, (int)ld_rows, (int)n_pairs, weights, mean_row, n_valid,
+                                                                 found_inf);
     GEOB_CHECK_LAUNCH();
     count_launches(1);
     return 0;

@@ -237,10 +237,13 @@ def split_tf32(weight):
     return out
 
 
-def group_norm(x, weight, bias, groups, eps=1e-5, negative_slope=None, residual=None):
-    """leaky(GroupNorm(x) + residual) over all rows (one pair); differentiable w.r.t. x, weight, bias and residual"""
+def group_norm(x, weight, bias, groups, eps=1e-5, negative_slope=None, residual=None, cloud_rows=None):
+    """leaky(GroupNorm(x) + residual) over all rows (one pair), or with per-pair statistics given ``cloud_rows`` (2B host ints, as
+    ``group_norm_batched``); differentiable w.r.t. x, weight, bias and residual"""
     if _needs_grad(x, weight, bias, residual):
-        return _GroupNorm.apply(x, weight, bias, residual, int(groups), float(eps), negative_slope)
+        return _GroupNorm.apply(x, weight, bias, residual, int(groups), float(eps), negative_slope, cloud_rows)
+    if cloud_rows is not None:
+        return group_norm_batched(x, weight, bias, groups, cloud_rows, eps, negative_slope, _detach(residual))
     return _group_norm(x, weight, bias, groups, eps, negative_slope, residual)
 
 
@@ -274,20 +277,27 @@ def group_norm_backward_batched(x, y, weight, groups, cloud_rows, grad_y, eps=1e
 
 class _GroupNorm(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, weight, bias, residual, groups, eps, negative_slope):
-        y = _group_norm(x, weight, bias, groups, eps, negative_slope, residual)
+    def forward(ctx, x, weight, bias, residual, groups, eps, negative_slope, cloud_rows):
+        if cloud_rows is None:
+            y = _group_norm(x, weight, bias, groups, eps, negative_slope, residual)
+        else:
+            y = group_norm_batched(x, weight, bias, groups, cloud_rows, eps, negative_slope, _detach(residual))
         ctx.save_for_backward(x, y, weight)
-        ctx.args = (groups, eps, negative_slope)
+        ctx.args = (groups, eps, negative_slope, _seg_rows(cloud_rows, x.shape[0]))
         return y
 
     @staticmethod
     def backward(ctx, grad):
         x, y, weight = ctx.saved_tensors
-        groups, eps, slope = ctx.args
+        groups, eps, slope, rows = ctx.args
         need = ctx.needs_input_grad
-        gx, gw, gb, gr = group_norm_backward_batched(x, y, weight, groups, [x.shape[0], 0], grad.contiguous(), eps, slope, need[3], need[1],
-                                                     need[2])
-        return gx if need[0] else None, gw, gb, gr, None, None, None
+        gx, gw, gb, gr = group_norm_backward_batched(x, y, weight, groups, rows, grad.contiguous(), eps, slope, need[3], need[1], need[2])
+        return gx if need[0] else None, gw, gb, gr, None, None, None, None
+
+
+def _seg_rows(cloud_rows, n_rows):
+    """the per-pair row layout the backward entry points take: ``cloud_rows``, or one pair of all rows"""
+    return [n_rows, 0] if cloud_rows is None else [int(r) for r in cloud_rows]
 
 
 def _group_norm(x, weight, bias, groups, eps=1e-5, negative_slope=None, residual=None):
@@ -303,32 +313,39 @@ def _group_norm(x, weight, bias, groups, eps=1e-5, negative_slope=None, residual
     return y
 
 
-def linear_group_norm(x, weight, bias, gn_weight, gn_bias, groups, eps=1e-5, negative_slope=None, residual=None):
-    """UnaryBlock: leaky(GroupNorm(x @ weight.T + bias) + residual); statistics from the GEMM epilogue on the wgmma path.
-    Differentiable w.r.t. every float input (the autograd path keeps its own copy of the pre-norm activation)."""
+def linear_group_norm(x, weight, bias, gn_weight, gn_bias, groups, eps=1e-5, negative_slope=None, residual=None, cloud_rows=None):
+    """UnaryBlock: leaky(GroupNorm(x @ weight.T + bias) + residual); statistics from the GEMM epilogue on the wgmma path, per pair
+    with ``cloud_rows`` (``linear_group_norm_batched``).  Differentiable w.r.t. every float input (the autograd path keeps its own
+    copy of the pre-norm activation)."""
     if _needs_grad(x, weight, bias, gn_weight, gn_bias, residual):
-        return _LinearGroupNorm.apply(x, weight, bias, gn_weight, gn_bias, residual, int(groups), float(eps), negative_slope)
+        return _LinearGroupNorm.apply(x, weight, bias, gn_weight, gn_bias, residual, int(groups), float(eps), negative_slope, cloud_rows)
+    if cloud_rows is not None:
+        return linear_group_norm_batched(x, weight, bias, gn_weight, gn_bias, groups, cloud_rows, eps, negative_slope, _detach(residual))
     return _linear_group_norm(x, weight, bias, gn_weight, gn_bias, groups, eps, negative_slope, residual)
 
 
 class _LinearGroupNorm(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, weight, bias, gn_weight, gn_bias, residual, groups, eps, negative_slope):
+    def forward(ctx, x, weight, bias, gn_weight, gn_bias, residual, groups, eps, negative_slope, cloud_rows):
         pre = torch.empty((x.shape[0], weight.shape[0]), dtype=_f32, device=x.device)
-        y = _linear_group_norm(x, weight, bias, gn_weight, gn_bias, groups, eps, negative_slope, residual, pre=pre)
+        if cloud_rows is None:
+            y = _linear_group_norm(x, weight, bias, gn_weight, gn_bias, groups, eps, negative_slope, residual, pre=pre)
+        else:
+            y = linear_group_norm_batched(x, weight, bias, gn_weight, gn_bias, groups, cloud_rows, eps, negative_slope, _detach(residual),
+                                          pre=pre)
         ctx.save_for_backward(x, weight, gn_weight, pre, y)
-        ctx.args = (groups, eps, negative_slope)
+        ctx.args = (groups, eps, negative_slope, _seg_rows(cloud_rows, pre.shape[0]))
         return y
 
     @staticmethod
     def backward(ctx, grad):
         x, weight, gn_weight, pre, y = ctx.saved_tensors
-        groups, eps, slope = ctx.args
+        groups, eps, slope, rows = ctx.args
         need = ctx.needs_input_grad
-        gpre, ggw, ggb, gr = group_norm_backward_batched(pre, y, gn_weight, groups, [pre.shape[0], 0], grad.contiguous(), eps, slope,
-                                                         need[5], need[3], need[4])
+        gpre, ggw, ggb, gr = group_norm_backward_batched(pre, y, gn_weight, groups, rows, grad.contiguous(), eps, slope, need[5], need[3],
+                                                         need[4])
         gx, gw, gb = linear_backward(x, weight, gpre, need[0], need[1], need[2]) if any(need[:3]) else (None, None, None)
-        return gx, gw, gb, ggw, ggb, gr, None, None, None
+        return gx, gw, gb, ggw, ggb, gr, None, None, None, None
 
 
 def _linear_group_norm(x, weight, bias, gn_weight, gn_bias, groups, eps=1e-5, negative_slope=None, residual=None, pre=None):
@@ -352,45 +369,47 @@ def _linear_group_norm(x, weight, bias, gn_weight, gn_bias, groups, eps=1e-5, ne
 
 
 def kpconv_group_norm(s_feats, q_points, s_points, neighbor_indices, kernel_points, weights, bias, sigma, gn_weight, gn_bias, groups,
-                      eps=1e-5, negative_slope=0.1, weights_t=None):
-    """ConvBlock / conv part of ResidualBlock: leaky(GroupNorm(KPConv(...))).  Differentiable w.r.t. s_feats, the weights,
-    the biases and the GroupNorm affine (the autograd path keeps its own copy of the pre-norm activation)."""
+                      eps=1e-5, negative_slope=0.1, weights_t=None, cloud_rows=None):
+    """ConvBlock / conv part of ResidualBlock: leaky(GroupNorm(KPConv(...))), with per-pair statistics given ``cloud_rows`` (query
+    rows per cloud).  Differentiable w.r.t. s_feats, the weights, the biases and the GroupNorm affine (the autograd path keeps its
+    own copy of the pre-norm activation)."""
     m, h = neighbor_indices.shape
     k, cin, cout = weights.shape
     if not (KPCONV_MODE == 'tc' and cin % 32 == 0 and cout % 16 == 0 and cout >= 32 and (cout <= 128 or cout % 128 == 0) and m >= 64):
         x = kpconv(s_feats, q_points, s_points, neighbor_indices, kernel_points, weights, bias, sigma, weights_t=weights_t)
-        return group_norm(x, gn_weight, gn_bias, groups, eps, negative_slope=negative_slope)
+        return group_norm(x, gn_weight, gn_bias, groups, eps, negative_slope=negative_slope, cloud_rows=cloud_rows)
     if _needs_grad(s_feats, weights, bias, gn_weight, gn_bias):
         return _KPConvGroupNorm.apply(s_feats, weights, bias, gn_weight, gn_bias, q_points, s_points, neighbor_indices, kernel_points,
-                                      float(sigma), int(groups), float(eps), negative_slope, weights_t)
+                                      float(sigma), int(groups), float(eps), negative_slope, weights_t, cloud_rows)
     return _kpconv_group_norm(s_feats, q_points, s_points, neighbor_indices, kernel_points, weights, bias, sigma, gn_weight, gn_bias,
-                              groups, eps, negative_slope, weights_t)
+                              groups, eps, negative_slope, weights_t, cloud_rows=cloud_rows)
 
 
 class _KPConvGroupNorm(torch.autograd.Function):
     @staticmethod
     def forward(ctx, s_feats, weights, bias, gn_weight, gn_bias, q_points, s_points, neighbor_indices, kernel_points, sigma, groups, eps,
-                negative_slope, weights_t):
+                negative_slope, weights_t, cloud_rows):
         pre = torch.empty((neighbor_indices.shape[0], weights.shape[2]), dtype=_f32, device=s_feats.device)
         y = _kpconv_group_norm(s_feats, q_points, s_points, neighbor_indices, kernel_points, weights, bias, sigma, gn_weight, gn_bias,
-                               groups, eps, negative_slope, weights_t, pre=pre)
+                               groups, eps, negative_slope, weights_t, pre=pre, cloud_rows=cloud_rows)
         ctx.save_for_backward(s_feats, weights, gn_weight, q_points, s_points, neighbor_indices, kernel_points, pre, y)
-        ctx.args = (sigma, groups, eps, negative_slope)
+        ctx.args = (sigma, groups, eps, negative_slope, _seg_rows(cloud_rows, pre.shape[0]))
         return y
 
     @staticmethod
     def backward(ctx, grad):
         s_feats, weights, gn_weight, q, s, nbr, kp, pre, y = ctx.saved_tensors
-        sigma, groups, eps, slope = ctx.args
+        sigma, groups, eps, slope, rows = ctx.args
         need = ctx.needs_input_grad
-        gpre, ggw, ggb, _ = group_norm_backward_batched(pre, y, gn_weight, groups, [pre.shape[0], 0], grad.contiguous(), eps, slope, False,
-                                                        need[3], need[4])
+        gpre, ggw, ggb, _ = group_norm_backward_batched(pre, y, gn_weight, groups, rows, grad.contiguous(), eps, slope, False, need[3],
+                                                        need[4])
         gf, gw, gb = kpconv_backward(s_feats, q, s, nbr, kp, weights, sigma, gpre, need[0], need[1], need[2])
-        return gf, gw, gb, ggw, ggb, None, None, None, None, None, None, None, None, None
+        return gf, gw, gb, ggw, ggb, None, None, None, None, None, None, None, None, None, None
 
 
 def _kpconv_group_norm(s_feats, q_points, s_points, neighbor_indices, kernel_points, weights, bias, sigma, gn_weight, gn_bias, groups,
-                       eps=1e-5, negative_slope=0.1, weights_t=None, pre=None):
+                       eps=1e-5, negative_slope=0.1, weights_t=None, pre=None, cloud_rows=None):
+    """``cloud_rows``: per-pair statistics (``geob200_kpconv_group_norm_batched``)"""
     m, h = neighbor_indices.shape
     k, cin, cout = weights.shape
     s_feats, weights, bias, gn_weight, gn_bias = _detach(s_feats), _detach(weights), _detach(bias), _detach(gn_weight), _detach(gn_bias)
@@ -404,8 +423,16 @@ def _kpconv_group_norm(s_feats, q_points, s_points, neighbor_indices, kernel_poi
     if pre is None:
         pre = scratch((m, cout), dev, 'pre_norm')
     y = torch.empty((m, cout), dtype=_f32, device=dev)
-    gws = _gn_workspace(dev, groups, m, cout)
     ws = L.workspace(lib.geob200_kpconv_tc_workspace_bytes(m, ns, cin), dev, 'kpconv_tc')
+    if cloud_rows is not None:
+        gws = _gn_workspace(dev, groups, m, cout, n_pairs=len(cloud_rows) // 2)
+        L.check(lib.geob200_kpconv_group_norm_batched(
+            s_feats.data_ptr(), q_points.data_ptr(), s_points.data_ptr(), neighbor_indices.data_ptr(), m, ns, h, kernel_points.data_ptr(), k,
+            weights_t.data_ptr(), L.ptr(bias), cin, cout, float(sigma), groups, gn_weight.data_ptr(), gn_bias.data_ptr(), float(eps),
+            int(negative_slope is not None), float(negative_slope or 0.0), pre.data_ptr(), y.data_ptr(), gws.data_ptr(), gws.numel(),
+            ws.data_ptr(), ws.numel(), L.stream_ptr(), len(cloud_rows) // 2, _host_i64(cloud_rows)), 'kpconv_group_norm_batched')
+        return y
+    gws = _gn_workspace(dev, groups, m, cout)
     L.check(lib.geob200_kpconv_group_norm(s_feats.data_ptr(), q_points.data_ptr(), s_points.data_ptr(), neighbor_indices.data_ptr(),
                                           m, ns, h, kernel_points.data_ptr(), k, weights_t.data_ptr(), L.ptr(bias), cin, cout,
                                           float(sigma), groups, gn_weight.data_ptr(), gn_bias.data_ptr(), float(eps),
@@ -434,13 +461,16 @@ def group_norm_batched(x, weight, bias, groups, cloud_rows, eps=1e-5, negative_s
     return y
 
 
-def linear_group_norm_batched(x, weight, bias, gn_weight, gn_bias, groups, cloud_rows, eps=1e-5, negative_slope=None, residual=None):
-    """linear_group_norm with per-pair GroupNorm statistics (see group_norm_batched)"""
+def linear_group_norm_batched(x, weight, bias, gn_weight, gn_bias, groups, cloud_rows, eps=1e-5, negative_slope=None, residual=None,
+                              pre=None):
+    """linear_group_norm with per-pair GroupNorm statistics (see group_norm_batched); ``pre``: tensor to receive the pre-norm
+    activation (default: a shared scratch buffer)"""
     x, weight, bias, gn_weight, gn_bias = _detach(x), _detach(weight), _detach(bias), _detach(gn_weight), _detach(gn_bias)
     m, k = x.shape
     n = weight.shape[0]
     np_ = len(cloud_rows) // 2
-    pre = scratch((m, n), x.device, 'pre_norm')
+    if pre is None:
+        pre = scratch((m, n), x.device, 'pre_norm')
     y = torch.empty((m, n), dtype=_f32, device=x.device)
     ws = _gn_workspace(x.device, groups, m, n, n_pairs=np_)
     L.check(L.lib().geob200_linear_group_norm_batched(x.data_ptr(), x.stride(0), weight.data_ptr(), L.ptr(bias), m, n, k, groups,
@@ -451,21 +481,41 @@ def linear_group_norm_batched(x, weight, bias, gn_weight, gn_bias, groups, cloud
     return y
 
 
-def maxpool(x, neighbor_indices):
-    """differentiable w.r.t. x (``maxpool_backward_batched``)"""
+def maxpool(x, neighbor_indices, cloud_rows=None, cloud_max=None):
+    """differentiable w.r.t. x (``maxpool_backward_batched``).  A batch of pairs (``cloud_rows``: query rows per cloud, 2B host ints;
+    ``cloud_max``: ``cloud_max_count`` of the table) pools pair p's rows over its own table width only (``geob200_maxpool_batched``)."""
+    if (cloud_rows is None) != (cloud_max is None):
+        raise RuntimeError('maxpool: cloud_rows and cloud_max come together')
     if _needs_grad(x):
-        return _Maxpool.apply(x, neighbor_indices)
-    return _maxpool(x, neighbor_indices)
+        return _Maxpool.apply(x, neighbor_indices, cloud_rows, cloud_max)
+    return _maxpool(x, neighbor_indices, cloud_rows, cloud_max)
 
 
-def _maxpool(x, neighbor_indices):
+def _maxpool(x, neighbor_indices, cloud_rows=None, cloud_max=None):
     x = _detach(x)
     _f(x, 'x'); L.require_cuda(neighbor_indices, 'neighbor_indices', _i64)
     m, h = neighbor_indices.shape
     y = torch.empty((m, x.shape[1]), dtype=_f32, device=x.device)
+    if cloud_rows is not None:
+        L.require_cuda(cloud_max, 'cloud_max', _i32)
+        if cloud_max.numel() != len(cloud_rows):
+            raise RuntimeError('maxpool: cloud_max needs one entry per cloud')
+        L.check(L.lib().geob200_maxpool_batched(x.data_ptr(), neighbor_indices.data_ptr(), m, x.shape[0], h, x.shape[1], cloud_max.data_ptr(),
+                                                len(cloud_rows) // 2, _host_i64(cloud_rows), y.data_ptr(), L.stream_ptr()), 'maxpool_batched')
+        return y
     L.check(L.lib().geob200_maxpool(x.data_ptr(), neighbor_indices.data_ptr(), m, x.shape[0], h, x.shape[1],
                                     y.data_ptr(), L.stream_ptr()), 'maxpool')
     return y
+
+
+def cloud_max_count(neighbor_indices, n_support, cloud_rows):
+    """(2B,) device int32: per cloud the widest row (number of real neighbours) of the (n_query, H) table ``neighbor_indices`` whose
+    query rows are laid out by ``cloud_rows`` (2B host ints) -- the per-pair widths of the batched max-pool"""
+    L.require_cuda(neighbor_indices, 'neighbor_indices', _i64)
+    out = torch.empty((len(cloud_rows),), dtype=_i32, device=neighbor_indices.device)
+    L.check(L.lib().geob200_cloud_max_count(neighbor_indices.data_ptr(), neighbor_indices.shape[0], int(n_support), neighbor_indices.shape[1],
+                                            len(cloud_rows) // 2, _host_i64(cloud_rows), out.data_ptr(), L.stream_ptr()), 'cloud_max_count')
+    return out
 
 
 def maxpool_backward_batched(x, neighbor_indices, cloud_rows, grad_y, cloud_max=None):
@@ -494,14 +544,15 @@ def maxpool_backward_batched(x, neighbor_indices, cloud_rows, grad_y, cloud_max=
 
 class _Maxpool(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, neighbor_indices):
-        ctx.save_for_backward(x, neighbor_indices)
-        return _maxpool(x, neighbor_indices)
+    def forward(ctx, x, neighbor_indices, cloud_rows, cloud_max):
+        ctx.save_for_backward(x, neighbor_indices, cloud_max)
+        ctx.rows = _seg_rows(cloud_rows, neighbor_indices.shape[0])
+        return _maxpool(x, neighbor_indices, cloud_rows, cloud_max)
 
     @staticmethod
     def backward(ctx, grad):
-        x, nbr = ctx.saved_tensors
-        return maxpool_backward_batched(x, nbr, [nbr.shape[0], 0], grad.contiguous()), None
+        x, nbr, cloud_max = ctx.saved_tensors
+        return maxpool_backward_batched(x, nbr, ctx.rows, grad.contiguous(), cloud_max), None, None, None
 
 
 def upsample_concat(x, upsample_indices, skip=None):
@@ -686,10 +737,11 @@ class GseTable:
         self.blob, self.channels, self.inv_step, self.d_max, self.a_max = blob, channels, inv_step, d_max, a_max
 
 
-def gse_table(div_term, wd_t, wa_t, bd, ba, sigma_a, inv_step=None, d_max=None):
+def gse_table(div_term, wd_t, wa_t, bd, ba, sigma_a, inv_step=None, d_max=None, sync=True):
     """Tabulate the two projections of GeometricStructureEmbedding for the given weights (wd_t / wa_t: transposed nn.Linear
     weights (in, out)).  Angle indices lie in [0, 180 / sigma_a]; distance indices above ``d_max`` fall back to the direct
-    evaluation inside ``gse_embed*``.  Returns after the build has COMPLETED, so any stream may use the table."""
+    evaluation inside ``gse_embed*``.  Returns after the build has COMPLETED, so any stream may use the table; ``sync=False``
+    returns at once (only the current stream may use it before the caller waits for it)."""
     for t, name in ((div_term, 'div_term'), (wd_t, 'wd_t'), (wa_t, 'wa_t'), (bd, 'bd'), (ba, 'ba')):
         L.require_cuda(t, name, _f32)
     c = int(wd_t.shape[0])
@@ -703,7 +755,8 @@ def gse_table(div_term, wd_t, wa_t, bd, ba, sigma_a, inv_step=None, d_max=None):
     blob = torch.empty(nbytes, dtype=_u8, device=wd_t.device)
     L.check(lib.geob200_gse_table_build(div_term.data_ptr(), wd_t.data_ptr(), wa_t.data_ptr(), bd.data_ptr(), ba.data_ptr(), c,
                                         inv_step, d_max, a_max, blob.data_ptr(), nbytes, L.stream_ptr()), 'gse_table_build')
-    torch.cuda.current_stream(wd_t.device).synchronize()
+    if sync:
+        torch.cuda.current_stream(wd_t.device).synchronize()
     return GseTable(blob, c, inv_step, d_max, a_max)
 
 
@@ -830,15 +883,8 @@ def attention(q, k, v, heads, qp=None, qb=None, embed=None, out=None, streaming=
     if _needs_grad(q, k, v, qp, qb, embed):
         if not streaming:
             raise RuntimeError('attention: the backward needs the probabilities of the streaming forward')
-        srcs, keys, where = [], [], []
-        for t in (q, k, v):
-            base, r0, col = _column_source(t)
-            key = (id(base), r0, t.shape[0])
-            if key not in keys:
-                keys.append(key)
-                srcs.append(base if (r0 == 0 and t.shape[0] == base.shape[0]) else base[r0:r0 + t.shape[0]])
-            where.append((keys.index(key), col))
-        y = _Attention.apply(int(heads), int(q.shape[1]), tuple(where), qp, qb, embed, *srcs)
+        srcs, where = _att_sources(q, k, v)
+        y = _Attention.apply(int(heads), int(q.shape[1]), where, qp, qb, embed, *srcs)
         return y if out is None else out.copy_(y)
     return _attention(q, k, v, heads, qp, qb, embed, out, streaming)
 
@@ -931,8 +977,16 @@ def attention_backward_batched(items, heads):
             raise RuntimeError('attention_backward_batched: the items\' gradients must share row strides')
         gstrides = gst
         structure = e is not None and it.get('structure', True)
-        g += ([torch.empty((n, heads, c), dtype=_f32, device=dev), torch.empty((n, heads), dtype=_f32, device=dev),
-               torch.empty((n, m, c), dtype=_f32, device=dev)] if structure else [None, None, None])
+        if structure:
+            for name, shape in (('grad_qp', (n, heads, c)), ('grad_qb', (n, heads)), ('grad_embed', (n, m, c))):
+                t = it.get(name)
+                if t is None:
+                    t = torch.empty(shape, dtype=_f32, device=dev)
+                elif not t.is_cuda or t.dtype != _f32 or t.numel() != math.prod(shape) or not t.is_contiguous():
+                    raise RuntimeError(f'attention_backward_batched: item {j}: {name} must be a contiguous float32 CUDA view of {shape} values')
+                g.append(t)
+        else:
+            g += [None, None, None]
         arr[j] = _AttItem(q.data_ptr(), k.data_ptr(), v.data_ptr(), L.ptr(qp), L.ptr(qb), L.ptr(e), o.data_ptr(), n, m)
         garr[j] = _AttGradItem(probs.data_ptr(), go.data_ptr(), *(L.ptr(t) for t in g))
         res.append(tuple(g))
@@ -960,9 +1014,8 @@ class _Attention(torch.autograd.Function):
     def forward(ctx, heads, c, where, qp, qb, embed, *srcs):
         q, k, v = (srcs[i][:, col:col + c] for i, col in where)
         n, m = q.shape[0], k.shape[0]
-        # the streaming forward (the one that leaves the probabilities in its workspace) takes C = 128 / 256 and the keys whose
-        # scores fit its softmax kernel's shared memory (attention_streaming_batch)
-        if c not in (128, 256) or 4 * (2 * heads * ((m + 3) // 4 * 4) + 16 * c) > 200 * 1024:
+        # only the streaming forward leaves the probabilities in its workspace (geob200_attention_batched_keeps_probs)
+        if not _keeps_probs([(n, m)], c, heads):
             raise RuntimeError(f'attention backward: channels {c} (128 or 256) or keys {m} outside the streaming forward')
         buf, probs = attention_probs(n, m, heads, q.device)
         out = _attention(q, k, v, heads, qp, qb, embed, probs=buf)
@@ -982,6 +1035,128 @@ class _Attention(torch.autograd.Function):
         g = attention_backward_batched([item], ctx.heads)[0]
         return (None, None, None, g[3] if n_qp else None, g[4] if n_qb else None, g[5] if n_e else None,
                 *(gs if need else None for gs, need in zip(gsrc, ctx.needs_input_grad[6:])))
+
+
+ATT_MAX_ITEMS = 32          # GEOB200_ATT_MAX_ITEMS: items whose probabilities one geob200_attention_batched call leaves in place
+
+
+def _keeps_probs(rows, c, heads):
+    """whether the streaming forward takes every (n_query, n_key) item of ``rows`` in one launch pair, leaving its probabilities in
+    the workspace (geob200_attention_batched_keeps_probs)"""
+    arr = (_AttItem * len(rows))(*[_AttItem(None, None, None, None, None, None, None, n, m) for n, m in rows])
+    return L.lib().geob200_attention_batched_keeps_probs(arr, len(rows), c, heads) == 1
+
+
+def _att_sources(q, k, v):
+    """the row blocks q, k and v are column slices of (one per distinct block) and where each reads: (srcs, ((src, col) x 3))"""
+    srcs, keys, where = [], [], []
+    for t in (q, k, v):
+        base, r0, col = _column_source(t)
+        key = (id(base), r0, t.shape[0])
+        if key not in keys:
+            keys.append(key)
+            srcs.append(base if (r0 == 0 and t.shape[0] == base.shape[0]) else base[r0:r0 + t.shape[0]])
+        where.append((keys.index(key), col))
+    return srcs, tuple(where)
+
+
+def attention_batched(q, k, v, heads, q_rows, k_rows, qp=None, qb=None, embed=None):
+    """Several attention items in one launch pair (``geob200_attention_batched``, the batched transformer's kernels): item i is
+    query rows sum(q_rows[:i]) .. + q_rows[i] of q (and of qp (N, heads, C) / qb (N, heads)) against key rows sum(k_rows[:i]) .. +
+    k_rows[i] of k and v (column slices allowed); a self-attention item reads its (q_rows[i], k_rows[i], C) structure embedding at
+    rows sum_{j<i} q_rows[j] * k_rows[j] of the flat ``embed`` (sum q_rows * k_rows, C).  Returns the (N, C) output of all items.
+    Differentiable w.r.t. q, k, v, qp, qb and embed: the forward leaves every item's probabilities in a buffer owned by the autograd
+    node (at most ATT_MAX_ITEMS items, C = 128 or 256, streaming path), and the backward is one ``attention_backward_batched`` call."""
+    q_rows, k_rows = [int(r) for r in q_rows], [int(r) for r in k_rows]
+    if _needs_grad(q, k, v, qp, qb, embed):
+        srcs, where = _att_sources(q, k, v)
+        return _AttentionBatched.apply(int(heads), int(q.shape[1]), where, tuple(q_rows), tuple(k_rows), qp, qb, embed, *srcs)
+    return _attention_batched(q, k, v, heads, q_rows, k_rows, qp, qb, embed)[0]
+
+
+def _attention_batched(q, k, v, heads, q_rows, k_rows, qp=None, qb=None, embed=None, probs=False):
+    """(out, probability buffer or None, per-item byte offsets into it); ``probs``: run in a fresh buffer whose item layout is
+    the documented one of geob200_attention_batched, instead of the shared scratch"""
+    q, k, v, qp, qb, embed = (_detach(t) for t in (q, k, v, qp, qb, embed))
+    _rows(q, 'q'); _rows(k, 'k'); _rows(v, 'v')
+    n_items, c = len(q_rows), q.shape[1]
+    if n_items < 1 or len(k_rows) != n_items or min(q_rows) < 1 or min(k_rows) < 1:
+        raise RuntimeError('attention_batched: one positive query and key row count per item')
+    if sum(q_rows) != q.shape[0] or sum(k_rows) != k.shape[0] or v.shape[0] != k.shape[0]:
+        raise RuntimeError(f'attention_batched: the items must cover the {q.shape[0]} query and {k.shape[0]} key rows')
+    self_att = embed is not None
+    if self_att:
+        for t, name in ((qp, 'qp'), (qb, 'qb'), (embed, 'embed')):
+            if t is None or not t.is_contiguous():
+                raise RuntimeError(f'attention_batched: {name} must be a contiguous tensor')
+            _f(t, name)
+        if embed.numel() != sum(a * b for a, b in zip(q_rows, k_rows)) * c:
+            raise RuntimeError('attention_batched: embed must hold sum(q_rows * k_rows) rows of C values')
+    dev = q.device
+    out = torch.empty((q.shape[0], c), dtype=_f32, device=dev)
+    arr = (_AttItem * n_items)()
+    qo = ko = eo = 0
+    for i, (n, m) in enumerate(zip(q_rows, k_rows)):
+        arr[i] = _AttItem(q.data_ptr() + 4 * qo * q.stride(0), k.data_ptr() + 4 * ko * k.stride(0), v.data_ptr() + 4 * ko * v.stride(0),
+                          qp.data_ptr() + 4 * qo * heads * c if self_att else None, qb.data_ptr() + 4 * qo * heads if self_att else None,
+                          embed.data_ptr() + 4 * eo * c if self_att else None, out.data_ptr() + 4 * qo * c, n, m)
+        qo, ko, eo = qo + n, ko + m, eo + n * m
+    lib = L.lib()
+    nbytes = lib.geob200_attention_batched_workspace_bytes(arr, n_items, heads)
+    buf, offs = None, None
+    if probs:
+        if not lib.geob200_attention_batched_keeps_probs(arr, n_items, c, heads):
+            raise RuntimeError(f'attention backward: {n_items} items (<= {ATT_MAX_ITEMS}), channels {c} (128 or 256) or keys outside the '
+                               'streaming forward')
+        buf = torch.empty(nbytes, dtype=_u8, device=dev)
+        offs, o = [], 0
+        for n, m in zip(q_rows, k_rows):
+            offs.append(o)
+            o += (n * m * heads * 4 + 255) // 256 * 256
+        ws = buf
+    else:
+        ws = L.workspace(nbytes, dev, tag='attention')
+    L.check(lib.geob200_attention_batched(arr, n_items, q.stride(0), k.stride(0), v.stride(0), c, c, heads, ws.data_ptr(), ws.numel(),
+                                          L.stream_ptr()), 'attention_batched')
+    return out, buf, offs
+
+
+class _AttentionBatched(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, heads, c, where, q_rows, k_rows, qp, qb, embed, *srcs):
+        q, k, v = (srcs[i][:, col:col + c] for i, col in where)
+        out, buf, offs = _attention_batched(q, k, v, heads, q_rows, k_rows, qp, qb, embed, probs=True)
+        ctx.save_for_backward(qp, qb, embed, out, buf, *srcs)
+        ctx.heads, ctx.c, ctx.where, ctx.q_rows, ctx.k_rows, ctx.offs = heads, c, where, q_rows, k_rows, offs
+        return out
+
+    @staticmethod
+    def backward(ctx, grad):
+        qp, qb, embed, out, buf, *srcs = ctx.saved_tensors
+        c, H = ctx.c, ctx.heads
+        q, k, v = (srcs[i][:, col:col + c] for i, col in ctx.where)
+        gsrc, (gq, gk, gv) = _source_grads(srcs, ctx.where, c)
+        n_qp, n_qb, n_e = ctx.needs_input_grad[5:8]
+        grad = grad.contiguous()
+        structure = embed is not None and (n_qp or n_qb or n_e)
+        if structure:          # one gradient tensor per input, the items write their rows of it
+            gqp, gqb, ge = torch.empty_like(qp), torch.empty_like(qb), torch.empty_like(embed)
+        items, qo, ko, eo = [], 0, 0, 0
+        for n, m, off in zip(ctx.q_rows, ctx.k_rows, ctx.offs):
+            rq, rk = slice(qo, qo + n), slice(ko, ko + m)
+            it = dict(q=q[rq], k=k[rk], v=v[rk], out=out[rq], probs=buf[off:off + n * m * H * 4].view(_f32).view(n, H, m), grad_out=grad[rq],
+                      grad_q=gq[rq], grad_k=gk[rk], grad_v=gv[rk])
+            if embed is not None:
+                it.update(qp=qp[rq], qb=qb[rq], embed=embed.view(-1, c)[eo:eo + n * m], structure=structure)
+                if structure:
+                    it.update(grad_qp=gqp[rq], grad_qb=gqb[rq], grad_embed=ge.view(-1, c)[eo:eo + n * m])
+            items.append(it)
+            qo, ko, eo = qo + n, ko + m, eo + n * m
+        attention_backward_batched(items, H)
+        if not structure:
+            gqp = gqb = ge = None
+        return (None, None, None, None, None, gqp if n_qp else None, gqb if n_qb else None, ge if n_e else None,
+                *(gs if need else None for gs, need in zip(gsrc, ctx.needs_input_grad[8:])))
 
 
 def head_project(q, wp_t, bp, heads):
@@ -2280,3 +2455,26 @@ def nonfinite_check(tensors, found_inf=None):
     L.check(L.lib().geob200_nonfinite_check(table.data_ptr(), table[n:].data_ptr(), n, max(t.numel() for t in tensors),
                                             found_inf.data_ptr(), L.stream_ptr()), 'nonfinite_check')
     return found_inf
+
+
+def batch_loss_weights(loss_rows, mean_row=None, n_valid=None, found_inf=None):
+    """Loss weights of a batched training step (``geob200_batch_loss_weights``, one launch): pair p of the (B, >= 3) [loss, c_loss,
+    f_loss] rows is valid when its row is finite.  Returns (w (B,) = valid_p / n_valid, mean_row (3,) = the fixed-order sum over
+    the valid pairs of w_p * row p, NaN without one).  ``n_valid`` (1-element fp32) receives the count; ``found_inf`` (1-element fp32)
+    is set to 1 when no pair is valid and left alone otherwise.  No host synchronisation."""
+    loss_rows = _detach(loss_rows)
+    _f(loss_rows, 'loss_rows')
+    if loss_rows.dim() != 2 or loss_rows.shape[1] < 3 or loss_rows.stride(1) != 1:
+        raise RuntimeError('batch_loss_weights: loss_rows must be (B, >= 3) with unit inner stride')
+    B, dev = loss_rows.shape[0], loss_rows.device
+    w = torch.empty((B,), dtype=_f32, device=dev)
+    if mean_row is None:
+        mean_row = torch.empty((3,), dtype=_f32, device=dev)
+    if found_inf is None:
+        found_inf = torch.zeros((), dtype=_f32, device=dev)
+    for t, name, n in ((mean_row, 'mean_row', 3), (n_valid, 'n_valid', 1), (found_inf, 'found_inf', 1)):
+        if t is not None and (_f(t, name).numel() != n or not t.is_contiguous() or t.device != dev):
+            raise RuntimeError(f'batch_loss_weights: {name} must be a contiguous float32 tensor of {n} values on {dev}')
+    L.check(L.lib().geob200_batch_loss_weights(loss_rows.data_ptr(), loss_rows.stride(0), B, w.data_ptr(), mean_row.data_ptr(), L.ptr(n_valid),
+                                               found_inf.data_ptr(), L.stream_ptr()), 'batch_loss_weights')
+    return w, mean_row

@@ -147,16 +147,22 @@ class OverallLoss(nn.Module):
         return {'loss': t[0], 'c_loss': t[1], 'f_loss': t[2]}
 
     def graph_rows(self, output_dict, data_dict):
-        """(1, 3) [loss, c_loss, f_loss] with gradients to the coarse features and the matching scores (the value kernels' bits)"""
+        """(B, 3) [loss, c_loss, f_loss] of the B pairs of the output dict with gradients to the coarse features and the matching
+        scores (the value kernels' bits).  One pair, or the stacked output of ``GeoTransformer.forward_train_batch`` (its
+        ``_cloud_nodes`` give B and the pairs' superpoint rows, ``_stacked['gt_transforms']`` the (B, 4, 4) transforms)."""
         rf, sf = output_dict['ref_feats_c'], output_dict['src_feats_c']
         counts = _counts(output_dict)
         gi = output_dict['gt_node_corr_indices']
+        cloud_nodes = output_dict.get('_cloud_nodes') or (rf.shape[0], sf.shape[0])
+        B = len(cloud_nodes) // 2
         n_gt = counts.get('gt')
-        n_gt = n_gt.reshape(1) if n_gt is not None else torch.full((1,), gi.shape[0], dtype=torch.int32, device=rf.device)
-        coarse = dict(cloud_nodes=(rf.shape[0], sf.shape[0]), gt_indices=gi, gt_overlaps=output_dict['gt_node_corr_overlaps'],
-                      gt_count=n_gt, params=self.coarse_loss.params())
+        n_gt = n_gt.reshape(B) if n_gt is not None else torch.full((1,), gi.shape[0], dtype=torch.int32, device=rf.device)
+        coarse = dict(cloud_nodes=cloud_nodes, gt_indices=gi, gt_overlaps=output_dict['gt_node_corr_overlaps'], gt_count=n_gt,
+                      params=self.coarse_loss.params())
         rp, sp, rm, sm, scores, T = FineMatchingLoss.inputs(output_dict, data_dict)
+        if B > 1:
+            T = output_dict['_stacked']['gt_transforms']
         n_p = counts.get('node_corr')
-        fine = dict(n_pairs=1, ref_knn_points=rp, src_knn_points=sp, ref_knn_masks=rm, src_knn_masks=sm, transforms=T,
-                    positive_radius=self.fine_loss.positive_radius, patch_count=None if n_p is None else n_p.reshape(1))
+        fine = dict(n_pairs=B, ref_knn_points=rp, src_knn_points=sp, ref_knn_masks=rm, src_knn_masks=sm, transforms=T,
+                    positive_radius=self.fine_loss.positive_radius, patch_count=None if n_p is None else n_p.reshape(B))
         return GF.matching_losses_batched(rf, sf, scores, coarse, fine, (self.weight_coarse_loss, self.weight_fine_loss))

@@ -304,6 +304,70 @@ class GeoTransformer(nn.Module):
                     _stacked=dict(gt=(gt_idx, gt_ov, gt_cnt), coarse=(m_corr, m_count), lgr=(rcp, scp, n_corr), transforms=T,
                                   cloud_nodes=cn, cloud_points=c0, points=points0))
 
+    def forward_train_batch(self, data_dict, seed, iteration, targets=None):
+        """``forward_train`` of the B pairs of one collated batch (``registration_collate_fn_stack_mode``, stack order
+        [ref_1..ref_B, src_1..src_B]), the step the reference gets from B-rank DistributedDataParallel.  Per pair it does what
+        ``forward_train`` does; the backbone and the transformer run ONCE over the stacked rows, with a graph to every parameter
+        and the kernel sequence of the native drivers' ``forward_batch`` (per-pair GroupNorm statistics, per-pair max-pool widths,
+        one structure-embedding launch, batched attention, one in_proj / out_proj GEMM over all rows), so ``feats_c``,
+        ``feats_f`` and ``y_n`` are its bits.  Pair p's targets come from the Philox stream (``seed``, ``iteration``, p): one
+        ``superpoint_targets_batched`` launch for all pairs.  ``targets``: a list of B (ref indices, src indices, overlaps) tuples
+        replacing the draw.
+
+        Returns one dict of stacked full-capacity buffers: ``ref_feats_c`` / ``src_feats_c`` = the ref / src blocks of y_n, the
+        gt rows of all pairs, the target patches (pair p's patch q at row p * K + q of the ref / src patch tensors and of
+        ``matching_scores``), ``_cloud_nodes`` and the device counts under ``_counts`` ((B,) each), ``_stacked`` for the metrics
+        and ``_features`` = (feats_c, feats_f, y_n).  No host synchronisation."""
+        B = int(data_dict.get('batch_size', 1))
+        transform = data_dict.get('transform')
+        if transform is None:
+            raise ValueError('forward_train_batch: the training forward needs the ground-truth transforms')
+        dev = data_dict['features'].device
+        lens_h = data_dict.get('lengths_host') or [l.tolist() for l in data_dict['lengths']]
+        fl, K = self.fine_level, self.num_points_in_patch
+        cn, cf, c0 = [int(v) for v in lens_h[-1]], [int(v) for v in lens_h[fl]], [int(v) for v in lens_h[0]]
+        points_c, points_f, points0 = data_dict['points'][-1], data_dict['points'][fl], data_dict['points'][0]
+        transforms = (torch.stack(list(transform)) if isinstance(transform, (list, tuple)) else transform).reshape(B, 4, 4).contiguous()
+        R, Rf, R0 = sum(cn[:B]), sum(cf[:B]), sum(c0[:B])
+
+        _, node_masks, knn_idx, knn_masks = GF.point_to_node_partition_batched(points_f, points_c, cf, cn, K)
+        _, _, all_pts = GF.gather_patches_batched(None, 0, cn, cf, knn_idx, knn_masks, points_f)
+        gt_idx, gt_ov, gt_cnt = GF.node_correspondences_batched(points_c, all_pts, node_masks, knn_masks, cn, transforms,
+                                                                self.matching_radius)
+
+        feats_list = self.backbone(data_dict['features'], data_dict)
+        feats_c, feats_f = feats_list[-1], feats_list[0]
+        y_n = GF.l2_normalize(self.transformer.forward_batched_grad(points_c, feats_c, cn))
+
+        cm, fm = self.coarse_matching, self.fine_matching
+        with torch.no_grad():
+            m_corr, _, m_count = GF.superpoint_matching_batched(y_n.detach(), node_masks, cn, cm.num_correspondences,
+                                                                cm.dual_normalization)
+            if targets is None:
+                kc = self.cfg.coarse_matching.num_targets
+                corr, node_scores, corr_count = GF.superpoint_targets_batched(
+                    gt_idx, gt_ov, gt_cnt, cn, self.cfg.coarse_matching.overlap_threshold, kc, seed, iteration)
+            else:
+                corr, node_scores, corr_count = _forced_targets(targets, B, dev)
+                kc = corr.shape[1]
+            k_idx, k_masks, k_pts = GF.gather_patches_batched(corr, kc, cn, cf, knn_idx, knn_masks, points_f)
+        r, s = slice(0, B * kc), slice(B * kc, 2 * B * kc)
+        raw_scores = GF.patch_scores_batched(feats_f, cf, k_idx[r], k_idx[s])
+        scores = self.optimal_transport(raw_scores, k_masks[r], k_masks[s])
+        with torch.no_grad():
+            rcp, scp, cs, T, n_corr = GF.local_global_registration_batched(
+                B, k_pts[r], k_pts[s], k_masks[r], k_masks[s], scores.detach(), fm.k, fm.acceptance_radius, fm.mutual,
+                fm.confidence_threshold, fm.correspondence_threshold, fm.num_refinement_steps)
+        return dict(ref_points_c=points_c[:R], src_points_c=points_c[R:], ref_points_f=points_f[:Rf], src_points_f=points_f[Rf:],
+                    ref_points=points0[:R0], src_points=points0[R0:], ref_feats_c=y_n[:R], src_feats_c=y_n[R:],
+                    ref_feats_f=feats_f[:Rf], src_feats_f=feats_f[Rf:], gt_node_corr_indices=gt_idx, gt_node_corr_overlaps=gt_ov,
+                    node_corr_scores=node_scores, ref_node_corr_knn_points=k_pts[r], src_node_corr_knn_points=k_pts[s],
+                    ref_node_corr_knn_masks=k_masks[r], src_node_corr_knn_masks=k_masks[s], matching_scores=scores,
+                    matching_scores_raw=raw_scores, target_corr=corr, _cloud_nodes=cn, _features=(feats_c, feats_f, y_n),
+                    _counts=dict(node_corr=corr_count, coarse=m_count, corr=n_corr, gt=gt_cnt),
+                    _stacked=dict(gt=(gt_idx, gt_ov, gt_cnt), coarse=(m_corr, m_count), lgr=(rcp, scp, n_corr), transforms=T,
+                                  gt_transforms=transforms, cloud_nodes=cn, cloud_points=c0, points=points0))
+
     def forward(self, data_dict, taps=None):
         """``forward_batch`` with its defaults: the output dict of a single pair (the reference's contract), the list of output
         dicts for a batch of several pairs.  ``taps`` and ``data_dict['forced_node_corr']``: see ``forward_batch``."""
@@ -341,6 +405,22 @@ def _forced_node_corr(forced, device):
     if not ref.shape[0] == src.shape[0] == scores.shape[0]:
         raise ValueError('forced_node_corr: the ref indices, src indices and scores must have the same length')
     return torch.stack([ref, src]), scores.reshape(1, -1)
+
+
+def _forced_targets(targets, B, device):
+    """per-pair teacher-forced targets [(ref indices (k_p,), src indices (k_p,), overlaps (k_p,))] * B -> the layout of
+    ``superpoint_targets_batched``: corr (2B, max k_p) int64 (-1 past a count), scores (B, max k_p) (0 past it), counts (B,) int32"""
+    if len(targets) != B:
+        raise ValueError(f'forward_train_batch: targets must hold one (ref, src, overlaps) tuple per pair ({B})')
+    forced = [_forced_node_corr(t, device) for t in targets]
+    k = max(max(c.shape[1] for c, _ in forced), 1)
+    corr = torch.full((2 * B, k), -1, dtype=torch.int64, device=device)
+    scores = torch.zeros((B, k), dtype=torch.float32, device=device)
+    for p, (c, sc) in enumerate(forced):
+        n = c.shape[1]
+        corr[p, :n], corr[B + p, :n], scores[p, :n] = c[0], c[1], sc[0]
+    counts = torch.tensor([c.shape[1] for c, _ in forced], dtype=torch.int32).to(device, non_blocking=True)
+    return corr, scores, counts
 
 
 def trim_outputs(outs):

@@ -36,21 +36,30 @@ class GeometricStructureEmbedding(nn.Module):
             return None
         return self._weights_table()
 
-    def _weights_table(self):
+    def _weights_table(self, sync=True):
         """the version-keyed table of ``table`` whatever GF.GSE_MODE: the structure embedding's backward picks the winning angle
-        term with its lookups"""
+        term with its lookups.  ``sync=False`` (the training forward, after every optimizer step) builds it without waiting for the
+        device: it is then used on the current stream only, and the first ``sync`` caller waits for its build."""
         params = (self.proj_d.weight, self.proj_d.bias, self.proj_a.weight, self.proj_a.bias)
         key = tuple((p.data_ptr(), p._version) for p in params) + (GF.GSE_TABLE_INV_STEP, GF.GSE_TABLE_D_MAX, float(self.sigma_a))
         hit = self._table
-        if hit is None or hit[0] != key:
+        if hit is None or hit[0] != key or (sync and hit[2] is not None):
             with _TABLE_LOCK:
                 hit = self._table
                 if hit is None or hit[0] != key:
                     wd_t = self.proj_d.weight.detach().t().contiguous()
                     wa_t = self.proj_a.weight.detach().t().contiguous()
                     tab = GF.gse_table(self.embedding.div_term, wd_t, wa_t, self.proj_d.bias.detach().contiguous(),
-                                       self.proj_a.bias.detach().contiguous(), self.sigma_a)
-                    hit = (key, tab)
+                                       self.proj_a.bias.detach().contiguous(), self.sigma_a, sync=sync)
+                    built = None
+                    if not sync:
+                        built = torch.cuda.Event()
+                        built.record()
+                    hit = (key, tab, built)
+                    self._table = hit
+                elif sync and hit[2] is not None:
+                    hit[2].synchronize()
+                    hit = (hit[0], hit[1], None)
                     self._table = hit
         return hit[1]
 
@@ -90,6 +99,25 @@ class GeometricStructureEmbedding(nn.Module):
         return GF.gse_embed(d, a, self.embedding.div_term, self.proj_d.weight, self.proj_a.weight, self.proj_d.bias, self.proj_a.bias,
                             wd_t, wa_t, table=self._weights_table())
 
+    def forward_flat_grad(self, points, cloud_rows):
+        """The structure embeddings of several stacked clouds (``cloud_rows``: their row counts) as ONE flat (sum n_c^2, C) tensor,
+        cloud after cloud, with the graph to proj_d / proj_a: one ``gse_indices_batched`` and one ``gse_embed_flat`` launch, the
+        kernels of the batched forward (``GeoTransformer.forward_batch``), so the values are its bits.  The backward
+        (``geob200_gse_embed_backward``) sums over all rows of all clouds."""
+        rows = [int(r) for r in cloud_rows]
+        n2 = sum(r * r for r in rows)
+        dev = points.device
+        d = torch.empty((n2,), dtype=torch.float32, device=dev)
+        a = torch.empty((n2, self.angle_k), dtype=torch.float32, device=dev)
+        GF.gse_indices_batched(points, rows, self.sigma_d, self.sigma_a, self.angle_k, d, a)
+        wd_t = self._cache.get('wd_t', self.proj_d.weight, lambda w: w.t().contiguous())
+        wa_t = self._cache.get('wa_t', self.proj_a.weight, lambda w: w.t().contiguous())
+        p = (self.proj_d.weight, self.proj_a.weight, self.proj_d.bias, self.proj_a.bias)
+        if GF._needs_grad(*p):
+            return GF.gse_embed_flat(d, a, n2, self.embedding.div_term, *p, wd_t, wa_t, None, table=self._weights_table(sync=False))
+        out = torch.empty((n2, self.proj_d.out_features), dtype=torch.float32, device=dev)
+        return GF.gse_embed_flat(d, a, n2, self.embedding.div_term, *(t.detach() for t in p), wd_t, wa_t, out, table=self.table())
+
 
 class GeometricTransformer(nn.Module):
     """reference ``geotransformer.py:75-155``."""
@@ -127,6 +155,17 @@ class GeometricTransformer(nn.Module):
         if batched:
             return rf.unsqueeze(0), sf.unsqueeze(0)
         return rf, sf
+
+
+    def forward_batched_grad(self, points_c, feats_c, cloud_rows):
+        """The transformer (with in_proj and out_proj, before the L2 normalisation) over the stacked superpoints of B pairs (stack order
+        [ref_1..ref_B, src_1..src_B], ``cloud_rows``: the 2B row counts), with the graph to every parameter and to ``feats_c``: the
+        kernels of the batched native forward in its order (one structure-embedding launch for all clouds, one in_proj / out_proj
+        GEMM over all rows, ``RPEConditionalTransformer.forward_batched_grad``)."""
+        E = self.embedding.forward_flat_grad(points_c, cloud_rows)
+        x = GF.linear(feats_c, self.in_proj.weight, self.in_proj.bias)
+        x = self.transformer.forward_batched_grad(x, cloud_rows, E)
+        return GF.linear(x, self.out_proj.weight, self.out_proj.bias)
 
 
 class SuperPointMatching(nn.Module):

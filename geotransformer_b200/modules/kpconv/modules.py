@@ -40,11 +40,12 @@ class KPConv(nn.Module):
         return GF.kpconv(s_feats, q_points, s_points, neighbor_indices, self.kernel_points, self.weights, self.bias,
                          self.sigma, weights_t=self._weights_t())
 
-    def forward_norm(self, s_feats, q_points, s_points, neighbor_indices, norm, negative_slope):
-        """KPConv -> GroupNorm -> LeakyReLU as one fused op (GroupNorm statistics from the GEMM epilogue)"""
+    def forward_norm(self, s_feats, q_points, s_points, neighbor_indices, norm, negative_slope, cloud_rows=None):
+        """KPConv -> GroupNorm -> LeakyReLU as one fused op (GroupNorm statistics from the GEMM epilogue; per pair with
+        ``cloud_rows``, the query rows per cloud of a batch)"""
         return GF.kpconv_group_norm(s_feats, q_points, s_points, neighbor_indices, self.kernel_points, self.weights, self.bias,
                                     self.sigma, norm.norm.weight, norm.norm.bias, norm.num_groups, norm.norm.eps,
-                                    negative_slope=negative_slope, weights_t=self._weights_t())
+                                    negative_slope=negative_slope, weights_t=self._weights_t(), cloud_rows=cloud_rows)
 
     def __repr__(self):
         return (f'KPConv(kernel_size: {self.kernel_size}, in_channels: {self.in_channels}, out_channels: '
@@ -94,13 +95,14 @@ class UnaryBlock(nn.Module):
         self.norm = GroupNorm(group_norm, out_channels)
         self.leaky_relu = nn.LeakyReLU(0.1) if has_relu else None
 
-    def forward(self, x, residual=None, residual_slope=None):
+    def forward(self, x, residual=None, residual_slope=None, cloud_rows=None):
+        """``cloud_rows``: rows per cloud of a batch of pairs (per-pair GroupNorm statistics), None for one pair"""
         slope = self.leaky_relu.negative_slope if self.leaky_relu is not None else None
         if residual is not None:      # fused tail of ResidualBlock: leaky(norm(x) + shortcut)
             slope = residual_slope
         n = self.norm
         return GF.linear_group_norm(x, self.mlp.weight, self.mlp.bias, n.norm.weight, n.norm.bias, n.num_groups, n.norm.eps,
-                                    negative_slope=slope, residual=residual)
+                                    negative_slope=slope, residual=residual, cloud_rows=cloud_rows)
 
 
 class LastUnaryBlock(nn.Module):
@@ -128,8 +130,9 @@ class ConvBlock(nn.Module):
         self.norm = GroupNorm(group_norm, out_channels)
         self.leaky_relu = nn.LeakyReLU(negative_slope=negative_slope)
 
-    def forward(self, s_feats, q_points, s_points, neighbor_indices):
-        return self.KPConv.forward_norm(s_feats, q_points, s_points, neighbor_indices, self.norm, self.leaky_relu.negative_slope)
+    def forward(self, s_feats, q_points, s_points, neighbor_indices, cloud_rows=None):
+        return self.KPConv.forward_norm(s_feats, q_points, s_points, neighbor_indices, self.norm, self.leaky_relu.negative_slope,
+                                        cloud_rows=cloud_rows)
 
 
 class ResidualBlock(nn.Module):
@@ -152,13 +155,20 @@ class ResidualBlock(nn.Module):
             self.unary_shortcut = nn.Identity()
         self.leaky_relu = nn.LeakyReLU(0.1)
 
-    def forward(self, s_feats, q_points, s_points, neighbor_indices):
-        x = self.unary1(s_feats)
-        x = self.KPConv.forward_norm(x, q_points, s_points, neighbor_indices, self.norm_conv, self.leaky_relu.negative_slope)
-        shortcut = GF.maxpool(s_feats, neighbor_indices) if self.strided else s_feats
-        shortcut = self.unary_shortcut(shortcut)
+    def forward(self, s_feats, q_points, s_points, neighbor_indices, s_rows=None, q_rows=None, cloud_max=None):
+        """``s_rows`` / ``q_rows``: support / query rows per cloud of a batch of pairs (per-pair GroupNorm statistics), and for a
+        strided block ``cloud_max`` (``GF.cloud_max_count`` of its table): the max-pool's per-pair widths.  None for one pair."""
+        x = s_feats if isinstance(self.unary1, nn.Identity) else self.unary1(s_feats, cloud_rows=s_rows)
+        x = self.KPConv.forward_norm(x, q_points, s_points, neighbor_indices, self.norm_conv, self.leaky_relu.negative_slope,
+                                     cloud_rows=q_rows)
+        if self.strided:
+            shortcut = GF.maxpool(s_feats, neighbor_indices, q_rows, cloud_max) if q_rows is not None else GF.maxpool(s_feats, neighbor_indices)
+        else:
+            shortcut = s_feats
+        if not isinstance(self.unary_shortcut, nn.Identity):
+            shortcut = self.unary_shortcut(shortcut, cloud_rows=q_rows)
         # unary2 (Linear+GroupNorm) + shortcut add + LeakyReLU in one normalisation pass
-        return self.unary2(x, residual=shortcut, residual_slope=self.leaky_relu.negative_slope)
+        return self.unary2(x, residual=shortcut, residual_slope=self.leaky_relu.negative_slope, cloud_rows=q_rows)
 
 
 def maxpool(x, neighbor_indices):

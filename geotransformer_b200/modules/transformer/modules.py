@@ -316,6 +316,41 @@ class RPEConditionalTransformer(nn.Module):
         return x
 
 
+    def forward_batched_grad(self, x, cloud_rows, embeddings):
+        """The transformer over the stacked rows of B pairs with the graph, the kernel sequence of
+        ``geob200_transformer_forward_batched``: x rows in stack order [ref_1..ref_B, src_1..src_B] (``cloud_rows``: their 2B row
+        counts), ``embeddings`` the flat structure embeddings of the 2B clouds one after the other (sum n_c^2, C).  Every Linear /
+        LayerNorm runs once over all rows (the ref block and the src block are contiguous, so a cross layer's projections are single
+        GEMMs too); attention runs as one batched launch pair per phase, one item per cloud (self) or per pair (cross)."""
+        rows = [int(r) for r in cloud_rows]
+        B = len(rows) // 2
+        R, c = sum(rows[:B]), x.shape[1]
+        ref, src = rows[:B], rows[B:]
+        for i, block in enumerate(self.blocks):
+            layer = self.layers[i]
+            mha = layer.attention.attention
+            h = mha.num_heads
+            if block == 'self':
+                w, b = _concat(mha, ('proj_q', 'proj_k', 'proj_v'))
+                qkv = GF.linear(x, w, b)
+                q, k, v = qkv[:, :c], qkv[:, c:2 * c], qkv[:, 2 * c:]
+                qp, qb = GF.head_project(q, mha.proj_p.weight.t(), mha.proj_p.bias, h)
+                hidden = GF.attention_batched(q, k, v, h, rows, rows, qp=qp, qb=qb, embed=embeddings)
+                x = _tail(layer, hidden, x)
+            else:
+                wkv, bkv = _concat(mha, ('proj_k', 'proj_v'))
+                x0, x1 = x[:R], x[R:]
+                q0 = GF.linear(x0, mha.proj_q.weight, mha.proj_q.bias)
+                kv1 = GF.linear(x1, wkv, bkv)
+                y0 = _tail(layer, GF.attention_batched(q0, kv1[:, :c], kv1[:, c:], h, ref, src), x0)
+                mem = x0 if self.parallel else y0
+                q1 = GF.linear(x1, mha.proj_q.weight, mha.proj_q.bias)
+                kv0 = GF.linear(mem, wkv, bkv)
+                y1 = _tail(layer, GF.attention_batched(q1, kv0[:, :c], kv0[:, c:], h, src, ref), x1)
+                x = torch.cat([y0, y1])
+        return x
+
+
 def _concat(mha, names):
     """the fused projection weight / bias of ``_fused``, concatenated from the parameters themselves (with their graph)"""
     return (torch.cat([getattr(mha, n).weight for n in names], dim=0), torch.cat([getattr(mha, n).bias for n in names], dim=0))

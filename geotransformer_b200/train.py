@@ -9,6 +9,13 @@ settings (Adam, L2 weight decay), so its ``state_dict`` and the snapshot ``{'epo
 read-back (the reference applies such an update unless ``run_grad_check`` is set, which stops in a debugger).
 
 The loss, the Evaluator's metrics and the skip flag of a step come back in one packed device-to-host copy and one event wait.
+
+``batch_size`` B > 1 trains B pairs per step on one device (``train_batch``): the step the reference takes with B-rank
+DistributedDataParallel.  One forward over the collated batch (``GeoTransformer.forward_train_batch``), the (B, 3) loss rows of
+all pairs, and one backward of their mean over the valid pairs (``functional.batch_loss_weights``: a pair whose loss row is not
+finite -- no ground truth or no targets -- is dropped from the mean instead of skipping the step).  With all pairs valid the
+gradient is DDP's (1/B) sum_p g_p; with ``scale_lr`` the learning rates are multiplied by B as the reference's
+``register_optimizer`` multiplies them by the world size.
 """
 import math
 
@@ -60,6 +67,17 @@ def make_scheduler(optimizer, cfg):
     return torch.optim.lr_scheduler.StepLR(optimizer, o.lr_decay_steps, gamma=o.lr_decay)
 
 
+def make_optimizer_and_scheduler(model, cfg, batch_size=1, scale_lr=True):
+    """``make_optimizer``, then (``scale_lr``) every param group's lr multiplied by ``batch_size``, then ``make_scheduler``: the
+    reference's order (``register_optimizer`` scales by the DDP world size before the experiment builds its scheduler), so the
+    scheduler's base lrs are the scaled ones.  ``batch_size`` 1 gives ``make_optimizer`` / ``make_scheduler`` unchanged."""
+    optimizer = make_optimizer(model, cfg)
+    if scale_lr:
+        for g in optimizer.param_groups:
+            g['lr'] = g['lr'] * batch_size
+    return optimizer, make_scheduler(optimizer, cfg)
+
+
 def fused_optimizer_state(state):
     """an Adam ``state_dict`` (the reference saves an unfused one: step counts on the host) made loadable into ``make_optimizer``'s
     fused Adam: ``load_state_dict`` takes the saved group options, so they are set to fused here, and with them it moves the step
@@ -70,25 +88,33 @@ def fused_optimizer_state(state):
 
 # packed per-step row on the device: [loss, c_loss, f_loss | PIR, IR, RRE, RTE, RMSE, RR, #corr, #gt | found_inf]
 _ROW = 12
+# a batched step appends [n_valid] and per pair [loss, c_loss, f_loss | the 8 metrics]
+_PAIR_ROW = 11
+# attention items of one batched launch pair whose probabilities the backward reads (GEOB200_ATT_MAX_ITEMS): one per cloud
+MAX_BATCH = GF.ATT_MAX_ITEMS // 2
 
 
 class TrainingEngine:
-    def __init__(self, model, cfg, neighbor_limits, seed=None, device=None):
+    def __init__(self, model, cfg, neighbor_limits, seed=None, device=None, batch_size=1, scale_lr=True):
         """``model``: a GeoTransformer on its device with its weights loaded.  ``seed`` keys the target sampler's Philox stream
-        (default ``cfg.seed``); target draws depend on (seed, iteration) only, so a resumed run draws what an uninterrupted one
-        would."""
+        (default ``cfg.seed``); target draws depend on (seed, iteration, pair) only, so a resumed run draws what an uninterrupted one
+        would.  ``batch_size``: pairs per ``train_batch`` step (1 .. MAX_BATCH); with ``scale_lr`` every param group's lr is
+        multiplied by it before the scheduler is built (the reference scales by the DDP world size in ``register_optimizer``)."""
         if cfg.optim.grad_acc_steps != 1:
             raise NotImplementedError('grad_acc_steps > 1 (1 in every shipped config)')
+        if not 1 <= int(batch_size) <= MAX_BATCH:
+            raise ValueError(f'batch_size must be in 1..{MAX_BATCH}')
         self.model, self.cfg, self.limits = model, cfg, neighbor_limits
+        self.batch_size = int(batch_size)
         self.seed = int(cfg.seed if seed is None else seed)
         self.device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
         self.loss_func = OverallLoss(cfg)
         self.evaluator = Evaluator(cfg)
-        self.optimizer = make_optimizer(model, cfg)
-        self.scheduler = make_scheduler(self.optimizer, cfg)
+        self.optimizer, self.scheduler = make_optimizer_and_scheduler(model, cfg, self.batch_size, scale_lr)
         self.per_iteration = cfg.name == 'modelnet'
         self.epoch, self.iteration = 0, 0
         self.found_inf = torch.zeros((), dtype=torch.float32, device=self.device)   # 0-dim: fused Adam subtracts it from its 0-dim step counts
+        self.no_valid = torch.zeros((), dtype=torch.float32, device=self.device)    # a batched step's "no valid pair" flag
         self.row_dev = torch.zeros((_ROW,), dtype=torch.float32, device=self.device)
         self.row_host = torch.zeros((_ROW,), dtype=torch.float32).pin_memory()
         self.stage_events = None       # set to a list to receive (label, CUDA event) marks of every step (tools/train_bench.py)
@@ -150,10 +176,92 @@ class TrainingEngine:
         res['skipped'] = v[11] != 0.0
         return res
 
+    def train_batch(self, pairs):
+        """one optimisation step on 1 .. batch_size pairs: the mean over the valid pairs of their losses (a pair is valid when its
+        [loss, c_loss, f_loss] row is finite).  Returns loss, c_loss, f_loss (that mean) and the Evaluator's metrics averaged over
+        all pairs, ``per_pair`` (one dict of losses and metrics per pair), ``lr``, ``skipped`` (a non-finite gradient or no valid
+        pair: no update) and ``masked_pairs`` (pairs left out of the mean).  Everything comes back in one packed device-to-host
+        copy and one event wait; nothing else waits for the device after the collate."""
+        B = len(pairs)
+        if not 1 <= B <= self.batch_size:
+            raise ValueError(f'train_batch: 1..{self.batch_size} pairs per step, got {B}')
+        model, b = self.model, self.cfg.backbone
+        self.iteration += 1
+        self._mark('start')
+        data = registration_collate_fn_stack_mode(list(pairs), b.num_stages, b.init_voxel_size, b.init_radius, self.limits, device=self.device)
+        self._mark('collate')
+        out = model.forward_train_batch(data, self.seed, self.iteration)
+        self._mark('forward')
+        rows = self.loss_func.graph_rows(out, data)
+        packed = self._packed(B)
+        self.no_valid.zero_()
+        w, _ = GF.batch_loss_weights(rows, mean_row=packed[:3], n_valid=packed[_ROW:_ROW + 1], found_inf=self.no_valid)
+        upstream = torch.zeros_like(rows)
+        upstream[:, 0].copy_(w)
+        self._mark('loss')
+        rows.backward(upstream)
+        self._mark('backward')
+        checked = [p.grad for p in model.parameters() if p.grad is not None] + [packed[:3]]
+        GF.nonfinite_check(checked, self.found_inf)
+        torch.maximum(self.found_inf, self.no_valid, out=self.found_inf)     # a step without a valid pair is skipped too
+        self._mark('guard')
+        lr = self.optimizer.param_groups[0]['lr']
+        optimizer_step(self.optimizer, self.found_inf)
+        self.optimizer.zero_grad(set_to_none=True)
+        self._mark('optimizer')
+        with torch.no_grad():
+            per = packed[_ROW + 1:].view(B, _PAIR_ROW)
+            per[:, :3].copy_(rows.detach())
+            st, ev = out['_stacked'], self.evaluator
+            gt_idx, gt_ov, gt_cnt = st['gt']
+            (m_corr, m_cnt), (rcp, scp, n_corr) = st['coarse'], st['lgr']
+            GF.evaluate_batched(gt_idx, gt_ov, gt_cnt, m_corr, m_cnt, rcp, scp, n_corr, st['gt_transforms'], st['transforms'], st['points'],
+                                st['cloud_nodes'], st['cloud_points'], ev.mode, ev.acceptance_overlap, ev.acceptance_radius, per[:, 3:],
+                                ev.acceptance_rmse, ev.acceptance_rre, ev.acceptance_rte)
+            torch.mean(per[:, 3:], dim=0, out=packed[3:11])          # the metrics of all pairs, as the reference's all_reduce_tensors
+            packed[11].copy_(self.found_inf)
+        self._mark('metrics')
+        host = self._host[:packed.numel()]
+        host.copy_(packed, non_blocking=True)
+        done = torch.cuda.Event()
+        done.record()
+        if self.per_iteration:
+            self.scheduler.step()
+        done.synchronize()
+        v = host.tolist()
+        res = self._result(v[:_ROW])
+        res['lr'] = lr
+        n_valid = int(v[_ROW])
+        res['masked_pairs'] = B - n_valid
+        res['skipped'] = v[11] != 0.0
+        res['per_pair'] = [self._result(v[_ROW + 1 + p * _PAIR_ROW:_ROW + 1 + (p + 1) * _PAIR_ROW]) for p in range(B)]
+        return res
+
+    def _packed(self, B):
+        """the device buffer of one batched step's results: [the step row (_ROW) | n_valid | B per-pair rows], and its pinned mirror"""
+        n = _ROW + 1 + B * _PAIR_ROW
+        if getattr(self, '_packed_dev', None) is None or self._packed_dev.numel() < n:
+            self._packed_dev = torch.zeros((_ROW + 1 + self.batch_size * _PAIR_ROW,), dtype=torch.float32, device=self.device)
+            self._host = torch.zeros((self._packed_dev.numel(),), dtype=torch.float32).pin_memory()
+        return self._packed_dev[:n]
+
+    def _result(self, v):
+        res = dict(zip(LOSS_KEYS, v[:3]))
+        res.update(zip(METRIC_KEYS, v[3:9]))
+        if self.evaluator.mode == 1:
+            del res['RMSE']
+        return res
+
     def train_epoch(self, pairs):
-        """``train_step`` over ``pairs``, then the per-epoch scheduler step (3DMatch, KITTI); returns the step results"""
+        """one epoch over ``pairs``, then the per-epoch scheduler step (3DMatch, KITTI); returns the step results.  With
+        batch_size 1: ``train_step`` per pair; otherwise ``train_batch`` on consecutive groups of batch_size pairs, a trailing
+        partial group being a step of fewer pairs (``iteration`` counts steps)."""
         self.epoch += 1
-        results = [self.train_step(p) for p in pairs]
+        if self.batch_size == 1:
+            results = [self.train_step(p) for p in pairs]
+        else:
+            pairs = list(pairs)
+            results = [self.train_batch(pairs[i:i + self.batch_size]) for i in range(0, len(pairs), self.batch_size)]
         if not self.per_iteration:
             self.scheduler.step()
         return results

@@ -122,10 +122,24 @@ int geob200_linear_group_norm_batched(const float* x, int64_t ldx, const float* 
                                       int64_t groups, const float* gamma, const float* beta, float eps, const float* residual, int leaky,
                                       float slope, float* pre_norm, float* y, void* workspace, size_t workspace_bytes, void* stream,
                                       int64_t n_pairs, const int64_t* cloud_rows_h);
+/* geob200_kpconv_group_norm with per-pair statistics from the GEMM epilogue partials (the batched native backbone's kernels);
+ * cloud_rows_h: query rows per cloud.  GroupNorm workspace as geob200_linear_group_norm_batched. */
+int geob200_kpconv_group_norm_batched(const float* s_feats, const float* q_points, const float* s_points, const int64_t* neighbors,
+                                      int64_t n_query, int64_t n_support, int64_t n_neighbors, const float* kernel_points, int64_t n_kernel,
+                                      const float* weights_t, const float* bias, int64_t c_in, int64_t c_out, float sigma, int64_t groups,
+                                      const float* gamma, const float* beta, float eps, int leaky, float slope, float* pre_norm, float* y,
+                                      void* gn_workspace, size_t gn_workspace_bytes, void* workspace, size_t workspace_bytes, void* stream,
+                                      int64_t n_pairs, const int64_t* cloud_rows_h);
 
 /* maxpool over neighbour rows with a zero shadow row (functional.py:54-67) */
 int geob200_maxpool(const float* x, const int64_t* neighbors, int64_t n_query, int64_t n_support, int64_t n_neighbors,
                     int64_t channels, float* y, void* stream);
+/* maxpool of a batch of pairs: pair p's rows see the first min(n_neighbors, max(cloud_max[p], cloud_max[B + p])) columns only
+ * (cloud_max: device int32[2 * n_pairs] of geob200_cloud_max_count; cloud_rows_h[2 * n_pairs]: query rows per cloud), as the
+ * batched native backbone's strided blocks */
+int geob200_maxpool_batched(const float* x, const int64_t* neighbors, int64_t n_query, int64_t n_support, int64_t n_neighbors,
+                            int64_t channels, const int32_t* cloud_max, int64_t n_pairs, const int64_t* cloud_rows_h, float* y,
+                            void* stream);
 
 /* cloud_max[c] (device int32[2 * n_pairs]) = widest row (number of real neighbours) among the query rows of cloud c: the batched
  * backbone's maxpool ignores the columns of pair p past min(n_neighbors, max(cloud_max[p], cloud_max[B + p])), as
@@ -267,12 +281,20 @@ int geob200_attention(const float* q, int64_t ldq, const float* k, int64_t ldk, 
                       const float* qb, const float* embed, int64_t n_query, int64_t n_key, int64_t channels, int64_t heads,
                       float* out, int64_t ldo, void* workspace, size_t workspace_bytes, void* stream);
 /* A batch of independent attention problems that share channels, heads and row strides (the clouds / pairs of a batched
- * forward) in ONE launch pair; all items with embed (self-attention) or all without (cross-attention). */
+ * forward) in ONE launch pair; all items with embed (self-attention) or all without (cross-attention).
+ * Probability layout: with at most GEOB200_ATT_MAX_ITEMS items, C = 128 or 256 and every item on the streaming path, item i's
+ * softmax probabilities (n_query, heads, n_key) fp32 are left in the workspace at byte offset
+ * sum_{j < i} align_up(n_query_j * n_key_j * heads * 4, 256) (the backward reads them there).  Larger batches run in chunks of
+ * GEOB200_ATT_MAX_ITEMS items that reuse the workspace from its start. */
+#define GEOB200_ATT_MAX_ITEMS 32
 typedef struct { const float* q; const float* k; const float* v; const float* qp; const float* qb; const float* embed; float* out;
                  int64_t n_query, n_key; } geob200_att_item_t;
 size_t geob200_attention_batched_workspace_bytes(const geob200_att_item_t* items_h, int64_t n_items, int64_t heads);
 int geob200_attention_batched(const geob200_att_item_t* items_h, int64_t n_items, int64_t ldq, int64_t ldk, int64_t ldv, int64_t ldo,
                               int64_t channels, int64_t heads, void* workspace, size_t workspace_bytes, void* stream);
+/* 1 when geob200_attention_batched with a workspace leaves every item's probabilities at the layout above (at most
+ * GEOB200_ATT_MAX_ITEMS items, all on the streaming path), else 0 (host only, no launch) */
+int geob200_attention_batched_keeps_probs(const geob200_att_item_t* items_h, int64_t n_items, int64_t channels, int64_t heads);
 /* self-attention kernels: 1 (default) = TMA-staged E stream (cp.async.bulk ring, q.k and P.v as tiled passes), 0 = the
  * lanes<->channels cp.async kernels */
 int geob200_set_attention_tma(int on);
@@ -685,6 +707,13 @@ int geob200_superpoint_targets_batched(const int64_t* gt_indices, const float* g
  * DEVICE tables ptrs / numels is NaN or +-Inf, else 0.  max_numel (host) = the largest numel, sizes the grid.  One launch. */
 int geob200_nonfinite_check(const float* const* ptrs, const int64_t* numels, int64_t n_tensors, int64_t max_numel, float* found_inf,
                             void* stream);
+
+/* Loss weights of a batched training step, one launch: pair p is valid when row p of loss_rows (n_pairs, >= 3 at row stride
+ * ld_rows: [loss, c_loss, f_loss]) is finite.  weights[p] = valid_p / n_valid (the upstream gradient of column 0), mean_row[0..2] =
+ * sum over the valid pairs, in pair order, of weights[p] * row p (fp32, every product rounded), n_valid (may be NULL) = the count as
+ * a float.  With no valid pair: weights 0, mean_row NaN and found_inf[0] = 1; otherwise found_inf is not written. */
+int geob200_batch_loss_weights(const float* loss_rows, int64_t ld_rows, int64_t n_pairs, float* weights, float* mean_row, float* n_valid,
+                               float* found_inf, void* stream);
 
 #ifdef __cplusplus
 }
