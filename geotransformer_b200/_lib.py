@@ -152,6 +152,11 @@ _sig('geob200_batch_loss_weights', c_int, P, I64, I64, P, P, P, P, P)
 _sig('geob200_kpconv_group_norm_batched', c_int, P, P, P, P, I64, I64, I64, P, I64, P, P, I64, I64, F, I64, P, P, F, c_int, F, P, P, P,
      SZ, P, SZ, P, I64, P)
 _sig('geob200_maxpool_batched', c_int, P, P, I64, I64, I64, I64, P, I64, P, P, P)
+_sig('geob200_augment_pairs_batched_workspace_bytes', SZ, I64)
+_sig('geob200_augment_pairs_batched', c_int, P, P, I64, P, c_int, I64, D, D, D, D, D, ctypes.c_uint64, ctypes.c_uint64, I64, P, P, P, P, P,
+     SZ, P)
+_sig('geob200_modelnet_pairs_batched_workspace_bytes', SZ, I64)
+_sig('geob200_modelnet_pairs_batched', c_int, P, P, I64, I64, D, D, D, D, ctypes.c_uint64, ctypes.c_uint64, I64, P, P, P, P, P, SZ, P)
 
 
 def lib():

@@ -56,6 +56,8 @@ def make_cfg(name='3dmatch'):
         c.eval.update(acceptance_radius=0.1, rmse_threshold=0.2, rre_threshold=15.0, rte_threshold=0.3)
         c.neighbor_limits = [38, 36, 36, 38]  # reference demo.py:52
         c.optim.update(lr_decay=0.95, lr_decay_steps=1, max_epoch=40)            # StepLR per epoch
+        # training data (config.py:38-44): point limit, rotation of one cloud, uniform noise (augment.py)
+        c.train = Cfg(point_limit=30000, use_augmentation=True, augmentation_noise=0.005, augmentation_rotation=1.0)
     elif name == 'kitti':
         c.backbone.update(num_stages=5, init_voxel_size=0.3, base_radius=4.25)
         c.model.update(ground_truth_matching_radius=0.6, num_points_in_patch=128, fine_level=1)
@@ -67,6 +69,9 @@ def make_cfg(name='3dmatch'):
         c.fine_loss.positive_radius = 0.6
         c.ransac.update(distance_threshold=0.3, num_points=4, num_iterations=50000)
         c.optim.update(lr_decay=0.95, lr_decay_steps=4, max_epoch=160)           # StepLR per epoch
+        # training data (config.py:36-45): point limit, noise, rotation of one cloud, scale, shift (augment.py)
+        c.train = Cfg(point_limit=30000, use_augmentation=True, augmentation_noise=0.01, augmentation_min_scale=0.8,
+                      augmentation_max_scale=1.2, augmentation_shift=2.0, augmentation_rotation=1.0)
         c.neighbor_limits = None  # calibrated (reference utils/data.py:192-217)
     elif name == 'modelnet':
         c.backbone.update(num_stages=3, init_voxel_size=0.05, base_radius=2.5)
@@ -76,6 +81,10 @@ def make_cfg(name='3dmatch'):
         c.fine_matching.update(topk=3, acceptance_radius=0.1)
         c.eval.update(acceptance_radius=0.1, rre_threshold=1.0, rte_threshold=0.1)
         c.optim.update(warmup_steps=10000, eta_init=0.1, eta_min=0.1, max_iteration=400000)   # warm-up cosine per iteration
+        # training pairs synthesised from raw shapes (config.py:31-47; augment.py)
+        c.data = Cfg(num_points=717, voxel_size=None, rotation_magnitude=45.0, translation_magnitude=0.5, keep_ratio=0.7,
+                     crop_method='plane', asymmetric=True, twice_sample=True, twice_transform=False)
+        c.train = Cfg(noise_magnitude=0.05, class_indices='all')
         c.neighbor_limits = None
     else:
         raise ValueError(f'unknown config {name}')

@@ -1,0 +1,619 @@
+// Training-data augmentation on the device: the per-iteration pair augmentation of the reference's 3DMatch and KITTI training
+// sets and the ModelNet pair synthesis from one raw shape.
+//
+// Reference: geotransformer/datasets/registration/threedmatch/dataset.py (_load_point_cloud, _augment_point_cloud),
+//            geotransformer/datasets/registration/kitti/dataset.py (_load_point_cloud, _augment_point_cloud),
+//            geotransformer/datasets/registration/modelnet/dataset.py (__getitem__) and geotransformer/transforms/functional.py.
+// Semantics and random streams: include/geob200.h and DESIGN.md section 3b.  Every draw is Philox4x32-10 keyed by
+// (seed, tag of stream and cloud) with counter (index, iteration, pair_base + p), so the result is a function of the inputs and
+// (seed, iteration, pair id) only -- never of the launch geometry or the rest of the batch.  The per-point arithmetic of the
+// 3DMatch / KITTI modes is fp64 with explicit roundings (__dmul_rn / __dadd_rn: no contraction) and one rounding to fp32, so its
+// numpy restatement (oracle/augment_oracle.py) reproduces it bit for bit.  No float atomics.
+#include "common.cuh"
+#include "compaction.cuh"
+#include "geob200.h"
+#include "philox.cuh"
+#include "radix_select.cuh"
+
+namespace geob200 {
+
+constexpr int AUG_THREADS = 1024;          // chunk_rank needs 32 warps
+constexpr int AUG_POINT_THREADS = 256;
+constexpr int MN_THREADS = 512;
+constexpr int AUG_RECORD = 20;             // [u0 .. u10 | R row-major]
+constexpr int MN_MAX_SHAPE = 8192;
+constexpr int MN_MAX_POINTS = 4096;
+
+// stream tags, XORed into the high key word; tag 0 is the target sampler's and RANSAC's key
+enum AugStream : uint32_t { AUG_PAIR = 1, AUG_LIMIT = 2, AUG_NOISE = 3, AUG_SAMPLE = 4, AUG_JITTER = 5 };
+__host__ __device__ constexpr uint32_t aug_tag(uint32_t stream, uint32_t cloud) { return GEOB200_AUGMENT_TAG_BASE | (stream << 4) | cloud; }
+
+struct AugKey {
+    uint32_t k0, k1, it_lo, it_hi;
+};
+
+__device__ __forceinline__ void aug_words(uint32_t w[4], uint32_t index, uint32_t pair, const AugKey& k, uint32_t tag) {
+    w[0] = index; w[1] = k.it_lo; w[2] = k.it_hi; w[3] = pair;
+    philox4x32_10(w, k.k0, k.k1 ^ tag);
+}
+
+// 53-bit uniform in [0, 1) from two words: ((a >> 5) 2^26 + (b >> 6)) 2^-53, exact
+__device__ __forceinline__ double u53(uint32_t a, uint32_t b) {
+    return __dmul_rn(__dadd_rn(__dmul_rn((double)(a >> 5), 67108864.0), (double)(b >> 6)), 0x1p-53);
+}
+__device__ __forceinline__ double u32(uint32_t w) { return __dmul_rn((double)w, 0x1p-32); }
+
+// the per-pair uniforms u0 .. u_{n-1} (n <= 11): Philox call i (counter index i) gives u_{2i} from words 0, 1 and u_{2i+1} from
+// words 2, 3; unused slots are 0
+__device__ __forceinline__ void pair_uniforms(double (&u)[11], int n, uint32_t pair, const AugKey& k) {
+#pragma unroll
+    for (int i = 0; i < 6; ++i) {
+        uint32_t w[4];
+        aug_words(w, (uint32_t)i, pair, k, aug_tag(AUG_PAIR, 0));
+        u[2 * i] = 2 * i < n ? u53(w[0], w[1]) : 0.0;
+        if (2 * i + 1 < 11) u[2 * i + 1] = 2 * i + 1 < n ? u53(w[2], w[3]) : 0.0;
+    }
+}
+
+// scipy Rotation.from_euler('zyx', (a, b, c)).as_matrix(), extrinsic: Rx(c) Ry(b) Rz(a), row-major
+__device__ __forceinline__ void euler_zyx(double a, double b, double c, double (&R)[9]) {
+    double sa, ca, sb, cb, sc, cc;
+    sincos(a, &sa, &ca); sincos(b, &sb, &cb); sincos(c, &sc, &cc);
+    R[0] = __dmul_rn(cb, ca);
+    R[1] = -__dmul_rn(cb, sa);
+    R[2] = sb;
+    R[3] = __dadd_rn(__dmul_rn(cc, sa), __dmul_rn(__dmul_rn(sc, sb), ca));
+    R[4] = __dsub_rn(__dmul_rn(cc, ca), __dmul_rn(__dmul_rn(sc, sb), sa));
+    R[5] = -__dmul_rn(sc, cb);
+    R[6] = __dsub_rn(__dmul_rn(sc, sa), __dmul_rn(__dmul_rn(cc, sb), ca));
+    R[7] = __dadd_rn(__dmul_rn(sc, ca), __dmul_rn(__dmul_rn(cc, sb), sa));
+    R[8] = __dmul_rn(cc, cb);
+}
+
+// row i of M times v: (M[i,0] v0 + M[i,1] v1) + M[i,2] v2
+__device__ __forceinline__ double row_dot(const double* M, int i, double v0, double v1, double v2) {
+    return __dadd_rn(__dadd_rn(__dmul_rn(M[3 * i], v0), __dmul_rn(M[3 * i + 1], v1)), __dmul_rn(M[3 * i + 2], v2));
+}
+// column i of M times v: (M[0,i] v0 + M[1,i] v1) + M[2,i] v2
+__device__ __forceinline__ double col_dot(const double* M, int i, double v0, double v1, double v2) {
+    return __dadd_rn(__dadd_rn(__dmul_rn(M[i], v0), __dmul_rn(M[3 + i], v1)), __dmul_rn(M[6 + i], v2));
+}
+
+__device__ __forceinline__ void write_record(double* rec, const double (&u)[11], const double (&R)[9]) {
+#pragma unroll
+    for (int i = 0; i < 11; ++i) rec[i] = u[i];
+#pragma unroll
+    for (int i = 0; i < 9; ++i) rec[11 + i] = R[i];
+}
+
+// ---- 3DMatch / KITTI ---------------------------------------------------------------------------------------------------------
+
+// Point limit, grid (1, 2B), AUG_THREADS.  Cloud c with n <= limit: origin = 0 .. n-1.  Otherwise the `limit` smallest keys
+// (philox(j) << 32) | j, written in ascending j.  word: workspace, In.start[c] + j.
+__global__ void __launch_bounds__(AUG_THREADS) point_limit_kernel(const __grid_constant__ Segs In, const __grid_constant__ Segs Out,
+                                                                 int B, int limit, AugKey key, uint32_t pair_base,
+                                                                 uint32_t* __restrict__ word, int* __restrict__ origin) {
+    __shared__ unsigned hist[256];
+    __shared__ unsigned prefix_s, kth_s;
+    __shared__ int warp_tot[32];
+    const int c = blockIdx.y, n = In.count[c];
+    const uint32_t pair = pair_base + (uint32_t)(c % B), tag = aug_tag(AUG_LIMIT, c >= B ? 1u : 0u);
+    int* out = origin + Out.start[c];
+    if (n <= limit) {
+        for (int j = threadIdx.x; j < n; j += AUG_THREADS) out[j] = j;
+        return;
+    }
+    word += In.start[c];
+    for (int j = threadIdx.x; j < n; j += AUG_THREADS) {
+        uint32_t w[4];
+        aug_words(w, (uint32_t)j, pair, key, tag);
+        word[j] = w[0];
+    }
+    __syncthreads();
+    // the `limit` smallest (word, j) = the `limit` largest ~word, ties at the threshold to the lowest j
+    unsigned thr;
+    int need_eq;
+    radix_select_kth((long long)n, limit, [&](long long j) { return ~word[j]; }, hist, &prefix_s, &kth_s, thr, need_eq);
+    int kept = 0, eq = 0;
+    for (int base = 0; base < n; base += AUG_THREADS) {
+        const int j = base + threadIdx.x;
+        const unsigned b = j < n ? ~word[j] : 0u;
+        const bool fe = j < n && b == thr;
+        int te;
+        const int re = chunk_rank(fe, warp_tot, &te);
+        const bool f = j < n && (b > thr || (fe && eq + re < need_eq));
+        int tot;
+        const int r = chunk_rank(f, warp_tot, &tot);
+        if (f) out[kept + r] = j;
+        kept += tot; eq += te;
+    }
+}
+
+struct AugParams {
+    int mode;
+    double noise, rotation_factor, min_scale, max_scale, shift;
+};
+
+// Per-point pass, grid (ceil(Out.max / AUG_POINT_THREADS), 2B).  Thread 0 of every CTA draws its pair's uniforms and R (a few
+// Philox calls); the first CTA of each ref cloud also writes the pair's record and transform.
+__global__ void __launch_bounds__(AUG_POINT_THREADS) augment_points_kernel(
+        const float* __restrict__ points, const __grid_constant__ Segs In, const __grid_constant__ Segs Out,
+        const int* __restrict__ origin, const float* __restrict__ T_in, int B, AugParams P, AugKey key, uint32_t pair_base,
+        float* __restrict__ out, float* __restrict__ T_out, double* __restrict__ record) {
+    __shared__ double prm[16];             // R (9), this cloud rotated, scale, shift (3)
+    const int c = blockIdx.y, p = c % B;
+    const bool src = c >= B, kitti = P.mode == GEOB200_AUGMENT_KITTI;
+    const uint32_t pair = pair_base + (uint32_t)p;
+    if (threadIdx.x == 0) {
+        double u[11], R[9];
+        pair_uniforms(u, kitti ? 11 : 4, pair, key);
+        // numpy: rand(3) * pi * 2 / rotation_factor
+        euler_zyx(__ddiv_rn(__dmul_rn(__dmul_rn(u[0], M_PI), 2.0), P.rotation_factor),
+                  __ddiv_rn(__dmul_rn(__dmul_rn(u[1], M_PI), 2.0), P.rotation_factor),
+                  __ddiv_rn(__dmul_rn(__dmul_rn(u[2], M_PI), 2.0), P.rotation_factor), R);
+        const bool rot_ref = u[3] > 0.5;
+        // numpy: min + (max - min) * u;  uniform(-s, s) = -s + (s - -s) * u
+        const double scale = kitti ? __dadd_rn(P.min_scale, __dmul_rn(__dsub_rn(P.max_scale, P.min_scale), u[4])) : 1.0;
+        const double w2 = __dsub_rn(P.shift, -P.shift);
+        double rs[3], ss[3];
+#pragma unroll
+        for (int i = 0; i < 3; ++i) {
+            rs[i] = kitti ? __dadd_rn(-P.shift, __dmul_rn(w2, u[5 + i])) : 0.0;
+            ss[i] = kitti ? __dadd_rn(-P.shift, __dmul_rn(w2, u[8 + i])) : 0.0;
+        }
+#pragma unroll
+        for (int i = 0; i < 9; ++i) prm[i] = R[i];
+        prm[9] = (src ? !rot_ref : rot_ref) ? 1.0 : 0.0;
+        prm[10] = scale;
+#pragma unroll
+        for (int i = 0; i < 3; ++i) prm[11 + i] = src ? ss[i] : rs[i];
+        if (!src && blockIdx.x == 0) {
+            write_record(record + (long long)p * AUG_RECORD, u, R);
+            double G[9], g[3], N[9], t[3];
+            const float* T = T_in + 16ll * p;
+#pragma unroll
+            for (int i = 0; i < 3; ++i) {
+#pragma unroll
+                for (int j = 0; j < 3; ++j) G[3 * i + j] = (double)T[4 * i + j];
+                g[i] = (double)T[4 * i + 3];
+            }
+            if (rot_ref) {                 // rotation = R_aug R_gt, translation = R_aug t_gt
+#pragma unroll
+                for (int i = 0; i < 3; ++i) {
+#pragma unroll
+                    for (int j = 0; j < 3; ++j) N[3 * i + j] = row_dot(R, i, G[j], G[3 + j], G[6 + j]);
+                    t[i] = row_dot(R, i, g[0], g[1], g[2]);
+                }
+            } else {                       // rotation = R_gt R_aug^T
+#pragma unroll
+                for (int i = 0; i < 3; ++i) {
+#pragma unroll
+                    for (int j = 0; j < 3; ++j) N[3 * i + j] = row_dot(G, i, R[3 * j], R[3 * j + 1], R[3 * j + 2]);
+                    t[i] = g[i];
+                }
+            }
+            if (kitti) {                   // translation = -(R' src_shift) + scale t' + ref_shift
+#pragma unroll
+                for (int i = 0; i < 3; ++i) t[i] = __dmul_rn(t[i], scale);
+                double m[3];
+#pragma unroll
+                for (int i = 0; i < 3; ++i) m[i] = row_dot(N, i, ss[0], ss[1], ss[2]);
+#pragma unroll
+                for (int i = 0; i < 3; ++i) t[i] = __dadd_rn(__dadd_rn(-m[i], t[i]), rs[i]);
+            }
+            float* To = T_out + 16ll * p;
+#pragma unroll
+            for (int i = 0; i < 3; ++i) {
+#pragma unroll
+                for (int j = 0; j < 3; ++j) To[4 * i + j] = __double2float_rn(N[3 * i + j]);
+                To[4 * i + 3] = __double2float_rn(t[i]);
+                To[12 + i] = 0.0f;
+            }
+            To[15] = 1.0f;
+        }
+    }
+    __syncthreads();
+    const int r = blockIdx.x * AUG_POINT_THREADS + threadIdx.x;
+    if (r >= Out.count[c]) return;
+    const long long o = (long long)Out.start[c] + r;
+    const int j = origin[o];
+    const float* q = points + 3ll * (In.start[c] + j);
+    double x = (double)q[0], y = (double)q[1], z = (double)q[2];
+    uint32_t w[4];
+    aug_words(w, (uint32_t)j, pair, key, aug_tag(AUG_NOISE, src ? 1u : 0u));
+    // numpy: (rand - 0.5) * noise
+    const double n0 = __dmul_rn(__dadd_rn(u32(w[0]), -0.5), P.noise);
+    const double n1 = __dmul_rn(__dadd_rn(u32(w[1]), -0.5), P.noise);
+    const double n2 = __dmul_rn(__dadd_rn(u32(w[2]), -0.5), P.noise);
+    const bool rotated = prm[9] != 0.0;
+    if (kitti) {                           // noise, rotation, scale, shift
+        x = __dadd_rn(x, n0); y = __dadd_rn(y, n1); z = __dadd_rn(z, n2);
+        if (rotated) {
+            const double a = row_dot(prm, 0, x, y, z), b = row_dot(prm, 1, x, y, z), d = row_dot(prm, 2, x, y, z);
+            x = a; y = b; z = d;
+        }
+        x = __dadd_rn(__dmul_rn(x, prm[10]), prm[11]);
+        y = __dadd_rn(__dmul_rn(y, prm[10]), prm[12]);
+        z = __dadd_rn(__dmul_rn(z, prm[10]), prm[13]);
+    } else {                               // rotation, noise
+        if (rotated) {
+            const double a = row_dot(prm, 0, x, y, z), b = row_dot(prm, 1, x, y, z), d = row_dot(prm, 2, x, y, z);
+            x = a; y = b; z = d;
+        }
+        x = __dadd_rn(x, n0); y = __dadd_rn(y, n1); z = __dadd_rn(z, n2);
+    }
+    out[3 * o] = __double2float_rn(x);
+    out[3 * o + 1] = __double2float_rn(y);
+    out[3 * o + 2] = __double2float_rn(z);
+}
+
+// ---- ModelNet ---------------------------------------------------------------------------------------------------------------
+
+// order-preserving map of a double to 64 bits (larger value -> larger key); -0.0 is taken as +0.0
+__device__ __forceinline__ unsigned long long ordered_key(double d) {
+    const unsigned long long b = (unsigned long long)__double_as_longlong(__dadd_rn(d, 0.0));
+    return (b >> 63) ? ~b : (b | 0x8000000000000000ull);
+}
+
+// radix_select_kth over 64-bit keys: MSB-first 8-bit digits, ties at the threshold to the lowest indices (need_eq of them)
+template <class Key>
+__device__ __forceinline__ void radix_select_kth64(int total, int k, Key key, unsigned* hist, unsigned long long* prefix_s,
+                                                   unsigned* kth_s, unsigned long long& thr, int& need_eq) {
+    unsigned long long prefix = 0, mask = 0;
+    int remaining = k;
+    for (int shift = 56; shift >= 0; shift -= 8) {
+        for (int i = threadIdx.x; i < 256; i += blockDim.x) hist[i] = 0;
+        __syncthreads();
+        for (int t = threadIdx.x; t < total; t += blockDim.x) {
+            const unsigned long long b = key(t);
+            if ((b & mask) == prefix) atomicAdd(&hist[(unsigned)(b >> shift) & 255u], 1u);
+        }
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            int rem = remaining;
+            int d = 255;
+            for (; d > 0; --d) {
+                if ((int)hist[d] >= rem) break;
+                rem -= (int)hist[d];
+            }
+            *prefix_s = prefix | ((unsigned long long)d << shift);
+            *kth_s = (unsigned)rem;
+        }
+        __syncthreads();
+        prefix = *prefix_s;
+        remaining = (int)*kth_s;
+        mask |= (255ull << shift);
+        __syncthreads();
+    }
+    thr = prefix;
+    need_eq = remaining;
+}
+
+struct MnParams {
+    int num_points, sort_n;                // sort_n: num_points rounded up to a power of two
+    double keep_ratio, rotation_magnitude, translation_magnitude, noise_magnitude;
+};
+
+// round(keep N) as the reference's int(floor(N keep + 0.5))
+__host__ __device__ __forceinline__ int crop_count(int n, double keep) { return (int)floor((double)n * keep + 0.5); }
+
+// ModelNet pair draws of pair `pair` by one thread: prm = [R (9), t (3), this cloud's plane normal (3)]; the ref cloud also writes
+// the record row and the transform.  Not inlined: one thread runs it, and its registers stay out of the kernel's loops.
+__device__ __noinline__ void modelnet_draws(const MnParams& P, const AugKey& key, uint32_t pair, int src, double* prm,
+                                            double* record, float* T_out) {
+        double u[11], R[9];
+    pair_uniforms(u, 10, pair, key);
+    // numpy: rand(3) * pi * rotation_magnitude / 180; uniform(-m, m) = -m + (m - -m) u
+    euler_zyx(__ddiv_rn(__dmul_rn(__dmul_rn(u[0], M_PI), P.rotation_magnitude), 180.0),
+              __ddiv_rn(__dmul_rn(__dmul_rn(u[1], M_PI), P.rotation_magnitude), 180.0),
+              __ddiv_rn(__dmul_rn(__dmul_rn(u[2], M_PI), P.rotation_magnitude), 180.0), R);
+    const double tw = __dsub_rn(P.translation_magnitude, -P.translation_magnitude);
+    double t[3];
+#pragma unroll
+    for (int i = 0; i < 3; ++i) t[i] = __dadd_rn(-P.translation_magnitude, __dmul_rn(tw, u[3 + i]));
+    // random_sample_plane: phi = uniform(0, 2 pi), theta = uniform(0, pi)
+    const double phi = __dmul_rn(__dsub_rn(2.0 * M_PI, 0.0), src ? u[8] : u[6]);
+    const double theta = __dmul_rn(__dsub_rn(M_PI, 0.0), src ? u[9] : u[7]);
+    double sp, cp, st, ct;
+    sincos(phi, &sp, &cp); sincos(theta, &st, &ct);
+#pragma unroll
+    for (int i = 0; i < 9; ++i) prm[i] = R[i];
+#pragma unroll
+    for (int i = 0; i < 3; ++i) prm[9 + i] = t[i];
+    prm[12] = __dmul_rn(st, cp); prm[13] = __dmul_rn(st, sp); prm[14] = ct;
+    if (!src) {
+        write_record(record, u, R);
+        float* To = T_out;
+#pragma unroll
+        for (int i = 0; i < 3; ++i) {
+#pragma unroll
+            for (int j = 0; j < 3; ++j) To[4 * i + j] = __double2float_rn(R[3 * i + j]);
+            To[4 * i + 3] = __double2float_rn(t[i]);
+            To[12 + i] = 0.0f;
+        }
+        To[15] = 1.0f;
+    }
+}
+
+// One CTA per cloud, grid (1, 2B), MN_THREADS; cloud c reads shape c % B.  Dynamic shared memory: the fp64 reduction scratch
+// (3 x MN_THREADS), the cropped rows and their sample words (crop_max each), the sort keys (sort_n).  dkey: workspace, the
+// distance keys of cloud c at 2 In.start[c % B] + (c >= B) In.count[c % B] + j.
+__global__ void __launch_bounds__(MN_THREADS) modelnet_pairs_kernel(
+        const float* __restrict__ shapes, const __grid_constant__ Segs In, int B, MnParams P, int crop_max, AugKey key,
+        uint32_t pair_base, unsigned long long* __restrict__ dkey, float* __restrict__ out, int* __restrict__ origin,
+        float* __restrict__ T_out, double* __restrict__ record) {
+    extern __shared__ __align__(16) unsigned char smem[];
+    double* red = reinterpret_cast<double*>(smem);
+    unsigned long long* sk = reinterpret_cast<unsigned long long*>(red + 3 * MN_THREADS);
+    int* crow = reinterpret_cast<int*>(sk + P.sort_n);
+    uint32_t* cword = reinterpret_cast<uint32_t*>(crow + crop_max);
+    __shared__ double prm[18];             // R (9), t (3), plane normal (3), mean (3)
+    __shared__ double inv_scale_s, inv_t[3];
+    __shared__ unsigned hist[256];
+    __shared__ unsigned long long prefix64_s;
+    __shared__ unsigned prefix_s, kth_s;
+    __shared__ int warp_tot[MN_THREADS / 32];
+    const int c = blockIdx.y, p = c % B, src = c >= B ? 1 : 0;
+    const int N = In.count[p], tid = threadIdx.x;
+    const float* pts = shapes + 3ll * In.start[p];
+    dkey += 2ll * In.start[p] + (long long)src * N;
+    const uint32_t pair = pair_base + (uint32_t)p;
+
+    if (tid == 0) modelnet_draws(P, key, pair, src, prm, record + (long long)p * AUG_RECORD, T_out + 16ll * p);
+    // 1. normalise: mean in a fixed order (per-thread strided sums, then a tree), then the largest norm
+    double sx = 0.0, sy = 0.0, sz = 0.0;
+    for (int j = tid; j < N; j += MN_THREADS) {
+        sx = __dadd_rn(sx, (double)pts[3 * j]); sy = __dadd_rn(sy, (double)pts[3 * j + 1]); sz = __dadd_rn(sz, (double)pts[3 * j + 2]);
+    }
+    red[tid] = sx; red[MN_THREADS + tid] = sy; red[2 * MN_THREADS + tid] = sz;
+    __syncthreads();
+    for (int s = MN_THREADS / 2; s > 0; s >>= 1) {
+        if (tid < s) {
+#pragma unroll
+            for (int i = 0; i < 3; ++i) red[i * MN_THREADS + tid] = __dadd_rn(red[i * MN_THREADS + tid], red[i * MN_THREADS + tid + s]);
+        }
+        __syncthreads();
+    }
+    if (tid == 0) {
+#pragma unroll
+        for (int i = 0; i < 3; ++i) prm[15 + i] = __ddiv_rn(red[i * MN_THREADS], (double)N);
+    }
+    __syncthreads();
+    const double mx = prm[15], my = prm[16], mz = prm[17];
+    double nmax = 0.0;
+    for (int j = tid; j < N; j += MN_THREADS) {
+        const double x = __dsub_rn((double)pts[3 * j], mx), y = __dsub_rn((double)pts[3 * j + 1], my), z = __dsub_rn((double)pts[3 * j + 2], mz);
+        nmax = fmax(nmax, __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(x, x), __dmul_rn(y, y)), __dmul_rn(z, z))));
+    }
+    red[tid] = nmax;
+    __syncthreads();
+    for (int s = MN_THREADS / 2; s > 0; s >>= 1) {
+        if (tid < s) red[tid] = fmax(red[tid], red[tid + s]);
+        __syncthreads();
+    }
+    if (tid == 0) inv_scale_s = red[0];
+    __syncthreads();
+    const double scale = inv_scale_s;
+    // 2. the cloud's point j: normalised, and for src the image under the inverse transform (p R + (-R^T t)); R, t and the
+    //    inverse translation are read from shared memory
+    if (tid == 0) {
+#pragma unroll
+        for (int i = 0; i < 3; ++i) inv_t[i] = -col_dot(prm, i, prm[9], prm[10], prm[11]);
+    }
+    __syncthreads();
+    auto point = [&](int j, double& x, double& y, double& z) {
+        x = __ddiv_rn(__dsub_rn((double)pts[3 * j], mx), scale);
+        y = __ddiv_rn(__dsub_rn((double)pts[3 * j + 1], my), scale);
+        z = __ddiv_rn(__dsub_rn((double)pts[3 * j + 2], mz), scale);
+        if (src) {
+            const double a = __dadd_rn(col_dot(prm, 0, x, y, z), inv_t[0]);
+            const double b = __dadd_rn(col_dot(prm, 1, x, y, z), inv_t[1]);
+            const double d = __dadd_rn(col_dot(prm, 2, x, y, z), inv_t[2]);
+            x = a; y = b; z = d;
+        }
+    };
+    // 3. plane distances
+    const double n0 = prm[12], n1 = prm[13], n2 = prm[14];
+    for (int j = tid; j < N; j += MN_THREADS) {
+        double x, y, z;
+        point(j, x, y, z);
+        dkey[j] = ordered_key(__dadd_rn(__dadd_rn(__dmul_rn(x, n0), __dmul_rn(y, n1)), __dmul_rn(z, n2)));
+    }
+    __syncthreads();
+    // 4. crop: the K largest distances, ties to the lowest row, in ascending row with their sample words
+    const int K = crop_count(N, P.keep_ratio);
+    unsigned long long thr64;
+    int need_eq;
+    radix_select_kth64(N, K, [&](int j) { return dkey[j]; }, hist, &prefix64_s, &kth_s, thr64, need_eq);
+    {
+        int kept = 0, eq = 0;
+        for (int base = 0; base < N; base += MN_THREADS) {
+            const int j = base + tid;
+            const unsigned long long b = j < N ? dkey[j] : 0ull;
+            const bool fe = j < N && b == thr64;
+            int te;
+            const int re = chunk_rank<MN_THREADS / 32>(fe, warp_tot, &te);
+            const bool f = j < N && (b > thr64 || (fe && eq + re < need_eq));
+            int tot;
+            const int r = chunk_rank<MN_THREADS / 32>(f, warp_tot, &tot);
+            if (f) {
+                uint32_t w[4];
+                aug_words(w, (uint32_t)j, pair, key, aug_tag(AUG_SAMPLE, (uint32_t)src));
+                crow[kept + r] = j;
+                cword[kept + r] = w[0];
+            }
+            kept += tot; eq += te;
+        }
+    }
+    __syncthreads();
+    // 5. sample and shuffle: the num_points smallest keys (word << 32) | row, in key order
+    const int M = P.num_points;
+    if (K > M) {
+        unsigned thr;
+        int ne;
+        radix_select_kth((long long)K, M, [&](long long i) { return ~cword[i]; }, hist, &prefix_s, &kth_s, thr, ne);
+        int kept = 0, eq = 0;
+        for (int base = 0; base < K; base += MN_THREADS) {
+            const int i = base + tid;
+            const unsigned b = i < K ? ~cword[i] : 0u;
+            const bool fe = i < K && b == thr;
+            int te;
+            const int re = chunk_rank<MN_THREADS / 32>(fe, warp_tot, &te);
+            const bool f = i < K && (b > thr || (fe && eq + re < ne));
+            int tot;
+            const int r = chunk_rank<MN_THREADS / 32>(f, warp_tot, &tot);
+            if (f) sk[kept + r] = ((unsigned long long)cword[i] << 32) | (unsigned)crow[i];
+            kept += tot; eq += te;
+        }
+    } else {
+        for (int i = tid; i < K; i += MN_THREADS) sk[i] = ((unsigned long long)cword[i] << 32) | (unsigned)crow[i];
+    }
+    for (int i = M + tid; i < P.sort_n; i += MN_THREADS) sk[i] = ~0ull;
+    __syncthreads();
+    for (int k = 2; k <= P.sort_n; k <<= 1) {              // bitonic sort, ascending
+        for (int h = k >> 1; h > 0; h >>= 1) {
+            for (int i = tid; i < P.sort_n; i += MN_THREADS) {
+                const int l = i ^ h;
+                if (l > i) {
+                    const unsigned long long a = sk[i], b = sk[l];
+                    if ((a > b) == ((i & k) == 0)) { sk[i] = b; sk[l] = a; }
+                }
+            }
+            __syncthreads();
+        }
+    }
+    // 6. jitter: clip(0.01 N(0, 1), +-noise_magnitude) by Box-Muller from the row's words, one rounding to fp32
+    const long long o0 = (long long)c * M;
+    for (int r = tid; r < M; r += MN_THREADS) {
+        const int j = (int)(unsigned)(sk[r] & 0xFFFFFFFFull);
+        double x, y, z;
+        point(j, x, y, z);
+        uint32_t w[4];
+        aug_words(w, (uint32_t)j, pair, key, aug_tag(AUG_JITTER, (uint32_t)src));
+        const double r0 = sqrt(-2.0 * log(__dsub_rn(1.0, u32(w[0])))), r1 = sqrt(-2.0 * log(__dsub_rn(1.0, u32(w[2]))));
+        double s0, c0, s1, c1;
+        sincos(__dmul_rn(2.0 * M_PI, u32(w[1])), &s0, &c0);
+        sincos(__dmul_rn(2.0 * M_PI, u32(w[3])), &s1, &c1);
+        const double m = P.noise_magnitude;
+        const double jx = fmin(fmax(__dmul_rn(0.01, __dmul_rn(r0, c0)), -m), m);
+        const double jy = fmin(fmax(__dmul_rn(0.01, __dmul_rn(r0, s0)), -m), m);
+        const double jz = fmin(fmax(__dmul_rn(0.01, __dmul_rn(r1, c1)), -m), m);
+        origin[o0 + r] = j;
+        out[3 * (o0 + r)] = __double2float_rn(__dadd_rn(x, jx));
+        out[3 * (o0 + r) + 1] = __double2float_rn(__dadd_rn(y, jy));
+        out[3 * (o0 + r) + 2] = __double2float_rn(__dadd_rn(z, jz));
+    }
+}
+
+static int next_pow2(int n) {
+    int p = 1;
+    while (p < n) p <<= 1;
+    return p;
+}
+
+static AugKey make_key(uint64_t seed, uint64_t iteration) {
+    return AugKey{(uint32_t)seed, (uint32_t)(seed >> 32), (uint32_t)iteration, (uint32_t)(iteration >> 32)};
+}
+
+}  // namespace geob200
+
+using namespace geob200;
+
+extern "C" {
+
+size_t geob200_augment_pairs_batched_workspace_bytes(int64_t n_rows) {
+    return align_up(4 * (size_t)(n_rows > 0 ? n_rows : 0), 256) + 256;
+}
+
+int geob200_augment_pairs_batched(const float* points, const int64_t* lengths_h, int64_t n_pairs, const float* transforms, int mode,
+                                  int64_t point_limit, double noise, double rotation_factor, double min_scale, double max_scale,
+                                  double shift, uint64_t seed, uint64_t iteration, int64_t pair_base, float* out_points, int32_t* origin,
+                                  float* out_transforms, double* record, void* workspace, size_t workspace_bytes, void* stream) {
+    GEOB_REQUIRE(n_pairs > 0 && 2 * n_pairs <= GEOB_MAX_CLOUDS, "augment_pairs_batched: 1..%d pairs", GEOB_MAX_CLOUDS / 2);
+    GEOB_REQUIRE(mode == GEOB200_AUGMENT_3DMATCH || mode == GEOB200_AUGMENT_KITTI, "augment_pairs_batched: unknown mode %d", mode);
+    GEOB_REQUIRE(point_limit > 0 && point_limit < (1ll << 31), "augment_pairs_batched: point_limit must be in 1..2^31-1");
+    GEOB_REQUIRE(isfinite(noise) && noise >= 0.0, "augment_pairs_batched: noise must be finite and non-negative");
+    GEOB_REQUIRE(isfinite(rotation_factor) && rotation_factor > 0.0, "augment_pairs_batched: rotation_factor must be finite and positive");
+    GEOB_REQUIRE(isfinite(min_scale) && isfinite(max_scale) && min_scale <= max_scale,
+                 "augment_pairs_batched: scales must be finite with min_scale <= max_scale");
+    GEOB_REQUIRE(isfinite(shift) && shift >= 0.0, "augment_pairs_batched: shift must be finite and non-negative");
+    GEOB_REQUIRE(pair_base >= 0 && pair_base + n_pairs <= 0xFFFFFFFFll, "augment_pairs_batched: pair_base out of range");
+    GEOB_REQUIRE(lengths_h != nullptr, "augment_pairs_batched: null lengths");
+    GEOB_REQUIRE(points != nullptr && transforms != nullptr && out_points != nullptr && origin != nullptr && out_transforms != nullptr &&
+                     record != nullptr,
+                 "augment_pairs_batched: null pointer");
+    const int B = (int)n_pairs;
+    int64_t kept[GEOB_MAX_CLOUDS];
+    for (int c = 0; c < 2 * B; ++c) {
+        GEOB_REQUIRE(lengths_h[c] > 0, "augment_pairs_batched: cloud %d is empty", c);
+        kept[c] = lengths_h[c] < point_limit ? lengths_h[c] : point_limit;
+    }
+    Segs In, Out;
+    if (segs_from_counts(&In, 2 * B, lengths_h) || segs_from_counts(&Out, 2 * B, kept)) return -1;
+    const int64_t rows = (int64_t)In.start[2 * B - 1] + In.count[2 * B - 1];
+    GEOB_REQUIRE(workspace != nullptr && workspace_bytes >= geob200_augment_pairs_batched_workspace_bytes(rows),
+                 "augment_pairs_batched: workspace too small");
+    Arena ar(workspace, workspace_bytes);
+    uint32_t* word = ar.take<uint32_t>((size_t)rows);
+    GEOB_REQUIRE(ar.ok(), "augment_pairs_batched: workspace accounting error");
+    cudaStream_t st = (cudaStream_t)stream;
+    const AugKey key = make_key(seed, iteration);
+    point_limit_kernel<<<dim3(1, 2 * B), AUG_THREADS, 0, st>>>(In, Out, B, (int)point_limit, key, (uint32_t)pair_base, word, origin);
+    GEOB_CHECK_LAUNCH();
+    const AugParams P{mode, noise, rotation_factor, min_scale, max_scale, shift};
+    const unsigned gx = (unsigned)((Out.max + AUG_POINT_THREADS - 1) / AUG_POINT_THREADS);
+    augment_points_kernel<<<dim3(gx, 2 * B), AUG_POINT_THREADS, 0, st>>>(points, In, Out, origin, transforms, B, P, key, (uint32_t)pair_base,
+                                                                       out_points, out_transforms, record);
+    GEOB_CHECK_LAUNCH();
+    count_launches(2);
+    return 0;
+}
+
+size_t geob200_modelnet_pairs_batched_workspace_bytes(int64_t n_rows) {
+    return align_up(16 * (size_t)(n_rows > 0 ? n_rows : 0), 256) + 256;
+}
+
+int geob200_modelnet_pairs_batched(const float* shapes, const int64_t* lengths_h, int64_t n_pairs, int64_t num_points, double keep_ratio,
+                                   double rotation_magnitude, double translation_magnitude, double noise_magnitude, uint64_t seed,
+                                   uint64_t iteration, int64_t pair_base, float* out_points, int32_t* origin, float* out_transforms,
+                                   double* record, void* workspace, size_t workspace_bytes, void* stream) {
+    GEOB_REQUIRE(n_pairs > 0 && 2 * n_pairs <= GEOB_MAX_CLOUDS, "modelnet_pairs_batched: 1..%d pairs", GEOB_MAX_CLOUDS / 2);
+    GEOB_REQUIRE(num_points > 0 && num_points <= MN_MAX_POINTS, "modelnet_pairs_batched: num_points must be in 1..%d", MN_MAX_POINTS);
+    GEOB_REQUIRE(isfinite(keep_ratio) && keep_ratio > 0.0 && keep_ratio <= 1.0, "modelnet_pairs_batched: keep_ratio must be in (0, 1]");
+    GEOB_REQUIRE(isfinite(rotation_magnitude) && isfinite(translation_magnitude) && isfinite(noise_magnitude) &&
+                     rotation_magnitude >= 0.0 && translation_magnitude >= 0.0 && noise_magnitude >= 0.0,
+                 "modelnet_pairs_batched: magnitudes must be finite and non-negative");
+    GEOB_REQUIRE(pair_base >= 0 && pair_base + n_pairs <= 0xFFFFFFFFll, "modelnet_pairs_batched: pair_base out of range");
+    GEOB_REQUIRE(lengths_h != nullptr, "modelnet_pairs_batched: null lengths");
+    GEOB_REQUIRE(shapes != nullptr && out_points != nullptr && origin != nullptr && out_transforms != nullptr && record != nullptr,
+                 "modelnet_pairs_batched: null pointer");
+    const int B = (int)n_pairs;
+    int crop_max = 0;
+    for (int p = 0; p < B; ++p) {
+        GEOB_REQUIRE(lengths_h[p] > 0 && lengths_h[p] <= MN_MAX_SHAPE, "modelnet_pairs_batched: shape %d has %lld points (1..%d)", p,
+                     (long long)lengths_h[p], MN_MAX_SHAPE);
+        const int K = crop_count((int)lengths_h[p], keep_ratio);
+        GEOB_REQUIRE(K >= num_points, "modelnet_pairs_batched: shape %d keeps round(%g * %lld) = %d < num_points = %lld points", p,
+                     keep_ratio, (long long)lengths_h[p], K, (long long)num_points);
+        crop_max = K > crop_max ? K : crop_max;
+    }
+    Segs In;
+    if (segs_from_counts(&In, B, lengths_h)) return -1;
+    const int64_t rows = (int64_t)In.start[B - 1] + In.count[B - 1];
+    GEOB_REQUIRE(workspace != nullptr && workspace_bytes >= geob200_modelnet_pairs_batched_workspace_bytes(rows),
+                 "modelnet_pairs_batched: workspace too small");
+    Arena ar(workspace, workspace_bytes);
+    unsigned long long* dkey = ar.take<unsigned long long>(2 * (size_t)rows);
+    GEOB_REQUIRE(ar.ok(), "modelnet_pairs_batched: workspace accounting error");
+    MnParams P{(int)num_points, next_pow2((int)num_points), keep_ratio, rotation_magnitude, translation_magnitude, noise_magnitude};
+    const size_t smem = 3 * MN_THREADS * sizeof(double) + (size_t)P.sort_n * 8 + (size_t)crop_max * 8;
+    if (smem > 48 * 1024 && ensure_max_smem((const void*)modelnet_pairs_kernel)) return -1;
+    modelnet_pairs_kernel<<<dim3(1, 2 * B), MN_THREADS, smem, (cudaStream_t)stream>>>(shapes, In, B, P, crop_max, make_key(seed, iteration),
+                                                                                     (uint32_t)pair_base, dkey, out_points, origin,
+                                                                                     out_transforms, record);
+    GEOB_CHECK_LAUNCH();
+    count_launches(1);
+    return 0;
+}
+
+}  // extern "C"

@@ -11,6 +11,7 @@
 //     pair id = pair_base + p, word 0.  The draw of a pair depends on (seed, iteration, pair id, candidates) only.
 // One CTA per pair; integer shared-memory counters only (no float atomics), so the result is a function of the inputs.
 #include "common.cuh"
+#include "compaction.cuh"
 #include "geob200.h"
 #include "philox.cuh"
 #include "radix_select.cuh"
@@ -23,24 +24,6 @@ __device__ __forceinline__ uint32_t target_word(uint32_t j, uint32_t it_lo, uint
     uint32_t c[4] = {j, it_lo, it_hi, pair};
     philox4x32_10(c, k0, k1);
     return c[0];
-}
-
-// Ordered compaction of one 1024-wide chunk: flag of this thread -> its rank among the flagged threads of the chunk (in thread
-// order); *chunk_total receives the chunk's count.  warp_tot: 32 shared words.
-__device__ __forceinline__ int chunk_rank(bool flag, int* warp_tot, int* chunk_total) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const unsigned bal = __ballot_sync(0xffffffffu, flag);
-    if (lane == 0) warp_tot[warp] = __popc(bal);
-    __syncthreads();
-    int off = __popc(bal & ((1u << lane) - 1u)), tot = 0;
-    for (int w = 0; w < 32; ++w) {
-        const int c = warp_tot[w];
-        off += w < warp ? c : 0;
-        tot += c;
-    }
-    __syncthreads();                       // warp_tot is reused by the next chunk
-    *chunk_total = tot;
-    return off;
 }
 
 // Grid (1, B), ST_THREADS threads.  Pair p reads its gt rows at G.start[p] (first min(gt_count[p], G.count[p]) valid) and writes

@@ -2478,3 +2478,76 @@ def batch_loss_weights(loss_rows, mean_row=None, n_valid=None, found_inf=None):
     L.check(L.lib().geob200_batch_loss_weights(loss_rows.data_ptr(), loss_rows.stride(0), B, w.data_ptr(), mean_row.data_ptr(), L.ptr(n_valid),
                                                found_inf.data_ptr(), L.stream_ptr()), 'batch_loss_weights')
     return w, mean_row
+
+
+AUGMENT_3DMATCH, AUGMENT_KITTI = 0, 1
+AUGMENT_RECORD = 20
+
+
+def _seed_iteration(seed, iteration, what):
+    seed, iteration = int(seed), int(iteration)
+    if not (0 <= seed < 1 << 64 and 0 <= iteration < 1 << 64):
+        raise ValueError(f'{what}: seed and iteration must be 64-bit unsigned integers')
+    return seed, iteration
+
+
+def augment_pairs_batched(points, lengths, transforms, mode, point_limit, noise, rotation_factor=1.0, min_scale=1.0, max_scale=1.0,
+                          shift=0.0, seed=0, iteration=0, pair_base=0):
+    """3DMatch (``mode`` AUGMENT_3DMATCH) / KITTI (AUGMENT_KITTI) training-pair augmentation of B pairs (``geob200_augment_pairs_batched``,
+    two launches).  ``points``: raw clouds stacked [ref_0..ref_{B-1}, src_0..src_{B-1}] with ``lengths`` (2B host ints);
+    ``transforms`` (B, 4, 4) fp32 ground truth.  Pair p draws from the streams (seed, iteration, pair_base + p).  Returns (points,
+    lengths_host (list of min(n, point_limit)), transforms (B, 4, 4) fp32, origin (rows,) int32 = each row's row in its input cloud,
+    record (B, 20) fp64 = [u0..u10 | R]).  No host synchronisation."""
+    _f(points, 'points'); _f(transforms, 'transforms')
+    lengths = [int(v) for v in lengths]
+    B = len(lengths) // 2
+    if B < 1 or len(lengths) != 2 * B:
+        raise RuntimeError('augment_pairs_batched: lengths must hold 2B counts')
+    if points.dim() != 2 or points.shape[1] != 3 or points.shape[0] != sum(lengths):
+        raise RuntimeError(f'augment_pairs_batched: points must be (sum(lengths), 3), got {tuple(points.shape)}')
+    if transforms.numel() != 16 * B:
+        raise RuntimeError(f'augment_pairs_batched: transforms must be ({B}, 4, 4)')
+    seed, iteration = _seed_iteration(seed, iteration, 'augment_pairs_batched')
+    limit = int(point_limit)
+    out_len = [min(n, limit) for n in lengths]
+    dev = points.device
+    lib = L.lib()
+    ws = L.workspace(lib.geob200_augment_pairs_batched_workspace_bytes(sum(lengths)), dev, tag='augment')
+    out = torch.empty((sum(out_len), 3), dtype=_f32, device=dev)
+    origin = torch.empty((sum(out_len),), dtype=_i32, device=dev)
+    T = torch.empty((B, 4, 4), dtype=_f32, device=dev)
+    record = torch.empty((B, AUGMENT_RECORD), dtype=torch.float64, device=dev)
+    L.check(lib.geob200_augment_pairs_batched(points.data_ptr(), _host_i64(lengths), B, transforms.data_ptr(), int(mode), limit, float(noise),
+                                              float(rotation_factor), float(min_scale), float(max_scale), float(shift), seed, iteration,
+                                              int(pair_base), out.data_ptr(), origin.data_ptr(), T.data_ptr(), record.data_ptr(),
+                                              ws.data_ptr(), ws.numel(), L.stream_ptr()), 'augment_pairs_batched')
+    return out, out_len, T, origin, record
+
+
+def modelnet_pairs_batched(shapes, lengths, num_points, keep_ratio, rotation_magnitude, translation_magnitude, noise_magnitude, seed=0,
+                           iteration=0, pair_base=0):
+    """ModelNet training pairs from B raw shapes (``geob200_modelnet_pairs_batched``, one launch): ``shapes`` stacked with ``lengths``
+    (B host ints, each <= 8192 with round(keep_ratio N) >= num_points).  Returns (points (2B num_points, 3) stacked [ref..., src...],
+    lengths_host, transforms (B, 4, 4) fp32, origin (int32, the raw shape row of every output row), record (B, 20) fp64).  No host
+    synchronisation."""
+    _f(shapes, 'shapes')
+    lengths = [int(v) for v in lengths]
+    B = len(lengths)
+    if B < 1:
+        raise RuntimeError('modelnet_pairs_batched: no shapes')
+    if shapes.dim() != 2 or shapes.shape[1] != 3 or shapes.shape[0] != sum(lengths):
+        raise RuntimeError(f'modelnet_pairs_batched: shapes must be (sum(lengths), 3), got {tuple(shapes.shape)}')
+    seed, iteration = _seed_iteration(seed, iteration, 'modelnet_pairs_batched')
+    m = int(num_points)
+    dev = shapes.device
+    lib = L.lib()
+    ws = L.workspace(lib.geob200_modelnet_pairs_batched_workspace_bytes(sum(lengths)), dev, tag='augment')
+    out = torch.empty((2 * B * max(m, 0), 3), dtype=_f32, device=dev)
+    origin = torch.empty((2 * B * max(m, 0),), dtype=_i32, device=dev)
+    T = torch.empty((B, 4, 4), dtype=_f32, device=dev)
+    record = torch.empty((B, AUGMENT_RECORD), dtype=torch.float64, device=dev)
+    L.check(lib.geob200_modelnet_pairs_batched(shapes.data_ptr(), _host_i64(lengths), B, m, float(keep_ratio), float(rotation_magnitude),
+                                               float(translation_magnitude), float(noise_magnitude), seed, iteration, int(pair_base),
+                                               out.data_ptr(), origin.data_ptr(), T.data_ptr(), record.data_ptr(), ws.data_ptr(),
+                                               ws.numel(), L.stream_ptr()), 'modelnet_pairs_batched')
+    return out, [m] * (2 * B), T, origin, record

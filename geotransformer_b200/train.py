@@ -95,17 +95,24 @@ MAX_BATCH = GF.ATT_MAX_ITEMS // 2
 
 
 class TrainingEngine:
-    def __init__(self, model, cfg, neighbor_limits, seed=None, device=None, batch_size=1, scale_lr=True):
+    def __init__(self, model, cfg, neighbor_limits, seed=None, device=None, batch_size=1, scale_lr=True, augment=False):
         """``model``: a GeoTransformer on its device with its weights loaded.  ``seed`` keys the target sampler's Philox stream
         (default ``cfg.seed``); target draws depend on (seed, iteration, pair) only, so a resumed run draws what an uninterrupted one
         would.  ``batch_size``: pairs per ``train_batch`` step (1 .. MAX_BATCH); with ``scale_lr`` every param group's lr is
-        multiplied by it before the scheduler is built (the reference scales by the DDP world size in ``register_optimizer``)."""
+        multiplied by it before the scheduler is built (the reference scales by the DDP world size in ``register_optimizer``).
+        ``augment``: every step trains on its pairs augmented on the device as the reference's training set does
+        (``augment.augmented_collate`` with (seed, iteration); pair p of a step draws from stream p); for ModelNet a pair is then a raw
+        shape ``{'points': (N, 3)}``.  Off: the pairs are trained on as given."""
         if cfg.optim.grad_acc_steps != 1:
             raise NotImplementedError('grad_acc_steps > 1 (1 in every shipped config)')
         if not 1 <= int(batch_size) <= MAX_BATCH:
             raise ValueError(f'batch_size must be in 1..{MAX_BATCH}')
         self.model, self.cfg, self.limits = model, cfg, neighbor_limits
         self.batch_size = int(batch_size)
+        self.augment = bool(augment)
+        if self.augment:
+            from .augment import check_options
+            check_options(cfg)
         self.seed = int(cfg.seed if seed is None else seed)
         self.device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
         self.loss_func = OverallLoss(cfg)
@@ -130,10 +137,10 @@ class TrainingEngine:
         """one optimisation step on ``pair`` (dict with ref_points / src_points / ref_feats / src_feats / transform); returns the
         reference's train_step result: loss, c_loss, f_loss and the Evaluator's metrics (no RMSE for KITTI), plus ``lr`` (of this
         step) and ``skipped`` (a non-finite gradient: no update)"""
-        model, b = self.model, self.cfg.backbone
+        model = self.model
         self.iteration += 1
         self._mark('start')
-        data = registration_collate_fn_stack_mode([pair], b.num_stages, b.init_voxel_size, b.init_radius, self.limits, device=self.device)
+        data = self._collate([pair])
         self._mark('collate')
         out = model.forward_train(data, self.seed, self.iteration)
         self._mark('forward')
@@ -185,10 +192,10 @@ class TrainingEngine:
         B = len(pairs)
         if not 1 <= B <= self.batch_size:
             raise ValueError(f'train_batch: 1..{self.batch_size} pairs per step, got {B}')
-        model, b = self.model, self.cfg.backbone
+        model = self.model
         self.iteration += 1
         self._mark('start')
-        data = registration_collate_fn_stack_mode(list(pairs), b.num_stages, b.init_voxel_size, b.init_radius, self.limits, device=self.device)
+        data = self._collate(list(pairs))
         self._mark('collate')
         out = model.forward_train_batch(data, self.seed, self.iteration)
         self._mark('forward')
@@ -236,6 +243,14 @@ class TrainingEngine:
         res['skipped'] = v[11] != 0.0
         res['per_pair'] = [self._result(v[_ROW + 1 + p * _PAIR_ROW:_ROW + 1 + (p + 1) * _PAIR_ROW]) for p in range(B)]
         return res
+
+    def _collate(self, pairs):
+        """the step's collate: the plain stack-mode collate, or with ``augment`` the device augmentation keyed by (seed, iteration)"""
+        if self.augment:
+            from .augment import augmented_collate
+            return augmented_collate(pairs, self.cfg, self.limits, self.seed, self.iteration, device=self.device)
+        b = self.cfg.backbone
+        return registration_collate_fn_stack_mode(pairs, b.num_stages, b.init_voxel_size, b.init_radius, self.limits, device=self.device)
 
     def _packed(self, B):
         """the device buffer of one batched step's results: [the step row (_ROW) | n_valid | B per-pair rows], and its pinned mirror"""

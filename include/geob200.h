@@ -715,6 +715,56 @@ int geob200_nonfinite_check(const float* const* ptrs, const int64_t* numels, int
 int geob200_batch_loss_weights(const float* loss_rows, int64_t ld_rows, int64_t n_pairs, float* weights, float* mean_row, float* n_valid,
                                float* found_inf, void* stream);
 
+/* ---- training-data augmentation (datasets/registration/{threedmatch,kitti,modelnet}/dataset.py) -------------------------------
+ *
+ * Random streams.  Every draw is Philox4x32-10 (the generator of the target sampler and RANSAC) with
+ *   key     = (seed lo, seed hi ^ tag),  tag = GEOB200_AUGMENT_TAG_BASE | stream << 4 | cloud  (cloud 0 = ref, 1 = src),
+ *             stream 1 pair draws (cloud 0 only), 2 point-limit keys, 3 noise, 4 sample keys, 5 jitter;
+ *   counter = (index, iteration lo, iteration hi, pair_base + p).
+ * The target sampler and RANSAC use tag 0, so no augmentation stream shares their key.
+ * Pair draws: call i (index i) gives u_{2i} = ((w0 >> 5) 2^26 + (w1 >> 6)) 2^-53 and u_{2i+1} from (w2, w3) likewise.
+ *   3DMatch: u0..u2 Euler angles 2 pi u / rotation_factor, u3 the coin (u3 > 0.5 rotates ref, else src);
+ *   KITTI:   additionally u4 scale min + (max - min) u4, u5..u7 ref shift -s + 2s u, u8..u10 src shift;
+ *   ModelNet: u0..u2 Euler angles pi rotation_magnitude / 180 u, u3..u5 translation -m + 2m u, (u6, u7) ref plane and (u8, u9) src
+ *   plane: phi = 2 pi u, theta = pi u, normal (sin theta cos phi, sin theta sin phi, cos theta).
+ *   R = scipy's Rotation.from_euler('zyx', (a, b, c)) = Rx(c) Ry(b) Rz(a).
+ * Per-point words: index = the point's row in its input cloud (raw shape for ModelNet); uniforms w 2^-32.
+ *   point limit: key (w0 << 32) | row;  noise: u = w0, w1, w2;  sample: key (w0 << 32) | row;  jitter: Box-Muller
+ *   z0, z1 = sqrt(-2 ln(1 - u0)) (cos, sin)(2 pi u1), z2 = sqrt(-2 ln(1 - u2)) cos(2 pi u3).
+ * record (n_pairs, 20) fp64: [u0 .. u10 | R row-major], unused slots 0.  transforms / out_transforms: (n_pairs, 4, 4) fp32. */
+#define GEOB200_AUGMENT_3DMATCH 0
+#define GEOB200_AUGMENT_KITTI 1
+#define GEOB200_AUGMENT_TAG_BASE 0xA6000000u
+
+/* 3DMatch / KITTI training-pair augmentation, two launches for any n_pairs (1 .. 32).  points: raw clouds stacked
+ * [ref_0..ref_{B-1}, src_0..src_{B-1}] with host lengths_h[2B] (each >= 1); transforms (B, 4, 4) ground truth (ref = T src).
+ * Cloud c keeps min(n_c, point_limit) rows: all in order when n_c <= point_limit, else the point_limit smallest point-limit keys
+ * in ascending row (a uniform subset).  origin (int32, same rows as out_points): the row of each output point in its input cloud.
+ * Per point, in fp64 with every operation rounded (no contraction) and one rounding to fp32:
+ *   3DMATCH: rotate (rows of R, ((r0 x + r1 y) + r2 z)) if this cloud is the rotated one, then + (u - 0.5) noise;
+ *   KITTI:   + (u - 0.5) noise, rotate if rotated, * scale, + this cloud's shift.
+ * out_transforms: rotated ref -> (R R_gt, R t_gt); rotated src -> (R_gt R^T, t_gt); KITTI then t = (-(R' src_shift) + scale t)
+ * + ref_shift; computed in fp64 and rounded once.  workspace: geob200_augment_pairs_batched_workspace_bytes(sum of lengths). */
+size_t geob200_augment_pairs_batched_workspace_bytes(int64_t n_rows);
+int geob200_augment_pairs_batched(const float* points, const int64_t* lengths_h, int64_t n_pairs, const float* transforms, int mode,
+                                  int64_t point_limit, double noise, double rotation_factor, double min_scale, double max_scale,
+                                  double shift, uint64_t seed, uint64_t iteration, int64_t pair_base, float* out_points, int32_t* origin,
+                                  float* out_transforms, double* record, void* workspace, size_t workspace_bytes, void* stream);
+
+/* ModelNet pair synthesis (twice_sample, plane crop), one launch with one CTA per cloud for any n_pairs (1 .. 32).  shapes: B raw
+ * shapes stacked with host lengths_h[B], each 1 .. 8192 points with round(keep_ratio N) = floor(N keep_ratio + 0.5) >= num_points
+ * (1 .. 4096).  Per cloud, in fp64: normalise (subtract the mean, divide by the largest norm); src only: apply the inverse of the
+ * drawn transform; crop to the round(keep_ratio N) largest plane distances dot(p, n), ties to the lowest row; keep the num_points
+ * smallest sample keys of the cropped points and write them in key order (a uniformly random ordered subset); add the jitter
+ * clip(0.01 z, +-noise_magnitude); round to fp32.  out_points (2B num_points, 3) stacked [ref..., src...]; origin: the raw shape
+ * row; out_transforms: the drawn transform (ref = T src).  workspace: geob200_modelnet_pairs_batched_workspace_bytes(sum of
+ * lengths). */
+size_t geob200_modelnet_pairs_batched_workspace_bytes(int64_t n_rows);
+int geob200_modelnet_pairs_batched(const float* shapes, const int64_t* lengths_h, int64_t n_pairs, int64_t num_points, double keep_ratio,
+                                   double rotation_magnitude, double translation_magnitude, double noise_magnitude, uint64_t seed,
+                                   uint64_t iteration, int64_t pair_base, float* out_points, int32_t* origin, float* out_transforms,
+                                   double* record, void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
