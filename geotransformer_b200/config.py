@@ -85,6 +85,8 @@ def make_cfg(name='3dmatch'):
         c.data = Cfg(num_points=717, voxel_size=None, rotation_magnitude=45.0, translation_magnitude=0.5, keep_ratio=0.7,
                      crop_method='plane', asymmetric=True, twice_sample=True, twice_transform=False)
         c.train = Cfg(noise_magnitude=0.05, class_indices='all')
+        # validation and test pairs (config.py:53-54; datasets/modelnet.py)
+        c.test = Cfg(noise_magnitude=0.05, class_indices='all')
         c.neighbor_limits = None
     else:
         raise ValueError(f'unknown config {name}')

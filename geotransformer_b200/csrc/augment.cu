@@ -9,10 +9,15 @@
 // (seed, iteration, pair id) only -- never of the launch geometry or the rest of the batch.  The per-point arithmetic of the
 // 3DMatch / KITTI modes is fp64 with explicit roundings (__dmul_rn / __dadd_rn: no contraction) and one rounding to fp32, so its
 // numpy restatement (oracle/augment_oracle.py) reproduces it bit for bit.  No float atomics.
+//
+// ModelNet's validation and test pairs (deterministic=True) are the exception: the reference seeds numpy's global generator with
+// the pair's dataset index, so modelnet_benchmark_kernel draws from numpy's own legacy stream (numpy_random.cuh) in the reference's
+// order and reproduces its pairs bit for bit (oracle/modelnet_benchmark_oracle.py).
 #include "common.cuh"
 #include "compaction.cuh"
 #include "geob200.h"
 #include "philox.cuh"
+#include "numpy_random.cuh"
 #include "radix_select.cuh"
 
 namespace geob200 {
@@ -505,6 +510,230 @@ __global__ void __launch_bounds__(MN_THREADS) modelnet_pairs_kernel(
     }
 }
 
+// ---- ModelNet validation / test pairs (deterministic) -------------------------------------------------------------------------
+
+constexpr int MNB_THREADS = 256;
+constexpr int MNB_MAX_PAIRS = 1024;        // pairs per launch; the entry point splits larger calls
+
+struct MnbPair {
+    long long start;                       // first row of the shape in `shapes`
+    int count;                             // its points
+    uint32_t index;                        // the dataset index, which seeds the pair's stream
+};
+
+// scipy's Rotation.from_euler('zyx', (a, b, c)).as_matrix() in scipy's own arithmetic: elementary quaternions (axis sin(angle / 2),
+// cos(angle / 2)), composed extrinsically q = qx(c) (qy(b) qz(a)) without normalisation, then the matrix of q.  euler_zyx's
+// direct product is the same rotation but not the same bits.
+__device__ __forceinline__ void quat_compose(const double (&p)[4], const double (&q)[4], double (&r)[4]) {
+    const double c0 = __dsub_rn(__dmul_rn(p[1], q[2]), __dmul_rn(p[2], q[1]));
+    const double c1 = __dsub_rn(__dmul_rn(p[2], q[0]), __dmul_rn(p[0], q[2]));
+    const double c2 = __dsub_rn(__dmul_rn(p[0], q[1]), __dmul_rn(p[1], q[0]));
+    r[0] = __dadd_rn(__dadd_rn(__dmul_rn(p[3], q[0]), __dmul_rn(q[3], p[0])), c0);
+    r[1] = __dadd_rn(__dadd_rn(__dmul_rn(p[3], q[1]), __dmul_rn(q[3], p[1])), c1);
+    r[2] = __dadd_rn(__dadd_rn(__dmul_rn(p[3], q[2]), __dmul_rn(q[3], p[2])), c2);
+    r[3] = __dsub_rn(__dmul_rn(p[3], q[3]),
+                     __dadd_rn(__dadd_rn(__dmul_rn(p[0], q[0]), __dmul_rn(p[1], q[1])), __dmul_rn(p[2], q[2])));
+}
+
+__device__ __forceinline__ void euler_zyx_scipy(double a, double b, double c, double (&R)[9]) {
+    double qz[4] = {0.0, 0.0, 0.0, 0.0}, qy[4] = {0.0, 0.0, 0.0, 0.0}, qx[4] = {0.0, 0.0, 0.0, 0.0}, t[4], q[4];
+    sincos(__dmul_rn(a, 0.5), &qz[2], &qz[3]);
+    sincos(__dmul_rn(b, 0.5), &qy[1], &qy[3]);
+    sincos(__dmul_rn(c, 0.5), &qx[0], &qx[3]);
+    quat_compose(qy, qz, t);
+    quat_compose(qx, t, q);
+    const double x2 = __dmul_rn(q[0], q[0]), y2 = __dmul_rn(q[1], q[1]), z2 = __dmul_rn(q[2], q[2]), w2 = __dmul_rn(q[3], q[3]);
+    const double xy = __dmul_rn(q[0], q[1]), zw = __dmul_rn(q[2], q[3]), xz = __dmul_rn(q[0], q[2]);
+    const double yw = __dmul_rn(q[1], q[3]), yz = __dmul_rn(q[1], q[2]), xw = __dmul_rn(q[0], q[3]);
+    R[0] = __dadd_rn(__dsub_rn(__dsub_rn(x2, y2), z2), w2);
+    R[1] = __dmul_rn(2.0, __dsub_rn(xy, zw));
+    R[2] = __dmul_rn(2.0, __dadd_rn(xz, yw));
+    R[3] = __dmul_rn(2.0, __dadd_rn(xy, zw));
+    R[4] = __dadd_rn(__dsub_rn(__dadd_rn(-x2, y2), z2), w2);
+    R[5] = __dmul_rn(2.0, __dsub_rn(yz, xw));
+    R[6] = __dmul_rn(2.0, __dsub_rn(xz, yw));
+    R[7] = __dmul_rn(2.0, __dadd_rn(yz, xw));
+    R[8] = __dadd_rn(__dadd_rn(__dsub_rn(-x2, y2), z2), w2);
+}
+
+// The permutation(n) of the stream (arange, then for i = n-1 .. 1 swap i with interval(i)) left in perm[0 .. n); lane 0 swaps.
+__device__ __forceinline__ void legacy_permutation(LegacyRandom& rng, int* perm, int n) {
+    const int lane = threadIdx.x & 31;
+    for (int i = lane; i < n; i += 32) perm[i] = i;
+    __syncwarp();
+    for (int i = n - 1; i > 0; --i) {
+        const int j = (int)rng.interval((uint32_t)i);
+        if (lane == 0) {
+            const int a = perm[i];
+            perm[i] = perm[j];
+            perm[j] = a;
+        }
+    }
+    __syncwarp();
+}
+
+// Every draw of one pair, in the reference's order, by the whole of warp 0 (warp-uniform): prm = [R (9), t (3), ref plane normal
+// (3), src plane normal (3), inverse translation -(R^T t) (3)]; sel (2 x M): the sampled positions in each cloud's crop order
+// (random_sample_points, padding included); shuf (2 x M): each cloud's final shuffle; jit (6 M, global): the clipped jitter of
+// ref then src in the order drawn; scratch: K words.
+__device__ __forceinline__ void mnb_draws(uint32_t index, int K, const MnParams& P, uint32_t* mt, double* prm, int* scratch, int* sel,
+                                       int* shuf, double* jit, float* T_out) {
+    const int lane = threadIdx.x & 31, M = P.num_points;
+    LegacyRandom rng{mt, 0, false, 0.0};
+    rng.seed(index);
+    // random_sample_transform: rand(3) pi magnitude / 180, Rotation.from_euler('zyx'); uniform(-m, m, 3)
+    double e[3], t[3], R[9];
+#pragma unroll
+    for (int i = 0; i < 3; ++i) e[i] = __ddiv_rn(__dmul_rn(__dmul_rn(rng.next_double(), M_PI), P.rotation_magnitude), 180.0);
+#pragma unroll
+    for (int i = 0; i < 3; ++i) t[i] = rng.uniform(-P.translation_magnitude, P.translation_magnitude);
+    euler_zyx_scipy(e[0], e[1], e[2], R);
+    // random_sample_plane of ref, then of src: phi = uniform(0, 2 pi), theta = uniform(0, pi)
+    double nrm[6];
+#pragma unroll
+    for (int c = 0; c < 2; ++c) {
+        const double phi = rng.uniform(0.0, 2.0 * M_PI), theta = rng.uniform(0.0, M_PI);
+        double sp, cp, st, ct;
+        sincos(phi, &sp, &cp); sincos(theta, &st, &ct);
+        nrm[3 * c] = __dmul_rn(st, cp); nrm[3 * c + 1] = __dmul_rn(st, sp); nrm[3 * c + 2] = ct;
+    }
+    if (lane == 0) {
+#pragma unroll
+        for (int i = 0; i < 9; ++i) prm[i] = R[i];
+#pragma unroll
+        for (int i = 0; i < 3; ++i) prm[9 + i] = t[i];
+#pragma unroll
+        for (int i = 0; i < 6; ++i) prm[12 + i] = nrm[i];
+#pragma unroll
+        for (int i = 0; i < 3; ++i) prm[18 + i] = -col_dot(R, i, t[0], t[1], t[2]);
+#pragma unroll
+        for (int i = 0; i < 3; ++i) {
+#pragma unroll
+            for (int j = 0; j < 3; ++j) T_out[4 * i + j] = __double2float_rn(R[3 * i + j]);
+            T_out[4 * i + 3] = __double2float_rn(t[i]);
+            T_out[12 + i] = 0.0f;
+        }
+        T_out[15] = 1.0f;
+    }
+    // random_sample_points of ref, then of src: the first M of permutation(K), or the permutation repeated and its head
+    for (int c = 0; c < 2; ++c) {
+        legacy_permutation(rng, scratch, K);
+        for (int r = lane; r < M; r += 32) sel[c * M + r] = scratch[r % K];
+        __syncwarp();
+    }
+    // random_jitter_points of ref, then of src: clip(0 + 0.01 gauss, +-noise_magnitude); the Gaussian cached by the last ref draw
+    // (3 M odd) is the first of src
+    for (int k = 0; k < 6 * M; ++k) {
+        const double g = fmin(fmax(__dadd_rn(0.0, __dmul_rn(0.01, rng.gauss_draw())), -P.noise_magnitude), P.noise_magnitude);
+        if (lane == 0) jit[k] = g;
+    }
+    // random_shuffle_points of ref, then of src
+    legacy_permutation(rng, shuf, M);
+    legacy_permutation(rng, shuf + M, M);
+}
+
+// One CTA per pair, grid (n, 1), MNB_THREADS.  Warp 0 consumes the pair's stream (mnb_draws) while warp 1 normalises the shape in
+// fp32; then the CTA orders each cloud's crop (bitonic sort of (distance desc, row asc)), maps the samples to shape rows, and writes
+// the jittered, shuffled points.  Dynamic shared memory: sort keys and rows (sort_n each; the draws' scratch aliases them), sel and
+// shuf (2 M each).  jit: workspace, 6 M doubles per pair of the launch.
+__global__ void __launch_bounds__(MNB_THREADS) modelnet_benchmark_kernel(
+        const float* __restrict__ shapes, const MnbPair* __restrict__ pairs, int total_pairs, int pair0, MnParams P,
+        double* __restrict__ jit_ws, float* __restrict__ out, int* __restrict__ origin, float* __restrict__ T_out) {
+    extern __shared__ __align__(16) unsigned char smem[];
+    unsigned long long* skey = reinterpret_cast<unsigned long long*>(smem);
+    int* srow = reinterpret_cast<int*>(skey + P.sort_n);
+    int* sel = srow + P.sort_n;
+    int* shuf = sel + 2 * P.num_points;
+    __shared__ uint32_t mt[MT_N];
+    __shared__ double prm[21];
+    __shared__ float mean_s[3], scale_s;
+    const int q = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, M = P.num_points;
+    const MnbPair pr = pairs[q];
+    const int N = pr.count, K = crop_count(N, P.keep_ratio);
+    const float* pts = shapes + 3ll * pr.start;
+    double* jit = jit_ws + 6ll * M * q;
+
+    if (warp == 0) {
+        mnb_draws(pr.index, K, P, mt, prm, reinterpret_cast<int*>(skey), sel, shuf, jit, T_out + 16ll * (pair0 + q));
+    } else if (warp == 1) {
+        // normalize_points in fp32: column sums in row order, / N; then the largest sqrt((x^2 + y^2) + z^2) of the centred points
+        if (lane < 3) {
+            float s = 0.0f;
+            for (int j = 0; j < N; ++j) s = __fadd_rn(s, pts[3 * j + lane]);
+            mean_s[lane] = __fdiv_rn(s, (float)N);
+        }
+        __syncwarp();
+        const float mx = mean_s[0], my = mean_s[1], mz = mean_s[2];
+        float nmax = 0.0f;
+        for (int j = lane; j < N; j += 32) {
+            const float x = __fsub_rn(pts[3 * j], mx), y = __fsub_rn(pts[3 * j + 1], my), z = __fsub_rn(pts[3 * j + 2], mz);
+            nmax = fmaxf(nmax, __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y)), __fmul_rn(z, z))));
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) nmax = fmaxf(nmax, __shfl_xor_sync(0xffffffffu, nmax, o));
+        if (lane == 0) scale_s = nmax;
+    }
+    __syncthreads();
+    const float mx = mean_s[0], my = mean_s[1], mz = mean_s[2], scale = scale_s;
+    // point j of cloud c: the normalised fp32 point, and for src its image p R + (-(R^T t)) in fp64
+    auto point = [&](int c, int j, double& x, double& y, double& z) {
+        x = (double)__fdiv_rn(__fsub_rn(pts[3 * j], mx), scale);
+        y = (double)__fdiv_rn(__fsub_rn(pts[3 * j + 1], my), scale);
+        z = (double)__fdiv_rn(__fsub_rn(pts[3 * j + 2], mz), scale);
+        if (c) {
+            const double a = __dadd_rn(col_dot(prm, 0, x, y, z), prm[18]);
+            const double b = __dadd_rn(col_dot(prm, 1, x, y, z), prm[19]);
+            const double d = __dadd_rn(col_dot(prm, 2, x, y, z), prm[20]);
+            x = a; y = b; z = d;
+        }
+    };
+    for (int c = 0; c < 2; ++c) {
+        // random_crop_point_cloud_with_plane: rows by descending (x nx + y ny) + z nz, ties to the lowest row; sorted ascending on
+        // (~ordered_key(d), row)
+        const double n0 = prm[12 + 3 * c], n1 = prm[13 + 3 * c], n2 = prm[14 + 3 * c];
+        for (int j = tid; j < P.sort_n; j += MNB_THREADS) {
+            unsigned long long k = ~0ull;
+            if (j < N) {
+                double x, y, z;
+                point(c, j, x, y, z);
+                k = ~ordered_key(__dadd_rn(__dadd_rn(__dmul_rn(x, n0), __dmul_rn(y, n1)), __dmul_rn(z, n2)));
+            }
+            skey[j] = k;
+            srow[j] = j < N ? j : 0x7fffffff;
+        }
+        __syncthreads();
+        for (int k = 2; k <= P.sort_n; k <<= 1) {          // bitonic sort, ascending
+            for (int h = k >> 1; h > 0; h >>= 1) {
+                for (int i = tid; i < P.sort_n; i += MNB_THREADS) {
+                    const int l = i ^ h;
+                    if (l > i) {
+                        const unsigned long long a = skey[i], b = skey[l];
+                        const int ra = srow[i], rb = srow[l];
+                        const bool gt = a > b || (a == b && ra > rb);
+                        if (gt == ((i & k) == 0)) { skey[i] = b; skey[l] = a; srow[i] = rb; srow[l] = ra; }
+                    }
+                }
+                __syncthreads();
+            }
+        }
+        // crop position -> shape row
+        for (int r = tid; r < M; r += MNB_THREADS) sel[c * M + r] = srow[sel[c * M + r]];
+        __syncthreads();
+    }
+    // jitter, shuffle, round to fp32: output s of cloud c is sample shuf[s] of that cloud
+    for (int i = tid; i < 2 * M; i += MNB_THREADS) {
+        const int c = i >= M ? 1 : 0, s = i - c * M, k = shuf[c * M + s], row = sel[c * M + k];
+        double x, y, z;
+        point(c, row, x, y, z);
+        const double* g = jit + 3ll * (c * M + k);
+        const long long o = ((long long)c * total_pairs + pair0 + q) * M + s;
+        origin[o] = row;
+        out[3 * o] = __double2float_rn(__dadd_rn(x, g[0]));
+        out[3 * o + 1] = __double2float_rn(__dadd_rn(y, g[1]));
+        out[3 * o + 2] = __double2float_rn(__dadd_rn(z, g[2]));
+    }
+}
+
 static int next_pow2(int n) {
     int p = 1;
     while (p < n) p <<= 1;
@@ -613,6 +842,70 @@ int geob200_modelnet_pairs_batched(const float* shapes, const int64_t* lengths_h
                                                                                      out_transforms, record);
     GEOB_CHECK_LAUNCH();
     count_launches(1);
+    return 0;
+}
+
+size_t geob200_modelnet_benchmark_pairs_batched_workspace_bytes(int64_t n_pairs, int64_t num_points) {
+    const size_t b = (size_t)(n_pairs < 1 ? 0 : n_pairs < MNB_MAX_PAIRS ? n_pairs : MNB_MAX_PAIRS);
+    const size_t m = (size_t)(num_points > 0 ? num_points : 0);
+    return align_up(b * sizeof(MnbPair), 256) + align_up(b * 6 * m * sizeof(double), 256) + 256;
+}
+
+int geob200_modelnet_benchmark_pairs_batched(const float* shapes, const int64_t* lengths_h, const int64_t* indices_h, int64_t n_pairs,
+                                             int64_t num_points, double keep_ratio, double rotation_magnitude, double translation_magnitude,
+                                             double noise_magnitude, float* out_points, int32_t* origin, float* out_transforms,
+                                             void* workspace, size_t workspace_bytes, void* stream) {
+    GEOB_REQUIRE(n_pairs > 0 && n_pairs < (1ll << 31) / MN_MAX_POINTS / 2, "modelnet_benchmark_pairs_batched: n_pairs must be in 1..%lld",
+                 (1ll << 31) / MN_MAX_POINTS / 2 - 1);
+    GEOB_REQUIRE(num_points > 0 && num_points <= MN_MAX_POINTS, "modelnet_benchmark_pairs_batched: num_points must be in 1..%d",
+                 MN_MAX_POINTS);
+    GEOB_REQUIRE(isfinite(keep_ratio) && keep_ratio > 0.0 && keep_ratio <= 1.0,
+                 "modelnet_benchmark_pairs_batched: keep_ratio must be in (0, 1]");
+    GEOB_REQUIRE(isfinite(rotation_magnitude) && isfinite(translation_magnitude) && isfinite(noise_magnitude) &&
+                     rotation_magnitude >= 0.0 && translation_magnitude >= 0.0 && noise_magnitude >= 0.0,
+                 "modelnet_benchmark_pairs_batched: magnitudes must be finite and non-negative");
+    GEOB_REQUIRE(lengths_h != nullptr && indices_h != nullptr, "modelnet_benchmark_pairs_batched: null lengths or indices");
+    GEOB_REQUIRE(shapes != nullptr && out_points != nullptr && origin != nullptr && out_transforms != nullptr,
+                 "modelnet_benchmark_pairs_batched: null pointer");
+    for (int64_t p = 0; p < n_pairs; ++p) {
+        GEOB_REQUIRE(lengths_h[p] > 0 && lengths_h[p] <= MN_MAX_SHAPE, "modelnet_benchmark_pairs_batched: shape %lld has %lld points (1..%d)",
+                     (long long)p, (long long)lengths_h[p], MN_MAX_SHAPE);
+        GEOB_REQUIRE(crop_count((int)lengths_h[p], keep_ratio) >= 1, "modelnet_benchmark_pairs_batched: shape %lld keeps no point",
+                     (long long)p);
+        GEOB_REQUIRE(indices_h[p] >= 0 && indices_h[p] <= 0xFFFFFFFFll, "modelnet_benchmark_pairs_batched: index %lld of pair %lld is "
+                     "not in 0..2^32-1", (long long)indices_h[p], (long long)p);
+    }
+    GEOB_REQUIRE(workspace != nullptr &&
+                     workspace_bytes >= geob200_modelnet_benchmark_pairs_batched_workspace_bytes(n_pairs, num_points),
+                 "modelnet_benchmark_pairs_batched: workspace too small");
+    const int B = (int)n_pairs, M = (int)num_points;
+    const int cap = B < MNB_MAX_PAIRS ? B : MNB_MAX_PAIRS;
+    Arena ar(workspace, workspace_bytes);
+    MnbPair* table = ar.take<MnbPair>((size_t)cap);
+    double* jit = ar.take<double>((size_t)cap * 6 * M);
+    GEOB_REQUIRE(ar.ok(), "modelnet_benchmark_pairs_batched: workspace accounting error");
+    cudaStream_t st = (cudaStream_t)stream;
+    MnbPair host[MNB_MAX_PAIRS];
+    long long start = 0;
+    int launches = 0;
+    for (int p0 = 0; p0 < B; p0 += cap) {
+        const int n = B - p0 < cap ? B - p0 : cap;
+        int nmax = 1;
+        for (int q = 0; q < n; ++q) {
+            host[q] = MnbPair{start, (int)lengths_h[p0 + q], (uint32_t)indices_h[p0 + q]};
+            start += lengths_h[p0 + q];
+            nmax = host[q].count > nmax ? host[q].count : nmax;
+        }
+        // from pageable memory: staged before the call returns, ordered before the launch on the stream
+        GEOB_CHECK_CUDA(cudaMemcpyAsync(table, host, (size_t)n * sizeof(MnbPair), cudaMemcpyHostToDevice, st));
+        const MnParams P{M, next_pow2(nmax), keep_ratio, rotation_magnitude, translation_magnitude, noise_magnitude};
+        const size_t smem = (size_t)P.sort_n * (sizeof(unsigned long long) + sizeof(int)) + (size_t)4 * M * sizeof(int);
+        if (smem > 48 * 1024 && ensure_max_smem((const void*)modelnet_benchmark_kernel)) return -1;
+        modelnet_benchmark_kernel<<<n, MNB_THREADS, smem, st>>>(shapes, table, B, p0, P, jit, out_points, origin, out_transforms);
+        GEOB_CHECK_LAUNCH();
+        ++launches;
+    }
+    count_launches(launches);
     return 0;
 }
 

@@ -2551,3 +2551,34 @@ def modelnet_pairs_batched(shapes, lengths, num_points, keep_ratio, rotation_mag
                                                out.data_ptr(), origin.data_ptr(), T.data_ptr(), record.data_ptr(), ws.data_ptr(),
                                                ws.numel(), L.stream_ptr()), 'modelnet_pairs_batched')
     return out, [m] * (2 * B), T, origin, record
+
+
+def modelnet_benchmark_pairs_batched(shapes, lengths, indices, num_points, keep_ratio, rotation_magnitude, translation_magnitude,
+                                     noise_magnitude):
+    """ModelNet validation / test pairs (``geob200_modelnet_benchmark_pairs_batched``): pair p is the reference's
+    ``ModelNetPairDataset(deterministic=True)`` item of dataset index ``indices[p]`` (0 .. 2^32-1), built from raw shape p of
+    ``shapes`` (stacked fp32, ``lengths`` host ints of 1 .. 8192) with numpy's legacy stream seeded by that index.  Returns (points
+    (2B num_points, 3) fp32 stacked [ref..., src...], lengths_host, transforms (B, 4, 4) fp32, origin (int32, the raw shape row of
+    every output row)).  No host synchronisation."""
+    _f(shapes, 'shapes')
+    lengths = [int(v) for v in lengths]
+    indices = [int(v) for v in indices]
+    B = len(lengths)
+    if B < 1 or len(indices) != B:
+        raise RuntimeError('modelnet_benchmark_pairs_batched: lengths and indices must hold one value per pair')
+    if shapes.dim() != 2 or shapes.shape[1] != 3 or shapes.shape[0] != sum(lengths) or not shapes.is_contiguous():
+        raise RuntimeError(f'modelnet_benchmark_pairs_batched: shapes must be contiguous (sum(lengths), 3), got {tuple(shapes.shape)}')
+    if any(not 0 <= i < 1 << 32 for i in indices):
+        raise RuntimeError('modelnet_benchmark_pairs_batched: indices must be in 0..2^32-1')
+    m = int(num_points)
+    dev = shapes.device
+    lib = L.lib()
+    ws = L.workspace(lib.geob200_modelnet_benchmark_pairs_batched_workspace_bytes(B, m), dev, tag='augment')
+    out = torch.empty((2 * B * max(m, 0), 3), dtype=_f32, device=dev)
+    origin = torch.empty((2 * B * max(m, 0),), dtype=_i32, device=dev)
+    T = torch.empty((B, 4, 4), dtype=_f32, device=dev)
+    L.check(lib.geob200_modelnet_benchmark_pairs_batched(shapes.data_ptr(), _host_i64(lengths), _host_i64(indices), B, m, float(keep_ratio),
+                                                         float(rotation_magnitude), float(translation_magnitude), float(noise_magnitude),
+                                                         out.data_ptr(), origin.data_ptr(), T.data_ptr(), ws.data_ptr(), ws.numel(),
+                                                         L.stream_ptr()), 'modelnet_benchmark_pairs_batched')
+    return out, [m] * (2 * B), T, origin

@@ -765,6 +765,32 @@ int geob200_modelnet_pairs_batched(const float* shapes, const int64_t* lengths_h
                                    uint64_t iteration, int64_t pair_base, float* out_points, int32_t* origin, float* out_transforms,
                                    double* record, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- ModelNet validation and test pairs (datasets/registration/modelnet/dataset.py, deterministic=True) ------------------------
+ *
+ * Pair p is the reference's val / test item of dataset index indices_h[p] (0 .. 2^32-1; the position in the class-filtered list),
+ * built from raw shape p (host lengths_h[p], 1 .. 8192 points, stacked in `shapes`) with twice_sample, a plane crop and no
+ * twice_transform.  One stream serves both clouds: numpy's legacy generator (MT19937) seeded as np.random.seed(index), consumed in
+ * the reference's order:
+ *   1. rand(3) -> Euler angles ((u pi) rotation_magnitude) / 180, R = scipy's from_euler('zyx', .) in its quaternion arithmetic;
+ *      uniform(-m, m) x 3 -> t (low + (high - low) u);
+ *   2. ref plane, then src plane: phi = uniform(0, 2 pi), theta = uniform(0, pi), n = (sin theta cos phi, sin theta sin phi, cos theta);
+ *   3. permutation(K) for ref, then src, K = floor(N keep_ratio + 0.5): the first num_points, or (K < num_points) the permutation
+ *      repeated and its head; permutation = arange, then for i = K-1 .. 1 swap i with the masked-rejection interval(i);
+ *   4. 3 num_points Gaussians for ref, then src (the polar method with its one-value cache, which carries from ref to src when
+ *      3 num_points is odd): jitter clip(0 + 0.01 g, +-noise_magnitude);
+ *   5. permutation(num_points) for ref, then src: the final order.
+ * Arithmetic: normalise in fp32 (column sums in row order, / N; subtract; divide by the largest sqrt((x^2 + y^2) + z^2)); src =
+ * ((R[0,i] x + R[1,i] y) + R[2,i] z) + t_inv[i] with t_inv = -(R^T t) alike, in fp64; distances (x nx + y ny) + z nz in fp64; crop
+ * order descending distance, ties to the lowest row; point + jitter in fp64, rounded to fp32 once.  No contraction anywhere.
+ * out_points (2B num_points, 3) stacked [ref_0..ref_{B-1}, src_0..src_{B-1}]; origin (int32, same rows): the raw shape row of each
+ * output point; out_transforms (B, 4, 4) fp32 [R | t] (ref = T src).  Any n_pairs (1 .. 262143): launches of up to 1024 pairs, one
+ * CTA per pair.  workspace: geob200_modelnet_benchmark_pairs_batched_workspace_bytes(n_pairs, num_points). */
+size_t geob200_modelnet_benchmark_pairs_batched_workspace_bytes(int64_t n_pairs, int64_t num_points);
+int geob200_modelnet_benchmark_pairs_batched(const float* shapes, const int64_t* lengths_h, const int64_t* indices_h, int64_t n_pairs,
+                                             int64_t num_points, double keep_ratio, double rotation_magnitude, double translation_magnitude,
+                                             double noise_magnitude, float* out_points, int32_t* origin, float* out_transforms,
+                                             void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
