@@ -72,7 +72,7 @@ _sig('geob200_gse_embed_workspace_bytes', SZ, I64, I64)
 _sig('geob200_gse_table_bytes', SZ, I64, I64, F, F)
 _sig('geob200_gse_table_build', c_int, P, P, P, P, P, I64, I64, F, F, P, SZ, P)
 _sig('geob200_gse_embed_table', c_int, P, P, I64, I64, P, SZ, I64, F, F, P, P, P, P, P, P, P)
-_sig('geob200_gse_embed_pairs', c_int, P, P, I64, I64, P, P, P, P, P, P, P, P, c_int, P, SZ, P)
+_sig('geob200_gse_embed_pairs', c_int, P, P, I64, I64, P, P, P, P, P, P, P, P, P, SZ, P)
 _sig('geob200_attention_workspace_bytes', SZ, I64, I64, I64)
 _sig('geob200_attention', c_int, P, I64, P, I64, P, I64, P, P, P, I64, I64, I64, I64, P, I64, P, SZ, P)
 _sig('geob200_set_attention_tma', c_int, c_int)

@@ -7,8 +7,8 @@
 // (N^2*4, C) x (C, C) GEMMs over them.  Here the sinusoid tile is generated on chip, contracted, and only
 // E (N,N,C) is written: the O(N^2 k C) intermediate never exists.
 //
-// This file holds the index kernel and the fp32 CUDA-core contraction (exact-fp32 reference path).  The
-// wgmma tensor-core contraction lives in gse_tc.cu and is selected by geob200_gse_embed_pairs().
+// This file holds the index kernel and the generic fp32 CUDA-core contraction for widths other than 128 and 256.
+// The wgmma tensor-core contraction for C = 128 and 256 lives in gse_tc.cu; geob200_gse_embed_pairs() picks by C.
 #include "common.cuh"
 #include "geob200.h"
 
@@ -100,114 +100,8 @@ __global__ void __launch_bounds__(256) gse_indices_kernel(const float* __restric
     }
 }
 
-// ---- fp32 contraction ------------------------------------------------------------------------------------
-// CTA tile: 32 (i,j) pairs = 128 sinusoid rows (d, a0, a1, a2) x C=256 outputs, K = 256 in chunks of 16.
-// A (sinusoids) is generated once into shared memory; WdT / WaT ((in, out) = transposed nn.Linear weights) are
-// streamed through shared memory.  Each thread owns 2 pairs x 4 sub-rows x 16 columns.
-constexpr int GSE_C = 256;
-constexpr int GSE_PAIRS = 32;
-constexpr int GSE_AST = GSE_C + 4;
-constexpr int GSE_BK = 16;
-
-__global__ void __launch_bounds__(256, 1) gse_embed_fp32_kernel(const float* __restrict__ d_idx, const float* __restrict__ a_idx,
-                                                                long long n_pairs, const float* __restrict__ div_term,
-                                                                const float* __restrict__ WdT, const float* __restrict__ WaT,
-                                                                const float* __restrict__ bd, const float* __restrict__ ba,
-                                                                float* __restrict__ E) {
-    extern __shared__ float sm[];
-    float* A = sm;                                    // [4][32][AST]
-    float* Bd = A + 4 * GSE_PAIRS * GSE_AST;          // [BK][256]
-    float* Ba = Bd + GSE_BK * GSE_C;                  // [BK][256]
-    const long long p0 = (long long)blockIdx.x * GSE_PAIRS;
-    {
-        // generate sinusoids: thread -> (row = t>>1 in [0,128), half of the 128 frequencies)
-        const int row = threadIdx.x >> 1, half = threadIdx.x & 1;
-        const int s = row >> 5, pr = row & 31;
-        const long long p = p0 + pr;
-        float x = 0.f;
-        if (p < n_pairs) x = (s == 0) ? d_idx[p] : a_idx[p * 3 + (s - 1)];
-        float* arow = A + (s * GSE_PAIRS + pr) * GSE_AST;
-        for (int f = half * 64; f < half * 64 + 64; ++f) {
-            float sv, cv;
-            sincosf(__fmul_rn(x, div_term[f]), &sv, &cv);
-            *reinterpret_cast<float2*>(arow + 2 * f) = make_float2(sv, cv);   // interleaved [sin, cos]
-        }
-    }
-    const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
-    float acc[2][4][16];
-#pragma unroll
-    for (int a = 0; a < 2; ++a)
-#pragma unroll
-        for (int s = 0; s < 4; ++s)
-#pragma unroll
-            for (int c = 0; c < 16; ++c) acc[a][s][c] = 0.f;
-
-    for (int k0 = 0; k0 < GSE_C; k0 += GSE_BK) {
-        __syncthreads();
-        for (int e = threadIdx.x; e < GSE_BK * GSE_C / 4; e += 256) {
-            reinterpret_cast<float4*>(Bd)[e] = reinterpret_cast<const float4*>(WdT + (long long)k0 * GSE_C)[e];
-            reinterpret_cast<float4*>(Ba)[e] = reinterpret_cast<const float4*>(WaT + (long long)k0 * GSE_C)[e];
-        }
-        __syncthreads();
-#pragma unroll
-        for (int kk = 0; kk < GSE_BK; kk += 4) {
-            float4 av[2][4];
-#pragma unroll
-            for (int a = 0; a < 2; ++a)
-#pragma unroll
-                for (int s = 0; s < 4; ++s)
-                    av[a][s] = *reinterpret_cast<const float4*>(A + (s * GSE_PAIRS + ty + 16 * a) * GSE_AST + k0 + kk);
-#pragma unroll
-            for (int u = 0; u < 4; ++u) {
-                float4 bdv[4], bav[4];
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                    bdv[j] = *reinterpret_cast<const float4*>(Bd + (kk + u) * GSE_C + tx * 4 + 64 * j);
-                    bav[j] = *reinterpret_cast<const float4*>(Ba + (kk + u) * GSE_C + tx * 4 + 64 * j);
-                }
-#pragma unroll
-                for (int a = 0; a < 2; ++a) {
-#pragma unroll
-                    for (int s = 0; s < 4; ++s) {
-                        const float4 v4 = av[a][s];
-                        const float xa = (u == 0) ? v4.x : (u == 1) ? v4.y : (u == 2) ? v4.z : v4.w;
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) {
-                            const float4 b = (s == 0) ? bdv[j] : bav[j];
-                            acc[a][s][4 * j + 0] = fmaf(xa, b.x, acc[a][s][4 * j + 0]);
-                            acc[a][s][4 * j + 1] = fmaf(xa, b.y, acc[a][s][4 * j + 1]);
-                            acc[a][s][4 * j + 2] = fmaf(xa, b.z, acc[a][s][4 * j + 2]);
-                            acc[a][s][4 * j + 3] = fmaf(xa, b.w, acc[a][s][4 * j + 3]);
-                        }
-                    }
-                }
-            }
-        }
-    }
-    // epilogue: E = (acc_d + bd) + max_k (acc_ak + ba)
-#pragma unroll
-    for (int a = 0; a < 2; ++a) {
-        const long long p = p0 + ty + 16 * a;
-        if (p >= n_pairs) continue;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            const int c = tx * 4 + 64 * j;
-            const float4 bdv = *reinterpret_cast<const float4*>(bd + c);
-            const float4 bav = *reinterpret_cast<const float4*>(ba + c);
-            float o[4];
-            const float bdd[4] = {bdv.x, bdv.y, bdv.z, bdv.w}, baa[4] = {bav.x, bav.y, bav.z, bav.w};
-#pragma unroll
-            for (int u = 0; u < 4; ++u) {
-                const float m = fmaxf(fmaxf(acc[a][1][4 * j + u] + baa[u], acc[a][2][4 * j + u] + baa[u]), acc[a][3][4 * j + u] + baa[u]);
-                o[u] = (acc[a][0][4 * j + u] + bdd[u]) + m;
-            }
-            *reinterpret_cast<float4*>(E + p * GSE_C + c) = make_float4(o[0], o[1], o[2], o[3]);
-        }
-    }
-}
-
-// Generic (any C multiple of 4, e.g. KITTI hidden_dim 128) fp32 contraction, one warp per pair; slower, used when
-// C != 256.  out channel c handled by lane-strided loop; sinusoid rows staged per warp in shared memory.
+// Generic (any C multiple of 4) fp32 contraction, one warp per pair; used when C is neither 128 nor 256.  out channel c
+// handled by lane-strided loop; sinusoid rows staged per warp in shared memory.
 __global__ void __launch_bounds__(256) gse_embed_generic_kernel(const float* __restrict__ d_idx, const float* __restrict__ a_idx,
                                                                 long long n_pairs, int C, const float* __restrict__ div_term,
                                                                 const float* __restrict__ WdT, const float* __restrict__ WaT,
@@ -248,9 +142,9 @@ __global__ void __launch_bounds__(256) gse_embed_generic_kernel(const float* __r
 
 using namespace geob200;
 
-// implemented in gse_tc.cu (wgmma tensor-core contraction); returns 1 if it does not handle this shape/mode
+// implemented in gse_tc.cu (wgmma 3xFP16 contraction); returns 1 for widths other than 128 and 256
 int geob200_gse_embed_tc(const float* d_idx, const float* a_idx, long long n_pairs, int C, const float* div_term,
-                         const float* Wd, const float* Wa, const float* bd, const float* ba, float* E, int mode,
+                         const float* Wd, const float* Wa, const float* bd, const float* ba, float* E,
                          void* workspace, size_t workspace_bytes, cudaStream_t st);
 
 extern "C" {
@@ -284,32 +178,20 @@ size_t geob200_gse_embed_workspace_bytes(int64_t n, int64_t channels) {
     return (size_t)(4 * channels * channels * 4 * 3 + 4096);   // room for split/packed weight copies of the tensor-core path
 }
 
-// mode: 0 = fp32 CUDA cores (exact-fp32 accumulation), 1 = wgmma 3xTF32 (fp32-accurate), 2 = wgmma 1xTF32,
-//       3 = wgmma 3xFP16 (fp32-accurate, half the tensor-pipe time of 3xTF32; default)
+// C = 128 or 256: the wgmma 3xFP16 contraction (fp32-accurate); any other width: the generic fp32 CUDA-core kernel
 int geob200_gse_embed_pairs(const float* d_indices, const float* a_indices, int64_t n_rows, int64_t channels, const float* div_term,
                             const float* wd_t, const float* wa_t, const float* wd, const float* wa, const float* bd, const float* ba,
-                            float* embeddings, int mode, void* workspace, size_t workspace_bytes, void* stream) {
+                            float* embeddings, void* workspace, size_t workspace_bytes, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     GEOB_REQUIRE(n_rows > 0 && channels > 0 && channels % 4 == 0, "gse_embed: bad shape");
     const long long n_pairs = (long long)n_rows;
-    if (mode != 0) {
-        int rc = geob200_gse_embed_tc(d_indices, a_indices, n_pairs, (int)channels, div_term, wd, wa, bd, ba, embeddings, mode,
-                                      workspace, workspace_bytes, st);
-        if (rc <= 0) return rc;
-        GEOB_REQUIRE(false, "gse_embed: tensor-core mode %d does not support C=%lld (C = 256: modes 1-4, C = 128: mode 3)", mode,
-                     (long long)channels);
-    }
-    if (channels == GSE_C) {
-        const size_t smem = sizeof(float) * (4 * GSE_PAIRS * GSE_AST + 2 * GSE_BK * GSE_C);
-        if (ensure_max_smem((const void*)gse_embed_fp32_kernel)) return -1;
-        gse_embed_fp32_kernel<<<(unsigned)((n_pairs + GSE_PAIRS - 1) / GSE_PAIRS), 256, smem, st>>>(
-            d_indices, a_indices, n_pairs, div_term, wd_t, wa_t, bd, ba, embeddings);
-    } else {
-        const size_t smem = sizeof(float) * 8 * 4 * channels;
-        GEOB_REQUIRE(smem <= 48 * 1024, "gse_embed: channels too large for the generic path");
-        gse_embed_generic_kernel<<<(unsigned)((n_pairs + 7) / 8), 256, smem, st>>>(d_indices, a_indices, n_pairs, (int)channels,
-                                                                                 div_term, wd_t, wa_t, bd, ba, embeddings);
-    }
+    const int rc = geob200_gse_embed_tc(d_indices, a_indices, n_pairs, (int)channels, div_term, wd, wa, bd, ba, embeddings, workspace,
+                                        workspace_bytes, st);
+    if (rc <= 0) return rc;
+    const size_t smem = sizeof(float) * 8 * 4 * channels;
+    GEOB_REQUIRE(smem <= 48 * 1024, "gse_embed: channels too large for the generic path");
+    gse_embed_generic_kernel<<<(unsigned)((n_pairs + 7) / 8), 256, smem, st>>>(d_indices, a_indices, n_pairs, (int)channels, div_term,
+                                                                             wd_t, wa_t, bd, ba, embeddings);
     GEOB_CHECK_LAUNCH();
     count_launches(1);
     return 0;

@@ -1,4 +1,4 @@
-// Hopper tensor-core (wgmma) contraction of the geometric structure embedding for C = 256 (and C = 128 in fp16).
+// Hopper tensor-core (wgmma) contraction of the geometric structure embedding for C = 256 and C = 128, 3xFP16.
 //
 // Reference semantics: geotransformer/modules/geotransformer/geotransformer.py:57-72
 //     E[p,:] = (Wd s(d_p) + bd) + max_k (Wa s(a_pk) + ba)          s(.) = C-wide interleaved sin/cos embedding
@@ -13,9 +13,7 @@
 //                            max over the three rows of a pair, adds the bias and stores E
 //   warps 8-11  generators : compute the sinusoid chunk (128 rows x 128 bytes) and store it straight into the K-major
 //                            SWIZZLE_128B layout (the A operand never exists in HBM); their first thread also streams the
-//                            pre-swizzled B chunk (packed once by gse_pack_b*_kernel) with cp.async.bulk onto the stage's mbarrier
-// Variants: 3xTF32 (NPASS = 3: a_hi b_hi + a_hi b_lo + a_lo b_hi, fp32-accurate), plain TF32 (NPASS = 1), and 3xFP16 (below),
-// the last also as a 2-CTA cluster that multicasts every B chunk into both CTAs.
+//                            pre-swizzled B chunk (packed once by gse_pack_b_f16_kernel) with cp.async.bulk onto the stage's mbarrier
 #include <cuda_fp16.h>
 
 #include "common.cuh"
@@ -27,10 +25,7 @@ namespace tc {
 
 using namespace hop;
 
-constexpr int C = 256;                 // output channels = MMA N
-constexpr int KTOT = 512;              // [angle | distance] sinusoids
-constexpr int KC = 32;                 // K elements per chunk = 128 bytes = one swizzle atom row
-constexpr int KC16 = 64;               // fp16 K elements per chunk
+constexpr int KC = 64;                 // fp16 K elements per chunk = 128 bytes = one swizzle atom row
 constexpr int PAIRS = 42;              // pairs per tile
 constexpr int ROWS = 128;              // tile rows (two warpgroups of M = 64)
 constexpr int A_BYTES = ROWS * 128;    // 16 KB
@@ -39,27 +34,8 @@ constexpr int NCONS_WARPS = 8;
 constexpr int NGEN_WARPS = 4;
 constexpr int NTHREADS = (NCONS_WARPS + NGEN_WARPS) * 32;
 
-// sin and cos of x for moderate |x| (embedding arguments are < ~100 rad): 3-term Cody-Waite reduction by pi/2 and
-// degree-7/8 minimax polynomials on [-pi/4, pi/4]; ~1 ulp, about a third of the instructions of sincosf.
-__device__ __forceinline__ void sincos_cw(float x, float& s, float& c) {
-    if (fabsf(x) > 48000.f) { sincosf(x, &s, &c); return; }
-    const float k = rintf(x * 0.636619772367581343f);
-    float r = fmaf(k, -1.57079601287841796875f, x);
-    r = fmaf(k, -3.1391647326017846353352069854736328125e-7f, r);
-    r = fmaf(k, -5.390302529957764765e-15f, r);
-    const float r2 = r * r;
-    const float sp = fmaf(r * r2, fmaf(r2, fmaf(r2, -1.9515295891e-4f, 8.3321608736e-3f), -1.6666654611e-1f), r);
-    const float cp = fmaf(r2 * r2, fmaf(r2, fmaf(r2, 2.443315711809948e-5f, -1.388731625493765e-3f), 4.166664568298827e-2f),
-                          fmaf(r2, -0.5f, 1.0f));
-    const int q = (int)k;
-    const float ss = (q & 1) ? cp : sp;
-    const float cc = (q & 1) ? sp : cp;
-    s = (q & 2) ? -ss : ss;
-    c = ((q + 1) & 2) ? -cc : cc;
-}
-
-// Cheaper variant for the fp16 kernels: same Cody-Waite reduction to [-pi/4, pi/4], then the SFU (sin.approx / cos.approx, abs
-// error ~4e-7 on that interval -- below the 2^-12 half-ulp of the fp16 hi/lo split that consumes the values).
+// sin and cos of x: Cody-Waite reduction by pi/2 to [-pi/4, pi/4], then the SFU (sin.approx / cos.approx, abs error ~4e-7 on
+// that interval -- below the 2^-12 half-ulp of the fp16 hi/lo split that consumes the values).
 __device__ __forceinline__ void sincos_sfu(float x, float& s, float& c) {
     if (fabsf(x) > 48000.f) { sincosf(x, &s, &c); return; }
     const float k = rintf(x * 0.636619772367581343f);
@@ -72,24 +48,6 @@ __device__ __forceinline__ void sincos_sfu(float x, float& s, float& c) {
     const float cc = (q & 1) ? sp : cp;
     s = (q & 2) ? -ss : ss;
     c = ((q + 1) & 2) ? -cc : cc;
-}
-
-// Packs B = [Wa | Wd] (row n = output channel, 512 K values) into per-chunk shared-memory images:
-// image[kc][n/8][n%8][(e/4) ^ (n%8)][e%4], hi part (tf32, round-to-nearest) and lo part (remainder).
-__global__ void __launch_bounds__(256) gse_pack_b_kernel(const float* __restrict__ Wd, const float* __restrict__ Wa,
-                                                         const float* __restrict__ bd, const float* __restrict__ ba,
-                                                         float* __restrict__ img_hi, float* __restrict__ img_lo,
-                                                         float* __restrict__ bias_sum) {
-    const int t = blockIdx.x * blockDim.x + threadIdx.x;
-    if (t < C) bias_sum[t] = ba[t] + bd[t];
-    if (t >= C * KTOT) return;
-    const int n = t / KTOT, k = t % KTOT;
-    const float w = (k < 256) ? Wa[n * 256 + k] : Wd[n * 256 + (k - 256)];
-    const float hi = tf32_rn(w);
-    const int kc = k / KC, e = k % KC;
-    const int dst = kc * (C * KC) + (n >> 3) * 256 + (n & 7) * 32 + (((e >> 2) ^ (n & 7)) << 2) + (e & 3);
-    img_hi[dst] = hi;
-    img_lo[dst] = w - hi;
 }
 
 // scale[0] = 2^-e with max|W| = m 2^e, m in [0.5,1)  ; scale[1] = 2^e
@@ -110,7 +68,8 @@ __global__ void __launch_bounds__(1024) gse_absmax_kernel(const float* __restric
     }
 }
 
-// CC = hidden dim (256: 3DMatch / ModelNet, 128: KITTI); B = [Wa | Wd] is (CC rows) x (2 CC halves)
+// CC = hidden dim (256: 3DMatch / ModelNet, 128: KITTI); B = [Wa | Wd] is (CC rows) x (2 CC halves), packed into per-chunk
+// shared-memory images image[kc][n/8][n%8][(e/8) ^ (n%8)][e%8], hi part (fp16 of the scaled weight) and lo part (remainder).
 template <int CC>
 __global__ void __launch_bounds__(256) gse_pack_b_f16_kernel(const float* __restrict__ Wd, const float* __restrict__ Wa,
                                                              const float* __restrict__ bd, const float* __restrict__ ba,
@@ -122,8 +81,8 @@ __global__ void __launch_bounds__(256) gse_pack_b_f16_kernel(const float* __rest
     const int n = t / (2 * CC), k = t % (2 * CC);
     const float w = ((k < CC) ? Wa[n * CC + k] : Wd[n * CC + (k - CC)]) * scale[0];
     const __half hi = __float2half_rn(w);
-    const int kc = k / KC16, e = k % KC16;
-    const int dst = kc * (CC * KC16) + (n >> 3) * 512 + (n & 7) * 64 + (((e >> 3) ^ (n & 7)) << 3) + (e & 7);
+    const int kc = k / KC, e = k % KC;
+    const int dst = kc * (CC * KC) + (n >> 3) * 512 + (n & 7) * 64 + (((e >> 3) ^ (n & 7)) << 3) + (e & 7);
     img_hi[dst] = hi;
     img_lo[dst] = __float2half_rn(w - __half2float(hi));
 }
@@ -134,68 +93,43 @@ __global__ void __launch_bounds__(256) gse_pack_b_f16_kernel(const float* __rest
 // the rate a tf32 one consumes K = 8: half the tensor-pipe time, half the B bytes, half the generator stores.  The sinusoids are
 // in [-1, 1] (lo <= 2^-12: fp16 subnormal spacing 6e-8 = fp32 epsilon); the weights are pre-scaled by a power of two to
 // [0.5, 1) (exact), undone in the epilogue.
-template <int CC, bool F16, int NPASS>
+template <int CC>
 struct Cfg {
-    static constexpr int KCH = F16 ? KC16 : KC;            // K elements per chunk
-    static constexpr int CP = CC / KCH;                    // chunks per part (angle, distance)
+    static constexpr int CP = CC / KC;                     // chunks per part (angle, distance)
     static constexpr int NCH = 2 * CP;                     // K chunks per tile
     static constexpr int BB = CC * 128;                    // bytes of one B chunk
-    static constexpr int NPART = NPASS == 3 ? 2 : 1;       // hi (+ lo) of each operand
-    static constexpr int A_PART = NPART * A_BYTES;
-    static constexpr int STAGE_BYTES = NPART * (A_BYTES + BB);
-    static constexpr int NSTAGE = NPASS == 3 ? 2 : 4;
+    static constexpr int STAGE_BYTES = 2 * (A_BYTES + BB); // hi and lo of both operands
+    static constexpr int NSTAGE = 2;
     static constexpr int SMEM = NSTAGE * STAGE_BYTES + ROWS * STAGE_LD * 4 + 1024 /*alignment slack*/ + 256 /*barriers*/;
 };
 
-// one 16-byte unit c (of 8 per 128-byte row) of the sinusoid row for argument x: tf32 = frequencies f0 + 2c, f0 + 2c + 1
-// (sin, cos interleaved), fp16 = frequencies f0 + 4c .. f0 + 4c + 3; hi part and (3-pass) lo part
-template <bool F16, int NPASS>
+// one 16-byte unit c (of 8 per 128-byte row) of the sinusoid row for argument x: frequencies f0 + 4c .. f0 + 4c + 3 (sin, cos
+// interleaved), hi part and lo part
 __device__ __forceinline__ void gen_unit(float x, const float* __restrict__ div_term, int f0, int c, uint4& hv, uint4& lv) {
-    if constexpr (F16) {
-        float v[8];
+    float v[8];
 #pragma unroll
-        for (int u = 0; u < 4; ++u) sincos_sfu(__fmul_rn(x, __ldg(div_term + f0 + 4 * c + u)), v[2 * u], v[2 * u + 1]);
-        __half2 hi[4], lo[4];
+    for (int u = 0; u < 4; ++u) sincos_sfu(__fmul_rn(x, __ldg(div_term + f0 + 4 * c + u)), v[2 * u], v[2 * u + 1]);
+    __half2 hi[4], lo[4];
 #pragma unroll
-        for (int u = 0; u < 4; ++u) {
-            const __half h0 = __float2half_rn(v[2 * u]), h1 = __float2half_rn(v[2 * u + 1]);
-            hi[u] = __halves2half2(h0, h1);
-            lo[u] = __halves2half2(__float2half_rn(v[2 * u] - __half2float(h0)), __float2half_rn(v[2 * u + 1] - __half2float(h1)));
-        }
-        hv = make_uint4(*reinterpret_cast<uint32_t*>(&hi[0]), *reinterpret_cast<uint32_t*>(&hi[1]), *reinterpret_cast<uint32_t*>(&hi[2]),
-                        *reinterpret_cast<uint32_t*>(&hi[3]));
-        lv = make_uint4(*reinterpret_cast<uint32_t*>(&lo[0]), *reinterpret_cast<uint32_t*>(&lo[1]), *reinterpret_cast<uint32_t*>(&lo[2]),
-                        *reinterpret_cast<uint32_t*>(&lo[3]));
-    } else {
-        float s0, c0, s1, c1;
-        sincos_cw(__fmul_rn(x, __ldg(div_term + f0 + 2 * c)), s0, c0);
-        sincos_cw(__fmul_rn(x, __ldg(div_term + f0 + 2 * c + 1)), s1, c1);
-        float4 hi = make_float4(s0, c0, s1, c1), lo = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (NPASS == 3) {
-            hi.x = tf32_rn(s0); lo.x = s0 - hi.x;
-            hi.y = tf32_rn(c0); lo.y = c0 - hi.y;
-            hi.z = tf32_rn(s1); lo.z = s1 - hi.z;
-            hi.w = tf32_rn(c1); lo.w = c1 - hi.w;
-        }
-        hv = *reinterpret_cast<uint4*>(&hi);
-        lv = *reinterpret_cast<uint4*>(&lo);
+    for (int u = 0; u < 4; ++u) {
+        const __half h0 = __float2half_rn(v[2 * u]), h1 = __float2half_rn(v[2 * u + 1]);
+        hi[u] = __halves2half2(h0, h1);
+        lo[u] = __halves2half2(__float2half_rn(v[2 * u] - __half2float(h0)), __float2half_rn(v[2 * u + 1] - __half2float(h1)));
     }
+    hv = make_uint4(*reinterpret_cast<uint32_t*>(&hi[0]), *reinterpret_cast<uint32_t*>(&hi[1]), *reinterpret_cast<uint32_t*>(&hi[2]),
+                    *reinterpret_cast<uint32_t*>(&hi[3]));
+    lv = make_uint4(*reinterpret_cast<uint32_t*>(&lo[0]), *reinterpret_cast<uint32_t*>(&lo[1]), *reinterpret_cast<uint32_t*>(&lo[2]),
+                    *reinterpret_cast<uint32_t*>(&lo[3]));
 }
 
-template <bool F16, int N>
-__device__ __forceinline__ void mma(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t acc) {
-    if constexpr (F16) wgmma_f16<N>(d, da, db, acc);
-    else wgmma_tf32<N>(d, da, db, acc);
-}
-
-// img_hi / img_lo: B images (float for tf32, __half for fp16); scale: fp16 weight scale (scale[1] undoes it), nullptr for tf32.
-// CLUSTER: the two CTAs of a cluster advance in lockstep and each streams one of the two B images into both.
-template <int CC, bool F16, int NPASS, bool CLUSTER>
-__device__ __forceinline__ void gse_embed_body(const float* __restrict__ d_idx, const float* __restrict__ a_idx, long long n_pairs,
-                                               const float* __restrict__ div_term, const void* __restrict__ img_hi,
-                                               const void* __restrict__ img_lo, const float* __restrict__ bias_sum,
-                                               const float* __restrict__ scale, float* __restrict__ E) {
-    using CF = Cfg<CC, F16, NPASS>;
+// img_hi / img_lo: the B images of gse_pack_b_f16_kernel; scale: the weight scale of gse_absmax_kernel (scale[1] undoes it).
+template <int CC>
+__global__ void __launch_bounds__(NTHREADS, 1) gse_embed_kernel(const float* __restrict__ d_idx, const float* __restrict__ a_idx,
+                                                                long long n_pairs, const float* __restrict__ div_term,
+                                                                const __half* __restrict__ img_hi, const __half* __restrict__ img_lo,
+                                                                const float* __restrict__ bias_sum, const float* __restrict__ scale,
+                                                                float* __restrict__ E) {
+    using CF = Cfg<CC>;
     constexpr int NSTAGE = CF::NSTAGE, R = CC / 2;
     extern __shared__ unsigned char smem_raw[];
     unsigned char* smem = (unsigned char*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);   // SWIZZLE_128B: 1024 B alignment
@@ -203,28 +137,22 @@ __device__ __forceinline__ void gse_embed_body(const float* __restrict__ d_idx, 
     uint64_t* bars = (uint64_t*)(xstage + ROWS * STAGE_LD);
     uint64_t* full = bars;                      // [NSTAGE] A generated + B landed
     uint64_t* empty = bars + NSTAGE;            // [NSTAGE] both consumer warpgroups are done with the stage
-    uint64_t* peer_empty = bars + 2 * NSTAGE;   // [NSTAGE] (cluster) the peer CTA's stage is free (remote arrive)
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const long long n_tiles = (n_pairs + PAIRS - 1) / PAIRS;
-    // cluster: same number of tile slots for every CTA; slots past n_tiles are idle, the pipeline still runs
-    const long long tile_end = CLUSTER ? (n_tiles + gridDim.x - 1) / gridDim.x * gridDim.x : n_tiles;
-    uint32_t cta_rank = 0;
-    if (CLUSTER) asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(cta_rank));
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < NSTAGE; ++s) { mbar_init(&full[s], NGEN_WARPS + 1); mbar_init(&empty[s], NCONS_WARPS); mbar_init(&peer_empty[s], 1); }
+        for (int s = 0; s < NSTAGE; ++s) { mbar_init(&full[s], NGEN_WARPS + 1); mbar_init(&empty[s], NCONS_WARPS); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
-    if (CLUSTER) asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 
     if (warp >= NCONS_WARPS) {
         // ===================== generators (+ B copier) =====================
         const int gt = threadIdx.x - NCONS_WARPS * 32;
         {   // padding rows 126,127 of every A buffer: zero once (their outputs are never read)
-            for (int e = gt; e < NSTAGE * CF::NPART * 64; e += NGEN_WARPS * 32) {
-                const int sidx = e / (CF::NPART * 64), rem = e % (CF::NPART * 64);
+            for (int e = gt; e < NSTAGE * 2 * 64; e += NGEN_WARPS * 32) {
+                const int sidx = e / (2 * 64), rem = e % (2 * 64);
                 float* base = (float*)(smem + sidx * CF::STAGE_BYTES + (rem / 64) * A_BYTES + 15 * 1024 + 6 * 128);
                 base[rem % 64] = 0.f;
             }
@@ -232,7 +160,7 @@ __device__ __forceinline__ void gse_embed_body(const float* __restrict__ d_idx, 
         }
         int s = 0;
         uint32_t ph = 0;
-        for (long long tile = blockIdx.x; tile < tile_end; tile += gridDim.x) {
+        for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
             const long long p0 = tile * PAIRS;
             for (int kc = 0; kc < CF::NCH; ++kc) {
                 mbar_wait(&empty[s], ph ^ 1u);
@@ -241,29 +169,13 @@ __device__ __forceinline__ void gse_embed_body(const float* __restrict__ d_idx, 
                     const size_t off = (size_t)kc * CF::BB;
                     const unsigned char* hi = (const unsigned char*)img_hi + off;
                     const unsigned char* lo = (const unsigned char*)img_lo + off;
-                    if (CLUSTER) {
-                        // tell the peer its copy into my stage may start, then wait until the peer's stage s is free too;
-                        // rank 0 streams the hi image, rank 1 the lo image, each multicast into both CTAs: every B byte leaves
-                        // L2 once per CTA pair instead of once per CTA
-                        uint32_t raddr;
-                        asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(raddr) : "r"(smem_u32(&peer_empty[s])), "r"(cta_rank ^ 1u));
-                        asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(raddr) : "memory");
-                        mbar_wait_cluster(&peer_empty[s], ph);
-                        mbar_arrive_expect_tx(&full[s], 2 * CF::BB);       // both halves land here (mine + the peer's multicast)
-                        asm volatile(
-                            "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;" ::"r"(
-                                smem_u32(st + CF::A_PART + (cta_rank == 0 ? 0 : CF::BB))),
-                            "l"(cta_rank == 0 ? hi : lo), "r"((uint32_t)CF::BB), "r"(smem_u32(&full[s])), "h"((unsigned short)3)
-                            : "memory");
-                    } else {
-                        mbar_arrive_expect_tx(&full[s], CF::NPART * CF::BB);
-                        bulk_g2s(st + CF::A_PART, hi, CF::BB, &full[s]);
-                        if (NPASS == 3) bulk_g2s(st + CF::A_PART + CF::BB, lo, CF::BB, &full[s]);
-                    }
+                    mbar_arrive_expect_tx(&full[s], 2 * CF::BB);
+                    bulk_g2s(st + 2 * A_BYTES, hi, CF::BB, &full[s]);
+                    bulk_g2s(st + 2 * A_BYTES + CF::BB, lo, CF::BB, &full[s]);
                 }
                 // work item = (tile row, 16-byte unit c).  Angle chunks (kc < CP) have 126 x 8 items; distance chunks have
                 // 42 x 8 items whose result is stored to the three rows (k = 0,1,2) of the pair.
-                const int f0 = (kc % CF::CP) * (CF::KCH / 2);
+                const int f0 = (kc % CF::CP) * (KC / 2);
                 const bool angle = kc < CF::CP;
                 const int n_items = (angle ? 3 * PAIRS : PAIRS) * 8;
                 for (int it = gt; it < n_items; it += NGEN_WARPS * 32) {
@@ -273,13 +185,13 @@ __device__ __forceinline__ void gse_embed_body(const float* __restrict__ d_idx, 
                     float x = 0.f;
                     if (p < n_pairs) x = angle ? __ldg(a_idx + p * 3 + rr / PAIRS) : __ldg(d_idx + p);
                     uint4 hv, lv;
-                    gen_unit<F16, NPASS>(x, div_term, f0, c, hv, lv);
+                    gen_unit(x, div_term, f0, c, hv, lv);
                     const int nrep = angle ? 1 : 3;
                     for (int rep = 0; rep < nrep; ++rep) {
                         const int r = angle ? rr : (rep * PAIRS + j);
                         const uint32_t off = (uint32_t)((r >> 3) * 1024 + (r & 7) * 128 + ((c ^ (r & 7)) << 4));
                         *reinterpret_cast<uint4*>(st + off) = hv;
-                        if (NPASS == 3) *reinterpret_cast<uint4*>(st + A_BYTES + off) = lv;
+                        *reinterpret_cast<uint4*>(st + A_BYTES + off) = lv;
                     }
                 }
                 fence_proxy_async();               // generic-proxy stores -> visible to the tensor core (async proxy)
@@ -291,10 +203,10 @@ __device__ __forceinline__ void gse_embed_body(const float* __restrict__ d_idx, 
     } else {
         // ===================== consumers =====================
         const int wg = warp >> 2, wq = warp & 3;
-        const float inv_scale = F16 ? scale[1] : 1.0f;
+        const float inv_scale = scale[1];
         int s = 0;
         uint32_t ph = 0;
-        for (long long tile = blockIdx.x; tile < tile_end; tile += gridDim.x) {
+        for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
             float acc[R];
 #pragma unroll
             for (int i = 0; i < R; ++i) acc[i] = 0.f;
@@ -303,16 +215,14 @@ __device__ __forceinline__ void gse_embed_body(const float* __restrict__ d_idx, 
                 mbar_wait(&full[s], ph);
                 const uint32_t st = smem_u32(smem + s * CF::STAGE_BYTES);
                 const uint64_t da_hi = make_desc(st + wg * (A_BYTES / 2)), da_lo = make_desc(st + A_BYTES + wg * (A_BYTES / 2));
-                const uint64_t db_hi = make_desc(st + CF::A_PART), db_lo = make_desc(st + CF::A_PART + CF::BB);
+                const uint64_t db_hi = make_desc(st + 2 * A_BYTES), db_lo = make_desc(st + 2 * A_BYTES + CF::BB);
                 wgmma_fence();
 #pragma unroll
                 for (int kk = 0; kk < 4; ++kk) {       // 4 MMAs of 32 bytes of K per 128-byte chunk
                     const uint64_t adv = (uint64_t)(kk * 2);
-                    mma<F16, CC>(acc, da_hi + adv, db_hi + adv, (kc == 0 && kk == 0) ? 0u : 1u);
-                    if (NPASS == 3) {
-                        mma<F16, CC>(acc, da_hi + adv, db_lo + adv, 1u);
-                        mma<F16, CC>(acc, da_lo + adv, db_hi + adv, 1u);
-                    }
+                    wgmma_f16<CC>(acc, da_hi + adv, db_hi + adv, (kc == 0 && kk == 0) ? 0u : 1u);
+                    wgmma_f16<CC>(acc, da_hi + adv, db_lo + adv, 1u);
+                    wgmma_f16<CC>(acc, da_lo + adv, db_hi + adv, 1u);
                 }
                 wgmma_commit();
                 wgmma_wait<1>();                     // the previous chunk's MMAs are done: its stage can be refilled
@@ -352,24 +262,28 @@ __device__ __forceinline__ void gse_embed_body(const float* __restrict__ d_idx, 
             }
         }
     }
-    // no CTA leaves while its peer may still write to it
-    if (CLUSTER) asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 
-template <int CC, bool F16, int NPASS>
-__global__ void __launch_bounds__(NTHREADS, 1) gse_embed_kernel(const float* __restrict__ d_idx, const float* __restrict__ a_idx,
-                                                                long long n_pairs, const float* __restrict__ div_term,
-                                                                const void* __restrict__ img_hi, const void* __restrict__ img_lo,
-                                                                const float* __restrict__ bias_sum, const float* __restrict__ scale,
-                                                                float* __restrict__ E) {
-    gse_embed_body<CC, F16, NPASS, false>(d_idx, a_idx, n_pairs, div_term, img_hi, img_lo, bias_sum, scale, E);
-}
-
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NTHREADS, 1)
-    gse_embed_f16_cluster_kernel(const float* __restrict__ d_idx, const float* __restrict__ a_idx, long long n_pairs,
-                                 const float* __restrict__ div_term, const void* __restrict__ img_hi, const void* __restrict__ img_lo,
-                                 const float* __restrict__ bias_sum, const float* __restrict__ scale, float* __restrict__ E) {
-    gse_embed_body<C, true, 3, true>(d_idx, a_idx, n_pairs, div_term, img_hi, img_lo, bias_sum, scale, E);
+// weight scale -> packed B images -> the persistent contraction kernel, all on stream st
+template <int CC>
+int embed(const float* d_idx, const float* a_idx, long long n_pairs, const float* div_term, const float* Wd, const float* Wa,
+          const float* bd, const float* ba, float* E, void* workspace, size_t workspace_bytes, cudaStream_t st) {
+    const size_t img_halves = (size_t)CC * 2 * CC;
+    const size_t need = 2 * img_halves * sizeof(__half) + (CC + 2) * sizeof(float) + 1024;
+    GEOB_REQUIRE(workspace_bytes >= need, "gse_embed_tc: workspace too small (%zu < %zu)", workspace_bytes, need);
+    __half* h_hi = (__half*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+    __half* h_lo = h_hi + img_halves;
+    float* bsum = (float*)(h_lo + img_halves);
+    float* scale = bsum + CC;
+    const long long n_tiles = (n_pairs + PAIRS - 1) / PAIRS;
+    const int grid = (int)(n_tiles < (long long)num_sms() ? n_tiles : (long long)num_sms());
+    gse_absmax_kernel<CC><<<1, 1024, 0, st>>>(Wd, Wa, scale);
+    gse_pack_b_f16_kernel<CC><<<(unsigned)((img_halves + 255) / 256), 256, 0, st>>>(Wd, Wa, bd, ba, scale, h_hi, h_lo, bsum);
+    if (ensure_max_smem((const void*)gse_embed_kernel<CC>)) return -1;
+    gse_embed_kernel<CC><<<grid, NTHREADS, Cfg<CC>::SMEM, st>>>(d_idx, a_idx, n_pairs, div_term, h_hi, h_lo, bsum, scale, E);
+    GEOB_CHECK_LAUNCH();
+    count_launches(3);
+    return 0;
 }
 
 }  // namespace tc
@@ -378,67 +292,9 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NTHREADS, 1)
 using namespace geob200;
 
 int geob200_gse_embed_tc(const float* d_idx, const float* a_idx, long long n_pairs, int C, const float* div_term,
-                         const float* Wd, const float* Wa, const float* bd, const float* ba, float* E, int mode,
+                         const float* Wd, const float* Wa, const float* bd, const float* ba, float* E,
                          void* workspace, size_t workspace_bytes, cudaStream_t st) {
-    if (mode != 1 && mode != 2 && mode != 3 && mode != 4) return 1;
-    if (C == 128 && mode == 3) {
-        // hidden 128 (KITTI): the 3xFP16 kernel instantiated for N = 128, K = 2 x 128 (two angle + two distance chunks per tile)
-        constexpr int CC = 128;
-        const size_t img_halves = (size_t)CC * 2 * CC;
-        const size_t need = 2 * img_halves * sizeof(__half) + (CC + 2) * sizeof(float) + 1024;
-        GEOB_REQUIRE(workspace_bytes >= need, "gse_embed_tc: workspace too small (%zu < %zu)", workspace_bytes, need);
-        __half* h_hi = (__half*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
-        __half* h_lo = h_hi + img_halves;
-        float* bsum = (float*)(h_lo + img_halves);
-        float* scale = bsum + CC;
-        const long long n_tiles = (n_pairs + tc::PAIRS - 1) / tc::PAIRS;
-        const int grid = (int)(n_tiles < (long long)num_sms() ? n_tiles : (long long)num_sms());
-        tc::gse_absmax_kernel<CC><<<1, 1024, 0, st>>>(Wd, Wa, scale);
-        tc::gse_pack_b_f16_kernel<CC><<<(unsigned)((img_halves + 255) / 256), 256, 0, st>>>(Wd, Wa, bd, ba, scale, h_hi, h_lo, bsum);
-        if (ensure_max_smem((const void*)tc::gse_embed_kernel<CC, true, 3>)) return -1;
-        tc::gse_embed_kernel<CC, true, 3><<<grid, tc::NTHREADS, tc::Cfg<CC, true, 3>::SMEM, st>>>(d_idx, a_idx, n_pairs, div_term, h_hi, h_lo, bsum, scale, E);
-        GEOB_CHECK_LAUNCH();
-        count_launches(3);
-        return 0;
-    }
-    if (C != tc::C) return 1;
-    const size_t img_floats = (size_t)tc::C * tc::KTOT;
-    const size_t need = sizeof(float) * (2 * img_floats + tc::C) + 1024;
-    GEOB_REQUIRE(workspace_bytes >= need, "gse_embed_tc: workspace too small (%zu < %zu)", workspace_bytes, need);
-    float* img_hi = (float*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
-    float* img_lo = img_hi + img_floats;
-    float* bias_sum = img_lo + img_floats;
-    const long long n_tiles = (n_pairs + tc::PAIRS - 1) / tc::PAIRS;
-    const int grid = (int)(n_tiles < (long long)num_sms() ? n_tiles : (long long)num_sms());
-    if (mode == 3 || mode == 4) {
-        __half* h_hi = (__half*)img_hi;
-        __half* h_lo = h_hi + img_floats;
-        float* bsum = (float*)(h_lo + img_floats);
-        float* scale = bsum + tc::C;
-        tc::gse_absmax_kernel<tc::C><<<1, 1024, 0, st>>>(Wd, Wa, scale);
-        tc::gse_pack_b_f16_kernel<tc::C><<<(unsigned)((img_floats + 255) / 256), 256, 0, st>>>(Wd, Wa, bd, ba, scale, h_hi, h_lo, bsum);
-        if (ensure_max_smem((const void*)tc::gse_embed_kernel<tc::C, true, 3>) || ensure_max_smem((const void*)tc::gse_embed_f16_cluster_kernel)) return -1;
-        if (mode == 4) {
-            // CTA pairs (cluster of 2) share every B chunk through TMA multicast; grid = even number of CTAs, one per SM
-            int g2 = (int)((n_tiles + 1) / 2 < (long long)(num_sms() / 2) ? (n_tiles + 1) / 2 : (long long)(num_sms() / 2)) * 2;
-            tc::gse_embed_f16_cluster_kernel<<<g2, tc::NTHREADS, tc::Cfg<tc::C, true, 3>::SMEM, st>>>(d_idx, a_idx, n_pairs, div_term, h_hi, h_lo, bsum, scale, E);
-        } else
-            tc::gse_embed_kernel<tc::C, true, 3><<<grid, tc::NTHREADS, tc::Cfg<tc::C, true, 3>::SMEM, st>>>(d_idx, a_idx, n_pairs, div_term, h_hi, h_lo, bsum, scale, E);
-        GEOB_CHECK_LAUNCH();
-        count_launches(3);
-        return 0;
-    }
-    tc::gse_pack_b_kernel<<<(unsigned)((img_floats + 255) / 256), 256, 0, st>>>(Wd, Wa, bd, ba, img_hi, img_lo, bias_sum);
-    if (mode == 1) {
-        if (ensure_max_smem((const void*)tc::gse_embed_kernel<tc::C, false, 3>)) return -1;
-        tc::gse_embed_kernel<tc::C, false, 3><<<grid, tc::NTHREADS, tc::Cfg<tc::C, false, 3>::SMEM, st>>>(d_idx, a_idx, n_pairs, div_term, img_hi,
-                                                                                                        img_lo, bias_sum, nullptr, E);
-    } else {
-        if (ensure_max_smem((const void*)tc::gse_embed_kernel<tc::C, false, 1>)) return -1;
-        tc::gse_embed_kernel<tc::C, false, 1><<<grid, tc::NTHREADS, tc::Cfg<tc::C, false, 1>::SMEM, st>>>(d_idx, a_idx, n_pairs, div_term, img_hi,
-                                                                                                        img_lo, bias_sum, nullptr, E);
-    }
-    GEOB_CHECK_LAUNCH();
-    count_launches(2);
-    return 0;
+    if (C == 256) return tc::embed<256>(d_idx, a_idx, n_pairs, div_term, Wd, Wa, bd, ba, E, workspace, workspace_bytes, st);
+    if (C == 128) return tc::embed<128>(d_idx, a_idx, n_pairs, div_term, Wd, Wa, bd, ba, E, workspace, workspace_bytes, st);
+    return 1;
 }

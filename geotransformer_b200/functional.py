@@ -13,16 +13,15 @@ from . import _lib as L
 
 _f32, _i64, _u8, _i32 = torch.float32, torch.int64, torch.uint8, torch.int32
 
-# mode of the structure-embedding contraction (see geob200_gse_embed_pairs): 0 fp32 CUDA cores, 1 wgmma 3xTF32, 2 1xTF32,
-# 3 3xFP16 (fp32-accurate like 3xTF32 at half the tensor-pipe time), 4 3xFP16 on CTA pairs,
-# 5 tabulated projections (geob200_gse_embed_table: no contraction at all; default -- tests/gse_table_check.py compares its
-# accuracy and launch time with mode 3).  Mode 5 needs the ``table`` of the weights (``gse_table``; the modules build and
-# cache it); the functional ops called WITHOUT a table and without an explicit mode run the tensor-core contraction (mode 3).
-GSE_MODE = int(__import__('os').environ.get('GEOB200_GSE_MODE', '5'))
+# default ``mode`` of the structure embedding: 5 = tabulated projections (geob200_gse_embed_table: no contraction at all) when
+# the caller passes the ``table`` of the weights (``gse_table``; the modules build and cache it), the contraction without one;
+# 3 = always the contraction (geob200_gse_embed_pairs: wgmma 3xFP16 for C = 128 and 256, a generic fp32 kernel for other
+# widths).  tests/gse_table_check.py compares the accuracy and launch time of the two.
+GSE_MODE = 5
 # tabulation grid of mode 5: step 1 / GSE_TABLE_INV_STEP index units (power of two), distance indices up to GSE_TABLE_D_MAX
 # (larger ones are evaluated directly inside the kernel: correct, slow)
-GSE_TABLE_INV_STEP = int(__import__('os').environ.get('GEOB200_GSE_TABLE_INV_STEP', '256'))
-GSE_TABLE_D_MAX = float(__import__('os').environ.get('GEOB200_GSE_TABLE_D_MAX', '96'))
+GSE_TABLE_INV_STEP = 256
+GSE_TABLE_D_MAX = 96.0
 
 # Optional per-op CUDA-event timing on the launching stream (bench.py sets EVENTS = {} to collect
 # {op name: [(start_event, end_event), ...]}; None = off, zero overhead).
@@ -773,11 +772,13 @@ def _gse_embed_table(d_indices, a_indices, n_rows, div_term, wd, wa, bd, ba, tab
 
 
 def _gse_mode(mode, table):
-    """explicit mode wins (mode 5 without a table is an error, raised by ``_gse_embed_table``); the default is GSE_MODE, except
-    that the tabulated mode without a table means the caller has none: tensor-core contraction"""
-    if mode is not None:
-        return mode
-    return 3 if (GSE_MODE == 5 and table is None) else GSE_MODE
+    """mode None, 3 or 5: an explicit mode wins (mode 5 without a table is an error, raised by ``_gse_embed_table``); the default
+    is GSE_MODE, except that the tabulated mode without a table means the caller has none: the contraction (mode 3)"""
+    if mode is None:
+        mode = 3 if (GSE_MODE == 5 and table is None) else GSE_MODE
+    if mode not in (3, 5):
+        raise ValueError(f'gse_embed: mode {mode!r} unsupported (None, 3 = contraction or 5 = tabulated projections)')
+    return mode
 
 
 def gse_embed_flat(d_indices, a_indices, n_rows, div_term, wd, wa, bd, ba, wd_t, wa_t, out, mode=None, table=None):
@@ -797,16 +798,12 @@ def _gse_embed_flat(d_indices, a_indices, n_rows, div_term, wd, wa, bd, ba, wd_t
     mode = _gse_mode(mode, table)
     if mode == 5 and c in (128, 256):
         return _gse_embed_table(d_indices, a_indices, n_rows, div_term, wd, wa, bd, ba, table, out)
-    if c == 128 and mode != 0:
-        mode = 3                     # hidden_dim 128 (KITTI): the 3xFP16 wgmma kernel has an N = 128 instantiation
-    elif c != 256:
-        mode = 0                     # other widths: fp32 CUDA-core kernel
     lib = L.lib()
     ws = L.workspace(lib.geob200_gse_embed_workspace_bytes(1, c), d_indices.device, 'gse')
     with _timed('gse_embed'):
         L.check(lib.geob200_gse_embed_pairs(d_indices.data_ptr(), a_indices.data_ptr(), int(n_rows), c, div_term.data_ptr(),
                                             wd_t.data_ptr(), wa_t.data_ptr(), wd.data_ptr(), wa.data_ptr(), bd.data_ptr(),
-                                            ba.data_ptr(), out.data_ptr(), int(mode), ws.data_ptr(), ws.numel(), L.stream_ptr()),
+                                            ba.data_ptr(), out.data_ptr(), ws.data_ptr(), ws.numel(), L.stream_ptr()),
                 'gse_embed_pairs')
     return out
 

@@ -28,9 +28,10 @@ class GeometricStructureEmbedding(nn.Module):
         self._table = None
 
     def table(self):
-        """``functional.GseTable`` of the current projection weights when the tabulated mode (``GF.GSE_MODE == 5``) is on, else
-        None.  Rebuilt when any of the four parameters changes (version counters) or the grid settings do; built once and
-        complete before it is returned, so the engine's lanes (host thread + stream each) can share it."""
+        """``functional.GseTable`` of the current projection weights when the tabulated mode (``GF.GSE_MODE == 5``) is on and
+        hidden_dim is 128 or 256, else None (the structure embedding then runs the contraction).  Rebuilt when any of the four
+        parameters changes (version counters) or the grid constants ``GF.GSE_TABLE_INV_STEP`` / ``GF.GSE_TABLE_D_MAX`` do; built
+        once and complete before it is returned, so the engine's lanes (host thread + stream each) can share it."""
         c = self.proj_d.out_features
         if GF.GSE_MODE != 5 or c not in (128, 256):
             return None

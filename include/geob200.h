@@ -249,12 +249,12 @@ int geob200_gse_indices_batched(const float* points, int64_t n_clouds, const int
 /* GeometricStructureEmbedding.forward (geotransformer.py:57-72) given the indices: sinusoid -> proj_d / proj_a ->
  * max over k -> sum, fused, over a flat list of n_rows (anchor, point) index rows -- the n*n (i, j) pairs of one cloud, or of several
  * clouds concatenated: d_indices (n_rows,), a_indices (n_rows, 3) -> embeddings (n_rows, channels).  wd/wa are the nn.Linear
- * weights (out,in); wd_t/wa_t their transposes (in,out).
- * mode 0: fp32 CUDA cores; 1: wgmma 3xTF32; 2: wgmma 1xTF32; 3: wgmma 3xFP16 split (fp32-accurate, fastest). */
+ * weights (out,in); wd_t/wa_t their transposes (in,out).  channels 128 and 256 run a wgmma 3xFP16 split contraction
+ * (fp32-accurate), any other multiple of 4 a generic fp32 CUDA-core kernel. */
 size_t geob200_gse_embed_workspace_bytes(int64_t n, int64_t channels);
 int geob200_gse_embed_pairs(const float* d_indices, const float* a_indices, int64_t n_rows, int64_t channels, const float* div_term,
                             const float* wd_t, const float* wa_t, const float* wd, const float* wa, const float* bd, const float* ba,
-                            float* embeddings, int mode, void* workspace, size_t workspace_bytes, void* stream);
+                            float* embeddings, void* workspace, size_t workspace_bytes, void* stream);
 
 /* The same embedding through TABULATED projections (csrc/gse_table.cu).  proj_d(sinusoid(x)) and proj_a(sinusoid(x)) are
  * functions of one scalar, band-limited to 1 rad per index unit: geob200_gse_table_build tabulates both once per set of weights

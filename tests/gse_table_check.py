@@ -1,6 +1,6 @@
-"""Tabulated structure embedding (GSE mode 5, csrc/gse_table.cu) on the GPU: accuracy against the CPU oracle and the fp32 /
-tensor-core kernels, the direct-evaluation path for arguments beyond the table, and the time of one batch-sized launch next to
-the wgmma 3xFP16 kernel.  Prints one JSON line per check.  A CHECKER (lives under tests/ because it imports oracle/), not a
+"""Tabulated structure embedding (GSE mode 5, csrc/gse_table.cu) on the GPU: accuracy against the CPU oracle next to the
+tensor-core contraction (mode 3), the direct-evaluation path for arguments beyond the table, and the time of one batch-sized
+launch next to the wgmma 3xFP16 kernel.  Prints one JSON line per check.  A CHECKER (lives under tests/ because it imports oracle/), not a
 pytest module: ``python tests/gse_table_check.py``."""
 import json
 import math
@@ -43,7 +43,6 @@ def accuracy(c, n, sigma_d, extent, seed):
     for name, kw in (('table', {}), ('table_inv_step_64', {'inv_step': 64}), ('table_mostly_direct', {'d_max': float(d.max()) * 0.5})):
         got = GF.gse_embed(*args, mode=5, table=table_of(cu, **kw)).cpu()
         out[name + '_vs_oracle'] = float((got - want).abs().max())
-    out['fp32_kernel_vs_oracle'] = float((GF.gse_embed(*args, mode=0).cpu() - want).abs().max())
     out['tensor_core_3xfp16_vs_oracle'] = float((GF.gse_embed(*args, mode=3).cpu() - want).abs().max())
     out['scale'] = float(want.abs().max())
     print(json.dumps(out), flush=True)
