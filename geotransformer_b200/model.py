@@ -159,13 +159,12 @@ class GeoTransformer(nn.Module):
         wa_t = emb_mod._cache.get('wa_t', emb_mod.proj_a.weight, lambda w: w.t().contiguous())
         GF.gse_embed_flat(d_all, a_all, eo[-1], emb_mod.embedding.div_term, emb_mod.proj_d.weight.detach(), emb_mod.proj_a.weight.detach(),
                           emb_mod.proj_d.bias.detach(), emb_mod.proj_a.bias.detach(), wd_t, wa_t, E_all, table=emb_mod.table())
-        embs = [E_all[eo[c]:eo[c + 1]] for c in range(2 * B)]
         mark('structure_embedding')
         x = GF.linear(feats_c, tr.in_proj.weight, tr.in_proj.bias)
         if native is not None:
-            x = native.transformer_forward_batched(x, rows_c, embs)
+            x = native.transformer_forward_batched(x, rows_c, [E_all[eo[c]:eo[c + 1]] for c in range(2 * B)])
         else:
-            x = tr.transformer.forward_stacked(x, rows_c[0], embs[0], embs[1])
+            x = tr.transformer.forward_stacked(x, rows_c, E_all)
         y = GF.linear(x, tr.out_proj.weight, tr.out_proj.bias)
         y_n = GF.l2_normalize(y)
         mark('transformer')
@@ -270,8 +269,7 @@ class GeoTransformer(nn.Module):
 
         feats_list = self.backbone(data_dict['features'], data_dict)
         feats_c, feats_f = feats_list[-1], feats_list[0]
-        rc, sc = self.transformer(points_c[:n0].contiguous(), points_c[n0:].contiguous(), feats_c[:n0], feats_c[n0:])
-        y_n = GF.l2_normalize(torch.cat([rc, sc]))
+        y_n = GF.l2_normalize(self.transformer.forward_stacked(points_c, feats_c, cn))
 
         cm, fm = self.coarse_matching, self.fine_matching
         with torch.no_grad():
@@ -337,7 +335,7 @@ class GeoTransformer(nn.Module):
 
         feats_list = self.backbone(data_dict['features'], data_dict)
         feats_c, feats_f = feats_list[-1], feats_list[0]
-        y_n = GF.l2_normalize(self.transformer.forward_batched_grad(points_c, feats_c, cn))
+        y_n = GF.l2_normalize(self.transformer.forward_stacked(points_c, feats_c, cn))
 
         cm, fm = self.coarse_matching, self.fine_matching
         with torch.no_grad():

@@ -72,39 +72,23 @@ class GeometricStructureEmbedding(nn.Module):
         d, a = GF.gse_indices(pts.contiguous(), self.sigma_d, self.sigma_a, self.angle_k)
         return (d.unsqueeze(0), a.unsqueeze(0)) if squeeze else (d, a)
 
-    def forward(self, points, scratch_tag=None):
-        """``scratch_tag``: write E into the grow-only scratch buffer of that name (valid until the next call with the same
-        tag on this stream) instead of a fresh allocation; used by GeometricTransformer for its two embeddings.  E carries no
-        graph: ``forward_grad`` is the differentiable form."""
+    def forward(self, points):
+        """E of one (N, 3) cloud (or (1, N, 3), the reference's batch of one) as (N, N, C): ``forward_flat`` of that cloud, without a
+        graph also in grad mode (callers read E as values, e.g. convert it to numpy); ``forward_flat`` is the differentiable form."""
         squeeze = points.ndim == 3
         if squeeze and points.shape[0] != 1:
             raise NotImplementedError('one cloud per call (the reference model always passes B=1)')
         pts = (points[0] if squeeze else points).contiguous()
-        d, a = GF.gse_indices(pts, self.sigma_d, self.sigma_a, self.angle_k)
-        wd_t = self._cache.get('wd_t', self.proj_d.weight, lambda w: w.t().contiguous())
-        wa_t = self._cache.get('wa_t', self.proj_a.weight, lambda w: w.t().contiguous())
-        n, c = pts.shape[0], self.proj_d.out_features
-        out = GF.scratch((n, n, c), pts.device, scratch_tag) if scratch_tag is not None else None
-        emb = GF.gse_embed(d, a, self.embedding.div_term, self.proj_d.weight.detach(), self.proj_a.weight.detach(),
-                           self.proj_d.bias.detach(), self.proj_a.bias.detach(), wd_t, wa_t, out=out, table=self.table())
+        n = pts.shape[0]
+        with torch.no_grad():
+            emb = self.forward_flat(pts, [n]).view(n, n, -1)
         return emb.unsqueeze(0) if squeeze else emb
 
-    def forward_grad(self, points):
-        """``forward`` of one (N, 3) cloud with the graph to proj_d / proj_a (when they require grad in grad mode): E is a fresh tensor
-        the backward keeps (not a scratch view), computed by the same kernels, so its values are ``forward``'s bit for bit.  GeometricTransformer uses it in grad
-        mode; the backward takes the winning angle terms from the table of the current weights whatever GF.GSE_MODE."""
-        pts = points.contiguous()
-        d, a = GF.gse_indices(pts, self.sigma_d, self.sigma_a, self.angle_k)
-        wd_t = self._cache.get('wd_t', self.proj_d.weight, lambda w: w.t().contiguous())
-        wa_t = self._cache.get('wa_t', self.proj_a.weight, lambda w: w.t().contiguous())
-        return GF.gse_embed(d, a, self.embedding.div_term, self.proj_d.weight, self.proj_a.weight, self.proj_d.bias, self.proj_a.bias,
-                            wd_t, wa_t, table=self._weights_table())
-
-    def forward_flat_grad(self, points, cloud_rows):
+    def forward_flat(self, points, cloud_rows):
         """The structure embeddings of several stacked clouds (``cloud_rows``: their row counts) as ONE flat (sum n_c^2, C) tensor,
-        cloud after cloud, with the graph to proj_d / proj_a: one ``gse_indices_batched`` and one ``gse_embed_flat`` launch, the
-        kernels of the batched forward (``GeoTransformer.forward_batch``), so the values are its bits.  The backward
-        (``geob200_gse_embed_backward``) sums over all rows of all clouds."""
+        cloud after cloud: one ``gse_indices_batched`` and one ``gse_embed_flat`` launch, the kernels of the batched forward
+        (``GeoTransformer.forward_batch``), so the values are its bits.  E is always a fresh tensor.  In grad mode it carries the graph
+        to proj_d / proj_a when they require grad; the backward (``geob200_gse_embed_backward``) sums over all rows of all clouds."""
         rows = [int(r) for r in cloud_rows]
         n2 = sum(r * r for r in rows)
         dev = points.device
@@ -138,34 +122,22 @@ class GeometricTransformer(nn.Module):
         batched = ref_points.ndim == 3
         if batched:
             ref_points, src_points, ref_feats, src_feats = ref_points[0], src_points[0], ref_feats[0], src_feats[0]
-        if GF._needs_grad(ref_feats, src_feats, *self.parameters()):
-            # the graph's attention nodes keep E: fresh tensors, never the scratch the next forward overwrites (also with a frozen
-            # embedding, when forward_grad runs the no-grad kernels into a fresh tensor)
-            ref_emb, src_emb = self.embedding.forward_grad(ref_points), self.embedding.forward_grad(src_points)
-        else:
-            ref_emb = self.embedding(ref_points, scratch_tag='gse_ref')     # consumed inside this forward only
-            src_emb = self.embedding(src_points, scratch_tag='gse_src')
-        n0, n1 = ref_feats.shape[0], src_feats.shape[0]
-        # both clouds share every weight: keep them stacked [ref; src] through the whole transformer
-        x = torch.empty((n0 + n1, self.in_proj.out_features), dtype=torch.float32, device=ref_feats.device)
-        GF.linear(ref_feats, self.in_proj.weight, self.in_proj.bias, out=x[:n0])
-        GF.linear(src_feats, self.in_proj.weight, self.in_proj.bias, out=x[n0:])
-        x = self.transformer.forward_stacked(x, n0, ref_emb, src_emb)
-        y = GF.linear(x, self.out_proj.weight, self.out_proj.bias)
+        n0 = ref_feats.shape[0]
+        y = self.forward_stacked(torch.cat([ref_points, src_points]), torch.cat([ref_feats, src_feats]), [n0, src_feats.shape[0]])
         rf, sf = y[:n0], y[n0:]
         if batched:
             return rf.unsqueeze(0), sf.unsqueeze(0)
         return rf, sf
 
-
-    def forward_batched_grad(self, points_c, feats_c, cloud_rows):
+    def forward_stacked(self, points_c, feats_c, cloud_rows):
         """The transformer (with in_proj and out_proj, before the L2 normalisation) over the stacked superpoints of B pairs (stack order
-        [ref_1..ref_B, src_1..src_B], ``cloud_rows``: the 2B row counts), with the graph to every parameter and to ``feats_c``: the
-        kernels of the batched native forward in its order (one structure-embedding launch for all clouds, one in_proj / out_proj
-        GEMM over all rows, ``RPEConditionalTransformer.forward_batched_grad``)."""
-        E = self.embedding.forward_flat_grad(points_c, cloud_rows)
+        [ref_1..ref_B, src_1..src_B], ``cloud_rows``: the 2B row counts): the kernels of the batched native forward in its order
+        (one structure-embedding launch for all clouds, one in_proj / out_proj GEMM over all rows,
+        ``RPEConditionalTransformer.forward_stacked``).  In grad mode it carries the graph to every parameter that requires grad and
+        to ``feats_c``."""
+        E = self.embedding.forward_flat(points_c, cloud_rows)
         x = GF.linear(feats_c, self.in_proj.weight, self.in_proj.bias)
-        x = self.transformer.forward_batched_grad(x, cloud_rows, E)
+        x = self.transformer.forward_stacked(x, cloud_rows, E)
         return GF.linear(x, self.out_proj.weight, self.out_proj.bias)
 
 

@@ -186,14 +186,14 @@ class TransformerLayer(nn.Module):
         return self.output(hidden), scores
 
 
-def _tail(layer, hidden, inp, out=None):
+def _tail(layer, hidden, inp):
     """attention.linear + residual LayerNorm, then the FFN block with its residual LayerNorm (5 launches)."""
     att, ffn = layer.attention, layer.output
     h = GF.linear(hidden, att.linear.weight, att.linear.bias)
     x = GF.add_layernorm(h, inp, att.norm.weight, att.norm.bias, att.norm.eps)
     y = GF.linear(x, ffn.expand.weight, ffn.expand.bias, relu=True)
     y = GF.linear(y, ffn.squeeze.weight, ffn.squeeze.bias)
-    return GF.add_layernorm(x, y, ffn.norm.weight, ffn.norm.bias, ffn.norm.eps, out=out)
+    return GF.add_layernorm(x, y, ffn.norm.weight, ffn.norm.bias, ffn.norm.eps)
 
 
 def _fused(cache, mha, names, layer):
@@ -209,6 +209,11 @@ def _fused(cache, mha, names, layer):
         hit = (stamp, (w, b))
         cache._c[key] = hit
     return hit[1]
+
+
+def _concat(mha, names):
+    """the fused projection weight / bias of ``_fused``, concatenated from the parameters themselves (with their graph)"""
+    return (torch.cat([getattr(mha, n).weight for n in names], dim=0), torch.cat([getattr(mha, n).bias for n in names], dim=0))
 
 
 class RPEConditionalTransformer(nn.Module):
@@ -229,128 +234,59 @@ class RPEConditionalTransformer(nn.Module):
         self.layers = nn.ModuleList(layers)
         self.return_attention_scores = return_attention_scores
         self.parallel = parallel
+        self._cache = _WeightCache()
 
     def forward(self, feats0, feats1, embeddings0, embeddings1, masks0=None, masks1=None):
         _no_masks(masks0=masks0, masks1=masks1)
-        n0 = feats0.shape[0]
-        x = torch.empty((n0 + feats1.shape[0], feats0.shape[1]), dtype=feats0.dtype, device=feats0.device)
-        x[:n0].copy_(feats0)
-        x[n0:].copy_(feats1)
-        x = self.forward_stacked(x, n0, embeddings0, embeddings1)
+        n0, n1, c = feats0.shape[0], feats1.shape[0], embeddings0.shape[-1]
+        E = torch.cat([embeddings0.reshape(n0 * n0, c), embeddings1.reshape(n1 * n1, c)])
+        x = self.forward_stacked(torch.cat([feats0, feats1]), [n0, n1], E)
         return x[:n0], x[n0:]
 
-    def forward_stacked(self, x, n0, embeddings0, embeddings1):
-        """Same computation on the stacked features [feats0; feats1] (they share every layer's weights): the q|k|v
-        projections of both clouds are ONE GEMM, the attention kernel reads them as column slices, and the
-        Linear/LayerNorm/FFN tail runs once per layer on all rows.  In grad mode the same kernels build the autograd graph
-        (``_forward_stacked_grad``)."""
-        if GF._needs_grad(x, embeddings0, embeddings1, *self.parameters()):
-            return self._forward_stacked_grad(x, n0, embeddings0, embeddings1)
-        if not hasattr(self, '_cache'):
-            self._cache = _WeightCache()
-        c = x.shape[1]
-        for i, block in enumerate(self.blocks):
-            layer = self.layers[i]
-            mha = layer.attention.attention
-            h = mha.num_heads
-            if block == 'self':
-                w, b = _fused(self._cache, mha, ('proj_q', 'proj_k', 'proj_v'), i)
-                qkv = GF.linear(x, w, b)                                          # (N0+N1, 3C)
-                q, k, v = qkv[:, :c], qkv[:, c:2 * c], qkv[:, 2 * c:]
-                wp_t = self._cache.get(f'wp_t{i}', mha.proj_p.weight, lambda p: p.t().contiguous())
-                qp, qb = GF.head_project(q, wp_t, mha.proj_p.bias.detach(), h)
-                hidden = torch.empty_like(x)
-                GF.attention(q[:n0], k[:n0], v[:n0], h, qp=qp[:n0], qb=qb[:n0], embed=embeddings0, out=hidden[:n0])
-                GF.attention(q[n0:], k[n0:], v[n0:], h, qp=qp[n0:], qb=qb[n0:], embed=embeddings1, out=hidden[n0:])
-                x = _tail(layer, hidden, x)
-            else:
-                wkv, bkv = _fused(self._cache, mha, ('proj_k', 'proj_v'), i)
-                y = torch.empty_like(x)
-                # feats0 <- layer(feats0, feats1)
-                q0 = GF.linear(x[:n0], mha.proj_q.weight, mha.proj_q.bias)
-                kv1 = GF.linear(x[n0:], wkv, bkv)
-                hid0 = GF.attention(q0, kv1[:, :c], kv1[:, c:], h)
-                _tail(layer, hid0, x[:n0], out=y[:n0])
-                # feats1 <- layer(feats1, feats0): sees the UPDATED feats0 unless `parallel`
-                mem = x[:n0] if self.parallel else y[:n0]
-                q1 = GF.linear(x[n0:], mha.proj_q.weight, mha.proj_q.bias)
-                kv0 = GF.linear(mem, wkv, bkv)
-                hid1 = GF.attention(q1, kv0[:, :c], kv0[:, c:], h)
-                _tail(layer, hid1, x[n0:], out=y[n0:])
-                x = y
-        return x
-
-    def _forward_stacked_grad(self, x, n0, embeddings0, embeddings1):
-        """``forward_stacked`` with the graph: the fused projection weights are concatenated from the parameters (autograd splits
-        their gradient back onto proj_q / proj_k / proj_v), proj_p enters head_project as its transposed view, and the two clouds'
-        halves are fresh tensors stacked by torch.cat (no in-place write into a tensor whose view a backward has saved).  Every
-        kernel is the no-grad path's, so the values are bit-identical."""
+    def forward_stacked(self, x, cloud_rows, embeddings):
+        """The transformer over the stacked rows of B pairs, the kernel sequence of ``geob200_transformer_forward_batched``: x rows in
+        stack order [ref_1..ref_B, src_1..src_B] (``cloud_rows``: their 2B row counts), ``embeddings`` the flat structure embeddings
+        of the 2B clouds one after the other (sum n_c^2, C).  Every Linear / LayerNorm runs once over all rows (the ref block and the
+        src block are contiguous, so a cross layer's projections are single GEMMs too); attention runs as one batched launch pair per
+        phase, one item per cloud (self) or per pair (cross).  Carries the graph in grad mode when an input or a parameter requires
+        grad; the kernels, and so the values, are the same either way."""
+        rows = [int(r) for r in cloud_rows]
         for i in range(len(self.blocks)):
-            x = self._layer_grad(i, x, n0, embeddings0, embeddings1)
+            x = self._layer(i, x, rows, embeddings)
         return x
 
-    def _layer_grad(self, i, x, n0, embeddings0, embeddings1):
-        """layer i of ``_forward_stacked_grad`` on the stacked rows x"""
-        c = x.shape[1]
-        block, layer = self.blocks[i], self.layers[i]
+    def _layer(self, i, x, rows, embeddings):
+        """layer i of ``forward_stacked`` on the stacked rows x"""
+        B, c = len(rows) // 2, x.shape[1]
+        ref, src = rows[:B], rows[B:]
+        layer = self.layers[i]
         mha = layer.attention.attention
         h = mha.num_heads
-        if block == 'self':
-            w, b = _concat(mha, ('proj_q', 'proj_k', 'proj_v'))
-            qkv = GF.linear(x, w, b)                                          # (N0+N1, 3C)
+        if self.blocks[i] == 'self':
+            (w, b), wp_t = self._weights(i, ('proj_q', 'proj_k', 'proj_v'))
+            qkv = GF.linear(x, w, b)
             q, k, v = qkv[:, :c], qkv[:, c:2 * c], qkv[:, 2 * c:]
-            qp, qb = GF.head_project(q, mha.proj_p.weight.t(), mha.proj_p.bias, h)
-            hid0 = GF.attention(q[:n0], k[:n0], v[:n0], h, qp=qp[:n0], qb=qb[:n0], embed=embeddings0)
-            hid1 = GF.attention(q[n0:], k[n0:], v[n0:], h, qp=qp[n0:], qb=qb[n0:], embed=embeddings1)
-            x = _tail(layer, torch.cat([hid0, hid1]), x)
-        else:
-            wkv, bkv = _concat(mha, ('proj_k', 'proj_v'))
-            q0 = GF.linear(x[:n0], mha.proj_q.weight, mha.proj_q.bias)
-            kv1 = GF.linear(x[n0:], wkv, bkv)
-            y0 = _tail(layer, GF.attention(q0, kv1[:, :c], kv1[:, c:], h), x[:n0])
-            mem = x[:n0] if self.parallel else y0
-            q1 = GF.linear(x[n0:], mha.proj_q.weight, mha.proj_q.bias)
-            kv0 = GF.linear(mem, wkv, bkv)
-            y1 = _tail(layer, GF.attention(q1, kv0[:, :c], kv0[:, c:], h), x[n0:])
-            x = torch.cat([y0, y1])
-        return x
+            qp, qb = GF.head_project(q, wp_t, mha.proj_p.bias, h)
+            return _tail(layer, GF.attention_batched(q, k, v, h, rows, rows, qp=qp, qb=qb, embed=embeddings), x)
+        (wkv, bkv), _ = self._weights(i, ('proj_k', 'proj_v'))
+        R = sum(ref)
+        x0, x1 = x[:R], x[R:]
+        q0 = GF.linear(x0, mha.proj_q.weight, mha.proj_q.bias)
+        kv1 = GF.linear(x1, wkv, bkv)
+        y0 = _tail(layer, GF.attention_batched(q0, kv1[:, :c], kv1[:, c:], h, ref, src), x0)
+        mem = x0 if self.parallel else y0          # the src update sees the UPDATED ref rows unless `parallel`
+        q1 = GF.linear(x1, mha.proj_q.weight, mha.proj_q.bias)
+        kv0 = GF.linear(mem, wkv, bkv)
+        y1 = _tail(layer, GF.attention_batched(q1, kv0[:, :c], kv0[:, c:], h, src, ref), x1)
+        return torch.cat([y0, y1])
 
-
-    def forward_batched_grad(self, x, cloud_rows, embeddings):
-        """The transformer over the stacked rows of B pairs with the graph, the kernel sequence of
-        ``geob200_transformer_forward_batched``: x rows in stack order [ref_1..ref_B, src_1..src_B] (``cloud_rows``: their 2B row
-        counts), ``embeddings`` the flat structure embeddings of the 2B clouds one after the other (sum n_c^2, C).  Every Linear /
-        LayerNorm runs once over all rows (the ref block and the src block are contiguous, so a cross layer's projections are single
-        GEMMs too); attention runs as one batched launch pair per phase, one item per cloud (self) or per pair (cross)."""
-        rows = [int(r) for r in cloud_rows]
-        B = len(rows) // 2
-        R, c = sum(rows[:B]), x.shape[1]
-        ref, src = rows[:B], rows[B:]
-        for i, block in enumerate(self.blocks):
-            layer = self.layers[i]
-            mha = layer.attention.attention
-            h = mha.num_heads
-            if block == 'self':
-                w, b = _concat(mha, ('proj_q', 'proj_k', 'proj_v'))
-                qkv = GF.linear(x, w, b)
-                q, k, v = qkv[:, :c], qkv[:, c:2 * c], qkv[:, 2 * c:]
-                qp, qb = GF.head_project(q, mha.proj_p.weight.t(), mha.proj_p.bias, h)
-                hidden = GF.attention_batched(q, k, v, h, rows, rows, qp=qp, qb=qb, embed=embeddings)
-                x = _tail(layer, hidden, x)
-            else:
-                wkv, bkv = _concat(mha, ('proj_k', 'proj_v'))
-                x0, x1 = x[:R], x[R:]
-                q0 = GF.linear(x0, mha.proj_q.weight, mha.proj_q.bias)
-                kv1 = GF.linear(x1, wkv, bkv)
-                y0 = _tail(layer, GF.attention_batched(q0, kv1[:, :c], kv1[:, c:], h, ref, src), x0)
-                mem = x0 if self.parallel else y0
-                q1 = GF.linear(x1, mha.proj_q.weight, mha.proj_q.bias)
-                kv0 = GF.linear(mem, wkv, bkv)
-                y1 = _tail(layer, GF.attention_batched(q1, kv0[:, :c], kv0[:, c:], h, src, ref), x1)
-                x = torch.cat([y0, y1])
-        return x
-
-
-def _concat(mha, names):
-    """the fused projection weight / bias of ``_fused``, concatenated from the parameters themselves (with their graph)"""
-    return (torch.cat([getattr(mha, n).weight for n in names], dim=0), torch.cat([getattr(mha, n).bias for n in names], dim=0))
+    def _weights(self, i, names):
+        """((w, b) of the named projections of layer i stacked for one GEMM, proj_p's transpose or None for a cross layer).  With a
+        graph to the layer's parameters they are taken from the parameters themselves (autograd splits the fused gradient back onto
+        each projection); without one they are the cached copies, rebuilt only when a parameter changes."""
+        mha = self.layers[i].attention.attention
+        rpe = isinstance(mha, RPEMultiHeadAttention)
+        if GF._needs_grad(*mha.parameters()):
+            return _concat(mha, names), (mha.proj_p.weight.t() if rpe else None)
+        wp_t = self._cache.get(f'wp_t{i}', mha.proj_p.weight, lambda p: p.t().contiguous()) if rpe else None
+        return _fused(self._cache, mha, names, i), wp_t

@@ -187,7 +187,7 @@ def test_batched_backbone_gradient_matches_fp64_autograd_of_the_mean(workload, c
 
 
 @pytest.mark.parametrize('workload,cfg_name,B', ORACLE_CASES + [('3dmatch20k', '3dmatch', 2)])
-def test_batched_transformer_gradient_matches_fp64_autograd_of_the_mean(workload, cfg_name, B, models):
+def test_stacked_transformer_gradient_matches_fp64_autograd_of_the_mean(workload, cfg_name, B, models):
     """the batched transformer (per-cloud self items, per-pair cross items, one structure-embedding launch) on the batch's own coarse
     features: every transformer parameter's gradient and the coarse-feature gradient of the mean over pairs of <y of pair p, G_p>
     against the mean over pairs of fp64 autograd of the restatement run on each pair alone"""
@@ -200,7 +200,7 @@ def test_batched_transformer_gradient_matches_fp64_autograd_of_the_mean(workload
     cn = [int(v) for v in data['lengths_host'][-1]]
     fc = feats_c.clone().requires_grad_(True)
     tr = model.transformer
-    y = tr.forward_batched_grad(pts, fc, cn)
+    y = tr.forward_stacked(pts, fc, cn)
     c_out = y.shape[1]
     shapes = [[(cn[p], c_out), (cn[B + p], c_out)] for p in range(B)]
     up = torch.zeros_like(y)

@@ -268,7 +268,8 @@ def _gse_ref(d, a, div, wd, bd, wa, ba):
 
 
 @pytest.mark.parametrize('cfg_name', ['3dmatch', 'kitti'])
-def test_structure_embedding_backward_matches_fp64_autograd(cfg_name, models):
+def test_flat_structure_embedding_backward_matches_fp64_autograd(cfg_name, models):
+    """forward_flat of one cloud: its graph's backward against fp64 autograd; its values are those of forward, which carries no graph"""
     cfg, sd, _ = models(cfg_name)
     emb = _fresh(cfg, sd).transformer.embedding
     c = emb.proj_d.out_features
@@ -287,7 +288,7 @@ def test_structure_embedding_backward_matches_fp64_autograd(cfg_name, models):
 
     w64 = _ref_grads(loss, params, torch.float64)
     w32 = _ref_grads(loss, params, torch.float32)
-    out = emb.forward_grad(pts)
+    out = emb.forward_flat(pts, [60]).view(60, 60, c)
     ref = emb(pts)
     assert not ref.requires_grad
     assert torch.equal(_bits(out.detach()), _bits(ref)), 'forward bits change with the graph'
@@ -298,7 +299,7 @@ def test_structure_embedding_backward_matches_fp64_autograd(cfg_name, models):
     grads = [p.grad.clone() for p in params]
     for p in params:
         p.grad = None
-    emb.forward_grad(pts).backward(up.cuda())
+    emb.forward_flat(pts, [60]).view(60, 60, c).backward(up.cuda())
     for a_, p in zip(grads, params):
         assert torch.equal(_bits(a_), _bits(p.grad)), 'two backward runs differ'
 
@@ -467,7 +468,7 @@ def test_sgd_step_rebuilds_cached_weights(models):
 
 
 @pytest.mark.parametrize('workload,cfg_name', BV.WORKLOADS)
-def test_every_layer_in_the_chain_matches_fp64_autograd(workload, cfg_name, models):
+def test_every_stacked_layer_matches_fp64_autograd(workload, cfg_name, models):
     """every piece of the whole transformer at the product's own activations and upstream gradients against fp64 autograd of its
     restatement, under the 10 x fp32-autograd rule: in_proj, each self / cross layer (parameters and input), out_proj, and the
     structure embedding's backward at the product's dE (near-ties of the angle max masked, see _near_ties)"""
@@ -478,28 +479,30 @@ def test_every_layer_in_the_chain_matches_fp64_autograd(workload, cfg_name, mode
     tr = model.transformer
     st = tr.transformer
     heads = cfg.geotransformer.num_heads
-    xs, embs = [], []
-    layer_grad = st._layer_grad
+    xs, flat = [], []
+    layer = st._layer
 
-    def tapped(i, x, n0, e0, e1):
+    def tapped(i, x, rows, E):
         if i == 0:
             x.retain_grad()
             xs.append(x)
-            for e in (e0, e1):
-                e.retain_grad()
-                embs.append(e)
-        y = layer_grad(i, x, n0, e0, e1)
+            E.retain_grad()
+            flat.append(E)
+        y = layer(i, x, rows, E)
         y.retain_grad()
         xs.append(y)
         return y
 
-    st._layer_grad = tapped
+    st._layer = tapped
     rfc, sfc = rf.clone().requires_grad_(True), sf.clone().requires_grad_(True)
     y0, y1 = tr(rp, sp, rfc, sfc)
     ups = [u.cuda() for u in BV.upstream([tuple(y0.shape), tuple(y1.shape)])]
     ((y0 * ups[0]).sum() + (y1 * ups[1]).sum()).backward()
-    del st._layer_grad
-    n0 = rp.shape[0]
+    del st._layer
+    n0, n1 = rp.shape[0], sp.shape[0]
+    E, dE = flat[0].detach(), flat[0].grad
+    # each cloud's E and dE: its row block of the flat E
+    embs = [(E[o:o + n * n].view(n, n, -1), dE[o:o + n * n].view(n, n, -1)) for o, n in ((0, n0), (n0 * n0, n1))]
     grads = dict(tr.named_parameters())
     up_all = torch.cat(ups).cpu()
     feats = torch.cat([rf, sf]).cpu()
@@ -519,7 +522,7 @@ def test_every_layer_in_the_chain_matches_fp64_autograd(workload, cfg_name, mode
 
     check('in_proj', ['in_proj.weight', 'in_proj.bias'], lin('in_proj'), feats, torch.cat([rfc.grad, sfc.grad]))
     check('out_proj', ['out_proj.weight', 'out_proj.bias'], lin('out_proj'), xs[-1], None)
-    e_cpu = [e.detach().cpu() for e in embs]
+    e_cpu = [e.cpu() for e, _ in embs]
     for i, block in enumerate(cfg.geotransformer.blocks):
         pre = f'transformer.layers.{i}.'
         keys = [k for k in grads if k.startswith(pre)]
@@ -543,9 +546,9 @@ def test_every_layer_in_the_chain_matches_fp64_autograd(workload, cfg_name, mode
     ekeys = ['embedding.proj_d.weight', 'embedding.proj_d.bias', 'embedding.proj_a.weight', 'embedding.proj_a.bias']
     got = [torch.zeros_like(grads[k]) for k in ekeys]
     ups_e, idx = [], []
-    for pts, e in zip((rp, sp), embs):
+    for pts, (_, de) in zip((rp, sp), embs):
         d, a = GF.gse_indices(pts, emb.sigma_d, emb.sigma_a, emb.angle_k)
-        de = e.grad.clone()
+        de = de.clone()
         de[_near_ties(a.cpu().double(), div, emb.proj_a.weight, emb.proj_a.bias).cuda()] = 0.0
         n = pts.shape[0]
         gwd, gbd, gwa, gba = GF.gse_embed_backward(d, a, n * n, emb.embedding.div_term, emb.proj_a.weight, emb.proj_a.bias, table,
