@@ -33,6 +33,9 @@ _sig('geob200_radius_search_workspace_bytes', SZ, I64, I64, I64)
 _sig('geob200_radius_search', c_int, P, I64, P, I64, P, P, I64, F, I64, P, P, P, P, SZ, P)
 
 _sig('geob200_neighbor_histogram', c_int, P, I64, I64, I64, I64, P, P)
+_sig('geob200_neighbor_histogram_batched', c_int, P, P, P, I64, I64, I64, I64, P, P, P, P)
+_sig('geob200_kernel_point_optimize', c_int, P, I64, I64, ctypes.c_uint64, D, P, P, P)
+_sig('geob200_kernel_point_instances', c_int, P, I64, P, P, I64, ctypes.c_uint64, P, P)
 _sig('geob200_kpconv_workspace_bytes', SZ, I64)
 _sig('geob200_kpconv', c_int, P, P, P, P, I64, I64, I64, P, I64, P, P, I64, I64, F, P, P, SZ, P)
 _sig('geob200_kpconv_tc_workspace_bytes', SZ, I64, I64, I64)

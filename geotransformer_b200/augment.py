@@ -45,10 +45,10 @@ def check_options(cfg):
             raise NotImplementedError('3DMatch rotated=True (off in every shipped training config)')
 
 
-def augment_stacked(pairs, cfg, seed, iteration, device):
+def augment_stacked(pairs, cfg, seed, iteration, device, pair_base=0):
     """the augmented clouds of ``pairs`` on the device: (points stacked [ref..., src...], lengths_host, transforms (B, 4, 4), origin,
     record), from ``functional.augment_pairs_batched`` (3DMatch, KITTI) or ``functional.modelnet_pairs_batched`` (ModelNet).  Pair p
-    draws from the streams (seed, iteration, p)."""
+    draws from the streams (seed, iteration, pair_base + p)."""
     check_options(cfg)
     if cfg.name == 'modelnet':
         shapes = [_t(d['points']) for d in pairs]
@@ -56,7 +56,7 @@ def augment_stacked(pairs, cfg, seed, iteration, device):
         raw = _stack_to_device([s.float() for s in shapes], device)
         d, tr = cfg.data, cfg.train
         return GF.modelnet_pairs_batched(raw, lengths, d.num_points, d.keep_ratio, d.rotation_magnitude, d.translation_magnitude,
-                                         tr.noise_magnitude, seed, iteration)
+                                         tr.noise_magnitude, seed, iteration, pair_base)
     clouds = [_t(d['ref_points']) for d in pairs] + [_t(d['src_points']) for d in pairs]
     lengths = [int(c.shape[0]) for c in clouds]
     raw = _stack_to_device([c.float() for c in clouds], device)
@@ -64,9 +64,10 @@ def augment_stacked(pairs, cfg, seed, iteration, device):
     tr = cfg.train
     if cfg.name == 'kitti':
         return GF.augment_pairs_batched(raw, lengths, T, GF.AUGMENT_KITTI, tr.point_limit, tr.augmentation_noise, tr.augmentation_rotation,
-                                        tr.augmentation_min_scale, tr.augmentation_max_scale, tr.augmentation_shift, seed, iteration)
+                                        tr.augmentation_min_scale, tr.augmentation_max_scale, tr.augmentation_shift, seed, iteration,
+                                        pair_base)
     return GF.augment_pairs_batched(raw, lengths, T, GF.AUGMENT_3DMATCH, tr.point_limit, tr.augmentation_noise, tr.augmentation_rotation,
-                                    seed=seed, iteration=iteration)
+                                    seed=seed, iteration=iteration, pair_base=pair_base)
 
 
 def augmented_collate(pairs, cfg, neighbor_limits, seed, iteration, device='cuda'):

@@ -717,6 +717,70 @@ __global__ void __launch_bounds__(256) neighbor_histogram_kernel(const long long
     if (c < hist_n) atomicAdd(&hist[c], 1);
 }
 
+// the batched calibration's stage tables: pointers, widths, row counts and each cloud's first row per stage
+struct HistStages {
+    const long long* nbr[GEOB200_MAX_STAGES];
+    long long rows[GEOB200_MAX_STAGES];
+    int width[GEOB200_MAX_STAGES];
+    int cloud_start[GEOB200_MAX_STAGES][2 * GEOB200_HIST_MAX_PAIRS + 1];
+};
+
+// one thread per row of stage blockIdx.y: the row's valid-entry count goes to the histogram of its pair (cloud c is pair c mod B)
+__global__ void __launch_bounds__(256) neighbor_histogram_batched_kernel(HistStages st, int num_stages, int batch, int hist_n,
+                                                                         int* __restrict__ hists) {
+    const int s = blockIdx.y;
+    const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= st.rows[s]) return;
+    const int w = st.width[s];
+    const long long* row = st.nbr[s] + r * w;
+    int c = 0;
+    for (int j = 0; j < w; ++j) c += row[j] < st.rows[s] ? 1 : 0;
+    if (c >= hist_n) return;
+    int cloud = 0;
+    while (cloud + 1 < 2 * batch && r >= st.cloud_start[s][cloud + 1]) ++cloud;
+    atomicAdd(&hists[((size_t)(cloud % batch) * num_stages + s) * hist_n + c], 1);
+}
+
+// the reference's early exit over the batch's pairs in order, continuing the running totals of earlier calls
+__global__ void __launch_bounds__(256) neighbor_histogram_stop_kernel(const int* __restrict__ hists, int num_stages, int batch,
+                                                                      int hist_n, long long threshold, int* __restrict__ totals,
+                                                                      int* __restrict__ stop) {
+    __shared__ long long row_sum[GEOB200_HIST_MAX_PAIRS * GEOB200_MAX_STAGES];
+    __shared__ long long base[GEOB200_MAX_STAGES];
+    __shared__ int last;
+    const int t = threadIdx.x;
+    for (int i = t; i < batch * num_stages; i += blockDim.x) {
+        long long v = 0;
+        for (int h = 0; h < hist_n; ++h) v += hists[(size_t)i * hist_n + h];
+        row_sum[i] = v;
+    }
+    for (int s = t; s < num_stages; s += blockDim.x) {
+        long long v = 0;
+        for (int h = 0; h < hist_n; ++h) v += totals[(size_t)s * hist_n + h];
+        base[s] = v;
+    }
+    __syncthreads();
+    if (t == 0) {
+        int found = -1;
+        for (int p = 0; p < batch && found < 0; ++p) {
+            bool all = true;
+            for (int s = 0; s < num_stages; ++s) {
+                base[s] += row_sum[p * num_stages + s];
+                all = all && base[s] > threshold;
+            }
+            if (all) found = p;
+        }
+        *stop = found;
+        last = found >= 0 ? found : batch - 1;
+    }
+    __syncthreads();
+    for (int i = t; i < num_stages * hist_n; i += blockDim.x) {
+        int v = totals[i];
+        for (int p = 0; p <= last; ++p) v += hists[(size_t)p * num_stages * hist_n + i];
+        totals[i] = v;
+    }
+}
+
 }  // namespace geob200
 
 using namespace geob200;
@@ -883,6 +947,45 @@ int geob200_neighbor_histogram(const int64_t* neighbors, int64_t n_rows, int64_t
         (const long long*)neighbors, (long long)n_rows, (int)width, (long long)n_support, (int)hist_n, hist);
     GEOB_CHECK_LAUNCH();
     count_launches(1);
+    return 0;
+}
+
+int geob200_neighbor_histogram_batched(const int64_t* const* neighbors, const int64_t* widths, const int64_t* cloud_rows,
+                                       int64_t num_stages, int64_t batch, int64_t hist_n, int64_t sample_threshold, int32_t* hists,
+                                       int32_t* totals, int32_t* stop, void* stream) {
+    GEOB_REQUIRE(num_stages >= 1 && num_stages <= GEOB200_MAX_STAGES, "neighbor_histogram_batched: num_stages must be in 1..%d",
+                 GEOB200_MAX_STAGES);
+    GEOB_REQUIRE(batch >= 1 && batch <= GEOB200_HIST_MAX_PAIRS, "neighbor_histogram_batched: batch must be in 1..%d",
+                 GEOB200_HIST_MAX_PAIRS);
+    GEOB_REQUIRE(hist_n >= 1 && hist_n <= (1 << 20), "neighbor_histogram_batched: hist_n must be in 1..2^20");
+    GEOB_REQUIRE(neighbors != nullptr && widths != nullptr && cloud_rows != nullptr && hists != nullptr && totals != nullptr &&
+                 stop != nullptr, "neighbor_histogram_batched: null pointer");
+    HistStages st;
+    long long max_rows = 0;
+    for (int s = 0; s < (int)num_stages; ++s) {
+        GEOB_REQUIRE(neighbors[s] != nullptr && widths[s] >= 1 && widths[s] <= (1 << 20),
+                     "neighbor_histogram_batched: stage %d has no table or a bad width", s);
+        long long row = 0;
+        for (int c = 0; c < 2 * (int)batch; ++c) {
+            GEOB_REQUIRE(cloud_rows[s * 2 * batch + c] >= 1, "neighbor_histogram_batched: stage %d cloud %d is empty", s, c);
+            st.cloud_start[s][c] = (int)row;
+            row += cloud_rows[s * 2 * batch + c];
+            GEOB_REQUIRE(row < (1LL << 31), "neighbor_histogram_batched: stage %d has 2^31 rows or more", s);
+        }
+        st.cloud_start[s][2 * batch] = (int)row;
+        st.nbr[s] = (const long long*)neighbors[s];
+        st.rows[s] = row;
+        st.width[s] = (int)widths[s];
+        max_rows = row > max_rows ? row : max_rows;
+    }
+    cudaStream_t cs = (cudaStream_t)stream;
+    GEOB_CHECK_CUDA(cudaMemsetAsync(hists, 0, sizeof(int32_t) * (size_t)batch * num_stages * hist_n, cs));
+    neighbor_histogram_batched_kernel<<<dim3((unsigned)((max_rows + 255) / 256), (unsigned)num_stages), 256, 0, cs>>>(
+        st, (int)num_stages, (int)batch, (int)hist_n, hists);
+    neighbor_histogram_stop_kernel<<<1, 256, 0, cs>>>(hists, (int)num_stages, (int)batch, (int)hist_n, (long long)sample_threshold,
+                                                      totals, stop);
+    GEOB_CHECK_LAUNCH();
+    count_launches(2);
     return 0;
 }
 

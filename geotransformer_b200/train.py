@@ -281,6 +281,22 @@ class TrainingEngine:
             self.scheduler.step()
         return results
 
+    def train_groups(self, groups, log=None):
+        """one epoch over the steps of an iterable of pair groups (``datasets.loader.PrefetchLoader.epoch``), pulled one at a time so
+        that only the loader's prefetched steps are held in memory; then the per-epoch scheduler step (3DMatch, KITTI).  As in
+        ``train_epoch``, steps are ``train_step`` with batch_size 1 and ``train_batch`` otherwise.  ``log(result)`` is called after
+        every step; returns the step results."""
+        self.epoch += 1
+        results = []
+        for group in groups:
+            res = self.train_step(group[0]) if self.batch_size == 1 else self.train_batch(group)
+            results.append(res)
+            if log is not None:
+                log(res)
+        if not self.per_iteration:
+            self.scheduler.step()
+        return results
+
     def _param_versions(self):
         return tuple((p.data_ptr(), p._version) for p in self.model.parameters())
 

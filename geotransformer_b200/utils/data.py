@@ -4,6 +4,8 @@ The reference runs this on CPU inside DataLoader worker processes (single-thread
 forked workers, so here the raw pair is moved to the device and collated in the main process on the current stream
 (the reference already has the switch for handing raw pairs through: ``precompute_data=False``, ``data.py:181-186``).
 """
+import ctypes
+
 import numpy as np
 import torch
 
@@ -122,3 +124,48 @@ def calibrate_neighbors_stack_mode(dataset, collate_fn, num_stages, voxel_size, 
     cum_sum = np.cumsum(neighbor_hists.T, axis=0)
     neighbor_limits = np.sum(cum_sum < (keep_ratio * cum_sum[hist_n - 1, :]), axis=0)
     return neighbor_limits
+
+
+# the augmentation "iteration" of the calibration's draws: training iterations count up from 1, so they never reach it
+CALIBRATION_ITERATION = (1 << 64) - 1
+HIST_MAX_PAIRS = 32         # GEOB200_HIST_MAX_PAIRS
+
+
+def calibrate_neighbors_augmented(pairs, cfg, seed, keep_ratio=0.8, sample_threshold=2000, chunk=16, device=None):
+    """the reference's ``calibrate_neighbors_stack_mode(train_dataset, ...)`` on the AUGMENTED training set: pair p is augmented
+    as ``augment.augment_stacked`` draws it from the streams (seed, CALIBRATION_ITERATION, p), and the histograms stop at the first
+    pair after which every stage has more than ``sample_threshold`` rows, as the reference's loop does.  ``chunk`` pairs are
+    augmented and collated at the histogram width in one go (``geob200_neighbor_histogram_batched``), with one read-back per
+    chunk.  ``pairs``: an indexable of training pairs (raw shapes for ModelNet).  Returns (neighbor limits, pairs used)."""
+    from .. import _lib as L
+    from ..augment import augment_stacked
+    if not 1 <= chunk <= HIST_MAX_PAIRS:
+        raise ValueError(f'chunk must be in 1..{HIST_MAX_PAIRS}')
+    device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
+    b = cfg.backbone
+    S, voxel_size, radius = b.num_stages, b.init_voxel_size, b.init_radius
+    hist_n = int(np.ceil(4 / 3 * np.pi * (radius / voxel_size + 1) ** 3))
+    totals = torch.zeros((S, hist_n), dtype=torch.int32, device=device)
+    hists = torch.empty((chunk, S, hist_n), dtype=torch.int32, device=device)
+    stop = torch.empty((1,), dtype=torch.int32, device=device)
+    lib = L.lib()
+    n, used = len(pairs), len(pairs)
+    with torch.cuda.device(device):
+        for base in range(0, n, chunk):
+            group = [pairs[i] for i in range(base, min(n, base + chunk))]
+            B = len(group)
+            points, lengths, _, _, _ = augment_stacked(group, cfg, seed, CALIBRATION_ITERATION, device, pair_base=base)
+            data = precompute_data_stack_mode(points, torch.LongTensor(lengths), S, voxel_size, radius, [hist_n] * S)
+            tables = data['neighbors']
+            ptrs = (ctypes.c_void_p * S)(*[t.data_ptr() for t in tables])
+            widths = np.array([t.shape[1] for t in tables], dtype=np.int64)
+            rows = np.array(data['lengths_host'], dtype=np.int64).reshape(S, 2 * B)
+            L.check(lib.geob200_neighbor_histogram_batched(ptrs, widths.ctypes.data, rows.ctypes.data, S, B, hist_n, sample_threshold,
+                                                           hists.data_ptr(), totals.data_ptr(), stop.data_ptr(), L.stream_ptr()),
+                    'neighbor_histogram_batched')
+            p = int(stop.item())
+            if p >= 0:
+                used = base + p + 1
+                break
+    cum_sum = np.cumsum(totals.cpu().numpy().T, axis=0)
+    return np.sum(cum_sum < (keep_ratio * cum_sum[hist_n - 1, :]), axis=0), used

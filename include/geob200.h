@@ -51,6 +51,36 @@ int geob200_radius_search(const float* q_points, int64_t n_query, const float* s
 int geob200_neighbor_histogram(const int64_t* neighbors, int64_t n_rows, int64_t width, int64_t n_support, int64_t hist_n,
                                int32_t* hist, void* stream);
 
+/* calibrate_neighbors_stack_mode over a batch of `batch` pairs at once (two launches).  neighbors: host array of num_stages device
+ * pointers to the batch's stacked neighbour tables (stage s: (sum of cloud_rows[s], widths[s]) int64, sentinel = its row count);
+ * cloud_rows: host (num_stages, 2 * batch) rows per cloud, clouds ordered [ref_0..ref_{B-1}, src_0..src_{B-1}].  hists (device
+ * int32 (batch, num_stages, hist_n)) receives one histogram per (pair, stage).  Then, in pair order, the pairs' row totals are
+ * added to the running totals of earlier calls (device int32 (num_stages, hist_n), in / out); the first pair after which every
+ * stage's total exceeds sample_threshold -- the reference's early exit -- is written to *stop (device int32, -1 if none), and
+ * totals receive the histograms of the pairs up to and including it (all pairs if none). */
+#define GEOB200_HIST_MAX_PAIRS 32
+int geob200_neighbor_histogram_batched(const int64_t* const* neighbors, const int64_t* widths, const int64_t* cloud_rows,
+                                       int64_t num_stages, int64_t batch, int64_t hist_n, int64_t sample_threshold, int32_t* hists,
+                                       int32_t* totals, int32_t* stop, void* stream);
+
+/* ---- kernel-point dispositions (reference modules/kpconv/kernel_points.py; csrc/kernel_points.cu) ----------------------------- */
+
+/* kernel_point_optimization_debug(1.0, num_points, num_kernels, 3, fixed='center', ratio) in fp64, one launch of one CTA: the
+ * potential descent of num_kernels candidates with the centre fixed and the reference's global stopping test, then the rescale to
+ * a mean radius of `ratio`.  init: device (num_kernels * num_points, 3) fp64 initial points (the accepted draws, centre rows
+ * included and zeroed), or NULL to draw them from Philox keyed by seed (the draw layout is documented in kernel_points.cu).
+ * points: device (num_kernels, num_points, 3) fp64 out.  info: device int32 [2] = {the candidate load_kernels picks, the
+ * iteration the descent stopped at (10000 if it never did)}. */
+#define GEOB200_KP_MAX_POINTS 30
+int geob200_kernel_point_optimize(const double* init, int64_t num_kernels, int64_t num_points, uint64_t seed, double ratio,
+                                  double* points, int32_t* info, void* stream);
+
+/* load_kernels' per-instance buffers: layer l gets (fp32(disposition) + N(0, 0.01^2) noise) * radii[l], rotated about z by
+ * theta ~ U(0, 2 pi), as fp32 (num_layers, num_points, 3) in out.  Draws are keyed by (seed, layer_ids[l]).  disposition: device
+ * (num_points, 3) fp64; radii: device fp64 [num_layers]; layer_ids: device int64 [num_layers]. */
+int geob200_kernel_point_instances(const double* disposition, int64_t num_points, const double* radii, const int64_t* layer_ids,
+                                   int64_t num_layers, uint64_t seed, float* out, void* stream);
+
 /* ---- KPConv-FPN backbone --------------------------------------------------------------------------------- */
 
 /* KPConv.forward (reference geotransformer/modules/kpconv/kpconv.py:79-122), fused gather -> kernel-point
