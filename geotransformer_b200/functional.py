@@ -2579,3 +2579,58 @@ def modelnet_benchmark_pairs_batched(shapes, lengths, indices, num_points, keep_
                                                          out.data_ptr(), origin.data_ptr(), T.data_ptr(), ws.data_ptr(), ws.numel(),
                                                          L.stream_ptr()), 'modelnet_benchmark_pairs_batched')
     return out, [m] * (2 * B), T, origin
+
+
+VOXEL_MAX_CLOUDS = 64
+_VOXEL_ERRORS = {1: 'a coordinate is NaN or infinite',
+                 2: 'voxel_size is too small (voxel_size * INT_MAX < the extent of the bounding box, as Open3D checks)',
+                 3: 'an axis spans 2^21 voxels or more (the limit of the packed voxel key): use a larger voxel_size'}
+
+
+def voxel_down_sample_batched(points, lengths, voxel_size, normals=None):
+    """Open3D's ``PointCloud::VoxelDownSample`` of up to 64 stacked clouds in one call (``geob200_voxel_down_sample``), in double.
+    ``points``: CUDA (sum(lengths), 3) float64, or float32 (widened exactly, as Open3D's ``Vector3dVector`` does); ``lengths``: B
+    host ints (empty clouds allowed); ``normals``: optional, like ``points``.  Each voxel's value is the input-order double sum of
+    its points divided by their count (normals likewise, not renormalised), in the iteration order of Open3D's voxel map (DESIGN.md
+    section 8a).  Returns (points (M, 3) float64, lengths (B,) int64[, normals (M, 3) float64]) on the device; M and the error
+    status are read back in one 8 (B + 1) byte copy.  Raises RuntimeError on a non-finite coordinate, a voxel size Open3D calls too
+    small, or an axis of 2^21 voxels or more."""
+    lengths = [int(v) for v in lengths]
+    B = len(lengths)
+    if not 1 <= B <= VOXEL_MAX_CLOUDS:
+        raise RuntimeError(f'voxel_down_sample_batched: 1..{VOXEL_MAX_CLOUDS} clouds per call, got {B}')
+    voxel_size = float(voxel_size)
+    if not (voxel_size > 0 and math.isfinite(voxel_size)):
+        raise RuntimeError(f'voxel_down_sample_batched: voxel_size must be positive and finite, got {voxel_size}')
+
+    def _as_f64(t, name):
+        if not isinstance(t, torch.Tensor) or not t.is_cuda:
+            raise RuntimeError(f'{name} must be a CUDA tensor (geotransformer_b200 has no CPU path)')
+        if t.dtype not in (torch.float32, torch.float64):
+            raise RuntimeError(f'{name} must be float32 or float64, got {t.dtype}')
+        t = t.to(torch.float64).contiguous()
+        if t.dim() != 2 or t.shape[1] != 3 or t.shape[0] != sum(lengths):
+            raise RuntimeError(f'voxel_down_sample_batched: {name} must be (sum(lengths), 3), got {tuple(t.shape)}')
+        return t
+
+    pts = _as_f64(points, 'points')
+    nrm = None if normals is None else _as_f64(normals, 'normals')
+    if nrm is not None and nrm.device != pts.device:
+        raise RuntimeError('voxel_down_sample_batched: points and normals must be on one device')
+    n, dev = pts.shape[0], pts.device
+    lib = L.lib()
+    ws = L.workspace(lib.geob200_voxel_down_sample_workspace_bytes(n, B), dev, tag='voxel')
+    out = torch.empty((n, 3), dtype=torch.float64, device=dev)
+    out_n = torch.empty((n, 3), dtype=torch.float64, device=dev) if nrm is not None else None
+    out_len = torch.empty((B + 1,), dtype=_i64, device=dev)
+    L.check(lib.geob200_voxel_down_sample(pts.data_ptr(), L.ptr(nrm), n, _host_i64(lengths), B, voxel_size, out.data_ptr(),
+                                          L.ptr(out_n), out_len.data_ptr(), ws.data_ptr(), ws.numel(), L.stream_ptr()),
+            'voxel_down_sample_batched')
+    host = out_len.cpu().tolist()
+    if host[B] != 0:
+        raise RuntimeError(f'voxel_down_sample_batched: {_VOXEL_ERRORS.get(host[B], f"error {host[B]}")}')
+    m = sum(host[:B])
+    res = (out[:m].clone(), out_len[:B])
+    if nrm is not None:
+        res = res + (out_n[:m].clone(),)
+    return res

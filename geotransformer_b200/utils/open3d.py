@@ -1,5 +1,8 @@
-"""Correspondence RANSAC and feature-matching RANSAC with the reference's interface (geotransformer/utils/open3d.py:133-198), on
-the device, without Open3D.
+"""Voxel downsampling, correspondence RANSAC and feature-matching RANSAC with the reference's interface
+(geotransformer/utils/open3d.py:57-65 and 133-198), on the device, without Open3D.
+
+``voxel_downsample`` follows Open3D's ``PointCloud::VoxelDownSample`` in double, values and order (DESIGN.md section 8a); it is
+pinned to a restatement of that function, not checked against an Open3D build.
 
 The estimates follow Open3D's registration_ransac_based_on_correspondence and (0.11's) registration_ransac_based_on_feature_matching
 as the reference calls them; the sampler, the tie rule and the fp32 scoring differ from Open3D (DESIGN.md section 3b), so the
@@ -17,6 +20,33 @@ def _points(x, name, device):
             raise RuntimeError(f'{name} must be a numpy array or a CUDA tensor (geotransformer_b200 has no CPU path)')
         return x.detach().to(torch.float32).contiguous()
     return torch.from_numpy(np.ascontiguousarray(x, dtype=np.float32)).to(device)
+
+
+def voxel_downsample(points, voxel_size, normals=None):
+    r"""Open3D's ``voxel_down_sample(voxel_size)`` of one cloud, with the reference's signature.
+
+    numpy input gives float64 numpy arrays, as ``np.asarray(pcd.points)`` does; a CUDA tensor gives float64 CUDA tensors.  float32
+    input is widened exactly, as ``Vector3dVector`` does.  Returns ``points``, or ``(points, normals)`` when normals are given
+    (averaged, not renormalised, as Open3D)."""
+    on_device = isinstance(points, torch.Tensor)
+    if on_device and not points.is_cuda:
+        raise RuntimeError('points must be a numpy array or a CUDA tensor (geotransformer_b200 has no CPU path)')
+    device = points.device if on_device else torch.device('cuda', torch.cuda.current_device())
+
+    def _f64(x, name):
+        if isinstance(x, torch.Tensor):
+            if not x.is_cuda:
+                raise RuntimeError(f'{name} must be a numpy array or a CUDA tensor (geotransformer_b200 has no CPU path)')
+            return x.detach().to(device=device, dtype=torch.float64).reshape(-1, 3).contiguous()
+        return torch.from_numpy(np.ascontiguousarray(x, dtype=np.float64).reshape(-1, 3)).to(device)
+
+    pts = _f64(points, 'points')
+    nrm = None if normals is None else _f64(normals, 'normals')
+    res = GF.voxel_down_sample_batched(pts, [pts.shape[0]], voxel_size, normals=nrm)
+    out = (res[0],) if normals is None else (res[0], res[2])
+    if not on_device:
+        out = tuple(x.cpu().numpy() for x in out)
+    return out[0] if normals is None else out
 
 
 def registration_with_ransac_from_correspondences(src_points, ref_points, correspondences=None, distance_threshold=0.05, ransac_n=3,

@@ -63,6 +63,24 @@ int geob200_neighbor_histogram_batched(const int64_t* const* neighbors, const in
                                        int64_t num_stages, int64_t batch, int64_t hist_n, int64_t sample_threshold, int32_t* hists,
                                        int32_t* totals, int32_t* stop, void* stream);
 
+/* ---- voxel downsampling (Open3D PointCloud::VoxelDownSample; csrc/voxel.cu) ------------------------------------------------- */
+
+/* Open3D's voxel downsampling of `batch` stacked clouds (lengths_h host int64[batch], empty clouds allowed), in double: voxel
+ * averages of the points (and of the normals if given, not renormalised) summed in input order, in the iteration order of
+ * Open3D's std::unordered_map keyed by hash_eigen (the contract is in DESIGN.md section 8a).  points / normals: device
+ * (n_points, 3) fp64; out_points / out_normals: device fp64 with room for n_points rows (normals and out_normals both given or
+ * both NULL); each cloud's voxels start at the sum of the earlier clouds' voxel counts.  out_lengths: device int64[batch + 1]
+ * receives the per-cloud voxel counts and then the status word: 0, or a GEOB200_VOXEL_* code for an error found on the device
+ * (every count is then 0 and no output is written).  Arguments are checked before any launch; no host synchronisation. */
+#define GEOB200_VOXEL_MAX_CLOUDS 64
+#define GEOB200_VOXEL_NONFINITE 1   /* a coordinate is NaN or infinite */
+#define GEOB200_VOXEL_TOO_SMALL 2   /* voxel * INT_MAX < the largest extent of the padded bounding box (Open3D's check) */
+#define GEOB200_VOXEL_AXIS_LIMIT 3  /* an axis spans 2^21 voxels or more (the packed voxel key holds 21 bits per axis) */
+size_t geob200_voxel_down_sample_workspace_bytes(int64_t n_points, int64_t batch);
+int geob200_voxel_down_sample(const double* points, const double* normals, int64_t n_points, const int64_t* lengths_h, int64_t batch,
+                              double voxel, double* out_points, double* out_normals, int64_t* out_lengths, void* workspace,
+                              size_t workspace_bytes, void* stream);
+
 /* ---- kernel-point dispositions (reference modules/kpconv/kernel_points.py; csrc/kernel_points.cu) ----------------------------- */
 
 /* kernel_point_optimization_debug(1.0, num_points, num_kernels, 3, fixed='center', ratio) in fp64, one launch of one CTA: the
