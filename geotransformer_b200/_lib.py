@@ -164,6 +164,7 @@ _sig('geob200_modelnet_pairs_batched_workspace_bytes', SZ, I64)
 _sig('geob200_modelnet_pairs_batched', c_int, P, P, I64, I64, D, D, D, D, ctypes.c_uint64, ctypes.c_uint64, I64, P, P, P, P, P, SZ, P)
 _sig('geob200_modelnet_benchmark_pairs_batched_workspace_bytes', SZ, I64, I64)
 _sig('geob200_modelnet_benchmark_pairs_batched', c_int, P, P, P, I64, I64, D, D, D, D, P, P, P, P, SZ, P)
+_sig('geob200_rotated_pairs_batched', c_int, P, c_int, P, P, I64, P, P, P, P, P)
 
 
 def lib():

@@ -13,6 +13,8 @@
 // ModelNet's validation and test pairs (deterministic=True) are the exception: the reference seeds numpy's global generator with
 // the pair's dataset index, so modelnet_benchmark_kernel draws from numpy's own legacy stream (numpy_random.cuh) in the reference's
 // order and reproduces its pairs bit for bit (oracle/modelnet_benchmark_oracle.py).
+// The rotated 3DMatch / 3DLoMatch benchmark follows the same convention: the pair of dataset index i draws its two rotations from
+// np.random.seed(i) (rotated_draws_kernel; oracle/rotated_oracle.py restates it in numpy).
 #include "common.cuh"
 #include "compaction.cuh"
 #include "geob200.h"
@@ -535,11 +537,63 @@ __device__ __forceinline__ void quat_compose(const double (&p)[4], const double 
                      __dadd_rn(__dadd_rn(__dmul_rn(p[0], q[0]), __dmul_rn(p[1], q[1])), __dmul_rn(p[2], q[2])));
 }
 
+// sin x and cos x correctly rounded for |x| <= 1.6 (the half-angles of Euler angles within +-pi, with margin): Horner's form of the
+// Taylor series in double-double, sin x = x (1 - x^2 / (2 3) (1 - x^2 / (4 5) (...))) and cos x = 1 - x^2 / (1 2) (1 - ...), 18
+// terms each (the first omitted term is below 2^-120 of the result), with every operation rounded explicitly (no contraction).
+// The double-double result is within about 2^-100 relative, so its rounding to double is the correctly rounded value unless the
+// exact value lies that close to a midpoint.  The device's sincos may be an ulp off; the host libm's (which scipy calls) is
+// correctly rounded except in rare near-tie cases.
+struct DD {
+    double hi, lo;
+};
+__device__ __forceinline__ DD dd_norm(double a, double b) {          // fast two-sum, |a| >= |b|
+    const double s = __dadd_rn(a, b);
+    return DD{s, __dsub_rn(b, __dsub_rn(s, a))};
+}
+__device__ __forceinline__ DD dd_mul(DD a, DD b) {
+    const double p = __dmul_rn(a.hi, b.hi);
+    const double e = __fma_rn(a.hi, b.hi, -p);
+    return dd_norm(p, __dadd_rn(e, __dadd_rn(__dmul_rn(a.hi, b.lo), __dmul_rn(a.lo, b.hi))));
+}
+__device__ __forceinline__ DD dd_div(DD a, double d) {               // a / d for an exact integer d
+    const double q = __ddiv_rn(a.hi, d);
+    const double r = __dadd_rn(__fma_rn(-q, d, a.hi), a.lo);
+    return dd_norm(q, __ddiv_rn(r, d));
+}
+__device__ __forceinline__ DD dd_one_minus(DD a) {                   // 1 - a
+    const double s = __dsub_rn(1.0, a.hi);
+    const double bb = __dsub_rn(s, 1.0);
+    const double e = __dadd_rn(__dsub_rn(1.0, __dsub_rn(s, bb)), __dsub_rn(-a.hi, bb));      // two-sum error of 1 + (-a.hi)
+    return dd_norm(s, __dsub_rn(e, a.lo));
+}
+__device__ __forceinline__ void sincos_cr(double x, double* s, double* c) {
+    const double p = __dmul_rn(x, x);
+    const DD x2 = dd_norm(p, __fma_rn(x, x, -p));
+    DD ts{1.0, 0.0}, tc{1.0, 0.0};
+#pragma unroll 1
+    for (int k = 18; k >= 1; --k) {
+        ts = dd_one_minus(dd_div(dd_mul(ts, x2), (double)((2 * k) * (2 * k + 1))));
+        tc = dd_one_minus(dd_div(dd_mul(tc, x2), (double)((2 * k - 1) * (2 * k))));
+    }
+    const double sp = __dmul_rn(x, ts.hi);
+    *s = __dadd_rn(sp, __dadd_rn(__fma_rn(x, ts.hi, -sp), __dmul_rn(x, ts.lo)));
+    *c = __dadd_rn(tc.hi, tc.lo);
+}
+
+// CR: the half-angles' sin and cos correctly rounded (sincos_cr; the rotated 3DMatch pairs), else the device's sincos (the ModelNet
+// pairs, unchanged)
+template <bool CR = false>
 __device__ __forceinline__ void euler_zyx_scipy(double a, double b, double c, double (&R)[9]) {
     double qz[4] = {0.0, 0.0, 0.0, 0.0}, qy[4] = {0.0, 0.0, 0.0, 0.0}, qx[4] = {0.0, 0.0, 0.0, 0.0}, t[4], q[4];
-    sincos(__dmul_rn(a, 0.5), &qz[2], &qz[3]);
-    sincos(__dmul_rn(b, 0.5), &qy[1], &qy[3]);
-    sincos(__dmul_rn(c, 0.5), &qx[0], &qx[3]);
+    if constexpr (CR) {
+        sincos_cr(__dmul_rn(a, 0.5), &qz[2], &qz[3]);
+        sincos_cr(__dmul_rn(b, 0.5), &qy[1], &qy[3]);
+        sincos_cr(__dmul_rn(c, 0.5), &qx[0], &qx[3]);
+    } else {
+        sincos(__dmul_rn(a, 0.5), &qz[2], &qz[3]);
+        sincos(__dmul_rn(b, 0.5), &qy[1], &qy[3]);
+        sincos(__dmul_rn(c, 0.5), &qx[0], &qx[3]);
+    }
     quat_compose(qy, qz, t);
     quat_compose(qx, t, q);
     const double x2 = __dmul_rn(q[0], q[0]), y2 = __dmul_rn(q[1], q[1]), z2 = __dmul_rn(q[2], q[2]), w2 = __dmul_rn(q[3], q[3]);
@@ -734,6 +788,99 @@ __global__ void __launch_bounds__(MNB_THREADS) modelnet_benchmark_kernel(
     }
 }
 
+// ---- Rotated 3DMatch / 3DLoMatch benchmark pairs ------------------------------------------------------------------------------
+
+constexpr int ROT_MAX_PAIRS = 64;          // pairs per launch; the entry point splits larger calls
+constexpr int ROT_THREADS = 256;
+
+// One launch's pairs, by value: its clouds are ref clouds 0 .. n-1 then src clouds 0 .. n-1, rows start[c] .. start[c+1] - 1 of the
+// launch; the ref rows begin at row ref_row0 of the call's stack and the src rows at src_row0.
+struct RotLaunch {
+    int n, pair0;
+    long long ref_row0, src_row0;
+    long long start[2 * ROT_MAX_PAIRS + 1];
+    uint32_t index[ROT_MAX_PAIRS];
+};
+
+// random_sample_rotation_v2: axis = rand(3) - 0.5; axis = axis / norm(axis) + 1e-8; theta = pi rand(); R = from_euler('zyx',
+// axis theta).  numpy's norm of three doubles is sqrt(dot), and OpenBLAS's dot is the FMA chain below.
+__device__ __forceinline__ void rotation_v2(LegacyRandom& rng, double (&R)[9]) {
+    double a[3];
+#pragma unroll
+    for (int i = 0; i < 3; ++i) a[i] = __dsub_rn(rng.next_double(), 0.5);
+    const double norm = __dsqrt_rn(__fma_rn(a[2], a[2], __fma_rn(a[1], a[1], __dmul_rn(a[0], a[0]))));
+    const double theta = __dmul_rn(M_PI, rng.next_double());
+    double e[3];
+#pragma unroll
+    for (int i = 0; i < 3; ++i) e[i] = __dmul_rn(__dadd_rn(__ddiv_rn(a[i], norm), 1e-8), theta);
+    euler_zyx_scipy<true>(e[0], e[1], e[2], R);
+}
+
+// numpy's 3 x 3 products in OpenBLAS's order: C = A B with A B[i, j] = fma(a2, b2, fma(a1, b1, a0 b0)) over row i of A and column
+// j of B (B_T: B is given transposed), and A v = fma(a2, v2, fma(a0, v0, a1 v1)) (dgemv)
+__device__ __forceinline__ double dot3_gemm(double a0, double a1, double a2, double b0, double b1, double b2) {
+    return __fma_rn(a2, b2, __fma_rn(a1, b1, __dmul_rn(a0, b0)));
+}
+
+// One warp per pair, grid (n): draws R_ref then R_src from np.random.seed(index) and composes the pair's transform in fp64:
+// rotation = R_ref rotation R_src^T, translation = R_ref translation; rounds it to fp32 once.
+__global__ void __launch_bounds__(32) rotated_draws_kernel(RotLaunch Lc, const double* __restrict__ T_in, float* __restrict__ T_out,
+                                                           double* __restrict__ rot) {
+    __shared__ uint32_t mt[MT_N];
+    const int q = blockIdx.x, p = Lc.pair0 + q;
+    LegacyRandom rng{mt, 0, false, 0.0};
+    rng.seed(Lc.index[q]);
+    double Rr[9], Rs[9];
+    rotation_v2(rng, Rr);
+    rotation_v2(rng, Rs);
+    if (threadIdx.x != 0) return;
+    const double* T = T_in + 16ll * p;
+    double A[9], t[3];
+#pragma unroll
+    for (int i = 0; i < 3; ++i) {
+#pragma unroll
+        for (int j = 0; j < 3; ++j) A[3 * i + j] = dot3_gemm(Rr[3 * i], Rr[3 * i + 1], Rr[3 * i + 2], T[j], T[4 + j], T[8 + j]);
+        t[i] = __fma_rn(Rr[3 * i + 2], T[11], __fma_rn(Rr[3 * i], T[3], __dmul_rn(Rr[3 * i + 1], T[7])));
+    }
+    float* o = T_out + 16ll * p;
+#pragma unroll
+    for (int i = 0; i < 3; ++i) {
+#pragma unroll
+        for (int j = 0; j < 3; ++j) o[4 * i + j] = __double2float_rn(dot3_gemm(A[3 * i], A[3 * i + 1], A[3 * i + 2], Rs[3 * j], Rs[3 * j + 1], Rs[3 * j + 2]));
+        o[4 * i + 3] = __double2float_rn(t[i]);
+        o[12 + i] = 0.0f;
+    }
+    o[15] = 1.0f;
+#pragma unroll
+    for (int i = 0; i < 9; ++i) {
+        rot[18ll * p + i] = Rr[i];
+        rot[18ll * p + 9 + i] = Rs[i];
+    }
+}
+
+// One thread per row of the launch: p R^T in fp64 in numpy's (N, 3) x (3, 3) order, fma(z, R[i,2], fma(y, R[i,1], x R[i,0])), rounded
+// to fp32 once.
+// Real: the clouds' type as the dataset files hold them (fp32 widens exactly).
+template <typename Real>
+__global__ void __launch_bounds__(ROT_THREADS) rotated_points_kernel(RotLaunch Lc, const Real* __restrict__ pts, const double* __restrict__ rot,
+                                                                     float* __restrict__ out) {
+    const long long r = (long long)blockIdx.x * ROT_THREADS + threadIdx.x;
+    const int nc = 2 * Lc.n;
+    if (r >= Lc.start[nc]) return;
+    int lo = 0, hi = nc - 1;                 // the cloud c with start[c] <= r < start[c + 1]
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (Lc.start[mid] <= r) lo = mid;
+        else hi = mid - 1;
+    }
+    const int c = lo, src = c >= Lc.n;
+    const long long row = src ? Lc.src_row0 + (r - Lc.start[Lc.n]) : Lc.ref_row0 + r;
+    const double* R = rot + 18ll * (Lc.pair0 + c - (src ? Lc.n : 0)) + 9 * src;
+    const double x = (double)pts[3 * row], y = (double)pts[3 * row + 1], z = (double)pts[3 * row + 2];
+#pragma unroll
+    for (int i = 0; i < 3; ++i) out[3 * row + i] = __double2float_rn(dot3_gemm(x, y, z, R[3 * i], R[3 * i + 1], R[3 * i + 2]));
+}
+
 static int next_pow2(int n) {
     int p = 1;
     while (p < n) p <<= 1;
@@ -904,6 +1051,59 @@ int geob200_modelnet_benchmark_pairs_batched(const float* shapes, const int64_t*
         modelnet_benchmark_kernel<<<n, MNB_THREADS, smem, st>>>(shapes, table, B, p0, P, jit, out_points, origin, out_transforms);
         GEOB_CHECK_LAUNCH();
         ++launches;
+    }
+    count_launches(launches);
+    return 0;
+}
+
+int geob200_rotated_pairs_batched(const void* points, int points_fp64, const int64_t* lengths_h, const int64_t* indices_h, int64_t n_pairs,
+                                  const double* transforms, float* out_points, float* out_transforms, double* rotations, void* stream) {
+    GEOB_REQUIRE(n_pairs > 0 && n_pairs <= (1ll << 30), "rotated_pairs_batched: n_pairs must be in 1..2^30");
+    GEOB_REQUIRE(points_fp64 == 0 || points_fp64 == 1, "rotated_pairs_batched: points_fp64 must be 0 or 1");
+    GEOB_REQUIRE(lengths_h != nullptr && indices_h != nullptr, "rotated_pairs_batched: null lengths or indices");
+    GEOB_REQUIRE(points != nullptr && transforms != nullptr && out_points != nullptr && out_transforms != nullptr && rotations != nullptr,
+                 "rotated_pairs_batched: null pointer");
+    long long rows = 0;
+    for (int64_t c = 0; c < 2 * n_pairs; ++c) {
+        GEOB_REQUIRE(lengths_h[c] > 0 && lengths_h[c] < (1ll << 31), "rotated_pairs_batched: cloud %lld has %lld points (1..2^31-1)",
+                     (long long)c, (long long)lengths_h[c]);
+        rows += lengths_h[c];
+        GEOB_REQUIRE(rows < (1ll << 31), "rotated_pairs_batched: more than 2^31-1 rows in all");
+    }
+    for (int64_t p = 0; p < n_pairs; ++p)
+        GEOB_REQUIRE(indices_h[p] >= 0 && indices_h[p] <= 0xFFFFFFFFll, "rotated_pairs_batched: index %lld of pair %lld is not in "
+                     "0..2^32-1", (long long)indices_h[p], (long long)p);
+    const int B = (int)n_pairs;
+    cudaStream_t st = (cudaStream_t)stream;
+    long long ref_row = 0, src_row = 0;
+    for (int p = 0; p < B; ++p) src_row += lengths_h[p];
+    int launches = 0;
+    for (int p0 = 0; p0 < B; p0 += ROT_MAX_PAIRS) {
+        RotLaunch Lc;
+        Lc.n = B - p0 < ROT_MAX_PAIRS ? B - p0 : ROT_MAX_PAIRS;
+        Lc.pair0 = p0;
+        Lc.ref_row0 = ref_row;
+        Lc.src_row0 = src_row;
+        long long s = 0;
+        for (int c = 0; c < 2 * Lc.n; ++c) {
+            Lc.start[c] = s;
+            s += lengths_h[c < Lc.n ? p0 + c : B + p0 + c - Lc.n];
+        }
+        Lc.start[2 * Lc.n] = s;
+        for (int q = 0; q < Lc.n; ++q) {
+            Lc.index[q] = (uint32_t)indices_h[p0 + q];
+            ref_row += lengths_h[p0 + q];
+            src_row += lengths_h[B + p0 + q];
+        }
+        rotated_draws_kernel<<<Lc.n, 32, 0, st>>>(Lc, transforms, out_transforms, rotations);
+        GEOB_CHECK_LAUNCH();
+        const unsigned grid = (unsigned)((s + ROT_THREADS - 1) / ROT_THREADS);
+        if (points_fp64)
+            rotated_points_kernel<<<grid, ROT_THREADS, 0, st>>>(Lc, (const double*)points, rotations, out_points);
+        else
+            rotated_points_kernel<<<grid, ROT_THREADS, 0, st>>>(Lc, (const float*)points, rotations, out_points);
+        GEOB_CHECK_LAUNCH();
+        launches += 2;
     }
     count_launches(launches);
     return 0;

@@ -3,6 +3,8 @@
     python -m geotransformer_b200.evaluate --config 3dmatch --benchmark 3DMatch --method lgr \\
         --features FEATURES --gt-root METADATA/benchmarks --registration-dir OUT [--num_corr 250,500,1000,2500,5000] [--verbose]
     python -m geotransformer_b200.evaluate --config kitti --method ransac --features FEATURES [--num_corr 5000]
+    python -m geotransformer_b200.evaluate --config 3dmatch --benchmark 3DMatch --method lgr --features FEATURES --protocol dgr \\
+        [--test-epoch E] [--num_corr 1000]
 
 It reads the ``.npz`` tree ``test.py`` (or ``RegistrationTester``) writes: 3DMatch ``<features>/<benchmark>/<scene>/<ref>_<src>.npz``,
 KITTI ``<features>/<seq>_<src>_<ref>.npz``, in the order ``eval.py`` visits them.  Per chunk of pairs the arrays are packed into one
@@ -12,6 +14,13 @@ registration error run there for the whole chunk, and one copy brings the per-pa
 reference's, on the host.  ``--gt-root`` is the directory holding ``<benchmark>/<scene>/gt.log`` and ``gt.info``; with
 ``--registration-dir`` each scene's estimates go to ``<dir>/<benchmark>/<scene>/est.log`` (``<dir>/num_corr_<k>/...`` per setting
 of a sweep).
+
+``--protocol dgr`` (3dmatch) is the experiments' ``eval_dgr.py`` instead: a pair is accepted when its RRE and RTE against the
+npz ``transform`` are under ``cfg.eval.rre_threshold`` / ``rte_threshold``, so it needs no ``--gt-root`` and writes no est.log.
+It is the protocol that can score the rotated benchmark (``test --rotated``), whose transforms are not gt.log's.  Its meters and
+lines are eval_dgr's, quirks included: a scene's RRE / RTE average its accepted pairs only and are NaN without one, the NaN reaches
+``mean_RRE`` / ``mean_RTE``, and the summary opens with ``Epoch {--test-epoch}``.  It reads the same ``<features>/<benchmark>/<scene>``
+layout as ``gtlog``.  Scoring a rotated tree with ``gtlog`` is meaningless: gt.log holds the un-rotated fragments' transforms.
 
 A sweep ``--num_corr 250,500`` orders each pair's correspondences once and selects once per setting; its results equal separate
 runs.  Where this differs from ``eval.py`` (DESIGN.md section 3b): ``--num_corr`` works for 3DMatch too (the reference's 3DMatch
@@ -122,7 +131,8 @@ class _Run:
         self.label, self.log, self.lines, self.pairs, self.estimates = label, log, [], [], []
         self.coarse = _meters(['precision', 'PMR>0', 'PMR>=0.1', 'PMR>=0.3', 'PMR>=0.5'])
         self.fine = _meters(['recall', 'inlier_ratio', 'overlap'])
-        self.reg = _meters(['recall', 'rre', 'rte', 'mean_rre', 'mean_rte', 'median_rre', 'median_rte'])
+        self.reg = _meters(['recall', 'rre', 'rte', 'mean_rre', 'mean_rte', 'median_rre', 'median_rte', 'overall_recall', 'overall_rre',
+                            'overall_rte'])
         self.scene_coarse, self.scene_fine, self.scene_reg = {}, {}, {}
 
     def emit(self, level, message):
@@ -131,13 +141,18 @@ class _Run:
             self.log(level, message if self.label is None else f'[num_corr={self.label}] {message}')
 
 
-def _load(path, config, gt):
+def _load(path, config, gt, dgr=False):
     d = np.load(path)
     item = {k: d[k] for k in ('ref_points_c', 'src_points_c', 'ref_node_corr_indices', 'src_node_corr_indices', 'ref_corr_points',
                               'src_corr_points', 'corr_scores', 'gt_node_corr_indices', 'transform', 'estimated_transform')}
     item['overlap'] = d['overlap'] if 'overlap' in d.files else np.float32('nan')
     ids = _ids(path)
-    if config == '3dmatch':
+    if config == '3dmatch' and dgr:                     # --protocol dgr: scored against the npz transform, gt.log is not read
+        item['ids'] = ids
+        item['has_cov'] = False
+        item['reg_gt'] = item['transform']
+        item['cov'] = np.zeros((6, 6), np.float32)
+    elif config == '3dmatch':
         item['ids'] = ids                                 # ref, src
         gt_indices, gt_logs, gt_infos = gt
         index = gt_indices[ids[0], ids[1]]
@@ -152,9 +167,9 @@ def _load(path, config, gt):
     return item
 
 
-def _device_rows(items, cfg, method, settings, first_pair, device):
+def _device_rows(items, cfg, method, settings, first_pair, device, rre_rte=False):
     """All device stages of a chunk; one (B, 3 + 24 * settings) float64 host array: sparse eval, then per setting the correspondence
-    metrics (4), the estimate (16) and the registration error (4)."""
+    metrics (4), the estimate (16) and the registration error (4).  rre_rte: accept by RRE / RTE for 3dmatch too (--protocol dgr)."""
     f32 = np.float32
     ref, cnt = _ragged([np.asarray(it['ref_corr_points'], f32).reshape(-1, 3) for it in items], (3,), f32)
     src, _ = _ragged([np.asarray(it['src_corr_points'], f32).reshape(-1, 3) for it in items], (3,), f32)
@@ -184,7 +199,7 @@ def _device_rows(items, cfg, method, settings, first_pair, device):
             T = GF.weighted_procrustes_counts(s, r, w, c).reshape(B, 16)
         else:
             raise ValueError(f'Unsupported registration method: {method}.')
-        if cfg.name == '3dmatch':
+        if cfg.name == '3dmatch' and not rre_rte:
             err = GF.registration_error_batched(reg_T, T, covariances=cov, has_covariance=has_cov, rmse_threshold=cfg.eval.rmse_threshold)
         else:
             err = GF.registration_error_batched(reg_T, T, rre_threshold=cfg.eval.rre_threshold, rte_threshold=cfg.eval.rte_threshold)
@@ -256,6 +271,72 @@ def _scene_end_3dmatch(run, scene_name, scene_abbr):
         r['recall'], r['mean_rre'], r['mean_rte'], r['median_rre'], r['median_rte']))
 
 
+def _pair_dgr(run, cfg, scene_abbr, item, v):
+    """eval_dgr.py's per-pair meters and line: every pair is scored by RRE / RTE against the npz transform"""
+    ref_frame, src_frame = item['ids']
+    c = v['precision']
+    sm = run.scene_meters
+    sm['precision'].update(c)
+    for name, ok in (('PMR>0', c > 0), ('PMR>=0.1', c >= 0.1), ('PMR>=0.3', c >= 0.3), ('PMR>=0.5', c >= 0.5)):
+        sm[name].update(float(ok))
+    sm['inlier_ratio'].update(v['inlier_ratio'])
+    sm['overlap'].update(v['overlap'])
+    sm['fmr'].update(float(v['inlier_ratio'] >= cfg.eval.inlier_ratio_threshold))
+    if v['accepted']:
+        for name in ('rre', 'rte'):
+            sm[name].update(v[name])
+            run.reg[f'overall_{name}'].update(v[name])
+    sm['rr'].update(float(v['accepted']))
+    run.reg['overall_recall'].update(float(v['accepted']))
+    return ('{}, id0: {}, id1: {}, OV: {:.3f}, c_PIR: {:.3f}, f_IR: {:.3f}, f_OV: {:.3f}, f_RS: {:.3f}, f_NU: {}, r_RRE: {:.3f}, '
+            'r_RTE: {:.3f}'.format(scene_abbr, ref_frame, src_frame, item['overlap'], c, v['inlier_ratio'], v['overlap'], v['residual'],
+                                   v['num_corr'], v['rre'], v['rte']))
+
+
+def _scene_end_dgr(run, scene_name, scene_abbr):
+    sm = run.scene_meters
+    c = {k: sm[k].mean() for k in ('precision', 'PMR>0', 'PMR>=0.1', 'PMR>=0.3', 'PMR>=0.5')}
+    for k, val in c.items():
+        run.coarse[k].update(val)
+    run.scene_coarse[scene_abbr] = c
+    f = {'recall': sm['fmr'].mean(), 'inlier_ratio': sm['inlier_ratio'].mean(), 'overlap': sm['overlap'].mean()}
+    for k, val in f.items():
+        run.fine[k].update(val)
+    run.scene_fine[scene_abbr] = {'recall': f['recall'], 'inlier_ratio': f['inlier_ratio']}
+    r = {'recall': sm['rr'].mean(), 'rre': sm['rre'].mean(), 'rte': sm['rte'].mean()}
+    for k, val in r.items():
+        run.reg[k].update(val)
+    run.scene_reg[scene_abbr] = r
+    run.emit(INFO, f'Scene_name: {scene_name}')
+    run.emit(INFO, '  Correspondence, , c_PIR: {:.3f}, c_PMR>0: {:.3f}, c_PMR>=0.1: {:.3f}, c_PMR>=0.3: {:.3f}, c_PMR>=0.5: {:.3f}, '
+                   'f_FMR: {:.3f}, f_IR: {:.3f}, f_OV: {:.3f}'.format(c['precision'], c['PMR>0'], c['PMR>=0.1'], c['PMR>=0.3'],
+                                                                      c['PMR>=0.5'], f['recall'], f['inlier_ratio'], f['overlap']))
+    run.emit(INFO, '  Registration, RR: {:.3f}, RRE: {:.3f}, RTE: {:.3f}'.format(r['recall'], r['rre'], r['rte']))
+
+
+def _final_dgr(run, test_epoch):
+    """eval_dgr.py's summary, its trailing ', ' included"""
+    run.emit(CRITICAL, 'Epoch {}'.format(test_epoch))
+    coarse = {k: m.mean() for k, m in run.coarse.items()}
+    fine = {'recall': run.fine['recall'].mean(), 'inlier_ratio': run.fine['inlier_ratio'].mean(),
+            'overlap': run.fine['overlap'].mean(), 'std': run.fine['recall'].std()}
+    run.emit(CRITICAL, _pmr('  Coarse Matching, ', coarse))
+    for abbr, m in run.scene_coarse.items():
+        run.emit(CRITICAL, _pmr(f'    {abbr}', m))
+    run.emit(CRITICAL, '  Fine Matching, FMR: {:.3f}, IR: {:.3f}, OV: {:.3f}, std: {:.3f}'.format(
+        fine['recall'], fine['inlier_ratio'], fine['overlap'], fine['std']))
+    for abbr, m in run.scene_fine.items():
+        run.emit(CRITICAL, '    {}, FMR: {:.3f}, IR: {:.3f}'.format(abbr, m['recall'], m['inlier_ratio']))
+    reg = {'recall': run.reg['overall_recall'].mean(), 'rre': run.reg['overall_rre'].mean(), 'rte': run.reg['overall_rte'].mean(),
+           'mean_recall': run.reg['recall'].mean(), 'mean_rre': run.reg['rre'].mean(), 'mean_rte': run.reg['rte'].mean()}
+    run.emit(CRITICAL, '  Registration, RR: {:.3f}, RRE: {:.3f}, RTE: {:.3f}, mean_RR: {:.3f}, mean_RRE: {:.3f}, mean_RTE: {:.3f}, '
+             .format(*reg.values()))
+    for abbr, m in run.scene_reg.items():
+        run.emit(CRITICAL, '    {}, RR: {:.3f}, RRE: {:.3f}, RTE: {:.3f}'.format(abbr, m['recall'], m['rre'], m['rte']))
+    return {'coarse': coarse, 'fine': fine, 'registration': reg, 'scenes': {'coarse': run.scene_coarse, 'fine': run.scene_fine,
+                                                                            'registration': run.scene_reg}}
+
+
 def _pmr(prefix, m):
     return ('{}, PIR: {:.3f}, PMR>0: {:.3f}, PMR>=0.1: {:.3f}, PMR>=0.3: {:.3f}, PMR>=0.5: {:.3f}'
             .format(prefix, m['precision'], m['PMR>0'], m['PMR>=0.1'], m['PMR>=0.3'], m['PMR>=0.5']))
@@ -287,16 +368,24 @@ def _final(run, config):
 
 
 def evaluate(config, method, features, benchmark=None, gt_root=None, num_corr=None, registration_dir=None, verbose=False, chunk=64,
-             log=None, device=None):
+             log=None, device=None, protocol='gtlog', test_epoch=None):
     """Runs the evaluation; returns ``{setting: {'summary', 'lines', 'pairs'}}`` with one entry per --num_corr value (key None
-    without --num_corr).  ``lines`` are the (logging level, message) pairs eval.py logs; ``pairs`` the per-pair values in
-    evaluation order.  ``log(level, message)`` receives the lines as they are produced."""
+    without --num_corr).  ``lines`` are the (logging level, message) pairs eval.py (protocol 'gtlog') or eval_dgr.py (protocol
+    'dgr', 3dmatch only; ``test_epoch`` is printed in its Epoch line) logs; ``pairs`` the per-pair values in evaluation order.
+    ``log(level, message)`` receives the lines as they are produced."""
     if config not in ('3dmatch', 'kitti'):
         raise ValueError(f'unsupported config {config!r} (3dmatch or kitti)')
     if method not in ('lgr', 'ransac', 'svd'):
         raise ValueError(f'Unsupported registration method: {method}.')
-    if config == '3dmatch' and (benchmark not in ('3DMatch', '3DLoMatch') or gt_root is None):
-        raise ValueError('3dmatch needs --benchmark 3DMatch or 3DLoMatch and --gt-root')
+    if protocol not in ('gtlog', 'dgr'):
+        raise ValueError(f"protocol must be 'gtlog' or 'dgr', got {protocol!r}")
+    dgr = protocol == 'dgr'
+    if dgr and config != '3dmatch':
+        raise ValueError("--protocol dgr is a 3dmatch evaluation (KITTI's eval.py already scores by RRE / RTE)")
+    if dgr and registration_dir is not None:
+        raise ValueError('--protocol dgr writes no est.log: drop --registration-dir')
+    if config == '3dmatch' and (benchmark not in ('3DMatch', '3DLoMatch') or (gt_root is None and not dgr)):
+        raise ValueError('3dmatch needs --benchmark 3DMatch or 3DLoMatch, and --gt-root unless --protocol dgr')
     cfg = make_cfg(config)
     settings = parse_num_corr(num_corr) if not isinstance(num_corr, list) else num_corr
     device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
@@ -309,18 +398,22 @@ def evaluate(config, method, features, benchmark=None, gt_root=None, num_corr=No
         if config == '3dmatch':
             abbr = get_scene_abbr(scene_name)
             num_fragments = get_num_fragments(scene_name)
-            gt = get_gt_logs_and_infos(os.path.join(gt_root, benchmark, scene_name), num_fragments)
+            if not dgr:
+                gt = get_gt_logs_and_infos(os.path.join(gt_root, benchmark, scene_name), num_fragments)
             for run in runs:
                 run.scene_meters = _meters(['precision', 'PMR>0', 'PMR>=0.1', 'PMR>=0.3', 'PMR>=0.5', 'fmr', 'inlier_ratio', 'overlap',
                                             'rr', 'rre', 'rte'])
                 run.estimates = []
         for base in range(0, len(files), max(int(chunk), 1)):
-            items = [_load(f, config, gt) for f in files[base:base + max(int(chunk), 1)]]
-            rows = _device_rows(items, cfg, method, settings, pair_id, device)
+            items = [_load(f, config, gt, dgr) for f in files[base:base + max(int(chunk), 1)]]
+            rows = _device_rows(items, cfg, method, settings, pair_id, device, rre_rte=dgr)
             for i, item in enumerate(items):
                 for j, run in enumerate(runs):
                     v = _pair_values(rows[i], j, item, method)
-                    if config == '3dmatch':
+                    if dgr:
+                        msg = _pair_dgr(run, cfg, abbr, item, v)
+                        v.update(scene=scene_name, id0=item['ids'][0], id1=item['ids'][1])
+                    elif config == '3dmatch':
                         msg = _pair_3dmatch(run, cfg, abbr, item, v)
                         run.estimates.append({'test_pair': item['ids'], 'num_fragments': num_fragments,
                                               'transform': v['estimated_transform']})
@@ -331,13 +424,17 @@ def evaluate(config, method, features, benchmark=None, gt_root=None, num_corr=No
                     if verbose:
                         run.emit(INFO, msg)
             pair_id += len(items)
-        if config == '3dmatch':
+        if dgr:
+            for run in runs:
+                _scene_end_dgr(run, scene_name, abbr)
+        elif config == '3dmatch':
             for k, run in zip(settings, runs):
                 if registration_dir is not None:
                     sub = registration_dir if len(settings) == 1 else os.path.join(registration_dir, f'num_corr_{k}')
                     write_log_file(os.path.join(sub, benchmark, scene_name, 'est.log'), run.estimates)
                 _scene_end_3dmatch(run, scene_name, abbr)
-    return {k: {'summary': _final(run, config), 'lines': run.lines, 'pairs': run.pairs} for k, run in zip(settings, runs)}
+    return {k: {'summary': _final_dgr(run, test_epoch) if dgr else _final(run, config), 'lines': run.lines, 'pairs': run.pairs}
+            for k, run in zip(settings, runs)}
 
 
 def _pair_kitti(run, cfg, item, v, index, n_total):
@@ -366,7 +463,10 @@ def make_parser():
     parser.add_argument('--method', choices=['lgr', 'ransac', 'svd'], required=True, help='registration method')
     parser.add_argument('--num_corr', default=None, help='number of correspondences for registration: one value or a comma list')
     parser.add_argument('--features', required=True, help='the tester\'s npz tree')
-    parser.add_argument('--gt-root', default=None, help='3dmatch: the directory holding <benchmark>/<scene>/gt.log and gt.info')
+    parser.add_argument('--protocol', choices=['gtlog', 'dgr'], default='gtlog',
+                        help="3dmatch: 'gtlog' scores against gt.log (eval.py), 'dgr' by RRE / RTE against the npz transform (eval_dgr.py)")
+    parser.add_argument('--test-epoch', type=int, default=None, help='dgr: the epoch its Epoch line prints')
+    parser.add_argument('--gt-root', default=None, help='3dmatch gtlog: the directory holding <benchmark>/<scene>/gt.log and gt.info')
     parser.add_argument('--registration-dir', default=None, help='3dmatch: where est.log files go')
     parser.add_argument('--verbose', action='store_true', help='log every pair')
     return parser
@@ -374,15 +474,20 @@ def make_parser():
 
 def main(argv=None):
     args = make_parser().parse_args(argv)
-    if args.config == '3dmatch' and (args.benchmark is None or args.gt_root is None):
-        make_parser().error('--config 3dmatch needs --benchmark and --gt-root')
+    if args.protocol == 'dgr' and args.config != '3dmatch':
+        make_parser().error("--protocol dgr is a 3dmatch evaluation (KITTI's eval.py already scores by RRE / RTE)")
+    if args.protocol == 'dgr' and args.registration_dir is not None:
+        make_parser().error('--protocol dgr writes no est.log: drop --registration-dir')
+    if args.config == '3dmatch' and (args.benchmark is None or (args.gt_root is None and args.protocol == 'gtlog')):
+        make_parser().error('--config 3dmatch needs --benchmark, and --gt-root unless --protocol dgr')
     try:
         settings = parse_num_corr(args.num_corr)
     except ValueError as e:
         make_parser().error(str(e))
     logging.basicConfig(level=logging.INFO, format='[%(asctime)s] %(message)s', stream=sys.stdout)
     return evaluate(args.config, args.method, args.features, benchmark=args.benchmark, gt_root=args.gt_root, num_corr=settings,
-                    registration_dir=args.registration_dir, verbose=args.verbose, log=lambda level, msg: _LOG.log(level, msg))
+                    registration_dir=args.registration_dir, verbose=args.verbose, log=lambda level, msg: _LOG.log(level, msg),
+                    protocol=args.protocol, test_epoch=args.test_epoch)
 
 
 if __name__ == '__main__':

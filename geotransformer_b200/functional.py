@@ -2581,6 +2581,37 @@ def modelnet_benchmark_pairs_batched(shapes, lengths, indices, num_points, keep_
     return out, [m] * (2 * B), T, origin
 
 
+def rotated_pairs_batched(points, lengths, indices, transforms):
+    """Rotated 3DMatch / 3DLoMatch test pairs (``geob200_rotated_pairs_batched``): pair p is the reference's
+    ``ThreeDMatchPairDataset(rotated=True)`` item of dataset index ``indices[p]`` (0 .. 2^32-1) with numpy's legacy stream seeded by
+    that index.  ``points``: CUDA (sum(lengths), 3) float32 or float64 (the clouds' file type: numpy rotates either in fp64), stacked [ref_0..ref_{B-1}, src_0..src_{B-1}]; ``lengths``: 2B host ints
+    (each >= 1); ``transforms``: (B, 4, 4) float64 [R | t] from the metadata (ref = T src).  Returns (points (sum(lengths), 3) fp32
+    in the input's layout, transforms (B, 4, 4) fp32, rotations (B, 2, 3, 3) float64: R_ref, R_src).  The half-angles' sin and cos are
+    correctly rounded, which the host libm that the reference calls is except in rare near-tie cases (DESIGN.md section 8a).  No
+    host synchronisation."""
+    if not isinstance(points, torch.Tensor) or not points.is_cuda or points.dtype not in (torch.float32, torch.float64):
+        raise RuntimeError('rotated_pairs_batched: points must be a CUDA float32 or float64 tensor (geotransformer_b200 has no CPU path)')
+    lengths = [int(v) for v in lengths]
+    indices = [int(v) for v in indices]
+    B = len(indices)
+    if B < 1 or len(lengths) != 2 * B:
+        raise RuntimeError('rotated_pairs_batched: indices must hold one value per pair and lengths two')
+    if points.dim() != 2 or points.shape[1] != 3 or points.shape[0] != sum(lengths) or not points.is_contiguous():
+        raise RuntimeError(f'rotated_pairs_batched: points must be contiguous (sum(lengths), 3), got {tuple(points.shape)}')
+    if any(not 0 <= i < 1 << 32 for i in indices):
+        raise RuntimeError('rotated_pairs_batched: indices must be in 0..2^32-1')
+    dev = points.device
+    T_in = torch.as_tensor(transforms, dtype=torch.float64).to(dev, non_blocking=True).contiguous()
+    if tuple(T_in.shape) != (B, 4, 4):
+        raise RuntimeError(f'rotated_pairs_batched: transforms must be ({B}, 4, 4), got {tuple(T_in.shape)}')
+    out = torch.empty(points.shape, dtype=_f32, device=dev)
+    T = torch.empty((B, 4, 4), dtype=_f32, device=dev)
+    rot = torch.empty((B, 2, 3, 3), dtype=torch.float64, device=dev)
+    L.check(L.lib().geob200_rotated_pairs_batched(points.data_ptr(), int(points.dtype == torch.float64), _host_i64(lengths), _host_i64(indices), B, T_in.data_ptr(),
+                                                  out.data_ptr(), T.data_ptr(), rot.data_ptr(), L.stream_ptr()), 'rotated_pairs_batched')
+    return out, T, rot
+
+
 VOXEL_MAX_CLOUDS = 64
 _VOXEL_ERRORS = {1: 'a coordinate is NaN or infinite',
                  2: 'voxel_size is too small (voxel_size * INT_MAX < the extent of the bounding box, as Open3D checks)',

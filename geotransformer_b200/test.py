@@ -1,7 +1,7 @@
 """Testing a snapshot on a benchmark from the dataset files, the experiments' ``test.py``.
 
     python -m geotransformer_b200.test --config 3dmatch --benchmark {3DMatch,3DLoMatch} --snapshot FILE --dataset-root DIR \\
-        --output-dir DIR [--neighbor-limits calibrate|config] [--seed S]
+        --output-dir DIR [--neighbor-limits calibrate|config] [--seed S] [--rotated]
     python -m geotransformer_b200.test --config kitti --snapshot FILE --dataset-root DIR --output-dir DIR
     python -m geotransformer_b200.test --config modelnet --snapshot FILE --dataset-root DIR --output-dir DIR
 
@@ -10,6 +10,9 @@ writes ``<output-dir>/features/<benchmark>/<scene>/<ref>_<src>.npz`` and KITTI `
 tree ``python -m geotransformer_b200.evaluate --features <output-dir>/features`` reads; ModelNet reports the metrics only, as the
 reference's ModelNet ``test.py`` does.  By default the neighbour limits are calibrated on the augmented training set, as the
 reference's ``test_data_loader`` does; ``--neighbor-limits config`` takes the config's limits instead (3DMatch only).
+``--rotated`` (3DMatch only) tests on the rotated benchmark: pair i's clouds get the rotations drawn from ``np.random.seed(i)``, and
+the ``.npz`` files hold the rotated points and transform; score them with ``evaluate --protocol dgr``, since gt.log is in the frame
+of the un-rotated fragments.
 """
 import argparse
 import os
@@ -20,12 +23,14 @@ from .config import make_cfg
 from .trainval import _log, log_string, training_set
 
 
-def benchmark_set(cfg, root, benchmark):
+def benchmark_set(cfg, root, benchmark, rotated=False):
+    if rotated and cfg.name != '3dmatch':
+        raise ValueError('--rotated is a 3dmatch benchmark')
     if cfg.name == '3dmatch':
         from .datasets.threedmatch import ThreeDMatchPairs
         if benchmark not in ('3DMatch', '3DLoMatch'):
             raise ValueError("--benchmark must be '3DMatch' or '3DLoMatch' for 3dmatch")
-        return ThreeDMatchPairs(root, benchmark)
+        return ThreeDMatchPairs(root, benchmark, rotated=rotated)
     if cfg.name == 'kitti':
         from .datasets.kitti import KittiPairs
         return KittiPairs(root, 'test')
@@ -33,7 +38,7 @@ def benchmark_set(cfg, root, benchmark):
     return ModelNetPairs(root, 'test', cfg)
 
 
-def run(config, snapshot, dataset_root, output_dir, benchmark=None, neighbor_limits='calibrate', seed=None):
+def run(config, snapshot, dataset_root, output_dir, benchmark=None, neighbor_limits='calibrate', seed=None, rotated=False):
     """the test of the module docstring; returns (summary, per-pair results)"""
     from .model import create_model
     from .tester import RegistrationTester
@@ -43,7 +48,7 @@ def run(config, snapshot, dataset_root, output_dir, benchmark=None, neighbor_lim
     device = torch.device('cuda', torch.cuda.current_device())
     os.makedirs(output_dir, exist_ok=True)
     log_file = os.path.join(output_dir, 'test.log')
-    test_set = benchmark_set(cfg, dataset_root, benchmark)
+    test_set = benchmark_set(cfg, dataset_root, benchmark, rotated=rotated)
     if neighbor_limits == 'calibrate':
         limits, used = calibrate_neighbors_augmented(training_set(cfg, dataset_root), cfg, seed)
         limits = [int(x) for x in limits]
@@ -82,12 +87,16 @@ def make_parser():
     p.add_argument('--output-dir', required=True)
     p.add_argument('--neighbor-limits', choices=['calibrate', 'config'], default='calibrate')
     p.add_argument('--seed', type=int, default=None, help='seed of the calibration draws (default cfg.seed)')
+    p.add_argument('--rotated', action='store_true', help='3dmatch only: the rotated benchmark (pair i rotated from np.random.seed(i))')
     return p
 
 
 def main(argv=None):
     a = make_parser().parse_args(argv)
-    run(a.config, a.snapshot, a.dataset_root, a.output_dir, benchmark=a.benchmark, neighbor_limits=a.neighbor_limits, seed=a.seed)
+    if a.rotated and a.config != '3dmatch':
+        make_parser().error('--rotated is a 3dmatch benchmark')
+    run(a.config, a.snapshot, a.dataset_root, a.output_dir, benchmark=a.benchmark, neighbor_limits=a.neighbor_limits, seed=a.seed,
+        rotated=a.rotated)
 
 
 if __name__ == '__main__':

@@ -65,11 +65,18 @@ class RegistrationTester:
 
     def run(self, dataset, log=None):
         """dataset: indexable of dicts with ref_points/src_points/ref_feats/src_feats/transform (+ scene_name, ref_frame,
-        src_frame, overlap as the reference datasets provide).  Returns (summary of mean metrics, per-pair results)."""
+        src_frame, overlap as the reference datasets provide).  A rotated ``ThreeDMatchPairs`` builds each chunk on the device with
+        ``rotated_batch``, which the engine takes without a copy through the host.  Returns (summary of mean metrics, per-pair
+        results)."""
         per_pair = []
         n = len(dataset)
+        device_chunk = getattr(dataset, 'rotated_batch', None) if getattr(dataset, 'rotated', False) else None
         for base in range(0, n, self.chunk):
-            items = [dataset[i] for i in range(base, min(n, base + self.chunk))]
+            stop = min(n, base + self.chunk)
+            if device_chunk is not None:
+                items = device_chunk(range(base, stop), device=self.engine.device)
+            else:
+                items = [dataset[i] for i in range(base, stop)]
             tensors = [{k: v for k, v in it.items() if isinstance(v, (np.ndarray, torch.Tensor))} for it in items]
             results = self.engine.register(tensors, keep_outputs=self.output_dir is not None)
             for it, res in zip(items, results):

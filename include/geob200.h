@@ -839,6 +839,23 @@ int geob200_modelnet_benchmark_pairs_batched(const float* shapes, const int64_t*
                                              double noise_magnitude, float* out_points, int32_t* origin, float* out_transforms,
                                              void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- Rotated 3DMatch / 3DLoMatch benchmark pairs (datasets/registration/threedmatch/dataset.py, rotated=True) -------------------
+ *
+ * Pair p is the reference's rotated test item of dataset index indices_h[p] (0 .. 2^32-1).  Its clouds are rows of `points` (fp32,
+ * or fp64 with points_fp64 = 1: the type the dataset's files hold, since numpy rotates them in fp64 either way; stacked [ref_0..ref_{B-1}, src_0..src_{B-1}] with host lengths_h[2B], each 1 .. 2^31-1 points, 2^31-1 rows in all) and its
+ * transform is transforms[p] (fp64 (4, 4), [R | t], ref = T src, from the metadata's fp64 rotation and translation).  One stream
+ * per pair: numpy's legacy generator seeded as np.random.seed(index), drawing random_sample_rotation_v2 for ref, then for src:
+ *   axis = rand(3) - 0.5; axis = axis / sqrt(fma(a2, a2, fma(a1, a1, a0 a0))) + 1e-8 (added after the division); theta = pi rand();
+ *   R = scipy's from_euler('zyx', axis theta) in its quaternion arithmetic.
+ * Outputs, in the layout of the inputs: out_points = fp32(p R^T), fma(z, R[i,2], fma(y, R[i,1], x R[i,0])) in fp64, numpy's own
+ * order (ref with R_ref, src with R_src); out_transforms (B, 4, 4) fp32 = fp32([R_ref R R_src^T | R_ref t]), the products in numpy's
+ * (OpenBLAS's) fp64 order: (A B)[i, j] = fma(a_i2, b_2j, fma(a_i1, b_1j, a_i0 b_0j)), (A v)[i] = fma(a_i2, v2, fma(a_i0, v0,
+ * a_i1 v1)); rotations (B, 2, 9) fp64: R_ref, R_src row-major.  The half-angles' sin and cos are correctly rounded (the host
+ * libm's differ from that only in rare near-tie cases, DESIGN §8a).  Any n_pairs (1 .. 2^30): launches of up to 64 pairs, each a
+ * one-warp-per-pair draw kernel and one grid over the rows.  No workspace. */
+int geob200_rotated_pairs_batched(const void* points, int points_fp64, const int64_t* lengths_h, const int64_t* indices_h, int64_t n_pairs,
+                                  const double* transforms, float* out_points, float* out_transforms, double* rotations, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
