@@ -686,6 +686,44 @@ __device__ __forceinline__ void mnb_draws(uint32_t index, int K, const MnParams&
     legacy_permutation(rng, shuf + M, M);
 }
 
+// normalize_points in fp32, by one warp: the column sums in row order, / N, to mean[3]; then the largest sqrt((x^2 + y^2) + z^2)
+// of the centred points to *scale.  The normalised coordinate is normalized(v, mean, scale).  The benchmark pairs and the raw
+// shapes share these two, so a pair's points and its raw_points come from the same normalisation.
+__device__ __forceinline__ void normalize_stats(const float* __restrict__ pts, int N, float* mean, float* scale) {
+    const int lane = threadIdx.x & 31;
+    if (lane < 3) {
+        float s = 0.0f;
+        for (int j = 0; j < N; ++j) s = __fadd_rn(s, pts[3 * j + lane]);
+        mean[lane] = __fdiv_rn(s, (float)N);
+    }
+    __syncwarp();
+    const float mx = mean[0], my = mean[1], mz = mean[2];
+    float nmax = 0.0f;
+    for (int j = lane; j < N; j += 32) {
+        const float x = __fsub_rn(pts[3 * j], mx), y = __fsub_rn(pts[3 * j + 1], my), z = __fsub_rn(pts[3 * j + 2], mz);
+        nmax = fmaxf(nmax, __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y)), __fmul_rn(z, z))));
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) nmax = fmaxf(nmax, __shfl_xor_sync(0xffffffffu, nmax, o));
+    if (lane == 0) *scale = nmax;
+}
+
+__device__ __forceinline__ float normalized(float v, float mean, float scale) { return __fdiv_rn(__fsub_rn(v, mean), scale); }
+
+// The ModelNet item's raw_points: normalize_points(shape) in fp32.  One CTA per shape, grid (n, 1), MNB_THREADS: warp 0 takes the
+// statistics, then the CTA writes the rows.  The output has the input's layout.
+__global__ void __launch_bounds__(MNB_THREADS) modelnet_raw_kernel(const float* __restrict__ shapes, const MnbPair* __restrict__ pairs,
+                                                                   float* __restrict__ out) {
+    __shared__ float mean_s[3], scale_s;
+    const MnbPair pr = pairs[blockIdx.x];
+    const float* pts = shapes + 3ll * pr.start;
+    if (threadIdx.x < 32) normalize_stats(pts, pr.count, mean_s, &scale_s);
+    __syncthreads();
+    const float scale = scale_s;
+    float* o = out + 3ll * pr.start;
+    for (int i = threadIdx.x; i < 3 * pr.count; i += MNB_THREADS) o[i] = normalized(pts[i], mean_s[i % 3], scale);
+}
+
 // One CTA per pair, grid (n, 1), MNB_THREADS.  Warp 0 consumes the pair's stream (mnb_draws) while warp 1 normalises the shape in
 // fp32; then the CTA orders each cloud's crop (bitonic sort of (distance desc, row asc)), maps the samples to shape rows, and writes
 // the jittered, shuffled points.  Dynamic shared memory: sort keys and rows (sort_n each; the draws' scratch aliases them), sel and
@@ -701,7 +739,7 @@ __global__ void __launch_bounds__(MNB_THREADS) modelnet_benchmark_kernel(
     __shared__ uint32_t mt[MT_N];
     __shared__ double prm[21];
     __shared__ float mean_s[3], scale_s;
-    const int q = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, M = P.num_points;
+    const int q = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, M = P.num_points;
     const MnbPair pr = pairs[q];
     const int N = pr.count, K = crop_count(N, P.keep_ratio);
     const float* pts = shapes + 3ll * pr.start;
@@ -710,30 +748,15 @@ __global__ void __launch_bounds__(MNB_THREADS) modelnet_benchmark_kernel(
     if (warp == 0) {
         mnb_draws(pr.index, K, P, mt, prm, reinterpret_cast<int*>(skey), sel, shuf, jit, T_out + 16ll * (pair0 + q));
     } else if (warp == 1) {
-        // normalize_points in fp32: column sums in row order, / N; then the largest sqrt((x^2 + y^2) + z^2) of the centred points
-        if (lane < 3) {
-            float s = 0.0f;
-            for (int j = 0; j < N; ++j) s = __fadd_rn(s, pts[3 * j + lane]);
-            mean_s[lane] = __fdiv_rn(s, (float)N);
-        }
-        __syncwarp();
-        const float mx = mean_s[0], my = mean_s[1], mz = mean_s[2];
-        float nmax = 0.0f;
-        for (int j = lane; j < N; j += 32) {
-            const float x = __fsub_rn(pts[3 * j], mx), y = __fsub_rn(pts[3 * j + 1], my), z = __fsub_rn(pts[3 * j + 2], mz);
-            nmax = fmaxf(nmax, __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y)), __fmul_rn(z, z))));
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) nmax = fmaxf(nmax, __shfl_xor_sync(0xffffffffu, nmax, o));
-        if (lane == 0) scale_s = nmax;
+        normalize_stats(pts, N, mean_s, &scale_s);
     }
     __syncthreads();
     const float mx = mean_s[0], my = mean_s[1], mz = mean_s[2], scale = scale_s;
     // point j of cloud c: the normalised fp32 point, and for src its image p R + (-(R^T t)) in fp64
     auto point = [&](int c, int j, double& x, double& y, double& z) {
-        x = (double)__fdiv_rn(__fsub_rn(pts[3 * j], mx), scale);
-        y = (double)__fdiv_rn(__fsub_rn(pts[3 * j + 1], my), scale);
-        z = (double)__fdiv_rn(__fsub_rn(pts[3 * j + 2], mz), scale);
+        x = (double)normalized(pts[3 * j], mx, scale);
+        y = (double)normalized(pts[3 * j + 1], my, scale);
+        z = (double)normalized(pts[3 * j + 2], mz, scale);
         if (c) {
             const double a = __dadd_rn(col_dot(prm, 0, x, y, z), prm[18]);
             const double b = __dadd_rn(col_dot(prm, 1, x, y, z), prm[19]);
@@ -1049,6 +1072,47 @@ int geob200_modelnet_benchmark_pairs_batched(const float* shapes, const int64_t*
         const size_t smem = (size_t)P.sort_n * (sizeof(unsigned long long) + sizeof(int)) + (size_t)4 * M * sizeof(int);
         if (smem > 48 * 1024 && ensure_max_smem((const void*)modelnet_benchmark_kernel)) return -1;
         modelnet_benchmark_kernel<<<n, MNB_THREADS, smem, st>>>(shapes, table, B, p0, P, jit, out_points, origin, out_transforms);
+        GEOB_CHECK_LAUNCH();
+        ++launches;
+    }
+    count_launches(launches);
+    return 0;
+}
+
+size_t geob200_modelnet_raw_points_batched_workspace_bytes(int64_t n_shapes) {
+    const size_t b = (size_t)(n_shapes < 1 ? 0 : n_shapes < MNB_MAX_PAIRS ? n_shapes : MNB_MAX_PAIRS);
+    return align_up(b * sizeof(MnbPair), 256) + 256;
+}
+
+int geob200_modelnet_raw_points_batched(const float* shapes, const int64_t* lengths_h, int64_t n_shapes, float* out_points,
+                                        void* workspace, size_t workspace_bytes, void* stream) {
+    GEOB_REQUIRE(n_shapes > 0 && n_shapes < (1ll << 31) / MN_MAX_SHAPE, "modelnet_raw_points_batched: n_shapes must be in 1..%lld",
+                 (1ll << 31) / MN_MAX_SHAPE - 1);
+    GEOB_REQUIRE(lengths_h != nullptr, "modelnet_raw_points_batched: null lengths");
+    GEOB_REQUIRE(shapes != nullptr && out_points != nullptr, "modelnet_raw_points_batched: null pointer");
+    for (int64_t p = 0; p < n_shapes; ++p)
+        GEOB_REQUIRE(lengths_h[p] > 0 && lengths_h[p] <= MN_MAX_SHAPE, "modelnet_raw_points_batched: shape %lld has %lld points (1..%d)",
+                     (long long)p, (long long)lengths_h[p], MN_MAX_SHAPE);
+    GEOB_REQUIRE(workspace != nullptr && workspace_bytes >= geob200_modelnet_raw_points_batched_workspace_bytes(n_shapes),
+                 "modelnet_raw_points_batched: workspace too small");
+    const int B = (int)n_shapes;
+    const int cap = B < MNB_MAX_PAIRS ? B : MNB_MAX_PAIRS;
+    Arena ar(workspace, workspace_bytes);
+    MnbPair* table = ar.take<MnbPair>((size_t)cap);
+    GEOB_REQUIRE(ar.ok(), "modelnet_raw_points_batched: workspace accounting error");
+    cudaStream_t st = (cudaStream_t)stream;
+    MnbPair host[MNB_MAX_PAIRS];
+    long long start = 0;
+    int launches = 0;
+    for (int p0 = 0; p0 < B; p0 += cap) {
+        const int n = B - p0 < cap ? B - p0 : cap;
+        for (int q = 0; q < n; ++q) {
+            host[q] = MnbPair{start, (int)lengths_h[p0 + q], 0u};
+            start += lengths_h[p0 + q];
+        }
+        // from pageable memory: staged before the call returns, ordered before the launch on the stream
+        GEOB_CHECK_CUDA(cudaMemcpyAsync(table, host, (size_t)n * sizeof(MnbPair), cudaMemcpyHostToDevice, st));
+        modelnet_raw_kernel<<<n, MNB_THREADS, 0, st>>>(shapes, table, out_points);
         GEOB_CHECK_LAUNCH();
         ++launches;
     }

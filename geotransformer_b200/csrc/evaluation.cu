@@ -945,3 +945,271 @@ int geob200_fine_matching_loss_backward_batched(const float* ref_knn_points, con
 }
 
 }  // extern "C"
+
+// ---- RPMNet's ModelNet metrics (modified Chamfer distance, anisotropic errors) --------------------------------------------------
+//
+// Reference: geotransformer/utils/registration.py:69-130 (compute_rotation_mse_and_mae, compute_translation_mse_and_mae,
+// compute_modified_chamfer_distance) and modules/registration/metrics.py:8-161.  The contract is in DESIGN.md section 8a:
+//   cd_pq = mean_i |fp32(est src_i) - raw_nn|, cd_qp = mean_j |ref_j - fp32((est gt^-1) raw)_nn|, exact nearest neighbours with fp64
+//   distances (feature_nn_launch, C = 3); transforms composed and applied in fp64 and rounded to fp32 once; per-pair sums in a fixed
+//   order.  r_mse / r_mae: scipy's from_matrix (polar factor unless the Gram matrix is within isclose(atol=1e-12) of I, Shepperd's
+//   quaternion) and as_euler('xyz', degrees=True) with its gimbal rule, differences not wrapped; t_mse / t_mae in fp32 as numpy.
+#include "feature_match.cuh"
+#include "kabsch.cuh"
+
+namespace geob200 {
+
+constexpr int RP_MAX_PAIRS = GEOB_MAX_CLOUDS / 2;
+constexpr int RP_THREADS = 256;
+
+struct RpLaunch {
+    int n;
+    int cap_q, cap_s;                          // rows per pair of the query (src, ref) and support (raw) buffers
+    long long raw0[RP_MAX_PAIRS], ref0[RP_MAX_PAIRS], src0[RP_MAX_PAIRS];
+    int n_raw[RP_MAX_PAIRS], n_ref[RP_MAX_PAIRS], n_src[RP_MAX_PAIRS];
+};
+
+__device__ __forceinline__ double det3(const double* m) {
+    return __dsub_rn(__dadd_rn(__dmul_rn(m[0], __dsub_rn(__dmul_rn(m[4], m[8]), __dmul_rn(m[5], m[7]))),
+                               __dmul_rn(m[2], __dsub_rn(__dmul_rn(m[3], m[7]), __dmul_rn(m[4], m[6])))),
+                     __dmul_rn(m[1], __dsub_rn(__dmul_rn(m[3], m[8]), __dmul_rn(m[5], m[6]))));
+}
+
+// scipy's Rotation.from_matrix(M).as_euler('xyz') in radians, M with det > 0 (fp32 values widened to fp64, as from_matrix does)
+__device__ void rp_euler_xyz(const double (&Min)[9], double (&e)[3]) {
+    double M[9];
+    for (int i = 0; i < 9; ++i) M[i] = Min[i];
+    bool orthogonal = true;                    // isclose(M M^T, I, rtol=1e-5, atol=1e-12) everywhere
+    for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j) {
+            const double g = __dadd_rn(__dadd_rn(__dmul_rn(M[3 * i], M[3 * j]), __dmul_rn(M[3 * i + 1], M[3 * j + 1])),
+                                       __dmul_rn(M[3 * i + 2], M[3 * j + 2]));
+            const double want = i == j ? 1.0 : 0.0;
+            if (!(fabs(g - want) <= 1e-12 + 1e-5 * want)) orthogonal = false;
+        }
+    if (!orthogonal) {                         // the polar factor U V^T of M = U S V^T: kabsch_rotation(M^T) (det M > 0: no flip)
+        double Mt[9];
+        for (int i = 0; i < 3; ++i)
+            for (int j = 0; j < 3; ++j) Mt[3 * i + j] = M[3 * j + i];
+        kabsch_rotation(Mt, M);
+    }
+    // Shepperd: argmax (first on ties) of [m00, m11, m22, trace]; quaternion (x, y, z, w), normalised
+    const double tr = __dadd_rn(__dadd_rn(M[0], M[4]), M[8]);
+    const double dec[4] = {M[0], M[4], M[8], tr};
+    int c = 0;
+    for (int k = 1; k < 4; ++k)
+        if (dec[k] > dec[c]) c = k;
+    double q[4];
+    if (c == 3) {
+        q[0] = __dsub_rn(M[7], M[5]); q[1] = __dsub_rn(M[2], M[6]); q[2] = __dsub_rn(M[3], M[1]); q[3] = __dadd_rn(1.0, tr);
+    } else {
+        const int i = c, j = (i + 1) % 3, k = (j + 1) % 3;
+        q[i] = __dadd_rn(__dsub_rn(1.0, tr), __dmul_rn(2.0, M[4 * i]));
+        q[j] = __dadd_rn(M[3 * j + i], M[3 * i + j]);
+        q[k] = __dadd_rn(M[3 * k + i], M[3 * i + k]);
+        q[3] = __dsub_rn(M[3 * k + j], M[3 * j + k]);
+    }
+    const double nq = __dsqrt_rn(__dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(q[0], q[0]), __dmul_rn(q[1], q[1])), __dmul_rn(q[2], q[2])),
+                                           __dmul_rn(q[3], q[3])));
+    for (int k = 0; k < 4; ++k) q[k] = __ddiv_rn(q[k], nq);
+    // as_euler, extrinsic 'xyz' (i, j, k = 0, 1, 2; sign = 1)
+    const double a = __dsub_rn(q[3], q[1]), b = __dadd_rn(q[0], q[2]), cc = __dadd_rn(q[1], q[3]), d = __dsub_rn(q[2], q[0]);
+    const double second = __dmul_rn(2.0, atan2(hypot(cc, d), hypot(a, b)));
+    const double half_sum = atan2(b, a), half_diff = atan2(d, cc);
+    if (fabs(second) <= 1e-7) {                // gimbal lock: third angle 0
+        e[0] = __dmul_rn(2.0, half_sum); e[2] = 0.0;
+    } else if (fabs(__dsub_rn(second, M_PI)) <= 1e-7) {
+        e[0] = -__dmul_rn(2.0, half_diff); e[2] = 0.0;
+    } else {
+        e[0] = __dsub_rn(half_sum, half_diff); e[2] = __dadd_rn(half_sum, half_diff);
+    }
+    e[1] = __dsub_rn(second, M_PI_2);
+    for (int k = 0; k < 3; ++k) {
+        if (e[k] < -M_PI) e[k] = __dadd_rn(e[k], 2.0 * M_PI);
+        else if (e[k] > M_PI) e[k] = __dsub_rn(e[k], 2.0 * M_PI);
+    }
+}
+
+// One thread per pair: the status (det <= 0 of gt or est), the anisotropic errors, and the two transforms the points kernel applies
+// (est, and est gt^-1 with gt^-1 = [A^-1 | -A^-1 t] by the adjugate), 12 doubles each, in xf.
+__global__ void __launch_bounds__(32) rp_pair_kernel(int n, const float* __restrict__ gt, const float* __restrict__ est,
+                                                     double* __restrict__ xf, double* __restrict__ out) {
+    const int p = threadIdx.x;
+    if (p >= n) return;
+    const float* G = gt + 16 * p;
+    const float* E = est + 16 * p;
+    double Rg[9], Re[9];
+    for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j) { Rg[3 * i + j] = (double)G[4 * i + j]; Re[3 * i + j] = (double)E[4 * i + j]; }
+    double* o = out + GEOB200_RPMNET_COLUMNS * p;
+    const double dg = det3(Rg), de = det3(Re);
+    o[7] = !(dg > 0.0) ? GEOB200_RPMNET_GT_DET : !(de > 0.0) ? GEOB200_RPMNET_EST_DET : 0;
+    if (o[7] == 0.0) {
+        double eg[3], ee[3];
+        rp_euler_xyz(Rg, eg);
+        rp_euler_xyz(Re, ee);
+        const double deg = 180.0 / M_PI;       // np.rad2deg
+        double s2 = 0.0, s1 = 0.0;
+        for (int k = 0; k < 3; ++k) {
+            const double t = __dsub_rn(__dmul_rn(eg[k], deg), __dmul_rn(ee[k], deg));
+            s2 = __dadd_rn(s2, __dmul_rn(t, t));
+            s1 = __dadd_rn(s1, fabs(t));
+        }
+        o[3] = __ddiv_rn(s2, 3.0);
+        o[4] = __ddiv_rn(s1, 3.0);
+    } else {
+        o[3] = o[4] = __longlong_as_double(0x7ff8000000000000ll);
+    }
+    float f2 = 0.0f, f1 = 0.0f;                // fp32 translation errors, as numpy's float32 mean of three
+    for (int i = 0; i < 3; ++i) {
+        const float t = __fsub_rn(G[4 * i + 3], E[4 * i + 3]);
+        f2 = __fadd_rn(f2, __fmul_rn(t, t));
+        f1 = __fadd_rn(f1, fabsf(t));
+    }
+    o[5] = (double)__fdiv_rn(f2, 3.0f);
+    o[6] = (double)__fdiv_rn(f1, 3.0f);
+    // est, then est gt^-1
+    double* x = xf + 24 * p;
+    for (int i = 0; i < 3; ++i) {
+        for (int j = 0; j < 3; ++j) x[4 * i + j] = Re[3 * i + j];
+        x[4 * i + 3] = (double)E[4 * i + 3];
+    }
+    double Ai[9];
+    const double id = 1.0 / dg;
+    Ai[0] = (Rg[4] * Rg[8] - Rg[5] * Rg[7]) * id; Ai[1] = (Rg[2] * Rg[7] - Rg[1] * Rg[8]) * id; Ai[2] = (Rg[1] * Rg[5] - Rg[2] * Rg[4]) * id;
+    Ai[3] = (Rg[5] * Rg[6] - Rg[3] * Rg[8]) * id; Ai[4] = (Rg[0] * Rg[8] - Rg[2] * Rg[6]) * id; Ai[5] = (Rg[2] * Rg[3] - Rg[0] * Rg[5]) * id;
+    Ai[6] = (Rg[3] * Rg[7] - Rg[4] * Rg[6]) * id; Ai[7] = (Rg[1] * Rg[6] - Rg[0] * Rg[7]) * id; Ai[8] = (Rg[0] * Rg[4] - Rg[1] * Rg[3]) * id;
+    double ti[3];
+    for (int i = 0; i < 3; ++i) ti[i] = -(Ai[3 * i] * G[3] + Ai[3 * i + 1] * G[7] + Ai[3 * i + 2] * G[11]);
+    double* y = x + 12;
+    for (int i = 0; i < 3; ++i) {
+        for (int j = 0; j < 3; ++j) y[4 * i + j] = Re[3 * i] * Ai[j] + Re[3 * i + 1] * Ai[3 + j] + Re[3 * i + 2] * Ai[6 + j];
+        y[4 * i + 3] = Re[3 * i] * ti[0] + Re[3 * i + 1] * ti[1] + Re[3 * i + 2] * ti[2] + x[4 * i + 3];
+    }
+}
+
+__device__ __forceinline__ void rp_apply(const double* T, const float* p, float* q) {
+    const double x = p[0], y = p[1], z = p[2];
+#pragma unroll
+    for (int i = 0; i < 3; ++i)
+        q[i] = __double2float_rn(__dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[4 * i], x), __dmul_rn(T[4 * i + 1], y)), __dmul_rn(T[4 * i + 2], z)),
+                                           T[4 * i + 3]));
+}
+
+// Grid (ceil(max rows / RP_THREADS), n): the padded nearest-neighbour inputs of pair p.  Queries: slot p = est src, slot n + p = ref;
+// supports: slot p = raw, slot n + p = (est gt^-1) raw.
+__global__ void __launch_bounds__(RP_THREADS) rp_points_kernel(const __grid_constant__ RpLaunch L, const float* __restrict__ raw,
+                                                               const float* __restrict__ ref, const float* __restrict__ src,
+                                                               const double* __restrict__ xf, float* __restrict__ Q, float* __restrict__ S,
+                                                               int32_t* __restrict__ nq, int32_t* __restrict__ ns) {
+    const int p = blockIdx.y, r = blockIdx.x * RP_THREADS + threadIdx.x, n = L.n;
+    const double* x = xf + 24 * p;
+    if (r == 0) { nq[p] = L.n_src[p]; nq[n + p] = L.n_ref[p]; ns[p] = L.n_raw[p]; ns[n + p] = L.n_raw[p]; }
+    if (r < L.n_src[p]) rp_apply(x, src + 3 * (L.src0[p] + r), Q + 3 * ((long long)p * L.cap_q + r));
+    if (r < L.n_ref[p]) {
+        const float* a = ref + 3 * (L.ref0[p] + r);
+        float* b = Q + 3 * ((long long)(n + p) * L.cap_q + r);
+        b[0] = a[0]; b[1] = a[1]; b[2] = a[2];
+    }
+    if (r < L.n_raw[p]) {
+        const float* a = raw + 3 * (L.raw0[p] + r);
+        float* b = S + 3 * ((long long)p * L.cap_s + r);
+        b[0] = a[0]; b[1] = a[1]; b[2] = a[2];
+        rp_apply(x + 12, a, S + 3 * ((long long)(n + p) * L.cap_s + r));
+    }
+}
+
+// One CTA per pair: the two means of the nearest-neighbour distances, each summed per thread in row order and then by a fixed tree,
+// so the bits do not depend on the batch.
+__global__ void __launch_bounds__(RP_THREADS) rp_reduce_kernel(int n, int cap_q, const int32_t* __restrict__ nq, const double* __restrict__ dist,
+                                                               double* __restrict__ out) {
+    __shared__ double part[RP_THREADS];
+    const int p = blockIdx.x, tid = threadIdx.x;
+    double mean[2];
+    for (int dir = 0; dir < 2; ++dir) {
+        const int slot = dir * n + p, rows = nq[slot];
+        const double* d = dist + (long long)slot * cap_q;
+        double s = 0.0;
+        for (int r = tid; r < rows; r += RP_THREADS) s = __dadd_rn(s, d[r]);
+        part[tid] = s;
+        __syncthreads();
+        for (int h = RP_THREADS / 2; h > 0; h >>= 1) {
+            if (tid < h) part[tid] = __dadd_rn(part[tid], part[tid + h]);
+            __syncthreads();
+        }
+        mean[dir] = __ddiv_rn(part[0], (double)rows);
+        __syncthreads();
+    }
+    if (tid == 0) {
+        double* o = out + GEOB200_RPMNET_COLUMNS * p;
+        o[0] = __dadd_rn(mean[0], mean[1]);
+        o[1] = mean[0];
+        o[2] = mean[1];
+    }
+}
+
+static size_t rp_workspace(int64_t n_pairs, int64_t cap_q, int64_t cap_s) {
+    const size_t B = (size_t)(n_pairs > 0 ? n_pairs : 0), q = (size_t)(cap_q > 0 ? cap_q : 0), s = (size_t)(cap_s > 0 ? cap_s : 0);
+    return align_up(24 * 8 * B, 256) + align_up(2 * B * q * 12, 256) + align_up(2 * B * s * 12, 256) + 2 * align_up(8 * B, 256) +
+           align_up(2 * B * q * 8, 256) + align_up(2 * B * q * 8, 256) + feature_nn_workspace(2 * (int64_t)B, q, s) + 256;
+}
+
+}  // namespace geob200
+
+extern "C" {
+
+size_t geob200_rpmnet_metrics_batched_workspace_bytes(int64_t n_pairs, int64_t cap_query, int64_t cap_raw) {
+    return rp_workspace(n_pairs, cap_query, cap_raw);
+}
+
+int geob200_rpmnet_metrics_batched(const float* raw, const int64_t* raw_lengths_h, const float* ref, const int64_t* ref_lengths_h,
+                                   const float* src, const int64_t* src_lengths_h, int64_t n_pairs, const float* gt_transforms,
+                                   const float* est_transforms, double* out, void* workspace, size_t workspace_bytes, void* stream) {
+    GEOB_REQUIRE(n_pairs > 0 && n_pairs <= RP_MAX_PAIRS, "rpmnet_metrics_batched: 1..%d pairs", RP_MAX_PAIRS);
+    GEOB_REQUIRE(raw_lengths_h != nullptr && ref_lengths_h != nullptr && src_lengths_h != nullptr, "rpmnet_metrics_batched: null lengths");
+    GEOB_REQUIRE(raw != nullptr && ref != nullptr && src != nullptr && gt_transforms != nullptr && est_transforms != nullptr && out != nullptr,
+                 "rpmnet_metrics_batched: null pointer");
+    RpLaunch L{};
+    L.n = (int)n_pairs;
+    long long r0 = 0, f0 = 0, s0 = 0;
+    for (int p = 0; p < L.n; ++p) {
+        GEOB_REQUIRE(raw_lengths_h[p] > 0 && ref_lengths_h[p] > 0 && src_lengths_h[p] > 0 && raw_lengths_h[p] < (1 << 28) &&
+                         ref_lengths_h[p] < (1 << 28) && src_lengths_h[p] < (1 << 28),
+                     "rpmnet_metrics_batched: pair %d needs 1..2^28-1 raw, ref and src points (got %lld, %lld, %lld)", p,
+                     (long long)raw_lengths_h[p], (long long)ref_lengths_h[p], (long long)src_lengths_h[p]);
+        L.raw0[p] = r0; L.ref0[p] = f0; L.src0[p] = s0;
+        L.n_raw[p] = (int)raw_lengths_h[p]; L.n_ref[p] = (int)ref_lengths_h[p]; L.n_src[p] = (int)src_lengths_h[p];
+        r0 += raw_lengths_h[p]; f0 += ref_lengths_h[p]; s0 += src_lengths_h[p];
+        L.cap_s = L.n_raw[p] > L.cap_s ? L.n_raw[p] : L.cap_s;
+        L.cap_q = L.n_ref[p] > L.cap_q ? L.n_ref[p] : L.cap_q;
+        L.cap_q = L.n_src[p] > L.cap_q ? L.n_src[p] : L.cap_q;
+    }
+    GEOB_REQUIRE(workspace != nullptr && workspace_bytes >= rp_workspace(n_pairs, L.cap_q, L.cap_s),
+                 "rpmnet_metrics_batched: workspace too small");
+    const int B = L.n;
+    Arena ar(workspace, workspace_bytes);
+    double* xf = ar.take<double>(24 * (size_t)B);
+    float* Q = ar.take<float>(2 * (size_t)B * L.cap_q * 3);
+    float* S = ar.take<float>(2 * (size_t)B * L.cap_s * 3);
+    int32_t* nq = ar.take<int32_t>(2 * (size_t)B);
+    int32_t* ns = ar.take<int32_t>(2 * (size_t)B);
+    int64_t* idx = ar.take<int64_t>(2 * (size_t)B * L.cap_q);
+    double* dist = ar.take<double>(2 * (size_t)B * L.cap_q);
+    const size_t nn_bytes = feature_nn_workspace(2 * (int64_t)B, L.cap_q, L.cap_s);
+    void* nn_ws = ar.take<char>(nn_bytes);
+    GEOB_REQUIRE(ar.ok(), "rpmnet_metrics_batched: workspace accounting error");
+    cudaStream_t st = (cudaStream_t)stream;
+    int launches = 0;
+    rp_pair_kernel<<<1, 32, 0, st>>>(B, gt_transforms, est_transforms, xf, out);
+    const int rows = L.cap_q > L.cap_s ? L.cap_q : L.cap_s;
+    rp_points_kernel<<<dim3((rows + RP_THREADS - 1) / RP_THREADS, B), RP_THREADS, 0, st>>>(L, raw, ref, src, xf, Q, S, nq, ns);
+    GEOB_CHECK_LAUNCH();
+    launches += 2;
+    if (feature_nn_launch(Q, S, 2 * B, L.cap_q, L.cap_s, 3, nq, ns, idx, dist, nullptr, nullptr, nn_ws, nn_bytes, st, &launches)) return -1;
+    rp_reduce_kernel<<<B, RP_THREADS, 0, st>>>(B, L.cap_q, nq, dist, out);
+    GEOB_CHECK_LAUNCH();
+    count_launches(launches + 1);
+    return 0;
+}
+
+}  // extern "C"

@@ -63,7 +63,8 @@ class ModelNetPairs:
     from the i-th shape of ``{root}/{subset}.pkl`` whose label passes the class filter, with the stream seeded by i.
 
     ``pairs[i]`` is a dict of device tensors ``ref_points`` / ``src_points`` (num_points, 3), ``ref_feats`` / ``src_feats``
-    (ones), ``transform`` (4, 4) and the ints ``label`` and ``index``; ``chunks()`` yields them as lists of up to ``chunk_size``.
+    (ones), ``transform`` (4, 4), ``raw_points`` (the normalised shape, which RPMNet's modified Chamfer distance measures against)
+    and the ints ``label`` and ``index``; ``chunks()`` yields them as lists of up to ``chunk_size``.
     Indexing builds (once) the chunk that holds the pair, so a sequential pass builds every pair once.  ``data_list`` stands in for
     the pkl's list of ``{'points', 'normals', 'label'}`` when given."""
 
@@ -98,12 +99,15 @@ class ModelNetPairs:
         raw = _stack_to_device(shapes, self.device)
         points, _, T, _ = GF.modelnet_benchmark_pairs_batched(raw, lengths, range(start, stop), m, d.keep_ratio, d.rotation_magnitude,
                                                               d.translation_magnitude, self.cfg.test.noise_magnitude)
+        raw_points = GF.modelnet_raw_points_batched(raw, lengths)
+        offsets = np.concatenate([[0], np.cumsum(lengths)]).tolist()
         B = stop - start
         ones = torch.ones((m, 1), dtype=torch.float32, device=self.device)
         # the engines read their inputs on worker streams that do not wait for this one: the chunk is complete on return
         torch.cuda.current_stream(self.device).synchronize()
         return [{'ref_points': points[p * m:(p + 1) * m], 'src_points': points[(B + p) * m:(B + p + 1) * m], 'ref_feats': ones,
-                 'src_feats': ones, 'transform': T[p], 'label': int(self.data_list[start + p]['label']), 'index': start + p}
+                 'src_feats': ones, 'transform': T[p], 'raw_points': raw_points[offsets[p]:offsets[p + 1]],
+                 'label': int(self.data_list[start + p]['label']), 'index': start + p}
                 for p in range(B)]
 
     def chunks(self):

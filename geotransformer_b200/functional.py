@@ -2581,6 +2581,71 @@ def modelnet_benchmark_pairs_batched(shapes, lengths, indices, num_points, keep_
     return out, [m] * (2 * B), T, origin
 
 
+def modelnet_raw_points_batched(shapes, lengths):
+    """The ModelNet items' ``raw_points`` (``geob200_modelnet_raw_points_batched``): ``normalize_points`` of each shape of ``shapes``
+    (stacked fp32, ``lengths`` host ints of 1 .. 8192) in fp32, with the normalisation ``modelnet_benchmark_pairs_batched`` applies.
+    Returns (sum(lengths), 3) fp32 in the input's layout.  No host synchronisation."""
+    _f(shapes, 'shapes')
+    lengths = [int(v) for v in lengths]
+    B = len(lengths)
+    if B < 1:
+        raise RuntimeError('modelnet_raw_points_batched: at least one shape')
+    if shapes.dim() != 2 or shapes.shape[1] != 3 or shapes.shape[0] != sum(lengths) or not shapes.is_contiguous():
+        raise RuntimeError(f'modelnet_raw_points_batched: shapes must be contiguous (sum(lengths), 3), got {tuple(shapes.shape)}')
+    lib = L.lib()
+    ws = L.workspace(lib.geob200_modelnet_raw_points_batched_workspace_bytes(B), shapes.device, tag='augment')
+    out = torch.empty(shapes.shape, dtype=_f32, device=shapes.device)
+    L.check(lib.geob200_modelnet_raw_points_batched(shapes.data_ptr(), _host_i64(lengths), B, out.data_ptr(), ws.data_ptr(), ws.numel(),
+                                                    L.stream_ptr()), 'modelnet_raw_points_batched')
+    return out
+
+
+RPMNET_MAX_PAIRS = 32
+RPMNET_COLUMNS = ('CD', 'CD_pq', 'CD_qp', 'r_mse', 'r_mae', 't_mse', 't_mae')
+_RPMNET_STATUS = {1: 'gt_transform', 2: 'est_transform'}
+
+
+def rpmnet_metrics_batched(raw, raw_lengths, ref, ref_lengths, src, src_lengths, gt_transforms, est_transforms, check=True):
+    """RPMNet's ModelNet metrics of B (1 .. 32) pairs in one call (``geob200_rpmnet_metrics_batched``, contract in DESIGN.md
+    section 8a).  ``raw`` / ``ref`` / ``src``: stacked CUDA fp32 (sum(lengths), 3) clouds with host lengths (each >= 1);
+    ``gt_transforms`` / ``est_transforms``: (B, 4, 4) fp32 on the same device.  Returns (B, 8) float64 rows
+    [CD, CD_pq, CD_qp, r_mse, r_mae, t_mse, t_mae, status] on the device.  ``check``: read the status column back (one copy) and
+    raise ValueError naming the first pair whose gt or estimated rotation has det <= 0, as scipy's from_matrix does; without it
+    nothing is synchronised and such rows hold NaN r_mse / r_mae and a non-zero status."""
+    lens = [[int(v) for v in x] for x in (raw_lengths, ref_lengths, src_lengths)]
+    B = len(lens[0])
+    if not 1 <= B <= RPMNET_MAX_PAIRS or len(lens[1]) != B or len(lens[2]) != B:
+        raise RuntimeError(f'rpmnet_metrics_batched: 1..{RPMNET_MAX_PAIRS} pairs with one raw, ref and src length each, got '
+                           f'{[len(x) for x in lens]}')
+    for name, t, n in (('raw', raw, lens[0]), ('ref', ref, lens[1]), ('src', src, lens[2])):
+        _f(t, name)
+        if t.dim() != 2 or t.shape[1] != 3 or t.shape[0] != sum(n) or not t.is_contiguous():
+            raise RuntimeError(f'rpmnet_metrics_batched: {name} must be contiguous (sum(lengths), 3), got {tuple(t.shape)}')
+        if min(n) < 1:
+            raise RuntimeError(f'rpmnet_metrics_batched: every {name} cloud needs at least one point')
+    dev = raw.device
+    gt, est = (t.contiguous() for t in (gt_transforms, est_transforms))
+    for name, t in (('gt_transforms', gt), ('est_transforms', est)):
+        _f(t, name)
+        if tuple(t.shape) != (B, 4, 4) or t.device != dev:
+            raise RuntimeError(f'rpmnet_metrics_batched: {name} must be ({B}, 4, 4) on the clouds\' device, got {tuple(t.shape)}')
+    if ref.device != dev or src.device != dev:
+        raise RuntimeError('rpmnet_metrics_batched: raw, ref and src must be on one device')
+    lib = L.lib()
+    ws = L.workspace(lib.geob200_rpmnet_metrics_batched_workspace_bytes(B, max(lens[1] + lens[2]), max(lens[0])), dev, tag='rpmnet')
+    out = torch.empty((B, 8), dtype=torch.float64, device=dev)
+    L.check(lib.geob200_rpmnet_metrics_batched(raw.data_ptr(), _host_i64(lens[0]), ref.data_ptr(), _host_i64(lens[1]), src.data_ptr(),
+                                               _host_i64(lens[2]), B, gt.data_ptr(), est.data_ptr(), out.data_ptr(), ws.data_ptr(),
+                                               ws.numel(), L.stream_ptr()), 'rpmnet_metrics_batched')
+    if check:
+        status = out[:, 7].cpu().tolist()
+        for p, s in enumerate(status):
+            if s != 0:
+                raise ValueError(f'rpmnet_metrics_batched: pair {p}: non-positive determinant (left-handed or null coordinate frame) '
+                                 f'in the rotation of {_RPMNET_STATUS.get(int(s), f"status {s}")}')
+    return out
+
+
 def rotated_pairs_batched(points, lengths, indices, transforms):
     """Rotated 3DMatch / 3DLoMatch test pairs (``geob200_rotated_pairs_batched``): pair p is the reference's
     ``ThreeDMatchPairDataset(rotated=True)`` item of dataset index ``indices[p]`` (0 .. 2^32-1) with numpy's legacy stream seeded by

@@ -3,7 +3,7 @@
     python -m geotransformer_b200.test --config 3dmatch --benchmark {3DMatch,3DLoMatch} --snapshot FILE --dataset-root DIR \\
         --output-dir DIR [--neighbor-limits calibrate|config] [--seed S] [--rotated]
     python -m geotransformer_b200.test --config kitti --snapshot FILE --dataset-root DIR --output-dir DIR
-    python -m geotransformer_b200.test --config modelnet --snapshot FILE --dataset-root DIR --output-dir DIR
+    python -m geotransformer_b200.test --config modelnet --snapshot FILE --dataset-root DIR --output-dir DIR [--rpmnet-metrics]
 
 ``RegistrationTester`` runs the model over the benchmark's pairs and logs the reference's per-pair and summary lines.  3DMatch
 writes ``<output-dir>/features/<benchmark>/<scene>/<ref>_<src>.npz`` and KITTI ``<output-dir>/features/<seq>_<src>_<ref>.npz``, the
@@ -12,7 +12,8 @@ reference's ModelNet ``test.py`` does.  By default the neighbour limits are cali
 reference's ``test_data_loader`` does; ``--neighbor-limits config`` takes the config's limits instead (3DMatch only).
 ``--rotated`` (3DMatch only) tests on the rotated benchmark: pair i's clouds get the rotations drawn from ``np.random.seed(i)``, and
 the ``.npz`` files hold the rotated points and transform; score them with ``evaluate --protocol dgr``, since gt.log is in the frame
-of the un-rotated fragments.
+of the un-rotated fragments.  ``--rpmnet-metrics`` (ModelNet only) also scores every pair with RPMNet's metrics (modified Chamfer
+distance, anisotropic rotation and translation MSE / MAE) and logs their means as ``rpmnet_<name>``.
 """
 import argparse
 import os
@@ -38,12 +39,15 @@ def benchmark_set(cfg, root, benchmark, rotated=False):
     return ModelNetPairs(root, 'test', cfg)
 
 
-def run(config, snapshot, dataset_root, output_dir, benchmark=None, neighbor_limits='calibrate', seed=None, rotated=False):
+def run(config, snapshot, dataset_root, output_dir, benchmark=None, neighbor_limits='calibrate', seed=None, rotated=False,
+        rpmnet_metrics=False):
     """the test of the module docstring; returns (summary, per-pair results)"""
     from .model import create_model
     from .tester import RegistrationTester
     from .utils.data import calibrate_neighbors_augmented
     cfg = make_cfg(config)
+    if rpmnet_metrics and cfg.name != 'modelnet':
+        raise ValueError('--rpmnet-metrics is a modelnet benchmark')
     seed = int(cfg.seed if seed is None else seed)
     device = torch.device('cuda', torch.cuda.current_device())
     os.makedirs(output_dir, exist_ok=True)
@@ -69,7 +73,7 @@ def run(config, snapshot, dataset_root, output_dir, benchmark=None, neighbor_lim
     else:
         feature_dir = os.path.join(output_dir, 'features', benchmark) if cfg.name == '3dmatch' else os.path.join(output_dir, 'features')
         layout = cfg.name
-    tester = RegistrationTester(cfg, model, limits, output_dir=feature_dir, device=device, layout=layout)
+    tester = RegistrationTester(cfg, model, limits, output_dir=feature_dir, device=device, layout=layout, rpmnet_metrics=rpmnet_metrics)
     try:
         summary, per_pair = tester.run(test_set, log=lambda m: _log(log_file, m))
     finally:
@@ -88,6 +92,8 @@ def make_parser():
     p.add_argument('--neighbor-limits', choices=['calibrate', 'config'], default='calibrate')
     p.add_argument('--seed', type=int, default=None, help='seed of the calibration draws (default cfg.seed)')
     p.add_argument('--rotated', action='store_true', help='3dmatch only: the rotated benchmark (pair i rotated from np.random.seed(i))')
+    p.add_argument('--rpmnet-metrics', action='store_true',
+                   help="modelnet only: also report RPMNet's metrics (Chamfer distance, anisotropic MSE / MAE) as rpmnet_<name>")
     return p
 
 
@@ -95,8 +101,10 @@ def main(argv=None):
     a = make_parser().parse_args(argv)
     if a.rotated and a.config != '3dmatch':
         make_parser().error('--rotated is a 3dmatch benchmark')
+    if a.rpmnet_metrics and a.config != 'modelnet':
+        raise ValueError('--rpmnet-metrics is a modelnet benchmark')
     run(a.config, a.snapshot, a.dataset_root, a.output_dir, benchmark=a.benchmark, neighbor_limits=a.neighbor_limits, seed=a.seed,
-        rotated=a.rotated)
+        rotated=a.rotated, rpmnet_metrics=a.rpmnet_metrics)
 
 
 if __name__ == '__main__':

@@ -856,6 +856,32 @@ int geob200_modelnet_benchmark_pairs_batched(const float* shapes, const int64_t*
 int geob200_rotated_pairs_batched(const void* points, int points_fp64, const int64_t* lengths_h, const int64_t* indices_h, int64_t n_pairs,
                                   const double* transforms, float* out_points, float* out_transforms, double* rotations, void* stream);
 
+/* ---- ModelNet raw shapes and RPMNet's metrics (datasets/registration/modelnet/dataset.py raw_points; utils/registration.py) ----- */
+
+/* The ModelNet item's raw_points: normalize_points(shape) in fp32 for each of n_shapes stacked shapes (host lengths_h, 1 .. 8192
+ * points each), with the arithmetic the benchmark pairs use (the same device function).  out_points has the layout of shapes.
+ * Launches of up to 1024 shapes, one CTA per shape.  workspace: geob200_modelnet_raw_points_batched_workspace_bytes(n_shapes). */
+size_t geob200_modelnet_raw_points_batched_workspace_bytes(int64_t n_shapes);
+int geob200_modelnet_raw_points_batched(const float* shapes, const int64_t* lengths_h, int64_t n_shapes, float* out_points,
+                                        void* workspace, size_t workspace_bytes, void* stream);
+
+/* RPMNet's ModelNet metrics of n_pairs (1 .. 32) pairs (the contract is in DESIGN.md section 8a).  raw / ref / src: stacked fp32
+ * clouds with host lengths (each 1 .. 2^28-1); gt_transforms / est_transforms: device (n_pairs, 4, 4) fp32.  out: device
+ * (n_pairs, GEOB200_RPMNET_COLUMNS) fp64 rows [cd, cd_pq, cd_qp, r_mse, r_mae, t_mse, t_mae, status]:
+ *   cd_pq: mean exact nearest-neighbour distance from fp32(est src) to raw; cd_qp: from ref to fp32((est gt^-1) raw); cd their sum;
+ *   r_mse / r_mae: of the Euler angles ('xyz', degrees) of scipy's from_matrix, unwrapped differences; t_mse / t_mae in fp32;
+ *   status: 0, or GEOB200_RPMNET_GT_DET / GEOB200_RPMNET_EST_DET when that rotation has det <= 0 (r_mse / r_mae are then NaN).
+ * The rows are independent of the batch: one n-pair call equals n one-pair calls bit for bit.  No host synchronisation.
+ * workspace: geob200_rpmnet_metrics_batched_workspace_bytes(n_pairs, max ref / src length, max raw length). */
+#define GEOB200_RPMNET_MAX_PAIRS 32
+#define GEOB200_RPMNET_COLUMNS 8
+#define GEOB200_RPMNET_GT_DET 1
+#define GEOB200_RPMNET_EST_DET 2
+size_t geob200_rpmnet_metrics_batched_workspace_bytes(int64_t n_pairs, int64_t cap_query, int64_t cap_raw);
+int geob200_rpmnet_metrics_batched(const float* raw, const int64_t* raw_lengths_h, const float* ref, const int64_t* ref_lengths_h,
+                                   const float* src, const int64_t* src_lengths_h, int64_t n_pairs, const float* gt_transforms,
+                                   const float* est_transforms, double* out, void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
