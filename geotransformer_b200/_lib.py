@@ -36,6 +36,9 @@ _sig('geob200_neighbor_histogram', c_int, P, I64, I64, I64, I64, P, P)
 _sig('geob200_neighbor_histogram_batched', c_int, P, P, P, I64, I64, I64, I64, P, P, P, P)
 _sig('geob200_voxel_down_sample_workspace_bytes', SZ, I64, I64)
 _sig('geob200_voxel_down_sample', c_int, P, P, I64, P, I64, D, P, P, P, P, SZ, P)
+_sig('geob200_estimate_normals_workspace_bytes', SZ, I64, I64)
+_sig('geob200_estimate_normals', c_int, P, I64, P, I64, I64, D, P, P, P, P, P, SZ, P)
+_sig('geob200_regularize_normals', c_int, P, P, I64, c_int, c_int, P, P)
 _sig('geob200_kernel_point_optimize', c_int, P, I64, I64, ctypes.c_uint64, D, P, P, P)
 _sig('geob200_kernel_point_instances', c_int, P, I64, P, P, I64, ctypes.c_uint64, P, P)
 _sig('geob200_kpconv_workspace_bytes', SZ, I64)

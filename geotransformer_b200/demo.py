@@ -1,14 +1,16 @@
 """Register two point clouds with a 3DMatch snapshot, the experiment's ``demo.py``.
 
     python -m geotransformer_b200.demo --src-file SRC.npy --ref-file REF.npy [--gt-file GT.npy] --weights FILE \\
-        [--voxel-size V] [--output DIR]
+        [--voxel-size V] [--output DIR [--normals]]
 
 Ones as features, the 3DMatch config's fixed neighbour limits [38, 36, 36, 38] and ``state_dict['model']`` of the snapshot, as the
 reference.  ``--voxel-size`` first downsamples both clouds on the device with Open3D's voxel downsampling
 (``utils.open3d.voxel_downsample``), for clouds that are not already at the training voxel size.  With ``--gt-file`` the reference's
 ``RRE(deg): ..., RTE(m): ...`` line is printed.  Instead of Open3D windows, ``--output`` writes ``estimated_transform.npy`` and
 ``registration.ply``: an ASCII PLY of the ref points in ``custom_yellow`` and the src points aligned by the estimate in
-``custom_blue``.  3DMatch only, as the reference's demo: KITTI's neighbour limits are calibrated, not fixed.
+``custom_blue``.  With ``--normals`` the PLY also holds ``nx ny nz``, so it can be viewed shaded as the reference shows it: the
+ref normals are ``utils.open3d.estimate_normals(ref)``, the src normals are estimated on the unaligned src and rotated by the
+estimate's R, as Open3D's ``PointCloud.transform`` does in the reference demo.  3DMatch only, as the reference's demo: KITTI's neighbour limits are calibrated, not fixed.
 """
 import argparse
 import os
@@ -42,19 +44,33 @@ def load_data(src_file, ref_file, gt_file=None, voxel_size=None):
     return data_dict
 
 
-def write_ply(path, ref_points, src_points):
-    """ASCII PLY: ref in custom_yellow, then src in custom_blue"""
+def write_ply(path, ref_points, src_points, ref_normals=None, src_normals=None):
+    """ASCII PLY: ref in custom_yellow, then src in custom_blue; with normals (both or neither) also nx ny nz per vertex"""
     rows = [(p, CUSTOM_YELLOW) for p in ref_points] + [(p, CUSTOM_BLUE) for p in src_points]
+    normals = None if ref_normals is None else list(ref_normals) + list(src_normals)
     with open(path, 'w') as f:
         f.write('ply\nformat ascii 1.0\n')
         f.write(f'element vertex {len(rows)}\n')
         f.write('property float x\nproperty float y\nproperty float z\n')
+        if normals is not None:
+            f.write('property double nx\nproperty double ny\nproperty double nz\n')
         f.write('property uchar red\nproperty uchar green\nproperty uchar blue\nend_header\n')
-        for p, c in rows:
-            f.write(f'{float(p[0]):.9g} {float(p[1]):.9g} {float(p[2]):.9g} {c[0]} {c[1]} {c[2]}\n')
+        for r, (p, c) in enumerate(rows):
+            nrm = '' if normals is None else f'{float(normals[r][0]):.17g} {float(normals[r][1]):.17g} {float(normals[r][2]):.17g} '
+            f.write(f'{float(p[0]):.9g} {float(p[1]):.9g} {float(p[2]):.9g} {nrm}{c[0]} {c[1]} {c[2]}\n')
 
 
-def run(src_file, ref_file, weights, gt_file=None, voxel_size=None, output=None):
+def registration_normals(ref_points, src_points, estimated_transform):
+    """the shaded view's normals: ref's from estimate_normals, src's estimated on the unaligned src and rotated by the estimate's R
+    in double (Open3D's TransformNormals); both (N, 3) float64 numpy"""
+    from .utils.open3d import estimate_normals
+    ref_normals = estimate_normals(np.asarray(ref_points))
+    src_normals = estimate_normals(np.asarray(src_points))
+    R = np.asarray(estimated_transform)[:3, :3].astype(np.float64)
+    return ref_normals, src_normals @ R.T
+
+
+def run(src_file, ref_file, weights, gt_file=None, voxel_size=None, output=None, normals=False):
     """the demo; returns (estimated transform (4, 4) float32 numpy, (rre, rte) or None)"""
     from .model import create_model
     from .utils.registration import compute_registration_error
@@ -79,7 +95,10 @@ def run(src_file, ref_file, weights, gt_file=None, voxel_size=None, output=None)
         ref_points = output_dict['ref_points'].cpu().numpy()
         src_points = output_dict['src_points'].cpu().numpy().astype(np.float64)
         aligned = src_points @ estimated_transform[:3, :3].T.astype(np.float64) + estimated_transform[:3, 3].astype(np.float64)
-        write_ply(os.path.join(output, 'registration.ply'), ref_points, aligned)
+        ref_normals = src_normals = None
+        if normals:
+            ref_normals, src_normals = registration_normals(ref_points, output_dict['src_points'].cpu().numpy(), estimated_transform)
+        write_ply(os.path.join(output, 'registration.ply'), ref_points, aligned, ref_normals, src_normals)
     return estimated_transform, errors
 
 
@@ -91,8 +110,11 @@ def main(argv=None):
     parser.add_argument('--weights', required=True, help='model weights file')
     parser.add_argument('--voxel-size', type=float, default=None, help='voxel-downsample both clouds first (Open3D semantics)')
     parser.add_argument('--output', default=None, help='directory for estimated_transform.npy and registration.ply')
+    parser.add_argument('--normals', action='store_true', help='with --output: estimate normals (Open3D semantics) into the PLY')
     args = parser.parse_args(argv)
-    run(args.src_file, args.ref_file, args.weights, args.gt_file, args.voxel_size, args.output)
+    if args.normals and args.output is None:
+        parser.error('--normals needs --output')
+    run(args.src_file, args.ref_file, args.weights, args.gt_file, args.voxel_size, args.output, args.normals)
 
 
 if __name__ == '__main__':

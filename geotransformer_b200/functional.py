@@ -2730,3 +2730,72 @@ def voxel_down_sample_batched(points, lengths, voxel_size, normals=None):
     if nrm is not None:
         res = res + (out_n[:m].clone(),)
     return res
+
+
+NORMALS_MAX_CLOUDS = 64
+NORMALS_MAX_KNN = 64
+
+
+def _normals_args(knn, radius):
+    if isinstance(knn, bool) or not hasattr(knn, '__index__') or not 1 <= int(knn) <= NORMALS_MAX_KNN:
+        raise ValueError(f'estimate_normals: knn must be an integer in 1..{NORMALS_MAX_KNN}, got {knn!r}')
+    if radius is not None:
+        radius = float(radius)
+        if not (radius > 0 and math.isfinite(radius)):
+            raise ValueError(f'estimate_normals: radius must be positive and finite, got {radius}')
+    return int(knn), radius
+
+
+def estimate_normals_batched(points, lengths, knn=30, radius=None, return_neighbors=False):
+    """Open3D's ``PointCloud::EstimateNormals`` (``KDTreeSearchParamKNN(knn)``, or ``KDTreeSearchParamHybrid(radius, knn)`` with a
+    radius; FastEigen3x3; no orientation) of up to 64 stacked clouds in one call (``geob200_estimate_normals``), in double.
+    ``points``: CUDA (sum(lengths), 3) float64, or float32 (widened exactly, as ``Vector3dVector`` does); ``lengths``: B host ints
+    (empty clouds allowed).  Returns the (N, 3) float64 normals on the device; with ``return_neighbors`` also each point's
+    neighbours ((N, knn) int32 in-cloud indices in ascending (squared distance, index), -1 past the count) and covariances ((N, 6)
+    float64: c00 c01 c02 c11 c12 c22).  The status word is read back once.  ``ValueError`` for knn outside 1..64, a radius that
+    is not positive, or a non-finite coordinate (DESIGN.md section 8a)."""
+    knn, radius = _normals_args(knn, radius)
+    lengths = [int(v) for v in lengths]
+    B = len(lengths)
+    if not 1 <= B <= NORMALS_MAX_CLOUDS:
+        raise ValueError(f'estimate_normals_batched: 1..{NORMALS_MAX_CLOUDS} clouds per call, got {B}')
+    if not isinstance(points, torch.Tensor) or not points.is_cuda:
+        raise RuntimeError('points must be a CUDA tensor (geotransformer_b200 has no CPU path)')
+    if points.dtype not in (torch.float32, torch.float64):
+        raise RuntimeError(f'points must be float32 or float64, got {points.dtype}')
+    pts = points.to(torch.float64).contiguous()
+    if pts.dim() != 2 or pts.shape[1] != 3 or pts.shape[0] != sum(lengths):
+        raise RuntimeError(f'estimate_normals_batched: points must be (sum(lengths), 3), got {tuple(pts.shape)}')
+    n, dev = pts.shape[0], pts.device
+    lib = L.lib()
+    ws = L.workspace(lib.geob200_estimate_normals_workspace_bytes(n, B), dev, tag='normals')
+    out = torch.empty((n, 3), dtype=torch.float64, device=dev)
+    nbr = torch.empty((n, knn), dtype=torch.int32, device=dev) if return_neighbors else None
+    cov = torch.empty((n, 6), dtype=torch.float64, device=dev) if return_neighbors else None
+    status = torch.empty((1,), dtype=_i64, device=dev)
+    L.check(lib.geob200_estimate_normals(pts.data_ptr(), n, _host_i64(lengths), B, knn, 0.0 if radius is None else radius,
+                                         out.data_ptr(), L.ptr(nbr), L.ptr(cov), status.data_ptr(), ws.data_ptr(), ws.numel(),
+                                         L.stream_ptr()), 'estimate_normals_batched')
+    st = int(status.item())
+    if st != 0:
+        raise ValueError('estimate_normals_batched: a coordinate is NaN or infinite' if st == 1 else f'estimate_normals_batched: error {st}')
+    return (out, nbr, cov) if return_neighbors else out
+
+
+def regularize_normals(points, normals, positive=True):
+    """The reference's ``regularize_normals`` (``utils/pointcloud.py``) on CUDA tensors, bit for bit with its numpy expression:
+    ``d = -(points * normals).sum(1)``, ``direction = d > 0``, then ``n * dir - n * (1 - dir)`` (``positive``) or the mirrored
+    form.  The dot products are taken in float32 when both inputs are float32 and in float64 otherwise; the result is float64
+    either way, as in numpy, where ``1 - direction`` is an int64 array."""
+    for t, name in ((points, 'points'), (normals, 'normals')):
+        if not isinstance(t, torch.Tensor) or not t.is_cuda:
+            raise RuntimeError(f'{name} must be a CUDA tensor (geotransformer_b200 has no CPU path)')
+    dt = torch.float32 if (points.dtype == torch.float32 and normals.dtype == torch.float32) else torch.float64
+    p = points.to(dt).reshape(-1, 3).contiguous()
+    nrm = normals.to(device=p.device, dtype=dt).reshape(-1, 3).contiguous()
+    if p.shape != nrm.shape:
+        raise ValueError(f'regularize_normals: points {tuple(points.shape)} and normals {tuple(normals.shape)} differ')
+    out = torch.empty(nrm.shape, dtype=torch.float64, device=nrm.device)
+    L.check(L.lib().geob200_regularize_normals(p.data_ptr(), nrm.data_ptr(), p.shape[0], int(dt == torch.float64), int(bool(positive)),
+                                               out.data_ptr(), L.stream_ptr()), 'regularize_normals')
+    return out.reshape(normals.shape)

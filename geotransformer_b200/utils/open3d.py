@@ -1,8 +1,9 @@
-"""Voxel downsampling, correspondence RANSAC and feature-matching RANSAC with the reference's interface
-(geotransformer/utils/open3d.py:57-65 and 133-198), on the device, without Open3D.
+"""Voxel downsampling, normal estimation, correspondence RANSAC and feature-matching RANSAC with the reference's interface
+(geotransformer/utils/open3d.py:49-65 and 133-198), on the device, without Open3D.
 
-``voxel_downsample`` follows Open3D's ``PointCloud::VoxelDownSample`` in double, values and order (DESIGN.md section 8a); it is
-pinned to a restatement of that function, not checked against an Open3D build.
+``voxel_downsample`` follows Open3D's ``PointCloud::VoxelDownSample`` in double, values and order, and ``estimate_normals``
+Open3D's ``PointCloud::EstimateNormals`` (DESIGN.md section 8a); both are pinned to restatements of those functions, not checked
+against an Open3D build.
 
 The estimates follow Open3D's registration_ransac_based_on_correspondence and (0.11's) registration_ransac_based_on_feature_matching
 as the reference calls them; the sampler, the tie rule and the fp32 scoring differ from Open3D (DESIGN.md section 3b), so the
@@ -108,3 +109,22 @@ def registration_with_ransac_from_feats(src_points, ref_points, src_feats, ref_f
     if on_device:
         return res['transform']
     return res['transform'].cpu().numpy().astype(np.float64)
+
+
+def estimate_normals(points, knn=30, radius=None):
+    r"""Open3D's ``pcd.estimate_normals()`` of one cloud, with the reference's signature (``knn`` and ``radius`` select
+    ``KDTreeSearchParamKNN(knn)`` or ``KDTreeSearchParamHybrid(radius, knn)``; the reference calls the default, knn 30).
+
+    numpy input gives a float64 numpy array, as ``np.asarray(pcd.normals)`` does; a CUDA tensor gives a float64 CUDA tensor.
+    float32 input is widened exactly, as ``Vector3dVector`` does.  Normals are not oriented (Open3D orients only against normals
+    the cloud already has)."""
+    on_device = isinstance(points, torch.Tensor)
+    if on_device and not points.is_cuda:
+        raise RuntimeError('points must be a numpy array or a CUDA tensor (geotransformer_b200 has no CPU path)')
+    if on_device:
+        pts = points.detach().to(torch.float64).reshape(-1, 3).contiguous()
+    else:
+        pts = torch.from_numpy(np.ascontiguousarray(points, dtype=np.float64).reshape(-1, 3)).to(
+            torch.device('cuda', torch.cuda.current_device()))
+    out = GF.estimate_normals_batched(pts, [pts.shape[0]], knn=knn, radius=radius)
+    return out if on_device else out.cpu().numpy()

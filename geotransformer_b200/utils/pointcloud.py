@@ -1,4 +1,5 @@
-"""``get_nearest_neighbor`` of ``geotransformer/utils/pointcloud.py:11-22`` on the device (exact brute force, csrc/feature_match.cu).
+"""``get_nearest_neighbor`` and ``regularize_normals`` of ``geotransformer/utils/pointcloud.py:11-37`` on the device
+(``get_nearest_neighbor``: exact brute force, csrc/feature_match.cu; ``regularize_normals``: csrc/normals.cu).
 
 Inputs are numpy arrays or CUDA tensors of points or descriptors (any width C in 1..1024), rounded to float32.  numpy inputs run
 on the current CUDA device and give numpy outputs; CUDA tensors give device tensors; a CPU tensor raises RuntimeError.
@@ -39,3 +40,25 @@ def get_nearest_neighbor(q_points, s_points, return_index=False):
     if not on_device:
         index, dist = index.cpu().numpy(), dist.cpu().numpy()
     return (dist, index) if return_index else dist
+
+
+def regularize_type(points_dtype, normals_dtype):
+    """the type in which the drop-in takes the point-normal dot products: numpy's type of ``points * normals`` for float inputs,
+    float32 only when both are float32 (the result is float64 either way)"""
+    both32 = np.dtype(points_dtype) == np.float32 and np.dtype(normals_dtype) == np.float32
+    return np.dtype(np.float32) if both32 else np.dtype(np.float64)
+
+
+def regularize_normals(points, normals, positive=True):
+    r"""Orient each normal by the sign of s_i = p_i . n_i, with the reference's signature.  ``positive=True`` makes the normals
+    face the origin: n_i is kept when s_i < 0 and negated otherwise.  ``positive=False`` makes them face away from it: n_i is
+    negated when s_i < 0 and kept otherwise.  The values, signed zeros included, and the float64 result type are those of the
+    reference's numpy code (DESIGN.md section 8a).  numpy inputs give a numpy array; CUDA tensors give a device tensor."""
+    device, on_device = _device(points, normals)
+    if on_device:
+        return GF.regularize_normals(points, normals, positive)
+    p, n = np.asarray(points), np.asarray(normals)
+    dt = regularize_type(p.dtype, n.dtype)
+    out = GF.regularize_normals(torch.from_numpy(np.ascontiguousarray(p, dtype=dt)).to(device),
+                                torch.from_numpy(np.ascontiguousarray(n, dtype=dt)).to(device), positive)
+    return out.cpu().numpy()

@@ -81,6 +81,30 @@ int geob200_voxel_down_sample(const double* points, const double* normals, int64
                               double voxel, double* out_points, double* out_normals, int64_t* out_lengths, void* workspace,
                               size_t workspace_bytes, void* stream);
 
+/* ---- normal estimation (Open3D PointCloud::EstimateNormals; csrc/normals.cu) ------------------------------------------------- */
+
+/* Open3D's EstimateNormals (FastEigen3x3, no orientation) of `batch` stacked clouds (lengths_h host int64[batch], empty clouds
+ * allowed), in double: per point the exact min(knn, N) nearest points of its cloud, itself included, ascending (squared distance,
+ * index); with radius > 0 only those with squared distance < radius^2 (KDTreeSearchParamHybrid), radius == 0 for none; the
+ * covariance from nine cumulants over them; the unit eigenvector of its smallest eigenvalue; (0, 0, 1) for fewer than 3
+ * neighbours or a zero-norm result (the contract is in DESIGN.md section 8a).  points: device (n_points, 3) fp64; out_normals:
+ * device (n_points, 3) fp64.  out_neighbors (optional, device int32 (n_points, knn)): each point's neighbours as in-cloud indices,
+ * -1 past the count; out_covariance (optional, device fp64 (n_points, 6)): c00 c01 c02 c11 c12 c22.  out_status: device int64[1],
+ * 0 or a GEOB200_NORMALS_* code for an error found on the device (no output is written then).  Arguments are checked before any
+ * launch; no host synchronisation. */
+#define GEOB200_NORMALS_MAX_CLOUDS 64
+#define GEOB200_NORMALS_MAX_KNN 64
+#define GEOB200_NORMALS_NONFINITE 1   /* a coordinate is NaN or infinite */
+size_t geob200_estimate_normals_workspace_bytes(int64_t n_points, int64_t batch);
+int geob200_estimate_normals(const double* points, int64_t n_points, const int64_t* lengths_h, int64_t batch, int64_t knn, double radius,
+                             double* out_normals, int32_t* out_neighbors, double* out_covariance, int64_t* out_status, void* workspace,
+                             size_t workspace_bytes, void* stream);
+/* The reference's regularize_normals (utils/pointcloud.py) row by row, bit for bit with numpy: points and normals device (n, 3),
+ * both fp32 (fp64 = 0) or both fp64; d = -(((x nx) + y ny) + z nz) in that type, dir = d > 0; out (device (n, 3) fp64) =
+ * n dir - n (1 - dir) (positive) or n (1 - dir) - n dir, with n dir in the input type and n (1 - dir) in fp64, as numpy promotes
+ * a bool and an int64 factor. */
+int geob200_regularize_normals(const void* points, const void* normals, int64_t n, int fp64, int positive, double* out, void* stream);
+
 /* ---- kernel-point dispositions (reference modules/kpconv/kernel_points.py; csrc/kernel_points.cu) ----------------------------- */
 
 /* kernel_point_optimization_debug(1.0, num_points, num_kernels, 3, fixed='center', ratio) in fp64, one launch of one CTA: the
